@@ -1,4 +1,4 @@
-"""3dunetcnn_b200 -- B200-native 3D U-Net forward/backward path behind the reference's model / loss / train /
+"""3dunetcnn_b200 -- H100-native (sm_90a) 3D U-Net forward/backward path behind the reference's model / loss / train /
 predict interface.  The directory name starts with a digit, so import it with
 ``importlib.import_module("3dunetcnn_b200")`` (tests/conftest.py and __graft_entry__.py do).
 """

@@ -17,7 +17,7 @@ void set_error(const char* fmt, ...) {
 }
 const char* get_error() { return g_err; }
 
-// opt-in until measured on B200 in both states (common.cuh: launch_pdl)
+// opt-in (common.cuh: launch_pdl)
 static const bool kPdlDefault = false;
 bool pdl_enabled() {
   static const bool on = getenv("B200UNET_PDL") ? atoi(getenv("B200UNET_PDL")) != 0 : kPdlDefault;
@@ -205,18 +205,6 @@ int b200unet_zscore(const float* x, int groups, int64_t spatial, int nonzero, do
 int b200unet_label_map(const float* p, int n_labels, int64_t spatial, const int32_t* labels, int act, float threshold,
                        int hierarchy, int sum_then_threshold, int16_t* out, void* stream) {
   return launch_label_map(p, n_labels, spatial, labels, act, threshold, hierarchy, sum_then_threshold, out, to_stream(stream));
-}
-
-int b200unet_umma_probe(const int32_t* tests, int ntests, float* out, void* stream) {
-  NOT_NULL(tests); NOT_NULL(out);
-  return launch_umma_probe(tests, ntests, out, to_stream(stream));
-}
-
-int b200unet_umma_rate(int n, int layout, int a_sbo, int b_sbo, int a_step, int inner, int reps, int ctas, int64_t* out,
-                       const void* copy_src, int copy_bytes, int commit_each_rep, void* stream) {
-  NOT_NULL(out);
-  return launch_umma_rate(n, layout, a_sbo, b_sbo, a_step, inner, reps, ctas, reinterpret_cast<long long*>(out), copy_src,
-                          copy_bytes, commit_each_rep, to_stream(stream));
 }
 
 }  // extern "C"

@@ -59,8 +59,8 @@ static inline Act slice_c(const Act& a, int c0, int c) {
 }
 
 // Programmatic dependent launch (opt-in: B200UNET_PDL=1).  A kernel launched through launch_pdl may be scheduled while the previous
-// kernel of the stream still runs: its CTAs take SMs as that kernel's CTAs retire, run their set-up (barrier init, TMEM
-// allocation, descriptor prefetch) and block in pdl_wait() (ptx.cuh) until the previous kernel has completed and its writes are
+// kernel of the stream still runs: its CTAs take SMs as that kernel's CTAs retire, run their set-up (barrier init,
+// descriptor prefetch) and block in pdl_wait() (ptx.cuh) until the previous kernel has completed and its writes are
 // visible -- the launch latency and the set-up of every launch leave the critical path.  ONLY kernels that execute pdl_wait()
 // before their first access to global memory may be launched this way.
 bool pdl_enabled();

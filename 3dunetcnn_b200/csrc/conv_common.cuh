@@ -1,5 +1,5 @@
-// Shared pieces of the two implicit-GEMM convolution kernels (igemm_conv.cu: per-tap streaming tiles;
-// conv_halo.cu: halo-resident tiles): argument block, TMA map bundle and the fused epilogue.
+// Shared pieces of the implicit-GEMM convolution kernel (igemm_conv.cu): argument block, TMA map bundle and the fused
+// epilogue.
 #pragma once
 #include "kernels.h"
 #include "ptx.cuh"
@@ -11,8 +11,6 @@ struct ConvMaps {
   CUtensorMap a[2][2];  // [source][hi/lo]
   CUtensorMap b[2][2];
   CUtensorMap o[2];     // output tile stores (hi/lo): the epilogue stages 128 x BN tiles in shared memory and TMA-stores them
-  CUtensorMap side;     // halo kernel: the epilogue's side input (residual / GroupNorm input), box = one output plane tile; only
-                        // used to request its tiles into L2 ahead of the epilogue (cp.async.bulk.prefetch.tensor)
 };
 // parity-class mode of the streaming kernel (stride-2 data gradient): one output map per class and hi/lo
 struct ConvClassMaps {
@@ -128,12 +126,12 @@ __device__ __forceinline__ void conv_epilogue_prefetch(const ConvArgs& p, int n0
   }
 }
 
-// Fused epilogue for one 128-row accumulator tile living at TMEM address `tacc` (lane quadrant applied through
-// `lane_base`).  Columns are processed in groups of <= 64: the group's side input (residual / norm input) is loaded
-// into registers up front (one latency per group instead of one per 16-column chunk), then per 16-column chunk:
-// tcgen05.ld -> (+residual)(*scale) | GN/ReLU backward -> hi/lo store -> per-channel partial sums into s_stats.
+// Fused epilogue for one row of a 128-row fp32 accumulator tile in shared memory (`acc_row`: this thread's row).  Columns
+// are processed in groups of <= 64: the group's side input (residual / norm input) is loaded into registers up front (one
+// latency per group instead of one per 16-column chunk), then per 16-column chunk:
+// accumulator -> (+residual)(*scale) | GN/ReLU backward -> hi/lo store -> per-channel partial sums into s_stats (slot `wslot`).
 template <int BN>
-__device__ __forceinline__ void conv_epilogue_tile(const ConvArgs& p, uint32_t tacc, int lane_base, int lane, int n,
+__device__ __forceinline__ void conv_epilogue_tile(const ConvArgs& p, const float* acc_row, int wslot, int lane, int n,
                                                    int n0, long long vox, bool valid, float* s_stats,
                                                    const float4* s_coef, bool want_stats, bool edge, uint8_t* stage,
                                                    int row, bool split) {
@@ -165,12 +163,12 @@ __device__ __forceinline__ void conv_epilogue_tile(const ConvArgs& p, uint32_t t
       const int j = g0 / 16 + jj;
       const int c0 = n0 + j * 16;
       if (c0 < p.Cout) {
-        uint32_t r[16];
-        tmem_ld16(tacc + (static_cast<uint32_t>(lane_base) << 16) + j * 16, r);
-        tmem_ld_wait();
         float v[16], q[16];
 #pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+        for (int i = 0; i < 16; i += 4) {
+          const float4 a = *reinterpret_cast<const float4*>(acc_row + j * 16 + i);
+          v[i] = a.x; v[i + 1] = a.y; v[i + 2] = a.z; v[i + 3] = a.w;
+        }
 #pragma unroll
         for (int hf = 0; hf < 2; ++hf) {
           const int cc = c0 + hf * 8;
@@ -243,7 +241,7 @@ __device__ __forceinline__ void conv_epilogue_tile(const ConvArgs& p, uint32_t t
           const float s2 = warp_colsum16(q, lane);
           if ((lane & 1) == 0) {
             // s_stats: one private [BN][2] slot per epilogue warp (no shared-memory float atomics: they are CAS loops)
-            float2* mine = reinterpret_cast<float2*>(s_stats) + (lane_base >> 5) * BN + j * 16 + ((lane >> 1) & 15);
+            float2* mine = reinterpret_cast<float2*>(s_stats) + wslot * BN + j * 16 + ((lane >> 1) & 15);
             float2 acc = *mine;
             acc.x += s1; acc.y += s2;
             *mine = acc;

@@ -154,7 +154,7 @@ int launch_dice_fwd(const float* logits, const uint8_t* target, int N, int C, lo
   B200_CHECK_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 3 * N * C, st));
   long long per = (S + 1023) / 1024;
   int chunks = (int)(per < 1 ? 1 : per);
-  int cap = (148 * 8 + N * C - 1) / (N * C);
+  int cap = (132 * 8 + N * C - 1) / (N * C);
   if (chunks > cap) chunks = cap < 1 ? 1 : cap;
   if (flags & 64) k_dice_sums<float><<<dim3(chunks, N * C), 256, 0, st>>>(logits, reinterpret_cast<const float*>(target), S, f, sums);
   else k_dice_sums<uint8_t><<<dim3(chunks, N * C), 256, 0, st>>>(logits, target, S, f, sums);
@@ -169,7 +169,7 @@ int launch_dice_bwd(const float* logits, const uint8_t* target, int N, int C, lo
   DiceFlags f = unpack_flags(flags);
   long long per = (S + 1023) / 1024;
   int chunks = (int)(per < 1 ? 1 : per);
-  int cap = (148 * 8 + N * C - 1) / (N * C);
+  int cap = (132 * 8 + N * C - 1) / (N * C);
   if (chunks > cap) chunks = cap < 1 ? 1 : cap;
   if (flags & 64)
     k_dice_bwd<float><<<dim3(chunks, N * C), 256, 0, st>>>(logits, reinterpret_cast<const float*>(target), N, C, S, f, nr, dr, sums,

@@ -280,7 +280,7 @@ __global__ void __launch_bounds__(256) k_gn_apply(Act x, Act y, const float4* __
 
 static int ew_blocks(long long total, int threads) {
   long long b = (total + threads - 1) / threads;
-  long long cap = 148LL * 16;
+  long long cap = 132LL * 16;
   return (int)(b < cap ? (b > 0 ? b : 1) : cap);
 }
 
@@ -299,7 +299,7 @@ static int launch_gn_apply_impl(const Act& x, const Act& y, const float* coef, f
   const long long S = (long long)x.D * x.H * x.W;
   const int vper = threads / c8n;
   long long want = (S + 2LL * vper - 1) / (2LL * vper);
-  const long long cap = (148LL * 8 + x.N - 1) / x.N;
+  const long long cap = (132LL * 8 + x.N - 1) / x.N;
   int blocks = (int)(want < cap ? (want > 0 ? want : 1) : cap);
   if (fin) {
     B200_REQUIRE(x.C <= 1024, E_UNSUPPORTED, "gn_apply: fused finalize supports C <= 1024 (got %d)", x.C);
@@ -511,7 +511,7 @@ static int launch_gn_bwd_impl(const Act& dz, const Act& x, const float* coef, co
   const long long S = (long long)x.D * x.H * x.W;
   const int vper = threads / c8n;
   long long want = (S + 2LL * vper - 1) / (2LL * vper);
-  const long long cap = (148LL * 8 + x.N - 1) / x.N;
+  const long long cap = (132LL * 8 + x.N - 1) / x.N;
   int blocks = (int)(want < cap ? (want > 0 ? want : 1) : cap);
   if (fin) {
     B200_REQUIRE(x.C <= 1024, E_UNSUPPORTED, "gn_bwd: fused finalize supports C <= 1024 (got %d)", x.C);
@@ -604,7 +604,7 @@ int launch_act_bwd(const Act& g1, const Act* g2, const Act& c, const float* coef
   const long long S = (long long)c.D * c.H * c.W;
   const int vper = threads / c8n;
   long long want = (S + vper - 1) / vper;
-  const long long cap = (148LL * 4 + c.N - 1) / c.N;
+  const long long cap = (132LL * 4 + c.N - 1) / c.N;
   const int blocks = (int)(want < cap ? (want > 0 ? want : 1) : cap);
   Act none = make_act(nullptr, nullptr, 0, 0, 0, 0, 0, 0);
   k_act_bwd<<<dim3(blocks, c.N), threads, c.C * 2 * sizeof(double), st>>>(g1, g2 ? *g2 : none, c, reinterpret_cast<const float4*>(coef),
@@ -775,7 +775,7 @@ int launch_upsample2x_fwd(const Act& x, const Act& y, double* stats, int stats_l
   const long long nblk = (long long)(x.D + 1) * (x.H + 1) * (x.W + 1);
   B200_REQUIRE(nblk < (1LL << 31), E_UNSUPPORTED, "upsample: volume too large");
   long long want = (nblk + vper - 1) / vper;
-  const long long cap = (148LL * 8 + x.N - 1) / x.N;
+  const long long cap = (132LL * 8 + x.N - 1) / x.N;
   const int blocks = (int)(want < cap ? (want > 0 ? want : 1) : cap);
   k_upsample2x_fwd<<<dim3(blocks, x.N), threads, x.C * 2 * sizeof(double), st>>>(x, y, stats, stats_ld);
   B200_CHECK_CUDA(cudaGetLastError());

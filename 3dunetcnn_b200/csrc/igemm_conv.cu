@@ -1,19 +1,19 @@
-// 3-D convolution as an implicit GEMM on the sm_100a tensor cores.
+// 3-D convolution as an implicit GEMM on the sm_90a tensor cores (wgmma).
 //
-//   Y[v][co] = sum_{tap, ci} A[v*stride + tap - pad][ci] * Wp[tap][co][ci]          (fp32 accumulate in TMEM)
+//   Y[v][co] = sum_{tap, ci} A[v*stride + tap - pad][ci] * Wp[tap][co][ci]          (fp32 accumulate in registers)
 //
 // Replaces (forward, and data-gradient with flipped/transposed packed weights):
-//   nn.Conv3d k3 s1/s2 p1, bias-free    /root/reference/unet3d/models/pytorch/classification/resnet.py:12-17
-//   nn.Conv3d k1                        /root/reference/unet3d/models/pytorch/classification/resnet.py:20-22
+//   nn.Conv3d k3 s1/s2 p1, bias-free    unet3d/models/pytorch/classification/resnet.py:12-17 of the reference
+//   nn.Conv3d k1                        unet3d/models/pytorch/classification/resnet.py:20-22 of the reference
 // GEMM view: M = 128 output voxels (one tw x th x td spatial box of one sample), N = BN output channels,
-// K = taps x Cin walked in chunks of KC channels.  Per K step the producer thread issues two TMA loads:
+// K = taps x Cin walked in chunks of KC channels.  Per K step the producer warp issues two TMA loads:
 //   A: 5-D box (KC, tw, th, td, 1) of the NDHWC activation at the tap-shifted coordinate; the zero padding of the
 //      convolution is TMA out-of-bounds fill, stride-2 convolutions use the tensor map's element strides;
 //   B: 3-D box (KC, BN, 1) of the packed weights [tap][co][ci].
-// Both land K-major with the hardware swizzle that matches KC (128B/64B/32B) and feed tcgen05.mma
-// (cta_group::1, kind::f16, M=128, N=BN, K=16) issued by one thread; a STAGES-deep mbarrier ring decouples
-// TMA from MMA, tcgen05.commit releases ring slots and finally signals the epilogue warps.
-// Epilogue (4 warps, one TMEM lane quadrant each): tcgen05.ld -> registers ->
+// Both land K-major with the hardware swizzle that matches KC (128B/64B/32B) and feed wgmma.mma_async (m64nBNk16, bf16,
+// fp32 accumulate) issued by one warpgroup; a STAGES-deep mbarrier ring decouples TMA from the MMAs, and a ring slot is
+// handed back once the wgmma group reading it has retired.
+// Epilogue (the same warpgroup, one output voxel row per thread, through an fp32 tile in shared memory) ->
 //   mode 0: (+ residual) (* per-(n,c) dropout scale) -> bf16 hi[/lo] store, per-channel sum / sum-of-squares
 //           for the next GroupNorm (warp butterfly -> smem -> one double atomic per channel per CTA);
 //   mode 1: GroupNorm/ReLU backward: dz = dact * 1[A x + B > 0], per-channel (sum dz, sum dz*xhat).
@@ -23,40 +23,62 @@
 
 namespace b200 {
 
-// DEEP: the pipeline ring takes ~196 KB instead of 96 KB.  The 96 KB ring lets two CTAs share an SM (192 KB of loads in flight per
-// SM); a launch with no more CTAs than SMs has one CTA per SM whatever it allocates, and with three 32 KB stages in flight it is
-// bound by the L2 round trip (the 256-channel layers at 16^3: ~34 B/clk per SM, profiles/r02_layer_times.csv) -- those launches
-// take the deep ring.
-template <int BN, int KC, int DEEP = 0>
+// Kernel modes: per-tap streaming tiles, class mode (parity-class data gradient / k = s = 2 transposed convolution), and halo
+// mode: the 3x3x3 stride-1 source is loaded as ONE halo box (KC, 10, 18, 3) per K chunk for an 8 x 16 x 1 output tile, and the
+// 27 taps read it through shifted shared-memory descriptors (27x less activation traffic from L2 than per-tap boxes).
+enum ConvMode { CONV_STREAM = 0, CONV_CLASS = 1, CONV_HALO = 2 };
+
+// Shared memory: STAGES-deep TMA ring | fp32 accumulator tile [128][BN + 4] | (class mode) output staging | (halo mode) halo box
+// | aux.  Outside class mode the output staging tile reuses the ring: the CTA computes one tile, so every stage has been consumed
+// when the epilogue starts.  Class mode keeps the staging tile apart because the producer is already loading the next class.
+// BN <= 32 (<= 204 registers per thread) sizes the ring so that two CTAs share an SM (one CTA's epilogue overlaps the other's
+// MMAs) when that still leaves four stages; otherwise one CTA takes up to 227 KB.
+template <int BN, int KC, int MODE>
 struct ConvCfg {
   static constexpr int A_BYTES = 128 * KC * 2;
   static constexpr int B_BOX_BYTES = BN * KC * 2;
   static constexpr int B_BYTES = B_BOX_BYTES < 1024 ? 1024 : B_BOX_BYTES;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES_RAW = ((DEEP ? 196 : 96) * 1024) / STAGE_BYTES;
+  static constexpr int ACC_LD = BN + 4;                     // floats per accumulator row: 16-byte aligned, rows on staggered banks
+  static constexpr int ACC_BYTES = 128 * ACC_LD * 4;
+  static constexpr int AUX_BYTES = 1024 + 4 * BN * 2 * 4 + BN * 16;  // barriers | per-warp stats | coef
+  static constexpr int OUT_STAGING = 2 * 128 * BN * 2;    // hi + lo output tiles (class pairs: 256 rows of hi)
+  static constexpr int STG_BYTES = MODE == CONV_CLASS ? OUT_STAGING : 0;
+  static constexpr int RB = KC * 2;                        // bytes per voxel row of an activation tile
+  static constexpr int HALO_TX = 540 * RB;                 // 10 x 18 x 3 voxels
+  static constexpr int HALO_BYTES = MODE == CONV_HALO ? (HALO_TX + 1023) / 1024 * 1024 : 0;
+  static constexpr int FIXED = ACC_BYTES + STG_BYTES + HALO_BYTES + AUX_BYTES + 1024;   // +1024 alignment slack
+  static constexpr int SMEM_LIMIT = 232448;                // sm_90 opt-in dynamic shared memory per block
+  static constexpr int TWO_PER_SM = 115712;                // 228 KB per SM, 1 KB reserved per block
+  static constexpr int MIN_BLOCKS = BN <= 32 ? 2 : 1;      // 2 x 160 threads x <= 204 registers fit the 64 K register file
+  static constexpr int STAGES_2 = MIN_BLOCKS == 2 ? (TWO_PER_SM - FIXED) / STAGE_BYTES : 0;
+  static constexpr int STAGES_RAW = STAGES_2 >= 4 ? STAGES_2 : (SMEM_LIMIT - FIXED) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
-  static constexpr int TMEM_COLS = BN < 32 ? 32 : BN;
-  static constexpr int AUX_BYTES = 1024 + 4 * BN * 2 * 4 + BN * 16;  // barriers+slot | per-warp stats | coef
-  static constexpr int OUT_STAGING = 2 * 128 * BN * 2;    // hi + lo output tiles, aliased onto the pipeline stages
   static constexpr int PIPE_BYTES = STAGES * STAGE_BYTES > OUT_STAGING ? STAGES * STAGE_BYTES : OUT_STAGING;
-  static constexpr int SMEM_BYTES = PIPE_BYTES + AUX_BYTES + 1024;  // +1024 alignment slack
-  static constexpr uint32_t LAYOUT = KC == 64 ? UMMA_SW128 : KC == 32 ? UMMA_SW64 : UMMA_SW32;
+  static constexpr int SMEM_BYTES = PIPE_BYTES + FIXED;
+  static constexpr uint32_t LAYOUT = swizzle_for_row_bytes(KC * 2);
   static constexpr uint32_t SBO = 8 * KC * 2;
+  static_assert(STAGES >= 2 && SMEM_BYTES <= SMEM_LIMIT, "igemm_conv: configuration does not fit shared memory");
 };
 
-template <int BN, int KC, int DEEP>
-__global__ void __launch_bounds__(192) k_igemm_conv(const __grid_constant__ ConvMaps maps, const ConvArgs p,
-                                                    const __grid_constant__ ConvClassMaps cmaps) {
-  using Cfg = ConvCfg<BN, KC, DEEP>;
+// Warps 0-3: one consumer warpgroup (wgmma issue, then the epilogue, one output voxel row per thread); warp 4: TMA producer.
+template <int BN, int KC, int MODE>
+__global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_igemm_conv(const __grid_constant__ ConvMaps maps,
+                                                                                       const ConvArgs p,
+                                                                                       const __grid_constant__ ConvClassMaps cmaps) {
+  using Cfg = ConvCfg<BN, KC, MODE>;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment by pointer arithmetic on the __shared__ array: an integer round trip loses the address space and every
-  // shared-memory access below would compile to a generic LD.E / ST.E (ncu source view, round 2) instead of LDS / STS
+  // shared-memory access below would compile to a generic LD.E / ST.E instead of LDS / STS
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* aux = smem + Cfg::PIPE_BYTES;
+  float* s_acc = reinterpret_cast<float*>(smem + Cfg::PIPE_BYTES);
+  uint8_t* stage_out = MODE == CONV_CLASS ? smem + Cfg::PIPE_BYTES + Cfg::ACC_BYTES : smem;
+  uint8_t* halo = smem + Cfg::PIPE_BYTES + Cfg::ACC_BYTES + Cfg::STG_BYTES;
+  uint8_t* aux = halo + Cfg::HALO_BYTES;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
-  uint64_t* tfull_bar = empty_bar + Cfg::STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tfull_bar + 1);
+  uint64_t* halo_full = empty_bar + Cfg::STAGES;
+  uint64_t* halo_empty = halo_full + 1;
   float* s_stats = reinterpret_cast<float*>(aux + 1024);             // [4 warps][BN][2]
   float4* s_coef = reinterpret_cast<float4*>(aux + 1024 + 4 * BN * 8);   // [BN]
 
@@ -71,54 +93,59 @@ __global__ void __launch_bounds__(192) k_igemm_conv(const __grid_constant__ Conv
   const int w0 = wt * p.tw, h0 = ht * p.th, d0 = dt * p.td;
   const int n0 = blockIdx.y * BN;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     tma_prefetch_desc(&maps.a[0][0]);
     tma_prefetch_desc(&maps.b[0][0]);
+    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 4); }
+    mbar_init(halo_full, 1);
+    mbar_init(halo_empty, 4);
+    fence_barrier_init();
   }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-      mbar_init(tfull_bar, 1);
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc(tmem_slot, p.cls_mode ? (8 * BN < 32 ? 32 : 8 * BN) : Cfg::TMEM_COLS);   // class mode: one accumulator per parity class
-    tmem_relinquish();
-  }
-  pdl_wait();   // before the first global read (the coefficient table below); barrier init / TMEM allocation above overlap the previous kernel
-  if (warp >= 2) {
-    const int e = threadIdx.x - 64;
+  pdl_wait();   // before the first global read (the coefficient table below); the barrier set-up above overlaps the previous kernel
+  if (warp < 4) {
+    const int e = threadIdx.x;
     for (int i = e; i < 4 * BN * 2; i += 128) s_stats[i] = 0.f;
     if (p.mode == 1) {
       for (int c = e; c < BN; c += 128)
         s_coef[c] = (n0 + c < p.Cout) ? p.coef[(long long)n * p.coef_ld + n0 + c] : make_float4(0.f, 0.f, 0.f, 0.f);
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_launch_dependents();
 
-  // class mode: ONE CTA computes all eight parity classes of its voxel tile (27 tap products walked class by class into
-  // eight TMEM accumulators, then eight tile stores).  One CTA per class spent most of its life in set-up: 32768 CTAs of
-  // 1-8 K steps each took 0.47 ms for the 32-channel level-0 gradient.
+  // class mode: ONE CTA computes all eight parity classes of its voxel tile (27 tap products walked class by class, each class
+  // drained by the epilogue before the next one starts).  One CTA per class would spend most of its life in set-up.
   int total_iters = (p.ntaps[0] * p.kchunks[0] + p.ntaps[1] * p.kchunks[1]) * p.npass;
   if (p.cls_mode) {
     total_iters = 0;
     for (int c = 0; c < 8; ++c) total_iters += (int)p.cls_n[c] * p.kchunks[0] * p.npass;
   }
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ------------------------------------------------------------------ TMA producer (convergent, one lane issues)
-    {
-      const uint32_t issue = elect_one() ? 1u : 0u;
-      int it = 0;
-      for (int src = 0; src < 2; ++src) {
-        const int nt = p.ntaps[src];
-        if (nt == 0) continue;
-        const int ks = p.ksz[src], pad = p.pad[src], sd = p.stride[src];
-        for (int cls = 0; cls < (p.cls_mode ? 8 : 1); ++cls) {
+    const uint32_t issue = elect_one() ? 1u : 0u;
+    int it = 0;
+    for (int src = 0; src < 2; ++src) {
+      const int nt = p.ntaps[src];
+      if (nt == 0) continue;
+      const int ks = p.ksz[src], pad = p.pad[src], sd = p.stride[src];
+      if (MODE == CONV_HALO && src == 0) {
+        // one halo box per K chunk (its zero padding = TMA out-of-bounds fill), then the 27 taps' weight tiles
+        for (int kc = 0; kc < p.kchunks[0]; ++kc) {
+          mbar_wait(halo_empty, (kc & 1) ^ 1);
+          mbar_expect_tx_if(issue, halo_full, Cfg::HALO_TX);
+          tma_load_5d_if(issue, halo, &maps.a[0][0], halo_full, kc * KC, w0 - 1, h0 - 1, d0 - 1, n);
+          for (int tap = 0; tap < 27; ++tap) {
+            const int s = it % Cfg::STAGES;
+            mbar_wait(&empty_bar[s], ((it / Cfg::STAGES) & 1) ^ 1);
+            mbar_expect_tx_if(issue, &full_bar[s], Cfg::B_BOX_BYTES);
+            tma_load_3d_if(issue, smem + s * Cfg::STAGE_BYTES + Cfg::A_BYTES, &maps.b[0][0], &full_bar[s], kc * KC, n0, tap);
+            ++it;
+          }
+        }
+        continue;
+      }
+      for (int cls = 0; cls < (p.cls_mode ? 8 : 1); ++cls) {
         const int ntap_loop = p.cls_mode ? (int)p.cls_n[cls] : nt;
         for (int ti = 0; ti < ntap_loop; ++ti) {
           int tap = ti, cw, ch, cd;
@@ -143,107 +170,144 @@ __global__ void __launch_bounds__(192) k_igemm_conv(const __grid_constant__ Conv
             }
           }
         }
-        }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (convergent, one lane issues)
-    {
-      constexpr uint32_t idesc = make_idesc_bf16(128, BN, 0, 0);
-      constexpr uint32_t hi_d = desc_hi(Cfg::SBO, Cfg::LAYOUT);
-      const uint32_t tmem0 = __shfl_sync(0xffffffffu, tmem_base, 0);
-      const uint32_t smem0 = smem_u32(smem);
-      // class mode: iterations [cls_end[c-1], cls_end[c]) accumulate into accumulator c (TMEM columns c * BN ...)
-      int cur_cls = 0, cls_end = p.cls_mode ? (int)p.cls_n[0] * p.kchunks[0] * p.npass : total_iters, cls_first = 0;
-      for (int it = 0; it < total_iters; ++it) {
-        while (it >= cls_end) { ++cur_cls; cls_first = it; cls_end += (int)p.cls_n[cur_cls] * p.kchunks[0] * p.npass; }
-        const int s = it % Cfg::STAGES;
-        const uint32_t ph = (it / Cfg::STAGES) & 1;
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after();
-        const uint32_t a_lo = desc_lo(smem0 + s * Cfg::STAGE_BYTES, 16);
-        const uint32_t b_lo = desc_lo(smem0 + s * Cfg::STAGE_BYTES + Cfg::A_BYTES, 16);
-        const uint32_t acc = tmem0 + cur_cls * BN;
-        if (elect_one()) {   // one elected lane issues the stage (descriptors stay in uniform registers)
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumer warpgroup: wgmma, then the epilogue
+  // M = 128 output voxels as two m64 halves (rows 0-63 / 64-127 of the A tile), N = BN, K = 16 per instruction.
+  constexpr uint32_t hi_d = desc_hi(Cfg::SBO, Cfg::LAYOUT);
+  constexpr uint32_t HALF_M = (64 * KC * 2) >> 4;   // descriptor offset of A row 64
+  const uint32_t smem0 = smem_u32(smem);
+  const int row = threadIdx.x;
+  const int wl = row % p.tw, hl = (row / p.tw) % p.th, dl = row / (p.tw * p.th);
+  const int w = w0 + wl, h = h0 + hl, d = d0 + dl;
+  const bool valid = (w < p.Wo) && (h < p.Ho) && (d < p.Do);
+  const bool want_stats = (p.mode == 0) ? (p.stats != nullptr) : (p.bstats != nullptr);
+  const bool edge = p.zero_last && (w == p.Wo - 1 || h == p.Ho - 1 || d == p.Do - 1);
+  const bool split = p.out_lo != nullptr;
+  constexpr int CBO = BN < 64 ? BN : 64;
+  constexpr int SROWS_BOX = 128 * CBO * 2;
+  // side inputs (residual) are indexed in the OUTPUT tensor: in class mode that is voxel 2j + p of a 2x grid
+  auto vox_of = [&](int cls) -> long long {
+    return p.cls_mode
+        ? (((long long)n * (2 * p.Do) + 2 * d + ((cls >> 2) & 1)) * (2 * p.Ho) + 2 * h + ((cls >> 1) & 1)) * (2 * p.Wo) + 2 * w + (cls & 1)
+        : (((long long)n * p.Do + d) * p.Ho + h) * p.Wo + w;
+  };
+  for (int cls = 0; cls < (p.cls_mode ? 8 : 1); ++cls) conv_epilogue_prefetch(p, n0, BN, vox_of(cls), valid);   // -> L2 while the MMAs run
+
+  float acc[2][BN / 2];
 #pragma unroll
-          for (int k = 0; k < KC / 16; ++k)
-            umma_bf16(acc, desc_from(a_lo + 2 * k, hi_d), desc_from(b_lo + 2 * k, hi_d), idesc, (it > cls_first || k > 0) ? 1u : 0u);
-          umma_commit(&empty_bar[s]);
-          if (it == total_iters - 1) umma_commit(tfull_bar);
+  for (int i = 0; i < BN / 2; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+  // halo mode: the halo box holds rows ((dz * 18) + hy) * 10 + wx; output row r = h * 8 + w of tap (kd, kh, kw) reads halo row
+  // (kd * 18 + h + kh) * 10 + w + kw, so each 8-row group (one h) is 8 consecutive halo rows and the next group starts one halo
+  // row of 10 voxels further (SBO).  The descriptors start at arbitrary row offsets inside the swizzled box: the swizzle is a
+  // function of the absolute shared-memory address, for the TMA writes and for the wgmma reads alike.
+  constexpr uint32_t hi_halo = desc_hi(10 * Cfg::RB, Cfg::LAYOUT);
+  const uint32_t halo_lo0 = desc_lo(smem_u32(halo), 16);
+  const int halo_iters = MODE == CONV_HALO ? 27 * p.kchunks[0] : 0;
+  int it = 0;
+  for (int cls = 0; cls < (p.cls_mode ? 8 : 1); ++cls) {
+    const int n_it = p.cls_mode ? (int)p.cls_n[cls] * p.kchunks[0] * p.npass : total_iters;
+    int prev = -1;   // ring slot whose MMAs may still be reading it
+    for (int i = 0; i < n_it; ++i, ++it) {
+      const int s = it % Cfg::STAGES;
+      const bool from_halo = i < halo_iters;
+      const int tap = i % 27;
+      if (from_halo && tap == 0) mbar_wait(halo_full, (i / 27) & 1);
+      mbar_wait(&full_bar[s], (it / Cfg::STAGES) & 1);
+      uint32_t a_lo = desc_lo(smem0 + s * Cfg::STAGE_BYTES, 16), a_hi = hi_d, a_half = HALF_M;
+      if (MODE == CONV_HALO && from_halo) {
+        const int kd = tap / 9, kh = (tap / 3) % 3, kw = tap % 3;
+        a_lo = halo_lo0 + (((kd * 180 + kh * 10 + kw) * Cfg::RB) >> 4);
+        a_hi = hi_halo;
+        a_half = (80 * Cfg::RB) >> 4;   // rows 64-127 = h 8..15
+      }
+      const uint32_t b_lo = desc_lo(smem0 + s * Cfg::STAGE_BYTES + Cfg::A_BYTES, 16);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < KC / 16; ++k) {
+        const uint32_t accumulate = (i > 0 || k > 0) ? 1u : 0u;   // the first K step of a class overwrites the accumulator
+        Wgmma<BN>::template mma<0, 0>(acc[0], desc_from(a_lo + 2 * k, a_hi), desc_from(b_lo + 2 * k, hi_d), accumulate);
+        Wgmma<BN>::template mma<0, 0>(acc[1], desc_from(a_lo + a_half + 2 * k, a_hi), desc_from(b_lo + 2 * k, hi_d), accumulate);
+      }
+      wgmma_commit();
+      if (from_halo && tap == 26) {
+        // last tap of a halo box: the producer can load the next chunk's box only once every MMA reading this one is done,
+        // and the next MMA needs that box -- so drain here instead of deferring the hand-back by one stage
+        wgmma_wait<0>();
+        if (lane == 0) {
+          if (prev >= 0) mbar_arrive(&empty_bar[prev]);
+          mbar_arrive(&empty_bar[s]);
+          mbar_arrive(halo_empty);
         }
-        __syncwarp();
+        prev = -1;
+      } else {
+        wgmma_wait<1>();   // the previous stage's MMAs are complete: hand its slot back to the producer
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = s;
       }
     }
-  } else {
-    // ------------------------------------------------------------------ epilogue (4 warps = 128 TMEM lanes)
-    const int lane_base = (warp & 3) * 32;
-    const int row = lane_base + lane;
-    const int wl = row % p.tw, hl = (row / p.tw) % p.th, dl = row / (p.tw * p.th);
-    const int w = w0 + wl, h = h0 + hl, d = d0 + dl;
-    const bool valid = (w < p.Wo) && (h < p.Ho) && (d < p.Do);
-    const bool want_stats = (p.mode == 0) ? (p.stats != nullptr) : (p.bstats != nullptr);
-    const bool edge = p.zero_last && (w == p.Wo - 1 || h == p.Ho - 1 || d == p.Do - 1);
-    const bool split = p.out_lo != nullptr;
-    constexpr int CBO = BN < 64 ? BN : 64;
-    // side inputs (residual) are indexed in the OUTPUT tensor: in class mode that is voxel 2j + p of a 2x grid
-    auto vox_of = [&](int cls) -> long long {
-      return p.cls_mode
-          ? (((long long)n * (2 * p.Do) + 2 * d + ((cls >> 2) & 1)) * (2 * p.Ho) + 2 * h + ((cls >> 1) & 1)) * (2 * p.Wo) + 2 * w + (cls & 1)
-          : (((long long)n * p.Do + d) * p.Ho + h) * p.Wo + w;
-    };
-    for (int cls = 0; cls < (p.cls_mode ? 8 : 1); ++cls) conv_epilogue_prefetch(p, n0, BN, vox_of(cls), valid);   // -> L2 while the MMAs run
-    for (int cls = 0; cls < (p.cls_mode ? 8 : 1); ++cls) {
-      const long long vox = vox_of(cls);
-      // cls_pair: classes (pd, ph, 0) and (pd, ph, 1) interleave along W in ONE staging tile of 256 rows (row = output voxel
-      // (dl, hl, 2 wl + pw) of a box 2 tw wide) that is stored through the dense class-pair map after the second drain
-      const bool pair = p.cls_pair != 0, pair_first = pair && (cls & 1) == 0, pair_second = pair && (cls & 1) == 1;
-      if (cls == 0) {
-        asm volatile("bar.sync 1, 128;" ::: "memory");  // s_stats / s_coef initialised
-        mbar_wait(tfull_bar, 0);
-        tc_fence_after();
-      } else if (!pair_second) {
-        if (threadIdx.x == 64) tma_store_wait_read0();    // the previous stores have read the staging tile
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-      }
-      const int srow = pair ? (dl * p.th + hl) * (2 * p.tw) + 2 * wl + (cls & 1) : row;
-      constexpr int SROWS_BOX = 128 * CBO * 2;
-      // all MMAs have completed (tfull) => every pipeline stage has been consumed: the stage memory is free and is reused
-      // as the output staging tile [BN/CBO boxes][128 (pair: 256) rows][CBO] (+ lo tile), TMA-stored below
-      conv_epilogue_tile<BN>(p, tmem_base + cls * BN, lane_base, lane, n, n0, vox, valid, s_stats, s_coef, want_stats, edge, smem, srow, split);
-      if (pair_first) continue;     // the other W parity fills the odd rows of the same tile
-      fence_proxy_async();
-      tc_fence_before();
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (threadIdx.x == 64) {
-        if (pair) {
-          tma_store_5d(&cmaps.oc[cls & 6][0], smem, n0, 2 * w0, h0, d0, n);
-        } else {
-          const CUtensorMap* mo_hi = p.cls_mode ? &cmaps.oc[cls][0] : &maps.o[0];
-          const CUtensorMap* mo_lo = p.cls_mode ? &cmaps.oc[cls][1] : &maps.o[1];
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc[0]);
+    wgmma_fence_regs(acc[1]);
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+
+    // accumulator fragments -> s_acc (row-major), so that each thread drains one output voxel row below
+    const bool pair = p.cls_pair != 0, pair_first = pair && (cls & 1) == 0, pair_second = pair && (cls & 1) == 1;
+    if (cls > 0) {
+      if (!pair_second && threadIdx.x == 0) tma_store_wait_read0();    // the previous stores have read the staging tile
+      asm volatile("bar.sync 1, 128;" ::: "memory");                   // and every thread has read its s_acc row
+    }
 #pragma unroll
-          for (int cb = 0; cb < BN / CBO; ++cb) {
-            if (n0 + cb * CBO < p.Cout) {
-              tma_store_5d(mo_hi, smem + cb * SROWS_BOX, n0 + cb * CBO, w0, h0, d0, n);
-              if (split) tma_store_5d(mo_lo, smem + 128 * BN * 2 + cb * SROWS_BOX, n0 + cb * CBO, w0, h0, d0, n);
-            }
+    for (int hm = 0; hm < 2; ++hm) {
+      const int r0 = hm * 64 + warp * 16 + (lane >> 2);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = j * 8 + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(s_acc + r0 * Cfg::ACC_LD + c) = make_float2(acc[hm][4 * j], acc[hm][4 * j + 1]);
+        *reinterpret_cast<float2*>(s_acc + (r0 + 8) * Cfg::ACC_LD + c) = make_float2(acc[hm][4 * j + 2], acc[hm][4 * j + 3]);
+      }
+    }
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+
+    const long long vox = vox_of(cls);
+    // cls_pair: classes (pd, ph, 0) and (pd, ph, 1) interleave along W in ONE staging tile of 256 rows (row = output voxel
+    // (dl, hl, 2 wl + pw) of a box 2 tw wide) that is stored through the dense class-pair map after the second drain
+    const int srow = pair ? (dl * p.th + hl) * (2 * p.tw) + 2 * wl + (cls & 1) : row;
+    conv_epilogue_tile<BN>(p, s_acc + row * Cfg::ACC_LD, warp, lane, n, n0, vox, valid, s_stats, s_coef, want_stats, edge, stage_out,
+                           srow, split);
+    if (pair_first) continue;     // the other W parity fills the odd rows of the same tile
+    fence_proxy_async();
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    if (threadIdx.x == 0) {
+      if (pair) {
+        tma_store_5d(&cmaps.oc[cls & 6][0], stage_out, n0, 2 * w0, h0, d0, n);
+      } else {
+        const CUtensorMap* mo_hi = p.cls_mode ? &cmaps.oc[cls][0] : &maps.o[0];
+        const CUtensorMap* mo_lo = p.cls_mode ? &cmaps.oc[cls][1] : &maps.o[1];
+#pragma unroll
+        for (int cb = 0; cb < BN / CBO; ++cb) {
+          if (n0 + cb * CBO < p.Cout) {
+            tma_store_5d(mo_hi, stage_out + cb * SROWS_BOX, n0 + cb * CBO, w0, h0, d0, n);
+            if (split) tma_store_5d(mo_lo, stage_out + 128 * BN * 2 + cb * SROWS_BOX, n0 + cb * CBO, w0, h0, d0, n);
           }
         }
-        tma_store_commit();
       }
+      tma_store_commit();
     }
-    if (want_stats) {
-      const int e = threadIdx.x - 64;
-      double* dst = (p.mode == 0) ? p.stats : p.bstats;
-      const int ld = (p.mode == 0) ? p.stats_ld : p.coef_ld;
-      for (int c = e; c < BN * 2; c += 128) {
-        const float v = s_stats[c] + s_stats[BN * 2 + c] + s_stats[2 * BN * 2 + c] + s_stats[3 * BN * 2 + c];
-        if (n0 + (c >> 1) < p.Cout) atomicAdd(&dst[((long long)n * ld + n0) * 2 + c], (double)v);
-      }
-    }
-    if (threadIdx.x == 64) tma_store_wait_all();   // the staging tile must outlive the bulk store
   }
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, p.cls_mode ? (8 * BN < 32 ? 32 : 8 * BN) : Cfg::TMEM_COLS);
+  if (want_stats) {
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    double* dst = (p.mode == 0) ? p.stats : p.bstats;
+    const int ld = (p.mode == 0) ? p.stats_ld : p.coef_ld;
+    for (int c = threadIdx.x; c < BN * 2; c += 128) {
+      const float v = s_stats[c] + s_stats[BN * 2 + c] + s_stats[2 * BN * 2 + c] + s_stats[3 * BN * 2 + c];
+      if (n0 + (c >> 1) < p.Cout) atomicAdd(&dst[((long long)n * ld + n0) * 2 + c], (double)v);
+    }
+  }
+  if (threadIdx.x == 0) tma_store_wait_all();   // the staging tile must outlive the bulk store
 }
 
 // ----------------------------------------------------------------------------------------------- host side
@@ -255,43 +319,41 @@ static void pick_tile(int Wo, int Ho, int Do, int& tw, int& th, int& td) {
   td = rem / th;
 }
 
-template <int BN, int KC, int DEEP = 0>
+template <int BN, int KC, int MODE>
 static int launch_cfg(const ConvMaps& maps, const ConvArgs& args, dim3 grid, cudaStream_t st, const ConvClassMaps& cmaps) {
-  using Cfg = ConvCfg<BN, KC, DEEP>;
+  using Cfg = ConvCfg<BN, KC, MODE>;
   static bool attr_set[64] = {false};
   int dev = 0;
   B200_CHECK_CUDA(cudaGetDevice(&dev));
   if (dev < 64 && !attr_set[dev]) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(k_igemm_conv<BN, KC, DEEP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    B200_CHECK_CUDA(cudaFuncSetAttribute(k_igemm_conv<BN, KC, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::SMEM_BYTES));
     attr_set[dev] = true;
   }
-  launch_pdl(k_igemm_conv<BN, KC, DEEP>, grid, dim3(192), Cfg::SMEM_BYTES, st, maps, args, cmaps);
+  launch_pdl(k_igemm_conv<BN, KC, MODE>, grid, dim3(160), Cfg::SMEM_BYTES, st, maps, args, cmaps);
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;
 }
 
-static const int kIgemmDeepDefault = 1;   // measured: -12 % on the 256-channel 16^3 launches (profiles/r02_igemm_deep_ab.txt); B200UNET_IGEMM_DEEP=0 restores the 96 KB ring
-
-static int sm_count() {
-  static int cached[64] = {0};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev >= 64) return 148;
-  if (!cached[dev]) {
-    int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
-    cached[dev] = v;
-  }
-  return cached[dev];
+// Halo mode (see ConvMode) for 3x3x3 stride-1 convolutions (plus an optional fused 1x1x1 source) whose output planes fill the
+// 8 x 16 tile, in single-pass bf16.  Inputs wider than 64 channels take several halo boxes per tile, drained one after the other;
+// they stay on per-tap tiles unless voxels * Cout >= B200UNET_HALO_WIDE_MIN (tests set it to 0 to reach that path with
+// oracle-sized shapes; off by default: the forward category of the C2 step was slower with them in halo mode on the H100).  B200UNET_NO_HALO=1 keeps every launch on the per-tap kernel (A/B measurements).
+bool conv_halo_eligible(const ConvOp& op) {
+  static const bool off = getenv("B200UNET_NO_HALO") && atoi(getenv("B200UNET_NO_HALO")) != 0;
+  if (off || op.cls_mode) return false;
+  const ConvSrc& c = op.src[0];
+  if (c.ksz != 3 || c.stride != 1 || c.nopad) return false;
+  if (op.nsrc == 2 && (op.src[1].ksz != 1 || op.src[1].stride != 1)) return false;
+  for (int s = 0; s < op.nsrc; ++s)
+    if (op.src[s].x.lo || op.src[s].w_lo) return false;
+  long long wide_min = -1;
+  if (const char* e = getenv("B200UNET_HALO_WIDE_MIN")) wide_min = atoll(e);
+  if (c.x.C > 64 && (wide_min < 0 || (long long)op.out.N * op.out.D * op.out.H * op.out.W * op.out.C < wide_min)) return false;
+  return op.out.W >= 8 && op.out.H >= 16;
 }
 
 int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
-  static const bool no_halo = getenv("B200UNET_NO_HALO") != nullptr;
-  if (!no_halo && !op.cls_mode && (op.nsrc == 1 || op.nsrc == 2) && conv_halo_eligible(op)) return launch_conv_halo(op, sm_count(), st);
-  return launch_igemm_conv_streaming(op, st);
-}
-
-int launch_igemm_conv_streaming(const ConvOp& op, cudaStream_t st) {
   B200_REQUIRE(op.nsrc == 1 || op.nsrc == 2, E_INVALID, "igemm_conv: nsrc=%d", op.nsrc);
   const Act& out = op.out;
   B200_REQUIRE(out.C % 8 == 0 && out.ld % 8 == 0, E_UNSUPPORTED, "igemm_conv: Cout=%d (pitch %d) must be a multiple of 8",
@@ -331,9 +393,14 @@ int launch_igemm_conv_streaming(const ConvOp& op, cudaStream_t st) {
     for (int s = 0; s < op.nsrc; ++s)
       B200_REQUIRE(op.src[s].x.lo && op.src[s].w_lo, E_INVALID, "igemm_conv: split mode needs lo parts on every source");
   }
+  const bool halo = conv_halo_eligible(op);
+  if (halo) {   // one 8 x 16 output plane tile per CTA
+    a.tw = 8; a.th = 16; a.td = 1;
+    a.tiles_w = ceil_div(gW, a.tw); a.tiles_h = ceil_div(gH, a.th); a.tiles_d = gD;
+  }
   const int KC = cin_max > 32 ? 64 : cin_max > 16 ? 32 : 16;
   int BN = out.C > 64 ? 128 : out.C > 32 ? 64 : out.C > 16 ? 32 : 16;
-  if (op.cls_mode && BN > 64) BN = 64;   // eight accumulators of BN columns share the 512 TMEM columns
+  if (op.cls_mode && BN > 64) BN = 64;   // class mode keeps its staging tile beside the accumulator tile (ConvCfg)
   const Swz swz = swz_for_bytes(KC * 2);
   for (int s = 0; s < op.nsrc; ++s) {
     const ConvSrc& c = op.src[s];
@@ -348,6 +415,11 @@ int launch_igemm_conv_streaming(const ConvOp& op, cudaStream_t st) {
                             estride, swz, c.x.vD, c.x.vH, c.x.vW));
       B200_TRY(make_w_map(&maps.b[s][1], c.w_lo, a.ntaps[s], op.Cop, c.Cip, KC, BN, swz));
     }
+  }
+  if (halo) {
+    const ConvSrc& c = op.src[0];
+    B200_TRY(make_act_map(&maps.a[0][0], c.x.hi, c.x.N, c.x.D, c.x.H, c.x.W, c.x.C, c.x.ld, KC, 10, 18, 3, 1, swz, c.x.vD, c.x.vH,
+                          c.x.vW));
   }
   a.npass = split ? 3 : 1;
   a.mode = op.mode;
@@ -414,14 +486,16 @@ int launch_igemm_conv_streaming(const ConvOp& op, cudaStream_t st) {
     a.slope = op.slope; a.bstats = op.bstats;
   }
   dim3 grid((unsigned)((long long)a.N * a.tiles_d * a.tiles_h * a.tiles_w), (unsigned)ceil_div(out.C, BN), 1u);
-  // at most one CTA per SM: nothing is lost by taking the whole shared memory for a deeper ring (see ConvCfg); only the 64-channel
-  // K chunks have stages large enough for the 96 KB budget to cap the ring below six
-  static const int deep_env = getenv("B200UNET_IGEMM_DEEP") ? atoi(getenv("B200UNET_IGEMM_DEEP")) : kIgemmDeepDefault;
-  const bool deep = deep_env != 0 && !op.cls_mode && KC == 64 && (long long)grid.x * grid.y <= sm_count();
-  if (deep && BN == 128) return launch_cfg<128, 64, 1>(maps, a, grid, st, cmaps);
-  if (deep && BN == 64) return launch_cfg<64, 64, 1>(maps, a, grid, st, cmaps);
-#define B200_CONV_CASE(bn, kc) \
-  if (BN == bn && KC == kc) return launch_cfg<bn, kc>(maps, a, grid, st, cmaps);
+#define B200_CONV_CASE(bn, kc)                                                                                 \
+  if (BN == bn && KC == kc) {                                                                                  \
+    if (op.cls_mode) {                                                                                         \
+      if constexpr (bn <= 64) return launch_cfg<bn, kc, CONV_CLASS>(maps, a, grid, st, cmaps);                  \
+    } else if (halo) {                                                                                         \
+      return launch_cfg<bn, kc, CONV_HALO>(maps, a, grid, st, cmaps);                                          \
+    } else {                                                                                                   \
+      return launch_cfg<bn, kc, CONV_STREAM>(maps, a, grid, st, cmaps);                                        \
+    }                                                                                                          \
+  }
   B200_CONV_CASE(16, 16) B200_CONV_CASE(16, 32) B200_CONV_CASE(16, 64)
   B200_CONV_CASE(32, 16) B200_CONV_CASE(32, 32) B200_CONV_CASE(32, 64)
   B200_CONV_CASE(64, 16) B200_CONV_CASE(64, 32) B200_CONV_CASE(64, 64)

@@ -121,10 +121,8 @@ struct ConvOp {
                        // parity-class implicit GEMMs (27 tap products in total instead of 8 x 27) in one launch
 };
 
-int launch_igemm_conv(const ConvOp& op, cudaStream_t st);   // dispatcher: halo-resident kernel when eligible
-int launch_igemm_conv_streaming(const ConvOp& op, cudaStream_t st);
-bool conv_halo_eligible(const ConvOp& op);
-int launch_conv_halo(const ConvOp& op, int num_sms, cudaStream_t st);
+int launch_igemm_conv(const ConvOp& op, cudaStream_t st);
+bool conv_halo_eligible(const ConvOp& op);   // shape-only: does this convolution run in halo mode?
 
 // ---- tensor-core weight gradient (wgrad.cu):  dW[t][ci][co] += sum_v dy[v][co] * a[v*stride + t - pad][ci]
 struct WgradOp {
@@ -145,18 +143,8 @@ struct WgradOp {
 int launch_wgrad_reduce(const float* part, int splits, long long elems, float* dw, cudaStream_t st);   // dw = sum_s part[s]
 // worst-case bytes of the partial buffer for this shape on a device with num_sms SMs (host-only shape logic)
 size_t wgrad_partial_bytes(const WgradOp& op, int num_sms);
-int launch_wgrad(const WgradOp& op, cudaStream_t st);              // dispatcher: halo-resident kernel when eligible
-int launch_wgrad_streaming(const WgradOp& op, cudaStream_t st);
-bool wgrad_halo_eligible(const WgradOp& op);
+int launch_wgrad(const WgradOp& op, cudaStream_t st);              // dispatcher: SIMT register tile for narrow 1x1x1
 bool wgrad_1x1_narrow_eligible(const WgradOp& op);              // 1x1x1, <= 16 input channels: SIMT register tile
 int launch_wgrad_1x1_narrow(const WgradOp& op, cudaStream_t st);
-int launch_wgrad_halo(const WgradOp& op, int num_sms, cudaStream_t st);
-
-// ---- descriptor-semantics probe (probe.cu)
-// tests: host array [ntests][5] = (layout_mode 0:SW128 1:none, start_off_bytes, sbo_bytes, lbo_bytes, base_offset);
-// out: device float [ntests][2][128][64]  (encoding 0: A[r][k]=r, encoding 1: A[r][k]=k; B = identity) -> D[m][n]
-int launch_umma_probe(const int* tests, int ntests, float* out, cudaStream_t st);
-int launch_umma_rate(int N, int layout, int a_sbo, int b_sbo, int a_step, int inner, int reps, int ctas, long long* out,
-                     const void* copy_src, int copy_bytes, int commit_each_rep, cudaStream_t st);
 
 }  // namespace b200

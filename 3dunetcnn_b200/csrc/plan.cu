@@ -55,9 +55,8 @@ struct RunCtx {
   int part;            // backward only: -1 = the whole schedule; 0 / 1 = the part b200unet_plan_backward_part runs
 };
 
-// CAT_CONV_HALO: forward / data-gradient convolutions that run on the halo-resident kernel (conv_halo.cu); CAT_CONV_FWD and
-// CAT_CONV_DGRAD keep those of the streaming kernel (igemm_conv.cu), so that a per-kernel roofline can be reported
-enum Cat { CAT_CONV_FWD = 0, CAT_CONV_DGRAD, CAT_CONV_WGRAD, CAT_NORM, CAT_RESAMPLE, CAT_HEAD, CAT_PACK, CAT_OTHER, CAT_CONV_HALO, CAT_COUNT };
+// launch categories of the per-kernel profile (models.py _Plan.CATEGORIES names them in this order)
+enum Cat { CAT_CONV_FWD = 0, CAT_CONV_DGRAD, CAT_CONV_WGRAD, CAT_NORM, CAT_RESAMPLE, CAT_HEAD, CAT_PACK, CAT_OTHER, CAT_COUNT };
 
 struct Prof {
   std::vector<cudaEvent_t> ev;    // 2 per launch
@@ -133,7 +132,7 @@ struct b200unet_plan {
   size_t jobs_off = 0;                           // device copy: pack jobs then unpack jobs
   const void* jobs_uploaded_for = nullptr;       // workspace base the table was last uploaded into
   Prof* prof = nullptr;
-  double macs[CAT_COUNT] = {0, 0, 0, 0, 0, 0, 0, 0, 0};  // algorithmic MACs per forward+backward pass, by category
+  double macs[CAT_COUNT] = {0, 0, 0, 0, 0, 0, 0, 0};  // algorithmic MACs per forward+backward pass, by category
   size_t drop_off = 0;      // [N][base_width] floats: copy of the dropout scale of the last forward
   bool have_drop = false;
   bool deterministic = false;   // weight gradients: per-split partial sums + fixed-order reduction instead of fp32 atomics
@@ -299,20 +298,6 @@ static Act act_of(const Plan& P, const RunCtx& cx, TRef t) {
   return a;
 }
 
-// shape-only copy of the dispatch test (no pointers needed): does this convolution run on the halo-resident kernel?
-static bool goes_halo(const Plan& P, TRef a, int ksz, int stride, bool second_1x1, TRef out) {
-  const Buf& ab = P.bufs[a.buf];
-  const Buf& ob = P.bufs[out.buf];
-  ConvOp op;
-  memset(&op, 0, sizeof(op));
-  op.nsrc = second_1x1 ? 2 : 1;
-  op.src[0].x = make_act(nullptr, nullptr, ab.N, ab.D, ab.H, ab.W, a.c, ab.C);
-  op.src[0].ksz = ksz; op.src[0].stride = stride;
-  if (second_1x1) { op.src[1].ksz = 1; op.src[1].stride = 1; }
-  op.out = make_act(nullptr, nullptr, ob.N, ob.D, ob.H, ob.W, out.c, ob.C);
-  return conv_halo_eligible(op);
-}
-
 static void need_stats(Plan& P, int buf) {
   Buf& b = P.bufs[buf];
   if (b.stats_off >= 0) return;
@@ -402,7 +387,7 @@ static double conv_macs(const Plan& P, int ci, TRef out_like) {
 
 static void emit_conv_fwd(Plan& P, int ci, TRef a, int ci2, TRef a2, TRef res, TRef out, bool stats, bool scale) {
   if (stats) need_stats(P, out.buf);
- const int cat = goes_halo(P, a, P.convs[ci].ksz, P.convs[ci].stride, ci2 >= 0, out) ? CAT_CONV_HALO : CAT_CONV_FWD;
+  const int cat = CAT_CONV_FWD;
   P.macs[cat] += conv_macs(P, ci, out) + (ci2 >= 0 ? conv_macs(P, ci2, out) : 0.0);
   push_op(P.fwd, "conv_fwd " + P.convs[ci].name + " " + shape_of(P, a) + "->" + shape_of(P, out) + (ci2 >= 0 ? " +sample" : "") + (res.valid() ? " +res" : ""),
           [&P, ci, a, ci2, a2, res, out, stats, scale, cat](RunCtx& cx) -> int {
@@ -439,8 +424,8 @@ static int plan_num_sms() {
   int dev = 0, sms = 0;
   if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && sms > 0)
     return sms;
-  cudaGetLastError();   // planning on a host without a GPU: assume a B200
-  return 148;
+  cudaGetLastError();   // planning on a host without a GPU: assume an H100 SXM
+  return 132;
 }
 
 static void size_wgrad_partials(Plan& P, const Act& a, const Act& dy, int ksz, int stride, int nopad, int Cip, int Cop) {
@@ -493,7 +478,7 @@ static void emit_wgrad(Plan& P, int ci, TRef a, TRef dy) {
 // (ni >= 0, gn_x = raw input of the norm) or a plain epilogue (+res, *dropout scale).
 static void emit_dgrad(Plan& P, int ci, TRef dy, TRef out, int ni, TRef gn_x, TRef res, bool scale, double alg_macs,
                        bool cls_mode = false) {
-  const int cat = (!cls_mode && goes_halo(P, dy, P.convs[ci].ksz, P.convs[ci].transposed ? 2 : 1, false, out)) ? CAT_CONV_HALO : CAT_CONV_DGRAD;
+  const int cat = CAT_CONV_DGRAD;
   P.macs[cat] += alg_macs;
   push_op(P.bwd, std::string(ni >= 0 ? "dgrad+gnrelu " : "dgrad ") + P.convs[ci].name + " " + shape_of(P, dy) + "->" + shape_of(P, out),
           [&P, ci, dy, out, ni, gn_x, res, scale, cat, cls_mode](RunCtx& cx) -> int {

@@ -102,7 +102,7 @@ __global__ void k_tiles_normalize(float* __restrict__ out, const float* __restri
 
 static int grid_for(long long total, int block) {
   long long g = (total + block - 1) / block;
-  const long long cap = 148LL * 16;
+  const long long cap = 132LL * 16;
   return (int)(g < 1 ? 1 : g > cap ? cap : g);
 }
 
@@ -251,7 +251,7 @@ __global__ void k_zscore_apply(const float* __restrict__ x, long long S, int non
 int launch_zscore(const float* x, int groups, long long S, int nonzero, double* stats, float* y, cudaStream_t st) {
   B200_REQUIRE(x && y && stats && groups > 0 && S > 0, E_INVALID, "zscore: bad argument");
   B200_CHECK_CUDA(cudaMemsetAsync(stats, 0, sizeof(double) * 3 * groups, st));
-  int chunks = (148 * 8 + groups - 1) / groups;
+  int chunks = (132 * 8 + groups - 1) / groups;
   const long long per = (S + 1023) / 1024;
   if (chunks > per) chunks = (int)(per < 1 ? 1 : per);
   k_zscore_stats<<<dim3(chunks, groups), 256, 0, st>>>(x, S, nonzero, stats);

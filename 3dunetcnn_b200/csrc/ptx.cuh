@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_100a features the kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) and UMMA descriptors.
+// Thin inline-PTX wrappers for the sm_90a features the kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA) and its shared-memory descriptors.
 // Everything here is hand-written PTX; no CUTLASS/CuTe dependency.
 #pragma once
 #include <cstdint>
@@ -60,11 +60,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   const long long t0 = clock64();
   uint32_t n = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (((++n) & 0x3FFF) == 0 && clock64() - t0 > B200_SPIN_LIMIT_CYCLES) {
-      printf("b200unet: mbarrier wait timed out (block %d,%d,%d thread %d bar %u parity %u)\n", blockIdx.x, blockIdx.y,
-             blockIdx.z, threadIdx.x, smem_u32(bar), parity);
-      asm volatile("trap;");
-    }
+    // no printf here: a call inside the wgmma consumers' loop would make ptxas serialise every wgmma
+    if (((++n) & 0x3FFF) == 0 && clock64() - t0 > B200_SPIN_LIMIT_CYCLES) asm volatile("trap;");
   }
 }
 
@@ -99,7 +96,7 @@ __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk
 __device__ __forceinline__ void tma_store_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// predicated forms (see umma_bf16_if): convergent producer loops, one elected lane issues
+// predicated forms: convergent producer loops, one elected lane (elect_one(), evaluated once) issues
 __device__ __forceinline__ void mbar_expect_tx_if(uint32_t issue, uint64_t* bar, uint32_t bytes) {
   asm volatile(
       "{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\t"
@@ -116,14 +113,6 @@ __device__ __forceinline__ void tma_load_5d_if(uint32_t issue, void* smem_dst, c
       "r"(c3), "r"(c4), "r"(issue)
       : "memory");
 }
-// Side-effect-free request to pull one box of a tiled map into L2 (no shared-memory destination, no completion to wait for)
-__device__ __forceinline__ void tma_prefetch_l2_5d_if(uint32_t issue, const CUtensorMap* map, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %6, 0;\n\t"
-      "@q cp.async.bulk.prefetch.tensor.5d.L2.global.tile [%0, {%1, %2, %3, %4, %5}];\n\t}\n"
-      ::"l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4), "r"(issue)
-      : "memory");
-}
 __device__ __forceinline__ void tma_load_3d_if(uint32_t issue, void* smem_dst, const CUtensorMap* map, uint64_t* bar,
                                                int c0, int c1, int c2) {
   asm volatile(
@@ -134,130 +123,99 @@ __device__ __forceinline__ void tma_load_3d_if(uint32_t issue, void* smem_dst, c
       : "memory");
 }
 
-__device__ __forceinline__ void tma_load_4d_if(uint32_t issue, void* smem_dst, const CUtensorMap* map, uint64_t* bar,
-                                               int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %7, 0;\n\t"
-      "@q cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];\n\t}\n"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3),
-      "r"(issue)
-      : "memory");
-}
-
-// ----------------------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-// Programmatic dependent launch (common.cuh: launch_pdl).  pdl_wait: returns once the preceding kernel of the stream has completed
-// and its memory operations are visible (immediately when this grid was not launched with the attribute).
-// pdl_launch_dependents: this CTA no longer holds back the launch of the NEXT kernel; issued after the TMEM allocation so that a
-// dependent CTA that becomes resident beside this one can never take TMEM columns this CTA still has to allocate.
+// ----------------------------------------------------------------------------- programmatic dependent launch
+// (common.cuh: launch_pdl).  pdl_wait: returns once the preceding kernel of the stream has completed and its memory operations
+// are visible (immediately when this grid was not launched with the attribute).  pdl_launch_dependents: this CTA no longer
+// holds back the launch of the next kernel.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ----------------------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 operands from shared memory (descriptors), fp32 accumulator in the registers of
+// the four warps of a warpgroup.  Thread t of the warpgroup (warp w = t / 32, lane l) holds, for every 8-column block i,
+// d[4i + 0..1] = row 16w + l/4, columns 8i + 2(l%4) + {0, 1} and d[4i + 2..3] = the same columns of row 16w + l/4 + 8.
+// TA / TB = 1: the operand is MN-major (the contraction index is the slow axis of its shared-memory tile).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]; single thread issues.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Predicated forms for warp-convergent issue loops: every lane executes the (uniform) address arithmetic, only the
-// lane whose `issue` flag is set (elect_one(), evaluated once) issues.  Keeping the loop convergent lets ptxas hold
-// descriptors in uniform registers instead of emitting an ELECT / R2UR loop around every UTCHMMA.
-__device__ __forceinline__ void umma_bf16_if(uint32_t issue, uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "setp.ne.b32 q, %5, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(issue)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_if(uint32_t issue, uint64_t* bar) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\t"
-      "setp.ne.b32 q, %1, 0;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}\n"
-      ::"r"(smem_u32(bar)), "r"(issue)
-      : "memory");
-}
-// descriptor with a pre-encoded constant part: lo word = (addr >> 4) | (lbo >> 4) << 16 ; hi word constant
-__device__ __forceinline__ uint64_t desc_from(uint32_t lo, uint32_t hi) {
-  return (static_cast<uint64_t>(hi) << 32) | lo;
-}
+template <int N>
+struct Wgmma;
+template <>
+struct Wgmma<16> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void mma(float (&d)[8], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+  }
+};
+template <>
+struct Wgmma<32> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void mma(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+  }
+};
+template <>
+struct Wgmma<64> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void mma(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+  }
+};
+template <>
+struct Wgmma<128> {
+  template <int TA, int TB>
+  static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+  }
+};
+
+// ----------------------------------------------------------------------------- wgmma shared-memory descriptors
+//   bits [0,14)  start address >> 4        bits [16,30) leading-dim byte offset >> 4
+//   bits [32,46) stride-dim byte offset >> 4   bits [49,52) base offset   bits [62,64) layout: 0 none, 1 SW128, 2 SW64, 3 SW32
+// K-major swizzled tiles: SBO = bytes between 8-row groups (LBO unused); MN-major swizzled tiles: LBO = bytes between
+// swizzle atoms along M/N, SBO = bytes between 8-row groups along K.  A K step inside a swizzle atom adds its byte offset to the
+// start address (the hardware applies the swizzle on absolute address bits; tiles are 1024-byte aligned).
+enum : uint32_t { GMMA_SW_NONE = 0, GMMA_SW128 = 1, GMMA_SW64 = 2, GMMA_SW32 = 3 };
+
 __host__ __device__ constexpr uint32_t desc_hi(uint32_t sbo_bytes, uint32_t layout) {
-  return ((sbo_bytes >> 4) & 0x3FFF) | (1u << 14) | ((layout & 7u) << 29);
+  return ((sbo_bytes >> 4) & 0x3FFF) | ((layout & 3u) << 30);
 }
 __device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr, uint32_t lbo_bytes) {
   return ((smem_addr >> 4) & 0x3FFF) | (((lbo_bytes >> 4) & 0x3FFF) << 16);
 }
-
-// all previously issued MMAs of this thread -> arrive(1) on the mbarrier when complete
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+__device__ __forceinline__ uint64_t desc_from(uint32_t lo, uint32_t hi) {
+  return (static_cast<uint64_t>(hi) << 32) | lo;
 }
-// 32 lanes x 16 consecutive 32-bit columns: thread i of the warp gets lane (base+i), columns [col, col+16)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// 16 consecutive fp32 columns of this warp's 32 lanes <- 0 (accumulator initialisation without an overwriting MMA)
-__device__ __forceinline__ void tmem_zero16(uint32_t taddr) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1};"
-      ::"r"(taddr), "r"(0u)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ----------------------------------------------------------------------------- UMMA descriptors
-// Shared-memory matrix descriptor (PTX "matrix-descriptor", sm_100 version field = 1).
-//   bits [0,14)  start address >> 4        bits [16,30) leading-dim byte offset >> 4
-//   bits [32,46) stride-dim byte offset >> 4   bits [46,48) version = 1
-//   bits [49,52) base offset               bits [61,64) layout: 0 none, 2 SW128, 4 SW64, 6 SW32
-enum : uint32_t { UMMA_SW_NONE = 0, UMMA_SW128 = 2, UMMA_SW64 = 4, UMMA_SW32 = 6 };
-
-__host__ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                            uint32_t layout, uint32_t base_offset = 0) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(base_offset & 7) << 49;
-  d |= static_cast<uint64_t>(layout & 7) << 61;
-  return d;
-}
-
-// Instruction descriptor for kind::f16 with bf16 operands, fp32 accumulate.
-//   [4,6) c fmt (1 = f32)  [7,10) a fmt (1 = bf16)  [10,13) b fmt  [15] a major (1 = MN)  [16] b major
-//   [17,23) N >> 3   [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
+__host__ __device__ constexpr uint32_t swizzle_for_row_bytes(int bytes) {
+  return bytes >= 128 ? GMMA_SW128 : bytes >= 64 ? GMMA_SW64 : GMMA_SW32;
 }
 
 // ----------------------------------------------------------------------------- misc numeric helpers

@@ -1,5 +1,4 @@
-// Bandwidth-shaped rewrites of four small kernels that the round-1 per-launch timing (profiles/r01_final_layer_times.csv)
-// showed far from the HBM roofline:
+// Bandwidth-shaped rewrites of four small kernels that per-launch timing showed far from the HBM roofline:
 //   * weight packing / gradient unpacking: shared-memory tiled transposes (the straightforward gather read fp32 weights
 //     with a 108-byte stride between neighbouring threads)
 //   * trilinear x2 adjoint: the 4x4x4 neighbourhood of every output voxel comes from a shared-memory tile instead of 64
@@ -262,8 +261,7 @@ __global__ void __launch_bounds__(UD * UH * UW * (UCT / 8)) k_upsample2x_bwd_til
 }
 
 bool use_tiled_upsample_bwd() {
-  // measured on B200 (profiles/r02_layer_times_*.csv): 0.316 ms tiled vs 0.293 ms for the L1-cached gather version at
-  // 32ch 64^3 -> kept as an opt-in experiment
+  // slower than the L1-cached gather version where it was first measured -> kept as an opt-in experiment
   static const bool v = getenv("B200UNET_TILED_UPSAMPLE_BWD") != nullptr;
   return v;
 }
@@ -390,7 +388,7 @@ int launch_wgrad_1x1_narrow(const WgradOp& op, cudaStream_t st) {
   const int c8n = op.dy.C / 8;
   const int vper = 256 / c8n;
   const long long want = (op.a.voxels() + vper - 1) / vper;
-  const int blocks = (int)(want < 148 * 6 ? (want > 0 ? want : 1) : 148 * 6);
+  const int blocks = (int)(want < 132 * 6 ? (want > 0 ? want : 1) : 132 * 6);
   const size_t smem = (size_t)op.a.C * op.dy.C * sizeof(float);
   if (op.a.C == 8) k_wgrad_1x1_narrow<1><<<blocks, 256, smem, st>>>(op.a, op.dy, op.dw, op.Cop);
   else k_wgrad_1x1_narrow<2><<<blocks, 256, smem, st>>>(op.a, op.dy, op.dw, op.Cop);

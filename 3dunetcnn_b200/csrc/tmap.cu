@@ -107,23 +107,4 @@ int make_w_map(CUtensorMap* out, const bf16* ptr, int T, int R, int K, int boxK,
   return OK;
 }
 
-// Packed 3x3x3 weights [27 taps = kd*9 + khkw][R][K] viewed as (K, R, khkw = 9, kd = 3): one box (boxK, boxR, 1, 3) fetches
-// the kd = 0,1,2 tiles of one (kh,kw) back to back (the halo kernel stacks them along the MMA N dimension).
-int make_w_map_kd(CUtensorMap* out, const bf16* ptr, int R, int K, int boxK, int boxR, Swz swz) {
-  EncodeTiledFn enc = get_encode();
-  B200_REQUIRE(enc != nullptr, E_DRIVER, "cuTensorMapEncodeTiled not available (no CUDA driver?)");
-  B200_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, E_INVALID, "weight pointer not 16B aligned");
-  B200_REQUIRE((K * 2) % 16 == 0, E_INVALID, "packed weight K=%d not a multiple of 8", K);
-  cuuint64_t dims[4] = {(cuuint64_t)K, (cuuint64_t)R, 9, 3};
-  cuuint64_t strides[3] = {(cuuint64_t)K * 2, (cuuint64_t)R * K * 2, (cuuint64_t)9 * R * K * 2};
-  cuuint32_t box[4] = {(cuuint32_t)boxK, (cuuint32_t)boxR, 1, 3};
-  cuuint32_t es[4] = {1, 1, 1, 1};
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<bf16*>(ptr), dims, strides, box, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, to_cu(swz), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  B200_REQUIRE(r == CUDA_SUCCESS, E_DRIVER, "cuTensorMapEncodeTiled(w kd) failed: %d (R%d K%d box %d,%d swz%d)", (int)r, R, K,
-               boxK, boxR, (int)swz);
-  return OK;
-}
-
 }  // namespace b200

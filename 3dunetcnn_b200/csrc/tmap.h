@@ -22,13 +22,12 @@ int make_act_map_class(CUtensorMap* out, const bf16* ptr, int N, int D, int H, i
 
 // The two W-parity classes (pd, ph, 0) and (pd, ph, 1) together: logical dims (C, W, H/2, D/2, N) -- W dense, so that a store box
 // of 2 * boxW_class voxels per row writes whole 128-byte lines (64-byte pieces of single-class stores land in different lines:
-// the ncu capture of the level-0 stride-2 gradient showed one extra DRAM read of the whole output, profiles/r02_class_dgrad_ncu.txt).
+// a profile of the level-0 stride-2 gradient showed one extra DRAM read of the whole output).
 int make_act_map_classpair(CUtensorMap* out, const bf16* ptr, int N, int D, int H, int W, int C, int ld, int pd, int ph, int boxC,
                            int boxW, int boxH, int boxD, Swz swz);
 
 // 3-D map over packed weights [T][R][K] bf16 (K contiguous): dims (K, R, T); box (boxK, boxR, 1).
 int make_w_map(CUtensorMap* out, const bf16* ptr, int T, int R, int K, int boxK, int boxR, Swz swz, int boxT = 1);
-int make_w_map_kd(CUtensorMap* out, const bf16* ptr, int R, int K, int boxK, int boxR, Swz swz);
 
 static inline Swz swz_for_bytes(int bytes) { return bytes >= 128 ? SWZ_128 : bytes >= 64 ? SWZ_64 : SWZ_32; }
 

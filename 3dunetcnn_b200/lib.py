@@ -45,7 +45,7 @@ class NetDesc(C.Structure):
 
 
 def build_library(force: bool = False, verbose: bool = False) -> str:
-    """Compile libb200unet.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+    """Compile libb200unet.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
     if os.environ.get("B200UNET_LIB"):
         return LIB_PATH                       # an explicitly chosen variant is never rebuilt behind the caller's back
     if os.path.exists(LIB_PATH) and not force:
@@ -131,12 +131,10 @@ _SIGS = {
     "b200unet_plan_profile_dump": (C.c_int, [C.c_void_p, C.c_char_p]),
 }
 
-# diagnostics (include/b200unet_diag.h): hardware probes + SIMT cross-check, used by tools/ only
+# diagnostics (include/b200unet_diag.h): SIMT cross-check, used by tools/ only
 _DIAG_SIGS = {
     "b200unet_conv3d_simt": (C.c_int, [C.POINTER(Tensor5), C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                        C.POINTER(Tensor5), C.c_void_p]),
-    "b200unet_umma_rate": (C.c_int, [C.c_int] * 8 + [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
-    "b200unet_umma_probe": (C.c_int, [C.POINTER(C.c_int32), C.c_int, C.c_void_p, C.c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGS)
@@ -371,12 +369,3 @@ def dice_bwd(logits, target, flags, nr, dr, sums, grad_out, dlogits) -> None:
     check(load_library().b200unet_dice_bwd(logits.data_ptr(), target.data_ptr(), n, c, s, flags, nr, dr,
                                            sums.data_ptr(), grad_out.data_ptr(), dlogits.data_ptr(), stream_ptr()),
           "dice_bwd")
-
-
-def umma_probe(tests: Sequence[Sequence[int]]) -> torch.Tensor:
-    nt = len(tests)
-    arr = (C.c_int32 * (nt * 5))(*[int(v) for t in tests for v in t])
-    out = torch.zeros((nt, 2, 128, 64), dtype=torch.float32, device="cuda")
-    check(load_library().b200unet_umma_probe(arr, nt, out.data_ptr(), stream_ptr()), "umma_probe")
-    torch.cuda.synchronize()
-    return out

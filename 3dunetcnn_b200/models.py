@@ -7,7 +7,7 @@ Mirrors (paths relative to /root/reference):
 
 The module keeps canonical fp32 parameters under the reference's state-dict keys (so reference checkpoints load and
 checkpoints written here load into the reference), and runs forward/backward as ONE call each into libb200unet's
-whole-network plan (hand-written sm_100a kernels).  There is no PyTorch-op fallback: on a non-CUDA tensor, or if
+whole-network plan (hand-written sm_90a kernels).  There is no PyTorch-op fallback: on a non-CUDA tensor, or if
 the library is missing, ``forward`` raises.
 """
 from __future__ import annotations
@@ -81,11 +81,12 @@ class _Plan:
             return [0] * self.n_params
         return [int(self.lib.b200unet_plan_param_backward_part(self.handle, i)) for i in range(self.n_params)]
 
-    CATEGORIES = ("conv_fwd", "conv_dgrad", "conv_wgrad", "norm_act", "resample", "head", "weight_pack", "other", "conv_halo")
+    CATEGORIES = ("conv_fwd", "conv_dgrad", "conv_wgrad", "norm_act", "resample", "head", "weight_pack", "other")
 
     def algorithmic_macs(self):
-        arr = (C.c_double * 9)()
-        _lib.check(self.lib.b200unet_plan_algorithmic_macs(self.handle, arr, 9), "algorithmic_macs")
+        n = len(self.CATEGORIES)
+        arr = (C.c_double * n)()
+        _lib.check(self.lib.b200unet_plan_algorithmic_macs(self.handle, arr, n), "algorithmic_macs")
         return dict(zip(self.CATEGORIES, [float(v) for v in arr]))
 
     def profile_begin(self, max_launches: int) -> None:
@@ -95,9 +96,10 @@ class _Plan:
         _lib.check(self.lib.b200unet_plan_profile_dump(self.handle, path.encode()), "profile_dump")
 
     def profile_end(self):
-        ms = (C.c_double * 9)()
-        cnt = (C.c_int64 * 9)()
-        _lib.check(self.lib.b200unet_plan_profile_end(self.handle, ms, cnt, 9), "profile_end")
+        n = len(self.CATEGORIES)
+        ms = (C.c_double * n)()
+        cnt = (C.c_int64 * n)()
+        _lib.check(self.lib.b200unet_plan_profile_end(self.handle, ms, cnt, n), "profile_end")
         return {k: {"ms": float(m), "launches": int(c)} for k, m, c in zip(self.CATEGORIES, ms, cnt)}
 
     def __del__(self):
@@ -329,7 +331,7 @@ class _PlanModel(nn.Module):
 
 
 class UNet3D(_PlanModel):
-    """Drop-in for the reference ``UNet3D`` (same ctor kwargs, same state_dict), B200-native arithmetic.
+    """Drop-in for the reference ``UNet3D`` (same ctor kwargs, same state_dict), H100-native arithmetic.
 
     Extra kwarg ``precision``: ``"bf16"`` (default; single-pass bf16 tensor-core operands, fp32 accumulate) or
     ``"split"`` (hi/lo bf16 operand split, three MMAs per product: the parity mode that meets 1e-3 vs fp32).
@@ -651,7 +653,7 @@ def load_state_dict(model, state_dict, n_gpus, strict=False):
 
 
 def build_or_load_model(model_name, model_filename, n_gpus=0, strict=False, **kwargs):
-    """build.py:16-29.  ``n_gpus > 1`` in ONE process is the reference's DataParallel branch; the B200 path is one
+    """build.py:16-29.  ``n_gpus > 1`` in ONE process is the reference's DataParallel branch; this path is one
     process per GPU (see ``parallel.py``), so here every n_gpus >= 1 places the replica on the current device."""
     model = fetch_model_by_name(model_name, **kwargs)
     if n_gpus > 0:

@@ -67,8 +67,7 @@ class GraphedTrainStep:
     the ``.grad`` views of one persistent bucket, which ``grad_sync`` all-reduces in place.
 
     ``split_backward`` (default off; ``B200UNET_OVERLAP_ALLREDUCE=1`` turns it on wherever ``grad_sync`` can overlap, i.e. a
-    ``parallel.GradAllReduce`` with more than one rank -- measured neutral on two B200s, profiles/r02_overlap_ab.txt, so the
-    one-graph step stays the default): the step is captured as TWO graphs around the schedule's split point -- forward + loss +
+    ``parallel.GradAllReduce`` with more than one rank; the one-graph step stays the default): the step is captured as TWO graphs around the schedule's split point -- forward + loss +
     backward of head / decoder / deepest encoder level, then the backward of the shallow encoder levels.  Between the two
     replays ``grad_sync.begin()`` starts the all-reduce of the first ~90 % of the bucket on a side stream, so the exchange runs
     under the second graph; ``grad_sync.finish()`` reduces the small remainder (SURVEY.md 8e: bucketed, overlapped exchange; the
@@ -90,7 +89,7 @@ class GraphedTrainStep:
         self.loss = None
         self.warmup = int(warmup)
         self.device = device
-        # "global" (torch's default).  Measured on B200 / torch 2.11 (tools/graph_debug.py): "global" and "relaxed" capture the
+        # "global" (torch's default).  Observed with torch 2.11 (tools/graph_debug.py): "global" and "relaxed" capture the
         # step, "thread_local" does not -- autograd runs the backward of the step on its device worker thread, which may not
         # enqueue into a stream another thread is capturing in thread-local mode
         self.capture_error_mode = capture_error_mode
@@ -109,8 +108,8 @@ class GraphedTrainStep:
                 # No autograd graph of the warm-up may outlive this line.  While one is alive it keeps the parameters'
                 # AccumulateGrad nodes alive, and those remember the stream they were created on (this side stream); the
                 # captured backward would reuse them, autograd would synchronise the capturing stream with that
-                # non-capturing one, and the capture ends as cudaErrorStreamCaptureInvalidated (measured on B200 /
-                # torch 2.11 with tools/graph_debug2.py: 'replica' fails, 'del_loss' captures).
+                # non-capturing one, and the capture ends as cudaErrorStreamCaptureInvalidated (observed with
+                # torch 2.11 and tools/graph_debug2.py: 'replica' fails, 'del_loss' captures).
                 del loss
         torch.cuda.current_stream(self.device).wait_stream(side)
         torch.cuda.synchronize(self.device)

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- volumes/sec of the 3D U-Net hot path on B200.
+"""bench.py -- volumes/sec of the 3D U-Net hot path on an H100.
 
-  python bench.py --gpus N --steps K --warmup W [--config C2|C3|C5]     B200 arm (N>1: launched by torch.distributed.run)
+  python bench.py --gpus N --steps K --warmup W [--config C2|C3|C5] [--dump-outputs DIR]     GPU arm (N>1: torch.distributed.run)
   python bench.py --impl reference --gpus N --steps K ...               the reference's CPU implementation of the path
 
 Workloads (BASELINE.json `configs`): C2 (default, configs[1], the one `metric` is quoted on): 4-channel 128^3 volumes,
@@ -12,10 +12,15 @@ backward, [gradient all-reduce,] fused Adam.  C3 (configs[2]): the same at 160x1
 Prints ONE JSON line on rank 0.  `value`: inputs resident in HBM, CUDA-event timed, max over ranks; the step is replayed
 as a CUDA graph (train.GraphedTrainStep).  `e2e`: the same work through the reference-facing API
 (train.epoch_training(..., use_cuda_graph=True) / predict.volumetric_predictions) from pinned HOST buffers, H2D (and the
-result's D2H) inside the timed region.  `roofline`: the halo-resident implicit-GEMM convolution kernel k_conv_halo (the
-dominant kernel), algorithmic FLOPs / CUDA-event time summed over its launches against the measured bf16 peak.
+result's D2H) inside the timed region.  `roofline`: the implicit-GEMM convolution kernel k_igemm_conv (forward and data-gradient
+launches, the dominant kernel), algorithmic FLOPs / CUDA-event time summed over its launches against the bf16 peak.
 `cpu_baseline`: the oracle port of the reference model (torch CPU ops) on a bounded sample.  `cudnn_baseline`: the same
 op graph through torch/cuDNN under bf16 autocast on this GPU, timed in the same run (the bar SURVEY.md 8d names).
+
+--dump-outputs DIR: after the timed steps, what the last timed step computed is written as DIR/<name>.npy (float32 / float64):
+training configs the loss, a fixed seeded sample of the parameter gradients and of the parameters after the optimizer step;
+C5 a fixed seeded sample of the predicted volume.  Inputs and initial weights are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 import argparse
 import importlib
@@ -49,10 +54,8 @@ CONFIGS = {
                         "(27 tiles, 3 per forward) through predict.volumetric_predictions"),
 }
 
-# mean DRAM bytes per k_conv_halo launch in one C2 training step (ncu launch list under profiles/); refresh with
-# tools/gpu_trip_prof.sh + tools/summarize_ncu.py when the kernel or the dispatch changes
-NCU_TRAFFIC = {"bytes_per_launch": 339.6e6, "source": "profiles/r02_launches.txt (ncu dram__bytes_read.sum + dram__bytes_write.sum, "
-                                                      "mean over the kernel's launches of one C2 step)"}
+# elements of each sampled output array written by --dump-outputs (4 MB each in float32)
+DUMP_SAMPLE = 1 << 20
 
 
 def env_rank():
@@ -64,13 +67,14 @@ def measured_peaks():
     if os.path.exists(path):
         with open(path) as f:
             p = json.load(f)
-        return {"tflops": float(p.get("bf16_tflops_sustained", p.get("bf16_tflops", 1590.0))), "hbm_gbs": float(p.get("hbm_gbs", 6650.0)),
+        return {"tflops": float(p.get("bf16_tflops_sustained", p.get("bf16_tflops", 989.0))), "hbm_gbs": float(p.get("hbm_gbs", 3350.0)),
                 "source": "MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)"}
-    return {"tflops": 1590.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md): 1.59 PFLOP/s, 6.65 TB/s"}
+    return {"tflops": 989.0, "hbm_gbs": 3350.0,
+            "source": "NVIDIA H100 SXM data sheet (dense BF16 989 TFLOP/s, HBM3 3.35 TB/s at 700 W); not measured"}
 
 
 class ClockSampler:
-    """nvidia-smi sampling during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampling during the timed region (SM clock, power and throttle reasons beside the numbers)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -281,7 +285,21 @@ def cudnn_baseline(cfg, dev, steps=3):
     return out
 
 
-# ------------------------------------------------------------------------------------------------ B200 arm
+# ------------------------------------------------------------------------------------------------ GPU arm
+def sample(v):
+    """A fixed seeded sample of DUMP_SAMPLE elements of the flat tensor v (all of it when it is no larger)."""
+    if v.numel() <= DUMP_SAMPLE:
+        return v
+    idx = torch.randperm(v.numel(), generator=torch.Generator().manual_seed(1234))[:DUMP_SAMPLE].sort().values
+    return v[idx.to(v.device)]
+
+
+def dump_outputs(out_dir, arrays):
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, v in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), v.detach().cpu().numpy())
+
 class _Meta(torch.Tensor):
     """Minimal MetaTensor stand-in: volumetric_predictions requires ``.meta['filename_or_obj']`` (volumetric.py:11-51)."""
     meta = None
@@ -293,7 +311,7 @@ def run_b200_arm(args):
     rank, world, local = env_rank()
     cfg = CONFIGS[args.config]
     if not torch.cuda.is_available():
-        raise RuntimeError("bench.py: no CUDA device; the B200 arm has no CPU fallback")
+        raise RuntimeError("bench.py: no CUDA device; the GPU arm has no CPU fallback")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -347,11 +365,12 @@ def run_b200_arm(args):
                 use_graph = False
                 model._overwrite_grads = False
                 model.__dict__.pop("_graphed_steps", None)
+        last = {}
         if use_graph:
             overlapped = gstep.graph_tail is not None and world > 1
 
             def step_resident():
-                return gstep(x, t)
+                last["loss"] = gstep(x, t)
         else:
             model.use_flat_gradients(True)
 
@@ -361,13 +380,18 @@ def run_b200_arm(args):
                 loss.backward()
                 sync()
                 opt.step()
-                return loss
+                last["loss"] = loss
 
         for _ in range(warmup):
             step_resident()
         if rank == 0:
             sampler.start()
         ms_total = timed(step_resident, args.steps)
+        if args.dump_outputs and rank == 0:
+            grads = torch.cat([p.grad.detach().reshape(-1).float() for p in model.parameters()])
+            params = torch.cat([p.detach().reshape(-1).float() for p in model.parameters()])
+            dump_outputs(args.dump_outputs, {"loss": last["loss"].detach().double().reshape(1), "grad_sample": sample(grads),
+                                             "param_sample": sample(params)})
         plan = model._plan_for(x)
         launches_per_step = model.launches_last_forward + model.launches_last_backward + 3   # + Dice sums/finalize/bwd
 
@@ -402,14 +426,18 @@ def run_b200_arm(args):
         xh = torch.randn((batch, cfg["model"]["n_features"]) + cfg["volume"], generator=torch.Generator().manual_seed(100 + rank))
         x = xh.to(dev)
 
+        last = {}
+
         def step_resident():
             with torch.no_grad():
-                return inf(x, model)
+                last["pred"] = inf(x, model)
         for _ in range(warmup):
             step_resident()
         if rank == 0:
             sampler.start()
         ms_total = timed(step_resident, args.steps)
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, {"pred_sample": sample(last["pred"].reshape(-1).float())})
         tiles = torch.empty((cfg["sw_batch"], cfg["model"]["n_features"]) + cfg["roi"], device=dev)
         plan = model._plan_for(tiles, inference_only=True)
         n_fwd = 27 // cfg["sw_batch"]
@@ -458,11 +486,11 @@ def run_b200_arm(args):
     value = vols / (ms_total / 1e3)
     e2e_steps = args.steps
     e2e_value = vols_per_step * world * e2e_steps / (ms_e2e / 1e3)
-    conv_ms = prof["conv_halo"]["ms"]
-    conv_launches = prof["conv_halo"]["launches"]
-    conv_flops = 2.0 * macs["conv_halo"] * args.steps * reps
+    conv_ms = prof["conv_fwd"]["ms"] + prof["conv_dgrad"]["ms"]
+    conv_launches = prof["conv_fwd"]["launches"] + prof["conv_dgrad"]["launches"]
+    conv_flops = 2.0 * (macs["conv_fwd"] + macs["conv_dgrad"]) * args.steps * reps
     achieved = conv_flops / (conv_ms / 1e3) / 1e12 if conv_ms > 0 else 0.0
-    conv_keys = ("conv_halo", "conv_fwd", "conv_dgrad", "conv_wgrad")
+    conv_keys = ("conv_fwd", "conv_dgrad", "conv_wgrad")
     all_conv_ms = sum(prof[k]["ms"] for k in conv_keys)
     all_conv_flops = 2.0 * sum(macs[k] for k in conv_keys) * args.steps * reps
     kernels = {}
@@ -478,7 +506,7 @@ def run_b200_arm(args):
         "ms_per_step": ms_total / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "bf16" if args.precision == "bf16" else "bf16x3-split", "data": "synthetic",
         "config": {"workload": cfg["workload"], "global_batch": batch * world, "volume": list(cfg["volume"]), "parallelism": "dp%d" % world,
-                   "l2": "no flush: each step streams several GB of activations through HBM (>> 126 MB L2); every tensor is re-read from HBM",
+                   "l2": "no flush: each step streams several GB of activations through HBM (>> 50 MB L2); every tensor is re-read from HBM",
                    "step": ("CUDA-graph replay of forward+Dice+backward (train.GraphedTrainStep), eager fused Adam" if cfg["kind"] == "train" and use_graph
                             else "eager launches"),
                    "grad_sync": (("in-place NCCL all-reduce (AVG) of the flat gradient bucket in two slices: head/decoder/deepest-encoder gradients (~90 % of the "
@@ -488,9 +516,8 @@ def run_b200_arm(args):
         "e2e": {"value": e2e_value, "unit": UNIT, "ms_per_step": ms_e2e / e2e_steps, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h, "api": api},
         "gpu_launches": int(launches_per_step * args.steps),
         "clocks": clocks,
-        "roofline": {"bound": "tensor", "kernel": "k_conv_halo (halo-resident implicit-GEMM conv: forward + data-gradient launches)",
+        "roofline": {"bound": "tensor", "kernel": "k_igemm_conv (implicit-GEMM conv: forward + data-gradient launches)",
                      "achieved": achieved, "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": achieved / peaks["tflops"],
-                     "traffic": NCU_TRAFFIC["bytes_per_launch"] if args.config == "C2" else None, "traffic_source": NCU_TRAFFIC["source"],
                      "all_conv_kernels_tflops": all_conv_flops / (all_conv_ms / 1e3) / 1e12 if all_conv_ms > 0 else 0.0,
                      "launches_per_step": conv_launches / args.steps, "ms_per_step": conv_ms / args.steps,
                      "peak_source": peaks["source"],
@@ -524,6 +551,8 @@ def main():
     ap.add_argument("--precision", default="bf16", choices=["bf16", "split"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="eager launches instead of the CUDA-graph replayed step")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (a fixed seeded sample of large arrays)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference_arm(args)

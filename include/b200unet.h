@@ -1,4 +1,4 @@
-/* libb200unet -- C ABI of the B200-native 3D U-Net forward/backward hot path.
+/* libb200unet -- C ABI of the H100-native (sm_90a) 3D U-Net forward/backward hot path.
  *
  * The reference (ellisdg/3DUnetCNN) has no FFI: its extension seam is the Python name lookup
  * unet3d/models/build.py:9-13 (fetch_model_by_name) and unet3d/scripts/script_utils.py:61-77 (load_criterion).
@@ -58,7 +58,7 @@ int b200unet_unpack_wgrad(const float* g, int co, int ci, int cop, int cip, int 
                           void* stream);
 
 /* ---- convolution forward / data gradient: nn.Conv3d k{1,3} s{1,2} p=k/2, bias-free (resnet.py:12-22),
- * autograd's bwd-data when called with mode-1 packed weights.  Implicit GEMM on tcgen05 tensor cores. */
+ * autograd's bwd-data when called with mode-1 packed weights.  Implicit GEMM on wgmma tensor cores. */
 typedef struct b200unet_conv_desc {
   b200unet_tensor x[2];    /* A operands; x[1] only when nsrc == 2 (fused 1x1x1 `sample`, myronenko.py:42-45,53-54) */
   const void* w_hi[2];     /* packed weights per source */

@@ -1,8 +1,7 @@
 /* libb200unet diagnostics -- NOT part of the product ABI (include/b200unet.h).
  *
- * Hardware probes and a SIMT cross-check convolution used by tools/ (umma_rate.py, gpu_diag.py) while the kernels were
- * developed.  They live in the same shared object so that they see the same build flags, but nothing in the model /
- * training / inference path calls them.
+ * A SIMT cross-check convolution used by tools/gpu_diag.py while the kernels were developed.  It lives in the same shared
+ * object so that it sees the same build flags, but nothing in the model / training / inference path calls it.
  */
 #ifndef B200UNET_DIAG_H_
 #define B200UNET_DIAG_H_
@@ -15,16 +14,6 @@ extern "C" {
 /* ---- SIMT direct convolution on the same packed operands (cross-check only; not used by the model path) */
 int b200unet_conv3d_simt(const b200unet_tensor* x, const void* w_hi, const void* w_lo, int ksz, int stride,
                          const b200unet_tensor* y, void* stream);
-
-/* ---- tcgen05 shared-memory-descriptor probe (diagnostic; see profiles/ and DESIGN.md) */
-int b200unet_umma_probe(const int32_t* tests, int ntests, float* out, void* stream);
-/* tcgen05.mma issue-rate micro-benchmark (M=128, N=n, K=16): cycles for reps*inner MMAs per CTA -> out[cta].
- * copy_bytes > 0: a second warp streams bulk copies of copy_bytes (<= 32768, multiple of 16) from copy_src into
- * shared memory for the whole duration (operand-write pressure); bytes copied per CTA -> out[ctas + cta].
- * commit_each_rep: stage hand-back after every `inner` MMAs: bit 0 tcgen05.commit (to an unobserved mbarrier), bit 1 an
- * mbarrier wait that succeeds immediately, bit 2 tcgen05.fence::after_thread_sync. */
-int b200unet_umma_rate(int n, int layout, int a_sbo, int b_sbo, int a_step, int inner, int reps, int ctas, int64_t* out,
-                       const void* copy_src, int copy_bytes, int commit_each_rep, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,5 +1,5 @@
 """CPU restatement of ``monai.networks.nets.DynUNet`` (the model the reference's example configs train:
-examples/brats2020/brats2020_config.json:2-107) for the configuration subset the B200 path implements.
+examples/brats2020/brats2020_config.json:2-107) for the configuration subset the GPU path implements.
 TEST INFRASTRUCTURE ONLY (see ``oracle/__init__.py``).
 
 PARITY UNPINNED: MONAI is a third-party dependency that is not vendored under /root/reference and is not installed in this

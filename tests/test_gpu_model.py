@@ -1,4 +1,4 @@
-"""Whole-path parity on the GPU: the B200 UNet3D + fused Dice, called through the reference-facing module API
+"""Whole-path parity on the GPU: the GPU UNet3D + fused Dice, called through the reference-facing module API
 (which goes through the C-ABI plan), against (a) the committed golden fixtures produced by the unmodified
 reference, (b) the CPU oracle, and (c) size-independent properties at BASELINE.json's full 128^3 size.
 

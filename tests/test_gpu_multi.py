@@ -11,7 +11,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs on the box (run by tools/gpu_scale2_ab.sh: profiles/r02_overlap_ab.txt)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs on the box")
 def test_overlapped_exchange_matches_plain_exchange_over_nccl():
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
            "--master-port", str(29600 + os.getpid() % 300), os.path.join(ROOT, "tools", "ddp_check.py")]

@@ -1,8 +1,8 @@
 """Parity at the size BASELINE.json's north_star states it on: 4-channel 128^3 volumes, UNet3D base_width=32
-(/root/reference/unet3d/models/pytorch/segmentation/unet.py:47-50 driven as training_utils.py:101-112), against the CPU
+(reference unet3d/models/pytorch/segmentation/unet.py:47-50 driven as training_utils.py:101-112), against the CPU
 fp32 oracle ("the reference's own nn.Conv3d forward/backward").  At this size every production dispatch is active:
-the wide-input halo kernel (128->128@64^3, 256->256@32^3), TD=4 tiles, the streaming kernel on the 16^3 level, both
-weight-gradient kernels.  A C3-shaped crop (80 x 96 x 64: non-cubic tile walks, 10 x 12 x 8 at the bottleneck) is held
+halo mode of the convolution kernel in bf16 (incl. wide inputs: 128->128@64^3, 256->256@32^3), per-tap tiles in split
+precision and on the 16^3 level, the weight-gradient kernel.  A C3-shaped crop (80 x 96 x 64: non-cubic tile walks, 10 x 12 x 8 at the bottleneck) is held
 to the same bars.
 
 Tolerances (north_star): logits rel-L2 <= 1e-3 and |dDice| <= 1e-3 in `split` precision; every gradient norm within

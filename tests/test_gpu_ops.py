@@ -34,11 +34,11 @@ def _packed_to_torch(L, w, mode, split, cout, cin, ksz):
     (256, 256, (4, 4, 8), 3, 1), (24, 40, (5, 7, 9), 3, 1), (96, 192, (4, 4, 8), 3, 1), (64, 32, (8, 8, 8), 3, 1),
     (256, 128, (4, 4, 8), 1, 1), (8, 32, (6, 6, 6), 1, 1), (32, 32, (16, 16, 16), 3, 2), (64, 64, (8, 8, 8), 3, 2),
     (16, 16, (10, 6, 14), 3, 2),
-    # output plane >= 8 x 16 -> halo-resident kernel (conv_halo.cu); smaller planes -> streaming kernel (igemm_conv.cu)
+    # output plane >= 8 x 16 -> halo mode of igemm_conv.cu in bf16 (split precision and smaller planes: per-tap tiles)
     (32, 32, (8, 16, 16), 3, 1), (64, 32, (4, 16, 8), 3, 1), (8, 32, (16, 16, 16), 3, 1), (128, 128, (8, 16, 8), 3, 1),
     (256, 256, (2, 16, 8), 3, 1), (24, 40, (6, 18, 12), 3, 1), (96, 192, (3, 16, 8), 3, 1), (32, 64, (5, 24, 20), 3, 1),
     (16, 16, (1, 16, 8), 3, 1),
-    # 1x1x1 with a large output plane -> the halo kernel's centre-tap path
+    # 1x1x1 with a large output plane (per-tap tiles)
     (32, 64, (4, 16, 8), 1, 1), (8, 32, (5, 18, 12), 1, 1), (64, 32, (2, 16, 16), 1, 1), (24, 40, (3, 16, 9), 1, 1),
 ])
 def test_conv3d_forward(pkg, cin, cout, dims, ksz, stride, split):
@@ -65,9 +65,9 @@ def test_conv3d_forward(pkg, cin, cout, dims, ksz, stride, split):
     (128, 128, (5, 16, 16), "res"), (256, 256, (3, 16, 8), "res"),
 ])
 def test_conv3d_wide_inputs_on_halo_kernel(pkg, monkeypatch, cin, cout, dims, mode, split):
-    """Cin >= 128 on the halo kernel (64-channel output tiles: several N tiles per voxel tile, 3-8 K chunks per tile,
-    kd-stacked N = 192 MMAs).  In production that dispatch needs voxels * Cout >= 2^24; the threshold is lowered here so
-    that oracle-sized shapes reach it."""
+    """Cin >= 128 in halo mode (bf16; several N tiles per voxel tile, 2-4 halo boxes per tile).  That dispatch is off by
+    default and enabled here through B200UNET_HALO_WIDE_MIN so that it stays correct.  Split precision runs on per-tap
+    tiles."""
     monkeypatch.setenv("B200UNET_HALO_WIDE_MIN", "0")
     L = pkg.lib
     torch.manual_seed(cin * 3 + cout)
@@ -94,7 +94,7 @@ def test_conv3d_wide_inputs_on_halo_kernel(pkg, monkeypatch, cin, cout, dims, mo
 @pytest.mark.parametrize("split", [False, True])
 @pytest.mark.parametrize("ci,co,dims", [(128, 128, (4, 16, 8)), (192, 256, (2, 16, 16)), (128, 96, (5, 16, 8))])
 def test_conv3d_wide_inputs_on_halo_kernel_gn_backward_epilogue(pkg, monkeypatch, ci, co, dims, split):
-    """The same wide-input halo dispatch with the mode-1 (GroupNorm/ReLU backward) epilogue: the data gradient of a
+    """The same wide-input halo-mode dispatch with the mode-1 (GroupNorm/ReLU backward) epilogue: the data gradient of a
     co -> ci ... convolution seen from its output side, i.e. K = co >= 128 input channels of the GEMM."""
     monkeypatch.setenv("B200UNET_HALO_WIDE_MIN", "0")
     L = pkg.lib
@@ -129,7 +129,7 @@ def test_conv3d_wide_inputs_on_halo_kernel_gn_backward_epilogue(pkg, monkeypatch
 @pytest.mark.parametrize("cin,cout,r", [(32, 32, 64), (64, 64, 48), (64, 128, 32), (32, 64, 64), (128, 128, 32)])
 def test_conv3d_outputs_are_bitwise_repeatable(pkg, cin, cout, r):
     """Race detector: the stored activations involve no atomics, so repeated launches on identical inputs must agree
-    bit for bit (many persistent tiles per SM; a lost tcgen05 accumulate or a recycled staging buffer shows up here).
+    bit for bit (many persistent tiles per SM; a lost accumulate or a recycled staging buffer shows up here).
     Only the fp64 statistics may differ in the last bits (atomic order)."""
     L = pkg.lib
     torch.manual_seed(5)
@@ -180,7 +180,7 @@ def test_conv3d_fused_epilogue_residual_dropout_stats_concat_slice(pkg, split):
     per-channel statistics the next GroupNorm consumes."""
     L = pkg.lib
     torch.manual_seed(1)
-    n, ci, co, D = 2, 32, 32, 16          # 16^3: halo-resident kernel
+    n, ci, co, D = 2, 32, 32, 16          # 16^3: halo mode in bf16
     x = torch.randn(n, ci, D, D, D, device=DEV)
     w = torch.randn(co, ci, 3, 3, 3, device=DEV) / (ci * 27) ** 0.5
     r = torch.randn(n, co, D, D, D, device=DEV)
@@ -204,7 +204,7 @@ def test_conv3d_fused_epilogue_residual_dropout_stats_concat_slice(pkg, split):
 @pytest.mark.parametrize("D", [8, 16])
 def test_conv3d_two_sources_is_block_output(pkg, split, D):
     """conv2(a2) + sample(x): the residual block's second conv with the 1x1x1 `sample` as a second K-slab
-    (D=8: streaming kernel, D=16: halo-resident kernel)."""
+    (D=8: per-tap tiles, D=16: halo mode in bf16)."""
     L = pkg.lib
     torch.manual_seed(2)
     n, ci, co = 1, 8, 32
@@ -286,6 +286,8 @@ def test_stride2_data_gradient_by_parity_classes(pkg, ci, co, odims, with_res, s
     (8, 32, (8, 8, 16), 3, 1), (16, 16, (8, 8, 8), 3, 1), (64, 32, (8, 8, 8), 3, 1), (24, 40, (5, 7, 9), 3, 1),
     (96, 192, (4, 4, 8), 3, 1), (256, 128, (4, 4, 8), 1, 1), (8, 32, (8, 8, 8), 1, 1), (32, 32, (16, 16, 16), 3, 2),
     (64, 64, (8, 8, 8), 3, 2),
+    # 33..64 input channels with an output plane >= 8 x 16 -> halo mode of wgrad.cu in bf16
+    (64, 64, (4, 16, 8), 3, 1), (48, 32, (3, 18, 12), 3, 1), (40, 128, (2, 16, 16), 3, 1),
 ])
 def test_conv3d_weight_gradient(pkg, ci, co, dims, ksz, stride, split):
     L = pkg.lib

@@ -54,14 +54,24 @@ def test_state_dict_roundtrip_and_build_or_load(pkg, tmp_path):
     assert torch.equal(w[:, 2:], sd_small["encoder.layers.0.blocks.0.conv1.conv.weight"])
 
 
-@pytest.mark.skipif(not reference_available(), reason="reference tree not mounted (GPU box)")
-def test_checkpoint_interchange_with_reference(pkg):
+def test_checkpoint_interchange_with_reference(pkg, golden_dir):
+    """A reference checkpoint loads into this module and back: against the live class when the reference repository is
+    present, else against its state-dict spec stored by tests/golden/make_golden_live.py."""
+    import numpy as np
     kw = dict(n_features=4, n_outputs=3, base_width=8)
-    ref = reference_unet3d(**kw)
     mine = pkg.UNet3D(**kw)
-    mine.load_state_dict(ref.state_dict(), strict=True)           # reference checkpoint -> B200 module
-    ref.load_state_dict(mine.state_dict(), strict=True)           # and back
-    assert list(mine.state_dict()) == list(ref.state_dict())
+    if reference_available():
+        ref = reference_unet3d(**kw)
+        mine.load_state_dict(ref.state_dict(), strict=True)       # reference checkpoint -> this module
+        ref.load_state_dict(mine.state_dict(), strict=True)       # and back
+        assert list(mine.state_dict()) == list(ref.state_dict())
+        return
+    gold = np.load(os.path.join(golden_dir, "live_reference.npz"))
+    g = torch.Generator().manual_seed(0)
+    ref_sd = {str(k): torch.randn(eval(s), generator=g) for k, s in zip(gold["checkpoint_keys"], gold["checkpoint_shapes"])}
+    mine.load_state_dict(ref_sd, strict=True)
+    assert list(mine.state_dict()) == list(ref_sd)
+    assert all(torch.equal(mine.state_dict()[k], v) for k, v in ref_sd.items())
 
 
 def test_default_init_matches_torch_bounds(pkg):
@@ -137,8 +147,68 @@ def test_epoch_training_plumbing_cpu(pkg):
 
 
 # ------------------------------------------------------------------------------------------------ kernel index arithmetic
-# Executable restatement of the stacked-MMA bookkeeping of csrc/conv_halo.cu and csrc/wgrad_halo.cu: every (output plane,
-# kd tap) pair must be produced exactly once, into the accumulator columns the epilogue later reads.
+@pytest.mark.parametrize("KC", [16, 32, 64])
+def test_conv_halo_descriptor_rows_cover_the_tap_neighbourhood(KC):
+    """Halo mode of csrc/igemm_conv.cu: tap (kd, kh, kw) of output row r = h * 8 + w (8 x 16 tile) reads halo row
+    (kd * 18 + h + kh) * 10 + w + kw of the (KC, 10, 18, 3) box.  The descriptor starts at (kd * 180 + kh * 10 + kw) rows, each
+    8-row group (one h) is 8 consecutive halo rows, groups are SBO = 10 rows apart, and rows 64-127 start 80 rows further."""
+    rb = KC * 2
+    seen = set()
+    for tap in range(27):
+        kd, kh, kw = tap // 9, (tap // 3) % 3, tap % 3
+        start = (kd * 180 + kh * 10 + kw) * rb
+        assert start % 16 == 0 and (start >> 4) < (1 << 14)          # encodable descriptor start
+        for half in range(2):
+            for r in range(64):
+                row = half * 64 + r
+                h, w = row // 8, row % 8
+                addr = start + half * 80 * rb + (r // 8) * 10 * rb + (r % 8) * rb   # what the descriptor addresses
+                assert addr == ((kd * 18 + h + kh) * 10 + w + kw) * rb
+                assert addr + rb <= 540 * rb                                # inside the halo box
+                seen.add((tap, row))
+    assert len(seen) == 27 * 128
+
+
+def test_stride2_dgrad_parity_class_tap_lists():
+    """cls_mode 1 (igemm_conv.cu): dx[i] = sum_o sum_k dy[o] w[k] [2o + k - 1 == i].  With the flipped pack Wd[k'] = w[2 - k'],
+    class parity p lists (k', delta) with source index j + delta for output 2j + p; the 8 classes hold 27 tap products."""
+    import itertools
+    for p in (0, 1):
+        lst = [(k, 1 if k == 2 else 0) for k in range(3) if (k != 1 if p else k == 1)]
+        for j in range(1, 5):
+            i = 2 * j + p
+            direct = sorted((o, k) for o in range(0, 8) for k in range(3) if 2 * o + k - 1 == i)
+            via = sorted((j + delta, 2 - kp) for kp, delta in lst)      # (dy index, un-flipped w index)
+            assert direct == via
+    total = sum(len([k for k in range(3) if (k != 1 if pd else k == 1)]) * len([k for k in range(3) if (k != 1 if ph else k == 1)]) *
+                len([k for k in range(3) if (k != 1 if pw else k == 1)]) for pd, ph, pw in itertools.product((0, 1), repeat=3))
+    assert total == 27
+
+
+def test_transposed_conv_k2s2_roles():
+    """ConvTranspose3d(kernel = stride = 2): U[2j + p] = sum_ci X[j] W[ci][co][p] -> class p uses tap p (cls_mode 2); its data
+    gradient is the unpadded kernel-2 stride-2 convolution of dU and its weight gradient the same convolution's filter
+    gradient with roles swapped (checked numerically against torch in 1-D per axis)."""
+    import torch.nn.functional as F
+    torch.manual_seed(0)
+    x = torch.randn(1, 3, 5, dtype=torch.float64, requires_grad=True)
+    w = torch.randn(3, 4, 2, dtype=torch.float64, requires_grad=True)
+    u = F.conv_transpose1d(x, w, stride=2)
+    for p in (0, 1):
+        assert torch.allclose(u[0, :, p::2], torch.einsum("cj,co->oj", x[0], w[:, :, p]))
+    du = torch.randn_like(u)
+    u.backward(du)
+    dx = F.conv1d(du, w.permute(0, 1, 2).reshape(3, 4, 2), stride=2)          # V[p][ci][co] = w[ci][co][p], no padding
+    assert torch.allclose(dx, x.grad)
+    dw = torch.stack([torch.einsum("cj,oj->co", x[0].detach(), du[0, :, t::2]) for t in (0, 1)], dim=-1)
+    assert torch.allclose(dw, w.grad)
+
+
+# ------------------------------------------------------------------------------------------------ B200 halo-kernel bookkeeping
+# Restatements of the index arithmetic of the B200 halo kernels (kd-stacked tcgen05 MMAs of the convolution and the weight
+# gradient, incremental and three-box weight-stage offsets, multiply-high tile decode).  No sm_90a kernel uses this arithmetic:
+# the Hopper halo mode of csrc/igemm_conv.cu issues one tap per wgmma from directly computed row offsets (checked by
+# test_conv_halo_descriptor_rows_cover_the_tap_neighbourhood above).
 @pytest.mark.parametrize("TD", [1, 2, 4])
 def test_conv_halo_kd_stacking_covers_every_plane_tap_pair_once(TD):
     seen = {}
@@ -212,41 +282,6 @@ def test_conv_halo_kw_grouped_stage_offsets():
                 taps.add((kd, st, q, q * b_box + kd * 2048))    # B operand offset inside the stage
         a_off += 10 * rb
     assert len(taps) == 27 and len({t[3] for t in taps}) == 9   # 9 distinct tile offsets per stage x 3 stages
-
-
-def test_stride2_dgrad_parity_class_tap_lists():
-    """cls_mode 1 (igemm_conv.cu): dx[i] = sum_o sum_k dy[o] w[k] [2o + k - 1 == i].  With the flipped pack Wd[k'] = w[2 - k'],
-    class parity p lists (k', delta) with source index j + delta for output 2j + p; the 8 classes hold 27 tap products."""
-    import itertools
-    for p in (0, 1):
-        lst = [(k, 1 if k == 2 else 0) for k in range(3) if (k != 1 if p else k == 1)]
-        for j in range(1, 5):
-            i = 2 * j + p
-            direct = sorted((o, k) for o in range(0, 8) for k in range(3) if 2 * o + k - 1 == i)
-            via = sorted((j + delta, 2 - kp) for kp, delta in lst)      # (dy index, un-flipped w index)
-            assert direct == via
-    total = sum(len([k for k in range(3) if (k != 1 if pd else k == 1)]) * len([k for k in range(3) if (k != 1 if ph else k == 1)]) *
-                len([k for k in range(3) if (k != 1 if pw else k == 1)]) for pd, ph, pw in itertools.product((0, 1), repeat=3))
-    assert total == 27
-
-
-def test_transposed_conv_k2s2_roles():
-    """ConvTranspose3d(kernel = stride = 2): U[2j + p] = sum_ci X[j] W[ci][co][p] -> class p uses tap p (cls_mode 2); its data
-    gradient is the unpadded kernel-2 stride-2 convolution of dU and its weight gradient the same convolution's filter
-    gradient with roles swapped (checked numerically against torch in 1-D per axis)."""
-    import torch.nn.functional as F
-    torch.manual_seed(0)
-    x = torch.randn(1, 3, 5, dtype=torch.float64, requires_grad=True)
-    w = torch.randn(3, 4, 2, dtype=torch.float64, requires_grad=True)
-    u = F.conv_transpose1d(x, w, stride=2)
-    for p in (0, 1):
-        assert torch.allclose(u[0, :, p::2], torch.einsum("cj,co->oj", x[0], w[:, :, p]))
-    du = torch.randn_like(u)
-    u.backward(du)
-    dx = F.conv1d(du, w.permute(0, 1, 2).reshape(3, 4, 2), stride=2)          # V[p][ci][co] = w[ci][co][p], no padding
-    assert torch.allclose(dx, x.grad)
-    dw = torch.stack([torch.einsum("cj,oj->co", x[0].detach(), du[0, :, t::2]) for t in (0, 1)], dim=-1)
-    assert torch.allclose(dw, w.grad)
 
 
 def test_tile_decode_fast_division_restatement():

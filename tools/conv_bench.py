@@ -1,6 +1,5 @@
 """Per-layer micro-benchmark of the convolution kernels at the C2 layer shapes (batch 2): TFLOP/s per layer for
-forward (mode 0 + stats), the wgrad kernel, and optionally overrides via env (B200UNET_NO_HALO, B200UNET_HALO_TD,
-B200UNET_HALO_BN).  Usage: python tools/conv_bench.py [fwd|wgrad|all] [reps]"""
+forward (mode 0 + stats), the wgrad kernel; B200UNET_NO_HALO=1 keeps every convolution on the per-tap kernel (A/B).  Usage: python tools/conv_bench.py [fwd|wgrad|all] [reps]"""
 import importlib
 import json
 import os
@@ -36,7 +35,7 @@ def timeit(fn, reps):
 def main():
     what = sys.argv[1] if len(sys.argv) > 1 else "all"
     reps = int(sys.argv[2]) if len(sys.argv) > 2 else 10
-    tag = {k: os.environ.get(k) for k in ("B200UNET_NO_HALO", "B200UNET_HALO_TD", "B200UNET_HALO_BN") if os.environ.get(k)}
+    tag = {k: os.environ.get(k) for k in ("B200UNET_NO_HALO",) if os.environ.get(k)}
     tot_ms = {"fwd": 0.0, "wgrad": 0.0}
     tot_flop = 0.0
     for (ci, co, r) in SHAPES:

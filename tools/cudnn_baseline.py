@@ -1,5 +1,5 @@
 """The bar to meet: the reference model's op graph (oracle's functional restatement == the reference's nn.Module
-graph) executed by torch/cuDNN on the same B200: fp32 (TF32 off), and bf16 autocast (+channels_last_3d).
+graph) executed by torch/cuDNN on the same GPU: fp32 (TF32 off), and bf16 autocast (+channels_last_3d).
 Prints one JSON line per variant.  Not part of the product path."""
 import json
 import os

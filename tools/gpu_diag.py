@@ -1,6 +1,6 @@
 """On-GPU diagnostics: runs groups of kernel checks and prints error magnitudes (does not assert -- it is the
 bring-up tool; the pass/fail parity tests live in tests/).  Usage: python tools/gpu_diag.py <group> [...]
-Groups: probe elementwise conv wgrad model
+Groups: elementwise conv wgrad model
 References here are torch fp64 ops on the GPU (the pytest suite uses the CPU oracle)."""
 import importlib
 import json
@@ -48,40 +48,6 @@ def run(name, fn):
 
 def bf16r(x):
     return x.to(torch.bfloat16).float()
-
-
-# ---------------------------------------------------------------------------------------------- probe
-def group_probe():
-    tests = [
-        (0, 0, 1024, 0, 0),        # baseline SW128
-        (0, 128, 1024, 0, 0),      # start +1 row, base_offset 0
-        (0, 128, 1024, 0, 1),      # start +1 row, base_offset 1
-        (0, 384, 1024, 0, 0),      # +3 rows
-        (0, 384, 1024, 0, 3),
-        (0, 0, 1280, 0, 0),        # SBO = 10 rows
-        (0, 128, 1280, 0, 0),
-        (0, 128, 1280, 0, 1),
-        (0, 1024, 1024, 0, 0),     # +8 rows (aligned shift)
-        (0, 2048 + 256, 1280, 0, 0),
-        (1, 0, 128, 8192, 0),      # interleaved baseline
-        (1, 16, 128, 8192, 0),     # interleaved +1 row
-        (1, 0, 160, 8192, 0),      # interleaved SBO = 10 rows
-        (1, 48, 160, 8192, 0),
-    ]
-    out = L.umma_probe(tests).cpu()
-    m = torch.arange(128).view(128, 1).float()
-    n = torch.arange(64).view(1, 64).float()
-    for t, o in zip(tests, out):
-        mode, start, sbo, lbo, bo = t
-        rowbytes = 128 if mode == 0 else 16
-        exp_row = ((start // rowbytes) + (m % 8) + (m // 8) * (sbo // rowbytes)).expand(128, 64) % 256
-        exp_col = n.expand(128, 64)
-        ok_row = bool(torch.equal(o[0], exp_row))
-        ok_col = bool(torch.equal(o[1], exp_col))
-        frac_row = float((o[0] == exp_row).float().mean())
-        frac_col = float((o[1] == exp_col).float().mean())
-        report("probe mode%d start%d sbo%d lbo%d bo%d" % t, rows_ok=ok_row, cols_ok=ok_col, frac_row=frac_row,
-               frac_col=frac_col, sample_rows=str(o[0][:10, 0].int().tolist()), sample_cols=str(o[1][1, :10].int().tolist()))
 
 
 # ---------------------------------------------------------------------------------------------- elementwise
@@ -252,7 +218,7 @@ def group_conv():
         (96, 192, (4, 4, 8), 3, 1, False), (64, 128, (8, 8, 8), 1, 1, False), (256, 128, (4, 4, 8), 1, 1, False),
         (32, 32, (16, 16, 16), 3, 2, False), (64, 64, (8, 8, 8), 3, 2, False), (8, 8, (8, 8, 8), 3, 2, False),
         (32, 32, (5, 7, 9), 3, 1, False),
-        # halo-resident kernel (output plane >= 8 x 16)
+        # halo mode of the convolution kernel (output plane >= 8 x 16)
         (32, 32, (8, 16, 16), 3, 1, False), (64, 32, (4, 16, 8), 3, 1, False), (8, 32, (16, 16, 16), 3, 1, False),
         (128, 128, (8, 16, 8), 3, 1, False), (256, 256, (2, 16, 8), 3, 1, False), (24, 40, (6, 18, 12), 3, 1, False),
         (96, 192, (3, 16, 8), 3, 1, False), (32, 64, (5, 24, 20), 3, 1, False), (16, 16, (1, 16, 8), 3, 1, False),
@@ -431,7 +397,7 @@ def group_bench():
         run("bench %s" % (shape,), t)
 
 
-GROUPS = {"bench": group_bench, "probe": group_probe, "elementwise": group_elementwise, "conv": group_conv, "wgrad": group_wgrad,
+GROUPS = {"bench": group_bench, "elementwise": group_elementwise, "conv": group_conv, "wgrad": group_wgrad,
           "model": group_model}
 
 if __name__ == "__main__":
