@@ -1300,6 +1300,71 @@ __global__ void k_act_to_ncdhw(Act in, int C, float* __restrict__ y) {
   }
 }
 
+// ------------------------------------------------------------------------------------------------ network input gradient
+// dx[n][c][s] = (A dz + E x + F) + r  for the C real channels of the network input, in ONE pass from NDHWC bf16 (hi [+ lo])
+// to NCDHW fp32: the GroupNorm(+ReLU) backward of the first norm (dz is already masked by ReLU'; A from coef, (E, F) from the
+// coef2 gn_bwd_finalize left behind), the residual branch r (the `sample` data gradient or the identity gradient) and the
+// transpose.  dz.hi == nullptr switches the norm step off (dx = r).  A tile of kInputGradTile voxels is staged in shared
+// memory: the loads are 16-byte NDHWC vectors, the stores run along W (NCDHW), both coalesced.
+constexpr int kInputGradTile = 256;
+__global__ void __launch_bounds__(256) k_input_grad(Act dz, Act x, const float4* __restrict__ coef, const float2* __restrict__ coef2,
+                                                    int coef_ld, Act r, int C, float* __restrict__ dx) {
+  __shared__ float tile[16][kInputGradTile + 1];
+  __shared__ float s_a[16], s_e[16], s_f[16];
+  const int n = blockIdx.y;
+  const long long S = (long long)r.D * r.H * r.W;
+  const long long s0 = (long long)blockIdx.x * kInputGradTile;
+  const int c8n = (C + 7) / 8;
+  if (threadIdx.x < 16) {
+    const int c = threadIdx.x;
+    const bool on = dz.hi && c < C;
+    s_a[c] = on ? coef[(long long)n * coef_ld + c].x : 0.f;
+    s_e[c] = on ? coef2[(long long)n * coef_ld + c].x : 0.f;
+    s_f[c] = on ? coef2[(long long)n * coef_ld + c].y : 0.f;
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < kInputGradTile * c8n; t += blockDim.x) {
+    const int v = t / c8n, c8 = t % c8n;
+    const long long s = s0 + v;
+    if (s >= S) continue;
+    const long long vox = (long long)n * S + s;
+    float o[8];
+    load8(r.hi, r.lo, vox * r.ld + c8 * 8, o);
+    if (dz.hi) {
+      float g[8], xv[8];
+      load8(dz.hi, dz.lo, vox * dz.ld + c8 * 8, g);
+      load8(x.hi, x.lo, vox * x.ld + c8 * 8, xv);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int c = c8 * 8 + j;
+        o[j] = fmaf(s_a[c], g[j], fmaf(s_e[c], xv[j], s_f[c])) + o[j];   // the order of k_gn_bwd: norm term, then the residual
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) tile[c8 * 8 + j][v] = o[j];
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < kInputGradTile * C; t += blockDim.x) {
+    const int c = t / kInputGradTile, v = t % kInputGradTile;
+    const long long s = s0 + v;
+    if (s < S) dx[((long long)n * C + c) * S + s] = tile[c][v];
+  }
+}
+
+int launch_input_grad(const Act* dz, const Act* x, const float* coef, const float* coef2, int coef_ld, const Act& r, int C, float* dx,
+                      cudaStream_t st) {
+  B200_REQUIRE(C >= 1 && C <= 16 && r.C >= round_up(C, 8) && r.ld % 8 == 0, E_INVALID, "input_grad: C=%d, residual view %d/%d", C, r.C, r.ld);
+  B200_REQUIRE(!dz || (x && coef && coef2 && dz->C >= C && x->C >= C && coef_ld >= C), E_INVALID, "input_grad: norm operands");
+  Act none = make_act(nullptr, nullptr, 0, 0, 0, 0, 0, 0);
+  const long long S = (long long)r.D * r.H * r.W;
+  const long long tiles = (S + kInputGradTile - 1) / kInputGradTile;
+  B200_REQUIRE(tiles < (1LL << 31) && r.N <= 65535, E_UNSUPPORTED, "input_grad: extent too large");
+  k_input_grad<<<dim3((unsigned)tiles, r.N), 256, 0, st>>>(dz ? *dz : none, dz ? *x : none, reinterpret_cast<const float4*>(coef),
+                                                         reinterpret_cast<const float2*>(coef2), coef_ld, r, C, dx);
+  B200_CHECK_CUDA(cudaGetLastError());
+  return OK;
+}
+
 int launch_ncdhw_to_act(const float* x, int C, const Act& out, cudaStream_t st) {
   long long total = out.voxels() * (out.C / 8);
   k_ncdhw_to_act<<<ew_blocks(total, 256), 256, 0, st>>>(x, C, out);

@@ -58,6 +58,10 @@ int launch_bias_grad(const Act& dy, float* dbias, cudaStream_t st);   // dbias[c
 int launch_zero_insert(const Act& x, const Act& z, int od, int oh, int ow, cudaStream_t st);
 int launch_ncdhw_to_act(const float* x, int C, const Act& out, cudaStream_t st);
 int launch_act_to_ncdhw(const Act& in, int C, float* y, cudaStream_t st);
+// gradient of the network input, NCDHW fp32 [N][C][S]: dx = (A dz + E x + F) + r over the C real channels (coef [N][coef_ld][4],
+// coef2 [N][coef_ld][2] as left by the GroupNorm backward); dz == nullptr: dx = r (the layout transpose alone)
+int launch_input_grad(const Act* dz, const Act* x, const float* coef, const float* coef2, int coef_ld, const Act& r, int C, float* dx,
+                      cudaStream_t st);
 int launch_conv_simt(const Act& x, const bf16* whi, const bf16* wlo, int ksz, int stride, const Act& y,
                      cudaStream_t st);
 

@@ -47,6 +47,7 @@ struct RunCtx {
   float* logits;
   const float* dlogits;
   const float* drop;
+  float* dx;           // input-gradient ops only: NCDHW fp32 gradient of the network input
   cudaStream_t st;
   int launches;
   struct Prof* prof;
@@ -90,7 +91,7 @@ struct NormLayer {
 struct BlockRec {
   TRef X, a1, y1, a2, out;
   int n1, n2, c1, c2, cs;  // indices into norms / convs (cs = -1 when no sample conv)
-  bool first;              // first block of the network: no input gradient
+  bool first;              // first block of the network: no data gradient in the backward list (input_grad plans: emit_input_grad)
   bool scale_out;          // Dropout3d scale applied to this block's output
   bool scale_in;           // this block's input is the dropout output (its dX must be scaled)
 };
@@ -123,6 +124,8 @@ struct b200unet_plan {
   std::vector<ConvLayer> convs;
   std::vector<NormLayer> norms;
   std::vector<OpFn> fwd, bwd;
+  std::vector<OpFn> igrad;   // input_grad plans: d(loss)/d(x), run by b200unet_plan_input_grad after the backward
+  bool input_grad = false;
   size_t cur = 0;
   size_t stats_off = 0, stats_bytes = 0;  // zeroed at the start of every forward
   size_t bz_off = 0, bz_bytes = 0;        // zeroed at the start of every backward (bstats + dw accumulators)
@@ -477,10 +480,10 @@ static void emit_wgrad(Plan& P, int ci, TRef a, TRef dy) {
 // data gradient through conv `ci` (stride 1):  out = conv(dy, Wd)  with either the GN/ReLU backward epilogue
 // (ni >= 0, gn_x = raw input of the norm) or a plain epilogue (+res, *dropout scale).
 static void emit_dgrad(Plan& P, int ci, TRef dy, TRef out, int ni, TRef gn_x, TRef res, bool scale, double alg_macs,
-                       bool cls_mode = false) {
+                       bool cls_mode = false, std::vector<OpFn>* list = nullptr) {
   const int cat = CAT_CONV_DGRAD;
   P.macs[cat] += alg_macs;
-  push_op(P.bwd, std::string(ni >= 0 ? "dgrad+gnrelu " : "dgrad ") + P.convs[ci].name + " " + shape_of(P, dy) + "->" + shape_of(P, out),
+  push_op(list ? *list : P.bwd, std::string(ni >= 0 ? "dgrad+gnrelu " : "dgrad ") + P.convs[ci].name + " " + shape_of(P, dy) + "->" + shape_of(P, out),
           [&P, ci, dy, out, ni, gn_x, res, scale, cat, cls_mode](RunCtx& cx) -> int {
     const ConvLayer& c = P.convs[ci];
     ConvOp op;
@@ -568,7 +571,7 @@ static BlockRec build_block_fwd(Plan& P, const std::string& pre, TRef X, int cin
   r.c1 = new_conv(P, pre + ".conv1.conv.weight", C, cin_real, 3, 1, true);
   r.n2 = new_norm(P, pre + ".conv2.norm1", C, C, S);
   r.c2 = new_conv(P, pre + ".conv2.conv.weight", C, C, 3, 1, true);
-  r.cs = (cin_real != C) ? new_conv(P, pre + ".sample.weight", C, cin_real, 1, 1, !first) : -1;
+  r.cs = (cin_real != C) ? new_conv(P, pre + ".sample.weight", C, cin_real, 1, 1, !first || P.input_grad) : -1;
   r.a1 = full(P, new_buf(P, N, D, H, W, X.c));
   r.y1 = full(P, new_buf(P, N, D, H, W, C));
   r.a2 = full(P, new_buf(P, N, D, H, W, C));
@@ -583,6 +586,24 @@ static BlockRec build_block_fwd(Plan& P, const std::string& pre, TRef X, int cin
   release_buf(P, r.a2.buf);
   if (x_dead) release_if_whole(P, X);
   return r;
+}
+
+// input_grad plans: d(loss)/d(x) -> NCDHW fp32 from the first block's gradients (UNet3D: dz = the data gradient of its conv1
+// through the GroupNorm/ReLU epilogue, x = the packed network input, norm ni; r = the residual branch's gradient.  DynUNet: ni < 0,
+// r = the data gradient of input_block.conv1).  Backward buffers are never recycled in a training plan, so dz, x and r still hold
+// what the backward left in them.
+static void emit_input_grad(Plan& P, int ni, TRef dz, TRef x, TRef r) {
+  push_op(P.igrad, "input_grad " + shape_of(P, r), [&P, ni, dz, x, r](RunCtx& cx) -> int {
+    if (ni < 0) {
+      LAUNCHED(cx, CAT_RESAMPLE, launch_input_grad(nullptr, nullptr, nullptr, nullptr, 0, act_of(P, cx, r), P.d.n_features, cx.dx, cx.st));
+      return OK;
+    }
+    const NormLayer& n = P.norms[ni];
+    const Act a = act_of(P, cx, dz), b = act_of(P, cx, x);
+    LAUNCHED(cx, CAT_NORM, launch_input_grad(&a, &b, reinterpret_cast<const float*>(cx.ws + n.coef), reinterpret_cast<const float*>(cx.ws + n.coef2),
+                                             n.Cld, act_of(P, cx, r), P.d.n_features, cx.dx, cx.st));
+    return OK;
+  });
 }
 
 // returns the TRef of dX (kNone for the first block of the network)
@@ -601,6 +622,15 @@ static TRef build_block_bwd(Plan& P, const BlockRec& r, TRef dOut) {
   emit_dgrad(P, r.c1, dy1, dz1, r.n1, r.X, kNone, false, r.first ? 0.0 : conv_macs(P, r.c1, dy1));
   if (r.first) {   // no data gradient below the first block: only dgamma / dbeta of its first norm are needed
     emit_gn_bwd_finalize(P, r.n1);
+    if (P.input_grad) {
+      // dOut already carries the Dropout3d scale of this block's output (applied by whoever produced it): not applied again
+      TRef res = dOut;
+      if (r.cs >= 0) {
+        res = full(P, new_buf(P, N, D, H, W, r.X.c));
+        emit_dgrad(P, r.cs, dOut, res, -1, kNone, kNone, false, 0.0, false, &P.igrad);
+      }
+      emit_input_grad(P, r.n1, dz1, r.X, res);
+    }
     return kNone;
   }
   TRef dX = full(P, new_buf(P, N, D, H, W, r.X.c));
@@ -943,7 +973,7 @@ static DynBlock build_dyn_block_fwd(Plan& P, const std::string& pre, TRef X, int
   const long long S = (long long)D * H * W;
   DynBlock r;
   r.X = X; r.stride = stride; r.first = first;
-  r.k1 = new_conv(P, pre + ".conv1.conv.weight", C, cin_real, 3, stride, !first);
+  r.k1 = new_conv(P, pre + ".conv1.conv.weight", C, cin_real, 3, stride, !first || P.input_grad);
   r.k2 = new_conv(P, pre + ".conv2.conv.weight", C, C, 3, 1, true);
   r.n1 = new_norm_keys(P, pre + ".norm1", C, S);
   r.n2 = new_norm_keys(P, pre + ".norm2", C, S);
@@ -988,7 +1018,15 @@ static TRef build_dyn_block_bwd(Plan& P, const DynBlock& r, TRef g1, TRef g2) {
   TRef dc1 = full(P, new_buf(P, N, D, H, W, C));
   emit_gn_bwd(P, r.n1, dz1, r.c1, kNone, dc1, false);
   emit_wgrad(P, r.k1, r.X, dc1);
-  if (r.first) return kNone;
+  if (r.first) {
+    if (P.input_grad) {
+      const Buf& xb = P.bufs[r.X.buf];
+      TRef dX = full(P, new_buf(P, N, xb.D, xb.H, xb.W, r.X.c));
+      emit_dgrad(P, r.k1, dc1, dX, -1, kNone, kNone, false, 0.0, r.stride == 2, &P.igrad);
+      emit_input_grad(P, -1, kNone, kNone, dX);
+    }
+    return kNone;
+  }
   const Buf& xb = P.bufs[r.X.buf];
   TRef dX = full(P, new_buf(P, N, xb.D, xb.H, xb.W, r.X.c));
   emit_dgrad(P, r.k1, dc1, dX, -1, kNone, kNone, false, conv_macs(P, r.k1, dc1), /*cls_mode=*/r.stride == 2);
@@ -1207,6 +1245,13 @@ int b200unet_plan_create(const b200unet_net_desc* desc, b200unet_plan** out) {
   P->split = desc->split_precision != 0;
   P->infer = desc->inference_only != 0;
   P->deterministic = desc->deterministic != 0;
+  P->input_grad = desc->input_grad != 0;
+  if (P->input_grad && P->infer) {
+    set_error("plan_create: input_grad=1 on an inference_only plan (the input gradient needs the backward schedule)");
+    delete P;
+    *out = nullptr;
+    return E_INVALID;
+  }
   if (P->d.norm_groups <= 0) P->d.norm_groups = 8;
   if (P->d.feature_dilation <= 0) P->d.feature_dilation = 2;
   int s = build(*P);
@@ -1311,6 +1356,24 @@ static int run_backward(b200unet_plan* plan, const float* dlogits, const float* 
 int b200unet_plan_backward(b200unet_plan* plan, const float* dlogits, const float* const* params, float* const* grads,
                            void* workspace, void* stream) {
   return run_backward(plan, dlogits, params, grads, workspace, stream, -1);
+}
+
+int b200unet_plan_input_grad(b200unet_plan* plan, float* dx, void* workspace, void* stream) {
+  if (!plan || !dx || !workspace) { set_error("plan_input_grad: null argument"); return E_INVALID; }
+  if (!plan->input_grad) { set_error("plan_input_grad: this plan was created without input_grad=1"); return E_INVALID; }
+  RunCtx cx;
+  memset(&cx, 0, sizeof(cx));
+  cx.ws = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023));
+  cx.dx = dx;
+  cx.st = reinterpret_cast<cudaStream_t>(stream);
+  cx.prof = plan->prof;
+  cx.part = -1;
+  for (auto& op : plan->igrad) {
+    int s = op(cx);
+    if (s != OK) return s;
+  }
+  plan->last_launches = cx.launches;
+  return OK;
 }
 
 int b200unet_plan_backward_parts(const b200unet_plan* plan) { return (!plan || plan->infer) ? 0 : plan->bwd_split >= 0 ? 2 : 1; }

@@ -41,7 +41,7 @@ class NetDesc(C.Structure):
                 ("use_transposed_convolutions", C.c_int32), ("activation", C.c_int32),
                 ("split_precision", C.c_int32), ("batch", C.c_int32), ("depth", C.c_int32), ("height", C.c_int32),
                 ("width", C.c_int32), ("arch", C.c_int32), ("filters", C.c_int32 * 8), ("act_slope", C.c_float),
-                ("deterministic", C.c_int32), ("inference_only", C.c_int32)]
+                ("deterministic", C.c_int32), ("inference_only", C.c_int32), ("input_grad", C.c_int32)]
 
 
 def build_library(force: bool = False, verbose: bool = False) -> str:
@@ -120,6 +120,7 @@ _SIGS = {
                                         C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200unet_plan_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                          C.c_void_p, C.c_void_p]),
+    "b200unet_plan_input_grad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200unet_plan_backward_parts": (C.c_int, [C.c_void_p]),
     "b200unet_plan_param_backward_part": (C.c_int, [C.c_void_p, C.c_int]),
     "b200unet_plan_backward_part": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),

@@ -119,12 +119,13 @@ def _ptr_array(tensors: Sequence[torch.Tensor]):
 
 
 class _UNetFunction(torch.autograd.Function):
-    """forward+backward of the whole network as two library calls."""
+    """forward+backward of the whole network as two library calls (a third one for the input gradient)."""
 
     @staticmethod
-    def forward(ctx, model, x, drop, need_bwd, *params):
-        # need_bwd is decided by the caller: inside Function.forward autograd's grad mode is always off
-        plan = model._plan_for(x, inference_only=not need_bwd)
+    def forward(ctx, model, x, drop, need_bwd, need_dx, *params):
+        # need_bwd / need_dx are decided by the caller: inside Function.forward autograd's grad mode is always off.  need_dx
+        # selects a plan created with input_grad (same parameter-gradient launches, plus the input-gradient ops)
+        plan = model._plan_for(x, inference_only=not need_bwd, input_grad=need_dx)
         n, _, d, h, w = x.shape
         logits = torch.empty((n, model.n_outputs, d, h, w), dtype=torch.float32, device=x.device)
         with torch.cuda.device(x.device):   # the library launches on the current device's current stream
@@ -143,6 +144,7 @@ class _UNetFunction(torch.autograd.Function):
         if need_bwd:
             plan.serial += 1
         ctx.plan = plan
+        ctx.need_dx = bool(need_dx)
         ctx.serial = plan.serial
         ctx.model = model
         ctx.save_for_backward(*params)
@@ -161,10 +163,16 @@ class _UNetFunction(torch.autograd.Function):
                                "(one outstanding forward per input shape)" % (ctx.serial, plan.serial))
         params = ctx.saved_tensors
         model = ctx.model
+        need_dx = ctx.need_dx and ctx.needs_input_grad[1]
+        if need_dx and torch.is_grad_enabled():
+            raise RuntimeError("B200 %s: double backward (create_graph=True) through the input gradient is not supported"
+                               % type(model).__name__)
         dlogits = dlogits.contiguous().float()
+        dx = None
         with torch.cuda.device(dlogits.device):
             grads, direct = model._grad_targets(params, plan)
-            if model._defer_backward_tail and direct and plan.backward_parts() == 2:
+            # the input gradient reads what the whole backward leaves in the workspace: never deferred
+            if model._defer_backward_tail and direct and not need_dx and plan.backward_parts() == 2:
                 # two-part backward (train.GraphedTrainStep with a gradient exchange): part 0 -- head, decoder, deepest encoder
                 # level -- runs here; the caller runs the rest through finish_backward() after it has started the exchange of
                 # the gradients that are final now (model.flat_gradient_bucket_parts()[0])
@@ -174,10 +182,16 @@ class _UNetFunction(torch.autograd.Function):
             else:
                 _lib.check(plan.lib.b200unet_plan_backward(plan.handle, dlogits.data_ptr(), _ptr_array(params), _ptr_array(grads),
                                                            plan.workspace.data_ptr(), _lib.stream_ptr()), "plan_backward")
-        model.launches_last_backward = plan.last_launches()
+            model.launches_last_backward = plan.last_launches()
+            if need_dx:
+                n, _, d, h, w = dlogits.shape
+                dx = torch.empty((n, model.n_features, d, h, w), dtype=torch.float32, device=dlogits.device)
+                _lib.check(plan.lib.b200unet_plan_input_grad(plan.handle, dx.data_ptr(), plan.workspace.data_ptr(), _lib.stream_ptr()),
+                           "plan_input_grad")
+                model.launches_last_backward += plan.last_launches()
         if direct:                      # flat-bucket mode: the gradients already sit in the parameters' .grad views
-            return (None, None, None, None) + (None,) * len(params)
-        return (None, None, None, None) + tuple(grads)
+            return (None, dx, None, None, None) + (None,) * len(params)
+        return (None, dx, None, None, None) + tuple(grads)
 
 
 class _PlanModel(nn.Module):
@@ -220,13 +234,14 @@ class _PlanModel(nn.Module):
         return [sd[k] for k in self._keys]
 
     # ------------------------------------------------------------------ plan cache
-    def _plan_for(self, x: torch.Tensor, inference_only: bool = False) -> _Plan:
+    def _plan_for(self, x: torch.Tensor, inference_only: bool = False, input_grad: bool = False) -> _Plan:
         n, _, d, h, w = x.shape
-        key = (n, d, h, w, self.precision, x.device.index, bool(inference_only))
+        key = (n, d, h, w, self.precision, x.device.index, bool(input_grad), bool(inference_only))
         plan = self._plans.get(key)
         if plan is None:
             desc = self._net_desc(n, d, h, w)
             desc.inference_only = int(bool(inference_only))
+            desc.input_grad = int(bool(input_grad))
             desc.deterministic = int(self.deterministic and not inference_only)
             plan = _Plan(desc, x.device)
             spec = plan.param_spec()
@@ -309,9 +324,11 @@ class _PlanModel(nn.Module):
     _overwrite_grads = False   # set by train.GraphedTrainStep while it owns the step
 
     @staticmethod
-    def _needs_backward(params) -> bool:
-        """training plan (activations kept) iff autograd will ask for a backward; otherwise the forward-only plan"""
-        return bool(torch.is_grad_enabled() and any(p.requires_grad for p in params))
+    def _needs_backward(params, x: torch.Tensor) -> Tuple[bool, bool]:
+        """(training plan: activations kept, iff autograd will ask for a backward; otherwise the forward-only plan,
+        input gradient: the plan also produces d(loss)/d(x))"""
+        need_dx = bool(torch.is_grad_enabled() and x.requires_grad)
+        return bool(need_dx or (torch.is_grad_enabled() and any(p.requires_grad for p in params))), need_dx
 
     def _check_input(self, x: torch.Tensor, n_in: int) -> torch.Tensor:
         if not isinstance(x, torch.Tensor) or x.dim() != 5:
@@ -320,10 +337,10 @@ class _PlanModel(nn.Module):
             raise RuntimeError("B200 %s runs only on CUDA tensors (no CPU fallback); got device %s" % (type(self).__name__, x.device))
         if x.shape[1] != n_in:
             raise ValueError("expected %d input channels, got %d" % (n_in, x.shape[1]))
-        if x.requires_grad:
-            raise NotImplementedError("B200 %s does not produce input gradients" % type(self).__name__)
-        xp = x.as_subclass(torch.Tensor) if type(x) is not torch.Tensor else x   # MetaTensor -> plain view
-        xp = xp.detach().contiguous().float()
+        # MetaTensor -> plain view; as_subclass, contiguous and float stay on the autograd graph, so the input gradient
+        # reaches the caller's tensor
+        xp = x.as_subclass(torch.Tensor) if type(x) is not torch.Tensor else x
+        xp = xp.contiguous().float()
         params = self.ordered_parameters()
         if params[0].device != xp.device:
             raise RuntimeError("model parameters are on %s but the input is on %s" % (params[0].device, xp.device))
@@ -470,7 +487,7 @@ class UNet3D(_PlanModel):
             else:
                 keep = (torch.rand((xp.shape[0], self.base_width), device=xp.device) >= self.dropout_p)
                 drop = keep.float() / (1.0 - self.dropout_p)
-        return _UNetFunction.apply(self, xp, drop, self._needs_backward(params), *params)
+        return _UNetFunction.apply(self, xp, drop, *self._needs_backward(params, xp), *params)
 
 
 class AutocastUNet(UNet3D):
@@ -600,7 +617,7 @@ class DynUNet(_PlanModel):
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         xp = self._check_input(x, self.in_channels)
         params = self.ordered_parameters()
-        return _UNetFunction.apply(self, xp, None, self._needs_backward(params), *params)
+        return _UNetFunction.apply(self, xp, None, *self._needs_backward(params, xp), *params)
 
 
 _MODELS = {"UNet3D": UNet3D, "AutocastUNet": AutocastUNet, "AutoImplantUNet": AutoImplantUNet,

@@ -175,6 +175,9 @@ typedef struct b200unet_net_desc {
                                  sums, a second kernel adds them in a fixed order (bit-identical gradients run to run) */
   int32_t inference_only;     /* 1 = forward-only plan (volumetric.py:131-150 runs under no_grad): no backward schedule, no
                                  backward buffers, forward temporaries are recycled -> a much smaller workspace */
+  int32_t input_grad;         /* 1 = the plan can also produce d(loss)/d(x) (b200unet_plan_input_grad): saliency maps, adversarial
+                                 training, cascades whose input comes from a differentiable stage.  Costs the forward only the data-
+                                 gradient weight packs of the first block's convolutions.  Rejected with inference_only = 1. */
 } b200unet_net_desc;
 
 typedef struct b200unet_plan b200unet_plan;
@@ -206,7 +209,14 @@ int b200unet_plan_backward_parts(const b200unet_plan* plan);
 int b200unet_plan_param_backward_part(const b200unet_plan* plan, int i);
 int b200unet_plan_backward_part(b200unet_plan* plan, int part, const float* dlogits, const float* const* params, float* const* grads,
                                 void* workspace, void* stream);
-/* number of kernels the last forward / backward call launched (for bench.py's gpu_launches) */
+/* input gradient of a plan created with input_grad = 1: dx = d(loss)/d(x), NCDHW fp32 [N][n_features][D][H][W], overwritten.
+ * Runs after b200unet_plan_backward (or after backward_part(1)) on the same stream and workspace, before the next forward: it reads
+ * what that backward left in the workspace (the gradients reaching the first block, the packed input, the first norm's
+ * coefficients).  UNet3D: GroupNorm(+ReLU) backward of encoder.layers.0.blocks.0.conv1.norm1 + the data gradient of the block's
+ * 1x1x1 `sample` branch or its identity (myronenko.py:34-58); DynUNet: the data gradient of input_block.conv1.  The parameter
+ * gradients come from the backward alone: this call writes nothing but dx. */
+int b200unet_plan_input_grad(b200unet_plan* plan, float* dx, void* workspace, void* stream);
+/* number of kernels the last forward / backward / input-gradient call launched (for bench.py's gpu_launches) */
 int b200unet_plan_last_launches(const b200unet_plan* plan);
 
 /* per-category accounting for bench.py's roofline (categories: 0 conv fwd, 1 conv dgrad, 2 conv wgrad, 3 norm/act,
