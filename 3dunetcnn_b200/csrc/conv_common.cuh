@@ -53,30 +53,6 @@ struct ConvArgs {
   unsigned char cls_tap[8][8];
 };
 
-__device__ __forceinline__ void epi_load8(const bf16* hi, const bf16* lo, long long off, float* v) {
-  uint4 a = *reinterpret_cast<const uint4*>(hi + off);
-  v[0] = bf16_lo_to_f(a.x); v[1] = bf16_hi_to_f(a.x); v[2] = bf16_lo_to_f(a.y); v[3] = bf16_hi_to_f(a.y);
-  v[4] = bf16_lo_to_f(a.z); v[5] = bf16_hi_to_f(a.z); v[6] = bf16_lo_to_f(a.w); v[7] = bf16_hi_to_f(a.w);
-  if (lo) {
-    uint4 b = *reinterpret_cast<const uint4*>(lo + off);
-    v[0] += bf16_lo_to_f(b.x); v[1] += bf16_hi_to_f(b.x); v[2] += bf16_lo_to_f(b.y); v[3] += bf16_hi_to_f(b.y);
-    v[4] += bf16_lo_to_f(b.z); v[5] += bf16_hi_to_f(b.z); v[6] += bf16_lo_to_f(b.w); v[7] += bf16_hi_to_f(b.w);
-  }
-}
-__device__ __forceinline__ void epi_store8(bf16* hi, bf16* lo, long long off, const float* v) {
-  uint4 a;
-  a.x = pack_bf16x2(v[0], v[1]); a.y = pack_bf16x2(v[2], v[3]); a.z = pack_bf16x2(v[4], v[5]); a.w = pack_bf16x2(v[6], v[7]);
-  *reinterpret_cast<uint4*>(hi + off) = a;
-  if (lo) {
-    uint4 b;
-    b.x = pack_bf16x2(v[0] - bf16_lo_to_f(a.x), v[1] - bf16_hi_to_f(a.x));
-    b.y = pack_bf16x2(v[2] - bf16_lo_to_f(a.y), v[3] - bf16_hi_to_f(a.y));
-    b.z = pack_bf16x2(v[4] - bf16_lo_to_f(a.z), v[5] - bf16_hi_to_f(a.z));
-    b.w = pack_bf16x2(v[6] - bf16_lo_to_f(a.w), v[7] - bf16_hi_to_f(a.w));
-    *reinterpret_cast<uint4*>(lo + off) = b;
-  }
-}
-
 // Transposing butterfly: every lane holds 16 column values of its own row; on return lane l holds the sum over the
 // 32 rows of column ((l >> 1) & 15)  (lanes 2k and 2k+1 hold the same column).  16 shuffles instead of 80.
 __device__ __forceinline__ float warp_colsum16(float (&v)[16], int lane) {

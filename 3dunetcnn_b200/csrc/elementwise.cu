@@ -1,6 +1,6 @@
 // Bandwidth-bound kernels of the U-Net path (everything that is not a tensor-core contraction):
-// input packing, GroupNorm finalize/apply/backward, trilinear x2 up-sampling fwd/bwd, 1x1x1 head fwd/bwd,
-// weight packing and zero insertion.  All activations are NDHWC bf16 (hi [+ lo]) views; 8 channels (16 B) per
+// input packing, GroupNorm finalize/apply/backward, trilinear x2 up-sampling fwd/bwd, 1x1x1 head fwd/bwd
+// and zero insertion (weight packing: small_ops.cu).  All activations are NDHWC bf16 (hi [+ lo]) views; 8 channels (16 B) per
 // thread so every access is a 128-bit vector along the innermost (channel) axis.
 //
 // Reference semantics restated (paths relative to /root/reference):
@@ -13,36 +13,6 @@
 namespace b200 {
 
 // ------------------------------------------------------------------------------------------------ helpers
-__device__ __forceinline__ void load8(const bf16* hi, const bf16* lo, long long off, float (&v)[8]) {
-  uint4 a = *reinterpret_cast<const uint4*>(hi + off);
-  v[0] = bf16_lo_to_f(a.x); v[1] = bf16_hi_to_f(a.x);
-  v[2] = bf16_lo_to_f(a.y); v[3] = bf16_hi_to_f(a.y);
-  v[4] = bf16_lo_to_f(a.z); v[5] = bf16_hi_to_f(a.z);
-  v[6] = bf16_lo_to_f(a.w); v[7] = bf16_hi_to_f(a.w);
-  if (lo) {
-    uint4 b = *reinterpret_cast<const uint4*>(lo + off);
-    v[0] += bf16_lo_to_f(b.x); v[1] += bf16_hi_to_f(b.x);
-    v[2] += bf16_lo_to_f(b.y); v[3] += bf16_hi_to_f(b.y);
-    v[4] += bf16_lo_to_f(b.z); v[5] += bf16_hi_to_f(b.z);
-    v[6] += bf16_lo_to_f(b.w); v[7] += bf16_hi_to_f(b.w);
-  }
-}
-
-__device__ __forceinline__ void store8(bf16* hi, bf16* lo, long long off, const float (&v)[8]) {
-  uint4 a;
-  a.x = pack_bf16x2(v[0], v[1]); a.y = pack_bf16x2(v[2], v[3]);
-  a.z = pack_bf16x2(v[4], v[5]); a.w = pack_bf16x2(v[6], v[7]);
-  *reinterpret_cast<uint4*>(hi + off) = a;
-  if (lo) {
-    uint4 b;
-    b.x = pack_bf16x2(v[0] - bf16_lo_to_f(a.x), v[1] - bf16_hi_to_f(a.x));
-    b.y = pack_bf16x2(v[2] - bf16_lo_to_f(a.y), v[3] - bf16_hi_to_f(a.y));
-    b.z = pack_bf16x2(v[4] - bf16_lo_to_f(a.z), v[5] - bf16_hi_to_f(a.z));
-    b.w = pack_bf16x2(v[6] - bf16_lo_to_f(a.w), v[7] - bf16_hi_to_f(a.w));
-    *reinterpret_cast<uint4*>(lo + off) = b;
-  }
-}
-
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -910,9 +880,7 @@ __global__ void __launch_bounds__(128) k_upsample2x_bwd_blk(Act dy, Act dx) {
 int launch_upsample2x_bwd(const Act& dy, const Act& dx, cudaStream_t st) {
   B200_REQUIRE(dx.C % 8 == 0 && dy.C == dx.C, E_INVALID, "upsample_bwd: channel mismatch");
   B200_REQUIRE(dy.D == 2 * dx.D && dy.H == 2 * dx.H && dy.W == 2 * dx.W, E_UNSUPPORTED, "upsample_bwd: not 2x");
-  if (use_tiled_upsample_bwd()) return launch_upsample2x_bwd_tiled(dy, dx, st);
-  static const bool no_blk = getenv("B200UNET_UPSAMPLE_BWD_GATHER") != nullptr;   // A/B switch: the one-voxel-per-thread gather form
-  if (!no_blk && !dy.lo && !dx.lo && dx.D % 2 == 0 && dx.H % 2 == 0 && dx.W % 2 == 0 && dx.D >= 2 && dx.H >= 2 && dx.W >= 2) {
+  if (!dy.lo && !dx.lo && dx.D % 2 == 0 && dx.H % 2 == 0 && dx.W % 2 == 0 && dx.D >= 2 && dx.H >= 2 && dx.W >= 2) {
     const long long blocks = (long long)dx.N * (dx.D / 2) * (dx.H / 2) * (dx.W / 2) * (dx.C / 8);
     k_upsample2x_bwd_blk<<<ew_blocks(blocks, 128), 128, 0, st>>>(dy, dx);
     B200_CHECK_CUDA(cudaGetLastError());
@@ -1076,122 +1044,6 @@ int launch_head_bwd(const Act& x, const float* w, int n_out, const float* dlogit
 #undef B200_HEAD_CASE
   B200_CHECK_CUDA(cudaGetLastError());
   k_sum_slots<<<n_out * x.C, 128, 0, st>>>(scratch, blocks, n_out * x.C, dw);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return OK;
-}
-
-// ------------------------------------------------------------------------------------------------ weight packing
-// torch Conv3d weight fp32 [Co][Ci][T] (T = k^3 taps, kd-major) ->
-//   mode 0 (fwd)   : [T][Co][Ci]               B operand of  Y = conv(X, W)
-//   mode 1 (dgrad) : [T][Ci][Co] with taps flipped   B operand of  dX = conv(dY, flip(W)^T)
-//   mode 2 (convT fwd, torch ConvTranspose3d weight [Ci][Co][T]) : [T][Co][Ci] flipped
-__global__ void k_pack_weights(const float* __restrict__ w, int Co, int Ci, int Cop, int Cip, int T, int mode,
-                               bf16* __restrict__ hi, bf16* __restrict__ lo) {
-  // Co/Ci: real extents of the torch tensor; Cop/Cip: packed (zero padded) extents.
-  const long long total = (long long)T * Cop * Cip;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    float v = 0.f;
-    if (mode == 0 || mode == 2 || mode == 4) {   // forward layout [T][Cop][Cip]
-      const int ci = (int)(i % Cip); const int co = (int)((i / Cip) % Cop); const int t = (int)(i / ((long long)Cip * Cop));
-      if (ci < Ci && co < Co)
-        v = mode == 0 ? w[((long long)co * Ci + ci) * T + t] : w[((long long)ci * Co + co) * T + (mode == 2 ? T - 1 - t : t)];
-    } else {                                     // data-gradient layout [T][Cip][Cop]
-      const int co = (int)(i % Cop); const int ci = (int)((i / Cop) % Cip); const int t = (int)(i / ((long long)Cip * Cop));
-      if (ci < Ci && co < Co)
-        v = mode == 1 ? w[((long long)co * Ci + ci) * T + (T - 1 - t)] : w[((long long)ci * Co + co) * T + t];
-    }
-    bf16 h = __float2bfloat16_rn(v);
-    hi[i] = h;
-    if (lo) lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
-  }
-}
-
-int launch_pack_weights(const float* w, int Co, int Ci, int Cop, int Cip, int T, int mode, bf16* hi, bf16* lo,
-                        cudaStream_t st) {
-  long long total = (long long)T * Cop * Cip;
-  k_pack_weights<<<ew_blocks(total, 256), 256, 0, st>>>(w, Co, Ci, Cop, Cip, T, mode, hi, lo);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return OK;
-}
-
-// packed fp32 gradient [T][Ci][Co] (Co contiguous; what the wgrad kernel accumulates) -> torch layout [Co][Ci][T]
-// (mode 0) or ConvTranspose3d layout [Ci][Co][T] with flipped taps (mode 2).
-__global__ void k_unpack_wgrad(const float* __restrict__ g, int Co, int Ci, int Cop, int Cip, int T, int mode,
-                               float* __restrict__ out) {
-  // g: [T][Cip][Cop] (what the wgrad kernel accumulates); out: torch layout with the real extents.
-  const long long total = (long long)T * Co * Ci;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    if (mode == 0) {
-      const int t = (int)(i % T); const int ci = (int)((i / T) % Ci); const int co = (int)(i / ((long long)T * Ci));
-      out[i] = g[((long long)t * Cip + ci) * Cop + co];
-    } else {
-      const int t = (int)(i % T); const int co = (int)((i / T) % Co); const int ci = (int)(i / ((long long)T * Co));
-      out[i] = g[((long long)(T - 1 - t) * Cip + ci) * Cop + co];
-    }
-  }
-}
-
-int launch_unpack_wgrad(const float* g, int Co, int Ci, int Cop, int Cip, int T, int mode, float* out,
-                        cudaStream_t st) {
-  long long total = (long long)T * Co * Ci;
-  k_unpack_wgrad<<<ew_blocks(total, 256), 256, 0, st>>>(g, Co, Ci, Cop, Cip, T, mode, out);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return OK;
-}
-
-// ---- batched forms: one launch packs / unpacks every convolution of the network (blockIdx.y = job)
-__global__ void k_pack_all(PtrTable params, const PackJob* __restrict__ jobs, uint8_t* __restrict__ ws, int split) {
-  const PackJob j = jobs[blockIdx.y];
-  const float* __restrict__ w = reinterpret_cast<const float*>(params.p[j.pidx]);
-  bf16* hi = reinterpret_cast<bf16*>(ws + j.off_hi);
-  bf16* lo = split ? reinterpret_cast<bf16*>(ws + j.off_lo) : nullptr;
-  const long long total = (long long)j.T * j.Cop * j.Cip;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    float v = 0.f;
-    if (j.mode == 0 || j.mode == 2 || j.mode == 4) {
-      const int ci = (int)(i % j.Cip); const int co = (int)((i / j.Cip) % j.Cop); const int t = (int)(i / ((long long)j.Cip * j.Cop));
-      if (ci < j.Ci && co < j.Co)
-        v = j.mode == 0 ? w[((long long)co * j.Ci + ci) * j.T + t]
-                        : w[((long long)ci * j.Co + co) * j.T + (j.mode == 2 ? j.T - 1 - t : t)];
-    } else {
-      const int co = (int)(i % j.Cop); const int ci = (int)((i / j.Cop) % j.Cip); const int t = (int)(i / ((long long)j.Cip * j.Cop));
-      if (ci < j.Ci && co < j.Co)
-        v = j.mode == 1 ? w[((long long)co * j.Ci + ci) * j.T + (j.T - 1 - t)] : w[((long long)ci * j.Co + co) * j.T + t];
-    }
-    bf16 h = __float2bfloat16_rn(v);
-    hi[i] = h;
-    if (lo) lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
-  }
-}
-
-int launch_pack_all(const PtrTable& params, const PackJob* jobs_dev, int njobs, uint8_t* ws, bool split, cudaStream_t st) {
-  if (njobs == 0) return OK;
-  if (use_tiled_pack()) return launch_pack_all_tiled(params, jobs_dev, njobs, ws, split, st);
-  k_pack_all<<<dim3(48, njobs), 256, 0, st>>>(params, jobs_dev, ws, split ? 1 : 0);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return OK;
-}
-
-__global__ void k_unpack_all(PtrTable grads, const PackJob* __restrict__ jobs, const uint8_t* __restrict__ ws) {
-  const PackJob j = jobs[blockIdx.y];
-  float* __restrict__ out = const_cast<float*>(reinterpret_cast<const float*>(grads.p[j.pidx]));
-  const float* __restrict__ g = reinterpret_cast<const float*>(ws + j.off_hi);   // fp32 accumulator [T][Cip][Cop]
-  const long long total = (long long)j.T * j.Co * j.Ci;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    if (j.mode == 0) {
-      const int t = (int)(i % j.T); const int ci = (int)((i / j.T) % j.Ci); const int co = (int)(i / ((long long)j.T * j.Ci));
-      out[i] = g[((long long)t * j.Cip + ci) * j.Cop + co];
-    } else {   // ConvTranspose3d gradient layout [Ci][Co][T], taps flipped back
-      const int t = (int)(i % j.T); const int co = (int)((i / j.T) % j.Co); const int ci = (int)(i / ((long long)j.T * j.Co));
-      out[i] = g[((long long)(j.T - 1 - t) * j.Cip + ci) * j.Cop + co];
-    }
-  }
-}
-
-int launch_unpack_all(const PtrTable& grads, const PackJob* jobs_dev, int njobs, const uint8_t* ws, cudaStream_t st) {
-  if (njobs == 0) return OK;
-  if (use_tiled_pack()) return launch_unpack_all_tiled(grads, jobs_dev, njobs, ws, st);
-  k_unpack_all<<<dim3(48, njobs), 256, 0, st>>>(grads, jobs_dev, ws);
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;
 }

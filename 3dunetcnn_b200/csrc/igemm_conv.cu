@@ -455,8 +455,7 @@ int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
     }
     // single-pass bf16: the two W-parity classes of a (pd, ph) pair share one dense store (see tmap.h); the pair maps replace the
     // even classes' descriptors
-    static const bool no_pair = getenv("B200UNET_CLASS_PAIR") && atoi(getenv("B200UNET_CLASS_PAIR")) == 0;   // A/B switch
-    if (!split && !no_pair) {
+    if (!split) {
       for (int cls = 0; cls < 8; cls += 2)
         B200_TRY(make_act_map_classpair(&cmaps.oc[cls][0], out.hi, out.N, out.D, out.H, out.W, out.C, out.ld, (cls >> 2) & 1, (cls >> 1) & 1, cbo,
                                         2 * a.tw, a.th, a.td, swz_for_bytes(cbo * 2)));

@@ -22,8 +22,6 @@ int launch_gn_bwd(const Act& dz, const Act& x, const float* coef, const float* c
 int launch_add(const Act& a, const Act& b, const Act& y, cudaStream_t st);
 int launch_upsample2x_fwd(const Act& x, const Act& y, double* stats, int stats_ld, cudaStream_t st);
 int launch_upsample2x_bwd(const Act& dy, const Act& dx, cudaStream_t st);
-bool use_tiled_upsample_bwd();
-int launch_upsample2x_bwd_tiled(const Act& dy, const Act& dx, cudaStream_t st);
 int launch_head_fwd(const Act& x, const float* w, int n_out, int act_mode, float* logits, cudaStream_t st,
                     const float* bias = nullptr);
 int launch_head_dbias(const float* dlogits, int N, int NO, long long S, float* dbias, cudaStream_t st, float* scratch);
@@ -33,6 +31,8 @@ int launch_act_bwd(const Act& g1, const Act* g2, const Act& c, const float* coef
 int launch_head_bwd(const Act& x, const float* w, int n_out, const float* dlogits, const Act& dx, float* dw,
                     cudaStream_t st, float* scratch);   // scratch: head_bwd_scratch_bytes(n_out, C) (per-block partial sums)
 size_t head_bwd_scratch_bytes(int n_out, int C);
+// ---- weight packing / gradient unpacking (small_ops.cu): shared-memory tiled transposes
+// one tensor; Cop and Cip (the padded extents) must be multiples of 8, T <= 27
 int launch_pack_weights(const float* w, int Co, int Ci, int Cop, int Cip, int T, int mode, bf16* hi, bf16* lo,
                         cudaStream_t st);
 int launch_unpack_wgrad(const float* g, int Co, int Ci, int Cop, int Cip, int T, int mode, float* out,
@@ -50,10 +50,6 @@ struct PackJob {
 };
 int launch_pack_all(const PtrTable& params, const PackJob* jobs_dev, int njobs, uint8_t* ws, bool split, cudaStream_t st);
 int launch_unpack_all(const PtrTable& grads, const PackJob* jobs_dev, int njobs, const uint8_t* ws, cudaStream_t st);
-// shared-memory tiled / register-tiled rewrites (small_ops.cu); selected unless B200UNET_OLD_SMALL_OPS is set
-bool use_tiled_pack();
-int launch_pack_all_tiled(const PtrTable& params, const PackJob* jobs_dev, int njobs, uint8_t* ws, bool split, cudaStream_t st);
-int launch_unpack_all_tiled(const PtrTable& grads, const PackJob* jobs_dev, int njobs, const uint8_t* ws, cudaStream_t st);
 int launch_bias_grad(const Act& dy, float* dbias, cudaStream_t st);   // dbias[c] = sum over the VISIBLE voxels of dy
 int launch_zero_insert(const Act& x, const Act& z, int od, int oh, int ow, cudaStream_t st);
 int launch_ncdhw_to_act(const float* x, int C, const Act& out, cudaStream_t st);

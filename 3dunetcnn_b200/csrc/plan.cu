@@ -40,20 +40,23 @@ struct TRef {
 static const TRef kNone = {-1, 0, 0, 0};
 
 struct RunCtx {
-  uint8_t* ws;
-  const float* const* params;
-  float* const* grads;
-  const float* x;
-  float* logits;
-  const float* dlogits;
-  const float* drop;
-  float* dx;           // input-gradient ops only: NCDHW fp32 gradient of the network input
+  uint8_t* ws;                     // the caller's workspace, aligned up to 1 KiB
+  const float* const* params = nullptr;
+  float* const* grads = nullptr;
+  const float* x = nullptr;
+  float* logits = nullptr;
+  const float* dlogits = nullptr;
+  const float* drop = nullptr;
+  float* dx = nullptr;             // input-gradient ops only: NCDHW fp32 gradient of the network input
   cudaStream_t st;
-  int launches;
+  int launches = 0;
   struct Prof* prof;
-  const char* label;   // name of the op being launched (profiling only)
-  bool skip_pack;      // the packed bf16 weights in the workspace are current (parameters unchanged since the last forward)
-  int part;            // backward only: -1 = the whole schedule; 0 / 1 = the part b200unet_plan_backward_part runs
+  const char* label = nullptr;     // name of the op being launched (profiling only)
+  bool skip_pack = false;          // the packed bf16 weights in the workspace are current (parameters unchanged since the last forward)
+  int part = -1;                   // backward only: -1 = the whole schedule; 0 / 1 = the part b200unet_plan_backward_part runs
+  RunCtx(void* workspace, void* stream, struct Prof* p)
+      : ws(reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023))),
+        st(reinterpret_cast<cudaStream_t>(stream)), prof(p) {}
 };
 
 // launch categories of the per-kernel profile (models.py _Plan.CATEGORIES names them in this order)
@@ -369,7 +372,7 @@ static std::string shape_of(const Plan& P, TRef t) {
   return std::to_string(t.c) + "ch@" + std::to_string(b.D) + "x" + std::to_string(b.H) + "x" + std::to_string(b.W);
 }
 
-// ---- forward op emitters (weight packing is batched: see the k_pack_all launch at the head of the forward schedule)
+// ---- forward op emitters (weight packing is batched: see emit_prologue)
 static void emit_norm_fwd(Plan& P, int ni, TRef x, TRef y) {
   push_op(P.fwd, "gn_apply " + P.norms[ni].name + " " + shape_of(P, x), [&P, ni, x, y](RunCtx& cx) -> int {
     const NormLayer& n = P.norms[ni];
@@ -379,6 +382,24 @@ static void emit_norm_fwd(Plan& P, int ni, TRef x, TRef y) {
                                                  reinterpret_cast<float*>(cx.ws + n.coef), P.slope, cx.st));
     return OK;
   });
+}
+
+// A operand + packed weights of a convolution through layer c: its forward pack applied to x, or (dgrad) its data-gradient pack
+// applied to x = the gradient of its output.  A convolution reads its input at its stride and its output gradient at stride 1
+// (stride 2: parity-class mode); a transposed convolution reads its input at stride 1 (zero-inserted or parity-class mode) and
+// its output gradient at stride 2.
+static ConvSrc conv_src(const Plan& P, const RunCtx& cx, const ConvLayer& c, TRef x, bool dgrad) {
+  const bool up = c.transposed || c.up2;
+  ConvSrc s;
+  memset(&s, 0, sizeof(s));
+  s.x = act_of(P, cx, x);
+  s.w_hi = reinterpret_cast<bf16*>(cx.ws + (dgrad ? c.wd_hi : c.wf_hi));
+  s.w_lo = P.split ? reinterpret_cast<bf16*>(cx.ws + (dgrad ? c.wd_lo : c.wf_lo)) : nullptr;
+  s.ksz = c.ksz;
+  s.nopad = c.up2 ? 1 : 0;
+  s.stride = up ? (dgrad ? 2 : 1) : (dgrad ? 1 : c.stride);
+  s.Cip = dgrad ? c.Cop : c.Cip;   // K extent of the data-gradient pack [T][Cip][Cop] = Cop
+  return s;
 }
 
 // generic forward-weights conv:  out = (conv(a, W[ci]) [+ conv1x1(a2, W[ci2])] [+ res]) [* dropout]
@@ -398,18 +419,11 @@ static void emit_conv_fwd(Plan& P, int ci, TRef a, int ci2, TRef a2, TRef res, T
     ConvOp op;
     memset(&op, 0, sizeof(op));
     op.nsrc = 1;
-    op.src[0].x = act_of(P, cx, a);
-    op.src[0].w_hi = reinterpret_cast<bf16*>(cx.ws + c.wf_hi);
-    op.src[0].w_lo = P.split ? reinterpret_cast<bf16*>(cx.ws + c.wf_lo) : nullptr;
-    op.src[0].ksz = c.ksz; op.src[0].stride = c.stride; op.src[0].Cip = c.Cip;
+    op.src[0] = conv_src(P, cx, c, a, false);
     op.Cop = c.Cop;
     if (ci2 >= 0) {
-      const ConvLayer& c2 = P.convs[ci2];
       op.nsrc = 2;
-      op.src[1].x = act_of(P, cx, a2);
-      op.src[1].w_hi = reinterpret_cast<bf16*>(cx.ws + c2.wf_hi);
-      op.src[1].w_lo = P.split ? reinterpret_cast<bf16*>(cx.ws + c2.wf_lo) : nullptr;
-      op.src[1].ksz = c2.ksz; op.src[1].stride = c2.stride; op.src[1].Cip = c2.Cip;
+      op.src[1] = conv_src(P, cx, P.convs[ci2], a2, false);
     }
     op.out = act_of(P, cx, out);
     Act r;
@@ -490,11 +504,8 @@ static void emit_dgrad(Plan& P, int ci, TRef dy, TRef out, int ni, TRef gn_x, TR
     memset(&op, 0, sizeof(op));
     op.nsrc = 1;
     op.cls_mode = cls_mode ? 1 : 0;
-    op.src[0].x = act_of(P, cx, dy);
-    op.src[0].w_hi = reinterpret_cast<bf16*>(cx.ws + c.wd_hi);
-    op.src[0].w_lo = P.split ? reinterpret_cast<bf16*>(cx.ws + c.wd_lo) : nullptr;
-    op.src[0].ksz = c.ksz; op.src[0].stride = c.transposed ? 2 : 1; op.src[0].Cip = c.Cop;  // K extent of Wd = Cop
-    op.Cop = c.Cip;                                                       // rows of Wd = Cip
+    op.src[0] = conv_src(P, cx, c, dy, true);
+    op.Cop = c.Cip;   // rows of Wd = Cip
     op.out = act_of(P, cx, out);
     Act r, gx;
     if (res.valid()) { r = act_of(P, cx, res); op.res = &r; }
@@ -543,20 +554,95 @@ static void emit_gn_bwd(Plan& P, int ni, TRef dz, TRef x, TRef add1, TRef dx, bo
   });
 }
 
+// the per-parameter pointers (cx.params or cx.grads) as the batched (un)packing kernels take them
+static PtrTable ptr_table(const Plan& P, const float* const* p) {
+  PtrTable tbl;
+  memset(&tbl, 0, sizeof(tbl));
+  for (size_t i = 0; i < P.params.size(); ++i) tbl.p[i] = p[i];
+  return tbl;
+}
+
+// First op of every forward: zero the statistics arena, upload the job tables into a new workspace, pack all weights (one
+// launch) and pack the network input (with_input_stats: and its channel statistics, for a GroupNorm that reads it).
+static void emit_prologue(Plan& P, int b_in, bool with_input_stats) {
+  if (with_input_stats) need_stats(P, b_in);
+  push_op(P.fwd, "pack_weights+input_pack", [&P, b_in, with_input_stats](RunCtx& cx) -> int {
+    B200_CHECK_CUDA(cudaMemsetAsync(cx.ws + P.stats_off, 0, P.stats_bytes, cx.st));
+    if (P.jobs_uploaded_for != cx.ws) {     // (re)upload the constant job tables into this workspace
+      std::vector<PackJob> all(P.pack_jobs);
+      all.insert(all.end(), P.unpack_jobs.begin(), P.unpack_jobs.end());
+      B200_CHECK_CUDA(cudaMemcpyAsync(cx.ws + P.jobs_off, all.data(), sizeof(PackJob) * all.size(), cudaMemcpyHostToDevice, cx.st));
+      B200_CHECK_CUDA(cudaStreamSynchronize(cx.st));   // `all` is a temporary; happens once per workspace
+      P.jobs_uploaded_for = cx.ws;
+    }
+    if (!cx.skip_pack)
+      LAUNCHED(cx, CAT_PACK, launch_pack_all(ptr_table(P, cx.params), reinterpret_cast<const PackJob*>(cx.ws + P.jobs_off),
+                                             (int)P.pack_jobs.size(), cx.ws, P.split, cx.st));
+    TRef t = full(P, b_in);
+    LAUNCHED(cx, CAT_RESAMPLE, launch_input_pack(cx.x, P.d.n_features, act_of(P, cx, t), with_input_stats ? stats_ptr(P, cx, t) : nullptr,
+                                                 P.bufs[b_in].C, cx.st));
+    return OK;
+  });
+}
+
+// first op of every backward: zero the backward statistics and the weight-gradient accumulators
+static void emit_bwd_memset(Plan& P) {
+  push_op(P.bwd, "memset", [&P](RunCtx& cx) -> int {
+    B200_CHECK_CUDA(cudaMemsetAsync(cx.ws + P.bz_off, 0, P.bz_bytes, cx.st));
+    return OK;
+  });
+}
+
+// The 1x1x1 head (bias_param >= 0: with a bias).  Training plans also get its backward op; returns the gradient of Xfinal
+// (kNone in a forward-only plan).
+static TRef emit_head(Plan& P, TRef Xfinal, int w_param, int bias_param) {
+  P.head_param = w_param;
+  push_op(P.fwd, "head_fwd", [&P, Xfinal, bias_param](RunCtx& cx) -> int {
+    LAUNCHED(cx, CAT_HEAD, launch_head_fwd(act_of(P, cx, Xfinal), cx.params[P.head_param], P.d.n_outputs, P.d.activation, cx.logits, cx.st,
+                                           bias_param >= 0 ? cx.params[bias_param] : nullptr));
+    return OK;
+  });
+  if (P.infer) return kNone;
+  const Buf xb = P.bufs[Xfinal.buf];
+  const TRef g = full(P, new_buf(P, xb.N, xb.D, xb.H, xb.W, Xfinal.c));
+  touch(P, w_param);
+  touch(P, bias_param);
+  push_op(P.bwd, "head_bwd", [&P, Xfinal, g, bias_param](RunCtx& cx) -> int {
+    float* scratch = reinterpret_cast<float*>(cx.ws + P.head_part_off);
+    LAUNCHED(cx, CAT_HEAD, launch_head_bwd(act_of(P, cx, Xfinal), cx.params[P.head_param], P.d.n_outputs, cx.dlogits, act_of(P, cx, g),
+                                           cx.grads[P.head_param], cx.st, scratch));
+    if (bias_param >= 0) {
+      const Buf& b = P.bufs[Xfinal.buf];
+      LAUNCHED(cx, CAT_HEAD, launch_head_dbias(cx.dlogits, b.N, P.d.n_outputs, (long long)b.D * b.H * b.W, cx.grads[bias_param], cx.st,
+                                               scratch));
+    }
+    return OK;
+  });
+  return g;
+}
+
 // Everything pushed so far is part 0 of a two-part backward.  The op pushed here unpacks the weight gradients of part 0
 // (accumulator -> torch layout) and runs only under b200unet_plan_backward_part(part = 0): the whole-schedule call unpacks
-// every job in its last op as before.
+// every job in its last op (emit_unpack_wgrads).
 static void emit_bwd_split(Plan& P) {
   push_op(P.bwd, "unpack_wgrads (part 0)", [&P](RunCtx& cx) -> int {
     if (cx.part != 0 || P.unpack_split == 0) return OK;
-    PtrTable tbl;
-    memset(&tbl, 0, sizeof(tbl));
-    for (size_t i = 0; i < P.params.size(); ++i) tbl.p[i] = cx.grads[i];
     const PackJob* jobs = reinterpret_cast<const PackJob*>(cx.ws + P.jobs_off) + P.pack_jobs.size();
-    LAUNCHED(cx, CAT_PACK, launch_unpack_all(tbl, jobs, (int)P.unpack_split, cx.ws, cx.st));
+    LAUNCHED(cx, CAT_PACK, launch_unpack_all(ptr_table(P, cx.grads), jobs, (int)P.unpack_split, cx.ws, cx.st));
     return OK;
   });
   P.bwd_split = (int)P.bwd.size();
+}
+
+// last op of every backward: weight gradients, accumulator -> torch layout (one batched launch)
+static void emit_unpack_wgrads(Plan& P) {
+  push_op(P.bwd, "unpack_wgrads", [&P](RunCtx& cx) -> int {
+    // run as part 1 of a two-part backward, the jobs of part 0 were unpacked at the split (emit_bwd_split)
+    const size_t first = cx.part == 1 ? P.unpack_split : 0;
+    const PackJob* jobs = reinterpret_cast<const PackJob*>(cx.ws + P.jobs_off) + P.pack_jobs.size() + first;
+    LAUNCHED(cx, CAT_PACK, launch_unpack_all(ptr_table(P, cx.grads), jobs, (int)(P.unpack_jobs.size() - first), cx.ws, cx.st));
+    return OK;
+  });
 }
 
 // ------------------------------------------------------------------------------------------------ residual block
@@ -669,27 +755,7 @@ static int build_unet3d(Plan& P) {
   // ---------------- forward
   const int Cp_in = round_up(d.n_features, 8);
   const int b_in = new_buf(P, N, Ds[0], Hs[0], Ws[0], Cp_in);
-  need_stats(P, b_in);
-  push_op(P.fwd, "pack_weights+input_pack", [&P, b_in](RunCtx& cx) -> int {
-    B200_CHECK_CUDA(cudaMemsetAsync(cx.ws + P.stats_off, 0, P.stats_bytes, cx.st));
-    if (P.jobs_uploaded_for != cx.ws) {     // (re)upload the constant job tables into this workspace
-      std::vector<PackJob> all(P.pack_jobs);
-      all.insert(all.end(), P.unpack_jobs.begin(), P.unpack_jobs.end());
-      B200_CHECK_CUDA(cudaMemcpyAsync(cx.ws + P.jobs_off, all.data(), sizeof(PackJob) * all.size(), cudaMemcpyHostToDevice, cx.st));
-      B200_CHECK_CUDA(cudaStreamSynchronize(cx.st));   // `all` is a temporary; happens once per workspace
-      P.jobs_uploaded_for = cx.ws;
-    }
-    if (!cx.skip_pack) {
-      PtrTable tbl;
-      memset(&tbl, 0, sizeof(tbl));
-      for (size_t i = 0; i < P.params.size(); ++i) tbl.p[i] = cx.params[i];
-      LAUNCHED(cx, CAT_PACK, launch_pack_all(tbl, reinterpret_cast<const PackJob*>(cx.ws + P.jobs_off), (int)P.pack_jobs.size(),
-                                             cx.ws, P.split, cx.st));
-    }
-    TRef t = full(P, b_in);
-    LAUNCHED(cx, CAT_RESAMPLE, launch_input_pack(cx.x, P.d.n_features, act_of(P, cx, t), stats_ptr(P, cx, t), P.bufs[b_in].C, cx.st));
-    return OK;
-  });
+  emit_prologue(P, b_in, /*with_input_stats=*/true);
 
   std::vector<std::vector<BlockRec>> enc(L), dec(L);
   std::vector<int> cat(L, -1), down(L, -1);
@@ -791,35 +857,15 @@ static int build_unet3d(Plan& P) {
       cin = d.base_width;
     }
   }
-  const TRef Xfinal = X;
-  P.head_param = P.find_param("final_convolution.weight");
-  push_op(P.fwd, "head_fwd", [&P, Xfinal](RunCtx& cx) -> int {
-    LAUNCHED(cx, CAT_HEAD, launch_head_fwd(act_of(P, cx, Xfinal), cx.params[P.head_param], P.d.n_outputs, P.d.activation, cx.logits,
-                                 cx.st));
-    return OK;
-  });
+  if (!P.infer) {
+    B200_REQUIRE(d.activation == 0, E_UNSUPPORTED,
+                 "plan: activation inside the model (sigmoid/softmax) is inference-only; train on logits");
+    emit_bwd_memset(P);
+  }
+  TRef g = emit_head(P, X, P.find_param("final_convolution.weight"), -1);
 
   // ---------------- backward (training plans only)
   if (!P.infer) {
-  B200_REQUIRE(d.activation == 0, E_UNSUPPORTED,
-               "plan: activation inside the model (sigmoid/softmax) is inference-only; train on logits");
-  push_op(P.bwd, "memset", [&P](RunCtx& cx) -> int {
-    B200_CHECK_CUDA(cudaMemsetAsync(cx.ws + P.bz_off, 0, P.bz_bytes, cx.st));
-    return OK;
-  });
-  TRef g;
-  {
-    const Buf xb = P.bufs[Xfinal.buf];
-    g = full(P, new_buf(P, N, xb.D, xb.H, xb.W, Xfinal.c));
-    TRef gg = g;
-    touch(P, P.head_param);
-    push_op(P.bwd, "head_bwd", [&P, Xfinal, gg](RunCtx& cx) -> int {
-      LAUNCHED(cx, CAT_HEAD, launch_head_bwd(act_of(P, cx, Xfinal), cx.params[P.head_param], P.d.n_outputs, cx.dlogits,
-                                   act_of(P, cx, gg), cx.grads[P.head_param], cx.st,
-                                   reinterpret_cast<float*>(cx.ws + P.head_part_off)));
-      return OK;
-    });
-  }
   for (int b = d.decoder_blocks[L - 1] - 1; b >= 0; --b) g = build_block_bwd(P, dec[L - 1][b], g);
   std::vector<TRef> dskip_dec(L, kNone);
   for (int i = L - 2; i >= 0; --i) {
@@ -866,33 +912,13 @@ static int build_unet3d(Plan& P) {
       TRef gS = full(P, new_buf(P, N, Ds[lj], Hs[lj], Ws[lj], widths[lj]));
       // dropout scale belongs to the output of encoder block (0,0): that is this tensor iff level 0 has one block
       const bool sc = (lj == 0 && d.encoder_blocks[0] == 1);
-      static const bool zero_insert = getenv("B200UNET_S2_ZERO_INSERT") != nullptr;   // A/B switch: the round-1 formulation
-      if (zero_insert) {
-        TRef Z = full(P, new_buf(P, N, Ds[lj], Hs[lj], Ws[lj], widths[lj]));
-        push_op(P.bwd, "zero_insert " + shape_of(P, Z), [&P, gin, Z](RunCtx& cx) -> int {
-          LAUNCHED(cx, CAT_RESAMPLE, launch_zero_insert(act_of(P, cx, gin), act_of(P, cx, Z), 0, 0, 0, cx.st));
-          return OK;
-        });
-        emit_dgrad(P, down[lj], Z, gS, -1, kNone, dskip_dec[lj], sc, conv_macs(P, down[lj], gin));
-      } else {
-        // eight parity-class implicit GEMMs over the un-inserted gradient (27 tap products instead of 8 x 27), TMA-stored
-        // into their interleaved positions
-        emit_dgrad(P, down[lj], gin, gS, -1, kNone, dskip_dec[lj], sc, conv_macs(P, down[lj], gin), /*cls_mode=*/true);
-      }
+      // eight parity-class implicit GEMMs over the un-inserted gradient (27 tap products instead of 8 x 27), TMA-stored
+      // into their interleaved positions
+      emit_dgrad(P, down[lj], gin, gS, -1, kNone, dskip_dec[lj], sc, conv_macs(P, down[lj], gin), /*cls_mode=*/true);
       g = gS;
     }
   }
-  // weight gradients: accumulator -> torch layout (one batched launch)
-  push_op(P.bwd, "unpack_wgrads", [&P](RunCtx& cx) -> int {
-    PtrTable tbl;
-    memset(&tbl, 0, sizeof(tbl));
-    for (size_t i = 0; i < P.params.size(); ++i) tbl.p[i] = cx.grads[i];
-    // run as part 1 of a two-part backward, the jobs of part 0 were unpacked at the split (emit_bwd_split)
-    const size_t first = cx.part == 1 ? P.unpack_split : 0;
-    const PackJob* jobs = reinterpret_cast<const PackJob*>(cx.ws + P.jobs_off) + P.pack_jobs.size() + first;
-    LAUNCHED(cx, CAT_PACK, launch_unpack_all(tbl, jobs, (int)(P.unpack_jobs.size() - first), cx.ws, cx.st));
-    return OK;
-  });
+  emit_unpack_wgrads(P);
   }  // !P.infer
   return finish_build(P);
 }
@@ -1071,26 +1097,7 @@ static int build_dynunet(Plan& P) {
   // ---- forward
   const int Cp_in = round_up(d.n_features, 8);
   const int b_in = new_buf(P, N, Ds[0], Hs[0], Ws[0], Cp_in);
-  push_op(P.fwd, "pack_weights+input_pack", [&P, b_in](RunCtx& cx) -> int {
-    B200_CHECK_CUDA(cudaMemsetAsync(cx.ws + P.stats_off, 0, P.stats_bytes, cx.st));
-    if (P.jobs_uploaded_for != cx.ws) {
-      std::vector<PackJob> all(P.pack_jobs);
-      all.insert(all.end(), P.unpack_jobs.begin(), P.unpack_jobs.end());
-      B200_CHECK_CUDA(cudaMemcpyAsync(cx.ws + P.jobs_off, all.data(), sizeof(PackJob) * all.size(), cudaMemcpyHostToDevice, cx.st));
-      B200_CHECK_CUDA(cudaStreamSynchronize(cx.st));
-      P.jobs_uploaded_for = cx.ws;
-    }
-    if (!cx.skip_pack) {
-      PtrTable tbl;
-      memset(&tbl, 0, sizeof(tbl));
-      for (size_t i = 0; i < P.params.size(); ++i) tbl.p[i] = cx.params[i];
-      LAUNCHED(cx, CAT_PACK, launch_pack_all(tbl, reinterpret_cast<const PackJob*>(cx.ws + P.jobs_off), (int)P.pack_jobs.size(), cx.ws,
-                                             P.split, cx.st));
-    }
-    TRef t = full(P, b_in);
-    LAUNCHED(cx, CAT_RESAMPLE, launch_input_pack(cx.x, P.d.n_features, act_of(P, cx, t), nullptr, P.bufs[b_in].C, cx.st));
-    return OK;
-  });
+  emit_prologue(P, b_in, /*with_input_stats=*/false);
   std::vector<int> cat(L, -1);
   for (int i = 0; i + 1 < L; ++i) cat[i] = new_buf(P, N, Ds[i], Hs[i], Ws[i], 2 * F[i]);
   std::vector<DynBlock> enc(L), dec(L);
@@ -1119,10 +1126,7 @@ static int build_dynunet(Plan& P) {
         memset(&op, 0, sizeof(op));
         op.nsrc = 1;
         op.cls_mode = 2;
-        op.src[0].x = act_of(P, cx, Xin);
-        op.src[0].w_hi = reinterpret_cast<bf16*>(cx.ws + c.wf_hi);
-        op.src[0].w_lo = P.split ? reinterpret_cast<bf16*>(cx.ws + c.wf_lo) : nullptr;
-        op.src[0].ksz = 2; op.src[0].nopad = 1; op.src[0].stride = 1; op.src[0].Cip = c.Cip;
+        op.src[0] = conv_src(P, cx, c, Xin, false);
         op.Cop = c.Cop;
         op.out = act_of(P, cx, U);
         LAUNCHED(cx, CAT_CONV_FWD, launch_igemm_conv(op, cx.st));
@@ -1134,38 +1138,14 @@ static int build_dynunet(Plan& P) {
     dec[hi] = build_dyn_block_fwd(P, pre + ".conv_block", full(P, cat[hi]), 2 * F[hi], F[hi], 1, dest, false, /*x_dead=*/true);
     X = dest;
   }
-  const TRef Xfinal = X;
-  P.head_param = P.find_param("output_block.conv.conv.weight");
-  const int head_bias = P.find_param("output_block.conv.conv.bias");
-  push_op(P.fwd, "head_fwd", [&P, Xfinal, head_bias](RunCtx& cx) -> int {
-    LAUNCHED(cx, CAT_HEAD, launch_head_fwd(act_of(P, cx, Xfinal), cx.params[P.head_param], P.d.n_outputs, P.d.activation, cx.logits, cx.st,
-                                           cx.params[head_bias]));
-    return OK;
-  });
+  if (!P.infer) {
+    B200_REQUIRE(d.activation == 0, E_UNSUPPORTED, "plan: activation inside the model is inference-only; train on logits");
+    emit_bwd_memset(P);
+  }
+  TRef g = emit_head(P, X, P.find_param("output_block.conv.conv.weight"), P.find_param("output_block.conv.conv.bias"));
   if (P.infer) return finish_build(P);
 
   // ---- backward
-  B200_REQUIRE(d.activation == 0, E_UNSUPPORTED, "plan: activation inside the model is inference-only; train on logits");
-  push_op(P.bwd, "memset", [&P](RunCtx& cx) -> int {
-    B200_CHECK_CUDA(cudaMemsetAsync(cx.ws + P.bz_off, 0, P.bz_bytes, cx.st));
-    return OK;
-  });
-  TRef g;
-  {
-    const Buf xb = P.bufs[Xfinal.buf];
-    g = full(P, new_buf(P, N, xb.D, xb.H, xb.W, Xfinal.c));
-    TRef gg = g;
-    touch(P, P.head_param);
-    touch(P, head_bias);
-    push_op(P.bwd, "head_bwd", [&P, Xfinal, gg, head_bias](RunCtx& cx) -> int {
-      LAUNCHED(cx, CAT_HEAD, launch_head_bwd(act_of(P, cx, Xfinal), cx.params[P.head_param], P.d.n_outputs, cx.dlogits, act_of(P, cx, gg),
-                                             cx.grads[P.head_param], cx.st, reinterpret_cast<float*>(cx.ws + P.head_part_off)));
-      const Buf& b = P.bufs[Xfinal.buf];
-      LAUNCHED(cx, CAT_HEAD, launch_head_dbias(cx.dlogits, b.N, P.d.n_outputs, (long long)b.D * b.H * b.W, cx.grads[head_bias], cx.st,
-                                               reinterpret_cast<float*>(cx.ws + P.head_part_off)));
-      return OK;
-    });
-  }
   std::vector<TRef> dskip(L, kNone);
   for (int hi = 0; hi + 1 < L; ++hi) {     // decoder, top (level 0) to bottom
     const int lo = hi + 1;
@@ -1199,10 +1179,7 @@ static int build_dynunet(Plan& P) {
       ConvOp op;
       memset(&op, 0, sizeof(op));
       op.nsrc = 1;
-      op.src[0].x = act_of(P, cx, dU);
-      op.src[0].w_hi = reinterpret_cast<bf16*>(cx.ws + c.wd_hi);
-      op.src[0].w_lo = P.split ? reinterpret_cast<bf16*>(cx.ws + c.wd_lo) : nullptr;
-      op.src[0].ksz = 2; op.src[0].nopad = 1; op.src[0].stride = 2; op.src[0].Cip = c.Cop;
+      op.src[0] = conv_src(P, cx, c, dU, true);
       op.Cop = c.Cip;
       op.out = act_of(P, cx, gX);
       LAUNCHED(cx, CAT_CONV_DGRAD, launch_igemm_conv(op, cx.st));
@@ -1219,20 +1196,32 @@ static int build_dynunet(Plan& P) {
     // decoder, bottleneck and (six-level nets) the level above it are done
     if (i == (L >= 4 ? L - 2 : L - 1) && i > 0) emit_bwd_split(P);
   }
-  push_op(P.bwd, "unpack_wgrads", [&P](RunCtx& cx) -> int {
-    PtrTable tbl;
-    memset(&tbl, 0, sizeof(tbl));
-    for (size_t i = 0; i < P.params.size(); ++i) tbl.p[i] = cx.grads[i];
-    // run as part 1 of a two-part backward, the jobs of part 0 were unpacked at the split (emit_bwd_split)
-    const size_t first = cx.part == 1 ? P.unpack_split : 0;
-    const PackJob* jobs = reinterpret_cast<const PackJob*>(cx.ws + P.jobs_off) + P.pack_jobs.size() + first;
-    LAUNCHED(cx, CAT_PACK, launch_unpack_all(tbl, jobs, (int)(P.unpack_jobs.size() - first), cx.ws, cx.st));
-    return OK;
-  });
+  emit_unpack_wgrads(P);
   return finish_build(P);
 }
 
 static int build(Plan& P) { return P.d.arch == 1 ? build_dynunet(P) : build_unet3d(P); }
+
+// runs ops [first, last) of a schedule.  B200UNET_CAPTURE_DEBUG=1: after every op, check whether it invalidated an ongoing
+// CUDA-graph capture of the stream, and name it if so.
+static int run_ops(Plan& P, const std::vector<OpFn>& list, size_t first, size_t last, RunCtx& cx, const char* who) {
+  static const bool capdbg = getenv("B200UNET_CAPTURE_DEBUG") != nullptr;
+  for (size_t i = first; i < last; ++i) {
+    int s = list[i](cx);
+    if (s != OK) return s;
+    if (capdbg) {
+      cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+      cudaError_t e = cudaStreamIsCapturing(cx.st, &cs);
+      if (e != cudaSuccess || cs == cudaStreamCaptureStatusInvalidated) {
+        set_error("%s: stream capture invalidated at op '%s' (%s)", who, cx.label ? cx.label : "?", cudaGetErrorString(e));
+        cudaGetLastError();
+        return E_CUDA;
+      }
+    }
+  }
+  P.last_launches = cx.launches;
+  return OK;
+}
 
 }  // namespace b200
 
@@ -1285,12 +1274,8 @@ int b200unet_plan_forward(b200unet_plan* plan, const float* x, const float* cons
     return E_INVALID;
   }
   if (!plan || !x || !params || !workspace || !logits) { set_error("plan_forward: null argument"); return E_INVALID; }
-  RunCtx cx;
-  memset(&cx, 0, sizeof(cx));
-  cx.ws = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023));
+  RunCtx cx(workspace, stream, plan->prof);
   cx.params = params; cx.x = x; cx.logits = logits;
-  cx.st = reinterpret_cast<cudaStream_t>(stream);
-  cx.prof = plan->prof;
   cx.skip_pack = skip_pack && plan->jobs_uploaded_for == cx.ws;   // only valid on a workspace that has been packed before
   plan->have_drop = dropout_scale != nullptr;
   if (dropout_scale) {
@@ -1299,22 +1284,7 @@ int b200unet_plan_forward(b200unet_plan* plan, const float* x, const float* cons
                         cx.st) != cudaSuccess) { set_error("plan_forward: dropout copy failed"); return E_CUDA; }
     cx.drop = dst;
   }
-  static const bool capdbg = getenv("B200UNET_CAPTURE_DEBUG") != nullptr;
-  for (auto& op : plan->fwd) {
-    int s = op(cx);
-    if (s != OK) return s;
-    if (capdbg) {   // which op (if any) invalidates an ongoing CUDA-graph capture of this stream?
-      cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-      cudaError_t e = cudaStreamIsCapturing(cx.st, &cs);
-      if (e != cudaSuccess || cs == cudaStreamCaptureStatusInvalidated) {
-        set_error("plan_forward: stream capture invalidated at op '%s' (%s)", cx.label ? cx.label : "?", cudaGetErrorString(e));
-        cudaGetLastError();
-        return E_CUDA;
-      }
-    }
-  }
-  plan->last_launches = cx.launches;
-  return OK;
+  return run_ops(*plan, plan->fwd, 0, plan->fwd.size(), cx, "plan_forward");
 }
 
 static int run_backward(b200unet_plan* plan, const float* dlogits, const float* const* params, float* const* grads, void* workspace,
@@ -1325,32 +1295,13 @@ static int run_backward(b200unet_plan* plan, const float* dlogits, const float* 
     set_error("plan_backward_part: part %d of a schedule with %d part(s)", part, plan->bwd_split < 0 ? 1 : 2);
     return E_INVALID;
   }
-  RunCtx cx;
-  memset(&cx, 0, sizeof(cx));
-  cx.ws = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023));
+  RunCtx cx(workspace, stream, plan->prof);
   cx.params = params; cx.grads = grads; cx.dlogits = dlogits;
-  cx.st = reinterpret_cast<cudaStream_t>(stream);
-  cx.prof = plan->prof;
   cx.part = part;
   if (plan->have_drop) cx.drop = reinterpret_cast<float*>(cx.ws + plan->drop_off);
-  static const bool capdbg = getenv("B200UNET_CAPTURE_DEBUG") != nullptr;
   const size_t first = part == 1 ? (size_t)plan->bwd_split : 0;
   const size_t last = part == 0 ? (size_t)plan->bwd_split : plan->bwd.size();
-  for (size_t i = first; i < last; ++i) {
-    int s = plan->bwd[i](cx);
-    if (s != OK) return s;
-    if (capdbg) {
-      cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-      cudaError_t e = cudaStreamIsCapturing(cx.st, &cs);
-      if (e != cudaSuccess || cs == cudaStreamCaptureStatusInvalidated) {
-        set_error("plan_backward: stream capture invalidated at op '%s' (%s)", cx.label ? cx.label : "?", cudaGetErrorString(e));
-        cudaGetLastError();
-        return E_CUDA;
-      }
-    }
-  }
-  plan->last_launches = cx.launches;
-  return OK;
+  return run_ops(*plan, plan->bwd, first, last, cx, "plan_backward");
 }
 
 int b200unet_plan_backward(b200unet_plan* plan, const float* dlogits, const float* const* params, float* const* grads,
@@ -1361,19 +1312,9 @@ int b200unet_plan_backward(b200unet_plan* plan, const float* dlogits, const floa
 int b200unet_plan_input_grad(b200unet_plan* plan, float* dx, void* workspace, void* stream) {
   if (!plan || !dx || !workspace) { set_error("plan_input_grad: null argument"); return E_INVALID; }
   if (!plan->input_grad) { set_error("plan_input_grad: this plan was created without input_grad=1"); return E_INVALID; }
-  RunCtx cx;
-  memset(&cx, 0, sizeof(cx));
-  cx.ws = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023));
+  RunCtx cx(workspace, stream, plan->prof);
   cx.dx = dx;
-  cx.st = reinterpret_cast<cudaStream_t>(stream);
-  cx.prof = plan->prof;
-  cx.part = -1;
-  for (auto& op : plan->igrad) {
-    int s = op(cx);
-    if (s != OK) return s;
-  }
-  plan->last_launches = cx.launches;
-  return OK;
+  return run_ops(*plan, plan->igrad, 0, plan->igrad.size(), cx, "plan_input_grad");
 }
 
 int b200unet_plan_backward_parts(const b200unet_plan* plan) { return (!plan || plan->infer) ? 0 : plan->bwd_split >= 0 ? 2 : 1; }

@@ -226,4 +226,36 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
+// 8 consecutive channels (one 16-byte vector) of a bf16 tensor: value = hi (+ lo in split precision, lo != nullptr)
+__device__ __forceinline__ void load8(const __nv_bfloat16* hi, const __nv_bfloat16* lo, long long off, float (&v)[8]) {
+  uint4 a = *reinterpret_cast<const uint4*>(hi + off);
+  v[0] = bf16_lo_to_f(a.x); v[1] = bf16_hi_to_f(a.x);
+  v[2] = bf16_lo_to_f(a.y); v[3] = bf16_hi_to_f(a.y);
+  v[4] = bf16_lo_to_f(a.z); v[5] = bf16_hi_to_f(a.z);
+  v[6] = bf16_lo_to_f(a.w); v[7] = bf16_hi_to_f(a.w);
+  if (lo) {
+    uint4 b = *reinterpret_cast<const uint4*>(lo + off);
+    v[0] += bf16_lo_to_f(b.x); v[1] += bf16_hi_to_f(b.x);
+    v[2] += bf16_lo_to_f(b.y); v[3] += bf16_hi_to_f(b.y);
+    v[4] += bf16_lo_to_f(b.z); v[5] += bf16_hi_to_f(b.z);
+    v[6] += bf16_lo_to_f(b.w); v[7] += bf16_hi_to_f(b.w);
+  }
+}
+
+// hi = bf16(v), lo = bf16(v - hi), both round-to-nearest-even
+__device__ __forceinline__ void store8(__nv_bfloat16* hi, __nv_bfloat16* lo, long long off, const float (&v)[8]) {
+  uint4 a;
+  a.x = pack_bf16x2(v[0], v[1]); a.y = pack_bf16x2(v[2], v[3]);
+  a.z = pack_bf16x2(v[4], v[5]); a.w = pack_bf16x2(v[6], v[7]);
+  *reinterpret_cast<uint4*>(hi + off) = a;
+  if (lo) {
+    uint4 b;
+    b.x = pack_bf16x2(v[0] - bf16_lo_to_f(a.x), v[1] - bf16_hi_to_f(a.x));
+    b.y = pack_bf16x2(v[2] - bf16_lo_to_f(a.y), v[3] - bf16_hi_to_f(a.y));
+    b.z = pack_bf16x2(v[4] - bf16_lo_to_f(a.z), v[5] - bf16_hi_to_f(a.z));
+    b.w = pack_bf16x2(v[6] - bf16_lo_to_f(a.w), v[7] - bf16_hi_to_f(a.w));
+    *reinterpret_cast<uint4*>(lo + off) = b;
+  }
+}
+
 }  // namespace b200

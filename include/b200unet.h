@@ -50,7 +50,8 @@ int b200unet_ndhwc_to_ncdhw(const b200unet_tensor* in, int c_real, float* y, voi
  *   mode 0: [T][Cop][Cip]  forward;  mode 1: [T][Cip][Cop] taps flipped (data gradient);
  *   mode 2: ConvTranspose3d weight [Ci][Co][k^3] (decoder.py:101-102) -> [T][Cop][Cip] flipped;
  *   mode 3: the same weight -> [T][Cip][Cop] unflipped (its data gradient);  mode 4: -> [T][Cop][Cip] unflipped
- *   (forward of a kernel = stride transposed convolution, MONAI UnetUpBlock). */
+ *   (forward of a kernel = stride transposed convolution, MONAI UnetUpBlock).
+ *   Both entry points: cop and cip multiples of 8 and 1 <= taps <= 27, else B200UNET_E_UNSUPPORTED. */
 int b200unet_pack_weights(const float* w, int co, int ci, int cop, int cip, int taps, int mode, void* hi, void* lo,
                           void* stream);
 /* fp32 [T][Cip][Cop] accumulator -> torch gradient layout (mode 0: [Co][Ci][T]; mode 2: [Ci][Co][T] flipped) */

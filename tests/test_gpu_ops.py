@@ -419,6 +419,19 @@ def test_dice_edge_cases(pkg):
         crit(z, t0[:, :1])
 
 
+def _packed_layout(w, mode, cop, cip):
+    """fp32 restatement of a packed weight (kernels.h PackJob.mode), zero padded to (cop, cip)"""
+    if mode >= 2:                                   # ConvTranspose3d weight [Ci][Co][k^3]
+        w = w.transpose(0, 1)
+    co, ci = w.shape[:2]
+    t = w.reshape(co, ci, -1)
+    if mode in (1, 2):                              # taps flipped
+        t = t.flip(2)
+    out = torch.zeros(t.shape[2], cop, cip)
+    out[:, :co, :ci] = t.permute(2, 0, 1)
+    return out.transpose(1, 2) if mode in (1, 3) else out   # data-gradient layouts: [T][Cip][Cop]
+
+
 def test_weight_pack_unpack_roundtrip(pkg):
     L = pkg.lib
     torch.manual_seed(8)
@@ -429,6 +442,28 @@ def test_weight_pack_unpack_roundtrip(pkg):
     assert float(hi[:, :, 12:].float().abs().max()) == 0.0
     hi, lo, _, _, _ = L.pack_weights(w, 1, split=True, cip=16)
     assert rel((hi.float() + lo.float())[:, :12, :24], w.flip(2, 3, 4).permute(2, 3, 4, 1, 0).reshape(27, 12, 24)) < 1e-5
+    # packed bits: hi and lo round to nearest even, exactly as torch's own conversion does
+    for shape, modes in [((24, 12, 3, 3, 3), range(5)),
+                         ((320, 256, 3, 3, 3), (0, 1)),      # more 16 x 16 tiles than blocks
+                         ((16, 8, 2, 2, 2), (3, 4)),         # T = 8 ConvTranspose3d weight [Ci][Co][2][2][2]
+                         ((40, 12, 1, 1, 1), (0, 1))]:       # T = 1
+        w = torch.randn(*shape, device=DEV)
+        for mode in modes:
+            hi, lo, cop, cip, _ = L.pack_weights(w, mode, split=True)
+            ref = _packed_layout(w.cpu(), mode, cop, cip)
+            ref_hi = ref.bfloat16()
+            assert torch.equal(hi.cpu(), ref_hi), (shape, mode)
+            assert torch.equal(lo.cpu(), (ref - ref_hi.float()).bfloat16()), (shape, mode)
+    # unpacking is an exact copy: fp32 [T][Cip][Cop] -> [Co][Ci][T] (mode 0) or, taps flipped back, [Ci][Co][T] (mode 2)
+    co, ci, cop, cip, T = 20, 12, 24, 16, 27
+    g = torch.randn(T, cip, cop, device=DEV)
+    for mode, ref in [(0, g[:, :ci, :co].permute(2, 1, 0)), (2, g.flip(0)[:, :ci, :co].permute(1, 2, 0))]:
+        out = torch.empty(ref.shape, device=DEV)
+        L.check(L.load_library().b200unet_unpack_wgrad(g.data_ptr(), co, ci, cop, cip, T, mode, out.data_ptr(), L.stream_ptr()))
+        assert torch.equal(out, ref.contiguous()), mode
+    # the packed layouts are written in 8-channel chunks
+    with pytest.raises(RuntimeError, match="multiples of 8"):
+        L.pack_weights(w, 0, cip=12)
 
 
 def test_errors_are_loud(pkg):

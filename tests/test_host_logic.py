@@ -204,106 +204,6 @@ def test_transposed_conv_k2s2_roles():
     assert torch.allclose(dw, w.grad)
 
 
-# ------------------------------------------------------------------------------------------------ B200 halo-kernel bookkeeping
-# Restatements of the index arithmetic of the B200 halo kernels (kd-stacked tcgen05 MMAs of the convolution and the weight
-# gradient, incremental and three-box weight-stage offsets, multiply-high tile decode).  No sm_90a kernel uses this arithmetic:
-# the Hopper halo mode of csrc/igemm_conv.cu issues one tap per wgmma from directly computed row offsets (checked by
-# test_conv_halo_descriptor_rows_cover_the_tap_neighbourhood above).
-@pytest.mark.parametrize("TD", [1, 2, 4])
-def test_conv_halo_kd_stacking_covers_every_plane_tap_pair_once(TD):
-    seen = {}
-    for hq in range(TD + 2):                                   # halo plane = input depth d0 - 1 + hq
-        kdmin = max(0, hq - (TD - 1))
-        kdmax = min(2, hq)
-        nkd = kdmax - kdmin + 1
-        assert 1 <= nkd <= 3
-        d_slot0 = TD - 1 - hq + kdmin                          # accumulators sit in DESCENDING plane order (units of BN)
-        assert 0 <= d_slot0 and d_slot0 + nkd <= TD            # the N-stacked MMA stays inside the tile's accumulators
-        for j in range(nkd):
-            kd = kdmin + j                                     # weight row block kdmin + j  <->  column block d_slot0 + j
-            plane = TD - 1 - (d_slot0 + j)
-            assert plane == hq - kd                            # tap kd of output plane p reads halo plane p + kd
-            assert (plane, kd) not in seen
-            seen[(plane, kd)] = hq
-    assert sorted(seen) == [(p, kd) for p in range(TD) for kd in range(3)]
-
-
-@pytest.mark.parametrize("TD", [2, 4])
-def test_wgrad_halo_kd_stacking_pairs_each_halo_plane_with_the_right_dy_planes(TD):
-    seen = set()
-    for hq in range(TD + 2):
-        kdmin = max(0, hq - (TD - 1))
-        kdmax = min(2, hq)
-        nkd = kdmax - kdmin + 1
-        blk0 = 2 - kdmax                                       # column block b holds kd = 2 - b
-        dy0 = hq - kdmax                                       # first dY plane of the N atoms (ascending addresses)
-        assert 0 <= dy0 and dy0 + nkd <= TD and 0 <= blk0 and blk0 + nkd <= 3
-        for j in range(nkd):
-            kd = 2 - (blk0 + j)
-            assert dy0 + j == hq - kd                          # dY plane d pairs with input plane d + kd
-            seen.add((dy0 + j, kd))
-    assert seen == {(p, kd) for p in range(TD) for kd in range(3)}
-
-
-@pytest.mark.parametrize("stacked", [True, False])
-def test_conv_halo_incremental_tap_offsets(stacked):
-    """the rolled stage loop advances the A-descriptor offset incrementally (kw fastest, then kh, then kd)"""
-    rb = 4                                                     # halo row bytes >> 4 for KC = 32
-    a_off, kw, kh = 0, 0, 0
-    for st in range(9 if stacked else 27):
-        kd_, kh_, kw_ = (0, st // 3, st % 3) if stacked else (st // 9, (st // 3) % 3, st % 3)
-        assert a_off == ((kd_ * 18 + kh_) * 10 + kw_) * rb
-        a_off += rb
-        kw += 1
-        if kw == 3:
-            kw = 0
-            a_off += 7 * rb
-            kh += 1
-            if kh == 3:
-                kh = 0
-                a_off += 15 * 10 * rb
-
-
-def test_conv_halo_kw_grouped_stage_offsets():
-    """BN <= 32: a weight stage holds the kw = 0,1,2 boxes of one kh (HaloCfg::KWS = 3).  Stage st = kh advances the A offset by
-    one halo row (10 voxels); box q of the stage is kw = q (+1 voxel) and sits q boxes into the stage; the TMA box index of
-    the 4-D (Cin, Cout, khkw, kd) weight view is st * 3 + q."""
-    rb = 4
-    b_box = 3 * 2048                                           # three kd tiles of a 32 x 32 tap
-    a_off = 0
-    taps = set()
-    for st in range(3):
-        for q in range(3):
-            khkw = st * 3 + q
-            assert khkw == st * 3 + q and khkw // 3 == st and khkw % 3 == q
-            a_q = a_off + q * rb
-            for kd in range(3):
-                assert a_q + kd * 180 * rb == ((kd * 18 + st) * 10 + q) * rb
-                taps.add((kd, st, q, q * b_box + kd * 2048))    # B operand offset inside the stage
-        a_off += 10 * rb
-    assert len(taps) == 27 and len({t[3] for t in taps}) == 9   # 9 distinct tile offsets per stage x 3 stages
-
-
-def test_tile_decode_fast_division_restatement():
-    """conv_halo_kernel.cuh make_fastdiv / fast_divmod: q = umulhi(x, mul) >> shr with p = 31 + ceil(log2 d), mul = ceil(2^p / d),
-    shr = p - 32 must equal x // d for every tile index (x < 2^31) and every tile-count divisor."""
-    import random
-
-    def mk(d):
-        if d <= 1:
-            return 0, 0
-        lg = d.bit_length() - 1 + (1 if d & (d - 1) else 0)
-        p = 31 + lg
-        return ((1 << p) + d - 1) // d, p - 32
-    rnd = random.Random(0)
-    for d in list(range(1, 300)) + [511, 512, 513, 1000, 4096, 65535]:
-        mul, shr = mk(d)
-        assert mul < 2 ** 32
-        for x in list(range(0, 600)) + [rnd.randrange(0, 2 ** 31) for _ in range(300)] + [2 ** 31 - 1]:
-            q = (((x * mul) >> 32) >> shr) if d > 1 else x
-            assert q == x // d and x - q * d == x % d
-
-
 @pytest.mark.parametrize("n", [2, 4, 6, 10])
 def test_register_blocked_trilinear_adjoint_weights(n):
     """elementwise.cu:k_upsample2x_bwd_blk: per axis, block m (outputs 2m, 2m+1) meets dy indices 4m-1+i, i = 0..5, with the
