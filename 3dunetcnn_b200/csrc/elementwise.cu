@@ -933,7 +933,8 @@ __global__ void k_head_fwd(Act x, const float* __restrict__ w, const float* __re
 }
 
 int launch_head_fwd(const Act& x, const float* w, int n_out, int act_mode, float* logits, cudaStream_t st, const float* bias) {
-  B200_REQUIRE(n_out >= 1 && n_out <= 8, E_UNSUPPORTED, "head: n_outputs=%d > 8 unsupported", n_out);
+  if (n_out > 8) return launch_head_mma_fwd(x, w, n_out, act_mode, logits, st, bias);
+  B200_REQUIRE(n_out >= 1, E_UNSUPPORTED, "head: n_outputs=%d unsupported (1..%d)", n_out, B200_HEAD_MAX_OUTPUTS);
   B200_REQUIRE(x.C % 8 == 0, E_INVALID, "head: C=%d", x.C);
   k_head_fwd<<<ew_blocks(x.voxels(), 256), 256, n_out * x.C * sizeof(float), st>>>(x, w, bias, n_out, act_mode, logits);
   B200_CHECK_CUDA(cudaGetLastError());
@@ -1020,13 +1021,27 @@ __global__ void __launch_bounds__(128) k_sum_slots(const float* __restrict__ par
   if (threadIdx.x == 0) out[i] = s_acc[0];
 }
 
-size_t head_bwd_scratch_bytes(int n_out, int C) { return (size_t)1184 * n_out * C * sizeof(float); }
+size_t head_bwd_scratch_bytes(int n_out, int C) {
+  return n_out > 8 ? head_mma_bwd_scratch_bytes(n_out, C) : (size_t)1184 * n_out * C * sizeof(float);
+}
 
 int launch_head_bwd(const Act& x, const float* w, int n_out, const float* dlogits, const Act& dx, float* dw,
-                    cudaStream_t st, float* scratch) {
-  B200_REQUIRE(n_out >= 1 && n_out <= 8, E_UNSUPPORTED, "head_bwd: n_outputs=%d > 8 unsupported", n_out);
-  B200_REQUIRE(x.C % 8 == 0 && dx.C == x.C, E_INVALID, "head_bwd: channel mismatch");
+                    cudaStream_t st, float* scratch, float* dbias) {
   B200_REQUIRE(scratch != nullptr, E_INVALID, "head_bwd: needs head_bwd_scratch_bytes() of scratch");
+  if (n_out > 8) {   // one pass writes dx and the per-CTA partials of dw (and dbias); fixed-order slot sums follow
+    int slots = 0;
+    B200_TRY(launch_head_mma_bwd(x, w, n_out, dlogits, dx, dbias != nullptr, scratch, &slots, st));
+    k_sum_slots<<<n_out * x.C, 128, 0, st>>>(scratch, slots, n_out * x.C, dw);
+    B200_CHECK_CUDA(cudaGetLastError());
+    if (dbias) {
+      k_sum_slots<<<n_out, 128, 0, st>>>(scratch + (size_t)slots * n_out * x.C, slots, n_out, dbias);
+      B200_CHECK_CUDA(cudaGetLastError());
+    }
+    return OK;
+  }
+  B200_REQUIRE(n_out >= 1, E_UNSUPPORTED, "head_bwd: n_outputs=%d unsupported (1..%d)", n_out, B200_HEAD_MAX_OUTPUTS);
+  B200_REQUIRE(dbias == nullptr, E_INVALID, "head_bwd: the bias gradient of 1..8 outputs comes from launch_head_dbias");
+  B200_REQUIRE(x.C % 8 == 0 && dx.C == x.C, E_INVALID, "head_bwd: channel mismatch");
   const int c8n = x.C / 8;
   int threads = 256;
   while (threads % c8n) threads += 32;

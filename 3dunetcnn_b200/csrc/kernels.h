@@ -22,15 +22,26 @@ int launch_gn_bwd(const Act& dz, const Act& x, const float* coef, const float* c
 int launch_add(const Act& a, const Act& b, const Act& y, cudaStream_t st);
 int launch_upsample2x_fwd(const Act& x, const Act& y, double* stats, int stats_ld, cudaStream_t st);
 int launch_upsample2x_bwd(const Act& dy, const Act& dx, cudaStream_t st);
+// The 1x1x1 head takes 1..B200_HEAD_MAX_OUTPUTS outputs: 1..8 run the SIMT kernels below with fp32 weights, 9..128 the
+// tensor-core kernels of head.cu (launch_head_mma_*), chosen inside launch_head_fwd / launch_head_bwd from n_out alone.
+#define B200_HEAD_MAX_OUTPUTS 128
 int launch_head_fwd(const Act& x, const float* w, int n_out, int act_mode, float* logits, cudaStream_t st,
                     const float* bias = nullptr);
 int launch_head_dbias(const float* dlogits, int N, int NO, long long S, float* dbias, cudaStream_t st, float* scratch);
 // post-activation blocks: dz = (g1 [+ g2]) * act'(A c + B), bstats += (sum dz, sum dz*xhat)
 int launch_act_bwd(const Act& g1, const Act* g2, const Act& c, const float* coef, float slope, const Act& dz, double* bstats,
                    int bstats_ld, cudaStream_t st);
+// scratch: head_bwd_scratch_bytes(n_out, C) (per-block partial sums).  dbias (more than 8 outputs only; launch_head_dbias
+// serves 1..8): also write the bias gradient from the same pass.
 int launch_head_bwd(const Act& x, const float* w, int n_out, const float* dlogits, const Act& dx, float* dw,
-                    cudaStream_t st, float* scratch);   // scratch: head_bwd_scratch_bytes(n_out, C) (per-block partial sums)
+                    cudaStream_t st, float* scratch, float* dbias = nullptr);
 size_t head_bwd_scratch_bytes(int n_out, int C);
+// ---- tensor-core head, 9..128 outputs, C a multiple of 8 up to 64 (head.cu)
+int launch_head_mma_fwd(const Act& x, const float* w, int n_out, int act_mode, float* logits, cudaStream_t st, const float* bias);
+// writes the per-CTA partial sums (weight gradient, then bias gradient when want_dbias) of *slots CTAs into part
+int launch_head_mma_bwd(const Act& x, const float* w, int n_out, const float* dlogits, const Act& dx, int want_dbias, float* part,
+                        int* slots, cudaStream_t st);
+size_t head_mma_bwd_scratch_bytes(int n_out, int C);
 // ---- weight packing / gradient unpacking (small_ops.cu): shared-memory tiled transposes
 // one tensor; Cop and Cip (the padded extents) must be multiples of 8, T <= 27
 int launch_pack_weights(const float* w, int Co, int Ci, int Cop, int Cip, int T, int mode, bf16* hi, bf16* lo,
@@ -72,8 +83,8 @@ int launch_dice_bwd(const float* logits, const uint8_t* target, int N, int C, lo
 
 // ---- steps before / after the path (prepost.cu): sliding-window tiles, one-hot targets, z-score, label maps
 #define B200_MAX_TILES 16
-#define B200_MAX_LABEL_CHANNELS 16
-#define B200_MAX_LABEL_VALUES 64
+#define B200_MAX_LABEL_CHANNELS 128
+#define B200_MAX_LABEL_VALUES 256   // LabelTable (prepost.cu) stays a ~1.5 KB kernel parameter
 int launch_tiles_gather(const float* vol, int N, int C, int D, int H, int W, const int32_t* starts, int ntiles, int rd, int rh,
                         int rw, float* tiles, cudaStream_t st);
 int launch_tiles_scatter(const float* pred, int C, const int32_t* starts, int ntiles, int rd, int rh, int rw, const float* imp,

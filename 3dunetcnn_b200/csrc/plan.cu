@@ -594,7 +594,8 @@ static void emit_bwd_memset(Plan& P) {
 }
 
 // The 1x1x1 head (bias_param >= 0: with a bias).  Training plans also get its backward op; returns the gradient of Xfinal
-// (kNone in a forward-only plan).
+// (kNone in a forward-only plan).  launch_head_fwd / launch_head_bwd pick the kernels from n_outputs; above 8 outputs the
+// bias gradient comes out of the same backward pass instead of launch_head_dbias.
 static TRef emit_head(Plan& P, TRef Xfinal, int w_param, int bias_param) {
   P.head_param = w_param;
   push_op(P.fwd, "head_fwd", [&P, Xfinal, bias_param](RunCtx& cx) -> int {
@@ -609,9 +610,10 @@ static TRef emit_head(Plan& P, TRef Xfinal, int w_param, int bias_param) {
   touch(P, bias_param);
   push_op(P.bwd, "head_bwd", [&P, Xfinal, g, bias_param](RunCtx& cx) -> int {
     float* scratch = reinterpret_cast<float*>(cx.ws + P.head_part_off);
+    const bool fused_dbias = bias_param >= 0 && P.d.n_outputs > 8;
     LAUNCHED(cx, CAT_HEAD, launch_head_bwd(act_of(P, cx, Xfinal), cx.params[P.head_param], P.d.n_outputs, cx.dlogits, act_of(P, cx, g),
-                                           cx.grads[P.head_param], cx.st, scratch));
-    if (bias_param >= 0) {
+                                           cx.grads[P.head_param], cx.st, scratch, fused_dbias ? cx.grads[bias_param] : nullptr));
+    if (bias_param >= 0 && !fused_dbias) {
       const Buf& b = P.bufs[Xfinal.buf];
       LAUNCHED(cx, CAT_HEAD, launch_head_dbias(cx.dlogits, b.N, P.d.n_outputs, (long long)b.D * b.H * b.W, cx.grads[bias_param], cx.st,
                                                scratch));
@@ -737,7 +739,8 @@ static int build_unet3d(Plan& P) {
   B200_REQUIRE(L >= 2 && L <= 8, E_UNSUPPORTED, "plan: n_levels=%d unsupported (2..8)", L);
   B200_REQUIRE(d.base_width % 8 == 0, E_UNSUPPORTED, "plan: base_width=%d must be a multiple of 8", d.base_width);
   B200_REQUIRE(d.n_features >= 1 && d.n_features <= 16, E_UNSUPPORTED, "plan: n_features=%d unsupported", d.n_features);
-  B200_REQUIRE(d.n_outputs >= 1 && d.n_outputs <= 8, E_UNSUPPORTED, "plan: n_outputs=%d unsupported", d.n_outputs);
+  B200_REQUIRE(d.n_outputs >= 1 && d.n_outputs <= B200_HEAD_MAX_OUTPUTS, E_UNSUPPORTED, "plan: n_outputs=%d unsupported (1..%d)",
+               d.n_outputs, B200_HEAD_MAX_OUTPUTS);
   std::vector<int> widths, Ds, Hs, Ws;
   {
     int w = d.base_width, D = d.depth, H = d.height, W = d.width;
@@ -932,7 +935,10 @@ static int finish_build(Plan& P) {
   P.stats_off = P.alloc(P.stats_bytes);
   P.bz_off = P.alloc(P.bz_bytes);
   if (P.wg_part_bytes) P.wg_part_off = P.alloc(P.wg_part_bytes);
-  if (!P.infer) P.head_part_off = P.alloc(head_bwd_scratch_bytes(d.n_outputs, d.arch == 1 ? d.filters[0] : d.base_width));
+  const int head_c = d.arch == 1 ? d.filters[0] : d.base_width;
+  B200_REQUIRE(d.n_outputs <= 8 || head_c <= 64, E_UNSUPPORTED,
+               "plan: more than 8 outputs need at most 64 channels into the head, got %d", head_c);
+  if (!P.infer) P.head_part_off = P.alloc(head_bwd_scratch_bytes(d.n_outputs, head_c));
   for (size_t i = 0; i < P.convs.size(); ++i)
     B200_REQUIRE(P.convs[i].pw >= 0, E_INVALID, "plan: internal: conv %d has no parameter", (int)i);
   for (const ConvLayer& c : P.convs) {
@@ -1064,7 +1070,8 @@ static int build_dynunet(Plan& P) {
   const int L = d.n_levels, N = d.batch;
   B200_REQUIRE(L >= 2 && L <= 8, E_UNSUPPORTED, "plan: DynUNet with %d levels unsupported (2..8)", L);
   B200_REQUIRE(d.n_features >= 1 && d.n_features <= 16, E_UNSUPPORTED, "plan: in_channels=%d unsupported", d.n_features);
-  B200_REQUIRE(d.n_outputs >= 1 && d.n_outputs <= 8, E_UNSUPPORTED, "plan: out_channels=%d unsupported", d.n_outputs);
+  B200_REQUIRE(d.n_outputs >= 1 && d.n_outputs <= B200_HEAD_MAX_OUTPUTS, E_UNSUPPORTED, "plan: out_channels=%d unsupported (1..%d)",
+               d.n_outputs, B200_HEAD_MAX_OUTPUTS);
   P.slope = d.act_slope;
   std::vector<int> F, Ds, Hs, Ws;
   {

@@ -271,34 +271,37 @@ struct LabelMapArgs {
   int16_t labels[B200_MAX_LABEL_CHANNELS];
 };
 
+// Two passes over the channels and no per-thread array of L values (L goes up to 128): the first gives the maximum and the
+// softmax denominator, the second recomputes each activated value with the same float expression and folds it in channel order.
 __global__ void k_label_map(const float* __restrict__ p, long long S, LabelMapArgs a, int act, float thr, int hierarchy,
                             int sum_then_threshold, int16_t* __restrict__ out) {
   for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < S; v += (long long)gridDim.x * blockDim.x) {
-    float q[B200_MAX_LABEL_CHANNELS];
-    float mx = -INFINITY;
-    for (int c = 0; c < a.L; ++c) { q[c] = p[(long long)c * S + v]; mx = fmaxf(mx, q[c]); }
-    if (act == 1) {
-      for (int c = 0; c < a.L; ++c) q[c] = 1.f / (1.f + expf(-q[c]));
-    } else if (act == 2) {
-      float den = 0.f;
-      for (int c = 0; c < a.L; ++c) { q[c] = expf(q[c] - mx); den += q[c]; }
-      for (int c = 0; c < a.L; ++c) q[c] /= den;
-    }
+    float mx = -INFINITY, den = 0.f;
+    for (int c = 0; c < a.L; ++c) mx = fmaxf(mx, p[(long long)c * S + v]);
+    if (act == 2)
+      for (int c = 0; c < a.L; ++c) den += expf(p[(long long)c * S + v] - mx);
+    auto q = [&](int c) -> float {
+      const float x = p[(long long)c * S + v];
+      if (act == 1) return 1.f / (1.f + expf(-x));
+      if (act == 2) return expf(x - mx) / den;
+      return x;
+    };
     int16_t lab = 0;
     if (hierarchy) {
       bool roi = true;
       for (int c = 0; c < a.L; ++c) {
-        roi = roi && (q[c] > thr);
+        roi = roi && (q(c) > thr);
         if (roi) lab = a.labels[c];
       }
     } else {
       bool mask = false;
-      float sum = 0.f, best = q[0];
+      float sum = 0.f, best = q(0);
       int arg = 0;
       for (int c = 0; c < a.L; ++c) {
-        mask = mask || (q[c] > thr);
-        sum += q[c];
-        if (q[c] > best) { best = q[c]; arg = c; }   // torch.argmax: first maximal index
+        const float qc = q(c);
+        mask = mask || (qc > thr);
+        sum += qc;
+        if (qc > best) { best = qc; arg = c; }   // torch.argmax: first maximal index
       }
       if (sum_then_threshold) mask = sum > thr;
       if (mask) lab = a.labels[arg];

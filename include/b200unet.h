@@ -110,9 +110,13 @@ int b200unet_upsample2x_fwd(const b200unet_tensor* x, const b200unet_tensor* y, 
 int b200unet_upsample2x_bwd(const b200unet_tensor* dy, const b200unet_tensor* dx, void* stream);
 int b200unet_zero_insert(const b200unet_tensor* x, const b200unet_tensor* z, int od, int oh, int ow, void* stream);
 
-/* ---- final 1x1x1 convolution to NCDHW fp32 logits (variational.py:59-60,84-86); act: 0 none 1 sigmoid 2 softmax */
+/* ---- final 1x1x1 convolution to NCDHW fp32 logits (variational.py:59-60,84-86); act: 0 none 1 sigmoid 2 softmax.
+ * n_out is 1..128 and picks the kernels: 1..8 run a SIMT head with fp32 weights (any c that is a multiple of 8); 9..128 run
+ * a tensor-core head (bf16 MMAs with fp32 accumulation, c a multiple of 8 up to 64) that rounds the weights -- and in the
+ * backward dlogits -- to bf16, or splits them into bf16 hi + lo when x carries a lo plane.  Above 128: E_UNSUPPORTED. */
 int b200unet_head_fwd(const b200unet_tensor* x, const float* w, int n_out, int act, float* logits, void* stream);
-/* head_bwd reduces dw without floating-point atomics (bit-reproducible): `scratch` holds one partial per thread block */
+/* head_bwd reduces dw without floating-point atomics (bit-reproducible for both heads): `scratch` holds one partial per
+ * thread block */
 size_t b200unet_head_bwd_scratch_bytes(int n_out, int c);
 int b200unet_head_bwd(const b200unet_tensor* x, const float* w, int n_out, const float* dlogits,
                       const b200unet_tensor* dx, float* dw, float* scratch, void* stream);
@@ -150,7 +154,8 @@ int b200unet_one_hot(const float* data, int n, int64_t spatial, const float* val
                      int do_round, uint8_t* y, void* stream);
 int b200unet_zscore(const float* x, int groups, int64_t spatial, int nonzero, double* stats, float* y, void* stream);
 /* ---- the step after the path: activation (0 none, 1 sigmoid, 2 softmax) + threshold -> int16 label map of ONE sample
- * p [L][spatial] (utils/one_hot.py:46-118: label hierarchy, any/sum-then-threshold + argmax) */
+ * p [L][spatial] (utils/one_hot.py:46-118: label hierarchy, any/sum-then-threshold + argmax).  one_hot and label_map take
+ * 1..128 channels; one_hot at most 256 label values in all. */
 int b200unet_label_map(const float* p, int n_labels, int64_t spatial, const int32_t* labels, int act, float threshold,
                        int hierarchy, int sum_then_threshold, int16_t* out, void* stream);
 
