@@ -5,7 +5,6 @@
 #include <cstdlib>
 #include "kernels.h"
 #include "../../include/b200unet.h"
-#include "../../include/b200unet_diag.h"
 
 namespace b200 {
 static thread_local char g_err[1024] = "";
@@ -39,7 +38,7 @@ using namespace b200;
 
 extern "C" {
 
-int b200unet_version(void) { return 100; }
+int b200unet_version(void) { return 101; }
 const char* b200unet_last_error(void) { return get_error(); }
 
 int b200unet_ncdhw_to_ndhwc(const float* x, int c_real, const b200unet_tensor* out, void* stream) {
@@ -95,25 +94,11 @@ int b200unet_conv3d_wgrad(const b200unet_tensor* a, const b200unet_tensor* dy, i
   return launch_wgrad(op, to_stream(stream));
 }
 
-int b200unet_conv3d_simt(const b200unet_tensor* x, const void* w_hi, const void* w_lo, int ksz, int stride,
-                         const b200unet_tensor* y, void* stream) {
-  NOT_NULL(x); NOT_NULL(w_hi); NOT_NULL(y);
-  return launch_conv_simt(to_act(x), reinterpret_cast<const bf16*>(w_hi), reinterpret_cast<const bf16*>(w_lo), ksz,
-                          stride, to_act(y), to_stream(stream));
-}
-
-int b200unet_channel_stats(const b200unet_tensor* x, double* stats, int stats_ld, void* stream) {
-  NOT_NULL(x); NOT_NULL(stats);
-  return launch_channel_stats(to_act(x), stats, stats_ld, to_stream(stream));
-}
-int b200unet_gn_finalize(const double* stats, const float* gamma, const float* beta, int n, int c, int c_ld, int groups,
-                         int64_t spatial, float eps, float* coef, void* stream) {
-  NOT_NULL(stats); NOT_NULL(coef);
-  return launch_gn_finalize(stats, gamma, beta, n, c, c_ld, groups, spatial, eps, coef, to_stream(stream));
-}
-int b200unet_gn_apply(const b200unet_tensor* x, const b200unet_tensor* y, const float* coef, float slope, void* stream) {
-  NOT_NULL(x); NOT_NULL(y); NOT_NULL(coef);
-  return launch_gn_apply(to_act(x), to_act(y), coef, slope, to_stream(stream));
+int b200unet_gn_apply(const b200unet_tensor* x, const b200unet_tensor* y, const double* stats, const float* gamma,
+                      const float* beta, int c, int groups, float eps, float slope, float* coef, void* stream) {
+  NOT_NULL(x); NOT_NULL(y); NOT_NULL(stats); NOT_NULL(coef);
+  return launch_gn_apply(to_act(x), to_act(y), stats, gamma, beta, c, groups, (long long)x->d * x->h * x->w, eps, coef, slope,
+                         to_stream(stream));
 }
 int b200unet_gn_bwd_finalize(const double* bstats, const float* coef, const float* gamma, int n, int c, int c_ld,
                              int groups, int64_t spatial, float* coef2, float* dgamma, float* dbeta, void* stream) {
@@ -121,14 +106,15 @@ int b200unet_gn_bwd_finalize(const double* bstats, const float* coef, const floa
   return launch_gn_bwd_finalize(bstats, coef, gamma, n, c, c_ld, groups, spatial, coef2, dgamma, dbeta,
                                 to_stream(stream));
 }
-int b200unet_gn_bwd(const b200unet_tensor* dz, const b200unet_tensor* x, const float* coef, const float* coef2,
-                    const b200unet_tensor* add1, const b200unet_tensor* add2, const b200unet_tensor* dx, void* stream) {
-  NOT_NULL(dz); NOT_NULL(x); NOT_NULL(coef); NOT_NULL(coef2); NOT_NULL(dx);
+int b200unet_gn_bwd(const b200unet_tensor* dz, const b200unet_tensor* x, const float* coef, const double* bstats,
+                    const float* gamma, int c, int groups, float* dgamma, float* dbeta, const b200unet_tensor* add1,
+                    const b200unet_tensor* add2, const b200unet_tensor* dx, void* stream) {
+  NOT_NULL(dz); NOT_NULL(x); NOT_NULL(coef); NOT_NULL(bstats); NOT_NULL(dx);
   Act a1, a2;
   if (add1) a1 = to_act(add1);
   if (add2) a2 = to_act(add2);
-  return launch_gn_bwd(to_act(dz), to_act(x), coef, coef2, add1 ? &a1 : nullptr, add2 ? &a2 : nullptr, to_act(dx),
-                       nullptr, to_stream(stream));
+  return launch_gn_bwd(to_act(dz), to_act(x), coef, bstats, gamma, c, groups, (long long)x->d * x->h * x->w, dgamma, dbeta,
+                       add1 ? &a1 : nullptr, add2 ? &a2 : nullptr, to_act(dx), nullptr, to_stream(stream));
 }
 
 int b200unet_act_bwd(const b200unet_tensor* g1, const b200unet_tensor* g2, const b200unet_tensor* c, const float* coef, float slope,

@@ -1,5 +1,5 @@
 // Bandwidth-bound kernels of the U-Net path (everything that is not a tensor-core contraction):
-// input packing, GroupNorm finalize/apply/backward, trilinear x2 up-sampling fwd/bwd, 1x1x1 head fwd/bwd
+// input packing, GroupNorm apply/backward, trilinear x2 up-sampling fwd/bwd, 1x1x1 head fwd/bwd
 // and zero insertion (weight packing: small_ops.cu).  All activations are NDHWC bf16 (hi [+ lo]) views; 8 channels (16 B) per
 // thread so every access is a 128-bit vector along the innermost (channel) axis.
 //
@@ -75,105 +75,19 @@ int launch_input_pack(const float* x, int C, const Act& out, double* stats, int 
   return OK;
 }
 
-// ------------------------------------------------------------------------------------------------ channel stats (stand-alone)
-__global__ void k_channel_stats(Act x, double* __restrict__ stats, int stats_ld) {
-  // grid (blocks, N); each thread owns one 8-channel lane group and strides over voxels
-  const int n = blockIdx.y;
-  const int c8n = x.C / 8;
-  const long long S = (long long)x.D * x.H * x.W;
-  const int lane_c8 = threadIdx.x % c8n;
-  const int vslot = threadIdx.x / c8n;
-  const int vper = blockDim.x / c8n;
-  float a[8], b[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) a[j] = b[j] = 0.f;
-  if (vslot < vper) {
-    for (long long s = (long long)blockIdx.x * vper + vslot; s < S; s += (long long)gridDim.x * vper) {
-      float v[8];
-      load8(x.hi, x.lo, ((long long)n * S + s) * x.ld + lane_c8 * 8, v);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { a[j] += v[j]; b[j] += v[j] * v[j]; }
-    }
-  }
-  extern __shared__ double smd[];  // [C][2], fp64 so that the atomic order cannot reach the fp32 coefficients
-  for (int i = threadIdx.x; i < x.C * 2; i += blockDim.x) smd[i] = 0.0;
-  __syncthreads();
-  if (vslot < vper) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      atomicAdd(&smd[(lane_c8 * 8 + j) * 2 + 0], (double)a[j]);
-      atomicAdd(&smd[(lane_c8 * 8 + j) * 2 + 1], (double)b[j]);
-    }
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < x.C * 2; i += blockDim.x) atomicAdd(&stats[(long long)n * stats_ld * 2 + i], smd[i]);
-}
-
-int launch_channel_stats(const Act& x, double* stats, int stats_ld, cudaStream_t st) {
-  B200_REQUIRE(x.C % 8 == 0 && x.C <= 2048, E_INVALID, "channel_stats: C=%d", x.C);
-  long long S = (long long)x.D * x.H * x.W;
-  int threads = 256;
-  int c8n = x.C / 8;
-  if (c8n > threads) threads = round_up(c8n, 32);
-  int vper = threads / c8n;
-  long long want = (S + vper - 1) / vper;
-  int blocks = (int)(want < 296 ? want : 296);
-  k_channel_stats<<<dim3(blocks, x.N), threads, x.C * 2 * sizeof(double), st>>>(x, stats, stats_ld);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return OK;
-}
-
-// ------------------------------------------------------------------------------------------------ GroupNorm finalize
-// stats [N][Ctot][2] (sum, sumsq over the S voxels of each channel) -> coef [N][C][4] = (A, B, mu, rstd):
-//   z = A*x + B  with A = gamma*rstd, B = beta - mu*gamma*rstd ;  xhat = (x - mu)*rstd.    (biased variance, eps)
-// per-channel GroupNorm coefficients (A, B, mu, rstd) from the fp64 (sum, sumsq) statistics: y = A x + B
-__device__ __forceinline__ float4 gn_coef_of(const double* __restrict__ stats, const float* __restrict__ gamma,
-                                             const float* __restrict__ beta, int n, int c, int C, int Cld, int G, double S,
-                                             float eps) {
-  if (c >= C) return make_float4(0.f, 0.f, 0.f, 0.f);
-  const int cg = C / G, g = c / cg;
-  double s = 0, q = 0;
-  for (int j = 0; j < cg; ++j) {
-    s += stats[((long long)n * Cld + g * cg + j) * 2 + 0];
-    q += stats[((long long)n * Cld + g * cg + j) * 2 + 1];
-  }
-  const double m = S * cg;
-  const double mu = s / m;
-  double var = q / m - mu * mu;
-  if (var < 0) var = 0;
-  const double rstd = 1.0 / sqrt(var + (double)eps);
-  const double ga = gamma ? (double)gamma[c] : 1.0, be = beta ? (double)beta[c] : 0.0;
-  return make_float4((float)(ga * rstd), (float)(be - mu * ga * rstd), (float)mu, (float)rstd);
-}
-
-__global__ void k_gn_finalize(const double* __restrict__ stats, const float* __restrict__ gamma,
-                              const float* __restrict__ beta, int C, int Cld, int G, double S, float eps,
-                              float4* __restrict__ coef) {
-  // C real channels (gamma/beta length); Cld = pitch of stats/coef rows (>= C; padded channels get zero coefs)
-  const int n = blockIdx.x;
-  for (int c = threadIdx.x; c < Cld; c += blockDim.x)
-    coef[(long long)n * Cld + c] = gn_coef_of(stats, gamma, beta, n, c, C, Cld, G, S, eps);
-}
-
-int launch_gn_finalize(const double* stats, const float* gamma, const float* beta, int N, int C, int Cld, int G,
-                       long long S, float eps, float* coef, cudaStream_t st) {
-  B200_REQUIRE(G > 0 && C % G == 0 && Cld >= C, E_INVALID, "gn_finalize: C=%d not divisible by G=%d", C, G);
-  k_gn_finalize<<<N, 128, 0, st>>>(stats, gamma, beta, C, Cld, G, (double)S, eps, reinterpret_cast<float4*>(coef));
-  B200_CHECK_CUDA(cudaGetLastError());
-  return OK;
-}
-
 // ------------------------------------------------------------------------------------------------ GroupNorm apply (+ReLU / LeakyReLU)
+// stats [N][x.C][2] (sum, sumsq over the S voxels of each of the C real channels) -> coef [N][x.C] = (A, B, mu, rstd):
+//   z = A*x + B  with A = gamma*rstd, B = beta - mu*gamma*rstd ;  xhat = (x - mu)*rstd.    (biased variance, eps)
+// y = act(z); padded channels (C <= c < x.C) get zero coefficients.
 // grid (blocks, N); a thread keeps the same 8-channel chunk for its whole grid-stride loop (blockDim.x % c8n == 0),
 // so the affine coefficients live in registers and the loop body is load -> 8 FMA/max -> store, two voxels in flight.
-// FUSED: every block first derives the coefficients of its sample from the statistics (a few hundred fp64 loads, hidden
-// behind the other resident blocks) instead of a separate single-block finalize launch per norm layer (~7 us each, 80
-// launches per step); block 0 of each sample also stores them for the backward pass.
+// Every block first derives the coefficients of its sample from the statistics (a few hundred fp64 loads, hidden behind
+// the other resident blocks) instead of a separate single-block finalize launch per norm layer (~7 us each, 80 launches
+// per step); block 0 of each sample also stores them for the backward pass.
 struct GnFin {
   const double* stats; const float* gamma; const float* beta; int C; int G; double S; float eps; float4* coef_out;
 };
-template <bool FUSED>
-__global__ void __launch_bounds__(256) k_gn_apply(Act x, Act y, const float4* __restrict__ coef, float slope, GnFin f) {
+__global__ void __launch_bounds__(256) k_gn_apply(Act x, Act y, float slope, GnFin f) {
   pdl_wait();                 // launched through launch_pdl: the producer of x / of the statistics has completed past this line
   pdl_launch_dependents();
   const int c8n = x.C / 8;
@@ -183,43 +97,35 @@ __global__ void __launch_bounds__(256) k_gn_apply(Act x, Act y, const float4* __
   const int vslot = threadIdx.x / c8n;
   const int vper = blockDim.x / c8n;
   float ka[8], kb[8];
-  if constexpr (FUSED) {
-    // one global fp64 load pair per thread, the group sums then come from shared memory (a per-thread loop over the
-    // group's channels in global memory serialised up to 64 L2 latencies in front of every block)
-    __shared__ float2 s_ab[1024];
-    __shared__ double s_st[1024][2];
-    for (int c = threadIdx.x; c < x.C; c += blockDim.x) {
-      s_st[c][0] = c < f.C ? f.stats[((long long)n * x.C + c) * 2 + 0] : 0.0;
-      s_st[c][1] = c < f.C ? f.stats[((long long)n * x.C + c) * 2 + 1] : 0.0;
-    }
-    __syncthreads();
-    for (int c = threadIdx.x; c < x.C; c += blockDim.x) {
-      float4 k = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (c < f.C) {
-        const int cg = f.C / f.G, g = c / cg;
-        double sm_ = 0, q = 0;
-        for (int j = 0; j < cg; ++j) { sm_ += s_st[g * cg + j][0]; q += s_st[g * cg + j][1]; }
-        const double m = f.S * cg;
-        const double mu = sm_ / m;
-        double var = q / m - mu * mu;
-        if (var < 0) var = 0;
-        const double rstd = 1.0 / sqrt(var + (double)f.eps);
-        const double ga = f.gamma ? (double)f.gamma[c] : 1.0, be = f.beta ? (double)f.beta[c] : 0.0;
-        k = make_float4((float)(ga * rstd), (float)(be - mu * ga * rstd), (float)mu, (float)rstd);
-      }
-      s_ab[c] = make_float2(k.x, k.y);
-      if (blockIdx.x == 0) f.coef_out[(long long)n * x.C + c] = k;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { ka[j] = s_ab[c8 * 8 + j].x; kb[j] = s_ab[c8 * 8 + j].y; }
-  } else {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 k = __ldg(coef + (long long)n * x.C + c8 * 8 + j);
-      ka[j] = k.x; kb[j] = k.y;
-    }
+  // one global fp64 load pair per thread, the group sums then come from shared memory (a per-thread loop over the
+  // group's channels in global memory serialised up to 64 L2 latencies in front of every block)
+  __shared__ float2 s_ab[1024];
+  __shared__ double s_st[1024][2];
+  for (int c = threadIdx.x; c < x.C; c += blockDim.x) {
+    s_st[c][0] = c < f.C ? f.stats[((long long)n * x.C + c) * 2 + 0] : 0.0;
+    s_st[c][1] = c < f.C ? f.stats[((long long)n * x.C + c) * 2 + 1] : 0.0;
   }
+  __syncthreads();
+  for (int c = threadIdx.x; c < x.C; c += blockDim.x) {
+    float4 k = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (c < f.C) {
+      const int cg = f.C / f.G, g = c / cg;
+      double sm_ = 0, q = 0;
+      for (int j = 0; j < cg; ++j) { sm_ += s_st[g * cg + j][0]; q += s_st[g * cg + j][1]; }
+      const double m = f.S * cg;
+      const double mu = sm_ / m;
+      double var = q / m - mu * mu;
+      if (var < 0) var = 0;
+      const double rstd = 1.0 / sqrt(var + (double)f.eps);
+      const double ga = f.gamma ? (double)f.gamma[c] : 1.0, be = f.beta ? (double)f.beta[c] : 0.0;
+      k = make_float4((float)(ga * rstd), (float)(be - mu * ga * rstd), (float)mu, (float)rstd);
+    }
+    s_ab[c] = make_float2(k.x, k.y);
+    if (blockIdx.x == 0) f.coef_out[(long long)n * x.C + c] = k;
+  }
+  __syncthreads();
+#pragma unroll
+  for (int j = 0; j < 8; ++j) { ka[j] = s_ab[c8 * 8 + j].x; kb[j] = s_ab[c8 * 8 + j].y; }
   const long long base = (long long)n * S;
   const long long stride = (long long)gridDim.x * vper;
   long long s = (long long)blockIdx.x * vper + vslot;
@@ -261,40 +167,33 @@ static int ew_threads_for(int c8n) {
   return c8n <= 256 ? (256 / c8n) * c8n : c8n;
 }
 
-static int launch_gn_apply_impl(const Act& x, const Act& y, const float* coef, float slope, const GnFin* fin, cudaStream_t st) {
-  B200_REQUIRE(x.C % 8 == 0 && y.C == x.C, E_INVALID, "gn_apply: C=%d/%d", x.C, y.C);
+// block size and grid of k_gn_apply / k_gn_bwd (x.C <= 1024, so threads <= 256): two voxels per thread per grid step, at
+// most 8 blocks per SM over the whole batch
+static void gn_launch_dims(const Act& x, dim3& grid, dim3& block) {
   const int c8n = x.C / 8;
   const int threads = ew_threads_for(c8n);
-  B200_REQUIRE(threads <= 256, E_UNSUPPORTED, "gn_apply: C=%d unsupported", x.C);
   const long long S = (long long)x.D * x.H * x.W;
   const int vper = threads / c8n;
   long long want = (S + 2LL * vper - 1) / (2LL * vper);
   const long long cap = (132LL * 8 + x.N - 1) / x.N;
-  int blocks = (int)(want < cap ? (want > 0 ? want : 1) : cap);
-  if (fin) {
-    B200_REQUIRE(x.C <= 1024, E_UNSUPPORTED, "gn_apply: fused finalize supports C <= 1024 (got %d)", x.C);
-    launch_pdl(k_gn_apply<true>, dim3(blocks, x.N), dim3(threads), 0, st, x, y, (const float4*)nullptr, slope, *fin);
-  } else {
-    GnFin none;
-    memset(&none, 0, sizeof(none));
-    launch_pdl(k_gn_apply<false>, dim3(blocks, x.N), dim3(threads), 0, st, x, y, reinterpret_cast<const float4*>(coef), slope, none);
-  }
-  B200_CHECK_CUDA(cudaGetLastError());
-  return OK;
+  grid = dim3((int)(want < cap ? (want > 0 ? want : 1) : cap), x.N);
+  block = dim3(threads);
 }
 
-int launch_gn_apply(const Act& x, const Act& y, const float* coef, float slope, cudaStream_t st) {
-  return launch_gn_apply_impl(x, y, coef, slope, nullptr, st);
-}
-
-// statistics -> coefficients -> y = relu(A x + B) in one launch; coef_out [N][x.C] float4 is written for the backward pass
-int launch_gn_apply_fused(const Act& x, const Act& y, const double* stats, const float* gamma, const float* beta, int C,
-                          int G, long long S, float eps, float* coef_out, float slope, cudaStream_t st) {
-  B200_REQUIRE(G > 0 && C % G == 0 && C <= x.C, E_INVALID, "gn_apply_fused: C=%d G=%d", C, G);
+// statistics -> coefficients -> y = act(A x + B) in one launch; coef [N][x.C] float4 is written for the backward pass
+int launch_gn_apply(const Act& x, const Act& y, const double* stats, const float* gamma, const float* beta, int C, int G,
+                    long long S, float eps, float* coef, float slope, cudaStream_t st) {
+  B200_REQUIRE(x.C % 8 == 0 && y.C == x.C, E_INVALID, "gn_apply: C=%d/%d", x.C, y.C);
+  B200_REQUIRE(G > 0 && C % G == 0 && C <= x.C, E_INVALID, "gn_apply: C=%d G=%d", C, G);
+  B200_REQUIRE(x.C <= 1024, E_UNSUPPORTED, "gn_apply: C <= 1024 supported (got %d)", x.C);
   GnFin f;
   f.stats = stats; f.gamma = gamma; f.beta = beta; f.C = C; f.G = G; f.S = (double)S; f.eps = eps;
-  f.coef_out = reinterpret_cast<float4*>(coef_out);
-  return launch_gn_apply_impl(x, y, nullptr, slope, &f, st);
+  f.coef_out = reinterpret_cast<float4*>(coef);
+  dim3 grid, block;
+  gn_launch_dims(x, grid, block);
+  launch_pdl(k_gn_apply, grid, block, 0, st, x, y, slope, f);
+  B200_CHECK_CUDA(cudaGetLastError());
+  return OK;
 }
 
 // ------------------------------------------------------------------------------------------------ GroupNorm backward
@@ -302,21 +201,9 @@ int launch_gn_apply_fused(const Act& x, const Act& y, const double* stats, const
 // coef2 [N][C][2] = (E, F):   dx = A*dz + E*x + F      (A from coef)
 //   c1_g = (1/m) sum_{c in g} gamma_c S1_c ; c2_g = (1/m) sum gamma_c S2_c ; E = -rstd^2 c2 ; F = -rstd c1 + rstd^2 c2 mu
 // dgamma_c = sum_n S2 ; dbeta_c = sum_n S1   (written, not accumulated)
-// (E, F) of dx = A dz + E x + F for channel c of sample n, from the (sum dz, sum dz*xhat) statistics of its group
-__device__ __forceinline__ float2 gn_coef2_of(const double* __restrict__ bstats, const float4* __restrict__ coef,
-                                              const float* __restrict__ gamma, int n, int c, int C, int Cld, int G, double S) {
-  if (c >= C) return make_float2(0.f, 0.f);
-  const int cg = C / G, g = c / cg;
-  double c1 = 0, c2 = 0;
-  for (int j = 0; j < cg; ++j) {
-    const int cc = g * cg + j;
-    const double ga = gamma ? (double)gamma[cc] : 1.0;
-    c1 += ga * bstats[((long long)n * Cld + cc) * 2 + 0];
-    c2 += ga * bstats[((long long)n * Cld + cc) * 2 + 1];
-  }
-  const double m = S * cg;
-  c1 /= m; c2 /= m;
-  const float4 k = coef[(long long)n * Cld + c];
+// (E, F) of a channel from its group's gamma-weighted means c1 = sum gamma S1 / m, c2 = sum gamma S2 / m (m = S * cg values)
+// and the channel's forward coefficients k = (A, B, mu, rstd)
+__device__ __forceinline__ float2 gn_bwd_ef(double c1, double c2, float4 k) {
   const double mu = k.z, rstd = k.w;
   return make_float2((float)(-rstd * rstd * c2), (float)(-rstd * c1 + rstd * rstd * c2 * mu));
 }
@@ -342,9 +229,7 @@ __global__ void k_gn_bwd_finalize(const double* __restrict__ bstats, const float
       }
       const double m = S * cg;
       c1 /= m; c2 /= m;
-      const float4 k = coef[(long long)n * Cld + c];
-      const double mu = k.z, rstd = k.w;
-      coef2[(long long)n * Cld + c] = make_float2((float)(-rstd * rstd * c2), (float)(-rstd * c1 + rstd * rstd * c2 * mu));
+      coef2[(long long)n * Cld + c] = gn_bwd_ef(c1, c2, coef[(long long)n * Cld + c]);
       db += bstats[((long long)n * Cld + c) * 2 + 0];
       dg += bstats[((long long)n * Cld + c) * 2 + 1];
     }
@@ -363,13 +248,11 @@ int launch_gn_bwd_finalize(const double* bstats, const float* coef, const float*
 }
 
 // dx = (A*dz + E*x + F (+ add1) (+ add2)) [* scale]     grid (blocks, N), per-thread constant channel chunk
+// The blocks derive (E, F) themselves from the backward statistics and block (0, 0) also writes dgamma / dbeta (see k_gn_apply).
 struct GnBwdFin {
   const double* bstats; const float* gamma; int C; int G; int N; double S; float* dgamma; float* dbeta;
 };
-// FUSED: the blocks derive (E, F) themselves and block (0, 0) also writes dgamma / dbeta (see k_gn_apply)
-template <bool FUSED>
-__global__ void __launch_bounds__(256) k_gn_bwd(Act dz, Act x, const float4* __restrict__ coef,
-                                                const float2* __restrict__ coef2, Act add1, Act add2, Act dx,
+__global__ void __launch_bounds__(256) k_gn_bwd(Act dz, Act x, const float4* __restrict__ coef, Act add1, Act add2, Act dx,
                                                 const float* __restrict__ scale, GnBwdFin f) {
   pdl_wait();                 // launched through launch_pdl
   pdl_launch_dependents();
@@ -380,53 +263,41 @@ __global__ void __launch_bounds__(256) k_gn_bwd(Act dz, Act x, const float4* __r
   const int vslot = threadIdx.x / c8n;
   const int vper = blockDim.x / c8n;
   float ka[8], ke[8], kf[8], ks[8];
-  if constexpr (FUSED) {
-    __shared__ float2 s_ef[1024];
-    __shared__ double s_bs[1024][2];   // gamma-weighted backward statistics of every channel of this sample
-    for (int c = threadIdx.x; c < x.C; c += blockDim.x) {
-      const double ga = (c < f.C && f.gamma) ? (double)f.gamma[c] : 1.0;
-      s_bs[c][0] = c < f.C ? ga * f.bstats[((long long)n * x.C + c) * 2 + 0] : 0.0;
-      s_bs[c][1] = c < f.C ? ga * f.bstats[((long long)n * x.C + c) * 2 + 1] : 0.0;
-      if (blockIdx.x == 0 && n == 0 && c < f.C) {
-        double dg = 0, db = 0;
-        for (int nn = 0; nn < f.N; ++nn) {
-          db += f.bstats[((long long)nn * x.C + c) * 2 + 0];
-          dg += f.bstats[((long long)nn * x.C + c) * 2 + 1];
-        }
-        if (f.dgamma) f.dgamma[c] = (float)dg;
-        if (f.dbeta) f.dbeta[c] = (float)db;
+  __shared__ float2 s_ef[1024];
+  __shared__ double s_bs[1024][2];   // gamma-weighted backward statistics of every channel of this sample
+  for (int c = threadIdx.x; c < x.C; c += blockDim.x) {
+    const double ga = (c < f.C && f.gamma) ? (double)f.gamma[c] : 1.0;
+    s_bs[c][0] = c < f.C ? ga * f.bstats[((long long)n * x.C + c) * 2 + 0] : 0.0;
+    s_bs[c][1] = c < f.C ? ga * f.bstats[((long long)n * x.C + c) * 2 + 1] : 0.0;
+    if (blockIdx.x == 0 && n == 0 && c < f.C) {
+      double dg = 0, db = 0;
+      for (int nn = 0; nn < f.N; ++nn) {
+        db += f.bstats[((long long)nn * x.C + c) * 2 + 0];
+        dg += f.bstats[((long long)nn * x.C + c) * 2 + 1];
       }
+      if (f.dgamma) f.dgamma[c] = (float)dg;
+      if (f.dbeta) f.dbeta[c] = (float)db;
     }
-    __syncthreads();
-    for (int c = threadIdx.x; c < x.C; c += blockDim.x) {
-      float2 e = make_float2(0.f, 0.f);
-      if (c < f.C) {
-        const int cg = f.C / f.G, g = c / cg;
-        double c1 = 0, c2 = 0;
-        for (int j = 0; j < cg; ++j) { c1 += s_bs[g * cg + j][0]; c2 += s_bs[g * cg + j][1]; }
-        const double m = f.S * cg;
-        c1 /= m; c2 /= m;
-        const float4 k = coef[(long long)n * x.C + c];
-        const double mu = k.z, rstd = k.w;
-        e = make_float2((float)(-rstd * rstd * c2), (float)(-rstd * c1 + rstd * rstd * c2 * mu));
-      }
-      s_ef[c] = e;
+  }
+  __syncthreads();
+  for (int c = threadIdx.x; c < x.C; c += blockDim.x) {
+    float2 e = make_float2(0.f, 0.f);
+    if (c < f.C) {
+      const int cg = f.C / f.G, g = c / cg;
+      double c1 = 0, c2 = 0;
+      for (int j = 0; j < cg; ++j) { c1 += s_bs[g * cg + j][0]; c2 += s_bs[g * cg + j][1]; }
+      const double m = f.S * cg;
+      c1 /= m; c2 /= m;
+      e = gn_bwd_ef(c1, c2, coef[(long long)n * x.C + c]);
     }
-    __syncthreads();
+    s_ef[c] = e;
+  }
+  __syncthreads();
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      ka[j] = __ldg(coef + (long long)n * x.C + c8 * 8 + j).x;
-      ke[j] = s_ef[c8 * 8 + j].x; kf[j] = s_ef[c8 * 8 + j].y;
-      ks[j] = scale ? __ldg(scale + (long long)n * x.C + c8 * 8 + j) : 1.f;
-    }
-  } else {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 k = __ldg(coef + (long long)n * x.C + c8 * 8 + j);
-      const float2 e = __ldg(coef2 + (long long)n * x.C + c8 * 8 + j);
-      ka[j] = k.x; ke[j] = e.x; kf[j] = e.y;
-      ks[j] = scale ? __ldg(scale + (long long)n * x.C + c8 * 8 + j) : 1.f;
-    }
+  for (int j = 0; j < 8; ++j) {
+    ka[j] = __ldg(coef + (long long)n * x.C + c8 * 8 + j).x;
+    ke[j] = s_ef[c8 * 8 + j].x; kf[j] = s_ef[c8 * 8 + j].y;
+    ks[j] = scale ? __ldg(scale + (long long)n * x.C + c8 * 8 + j) : 1.f;
   }
   const long long base = (long long)n * S;
   const long long stride = (long long)gridDim.x * vper;
@@ -470,46 +341,22 @@ __global__ void __launch_bounds__(256) k_gn_bwd(Act dz, Act x, const float4* __r
   }
 }
 
-
-static int launch_gn_bwd_impl(const Act& dz, const Act& x, const float* coef, const float* coef2, const Act* add1,
-                              const Act* add2, const Act& dx, const float* scale, const GnBwdFin* fin, cudaStream_t st) {
-  B200_REQUIRE(x.C % 8 == 0 && dz.C == x.C && dx.C == x.C, E_INVALID, "gn_bwd: channel mismatch");
-  Act none = make_act(nullptr, nullptr, 0, 0, 0, 0, 0, 0);
-  const int c8n = x.C / 8;
-  const int threads = ew_threads_for(c8n);
-  B200_REQUIRE(threads <= 256, E_UNSUPPORTED, "gn_bwd: C=%d unsupported", x.C);
-  const long long S = (long long)x.D * x.H * x.W;
-  const int vper = threads / c8n;
-  long long want = (S + 2LL * vper - 1) / (2LL * vper);
-  const long long cap = (132LL * 8 + x.N - 1) / x.N;
-  int blocks = (int)(want < cap ? (want > 0 ? want : 1) : cap);
-  if (fin) {
-    B200_REQUIRE(x.C <= 1024, E_UNSUPPORTED, "gn_bwd: fused finalize supports C <= 1024 (got %d)", x.C);
-    launch_pdl(k_gn_bwd<true>, dim3(blocks, x.N), dim3(threads), 0, st, dz, x, reinterpret_cast<const float4*>(coef), (const float2*)nullptr,
-               add1 ? *add1 : none, add2 ? *add2 : none, dx, scale, *fin);
-  } else {
-    GnBwdFin nofin;
-    memset(&nofin, 0, sizeof(nofin));
-    launch_pdl(k_gn_bwd<false>, dim3(blocks, x.N), dim3(threads), 0, st, dz, x, reinterpret_cast<const float4*>(coef),
-               reinterpret_cast<const float2*>(coef2), add1 ? *add1 : none, add2 ? *add2 : none, dx, scale, nofin);
-  }
-  B200_CHECK_CUDA(cudaGetLastError());
-  return OK;
-}
-
-int launch_gn_bwd(const Act& dz, const Act& x, const float* coef, const float* coef2, const Act* add1, const Act* add2,
-                  const Act& dx, const float* scale, cudaStream_t st) {
-  return launch_gn_bwd_impl(dz, x, coef, coef2, add1, add2, dx, scale, nullptr, st);
-}
-
 // backward statistics -> (E, F), dgamma, dbeta -> dx = A dz + E x + F (+adds)(*scale) in one launch
-int launch_gn_bwd_fused(const Act& dz, const Act& x, const float* coef, const double* bstats, const float* gamma, int C, int G,
-                        long long S, float* dgamma, float* dbeta, const Act* add1, const Act* add2, const Act& dx,
-                        const float* scale, cudaStream_t st) {
-  B200_REQUIRE(G > 0 && C % G == 0 && C <= x.C, E_INVALID, "gn_bwd_fused: C=%d G=%d", C, G);
+int launch_gn_bwd(const Act& dz, const Act& x, const float* coef, const double* bstats, const float* gamma, int C, int G,
+                  long long S, float* dgamma, float* dbeta, const Act* add1, const Act* add2, const Act& dx,
+                  const float* scale, cudaStream_t st) {
+  B200_REQUIRE(x.C % 8 == 0 && dz.C == x.C && dx.C == x.C, E_INVALID, "gn_bwd: channel mismatch");
+  B200_REQUIRE(G > 0 && C % G == 0 && C <= x.C, E_INVALID, "gn_bwd: C=%d G=%d", C, G);
+  B200_REQUIRE(x.C <= 1024, E_UNSUPPORTED, "gn_bwd: C <= 1024 supported (got %d)", x.C);
   GnBwdFin f;
   f.bstats = bstats; f.gamma = gamma; f.C = C; f.G = G; f.N = x.N; f.S = (double)S; f.dgamma = dgamma; f.dbeta = dbeta;
-  return launch_gn_bwd_impl(dz, x, coef, nullptr, add1, add2, dx, scale, &f, st);
+  const Act none = make_act(nullptr, nullptr, 0, 0, 0, 0, 0, 0);
+  dim3 grid, block;
+  gn_launch_dims(x, grid, block);
+  launch_pdl(k_gn_bwd, grid, block, 0, st, dz, x, reinterpret_cast<const float4*>(coef), add1 ? *add1 : none,
+             add2 ? *add2 : none, dx, scale, f);
+  B200_CHECK_CUDA(cudaGetLastError());
+  return OK;
 }
 
 // ------------------------------------------------------------------------------------------------ activation backward (+ statistics)
@@ -623,30 +470,6 @@ int launch_head_dbias(const float* dlogits, int N, int NO, long long S, float* d
   k_head_dbias<<<dim3(blocks, NO), 256, 0, st>>>(dlogits, N, NO, S, part);
   B200_CHECK_CUDA(cudaGetLastError());
   k_head_dbias_sum<<<1, 32, 0, st>>>(part, blocks, NO, dbias);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return OK;
-}
-
-// ------------------------------------------------------------------------------------------------ element-wise add (y = a + b)
-__global__ void k_add(Act a, Act b, Act y) {
-  const int c8n = a.C / 8;
-  const long long total = a.voxels() * c8n;
-  for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
-    const int c8 = (int)(t % c8n);
-    const long long vox = t / c8n;
-    float u[8], v[8];
-    load8(a.hi, a.lo, vox * a.ld + c8 * 8, u);
-    load8(b.hi, b.lo, vox * b.ld + c8 * 8, v);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) u[j] += v[j];
-    store8(y.hi, y.lo, vox * y.ld + c8 * 8, u);
-  }
-}
-
-int launch_add(const Act& a, const Act& b, const Act& y, cudaStream_t st) {
-  B200_REQUIRE(a.C % 8 == 0 && a.C == b.C && a.C == y.C, E_INVALID, "add: channel mismatch");
-  long long total = a.voxels() * (a.C / 8);
-  k_add<<<ew_blocks(total, 256), 256, 0, st>>>(a, b, y);
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;
 }
@@ -1241,48 +1064,6 @@ int launch_ncdhw_to_act(const float* x, int C, const Act& out, cudaStream_t st) 
 int launch_act_to_ncdhw(const Act& in, int C, float* y, cudaStream_t st) {
   long long total = in.voxels() * (in.C / 8);
   k_act_to_ncdhw<<<ew_blocks(total, 256), 256, 0, st>>>(in, C, y);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return OK;
-}
-
-// ------------------------------------------------------------------------------------------------ SIMT direct conv (debug / cross-check only)
-// y[v][co] = sum_{t,ci} x[v*stride + t - pad][ci] * wp[t][co][ci]   with packed bf16 weights (mode-0 layout).
-__global__ void k_conv_simt(Act x, const bf16* __restrict__ whi, const bf16* __restrict__ wlo, int ksz, int stride,
-                            Act y) {
-  const long long total = y.voxels() * y.C;
-  const int pad = ksz / 2;
-  for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
-    const int co = (int)(t % y.C);
-    long long v = t / y.C;
-    const int w = (int)(v % y.W); v /= y.W;
-    const int h = (int)(v % y.H); v /= y.H;
-    const int d = (int)(v % y.D);
-    const int n = (int)(v / y.D);
-    float acc = 0.f;
-    for (int kd = 0; kd < ksz; ++kd)
-      for (int kh = 0; kh < ksz; ++kh)
-        for (int kw = 0; kw < ksz; ++kw) {
-          const int id = d * stride + kd - pad, ih = h * stride + kh - pad, iw = w * stride + kw - pad;
-          if (id < 0 || ih < 0 || iw < 0 || id >= x.D || ih >= x.H || iw >= x.W) continue;
-          const long long xo = ((((long long)n * x.D + id) * x.H + ih) * x.W + iw) * x.ld;
-          const long long wo = ((long long)((kd * ksz + kh) * ksz + kw) * y.C + co) * x.C;
-          for (int ci = 0; ci < x.C; ++ci) {
-            float xv = __bfloat162float(x.hi[xo + ci]) + (x.lo ? __bfloat162float(x.lo[xo + ci]) : 0.f);
-            float wv = __bfloat162float(whi[wo + ci]) + (wlo ? __bfloat162float(wlo[wo + ci]) : 0.f);
-            acc = fmaf(xv, wv, acc);
-          }
-        }
-    const long long yo = (t / y.C) * y.ld + co;
-    bf16 hv = __float2bfloat16_rn(acc);
-    y.hi[yo] = hv;
-    if (y.lo) y.lo[yo] = __float2bfloat16_rn(acc - __bfloat162float(hv));
-  }
-}
-
-int launch_conv_simt(const Act& x, const bf16* whi, const bf16* wlo, int ksz, int stride, const Act& y,
-                     cudaStream_t st) {
-  long long total = y.voxels() * y.C;
-  k_conv_simt<<<ew_blocks(total, 128), 128, 0, st>>>(x, whi, wlo, ksz, stride, y);
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;
 }

@@ -6,20 +6,16 @@ namespace b200 {
 
 // ---- bandwidth-bound kernels (elementwise.cu)
 int launch_input_pack(const float* x, int C, const Act& out, double* stats, int stats_ld, cudaStream_t st);
-int launch_channel_stats(const Act& x, double* stats, int stats_ld, cudaStream_t st);
-int launch_gn_finalize(const double* stats, const float* gamma, const float* beta, int N, int C, int Cld, int G,
-                       long long S, float eps, float* coef, cudaStream_t st);
-int launch_gn_apply(const Act& x, const Act& y, const float* coef, float slope, cudaStream_t st);
-int launch_gn_apply_fused(const Act& x, const Act& y, const double* stats, const float* gamma, const float* beta, int C,
-                          int G, long long S, float eps, float* coef_out, float slope, cudaStream_t st);
-int launch_gn_bwd_fused(const Act& dz, const Act& x, const float* coef, const double* bstats, const float* gamma, int C, int G,
-                        long long S, float* dgamma, float* dbeta, const Act* add1, const Act* add2, const Act& dx,
-                        const float* scale, cudaStream_t st);
+// GroupNorm(+ReLU / LeakyReLU) forward: statistics -> coefficients (coef [N][x.C][4], written) -> y; x.C <= 1024
+int launch_gn_apply(const Act& x, const Act& y, const double* stats, const float* gamma, const float* beta, int C, int G,
+                    long long S, float eps, float* coef, float slope, cudaStream_t st);
+// GroupNorm backward: backward statistics -> (E, F), dgamma, dbeta -> dx; x.C <= 1024
+int launch_gn_bwd(const Act& dz, const Act& x, const float* coef, const double* bstats, const float* gamma, int C, int G,
+                  long long S, float* dgamma, float* dbeta, const Act* add1, const Act* add2, const Act& dx,
+                  const float* scale, cudaStream_t st);
+// the same without dx (the first block's norm): dgamma, dbeta and (E, F) into coef2 [N][Cld][2] for launch_input_grad
 int launch_gn_bwd_finalize(const double* bstats, const float* coef, const float* gamma, int N, int C, int Cld, int G,
                            long long S, float* coef2, float* dgamma, float* dbeta, cudaStream_t st);
-int launch_gn_bwd(const Act& dz, const Act& x, const float* coef, const float* coef2, const Act* add1, const Act* add2,
-                  const Act& dx, const float* scale, cudaStream_t st);
-int launch_add(const Act& a, const Act& b, const Act& y, cudaStream_t st);
 int launch_upsample2x_fwd(const Act& x, const Act& y, double* stats, int stats_ld, cudaStream_t st);
 int launch_upsample2x_bwd(const Act& dy, const Act& dx, cudaStream_t st);
 // The 1x1x1 head takes 1..B200_HEAD_MAX_OUTPUTS outputs: 1..8 run the SIMT kernels below with fp32 weights, 9..128 the
@@ -69,8 +65,6 @@ int launch_act_to_ncdhw(const Act& in, int C, float* y, cudaStream_t st);
 // coef2 [N][coef_ld][2] as left by the GroupNorm backward); dz == nullptr: dx = r (the layout transpose alone)
 int launch_input_grad(const Act* dz, const Act* x, const float* coef, const float* coef2, int coef_ld, const Act& r, int C, float* dx,
                       cudaStream_t st);
-int launch_conv_simt(const Act& x, const bf16* whi, const bf16* wlo, int ksz, int stride, const Act& y,
-                     cudaStream_t st);
 
 // ---- Dice criterion (dice.cu)
 // flags: bit0 sigmoid, bit1 squared_pred, bit2 jaccard, bit3 batch, bit4 exclude background, bit5 reduction=sum,

@@ -377,9 +377,9 @@ static void emit_norm_fwd(Plan& P, int ni, TRef x, TRef y) {
   push_op(P.fwd, "gn_apply " + P.norms[ni].name + " " + shape_of(P, x), [&P, ni, x, y](RunCtx& cx) -> int {
     const NormLayer& n = P.norms[ni];
     // statistics -> coefficients -> normalise + ReLU in one launch (the coefficients are kept for the backward pass)
-    LAUNCHED(cx, CAT_NORM, launch_gn_apply_fused(act_of(P, cx, x), act_of(P, cx, y), stats_ptr(P, cx, x), cx.params[n.pg],
-                                                 cx.params[n.pb], n.C, n.G, n.S, 1e-5f,
-                                                 reinterpret_cast<float*>(cx.ws + n.coef), P.slope, cx.st));
+    LAUNCHED(cx, CAT_NORM, launch_gn_apply(act_of(P, cx, x), act_of(P, cx, y), stats_ptr(P, cx, x), cx.params[n.pg],
+                                           cx.params[n.pb], n.C, n.G, n.S, 1e-5f, reinterpret_cast<float*>(cx.ws + n.coef),
+                                           P.slope, cx.st));
     return OK;
   });
 }
@@ -546,10 +546,10 @@ static void emit_gn_bwd(Plan& P, int ni, TRef dz, TRef x, TRef add1, TRef dx, bo
     Act a1;
     if (add1.valid()) a1 = act_of(P, cx, add1);
     // finalize fused: (E, F), dgamma, dbeta are derived from the backward statistics inside the kernel
-    LAUNCHED(cx, CAT_NORM, launch_gn_bwd_fused(act_of(P, cx, dz), act_of(P, cx, x), reinterpret_cast<float*>(cx.ws + n.coef),
-                                               reinterpret_cast<double*>(cx.ws + P.bz_off + n.bstats), cx.params[n.pg], n.C,
-                                               n.G, n.S, cx.grads[n.pg], cx.grads[n.pb], add1.valid() ? &a1 : nullptr,
-                                               nullptr, act_of(P, cx, dx), (scale && cx.drop) ? cx.drop : nullptr, cx.st));
+    LAUNCHED(cx, CAT_NORM, launch_gn_bwd(act_of(P, cx, dz), act_of(P, cx, x), reinterpret_cast<float*>(cx.ws + n.coef),
+                                         reinterpret_cast<double*>(cx.ws + P.bz_off + n.bstats), cx.params[n.pg], n.C, n.G,
+                                         n.S, cx.grads[n.pg], cx.grads[n.pb], add1.valid() ? &a1 : nullptr, nullptr,
+                                         act_of(P, cx, dx), (scale && cx.drop) ? cx.drop : nullptr, cx.st));
     return OK;
   });
 }

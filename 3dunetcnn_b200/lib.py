@@ -78,14 +78,12 @@ _SIGS = {
     "b200unet_conv3d": (C.c_int, [C.POINTER(ConvDesc), C.c_void_p]),
     "b200unet_conv3d_wgrad": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_int, C.c_int, C.c_int, C.c_int,
                                         C.c_void_p, C.c_void_p]),
-    "b200unet_channel_stats": (C.c_int, [C.POINTER(Tensor5), C.c_void_p, C.c_int, C.c_void_p]),
-    "b200unet_gn_finalize": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
-                                       C.c_int64, C.c_float, C.c_void_p, C.c_void_p]),
-    "b200unet_gn_apply": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_float, C.c_void_p]),
+    "b200unet_gn_apply": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                    C.c_float, C.c_float, C.c_void_p, C.c_void_p]),
     "b200unet_gn_bwd_finalize": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                            C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "b200unet_gn_bwd": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_void_p, C.POINTER(Tensor5),
-                                  C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p]),
+    "b200unet_gn_bwd": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                  C.c_void_p, C.c_void_p, C.POINTER(Tensor5), C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p]),
     "b200unet_upsample2x_fwd": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_int, C.c_void_p]),
     "b200unet_upsample2x_bwd": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p]),
     "b200unet_zero_insert": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_int, C.c_int, C.c_int, C.c_void_p]),
@@ -132,14 +130,10 @@ _SIGS = {
     "b200unet_plan_profile_dump": (C.c_int, [C.c_void_p, C.c_char_p]),
 }
 
-# diagnostics (include/b200unet_diag.h): SIMT cross-check, used by tools/ only
-_DIAG_SIGS = {
-    "b200unet_conv3d_simt": (C.c_int, [C.POINTER(Tensor5), C.c_void_p, C.c_void_p, C.c_int, C.c_int,
-                                       C.POINTER(Tensor5), C.c_void_p]),
-}
+# entry points outside the product header (diagnostics), bound like _SIGS: none at present
+_DIAG_SIGS = {}
 
 EXPORTED_SYMBOLS = tuple(_SIGS)
-DIAG_SYMBOLS = tuple(_DIAG_SIGS)
 
 
 def load_library():
@@ -284,28 +278,14 @@ def conv3d_wgrad(a: Act, dy: Act, ksz: int, stride: int, cip: int, cop: int, dw:
                                                stream_ptr()), "conv3d_wgrad")
 
 
-def conv3d_simt(x: Act, w_hi, w_lo, ksz: int, stride: int, y: Act) -> None:
-    check(load_library().b200unet_conv3d_simt(C.byref(x.ct()), w_hi.data_ptr(),
-                                              w_lo.data_ptr() if w_lo is not None else None, ksz, stride,
-                                              C.byref(y.ct()), stream_ptr()), "conv3d_simt")
-
-
 def _p(t: Optional[torch.Tensor]):
     return t.data_ptr() if t is not None else None
 
 
-def channel_stats(x: Act, stats: torch.Tensor, stats_ld: int) -> None:
-    check(load_library().b200unet_channel_stats(C.byref(x.ct()), stats.data_ptr(), stats_ld, stream_ptr()), "stats")
-
-
-def gn_finalize(stats, gamma, beta, n, c, c_ld, groups, spatial, eps, coef) -> None:
-    check(load_library().b200unet_gn_finalize(stats.data_ptr(), _p(gamma), _p(beta), n, c, c_ld, groups, spatial, eps,
-                                              coef.data_ptr(), stream_ptr()), "gn_finalize")
-
-
-def gn_apply(x: Act, y: Act, coef, slope=0.0) -> None:
-    check(load_library().b200unet_gn_apply(C.byref(x.ct()), C.byref(y.ct()), coef.data_ptr(), slope, stream_ptr()),
-          "gn_apply")
+def gn_apply(x: Act, y: Act, stats, gamma, beta, c, groups, coef, eps=1e-5, slope=0.0) -> None:
+    """y = act(GroupNorm(x)) from the fp64 (sum, sumsq) statistics [n][x.c][2] of the c real channels; writes coef [n][x.c][4]"""
+    check(load_library().b200unet_gn_apply(C.byref(x.ct()), C.byref(y.ct()), stats.data_ptr(), _p(gamma), _p(beta), c, groups,
+                                           eps, slope, coef.data_ptr(), stream_ptr()), "gn_apply")
 
 
 def gn_bwd_finalize(bstats, coef, gamma, n, c, c_ld, groups, spatial, coef2, dgamma, dbeta) -> None:
@@ -314,13 +294,14 @@ def gn_bwd_finalize(bstats, coef, gamma, n, c, c_ld, groups, spatial, coef2, dga
           "gn_bwd_finalize")
 
 
-def gn_bwd(dz: Act, x: Act, coef, coef2, dx: Act, add1: Optional[Act] = None, add2: Optional[Act] = None) -> None:
+def gn_bwd(dz: Act, x: Act, coef, bstats, gamma, c, groups, dx: Act, dgamma=None, dbeta=None, add1: Optional[Act] = None,
+           add2: Optional[Act] = None) -> None:
+    """dx (+ add1 + add2) and dgamma / dbeta from the backward statistics bstats [n][x.c][2] = (sum dz, sum dz * xhat)"""
     a1 = add1.ct() if add1 is not None else None
     a2 = add2.ct() if add2 is not None else None
-    check(load_library().b200unet_gn_bwd(C.byref(dz.ct()), C.byref(x.ct()), coef.data_ptr(), coef2.data_ptr(),
-                                         C.byref(a1) if a1 is not None else None,
-                                         C.byref(a2) if a2 is not None else None, C.byref(dx.ct()), stream_ptr()),
-          "gn_bwd")
+    check(load_library().b200unet_gn_bwd(C.byref(dz.ct()), C.byref(x.ct()), coef.data_ptr(), bstats.data_ptr(), _p(gamma), c,
+                                         groups, _p(dgamma), _p(dbeta), C.byref(a1) if a1 is not None else None,
+                                         C.byref(a2) if a2 is not None else None, C.byref(dx.ct()), stream_ptr()), "gn_bwd")
 
 
 def upsample2x_fwd(x: Act, y: Act, stats=None, stats_ld=0) -> None:

@@ -76,7 +76,7 @@ typedef struct b200unet_conv_desc {
   int32_t stats_ld;
   int32_t mode;                 /* 0 plain epilogue; 1 GroupNorm+ReLU backward epilogue */
   const b200unet_tensor* gn_x;  /* mode 1: raw input of the norm */
-  const float* coef;            /* mode 1: [N][coef_ld][4] from b200unet_gn_finalize */
+  const float* coef;            /* mode 1: [N][coef_ld][4] from b200unet_gn_apply */
   int32_t coef_ld;
   float slope;                  /* 0 = ReLU (myronenko.py:14), 0.01 = LeakyReLU (DynUNet blocks) */
   double* bstats;               /* mode 1: [N][coef_ld][2] += (sum dz, sum dz*xhat) */
@@ -89,15 +89,23 @@ int b200unet_conv3d(const b200unet_conv_desc* desc, void* stream);
 int b200unet_conv3d_wgrad(const b200unet_tensor* a, const b200unet_tensor* dy, int ksz, int stride, int cip, int cop,
                           float* dw, void* stream);
 
-/* ---- GroupNorm(G, C, eps, affine) + ReLU (myronenko.py:17-31): statistics, apply, backward */
-int b200unet_channel_stats(const b200unet_tensor* x, double* stats, int stats_ld, void* stream);
-int b200unet_gn_finalize(const double* stats, const float* gamma, const float* beta, int n, int c, int c_ld, int groups,
-                         int64_t spatial, float eps, float* coef, void* stream);
-int b200unet_gn_apply(const b200unet_tensor* x, const b200unet_tensor* y, const float* coef, float slope, void* stream);
+/* ---- GroupNorm(G, C, eps, affine) + ReLU / LeakyReLU (myronenko.py:17-31): forward and backward, each in one launch.
+ * `c` real channels (the length of gamma / beta; NULL gamma = 1, NULL beta = 0) in `groups` groups, out of the x->c channels
+ * of the view; x->c is also the channel pitch of stats, coef and bstats.  x->c <= 1024, else B200UNET_E_UNSUPPORTED.
+ * The spatial extent is d*h*w of x.  gn_bwd_finalize takes the pitch (c_ld), batch and spatial extent explicitly.
+ *   gn_apply:        stats [n][x->c][2] fp64 (sum, sumsq) of each real channel -> coef [n][x->c][4] (A, B, mu, rstd), written
+ *                    for the backward (zeros on padded channels), and y = act(A x + B) with act(z) = z > 0 ? z : slope * z
+ *   gn_bwd:          bstats [n][x->c][2] fp64 (sum dz, sum dz * xhat) of dz = dL/d(norm output), already masked by act'
+ *                    (b200unet_conv3d mode 1, b200unet_act_bwd) -> dx = dL/dx (+ add1) (+ add2); writes dgamma, dbeta
+ *                    (either may be NULL)
+ *   gn_bwd_finalize: the same without dx: coef2 [n][c_ld][2] = (E, F) of dx = A dz + E x + F, dgamma and dbeta */
+int b200unet_gn_apply(const b200unet_tensor* x, const b200unet_tensor* y, const double* stats, const float* gamma,
+                      const float* beta, int c, int groups, float eps, float slope, float* coef, void* stream);
+int b200unet_gn_bwd(const b200unet_tensor* dz, const b200unet_tensor* x, const float* coef, const double* bstats,
+                    const float* gamma, int c, int groups, float* dgamma, float* dbeta, const b200unet_tensor* add1,
+                    const b200unet_tensor* add2, const b200unet_tensor* dx, void* stream);
 int b200unet_gn_bwd_finalize(const double* bstats, const float* coef, const float* gamma, int n, int c, int c_ld,
                              int groups, int64_t spatial, float* coef2, float* dgamma, float* dbeta, void* stream);
-int b200unet_gn_bwd(const b200unet_tensor* dz, const b200unet_tensor* x, const float* coef, const float* coef2,
-                    const b200unet_tensor* add1, const b200unet_tensor* add2, const b200unet_tensor* dx, void* stream);
 
 /* ---- post-activation blocks (conv -> norm -> act: MONAI UnetBasicBlock): gradient through the activation of
  * a = act(A c + B):  dz = (g1 [+ g2]) * act'(A c + B),  bstats[n][ch] += (sum dz, sum dz * xhat)  -> b200unet_gn_bwd */

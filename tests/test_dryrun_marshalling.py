@@ -197,7 +197,7 @@ def test_prepost_calls(pkg, stubbed):
     assert {"b200unet_one_hot", "b200unet_zscore", "b200unet_label_map"} <= set(stubbed)
 
 
-def test_per_kernel_wrappers_marshal(pkg, stubbed):
+def test_per_kernel_wrappers_marshal_fused_groupnorm(pkg, stubbed):
     """the thin wrappers tests/test_gpu_ops.py drives (conv3d, wgrad, GroupNorm, upsample, head, pack)"""
     L = pkg.lib
     a = L.Act(torch.zeros(1, 4, 8, 8, 8, dtype=torch.bfloat16))
@@ -207,8 +207,9 @@ def test_per_kernel_wrappers_marshal(pkg, stubbed):
     L.conv3d(a, w, None, 3, 1, b, 16, 8, res=b, stats=st, stats_ld=16, cls_mode=0)
     L.conv3d_wgrad(a, b, 3, 1, 8, 16, torch.zeros(27, 8, 16))
     coef = torch.zeros(1, 16, 4)
-    L.gn_finalize(st, None, None, 1, 16, 16, 8, 256, 1e-5, coef)
-    L.gn_apply(b, b, coef, 0.01)
+    L.gn_apply(b, b, st, None, None, 16, 8, coef, slope=0.01)
+    L.gn_bwd(b, b, coef, st, None, 16, 8, b, torch.zeros(16), torch.zeros(16), add1=b)
+    L.gn_bwd_finalize(st, coef, None, 1, 16, 16, 8, 1024, torch.zeros(1, 16, 2), None, None)
     L.head_bwd(b, torch.zeros(3, 16), 3, torch.zeros(1, 3, 4, 8, 8), b, torch.zeros(3, 16))
     L.pack_weights(torch.zeros(8, 16, 2, 2, 2), 4)
-    assert "b200unet_conv3d" in stubbed and "b200unet_head_bwd" in stubbed
+    assert {"b200unet_conv3d", "b200unet_gn_apply", "b200unet_gn_bwd", "b200unet_gn_bwd_finalize", "b200unet_head_bwd"} <= set(stubbed)

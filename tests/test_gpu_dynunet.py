@@ -110,7 +110,7 @@ def test_transposed_conv_k2s2_forward_dgrad_wgrad(pkg, ci, co, dims, split):
 
 
 @pytest.mark.parametrize("split", [False, True])
-def test_activation_backward_kernel(pkg, split):
+def test_activation_backward_kernel_on_fused_coefficients(pkg, split):
     """dz = (g1 + g2) * LeakyReLU'(A c + B) with (sum dz, sum dz*xhat): through head-less plumbing = compare with autograd of
     LeakyReLU(InstanceNorm(c)) for the statistics and the mask."""
     import ctypes as C
@@ -118,15 +118,14 @@ def test_activation_backward_kernel(pkg, split):
     lib = L.load_library()
     torch.manual_seed(3)
     n, ch, dims = 2, 24, (6, 10, 8)
-    S = dims[0] * dims[1] * dims[2]
     c = L.Act.from_ncdhw(torch.randn(n, ch, *dims, device=DEV) * 2 + 0.5, split=split)
     g1 = L.Act.from_ncdhw(torch.randn(n, ch, *dims, device=DEV), split=split)
     g2 = L.Act.from_ncdhw(torch.randn(n, ch, *dims, device=DEV), split=split)
     gamma, beta = torch.randn(ch, device=DEV) * 0.3 + 1, torch.randn(ch, device=DEV) * 0.2
-    stats = torch.zeros(n, ch, 2, dtype=torch.float64, device=DEV)
-    L.channel_stats(c, stats, ch)
+    cv = c.value().double()
+    stats = torch.stack([cv.sum(dim=(1, 2, 3)), (cv * cv).sum(dim=(1, 2, 3))], dim=-1).contiguous()   # fp64 (sum, sumsq)
     coef = torch.empty(n, ch, 4, device=DEV)
-    L.gn_finalize(stats, gamma, beta, n, ch, ch, ch, S, 1e-5, coef)       # G = C: instance norm
+    L.gn_apply(c, L.Act.empty(n, *dims, ch, split=split), stats, gamma, beta, ch, ch, coef, slope=0.01)   # G = C: instance norm
     dz = L.Act.empty(n, *dims, ch, split=split)
     bst = torch.zeros(n, ch, 2, dtype=torch.float64, device=DEV)
     g2t = g2.ct()

@@ -22,6 +22,13 @@ def rel(a, b):
     return float((a - b).norm() / (b.norm() + 1e-30))
 
 
+def _channel_stats(a):
+    """fp64 (sum, sumsq) [n][a.c][2] of every channel of view a, from the stored values: what the epilogue of the producing
+    convolution accumulates for the next GroupNorm"""
+    v = a.value().double()
+    return torch.stack([v.sum(dim=(1, 2, 3)), (v * v).sum(dim=(1, 2, 3))], dim=-1).contiguous()
+
+
 def _packed_to_torch(L, w, mode, split, cout, cin, ksz):
     hi, lo, cop, cip, T = L.pack_weights(w, mode, split=split)
     q = hi.float() + (lo.float() if split else 0)
@@ -93,7 +100,7 @@ def test_conv3d_wide_inputs_on_halo_kernel(pkg, monkeypatch, cin, cout, dims, mo
 
 @pytest.mark.parametrize("split", [False, True])
 @pytest.mark.parametrize("ci,co,dims", [(128, 128, (4, 16, 8)), (192, 256, (2, 16, 16)), (128, 96, (5, 16, 8))])
-def test_conv3d_wide_inputs_on_halo_kernel_gn_backward_epilogue(pkg, monkeypatch, ci, co, dims, split):
+def test_conv3d_wide_inputs_on_halo_kernel_gn_backward_epilogue_on_fused_coefficients(pkg, monkeypatch, ci, co, dims, split):
     """The same wide-input halo-mode dispatch with the mode-1 (GroupNorm/ReLU backward) epilogue: the data gradient of a
     co -> ci ... convolution seen from its output side, i.e. K = co >= 128 input channels of the GEMM."""
     monkeypatch.setenv("B200UNET_HALO_WIDE_MIN", "0")
@@ -107,11 +114,8 @@ def test_conv3d_wide_inputs_on_halo_kernel_gn_backward_epilogue(pkg, monkeypatch
     dy, x = L.Act.from_ncdhw(dyv, split=split), L.Act.from_ncdhw(xv, split=split)
     wdh, wdl, _, _, _ = L.pack_weights(w, 1, split=split)
     _, _, _, _, wq = _packed_to_torch(L, w, 0, split, co, ci, 3)
-    S = dims[0] * dims[1] * dims[2]
-    stats = torch.zeros(n, ci, 2, dtype=torch.float64, device=DEV)
-    L.channel_stats(x, stats, ci)
     coef = torch.empty(n, ci, 4, device=DEV)
-    L.gn_finalize(stats, gamma, beta, n, ci, ci, G, S, 1e-5, coef)
+    L.gn_apply(x, L.Act.empty(n, *dims, ci, split=split), _channel_stats(x), gamma, beta, ci, G, coef)
     bst = torch.zeros(n, ci, 2, dtype=torch.float64, device=DEV)
     dz = L.Act.empty(n, *dims, ci, split=split)
     L.conv3d(dy, wdh, wdl, 3, 1, dz, ci, co, mode=1, gn_x=x, coef=coef, coef_ld=ci, bstats=bst)
@@ -223,7 +227,7 @@ def test_conv3d_two_sources_is_block_output(pkg, split, D):
 
 @pytest.mark.parametrize("split", [False, True])
 @pytest.mark.parametrize("D", [8, 16])
-def test_conv3d_dgrad_groupnorm_relu_backward_epilogue(pkg, split, D):
+def test_conv3d_dgrad_groupnorm_relu_backward_epilogue_on_fused_coefficients(pkg, split, D):
     """dz = dgrad(dy) masked by ReLU'(GN(x)), plus per-channel (sum dz, sum dz*xhat): checked against autograd."""
     L = pkg.lib
     torch.manual_seed(3)
@@ -235,10 +239,8 @@ def test_conv3d_dgrad_groupnorm_relu_backward_epilogue(pkg, split, D):
     dy, x = L.Act.from_ncdhw(dyv, split=split), L.Act.from_ncdhw(xv, split=split)
     wdh, wdl, _, _, _ = L.pack_weights(w, 1, split=split)
     _, _, _, _, wq = _packed_to_torch(L, w, 0, split, co, ci, 3)
-    stats = torch.zeros(n, ci, 2, dtype=torch.float64, device=DEV)
-    L.channel_stats(x, stats, ci)
     coef = torch.empty(n, ci, 4, device=DEV)
-    L.gn_finalize(stats, gamma, beta, n, ci, ci, G, D ** 3, 1e-5, coef)
+    L.gn_apply(x, L.Act.empty(n, D, D, D, ci, split=split), _channel_stats(x), gamma, beta, ci, G, coef)
     bst = torch.zeros(n, ci, 2, dtype=torch.float64, device=DEV)
     dz = L.Act.empty(n, D, D, D, ci, split=split)
     L.conv3d(dy, wdh, wdl, 3, 1, dz, ci, co, mode=1, gn_x=x, coef=coef, coef_ld=ci, bstats=bst)
@@ -308,40 +310,63 @@ def test_conv3d_weight_gradient(pkg, ci, co, dims, ksz, stride, split):
 
 
 @pytest.mark.parametrize("split", [False, True])
-@pytest.mark.parametrize("C,G,dims", [(16, 8, (8, 12, 8)), (8, 8, (4, 4, 4)), (24, 24, (6, 4, 10)), (64, 8, (4, 4, 8))])
-def test_groupnorm_relu_forward_backward(pkg, C, G, dims, split):
+@pytest.mark.parametrize("C,G,dims", [(16, 8, (8, 12, 8)), (8, 8, (4, 4, 4)), (24, 24, (6, 4, 10)), (64, 8, (4, 4, 8)),
+                                      (4, 4, (5, 6, 7))])   # 4 real channels in an 8-channel view: the network's first norm
+def test_fused_groupnorm_relu_forward_backward(pkg, C, G, dims, split):
+    """The kernels every norm layer of the plans launches: statistics -> coefficients -> GroupNorm + ReLU in one launch, and
+    backward statistics -> dgamma, dbeta, dx in one launch; plus the first block's gn_bwd_finalize."""
     L = pkg.lib
     torch.manual_seed(C)
     n = 2
     S = dims[0] * dims[1] * dims[2]
     x = L.Act.from_ncdhw(torch.randn(n, C, *dims, device=DEV) * 2 + 0.5, split=split)
+    Cv = x.c                                                 # view channels (C padded to 8): pitch of stats, coef, bstats
     gamma, beta = torch.randn(C, device=DEV) * 0.3 + 1, torch.randn(C, device=DEV) * 0.2
-    stats = torch.zeros(n, C, 2, dtype=torch.float64, device=DEV)
-    L.channel_stats(x, stats, C)
-    coef = torch.empty(n, C, 4, device=DEV)
-    L.gn_finalize(stats, gamma, beta, n, C, C, G, S, 1e-5, coef)
-    y = L.Act.empty(n, *dims, C, split=split)
-    L.gn_apply(x, y, coef, 0.0)
+    stats = _channel_stats(x)
+    stats[:, C:] = 7.0                                       # padded channels: ignored
+    coef = torch.full((n, Cv, 4), float("nan"), device=DEV)  # every entry is written
+    y = L.Act.empty(n, *dims, Cv, split=split)
+    L.gn_apply(x, y, stats, gamma, beta, C, G, coef)
     xv = x.to_ncdhw(C).double().cpu()
     ref_np = np.maximum(group_norm(xv.numpy(), G, gamma.double().cpu().numpy(), beta.double().cpu().numpy()), 0)   # numpy oracle
     assert rel(y.to_ncdhw(C), torch.from_numpy(ref_np)) < TOL_STORE[split]
+    xg = xv.reshape(n, G, -1)
+    mu_ref = xg.mean(-1).repeat_interleave(C // G, dim=1)
+    rstd_ref = (xg.var(-1, unbiased=False) + 1e-5).rsqrt().repeat_interleave(C // G, dim=1)
+    a_ref = gamma.double().cpu() * rstd_ref
+    assert rel(coef[:, :C, 2], mu_ref) < 1e-6 and rel(coef[:, :C, 3], rstd_ref) < 1e-6
+    assert rel(coef[:, :C, 0], a_ref) < 1e-6 and rel(coef[:, :C, 1], beta.double().cpu() - mu_ref * a_ref) < 1e-6
+    if Cv > C:
+        assert float(coef[:, C:].abs().max()) == 0.0 and float(y.value()[..., C:].abs().max()) == 0.0
     # backward: dx = dL/dx given dz = dL/d(GN output)
     dz = L.Act.from_ncdhw(torch.randn(n, C, *dims, device=DEV), split=split)
     dzq = dz.to_ncdhw(C).double().cpu()
     xq = xv.clone().requires_grad_(True)
     g64, b64 = gamma.double().cpu().requires_grad_(True), beta.double().cpu().requires_grad_(True)
     F.group_norm(xq, G, g64, b64, 1e-5).backward(dzq)
-    mu, rstd = coef[..., 2].double().cpu(), coef[..., 3].double().cpu()
+    mu, rstd = coef[:, :C, 2].double().cpu(), coef[:, :C, 3].double().cpu()
     xhat = (xv - mu[:, :, None, None, None]) * rstd[:, :, None, None, None]
-    bst = torch.stack([dzq.sum(dim=(2, 3, 4)), (dzq * xhat).sum(dim=(2, 3, 4))], dim=-1).contiguous().to(DEV)
-    coef2 = torch.empty(n, C, 2, device=DEV)
-    dg, db = torch.empty(C, device=DEV), torch.empty(C, device=DEV)
-    L.gn_bwd_finalize(bst, coef, gamma, n, C, C, G, S, coef2, dg, db)
+    bst = torch.zeros(n, Cv, 2, dtype=torch.float64)
+    bst[:, :C] = torch.stack([dzq.sum(dim=(2, 3, 4)), (dzq * xhat).sum(dim=(2, 3, 4))], dim=-1)
+    bst = bst.to(DEV)
     add = L.Act.from_ncdhw(torch.randn(n, C, *dims, device=DEV), split=split)
-    dx = L.Act.empty(n, *dims, C, split=split)
-    L.gn_bwd(dz, x, coef, coef2, dx, add1=add)
+    dx = L.Act.empty(n, *dims, Cv, split=split)
+    dg, db = torch.full((C,), float("nan"), device=DEV), torch.full((C,), float("nan"), device=DEV)
+    L.gn_bwd(dz, x, coef, bst, gamma, C, G, dx, dg, db, add1=add)
     assert rel(dx.to_ncdhw(C), xq.grad + add.to_ncdhw(C).double().cpu()) < TOL_STORE[split]
     assert rel(dg, g64.grad) < 1e-5 and rel(db, b64.grad) < 1e-5
+    if Cv > C:
+        assert float(dx.value()[..., C:].abs().max()) == 0.0      # A = E = F = 0, and the padded add channels are zero
+    # the first block's norm: (E, F) of dx = A dz + E x + F for the input gradient, dgamma and dbeta
+    coef2 = torch.full((n, Cv, 2), float("nan"), device=DEV)
+    dg2, db2 = torch.empty(C, device=DEV), torch.empty(C, device=DEV)
+    L.gn_bwd_finalize(bst, coef, gamma, n, C, Cv, G, S, coef2, dg2, db2)
+    k, e = coef[:, :C].double().cpu(), coef2[:, :C].double().cpu()
+    dx2 = k[..., 0, None, None, None] * dzq + e[..., 0, None, None, None] * xv + e[..., 1, None, None, None]
+    assert rel(dx2, xq.grad) < TOL_STORE[True]
+    assert rel(dg2, g64.grad) < 1e-5 and rel(db2, b64.grad) < 1e-5
+    if Cv > C:
+        assert float(coef2[:, C:].abs().max()) == 0.0
 
 
 @pytest.mark.parametrize("split", [False, True])
