@@ -4,7 +4,7 @@ predict interface.  The directory name starts with a digit, so import it with
 """
 from . import lib, models, losses, train, predict, parallel, prepost  # noqa: F401
 from .models import UNet3D, AutocastUNet, AutoImplantUNet, DynUNet, fetch_model_by_name, build_or_load_model  # noqa: F401
-from .losses import DiceLoss  # noqa: F401
+from .losses import DiceLoss, DiceCELoss  # noqa: F401
 from .predict import SlidingWindowInferer, volumetric_predictions  # noqa: F401
 from .train import GraphedTrainStep, epoch_training, batch_loss  # noqa: F401
 

@@ -163,6 +163,28 @@ int b200unet_dice_bwd(const float* logits, const void* target, int n, int c, int
                          to_stream(stream));
 }
 
+static DiceCEDesc to_dice_ce(const b200unet_dice_ce_desc* d) {
+  DiceCEDesc r;
+  r.act = d->act; r.target_kind = d->target_kind; r.include_background = d->include_background; r.squared_pred = d->squared_pred;
+  r.jaccard = d->jaccard; r.batch = d->batch; r.reduction = d->reduction;
+  r.smooth_nr = d->smooth_nr; r.smooth_dr = d->smooth_dr; r.lambda_dice = d->lambda_dice; r.lambda_ce = d->lambda_ce;
+  return r;
+}
+size_t b200unet_dice_ce_scratch_bytes(const b200unet_dice_ce_desc* desc, int n, int c, int64_t spatial) {
+  if (!desc) { set_error("%s: null argument desc", __func__); return 0; }
+  return dice_ce_scratch_bytes(to_dice_ce(desc), n, c, spatial);
+}
+int b200unet_dice_ce_fwd(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c, int64_t spatial,
+                         void* scratch, float* loss, void* stream) {
+  NOT_NULL(desc); NOT_NULL(logits); NOT_NULL(target); NOT_NULL(scratch); NOT_NULL(loss);
+  return launch_dice_ce_fwd(to_dice_ce(desc), logits, target, n, c, spatial, scratch, loss, to_stream(stream));
+}
+int b200unet_dice_ce_bwd(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c, int64_t spatial,
+                         const void* scratch, const float* grad_out, float* dlogits, void* stream) {
+  NOT_NULL(desc); NOT_NULL(logits); NOT_NULL(target); NOT_NULL(scratch); NOT_NULL(grad_out); NOT_NULL(dlogits);
+  return launch_dice_ce_bwd(to_dice_ce(desc), logits, target, n, c, spatial, scratch, grad_out, dlogits, to_stream(stream));
+}
+
 int b200unet_tiles_gather(const float* vol, int n, int c, int d, int h, int w, const int32_t* starts, int ntiles, int rd, int rh,
                           int rw, float* tiles, void* stream) {
   NOT_NULL(vol); NOT_NULL(starts); NOT_NULL(tiles);

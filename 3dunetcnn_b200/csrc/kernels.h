@@ -75,6 +75,20 @@ int launch_dice_bwd(const float* logits, const uint8_t* target, int N, int C, lo
                     float smooth_nr, float smooth_dr, const double* sums, const float* grad_out, float* dlogits,
                     cudaStream_t st);
 
+// ---- Dice + cross-entropy criterion (dice_ce.cu); the fields mirror b200unet_dice_ce_desc
+struct DiceCEDesc {
+  int act;               // 0 identity, 1 sigmoid, 2 softmax over channels
+  int target_kind;       // 0 uint8 label map [N][1][S], 1 int64 label map, 2 uint8 [N][C][S], 3 fp32 [N][C][S]
+  int include_background, squared_pred, jaccard, batch;
+  int reduction;         // 0 mean, 1 sum
+  float smooth_nr, smooth_dr, lambda_dice, lambda_ce;
+};
+size_t dice_ce_scratch_bytes(const DiceCEDesc& d, int N, int C, long long S);   // 0: the shape or options are rejected
+int launch_dice_ce_fwd(const DiceCEDesc& d, const float* logits, const void* target, int N, int C, long long S, void* scratch,
+                       float* loss, cudaStream_t st);
+int launch_dice_ce_bwd(const DiceCEDesc& d, const float* logits, const void* target, int N, int C, long long S, const void* scratch,
+                       const float* grad_out, float* dlogits, cudaStream_t st);
+
 // ---- steps before / after the path (prepost.cu): sliding-window tiles, one-hot targets, z-score, label maps
 #define B200_MAX_TILES 16
 #define B200_MAX_LABEL_CHANNELS 128

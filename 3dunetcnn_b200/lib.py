@@ -34,6 +34,13 @@ class ConvDesc(C.Structure):
                 ("coef_ld", C.c_int32), ("slope", C.c_float), ("bstats", C.c_void_p), ("cls_mode", C.c_int32)]
 
 
+class DiceCEDesc(C.Structure):
+    """``b200unet_dice_ce_desc``: options of the Dice + cross-entropy criterion."""
+    _fields_ = [("act", C.c_int32), ("target_kind", C.c_int32), ("include_background", C.c_int32), ("squared_pred", C.c_int32),
+                ("jaccard", C.c_int32), ("batch", C.c_int32), ("reduction", C.c_int32), ("smooth_nr", C.c_float),
+                ("smooth_dr", C.c_float), ("lambda_dice", C.c_float), ("lambda_ce", C.c_float)]
+
+
 class NetDesc(C.Structure):
     _fields_ = [("n_features", C.c_int32), ("n_outputs", C.c_int32), ("base_width", C.c_int32),
                 ("n_levels", C.c_int32), ("encoder_blocks", C.c_int32 * 8), ("decoder_blocks", C.c_int32 * 8),
@@ -95,6 +102,11 @@ _SIGS = {
                                     C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200unet_dice_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_float,
                                     C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200unet_dice_ce_scratch_bytes": (C.c_size_t, [C.POINTER(DiceCEDesc), C.c_int, C.c_int, C.c_int64]),
+    "b200unet_dice_ce_fwd": (C.c_int, [C.POINTER(DiceCEDesc), C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p,
+                                       C.c_void_p, C.c_void_p]),
+    "b200unet_dice_ce_bwd": (C.c_int, [C.POINTER(DiceCEDesc), C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200unet_act_bwd": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_float,
                                    C.POINTER(Tensor5), C.c_void_p, C.c_int, C.c_void_p]),
     "b200unet_tiles_gather": (C.c_int, [C.c_void_p] + [C.c_int] * 5 + [C.POINTER(C.c_int32), C.c_int, C.c_int, C.c_int, C.c_int,
@@ -351,3 +363,45 @@ def dice_bwd(logits, target, flags, nr, dr, sums, grad_out, dlogits) -> None:
     check(load_library().b200unet_dice_bwd(logits.data_ptr(), target.data_ptr(), n, c, s, flags, nr, dr,
                                            sums.data_ptr(), grad_out.data_ptr(), dlogits.data_ptr(), stream_ptr()),
           "dice_bwd")
+
+
+# b200unet_dice_ce_desc.target_kind of each target form
+DICE_CE_TARGETS = {"label_u8": 0, "label_i64": 1, "onehot_u8": 2, "soft_f32": 3}
+_DICE_CE_ACTS = {None: 0, "sigmoid": 1, "softmax": 2}
+
+
+def dice_ce_desc(act=None, target_kind=0, include_background=True, squared_pred=False, jaccard=False, batch=False,
+                 reduction="mean", smooth_nr=1e-5, smooth_dr=1e-5, lambda_dice=1.0, lambda_ce=1.0) -> DiceCEDesc:
+    if reduction not in ("mean", "sum"):
+        raise ValueError("fused DiceCE supports reduction 'mean' or 'sum', got %r" % (reduction,))
+    d = DiceCEDesc()
+    d.act, d.target_kind = _DICE_CE_ACTS[act], int(target_kind)
+    d.include_background, d.squared_pred, d.jaccard, d.batch = (int(bool(v)) for v in (include_background, squared_pred, jaccard, batch))
+    d.reduction = int(reduction == "sum")
+    d.smooth_nr, d.smooth_dr, d.lambda_dice, d.lambda_ce = float(smooth_nr), float(smooth_dr), float(lambda_dice), float(lambda_ce)
+    return d
+
+
+def _nc_s(logits):
+    return logits.shape[0], logits.shape[1], logits[0, 0].numel()
+
+
+def dice_ce_scratch_bytes(desc: DiceCEDesc, n: int, c: int, s: int) -> int:
+    lib = load_library()
+    b = int(lib.b200unet_dice_ce_scratch_bytes(C.byref(desc), n, c, s))
+    if b == 0:
+        msg = lib.b200unet_last_error()
+        raise RuntimeError("libb200unet dice_ce_scratch_bytes rejected n=%d c=%d spatial=%d: %s" % (n, c, s, msg.decode() if msg else "?"))
+    return b
+
+
+def dice_ce_fwd(desc: DiceCEDesc, logits, target, scratch, loss) -> None:
+    n, c, s = _nc_s(logits)
+    check(load_library().b200unet_dice_ce_fwd(C.byref(desc), logits.data_ptr(), target.data_ptr(), n, c, s, scratch.data_ptr(),
+                                              loss.data_ptr(), stream_ptr()), "dice_ce_fwd")
+
+
+def dice_ce_bwd(desc: DiceCEDesc, logits, target, scratch, grad_out, dlogits) -> None:
+    n, c, s = _nc_s(logits)
+    check(load_library().b200unet_dice_ce_bwd(C.byref(desc), logits.data_ptr(), target.data_ptr(), n, c, s, scratch.data_ptr(),
+                                              grad_out.data_ptr(), dlogits.data_ptr(), stream_ptr()), "dice_ce_bwd")

@@ -139,6 +139,27 @@ int b200unet_dice_bwd(const float* logits, const void* target, int n, int c, int
                       float smooth_nr, float smooth_dr, const double* sums, const float* grad_out, float* dlogits,
                       void* stream);
 
+/* ---- Dice + cross-entropy criterion (monai.losses.DiceCELoss): loss = lambda_dice * Dice(act(x), t) + lambda_ce * CE(x, t).
+ * Dice is the formula above on p = act(x); include_background = 0 drops channel 0 after the activation.  CE is on the raw
+ * logits: -sum_c t_c log_softmax(x)_c for c > 1 (a label map is its one-hot row), BCEWithLogits(x, t) for c == 1; mean
+ * divides by n * spatial.  With c == 1 softmax is ignored and a uint8 label map is the target itself (int64: E_UNSUPPORTED).
+ * A label outside [0, c) is an all-zero target row.  logits NCDHW fp32, 1 <= c <= 128.
+ * scratch: b200unet_dice_ce_scratch_bytes() bytes (0 = the options or shape are rejected), written by fwd and read by bwd.
+ * It starts with sums [n][c][3] fp64 (I, P, T) and ce [n] fp64 (the summed CE terms of each sample).  No floating-point
+ * atomics: the loss and dlogits are bit-identical run to run. */
+typedef struct b200unet_dice_ce_desc {
+  int32_t act;                  /* 0 identity, 1 sigmoid, 2 softmax over channels */
+  int32_t target_kind;          /* 0 uint8 label map [n][1][spatial], 1 int64 label map, 2 uint8 [n][c][spatial], 3 fp32 [n][c][spatial] */
+  int32_t include_background, squared_pred, jaccard, batch;
+  int32_t reduction;            /* 0 mean, 1 sum */
+  float smooth_nr, smooth_dr, lambda_dice, lambda_ce;
+} b200unet_dice_ce_desc;
+size_t b200unet_dice_ce_scratch_bytes(const b200unet_dice_ce_desc* desc, int n, int c, int64_t spatial);
+int b200unet_dice_ce_fwd(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c,
+                         int64_t spatial, void* scratch, float* loss, void* stream);
+int b200unet_dice_ce_bwd(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c,
+                         int64_t spatial, const void* scratch, const float* grad_out, float* dlogits, void* stream);
+
 /* ---- sliding-window inference on the device (monai.inferers.SlidingWindowInferer as called by
  * predict/volumetric.py:147-148 and train/training_utils.py:106-107).  `starts`: HOST array [ntiles][4] of
  * (sample, d0, h0, w0), at most 16 tiles per call; volumes and tiles are NCDHW fp32.
