@@ -215,4 +215,15 @@ int b200unet_label_map(const float* p, int n_labels, int64_t spatial, const int3
   return launch_label_map(p, n_labels, spatial, labels, act, threshold, hierarchy, sum_then_threshold, out, to_stream(stream));
 }
 
+size_t b200unet_cc_scratch_bytes(int nvol, int d, int h, int w) { return cc_scratch_bytes(nvol, d, h, w); }
+int b200unet_cc_label(const uint8_t* mask, int nvol, int d, int h, int w, int connectivity, int32_t* labels, int32_t* counts,
+                      void* scratch, void* stream) {
+  NOT_NULL(mask); NOT_NULL(labels); NOT_NULL(counts); NOT_NULL(scratch);
+  return launch_cc_label(mask, nvol, d, h, w, connectivity, labels, counts, scratch, to_stream(stream));
+}
+int b200unet_cc_sort_by_size(int32_t* labels, int nvol, int d, int h, int w, int max_count, void* scratch, void* stream) {
+  NOT_NULL(labels); NOT_NULL(scratch);
+  return launch_cc_sort_by_size(labels, nvol, d, h, w, max_count, scratch, to_stream(stream));
+}
+
 }  // extern "C"

@@ -106,6 +106,12 @@ int launch_zscore(const float* x, int groups, long long S, int nonzero, double* 
 int launch_label_map(const float* p, int L, long long S, const int32_t* labels, int act, float thr, int hierarchy,
                      int sum_then_threshold, int16_t* out, cudaStream_t st);
 
+// ---- connected components of binary masks (ccl.cu)
+size_t cc_scratch_bytes(int nvol, int d, int h, int w);   // 0: the shape is rejected
+int launch_cc_label(const uint8_t* mask, int nvol, int d, int h, int w, int connectivity, int32_t* labels, int32_t* counts,
+                    void* scratch, cudaStream_t st);
+int launch_cc_sort_by_size(int32_t* labels, int nvol, int d, int h, int w, int max_count, void* scratch, cudaStream_t st);
+
 // ---- tensor-core implicit-GEMM convolution (igemm_conv.cu)
 struct ConvSrc {
   Act x;               // A operand (NDHWC bf16, hi[/lo])

@@ -121,6 +121,10 @@ _SIGS = {
     "b200unet_zscore": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200unet_label_map": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.POINTER(C.c_int32), C.c_int, C.c_float, C.c_int, C.c_int,
                                      C.c_void_p, C.c_void_p]),
+    "b200unet_cc_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    "b200unet_cc_label": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_void_p]),
+    "b200unet_cc_sort_by_size": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "b200unet_plan_create": (C.c_int, [C.POINTER(NetDesc), C.POINTER(C.c_void_p)]),
     "b200unet_plan_destroy": (None, [C.c_void_p]),
     "b200unet_plan_num_params": (C.c_int, [C.c_void_p]),
@@ -393,6 +397,36 @@ def dice_ce_scratch_bytes(desc: DiceCEDesc, n: int, c: int, s: int) -> int:
         msg = lib.b200unet_last_error()
         raise RuntimeError("libb200unet dice_ce_scratch_bytes rejected n=%d c=%d spatial=%d: %s" % (n, c, s, msg.decode() if msg else "?"))
     return b
+
+
+def cc_scratch_bytes(nvol: int, d: int, h: int, w: int) -> int:
+    lib = load_library()
+    b = int(lib.b200unet_cc_scratch_bytes(nvol, d, h, w))
+    if b == 0:
+        msg = lib.b200unet_last_error()
+        raise RuntimeError("libb200unet cc_scratch_bytes rejected %d x %d x %d x %d: %s" % (nvol, d, h, w, msg.decode() if msg else "?"))
+    return b
+
+
+def _need_c_order(**tensors) -> None:
+    for name, t in tensors.items():
+        if not t.is_contiguous():
+            raise ValueError("%s must be contiguous (C order): the kernels read it as a dense [nvol, d, h, w] array" % name)
+
+
+def cc_label(mask, connectivity, labels, counts, scratch) -> None:
+    """mask uint8 [nvol, d, h, w] -> raster-order labels int32 (same shape) and counts int32 [nvol]"""
+    _need_c_order(mask=mask, labels=labels)
+    nvol, d, h, w = mask.shape
+    check(load_library().b200unet_cc_label(mask.data_ptr(), nvol, d, h, w, connectivity, labels.data_ptr(), counts.data_ptr(),
+                                           scratch.data_ptr(), stream_ptr()), "cc_label")
+
+
+def cc_sort_by_size(labels, max_count, scratch) -> None:
+    _need_c_order(labels=labels)
+    nvol, d, h, w = labels.shape
+    check(load_library().b200unet_cc_sort_by_size(labels.data_ptr(), nvol, d, h, w, max_count, scratch.data_ptr(), stream_ptr()),
+          "cc_sort_by_size")
 
 
 def dice_ce_fwd(desc: DiceCEDesc, logits, target, scratch, loss) -> None:

@@ -4,6 +4,8 @@ Mirrors (paths relative to /root/reference):
   * ``unet3d/utils/one_hot.py:7-37``   ``compile_one_hot_encoding``  label map -> one-hot uint8 target
   * ``unet3d/utils/one_hot.py:46-118`` ``convert_one_hot_to_label_map`` (+ hierarchy)  prediction -> label map
   * ``unet3d/datasets/segmentation.py:77-87``  ``normalization="zero_mean"`` -> ``monai.transforms.NormalizeIntensity``
+  * ``examples/sppin/process.py:269-274``  SimpleITK ``ConnectedComponent`` + ``RelabelComponent`` -> ``connected_components``;
+    ``monai.transforms.KeepLargestConnectedComponent`` -> ``keep_largest_connected_component``
 
 Same names, argument meaning and error behaviour; tensors live on the GPU and every voxel is touched by one
 hand-written kernel of libb200unet instead of a chain of boolean-mask torch ops on the host.  No CPU fallback.
@@ -126,3 +128,102 @@ def convert_one_hot_to_label_map_using_hierarchy(one_hot_encoding, labels, thres
     """one_hot.py:92-110."""
     return convert_one_hot_to_label_map(one_hot_encoding, labels, axis=axis, threshold=threshold, dtype=dtype,
                                         label_hierarchy=True)
+
+
+def _check_connectivity(connectivity) -> int:
+    if isinstance(connectivity, bool) or connectivity not in (1, 2, 3):
+        raise ValueError("connectivity must be 1 (6 face neighbours), 2 (18) or 3 (26), got %r" % (connectivity,))
+    return int(connectivity)
+
+
+def _size_ordered_labels(m8: torch.Tensor, connectivity: int):
+    """m8 uint8 [nvol, d, h, w] -> (int32 labels numbered by decreasing size, CPU int32 counts [nvol]).  The counts are the one
+    device-to-host read: their maximum sizes the sort."""
+    m8 = m8.contiguous()                         # the kernels read a C-order [nvol, d, h, w] array
+    nvol, d, h, w = m8.shape
+    labels = torch.empty(m8.shape, dtype=torch.int32, device=m8.device)
+    counts = torch.empty(nvol, dtype=torch.int32, device=m8.device)
+    with torch.cuda.device(m8.device):
+        scratch = torch.empty(_lib.cc_scratch_bytes(nvol, d, h, w), dtype=torch.uint8, device=m8.device)
+        _lib.cc_label(m8, connectivity, labels, counts, scratch)
+        counts = counts.cpu()
+        _lib.cc_sort_by_size(labels, int(counts.max()), scratch)
+    return labels, counts
+
+
+def connected_components(mask: torch.Tensor, connectivity: int = 1):
+    """Label the connected components of a mask (..., D, H, W) on the device: nonzero is foreground, every leading index is an
+    independent volume, ``connectivity`` counts orthogonal hops (1 = 6 face neighbours, 2 = 18, 3 = 26) as in scipy and MONAI.
+
+    Returns ``(labels, counts)``: int32 labels of the mask's shape, 0 for background and 1..K numbered by decreasing component
+    size, equal sizes in raster order of their first voxel (SimpleITK ``ConnectedComponent`` followed by
+    ``RelabelComponent(sortByObjectSize=True)``), and K per volume as a CPU int64 tensor over the leading dimensions.  So the
+    largest component of a prediction is ``connected_components(pred > 0.5)[0] == 1``.  Exact: no tolerance, the same result
+    every run.  One device-to-host read (the counts)."""
+    connectivity = _check_connectivity(connectivity)
+    _need_cuda(mask, "connected_components")
+    m = _plain(mask)
+    if m.dim() < 3:
+        raise ValueError("connected_components: expected a mask (..., D, H, W), got shape %s" % (tuple(m.shape),))
+    lead, (d, h, w) = tuple(m.shape[:-3]), tuple(m.shape[-3:])
+    if m.numel() == 0:
+        return torch.zeros(m.shape, dtype=torch.int32, device=m.device), torch.zeros(lead, dtype=torch.int64)
+    if m.dtype == torch.uint8:
+        m8 = m
+    elif m.dtype == torch.bool:
+        m8 = m.view(torch.uint8)
+    else:
+        m8 = (m != 0).view(torch.uint8)
+    labels, counts = _size_ordered_labels(m8.reshape(-1, d, h, w), connectivity)
+    return labels.reshape(m.shape), counts.to(torch.int64).reshape(lead)
+
+
+def keep_largest_connected_component(img: torch.Tensor, applied_labels=None, is_onehot: Optional[bool] = None,
+                                     independent: bool = True, connectivity: Optional[int] = None, num_components: int = 1):
+    """``monai.transforms.KeepLargestConnectedComponent`` on a channel-first 3D image (C, D, H, W) on the device.
+
+    ``img`` is a label map (one channel) or a one-hot image; ``is_onehot`` None means C > 1.  ``applied_labels``: the label
+    values (label map) or channels (one-hot) to clean; None means every label value but 0, or every channel but 0.
+    ``independent``: clean each applied label on its own; otherwise their union is one foreground.  ``connectivity`` in orthogonal
+    hops (None = 3, the 26-neighbourhood); ``num_components`` components are kept.  Foreground voxels of the other components
+    are set to 0 in a new tensor of the input's dtype; the input is not modified.
+
+    Components are ranked by size, equal sizes in raster order of their first voxel (SimpleITK's ``RelabelComponent`` order).
+    MONAI ranks equal sizes with an unstable ``argsort``, so where components of equal size straddle the ``num_components``
+    cut the kept one may differ from MONAI's; everywhere else the result is MONAI's.  At most two device-to-host reads: the
+    component counts, and the label values when ``applied_labels`` is None on a label map."""
+    connectivity = _check_connectivity(3 if connectivity is None else connectivity)
+    _need_cuda(img, "keep_largest_connected_component")
+    x = _plain(img)
+    if x.dim() != 4:
+        raise ValueError("keep_largest_connected_component: expected a channel-first 3D image (C, D, H, W), got shape %s"
+                         % (tuple(x.shape),))
+    if x.numel() == 0:
+        return x.clone()
+    onehot = x.shape[0] > 1 if is_onehot is None else bool(is_onehot)
+    if applied_labels is not None:
+        applied = list(applied_labels) if isinstance(applied_labels, (list, tuple)) else [applied_labels]
+    elif onehot:
+        # MONAI takes the channels holding any foreground, minus 0; a channel without foreground changes nothing
+        applied = list(range(1, x.shape[0]))
+    else:
+        if x.shape[0] != 1:
+            raise ValueError("If input not one-hotted, should only be 1 channel, got %d." % x.shape[0])
+        applied = [v for v in torch.unique(x).tolist() if v != 0]
+    out = x.clone()
+    if not applied:
+        return out
+    if onehot:
+        idx = [int(i) for i in applied]
+        fg = x[idx] > 0 if independent else (x[idx] == 1).any(0, keepdim=True)
+    else:
+        fg = torch.stack([x[0] == v for v in applied])
+        if not independent:
+            fg = fg.any(0, keepdim=True)
+    labels, _ = _size_ordered_labels(fg.view(torch.uint8), connectivity)
+    drop = fg & (labels > num_components)
+    if onehot:
+        out[idx] = out[idx].masked_fill(drop, 0)
+    else:
+        out[0].masked_fill_(drop.any(0), 0)      # the label masks are disjoint
+    return out

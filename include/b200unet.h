@@ -188,6 +188,20 @@ int b200unet_zscore(const float* x, int groups, int64_t spatial, int nonzero, do
 int b200unet_label_map(const float* p, int n_labels, int64_t spatial, const int32_t* labels, int act, float threshold,
                        int hierarchy, int sum_then_threshold, int16_t* out, void* stream);
 
+/* ---- connected components of binary masks (the clean-up after the path: SimpleITK ConnectedComponent + RelabelComponent,
+ * MONAI KeepLargestConnectedComponent).  mask uint8 [nvol][d][h][w], nonzero = foreground; each volume is labelled on its own;
+ * d*h*w < 2^31.  connectivity in orthogonal hops: 1 = 6 face neighbours, 2 = 18 (+ edges), 3 = 26 (+ corners).
+ *   scratch_bytes: from the shape alone (0 = rejected); one buffer serves both calls.
+ *   label:         labels int32 [nvol][d][h][w]: 0 background, 1..K_v numbered in raster order of each component's first voxel
+ *                  (scipy.ndimage.label); counts int32 [nvol] = K_v.  The component sizes stay in scratch for sort_by_size.
+ *   sort_by_size:  in place, after label with the same scratch: renumber by decreasing size, equal sizes in raster order
+ *                  (RelabelComponent(sortByObjectSize=True)).  max_count = max_v K_v, read back by the caller.  Consumes the sizes.
+ * Exact integers, independent of scheduling. */
+size_t b200unet_cc_scratch_bytes(int nvol, int d, int h, int w);
+int b200unet_cc_label(const uint8_t* mask, int nvol, int d, int h, int w, int connectivity, int32_t* labels, int32_t* counts,
+                      void* scratch, void* stream);
+int b200unet_cc_sort_by_size(int32_t* labels, int nvol, int d, int h, int w, int max_count, void* scratch, void* stream);
+
 /* ---- whole-network plan: UNet3D forward/backward (segmentation/unet.py:7-50, classification/myronenko.py,
  * classification/decoder.py:73-130, autoencoder/variational.py:37-87) as one schedule of the kernels above. */
 typedef struct b200unet_net_desc {
