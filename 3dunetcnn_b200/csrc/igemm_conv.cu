@@ -54,6 +54,7 @@ struct ConvCfg {
   static constexpr int STAGES_2 = MIN_BLOCKS == 2 ? (TWO_PER_SM - FIXED) / STAGE_BYTES : 0;
   static constexpr int STAGES_RAW = STAGES_2 >= 4 ? STAGES_2 : (SMEM_LIMIT - FIXED) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
+  static constexpr int BLOCKS_PER_SM = STAGES_2 >= 4 ? 2 : 1;
   static constexpr int PIPE_BYTES = STAGES * STAGE_BYTES > OUT_STAGING ? STAGES * STAGE_BYTES : OUT_STAGING;
   static constexpr int SMEM_BYTES = PIPE_BYTES + FIXED;
   static constexpr uint32_t LAYOUT = swizzle_for_row_bytes(KC * 2);
@@ -335,8 +336,48 @@ static int launch_cfg(const ConvMaps& maps, const ConvArgs& args, dim3 grid, cud
   return OK;
 }
 
+// Every (BN, KC) the dispatch below instantiates.
+#define B200_CONV_CONFIGS(X)                                                                                   \
+  X(16, 16) X(16, 32) X(16, 64) X(32, 16) X(32, 32) X(32, 64) X(64, 16) X(64, 32) X(64, 64) X(128, 16) X(128, 32) X(128, 64)
+
+// KC follows the widest source among those with the largest kernel.  A fused 1x1x1 second source that is wider than the
+// 3x3x3 first source is walked in more K chunks instead: sizing KC to it would pad every one of the 27 taps of the first
+// source with zero channels (the 32-channel last decoder conv with its 64-channel `sample` ran at the cost of a 64-channel
+// convolution).  In single-pass bf16 the nonzero products accumulate in the same order either way, so the output is the
+// same bit for bit.
+static int conv_kc(const ConvOp& op) {
+  int k = 0;
+  for (int s = 1; s < op.nsrc; ++s)
+    if (op.src[s].ksz > op.src[k].ksz || (op.src[s].ksz == op.src[k].ksz && op.src[s].x.C > op.src[k].x.C)) k = s;
+  const int c = op.src[k].x.C;
+  return c > 32 ? 64 : c > 16 ? 32 : 16;
+}
+
+static int conv_bn(const ConvOp& op) {
+  const int BN = op.out.C > 64 ? 128 : op.out.C > 32 ? 64 : op.out.C > 16 ? 32 : 16;
+  return op.cls_mode && BN > 64 ? 64 : BN;   // class mode keeps its staging tile beside the accumulator tile (ConvCfg)
+}
+
+// Halo mode must not cost a configuration the second CTA per SM that per-tap tiles give it.  With KC = 64 and BN <= 32 the
+// halo box leaves room for fewer than four ring stages in half of the SM's shared memory; at one CTA per SM the 64 -> 32
+// channel convolutions of the C2 step (forward at 128^3, data gradient at 64^3) took 1.4x as long as on per-tap tiles at
+// two (H100 80GB HBM3, 400 W).  With a single K chunk per source the two modes accumulate in the same order.
+template <int BN, int KC>
+constexpr bool halo_keeps_occupancy() {
+  return ConvCfg<BN, KC, CONV_HALO>::BLOCKS_PER_SM >= ConvCfg<BN, KC, CONV_STREAM>::BLOCKS_PER_SM;
+}
+
+static bool halo_keeps_occupancy(int BN, int KC) {
+#define B200_HALO_OCC(bn, kc) \
+  if (BN == bn && KC == kc) return halo_keeps_occupancy<bn, kc>();
+  B200_CONV_CONFIGS(B200_HALO_OCC)
+#undef B200_HALO_OCC
+  return false;
+}
+
 // Halo mode (see ConvMode) for 3x3x3 stride-1 convolutions (plus an optional fused 1x1x1 source) whose output planes fill the
-// 8 x 16 tile, in single-pass bf16.  Inputs wider than 64 channels take several halo boxes per tile, drained one after the other;
+// 8 x 16 tile, in single-pass bf16, when it keeps the configuration's CTAs per SM.  Inputs wider than 64 channels take several
+// halo boxes per tile, drained one after the other;
 // they stay on per-tap tiles unless voxels * Cout >= B200UNET_HALO_WIDE_MIN (tests set it to 0 to reach that path with
 // oracle-sized shapes; off by default: the forward category of the C2 step was slower with them in halo mode on the H100).  B200UNET_NO_HALO=1 keeps every launch on the per-tap kernel (A/B measurements).
 bool conv_halo_eligible(const ConvOp& op) {
@@ -350,7 +391,7 @@ bool conv_halo_eligible(const ConvOp& op) {
   long long wide_min = -1;
   if (const char* e = getenv("B200UNET_HALO_WIDE_MIN")) wide_min = atoll(e);
   if (c.x.C > 64 && (wide_min < 0 || (long long)op.out.N * op.out.D * op.out.H * op.out.W * op.out.C < wide_min)) return false;
-  return op.out.W >= 8 && op.out.H >= 16;
+  return op.out.W >= 8 && op.out.H >= 16 && halo_keeps_occupancy(conv_bn(op), conv_kc(op));
 }
 
 int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
@@ -367,7 +408,6 @@ int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
   a.N = out.N; a.Do = gD; a.Ho = gH; a.Wo = gW; a.Cout = out.C;
   pick_tile(gW, gH, gD, a.tw, a.th, a.td);
   a.tiles_w = ceil_div(gW, a.tw); a.tiles_h = ceil_div(gH, a.th); a.tiles_d = ceil_div(gD, a.td);
-  int cin_max = 0;
   bool split = false;
   for (int s = 0; s < op.nsrc; ++s) {
     const ConvSrc& c = op.src[s];
@@ -386,7 +426,6 @@ int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
                      (c.x.W + 2 * pad - c.ksz) / c.stride + 1 == out.W,
                  E_INVALID, "igemm_conv: source %d dims %dx%dx%d (k%d s%d) do not produce output %dx%dx%d", s, c.x.D,
                  c.x.H, c.x.W, c.ksz, c.stride, out.D, out.H, out.W);
-    if (c.x.C > cin_max) cin_max = c.x.C;
     if (c.x.lo || c.w_lo) split = true;
   }
   if (split) {
@@ -398,9 +437,8 @@ int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
     a.tw = 8; a.th = 16; a.td = 1;
     a.tiles_w = ceil_div(gW, a.tw); a.tiles_h = ceil_div(gH, a.th); a.tiles_d = gD;
   }
-  const int KC = cin_max > 32 ? 64 : cin_max > 16 ? 32 : 16;
-  int BN = out.C > 64 ? 128 : out.C > 32 ? 64 : out.C > 16 ? 32 : 16;
-  if (op.cls_mode && BN > 64) BN = 64;   // class mode keeps its staging tile beside the accumulator tile (ConvCfg)
+  const int KC = conv_kc(op);
+  const int BN = conv_bn(op);
   const Swz swz = swz_for_bytes(KC * 2);
   for (int s = 0; s < op.nsrc; ++s) {
     const ConvSrc& c = op.src[s];
@@ -490,15 +528,12 @@ int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
     if (op.cls_mode) {                                                                                         \
       if constexpr (bn <= 64) return launch_cfg<bn, kc, CONV_CLASS>(maps, a, grid, st, cmaps);                  \
     } else if (halo) {                                                                                         \
-      return launch_cfg<bn, kc, CONV_HALO>(maps, a, grid, st, cmaps);                                          \
+      if constexpr (halo_keeps_occupancy<bn, kc>()) return launch_cfg<bn, kc, CONV_HALO>(maps, a, grid, st, cmaps); \
     } else {                                                                                                   \
       return launch_cfg<bn, kc, CONV_STREAM>(maps, a, grid, st, cmaps);                                        \
     }                                                                                                          \
   }
-  B200_CONV_CASE(16, 16) B200_CONV_CASE(16, 32) B200_CONV_CASE(16, 64)
-  B200_CONV_CASE(32, 16) B200_CONV_CASE(32, 32) B200_CONV_CASE(32, 64)
-  B200_CONV_CASE(64, 16) B200_CONV_CASE(64, 32) B200_CONV_CASE(64, 64)
-  B200_CONV_CASE(128, 16) B200_CONV_CASE(128, 32) B200_CONV_CASE(128, 64)
+  B200_CONV_CONFIGS(B200_CONV_CASE)
 #undef B200_CONV_CASE
   set_error("igemm_conv: no kernel for BN=%d KC=%d", BN, KC);
   return E_UNSUPPORTED;
