@@ -5,6 +5,7 @@
 #include <cstdlib>
 #include "kernels.h"
 #include "../../include/b200unet.h"
+#include "../../include/b200unet_diag.h"
 
 namespace b200 {
 static thread_local char g_err[1024] = "";
@@ -27,6 +28,51 @@ static Act to_act(const b200unet_tensor* t) {
   return make_act(reinterpret_cast<bf16*>(t->hi), reinterpret_cast<bf16*>(t->lo), t->n, t->d, t->h, t->w, t->c, t->ld);
 }
 static cudaStream_t to_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
+
+// b200unet_conv_desc (+ the diagnostics options) -> ConvOp; the residual and norm-input views live beside the op
+struct ConvOpHolder {
+  ConvOp op;
+  Act res, gx;
+};
+static int to_conv_op(const b200unet_conv_desc* d, const b200unet_diag_ext* ext, ConvOpHolder* h) {
+  ConvOp& op = h->op;
+  memset(&op, 0, sizeof(op));
+  op.nsrc = d->nsrc;
+  if (d->nsrc < 1 || d->nsrc > 2) { set_error("conv3d: nsrc=%d", d->nsrc); return E_INVALID; }
+  for (int s = 0; s < d->nsrc; ++s) {
+    op.src[s].x = to_act(&d->x[s]);
+    op.src[s].w_hi = reinterpret_cast<const bf16*>(d->w_hi[s]);
+    op.src[s].w_lo = reinterpret_cast<const bf16*>(d->w_lo[s]);
+    op.src[s].ksz = d->ksz[s]; op.src[s].stride = d->stride[s]; op.src[s].Cip = d->cip[s];
+    op.src[s].nopad = d->ksz[s] == 2 ? 1 : 0;   // kernel 2 = the unpadded kernel = stride case
+  }
+  op.Cop = d->cop;
+  op.out = to_act(&d->out);
+  if (d->res) { h->res = to_act(d->res); op.res = &h->res; }
+  op.scale = d->scale; op.stats = d->stats; op.stats_ld = d->stats_ld; op.mode = d->mode;
+  if (d->gn_x) { h->gx = to_act(d->gn_x); op.gn_x = &h->gx; }
+  op.coef = d->coef; op.coef_ld = d->coef_ld; op.slope = d->slope; op.bstats = d->bstats;
+  op.cls_mode = d->cls_mode;
+  if (ext) {
+    op.bias = ext->bias;
+    op.zero_last = ext->zero_last;
+    for (int s = 0; s < d->nsrc; ++s) {
+      op.src[s].x.vD = ext->x_vis[s][0]; op.src[s].x.vH = ext->x_vis[s][1]; op.src[s].x.vW = ext->x_vis[s][2];
+    }
+  }
+  return OK;
+}
+
+static void set_vis(Act& a, const int32_t* v) { a.vD = v[0]; a.vH = v[1]; a.vW = v[2]; }
+
+static WgradOp to_wgrad_op(const b200unet_tensor* a, const b200unet_tensor* dy, int ksz, int stride, int cip, int cop,
+                           const b200unet_diag_ext* ext) {
+  WgradOp op;
+  memset(&op, 0, sizeof(op));
+  op.a = to_act(a); op.dy = to_act(dy); op.ksz = ksz; op.stride = stride; op.nopad = ksz == 2 ? 1 : 0; op.Cip = cip; op.Cop = cop;
+  if (ext) { set_vis(op.a, ext->a_vis); set_vis(op.dy, ext->dy_vis); }
+  return op;
+}
 }  // namespace b200
 
 using namespace b200;
@@ -63,34 +109,16 @@ int b200unet_unpack_wgrad(const float* g, int co, int ci, int cop, int cip, int 
 
 int b200unet_conv3d(const b200unet_conv_desc* d, void* stream) {
   NOT_NULL(d);
-  ConvOp op;
-  memset(&op, 0, sizeof(op));
-  op.nsrc = d->nsrc;
-  if (d->nsrc < 1 || d->nsrc > 2) { set_error("conv3d: nsrc=%d", d->nsrc); return E_INVALID; }
-  for (int s = 0; s < d->nsrc; ++s) {
-    op.src[s].x = to_act(&d->x[s]);
-    op.src[s].w_hi = reinterpret_cast<const bf16*>(d->w_hi[s]);
-    op.src[s].w_lo = reinterpret_cast<const bf16*>(d->w_lo[s]);
-    op.src[s].ksz = d->ksz[s]; op.src[s].stride = d->stride[s]; op.src[s].Cip = d->cip[s];
-    op.src[s].nopad = d->ksz[s] == 2 ? 1 : 0;   // kernel 2 = the unpadded kernel = stride case
-  }
-  op.Cop = d->cop;
-  op.out = to_act(&d->out);
-  Act res, gx;
-  if (d->res) { res = to_act(d->res); op.res = &res; }
-  op.scale = d->scale; op.stats = d->stats; op.stats_ld = d->stats_ld; op.mode = d->mode;
-  if (d->gn_x) { gx = to_act(d->gn_x); op.gn_x = &gx; }
-  op.coef = d->coef; op.coef_ld = d->coef_ld; op.slope = d->slope; op.bstats = d->bstats;
-  op.cls_mode = d->cls_mode;
-  return launch_igemm_conv(op, to_stream(stream));
+  ConvOpHolder h;
+  B200_TRY(to_conv_op(d, nullptr, &h));
+  return launch_igemm_conv(h.op, to_stream(stream));
 }
 
 int b200unet_conv3d_wgrad(const b200unet_tensor* a, const b200unet_tensor* dy, int ksz, int stride, int cip, int cop,
                           float* dw, void* stream) {
   NOT_NULL(a); NOT_NULL(dy); NOT_NULL(dw);
-  WgradOp op;
-  memset(&op, 0, sizeof(op));
-  op.a = to_act(a); op.dy = to_act(dy); op.ksz = ksz; op.stride = stride; op.nopad = ksz == 2 ? 1 : 0; op.Cip = cip; op.Cop = cop; op.dw = dw;
+  WgradOp op = to_wgrad_op(a, dy, ksz, stride, cip, cop, nullptr);
+  op.dw = dw;
   return launch_wgrad(op, to_stream(stream));
 }
 
@@ -224,6 +252,74 @@ int b200unet_cc_label(const uint8_t* mask, int nvol, int d, int h, int w, int co
 int b200unet_cc_sort_by_size(int32_t* labels, int nvol, int d, int h, int w, int max_count, void* scratch, void* stream) {
   NOT_NULL(labels); NOT_NULL(scratch);
   return launch_cc_sort_by_size(labels, nvol, d, h, w, max_count, scratch, to_stream(stream));
+}
+
+// ---- diagnostics (include/b200unet_diag.h)
+int b200unet_diag_conv3d_route(const b200unet_conv_desc* desc, const b200unet_diag_ext* ext, b200unet_conv_route* route) {
+  NOT_NULL(desc); NOT_NULL(route);
+  ConvOpHolder h;
+  B200_TRY(to_conv_op(desc, ext, &h));
+  ConvRoute r;
+  B200_TRY(conv_route(h.op, &r));
+  route->kind = r.kind; route->bn = r.BN; route->kc = r.KC;
+  route->kchunks[0] = r.kchunks[0]; route->kchunks[1] = r.kchunks[1];
+  route->npass = r.npass; route->cls_pair = r.cls_pair;
+  route->tw = r.tw; route->th = r.th; route->td = r.td;
+  for (int i = 0; i < 3; ++i) route->grid[i] = r.grid[i];
+  route->stages = r.stages; route->blocks_per_sm = r.blocks_per_sm; route->smem_bytes = r.smem_bytes;
+  return OK;
+}
+
+int b200unet_diag_wgrad_route(const b200unet_tensor* a, const b200unet_tensor* dy, int ksz, int stride, int cip, int cop,
+                              const b200unet_diag_ext* ext, int deterministic, int num_sms, b200unet_wgrad_route* route) {
+  NOT_NULL(a); NOT_NULL(dy); NOT_NULL(route);
+  if (num_sms < 1) { set_error("%s: num_sms=%d", __func__, num_sms); return E_INVALID; }
+  WgradOp op = to_wgrad_op(a, dy, ksz, stride, cip, cop, ext);
+  float placeholder;
+  if (deterministic) op.part = &placeholder;   // only its presence matters to the route
+  WgradRoute r;
+  B200_TRY(wgrad_route(op, num_sms, &r));
+  route->kind = r.kind; route->ci8 = r.ci8;
+  route->cb = r.CB; route->bn = r.BN; route->qt = r.QT;
+  route->groups = r.groups; route->cotiles = r.cotiles; route->kblocks = r.kblocks; route->splits = r.splits; route->npass = r.npass;
+  route->tw = r.tw; route->th = r.th; route->td = r.td;
+  route->part_bytes = (int64_t)r.part_bytes;
+  return OK;
+}
+
+size_t b200unet_diag_wgrad_partial_bytes(const b200unet_tensor* a, const b200unet_tensor* dy, int ksz, int stride, int cip, int cop,
+                                         const b200unet_diag_ext* ext, int num_sms) {
+  if (!a || !dy || num_sms < 1) { set_error("%s: bad argument", __func__); return 0; }
+  return wgrad_partial_bytes(to_wgrad_op(a, dy, ksz, stride, cip, cop, ext), num_sms);
+}
+
+int b200unet_diag_conv3d_ex(const b200unet_conv_desc* desc, const b200unet_diag_ext* ext, void* stream) {
+  NOT_NULL(desc);
+  ConvOpHolder h;
+  B200_TRY(to_conv_op(desc, ext, &h));
+  return launch_igemm_conv(h.op, to_stream(stream));
+}
+
+// the weight gradient as the plans run it (plan.cu: run_wgrad)
+int b200unet_diag_wgrad_ex(const b200unet_tensor* a, const b200unet_tensor* dy, int ksz, int stride, int cip, int cop,
+                           const b200unet_diag_ext* ext, float* part, size_t part_bytes, int* splits, float* dw, void* stream) {
+  NOT_NULL(a); NOT_NULL(dy); NOT_NULL(dw);
+  WgradOp op = to_wgrad_op(a, dy, ksz, stride, cip, cop, ext);
+  op.dw = dw;
+  if (!part) return launch_wgrad(op, to_stream(stream));
+  int n = 0;
+  op.part = part; op.part_bytes = part_bytes; op.part_splits = &n;
+  B200_TRY(launch_wgrad(op, to_stream(stream)));
+  B200_REQUIRE(n >= 1, E_INVALID, "wgrad: deterministic weight gradient wrote no partial slots");
+  if (splits) *splits = n;
+  return launch_wgrad_reduce(part, n, (long long)ksz * ksz * ksz * cip * cop, dw, to_stream(stream));
+}
+
+int b200unet_diag_bias_grad(const b200unet_tensor* dy, const b200unet_diag_ext* ext, float* dbias, void* stream) {
+  NOT_NULL(dy); NOT_NULL(dbias);
+  Act y = to_act(dy);
+  if (ext) set_vis(y, ext->dy_vis);
+  return launch_bias_grad(y, dbias, to_stream(stream));
 }
 
 }  // extern "C"

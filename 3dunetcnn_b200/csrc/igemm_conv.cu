@@ -394,20 +394,38 @@ bool conv_halo_eligible(const ConvOp& op) {
   return op.out.W >= 8 && op.out.H >= 16 && halo_keeps_occupancy(conv_bn(op), conv_kc(op));
 }
 
-int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
+template <int BN_, int KC_, int MODE_>
+struct ConvKernel { static constexpr int BN = BN_, KC = KC_, MODE = MODE_; };
+
+// f(ConvKernel<BN, KC, MODE>{}) for the instantiated kernel of (kind, BN, KC): the one selection conv_route reports and
+// launch_igemm_conv launches.  E_UNSUPPORTED when no such kernel is instantiated.
+template <class F>
+static int with_conv_kernel(int kind, int BN, int KC, F&& f) {
+#define B200_CONV_CASE(bn, kc)                                                                              \
+  if (BN == bn && KC == kc) {                                                                               \
+    if (kind == CONV_KIND_CLASS1 || kind == CONV_KIND_CLASS2) {                                             \
+      if constexpr (bn <= 64) return f(ConvKernel<bn, kc, CONV_CLASS>{});                                   \
+    } else if (kind == CONV_KIND_HALO) {                                                                    \
+      if constexpr (halo_keeps_occupancy<bn, kc>()) return f(ConvKernel<bn, kc, CONV_HALO>{});              \
+    } else {                                                                                                \
+      return f(ConvKernel<bn, kc, CONV_STREAM>{});                                                          \
+    }                                                                                                       \
+  }
+  B200_CONV_CONFIGS(B200_CONV_CASE)
+#undef B200_CONV_CASE
+  set_error("igemm_conv: no kernel for BN=%d KC=%d (kind %d)", BN, KC, kind);
+  return E_UNSUPPORTED;
+}
+
+int conv_route(const ConvOp& op, ConvRoute* r) {
+  memset(r, 0, sizeof(*r));
   B200_REQUIRE(op.nsrc == 1 || op.nsrc == 2, E_INVALID, "igemm_conv: nsrc=%d", op.nsrc);
+  B200_REQUIRE(op.cls_mode >= 0 && op.cls_mode <= 2, E_INVALID, "igemm_conv: cls_mode=%d", op.cls_mode);
   const Act& out = op.out;
   B200_REQUIRE(out.C % 8 == 0 && out.ld % 8 == 0, E_UNSUPPORTED, "igemm_conv: Cout=%d (pitch %d) must be a multiple of 8",
                out.C, out.ld);
-  ConvArgs a;
-  memset(&a, 0, sizeof(a));
-  ConvMaps maps;
-  memset(&maps, 0, sizeof(maps));
   // class mode: the GEMM rows are the voxels of ONE parity class of the output = the source grid
   const int gD = op.cls_mode ? out.D / 2 : out.D, gH = op.cls_mode ? out.H / 2 : out.H, gW = op.cls_mode ? out.W / 2 : out.W;
-  a.N = out.N; a.Do = gD; a.Ho = gH; a.Wo = gW; a.Cout = out.C;
-  pick_tile(gW, gH, gD, a.tw, a.th, a.td);
-  a.tiles_w = ceil_div(gW, a.tw); a.tiles_h = ceil_div(gH, a.th); a.tiles_d = ceil_div(gD, a.td);
   bool split = false;
   for (int s = 0; s < op.nsrc; ++s) {
     const ConvSrc& c = op.src[s];
@@ -431,20 +449,56 @@ int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
   if (split) {
     for (int s = 0; s < op.nsrc; ++s)
       B200_REQUIRE(op.src[s].x.lo && op.src[s].w_lo, E_INVALID, "igemm_conv: split mode needs lo parts on every source");
+    B200_REQUIRE(out.lo != nullptr, E_INVALID, "igemm_conv: split mode needs a lo output");
+  }
+  if (op.res) B200_REQUIRE(op.res->C == out.C, E_INVALID, "igemm_conv: residual channel mismatch");
+  if (op.mode == 1) {
+    B200_REQUIRE(op.gn_x && op.coef, E_INVALID, "igemm_conv: mode 1 needs gn_x and coef");
+    B200_REQUIRE(op.gn_x->C == out.C, E_INVALID, "igemm_conv: gn_x channel mismatch");
   }
   const bool halo = conv_halo_eligible(op);
+  r->kind = op.cls_mode == 1 ? CONV_KIND_CLASS1 : op.cls_mode == 2 ? CONV_KIND_CLASS2 : halo ? CONV_KIND_HALO : CONV_KIND_TAP;
   if (halo) {   // one 8 x 16 output plane tile per CTA
-    a.tw = 8; a.th = 16; a.td = 1;
-    a.tiles_w = ceil_div(gW, a.tw); a.tiles_h = ceil_div(gH, a.th); a.tiles_d = gD;
+    r->tw = 8; r->th = 16; r->td = 1;
+  } else {
+    pick_tile(gW, gH, gD, r->tw, r->th, r->td);
   }
-  const int KC = conv_kc(op);
-  const int BN = conv_bn(op);
+  r->tiles_w = ceil_div(gW, r->tw); r->tiles_h = ceil_div(gH, r->th); r->tiles_d = ceil_div(gD, r->td);
+  r->KC = conv_kc(op);
+  r->BN = conv_bn(op);
+  for (int s = 0; s < op.nsrc; ++s) r->kchunks[s] = ceil_div(op.src[s].x.C, r->KC);
+  r->npass = split ? 3 : 1;
+  r->cls_pair = op.cls_mode && !split ? 1 : 0;
+  r->grid[0] = (int)((long long)out.N * r->tiles_d * r->tiles_h * r->tiles_w);
+  r->grid[1] = ceil_div(out.C, r->BN);
+  r->grid[2] = 1;
+  return with_conv_kernel(r->kind, r->BN, r->KC, [r](auto k) {
+    using Cfg = ConvCfg<decltype(k)::BN, decltype(k)::KC, decltype(k)::MODE>;
+    r->stages = Cfg::STAGES; r->blocks_per_sm = Cfg::BLOCKS_PER_SM; r->smem_bytes = Cfg::SMEM_BYTES;
+    return (int)OK;
+  });
+}
+
+int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
+  ConvRoute r;
+  B200_TRY(conv_route(op, &r));
+  const Act& out = op.out;
+  const bool split = r.npass == 3, halo = r.kind == CONV_KIND_HALO, cls = op.cls_mode != 0;
+  ConvArgs a;
+  memset(&a, 0, sizeof(a));
+  ConvMaps maps;
+  memset(&maps, 0, sizeof(maps));
+  a.N = out.N; a.Do = cls ? out.D / 2 : out.D; a.Ho = cls ? out.H / 2 : out.H; a.Wo = cls ? out.W / 2 : out.W; a.Cout = out.C;
+  a.tw = r.tw; a.th = r.th; a.td = r.td;
+  a.tiles_w = r.tiles_w; a.tiles_h = r.tiles_h; a.tiles_d = r.tiles_d;
+  const int KC = r.KC;
+  const int BN = r.BN;
   const Swz swz = swz_for_bytes(KC * 2);
   for (int s = 0; s < op.nsrc; ++s) {
     const ConvSrc& c = op.src[s];
     a.ntaps[s] = c.ksz * c.ksz * c.ksz; a.ksz[s] = c.ksz; a.stride[s] = c.stride; a.pad[s] = c.nopad ? 0 : c.ksz / 2;
-    a.kchunks[s] = ceil_div(c.x.C, KC);
-    const int estride = op.cls_mode ? 1 : c.stride;
+    a.kchunks[s] = r.kchunks[s];
+    const int estride = cls ? 1 : c.stride;
     B200_TRY(make_act_map(&maps.a[s][0], c.x.hi, c.x.N, c.x.D, c.x.H, c.x.W, c.x.C, c.x.ld, KC, a.tw, a.th, a.td,
                           estride, swz, c.x.vD, c.x.vH, c.x.vW));
     B200_TRY(make_w_map(&maps.b[s][0], c.w_hi, a.ntaps[s], op.Cop, c.Cip, KC, BN, swz));
@@ -459,43 +513,42 @@ int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
     B200_TRY(make_act_map(&maps.a[0][0], c.x.hi, c.x.N, c.x.D, c.x.H, c.x.W, c.x.C, c.x.ld, KC, 10, 18, 3, 1, swz, c.x.vD, c.x.vH,
                           c.x.vW));
   }
-  a.npass = split ? 3 : 1;
+  a.npass = r.npass;
   a.mode = op.mode;
   a.out_hi = out.hi; a.out_lo = out.lo; a.ldo = out.ld;
-  if (split) B200_REQUIRE(out.lo != nullptr, E_INVALID, "igemm_conv: split mode needs a lo output");
   ConvClassMaps cmaps;
   memset(&cmaps, 0, sizeof(cmaps));
-  if (op.cls_mode) {
+  if (cls) {
     // data gradient of y[o] = sum_k x[2o + k - 1] w[k]: dx[2j] = dy[j] w[1]; dx[2j+1] = dy[j] w[2] + dy[j+1] w[0].  With the
     // flipped pack Wd[k'] = w[2 - k'] (what emit_dgrad binds): even outputs use k' = 1 (delta 0), odd outputs k' = 0
     // (delta 0) and k' = 2 (delta +1); dy[j+1] beyond the grid reads as zero (TMA out-of-bounds fill).
     // cls_mode 2 (ConvTranspose3d, kernel = stride = 2): out[2j + p] = x[j] w[p], one tap per class
     a.cls_mode = op.cls_mode;
     const int cbo = BN < 64 ? BN : 64;
-    for (int cls = 0; cls < 8; ++cls) {
-      const int pd = (cls >> 2) & 1, ph = (cls >> 1) & 1, pw = cls & 1;
+    for (int c = 0; c < 8; ++c) {
+      const int pd = (c >> 2) & 1, ph = (c >> 1) & 1, pw = c & 1;
       int n = 0;
-      if (op.cls_mode == 2) a.cls_tap[cls][n++] = (unsigned char)cls;   // tap index kd*4 + kh*2 + kw = the class itself
+      if (op.cls_mode == 2) a.cls_tap[c][n++] = (unsigned char)c;   // tap index kd*4 + kh*2 + kw = the class itself
       else
       for (int kd = 0; kd < 3; ++kd)
         for (int kh = 0; kh < 3; ++kh)
           for (int kw = 0; kw < 3; ++kw) {
             const bool ok = (pd ? kd != 1 : kd == 1) && (ph ? kh != 1 : kh == 1) && (pw ? kw != 1 : kw == 1);
             if (!ok) continue;
-            a.cls_tap[cls][n++] = (unsigned char)((kd * 9 + kh * 3 + kw) | ((kw == 2) << 5) | ((kh == 2) << 6) | ((kd == 2) << 7));
+            a.cls_tap[c][n++] = (unsigned char)((kd * 9 + kh * 3 + kw) | ((kw == 2) << 5) | ((kh == 2) << 6) | ((kd == 2) << 7));
           }
-      a.cls_n[cls] = (unsigned char)n;
-      B200_TRY(make_act_map_class(&cmaps.oc[cls][0], out.hi, out.N, out.D, out.H, out.W, out.C, out.ld, pd, ph, pw, cbo, a.tw, a.th,
+      a.cls_n[c] = (unsigned char)n;
+      B200_TRY(make_act_map_class(&cmaps.oc[c][0], out.hi, out.N, out.D, out.H, out.W, out.C, out.ld, pd, ph, pw, cbo, a.tw, a.th,
                                   a.td, swz_for_bytes(cbo * 2)));
       if (split)
-        B200_TRY(make_act_map_class(&cmaps.oc[cls][1], out.lo, out.N, out.D, out.H, out.W, out.C, out.ld, pd, ph, pw, cbo, a.tw,
+        B200_TRY(make_act_map_class(&cmaps.oc[c][1], out.lo, out.N, out.D, out.H, out.W, out.C, out.ld, pd, ph, pw, cbo, a.tw,
                                     a.th, a.td, swz_for_bytes(cbo * 2)));
     }
     // single-pass bf16: the two W-parity classes of a (pd, ph) pair share one dense store (see tmap.h); the pair maps replace the
     // even classes' descriptors
-    if (!split) {
-      for (int cls = 0; cls < 8; cls += 2)
-        B200_TRY(make_act_map_classpair(&cmaps.oc[cls][0], out.hi, out.N, out.D, out.H, out.W, out.C, out.ld, (cls >> 2) & 1, (cls >> 1) & 1, cbo,
+    if (r.cls_pair) {
+      for (int c = 0; c < 8; c += 2)
+        B200_TRY(make_act_map_classpair(&cmaps.oc[c][0], out.hi, out.N, out.D, out.H, out.W, out.C, out.ld, (c >> 2) & 1, (c >> 1) & 1, cbo,
                                         2 * a.tw, a.th, a.td, swz_for_bytes(cbo * 2)));
       a.cls_pair = 1;
     }
@@ -509,34 +562,20 @@ int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
                             swz_for_bytes(cbo * 2)));
   }
   if (op.res) {
-    B200_REQUIRE(op.res->C == out.C, E_INVALID, "igemm_conv: residual channel mismatch");
     a.res_hi = op.res->hi; a.res_lo = op.res->lo; a.ldr = op.res->ld;
   }
   a.scale = op.scale;
   a.bias = op.bias; a.zero_last = op.zero_last;
   a.stats = op.stats; a.stats_ld = op.stats_ld;
   if (op.mode == 1) {
-    B200_REQUIRE(op.gn_x && op.coef, E_INVALID, "igemm_conv: mode 1 needs gn_x and coef");
-    B200_REQUIRE(op.gn_x->C == out.C, E_INVALID, "igemm_conv: gn_x channel mismatch");
     a.x_hi = op.gn_x->hi; a.x_lo = op.gn_x->lo; a.ldx = op.gn_x->ld;
     a.coef = reinterpret_cast<const float4*>(op.coef); a.coef_ld = op.coef_ld;
     a.slope = op.slope; a.bstats = op.bstats;
   }
-  dim3 grid((unsigned)((long long)a.N * a.tiles_d * a.tiles_h * a.tiles_w), (unsigned)ceil_div(out.C, BN), 1u);
-#define B200_CONV_CASE(bn, kc)                                                                                 \
-  if (BN == bn && KC == kc) {                                                                                  \
-    if (op.cls_mode) {                                                                                         \
-      if constexpr (bn <= 64) return launch_cfg<bn, kc, CONV_CLASS>(maps, a, grid, st, cmaps);                  \
-    } else if (halo) {                                                                                         \
-      if constexpr (halo_keeps_occupancy<bn, kc>()) return launch_cfg<bn, kc, CONV_HALO>(maps, a, grid, st, cmaps); \
-    } else {                                                                                                   \
-      return launch_cfg<bn, kc, CONV_STREAM>(maps, a, grid, st, cmaps);                                        \
-    }                                                                                                          \
-  }
-  B200_CONV_CONFIGS(B200_CONV_CASE)
-#undef B200_CONV_CASE
-  set_error("igemm_conv: no kernel for BN=%d KC=%d", BN, KC);
-  return E_UNSUPPORTED;
+  const dim3 grid((unsigned)r.grid[0], (unsigned)r.grid[1], (unsigned)r.grid[2]);
+  return with_conv_kernel(r.kind, BN, KC, [&](auto k) {
+    return launch_cfg<decltype(k)::BN, decltype(k)::KC, decltype(k)::MODE>(maps, a, grid, st, cmaps);
+  });
 }
 
 }  // namespace b200

@@ -146,6 +146,20 @@ struct ConvOp {
                        // parity-class implicit GEMMs (27 tap products in total instead of 8 x 27) in one launch
 };
 
+// The kernel a convolution runs on, decided from the op alone (no device or driver call): launch_igemm_conv launches exactly this.
+enum ConvKind { CONV_KIND_TAP = 0, CONV_KIND_HALO = 1, CONV_KIND_CLASS1 = 2, CONV_KIND_CLASS2 = 3 };
+struct ConvRoute {
+  int kind;                 // ConvKind
+  int BN, KC;
+  int kchunks[2];           // K chunks of KC channels per source
+  int npass;                // 1 bf16, 3 split precision
+  int cls_pair;             // class mode, bf16: the two W-parity classes share one staging tile and store
+  int tw, th, td;           // output voxel tile (class mode: of one parity class, on the source grid)
+  int tiles_w, tiles_h, tiles_d;
+  int grid[3];
+  int stages, blocks_per_sm, smem_bytes;   // ConvCfg of the instantiation
+};
+int conv_route(const ConvOp& op, ConvRoute* r);   // validates the op: OK or the error launch_igemm_conv would return
 int launch_igemm_conv(const ConvOp& op, cudaStream_t st);
 bool conv_halo_eligible(const ConvOp& op);   // shape-only: does this convolution run in halo mode?
 
@@ -168,6 +182,18 @@ struct WgradOp {
 int launch_wgrad_reduce(const float* part, int splits, long long elems, float* dw, cudaStream_t st);   // dw = sum_s part[s]
 // worst-case bytes of the partial buffer for this shape on a device with num_sms SMs (host-only shape logic)
 size_t wgrad_partial_bytes(const WgradOp& op, int num_sms);
+// The kernel a weight gradient runs on for a device with num_sms SMs (op.part set: deterministic mode), from the op alone.
+enum WgradKind { WGRAD_KIND_SIMT = 0, WGRAD_KIND_TAP = 1, WGRAD_KIND_HALO = 2 };
+struct WgradRoute {
+  int kind;                 // WgradKind
+  int ci8;                  // SIMT: input channels / 8
+  int CB, BN, QT;           // tensor-core kernels: channels per M box, N tile, M tiles per CTA
+  int nci, units, qtiles;   // CB chunks per tap, (tap, chunk) units, M tiles in total
+  int groups, cotiles, kblocks, splits, npass;
+  int tw, th, td;
+  size_t part_bytes;        // deterministic mode: splits * T * Cip * Cop * 4, the partial buffer this launch fills
+};
+int wgrad_route(const WgradOp& op, int num_sms, WgradRoute* r);
 int launch_wgrad(const WgradOp& op, cudaStream_t st);              // dispatcher: SIMT register tile for narrow 1x1x1
 bool wgrad_1x1_narrow_eligible(const WgradOp& op);              // 1x1x1, <= 16 input channels: SIMT register tile
 int launch_wgrad_1x1_narrow(const WgradOp& op, cudaStream_t st);

@@ -370,23 +370,85 @@ size_t wgrad_partial_bytes(const WgradOp& op, int num_sms) {
   return (size_t)splits * elems * sizeof(float);
 }
 
-int launch_wgrad(const WgradOp& op, cudaStream_t st) {
-  if (!op.part && wgrad_1x1_narrow_eligible(op)) return launch_wgrad_1x1_narrow(op, st);   // (the SIMT path reduces with atomics)
+template <int CB_, int BN_, bool HALO_>
+struct WgradKernel { static constexpr int CB = CB_, BN = BN_; static constexpr bool HALO = HALO_; };
+
+// Every (CB, BN) of the per-tap kernel and every BN of the halo kernel (CB = 64) that the dispatch instantiates.
+#define B200_WG_CONFIGS(X) \
+  X(16, 16) X(16, 32) X(16, 64) X(16, 128) X(32, 16) X(32, 32) X(32, 64) X(32, 128) X(64, 16) X(64, 32) X(64, 64) X(64, 128)
+#define B200_WG_HALO_CONFIGS(X) X(16) X(32) X(64) X(128)
+
+// f(WgradKernel<CB, BN, HALO>{}) for the tensor-core kernel of route r: the one selection wgrad_route reports and launch_wgrad
+// launches.  E_UNSUPPORTED when no such kernel is instantiated.
+template <class F>
+static int with_wgrad_kernel(const WgradRoute& r, F&& f) {
+  if (r.kind == WGRAD_KIND_HALO) {
+#define B200_WG_HALO_CASE(bn) \
+    if (r.CB == 64 && r.BN == bn) return f(WgradKernel<64, bn, true>{});
+    B200_WG_HALO_CONFIGS(B200_WG_HALO_CASE)
+#undef B200_WG_HALO_CASE
+  } else if (r.kind == WGRAD_KIND_TAP) {
+#define B200_WG_CASE(cb, bn) \
+    if (r.CB == cb && r.BN == bn) return f(WgradKernel<cb, bn, false>{});
+    B200_WG_CONFIGS(B200_WG_CASE)
+#undef B200_WG_CASE
+  }
+  set_error("wgrad: no kernel for CB=%d BN=%d (kind %d)", r.CB, r.BN, r.kind);
+  return E_UNSUPPORTED;
+}
+
+int wgrad_route(const WgradOp& op, int num_sms, WgradRoute* r) {
+  memset(r, 0, sizeof(*r));
   const Act& A = op.a;
   const Act& Y = op.dy;
+  if (!op.part && wgrad_1x1_narrow_eligible(op)) {   // (the SIMT path reduces with atomics)
+    B200_REQUIRE(A.N == Y.N && A.D == Y.D && A.H == Y.H && A.W == Y.W, E_INVALID, "wgrad_1x1_narrow: shape mismatch");
+    r->kind = WGRAD_KIND_SIMT;
+    r->ci8 = A.C / 8;
+    r->npass = 1;
+    return OK;
+  }
   B200_REQUIRE(op.ksz == 1 || op.ksz == 3 || (op.ksz == 2 && op.nopad && op.stride == 2), E_UNSUPPORTED,
                "wgrad: kernel_size=%d unsupported", op.ksz);
   B200_REQUIRE(op.stride == 1 || op.stride == 2, E_UNSUPPORTED, "wgrad: stride=%d unsupported", op.stride);
   B200_REQUIRE(A.C % 8 == 0 && Y.C % 8 == 0 && A.ld % 8 == 0 && Y.ld % 8 == 0, E_UNSUPPORTED,
                "wgrad: channels must be multiples of 8 (Ci=%d Co=%d)", A.C, Y.C);
   B200_REQUIRE(op.Cop % 4 == 0 && op.Cop >= Y.C && op.Cip >= A.C, E_INVALID, "wgrad: bad accumulator pitch");
-  B200_REQUIRE((reinterpret_cast<uintptr_t>(op.dw) & 15) == 0, E_INVALID, "wgrad: dw not 16B aligned");
   const int pad = op.nopad ? 0 : op.ksz / 2;
   B200_REQUIRE((A.D + 2 * pad - op.ksz) / op.stride + 1 == Y.D && (A.H + 2 * pad - op.ksz) / op.stride + 1 == Y.H &&
                    (A.W + 2 * pad - op.ksz) / op.stride + 1 == Y.W && A.N == Y.N,
                E_INVALID, "wgrad: shape mismatch");
   const bool split = A.lo != nullptr || Y.lo != nullptr;
   if (split) B200_REQUIRE(A.lo && Y.lo, E_INVALID, "wgrad: split mode needs lo parts on both operands");
+  const bool halo = wgrad_halo_eligible(op);
+  r->kind = halo ? WGRAD_KIND_HALO : WGRAD_KIND_TAP;
+  wgrad_tile(halo, op, r->tw, r->th, r->td);
+  const int ntaps = op.ksz * op.ksz * op.ksz;
+  r->CB = A.C > 32 ? 64 : A.C > 16 ? 32 : 16;
+  r->BN = Y.C > 64 ? 128 : Y.C > 32 ? 64 : Y.C > 16 ? 32 : 16;
+  r->nci = ceil_div(A.C, r->CB);
+  r->units = ntaps * r->nci;
+  r->qtiles = ceil_div(r->units, 128 / r->CB);
+  r->QT = 128 / r->BN;   // WgradCfg::QT
+  if (r->QT > r->qtiles) r->QT = r->qtiles;
+  r->groups = ceil_div(r->qtiles, r->QT);
+  r->QT = ceil_div(r->qtiles, r->groups);   // rebalance M tiles across groups
+  r->cotiles = ceil_div(Y.C, r->BN);
+  r->kblocks = Y.N * ceil_div(Y.D, r->td) * ceil_div(Y.H, r->th) * ceil_div(Y.W, r->tw);
+  r->splits = wgrad_stream_splits(op, num_sms, halo);
+  r->npass = split ? 3 : 1;
+  r->part_bytes = (size_t)r->splits * ntaps * op.Cip * op.Cop * sizeof(float);
+  return with_wgrad_kernel(*r, [](auto) { return (int)OK; });
+}
+
+int launch_wgrad(const WgradOp& op, cudaStream_t st) {
+  WgradRoute r;
+  B200_TRY(wgrad_route(op, device_sms(), &r));
+  if (r.kind == WGRAD_KIND_SIMT) return launch_wgrad_1x1_narrow(op, st);
+  const Act& A = op.a;
+  const Act& Y = op.dy;
+  B200_REQUIRE((reinterpret_cast<uintptr_t>(op.dw) & 15) == 0, E_INVALID, "wgrad: dw not 16B aligned");
+  const bool split = r.npass == 3, halo = r.kind == WGRAD_KIND_HALO;
 
   WgradArgs a;
   memset(&a, 0, sizeof(a));
@@ -394,34 +456,24 @@ int launch_wgrad(const WgradOp& op, cudaStream_t st) {
   memset(&maps, 0, sizeof(maps));
   a.N = Y.N; a.Do = Y.D; a.Ho = Y.H; a.Wo = Y.W;
   a.Ci = A.C; a.Co = Y.C; a.Cip = op.Cip; a.Cop = op.Cop;
-  const bool halo = wgrad_halo_eligible(op);
-  wgrad_tile(halo, op, a.tw, a.th, a.td);
+  a.tw = r.tw; a.th = r.th; a.td = r.td;
   a.tiles_w = ceil_div(Y.W, a.tw); a.tiles_h = ceil_div(Y.H, a.th); a.tiles_d = ceil_div(Y.D, a.td);
-  a.ksz = op.ksz; a.stride = op.stride; a.ntaps = op.ksz * op.ksz * op.ksz; a.pad = pad;
-  const int CB = A.C > 32 ? 64 : A.C > 16 ? 32 : 16;
-  const int BN = Y.C > 64 ? 128 : Y.C > 32 ? 64 : Y.C > 16 ? 32 : 16;
-  const int CBN = BN < 64 ? BN : 64;
-  a.nci = ceil_div(A.C, CB);
-  a.units = a.ntaps * a.nci;
-  const int bpm = 128 / CB;
-  a.qtiles = ceil_div(a.units, bpm);
-  a.qt = 128 / BN;   // WgradCfg::QT
-  if (a.qt > a.qtiles) a.qt = a.qtiles;
-  const int groups = ceil_div(a.qtiles, a.qt);
-  // rebalance M tiles across groups
-  a.qt = ceil_div(a.qtiles, groups);
-  const int cotiles = ceil_div(Y.C, BN);
-  a.kblocks = a.N * a.tiles_d * a.tiles_h * a.tiles_w;
-  const int splits = wgrad_stream_splits(op, device_sms(), halo);
-  a.splits = splits;
-  a.npass = split ? 3 : 1;
+  a.ksz = op.ksz; a.stride = op.stride; a.ntaps = op.ksz * op.ksz * op.ksz; a.pad = op.nopad ? 0 : op.ksz / 2;
+  const int CB = r.CB;
+  const int CBN = r.BN < 64 ? r.BN : 64;
+  a.nci = r.nci;
+  a.units = r.units;
+  a.qtiles = r.qtiles;
+  a.qt = r.QT;
+  a.kblocks = r.kblocks;
+  a.splits = r.splits;
+  a.npass = r.npass;
   a.dw = op.dw;
   if (op.part) {
     a.part = op.part;
     a.part_stride = (long long)a.ntaps * op.Cip * op.Cop;
-    B200_REQUIRE((size_t)splits * a.part_stride * sizeof(float) <= op.part_bytes, E_INVALID,
-                 "wgrad: deterministic partial buffer too small (%d splits)", splits);
-    if (op.part_splits) *op.part_splits = splits;
+    B200_REQUIRE(r.part_bytes <= op.part_bytes, E_INVALID, "wgrad: deterministic partial buffer too small (%d splits)", r.splits);
+    if (op.part_splits) *op.part_splits = r.splits;
   }
   if (halo)   // one (64, 10, 18, 3) box around the 8 x 16 x 1 voxel tile; the zero padding is TMA out-of-bounds fill
     B200_TRY(make_act_map(&maps.a[0], A.hi, A.N, A.D, A.H, A.W, A.C, A.ld, 64, 10, 18, 3, 1, SWZ_128, A.vD, A.vH, A.vW));
@@ -436,21 +488,10 @@ int launch_wgrad(const WgradOp& op, cudaStream_t st) {
     B200_TRY(make_act_map(&maps.dy[1], Y.lo, Y.N, Y.D, Y.H, Y.W, Y.C, Y.ld, CBN, a.tw, a.th, a.td, 1,
                           swz_for_bytes(CBN * 2), Y.vD, Y.vH, Y.vW));
   }
-  dim3 grid((unsigned)splits, (unsigned)groups, (unsigned)cotiles);
-  if (halo) {
-    if (BN == 16) return launch_wg<64, 16, true>(maps, a, grid, st);
-    if (BN == 32) return launch_wg<64, 32, true>(maps, a, grid, st);
-    if (BN == 64) return launch_wg<64, 64, true>(maps, a, grid, st);
-    if (BN == 128) return launch_wg<64, 128, true>(maps, a, grid, st);
-  }
-#define B200_WG_CASE(cb, bn) \
-  if (CB == cb && BN == bn) return launch_wg<cb, bn, false>(maps, a, grid, st);
-  B200_WG_CASE(16, 16) B200_WG_CASE(16, 32) B200_WG_CASE(16, 64) B200_WG_CASE(16, 128)
-  B200_WG_CASE(32, 16) B200_WG_CASE(32, 32) B200_WG_CASE(32, 64) B200_WG_CASE(32, 128)
-  B200_WG_CASE(64, 16) B200_WG_CASE(64, 32) B200_WG_CASE(64, 64) B200_WG_CASE(64, 128)
-#undef B200_WG_CASE
-  set_error("wgrad: no kernel for CB=%d BN=%d", CB, BN);
-  return E_UNSUPPORTED;
+  const dim3 grid((unsigned)r.splits, (unsigned)r.groups, (unsigned)r.cotiles);
+  return with_wgrad_kernel(r, [&](auto k) {
+    return launch_wg<decltype(k)::CB, decltype(k)::BN, decltype(k)::HALO>(maps, a, grid, st);
+  });
 }
 
 }  // namespace b200

@@ -18,6 +18,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200UNET_LIB") or os.path.join(_HERE, "libb200unet.so")
 CSRC = os.path.join(_HERE, "csrc")
 INCLUDE = os.path.join(os.path.dirname(_HERE), "include", "b200unet.h")
+INCLUDE_DIAG = os.path.join(os.path.dirname(_HERE), "include", "b200unet_diag.h")
 
 
 class Tensor5(C.Structure):
@@ -32,6 +33,28 @@ class ConvDesc(C.Structure):
                 ("out", Tensor5), ("res", C.POINTER(Tensor5)), ("scale", C.c_void_p), ("stats", C.c_void_p),
                 ("stats_ld", C.c_int32), ("mode", C.c_int32), ("gn_x", C.POINTER(Tensor5)), ("coef", C.c_void_p),
                 ("coef_ld", C.c_int32), ("slope", C.c_float), ("bstats", C.c_void_p), ("cls_mode", C.c_int32)]
+
+
+class DiagExt(C.Structure):
+    """``b200unet_diag_ext``: bias, zeroed high boundary and visible extents (include/b200unet_diag.h)."""
+    _fields_ = [("bias", C.c_void_p), ("zero_last", C.c_int32), ("x_vis", (C.c_int32 * 3) * 2), ("a_vis", C.c_int32 * 3),
+                ("dy_vis", C.c_int32 * 3)]
+
+
+class ConvRoute(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("bn", C.c_int32), ("kc", C.c_int32), ("kchunks", C.c_int32 * 2), ("npass", C.c_int32),
+                ("cls_pair", C.c_int32), ("tw", C.c_int32), ("th", C.c_int32), ("td", C.c_int32), ("grid", C.c_int32 * 3),
+                ("stages", C.c_int32), ("blocks_per_sm", C.c_int32), ("smem_bytes", C.c_int32)]
+
+
+class WgradRoute(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("ci8", C.c_int32), ("cb", C.c_int32), ("bn", C.c_int32), ("qt", C.c_int32),
+                ("groups", C.c_int32), ("cotiles", C.c_int32), ("kblocks", C.c_int32), ("splits", C.c_int32), ("npass", C.c_int32),
+                ("tw", C.c_int32), ("th", C.c_int32), ("td", C.c_int32), ("part_bytes", C.c_int64)]
+
+
+CONV_KINDS = ("tap", "halo", "class1", "class2")     # b200unet_conv_route.kind
+WGRAD_KINDS = ("simt", "tap", "halo")               # b200unet_wgrad_route.kind
 
 
 class DiceCEDesc(C.Structure):
@@ -58,7 +81,7 @@ def build_library(force: bool = False, verbose: bool = False) -> str:
     if os.path.exists(LIB_PATH) and not force:
         src_m = max(os.path.getmtime(os.path.join(CSRC, f)) for f in os.listdir(CSRC)
                     if f.endswith((".cu", ".cuh", ".h")) or f == "Makefile")
-        src_m = max(src_m, os.path.getmtime(INCLUDE))
+        src_m = max(src_m, os.path.getmtime(INCLUDE), os.path.getmtime(INCLUDE_DIAG))
         if os.path.getmtime(LIB_PATH) >= src_m:
             return LIB_PATH
     cmd = ["make", "-C", CSRC, "-j8"]
@@ -146,8 +169,16 @@ _SIGS = {
     "b200unet_plan_profile_dump": (C.c_int, [C.c_void_p, C.c_char_p]),
 }
 
-# entry points outside the product header (diagnostics), bound like _SIGS: none at present
-_DIAG_SIGS = {}
+# entry points outside the product header (include/b200unet_diag.h), bound like _SIGS
+_WG_ARGS = [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(DiagExt)]
+_DIAG_SIGS = {
+    "b200unet_diag_conv3d_route": (C.c_int, [C.POINTER(ConvDesc), C.POINTER(DiagExt), C.POINTER(ConvRoute)]),
+    "b200unet_diag_wgrad_route": (C.c_int, _WG_ARGS + [C.c_int, C.c_int, C.POINTER(WgradRoute)]),
+    "b200unet_diag_wgrad_partial_bytes": (C.c_size_t, _WG_ARGS + [C.c_int]),
+    "b200unet_diag_conv3d_ex": (C.c_int, [C.POINTER(ConvDesc), C.POINTER(DiagExt), C.c_void_p]),
+    "b200unet_diag_wgrad_ex": (C.c_int, _WG_ARGS + [C.c_void_p, C.c_size_t, C.POINTER(C.c_int), C.c_void_p, C.c_void_p]),
+    "b200unet_diag_bias_grad": (C.c_int, [C.POINTER(Tensor5), C.POINTER(DiagExt), C.c_void_p, C.c_void_p]),
+}
 
 EXPORTED_SYMBOLS = tuple(_SIGS)
 
@@ -256,6 +287,16 @@ def conv3d(x: Act, w_hi, w_lo, ksz: int, stride: int, out: Act, cop: int, cip: i
            stats: Optional[torch.Tensor] = None, stats_ld: int = 0, mode: int = 0, gn_x: Optional[Act] = None,
            coef: Optional[torch.Tensor] = None, coef_ld: int = 0, slope: float = 0.0,
            bstats: Optional[torch.Tensor] = None, cls_mode: int = 0) -> None:
+    d, keep = conv_desc(**locals())
+    check(load_library().b200unet_conv3d(C.byref(d), stream_ptr()), "conv3d")
+
+
+def conv_desc(x: Act, w_hi, w_lo, ksz: int, stride: int, out: Act, cop: int, cip: int, *, x2: Optional[Act] = None,
+              w2_hi=None, w2_lo=None, cip2: int = 0, res: Optional[Act] = None, scale: Optional[torch.Tensor] = None,
+              stats: Optional[torch.Tensor] = None, stats_ld: int = 0, mode: int = 0, gn_x: Optional[Act] = None,
+              coef: Optional[torch.Tensor] = None, coef_ld: int = 0, slope: float = 0.0,
+              bstats: Optional[torch.Tensor] = None, cls_mode: int = 0):
+    """``b200unet_conv_desc`` of a conv3d call, and the structures it points to (keep them alive while it is used)"""
     d = ConvDesc()
     d.x[0] = x.ct()
     d.w_hi[0] = w_hi.data_ptr()
@@ -286,7 +327,84 @@ def conv3d(x: Act, w_hi, w_lo, ksz: int, stride: int, out: Act, cop: int, cip: i
     d.slope = slope
     d.bstats = bstats.data_ptr() if bstats is not None else None
     d.cls_mode = cls_mode
-    check(load_library().b200unet_conv3d(C.byref(d), stream_ptr()), "conv3d")
+    return d, keep
+
+
+def diag_ext(bias: Optional[torch.Tensor] = None, zero_last: bool = False, x_vis=None, a_vis=None, dy_vis=None) -> DiagExt:
+    """``b200unet_diag_ext``; each *_vis is a (d, h, w) triple (x_vis: one per source), 0 = the full extent"""
+    e = DiagExt()
+    e.bias = _p(bias)
+    e.zero_last = int(bool(zero_last))
+    for s, v in enumerate(x_vis or ()):
+        e.x_vis[s][:] = list(v)
+    if a_vis is not None:
+        e.a_vis[:] = list(a_vis)
+    if dy_vis is not None:
+        e.dy_vis[:] = list(dy_vis)
+    return e
+
+
+def _route_dict(r) -> dict:
+    out = {}
+    for name, _ in r._fields_:
+        v = getattr(r, name)
+        out[name] = tuple(v) if not isinstance(v, int) else v
+    return out
+
+
+def conv3d_route(*args, ext: Optional[DiagExt] = None, **kw) -> dict:
+    """the kernel route b200unet_conv3d takes for these conv3d arguments (host-only query; RuntimeError if it refuses them).
+    ``kind`` is one of CONV_KINDS."""
+    d, keep = conv_desc(*args, **kw)
+    r = ConvRoute()
+    check(load_library().b200unet_diag_conv3d_route(C.byref(d), C.byref(ext) if ext is not None else None, C.byref(r)),
+          "diag_conv3d_route")
+    out = _route_dict(r)
+    out["kind"] = CONV_KINDS[r.kind]
+    return out
+
+
+def conv3d_ex(*args, ext: Optional[DiagExt] = None, **kw) -> None:
+    """conv3d with the options only the plans set (bias, zero_last, visible source extents)"""
+    d, keep = conv_desc(*args, **kw)
+    check(load_library().b200unet_diag_conv3d_ex(C.byref(d), C.byref(ext) if ext is not None else None, stream_ptr()),
+          "diag_conv3d_ex")
+
+
+def wgrad_route(a: Act, dy: Act, ksz: int, stride: int, cip: int, cop: int, *, deterministic: bool = False, num_sms: int = 132,
+                ext: Optional[DiagExt] = None) -> dict:
+    """the kernel route of a weight gradient on a device with num_sms SMs (host-only query).  ``kind`` is one of WGRAD_KINDS."""
+    r = WgradRoute()
+    check(load_library().b200unet_diag_wgrad_route(C.byref(a.ct()), C.byref(dy.ct()), ksz, stride, cip, cop,
+                                                   C.byref(ext) if ext is not None else None, int(bool(deterministic)), num_sms,
+                                                   C.byref(r)), "diag_wgrad_route")
+    out = _route_dict(r)
+    out["kind"] = WGRAD_KINDS[r.kind]
+    return out
+
+
+def wgrad_partial_bytes(a: Act, dy: Act, ksz: int, stride: int, cip: int, cop: int, num_sms: int = 132,
+                        ext: Optional[DiagExt] = None) -> int:
+    return int(load_library().b200unet_diag_wgrad_partial_bytes(C.byref(a.ct()), C.byref(dy.ct()), ksz, stride, cip, cop,
+                                                                C.byref(ext) if ext is not None else None, num_sms))
+
+
+def wgrad_ex(a: Act, dy: Act, ksz: int, stride: int, cip: int, cop: int, dw: torch.Tensor, *, part: Optional[torch.Tensor] = None,
+             part_bytes: Optional[int] = None, ext: Optional[DiagExt] = None) -> int:
+    """the weight gradient as the plans run it: atomics into dw (part None), or the deterministic partial sums in part
+    followed by their fixed-order reduction into dw.  Returns the number of partial slots written (0 with atomics)."""
+    splits = C.c_int(0)
+    nbytes = (part.numel() * part.element_size() if part is not None else 0) if part_bytes is None else part_bytes
+    check(load_library().b200unet_diag_wgrad_ex(C.byref(a.ct()), C.byref(dy.ct()), ksz, stride, cip, cop,
+                                                C.byref(ext) if ext is not None else None, _p(part), nbytes, C.byref(splits),
+                                                dw.data_ptr(), stream_ptr()), "diag_wgrad_ex")
+    return splits.value
+
+
+def bias_grad(dy: Act, dbias: torch.Tensor, ext: Optional[DiagExt] = None) -> None:
+    """dbias = sum of dy over its visible voxels (ext.dy_vis)"""
+    check(load_library().b200unet_diag_bias_grad(C.byref(dy.ct()), C.byref(ext) if ext is not None else None, dbias.data_ptr(),
+                                                 stream_ptr()), "diag_bias_grad")
 
 
 def conv3d_wgrad(a: Act, dy: Act, ksz: int, stride: int, cip: int, cop: int, dw: torch.Tensor) -> None:

@@ -31,6 +31,16 @@ def test_library_exports_exactly_the_declared_symbols(pkg):
     assert lib.b200unet_last_error() is not None
 
 
+def test_library_exports_the_diagnostics_header(pkg):
+    """include/b200unet_diag.h is bound by lib._DIAG_SIGS, outside the product surface"""
+    pkg.lib.load_library()
+    declared = _declared_symbols("b200unet_diag.h")
+    raw = C.CDLL(pkg.lib.LIB_PATH)
+    assert declared and all(hasattr(raw, name) for name in declared)
+    assert set(pkg.lib._DIAG_SIGS) == set(declared)
+    assert not set(declared) & set(pkg.lib.EXPORTED_SYMBOLS)
+
+
 def test_library_is_sm90a_wgmma(pkg):
     """The shipped binary must contain Hopper warpgroup-MMA + TMA SASS."""
     import shutil

@@ -35,13 +35,18 @@ def _packed_to_torch(L, w, mode, split, cout, cin, ksz):
     return hi, lo, cop, cip, q.double().cpu()[:, :cout, :cin].reshape(ksz, ksz, ksz, cout, cin).permute(3, 4, 0, 1, 2)
 
 
+# the forward shapes below that run on the halo kernel in bf16; (64, 32) has KC = 64 with BN = 32 and stays on per-tap tiles
+# (halo_keeps_occupancy), inputs wider than 64 channels unless B200UNET_HALO_WIDE_MIN allows them
+HALO_FORWARD = {(32, 32, (8, 16, 16)), (8, 32, (16, 16, 16)), (24, 40, (6, 18, 12)), (32, 64, (5, 24, 20)), (16, 16, (1, 16, 8))}
+
+
 @pytest.mark.parametrize("split", [False, True])
 @pytest.mark.parametrize("cin,cout,dims,ksz,stride", [
     (64, 64, (8, 8, 8), 3, 1), (32, 32, (8, 8, 16), 3, 1), (8, 32, (8, 8, 8), 3, 1), (128, 128, (4, 8, 8), 3, 1),
     (256, 256, (4, 4, 8), 3, 1), (24, 40, (5, 7, 9), 3, 1), (96, 192, (4, 4, 8), 3, 1), (64, 32, (8, 8, 8), 3, 1),
     (256, 128, (4, 4, 8), 1, 1), (8, 32, (6, 6, 6), 1, 1), (32, 32, (16, 16, 16), 3, 2), (64, 64, (8, 8, 8), 3, 2),
     (16, 16, (10, 6, 14), 3, 2),
-    # output plane >= 8 x 16 -> halo mode of igemm_conv.cu in bf16 (split precision and smaller planes: per-tap tiles)
+    # output plane >= 8 x 16: the halo kernel in bf16 where HALO_FORWARD lists it (the route is asserted)
     (32, 32, (8, 16, 16), 3, 1), (64, 32, (4, 16, 8), 3, 1), (8, 32, (16, 16, 16), 3, 1), (128, 128, (8, 16, 8), 3, 1),
     (256, 256, (2, 16, 8), 3, 1), (24, 40, (6, 18, 12), 3, 1), (96, 192, (3, 16, 8), 3, 1), (32, 64, (5, 24, 20), 3, 1),
     (16, 16, (1, 16, 8), 3, 1),
@@ -59,6 +64,8 @@ def test_conv3d_forward(pkg, cin, cout, dims, ksz, stride, split):
     pad = ksz // 2
     od = [(s + 2 * pad - ksz) // stride + 1 for s in dims]
     y = L.Act.empty(n, *od, cop, split=split, zero=True)
+    halo = not split and (cin, cout, dims) in HALO_FORWARD
+    assert L.conv3d_route(a, whi, wlo, ksz, stride, y, cop, cip)["kind"] == ("halo" if halo else "tap")
     L.conv3d(a, whi, wlo, ksz, stride, y, cop, cip)
     ref = F.conv3d(a.to_ncdhw(cin).double().cpu(), wq, stride=stride, padding=pad)
     assert rel(y.to_ncdhw(cout), ref) < TOL_STORE[split]
@@ -86,6 +93,7 @@ def test_conv3d_wide_inputs_on_halo_kernel(pkg, monkeypatch, cin, cout, dims, mo
     y = L.Act.empty(n, *dims, cop, split=split, zero=True)
     stats = torch.zeros(n, cop, 2, dtype=torch.float64, device=DEV)
     ref = F.conv3d(a.to_ncdhw(cin).double().cpu(), wq, padding=1)
+    assert L.conv3d_route(a, whi, wlo, 3, 1, y, cop, cip)["kind"] == ("tap" if split else "halo")
     if mode == "res":
         assert cop == cout                                   # the shapes above need no channel padding
         r = L.Act.from_ncdhw(torch.randn(n, cout, *dims, device=DEV), split=split)
@@ -118,7 +126,9 @@ def test_conv3d_wide_inputs_on_halo_kernel_gn_backward_epilogue_on_fused_coeffic
     L.gn_apply(x, L.Act.empty(n, *dims, ci, split=split), _channel_stats(x), gamma, beta, ci, G, coef)
     bst = torch.zeros(n, ci, 2, dtype=torch.float64, device=DEV)
     dz = L.Act.empty(n, *dims, ci, split=split)
-    L.conv3d(dy, wdh, wdl, 3, 1, dz, ci, co, mode=1, gn_x=x, coef=coef, coef_ld=ci, bstats=bst)
+    mode1 = dict(mode=1, gn_x=x, coef=coef, coef_ld=ci, bstats=bst)
+    assert L.conv3d_route(dy, wdh, wdl, 3, 1, dz, ci, co, **mode1)["kind"] == ("tap" if split else "halo")
+    L.conv3d(dy, wdh, wdl, 3, 1, dz, ci, co, **mode1)
     xq = x.to_ncdhw(ci).double().cpu().requires_grad_(True)
     z = F.group_norm(xq, G, gamma.double().cpu(), beta.double().cpu(), 1e-5)
     z.retain_grad()
@@ -184,7 +194,7 @@ def test_conv3d_fused_epilogue_residual_dropout_stats_concat_slice(pkg, split):
     per-channel statistics the next GroupNorm consumes."""
     L = pkg.lib
     torch.manual_seed(1)
-    n, ci, co, D = 2, 32, 32, 16          # 16^3: halo mode in bf16
+    n, ci, co, D = 2, 32, 32, 16
     x = torch.randn(n, ci, D, D, D, device=DEV)
     w = torch.randn(co, ci, 3, 3, 3, device=DEV) / (ci * 27) ** 0.5
     r = torch.randn(n, co, D, D, D, device=DEV)
@@ -193,7 +203,9 @@ def test_conv3d_fused_epilogue_residual_dropout_stats_concat_slice(pkg, split):
     scale = ((torch.rand(n, co, device=DEV) > 0.3).float() * 1.25).contiguous()
     cat = L.Act.empty(n, D, D, D, 2 * co, split=split, zero=True)
     stats = torch.zeros(n, 2 * co, 2, dtype=torch.float64, device=DEV)
-    L.conv3d(a, whi, wlo, 3, 1, cat.slice(co, co), cop, cip, res=res, scale=scale, stats=stats[:, co:], stats_ld=2 * co)
+    epi = dict(res=res, scale=scale, stats=stats[:, co:], stats_ld=2 * co)
+    assert L.conv3d_route(a, whi, wlo, 3, 1, cat.slice(co, co), cop, cip, **epi)["kind"] == ("tap" if split else "halo")
+    L.conv3d(a, whi, wlo, 3, 1, cat.slice(co, co), cop, cip, **epi)
     ref = (F.conv3d(a.to_ncdhw(ci).double().cpu(), wq, padding=1) + res.to_ncdhw(co).double().cpu()) * scale.double().cpu()[:, :, None, None, None]
     got = cat.slice(co, co).to_ncdhw(co)
     assert rel(got, ref) < TOL_STORE[split]
@@ -208,7 +220,7 @@ def test_conv3d_fused_epilogue_residual_dropout_stats_concat_slice(pkg, split):
 @pytest.mark.parametrize("D", [8, 16])
 def test_conv3d_two_sources_is_block_output(pkg, split, D):
     """conv2(a2) + sample(x): the residual block's second conv with the 1x1x1 `sample` as a second K-slab
-    (D=8: per-tap tiles, D=16: halo mode in bf16)."""
+    (D=8: per-tap tiles, D=16: the halo kernel in bf16)."""
     L = pkg.lib
     torch.manual_seed(2)
     n, ci, co = 1, 8, 32
@@ -220,6 +232,8 @@ def test_conv3d_two_sources_is_block_output(pkg, split, D):
     w2h, w2l, cop, cip, w2q = _packed_to_torch(L, w2, 0, split, co, co, 3)
     wsh, wsl, _, cips, wsq = _packed_to_torch(L, ws, 0, split, co, ci, 1)
     y = L.Act.empty(n, D, D, D, co, split=split)
+    route = L.conv3d_route(ah, w2h, w2l, 3, 1, y, cop, cip, x2=ax, w2_hi=wsh, w2_lo=wsl, cip2=cips)
+    assert route["kind"] == ("halo" if D == 16 and not split else "tap")
     L.conv3d(ah, w2h, w2l, 3, 1, y, cop, cip, x2=ax, w2_hi=wsh, w2_lo=wsl, cip2=cips)
     ref = F.conv3d(ah.to_ncdhw(co).double().cpu(), w2q, padding=1) + F.conv3d(ax.to_ncdhw(ci).double().cpu(), wsq)
     assert rel(y.to_ncdhw(co), ref) < TOL_STORE[split]
@@ -228,7 +242,9 @@ def test_conv3d_two_sources_is_block_output(pkg, split, D):
 @pytest.mark.parametrize("split", [False, True])
 @pytest.mark.parametrize("D", [8, 16])
 def test_conv3d_dgrad_groupnorm_relu_backward_epilogue_on_fused_coefficients(pkg, split, D):
-    """dz = dgrad(dy) masked by ReLU'(GN(x)), plus per-channel (sum dz, sum dz*xhat): checked against autograd."""
+    """dz = dgrad(dy) masked by ReLU'(GN(x)), plus per-channel (sum dz, sum dz*xhat): checked against autograd.  With K = 64 and
+    32 outputs both extents run on per-tap tiles (halo_keeps_occupancy); the mode-1 epilogue on the halo kernel is covered by the
+    halo mode-1 cases of tests/test_gpu_conv_routes.py."""
     L = pkg.lib
     torch.manual_seed(3)
     n, ci, co, G = 2, 32, 64, 8
@@ -243,7 +259,10 @@ def test_conv3d_dgrad_groupnorm_relu_backward_epilogue_on_fused_coefficients(pkg
     L.gn_apply(x, L.Act.empty(n, D, D, D, ci, split=split), _channel_stats(x), gamma, beta, ci, G, coef)
     bst = torch.zeros(n, ci, 2, dtype=torch.float64, device=DEV)
     dz = L.Act.empty(n, D, D, D, ci, split=split)
-    L.conv3d(dy, wdh, wdl, 3, 1, dz, ci, co, mode=1, gn_x=x, coef=coef, coef_ld=ci, bstats=bst)
+    mode1 = dict(mode=1, gn_x=x, coef=coef, coef_ld=ci, bstats=bst)
+    route = L.conv3d_route(dy, wdh, wdl, 3, 1, dz, ci, co, **mode1)
+    assert (route["kind"], route["bn"], route["kc"]) == ("tap", 32, 64)
+    L.conv3d(dy, wdh, wdl, 3, 1, dz, ci, co, **mode1)
     xq = x.to_ncdhw(ci).double().cpu().requires_grad_(True)
     z = F.group_norm(xq, G, gamma.double().cpu(), beta.double().cpu(), 1e-5)
     z.retain_grad()
@@ -288,7 +307,7 @@ def test_stride2_data_gradient_by_parity_classes(pkg, ci, co, odims, with_res, s
     (8, 32, (8, 8, 16), 3, 1), (16, 16, (8, 8, 8), 3, 1), (64, 32, (8, 8, 8), 3, 1), (24, 40, (5, 7, 9), 3, 1),
     (96, 192, (4, 4, 8), 3, 1), (256, 128, (4, 4, 8), 1, 1), (8, 32, (8, 8, 8), 1, 1), (32, 32, (16, 16, 16), 3, 2),
     (64, 64, (8, 8, 8), 3, 2),
-    # 33..64 input channels with an output plane >= 8 x 16 -> halo mode of wgrad.cu in bf16
+    # 33..64 input channels with an output plane >= 8 x 16: the halo kernel of wgrad.cu in bf16 (the route is asserted)
     (64, 64, (4, 16, 8), 3, 1), (48, 32, (3, 18, 12), 3, 1), (40, 128, (2, 16, 16), 3, 1),
 ])
 def test_conv3d_weight_gradient(pkg, ci, co, dims, ksz, stride, split):
@@ -301,6 +320,8 @@ def test_conv3d_weight_gradient(pkg, ci, co, dims, ksz, stride, split):
     dy = L.Act.from_ncdhw(torch.randn(n, co, *od, device=DEV), split=split)
     cip, cop, T = (ci + 7) // 8 * 8, (co + 7) // 8 * 8, ksz ** 3
     dw = torch.zeros(T, cip, cop, device=DEV)
+    halo = not split and ksz == 3 and stride == 1 and 32 < ci <= 64 and od[1] >= 16 and od[2] >= 8
+    assert L.wgrad_route(a, dy, ksz, stride, cip, cop)["kind"] == ("halo" if halo else "simt" if ksz == 1 and ci <= 16 else "tap")
     L.conv3d_wgrad(a, dy, ksz, stride, cip, cop, dw)
     out = torch.empty(co, ci, ksz, ksz, ksz, device=DEV)
     L.check(L.load_library().b200unet_unpack_wgrad(dw.data_ptr(), co, ci, cop, cip, T, 0, out.data_ptr(), L.stream_ptr()))
