@@ -56,6 +56,7 @@ static int to_conv_op(const b200unet_conv_desc* d, const b200unet_diag_ext* ext,
   if (ext) {
     op.bias = ext->bias;
     op.zero_last = ext->zero_last;
+    op.max_ctas = ext->max_ctas;
     for (int s = 0; s < d->nsrc; ++s) {
       op.src[s].x.vD = ext->x_vis[s][0]; op.src[s].x.vH = ext->x_vis[s][1]; op.src[s].x.vW = ext->x_vis[s][2];
     }
@@ -260,7 +261,7 @@ int b200unet_diag_conv3d_route(const b200unet_conv_desc* desc, const b200unet_di
   ConvOpHolder h;
   B200_TRY(to_conv_op(desc, ext, &h));
   ConvRoute r;
-  B200_TRY(conv_route(h.op, &r));
+  B200_TRY(conv_route(h.op, device_sms(), &r));
   route->kind = r.kind; route->bn = r.BN; route->kc = r.KC;
   route->kchunks[0] = r.kchunks[0]; route->kchunks[1] = r.kchunks[1];
   route->npass = r.npass; route->cls_pair = r.cls_pair;

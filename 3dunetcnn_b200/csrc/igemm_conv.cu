@@ -19,6 +19,7 @@
 //   mode 1: GroupNorm/ReLU backward: dz = dact * 1[A x + B > 0], per-channel (sum dz, sum dz*xhat).
 // Split-precision ("parity") mode runs three passes per K step: Ah*Wh, Al*Wh, Ah*Wl.
 #include <cstdlib>
+#include <type_traits>
 #include "conv_common.cuh"
 
 namespace b200 {
@@ -26,7 +27,9 @@ namespace b200 {
 // Kernel modes: per-tap streaming tiles, class mode (parity-class data gradient / k = s = 2 transposed convolution), and halo
 // mode: the 3x3x3 stride-1 source is loaded as ONE halo box (KC, 10, 18, 3) per K chunk for an 8 x 16 x 1 output tile, and the
 // 27 taps read it through shifted shared-memory descriptors (27x less activation traffic from L2 than per-tap boxes).
-enum ConvMode { CONV_STREAM = 0, CONV_CLASS = 1, CONV_HALO = 2 };
+// CONV_HALO_WS is halo mode on the persistent, weight-stationary kernel (k_igemm_conv_halo_ws) for the (BN, KC) whose 27 weight
+// tiles fit in shared memory beside the halo box; CONV_HALO runs the ring kernel below for the wider ones.
+enum ConvMode { CONV_STREAM = 0, CONV_CLASS = 1, CONV_HALO = 2, CONV_HALO_WS = 3 };
 
 // Shared memory: STAGES-deep TMA ring | fp32 accumulator tile [128][BN + 4] | (class mode) output staging | (halo mode) halo box
 // | aux.  Outside class mode the output staging tile reuses the ring: the CTA computes one tile, so every stage has been consumed
@@ -311,6 +314,230 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
   if (threadIdx.x == 0) tma_store_wait_all();   // the staging tile must outlive the bulk store
 }
 
+// Persistent, weight-stationary halo mode.  With one CTA per 8 x 16 x 1 tile, every CTA fetched all 27 weight tiles through the
+// ring for 27 short MMA batches, then drained and ran its epilogue with nothing queued behind it.  Here a CTA loads the 27 weight
+// tiles of its N tile once, behind one mbarrier, and walks the voxel tiles blockIdx.x, blockIdx.x + gridDim.x, ...  Per tile only
+// the halo box is loaded (into one of HALO_BUFS buffers, so that the next box loads while this tile's epilogue runs), the 27 taps
+// are one run of wgmmas with one commit, and a fused 1x1x1 second source streams its A and weight tiles through a two-stage
+// ring, one stage per K chunk.  The MMA order of every output row is that of the ring kernel: taps 0..26, k16 steps inside each,
+// then the second-source chunks.
+// Shared memory: resident weights [27][BN][KC] | region R | HALO_BUFS halo boxes | aux.  R holds, one after the other within a
+// tile, the second-source ring, the fp32 accumulator tile and the bf16 output staging tile: each thread copies its accumulator row
+// into registers before the staging tile overwrites it, and the producer refills the ring only once the previous tile's TMA store
+// has read the staging tile (r_free).  That is what lets BN 32 / KC 32 keep two CTAs per SM.
+template <int BN, int KC>
+struct HaloWsCfg {
+  static constexpr int A_BYTES = 128 * KC * 2;
+  static constexpr int B_BOX_BYTES = BN * KC * 2;
+  static constexpr int B_BYTES = B_BOX_BYTES < 1024 ? 1024 : B_BOX_BYTES;
+  static constexpr int STAGES = 2;                          // second-source ring
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int ACC_LD = BN + 4;
+  static constexpr int ACC_BYTES = 128 * ACC_LD * 4;        // > the 128 x BN bf16 staging tile
+  static constexpr int W_BYTES = (27 * B_BOX_BYTES + 1023) / 1024 * 1024;
+  static constexpr int R_RAW = STAGES * STAGE_BYTES > ACC_BYTES ? STAGES * STAGE_BYTES : ACC_BYTES;
+  static constexpr int R_BYTES = (R_RAW + 1023) / 1024 * 1024;
+  static constexpr int RB = KC * 2;
+  static constexpr int HALO_TX = 540 * RB;
+  static constexpr int HALO_BYTES = (HALO_TX + 1023) / 1024 * 1024;
+  static constexpr int AUX_BYTES = 1024 + 4 * BN * 2 * 4 + BN * 16;   // barriers | per-warp stats | coef
+  static constexpr int FIXED = W_BYTES + R_BYTES + AUX_BYTES + 1024;  // +1024 alignment slack
+  static constexpr int BLOCKS_PER_SM = BN <= 32 ? 2 : 1;
+  static constexpr int BUDGET = BLOCKS_PER_SM == 2 ? ConvCfg<BN, KC, CONV_STREAM>::TWO_PER_SM : ConvCfg<BN, KC, CONV_STREAM>::SMEM_LIMIT;
+  static constexpr int HALO_BUFS = FIXED + 2 * HALO_BYTES <= BUDGET ? 2 : 1;
+  static constexpr int SMEM_BYTES = FIXED + HALO_BUFS * HALO_BYTES;
+  // BN <= 64: the accumulator row a thread holds in registers during the epilogue stays at <= 64 floats
+  static constexpr bool FITS = BN <= 64 && SMEM_BYTES <= BUDGET;
+  static constexpr uint32_t LAYOUT = swizzle_for_row_bytes(KC * 2);
+  static constexpr uint32_t SBO = 8 * KC * 2;
+};
+
+template <int BN, int KC>
+__global__ void __launch_bounds__(160, (HaloWsCfg<BN, KC>::BLOCKS_PER_SM)) k_igemm_conv_halo_ws(const __grid_constant__ ConvMaps maps,
+                                                                                              const ConvArgs p) {
+  using Cfg = HaloWsCfg<BN, KC>;
+  static_assert(Cfg::FITS, "igemm_conv: weight-stationary halo configuration does not fit shared memory");
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* wts = smem;
+  uint8_t* reg = smem + Cfg::W_BYTES;
+  uint8_t* halo = reg + Cfg::R_BYTES;
+  uint8_t* aux = halo + Cfg::HALO_BUFS * Cfg::HALO_BYTES;
+  uint64_t* w_full = reinterpret_cast<uint64_t*>(aux);
+  uint64_t* halo_full = w_full + 1;               // [HALO_BUFS]
+  uint64_t* halo_empty = halo_full + 2;           // [HALO_BUFS]
+  uint64_t* full_bar = halo_empty + 2;            // [STAGES]
+  uint64_t* empty_bar = full_bar + Cfg::STAGES;   // [STAGES]
+  uint64_t* r_free = empty_bar + Cfg::STAGES;
+  float* s_stats = reinterpret_cast<float*>(aux + 1024);             // [4 warps][BN][2]
+  float4* s_coef = reinterpret_cast<float4*>(aux + 1024 + 4 * BN * 8);   // [BN]
+  float* s_acc = reinterpret_cast<float*>(reg);
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int ntiles = p.N * p.tiles_d * p.tiles_h * p.tiles_w;
+  const int n0 = blockIdx.y * BN;
+  auto tile_origin = [&](int t, int& w0, int& h0, int& d0, int& n) {
+    w0 = (t % p.tiles_w) * 8; t /= p.tiles_w;
+    h0 = (t % p.tiles_h) * 16; t /= p.tiles_h;
+    d0 = t % p.tiles_d;
+    n = t / p.tiles_d;
+  };
+
+  if (warp == 4 && lane == 0) {
+    tma_prefetch_desc(&maps.a[0][0]);
+    tma_prefetch_desc(&maps.b[0][0]);
+    mbar_init(w_full, 1);
+    for (int b = 0; b < Cfg::HALO_BUFS; ++b) { mbar_init(&halo_full[b], 1); mbar_init(&halo_empty[b], 4); }
+    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 4); }
+    mbar_init(r_free, 1);
+    fence_barrier_init();
+  }
+  pdl_wait();   // before the first global read; the barrier set-up above overlaps the previous kernel
+  if (warp < 4)
+    for (int i = threadIdx.x; i < 4 * BN * 2; i += 128) s_stats[i] = 0.f;
+  __syncthreads();
+  pdl_launch_dependents();
+
+  if (warp == 4) {
+    // ------------------------------------------------------------------ TMA producer (convergent, one lane issues)
+    const uint32_t issue = elect_one() ? 1u : 0u;
+    mbar_expect_tx_if(issue, w_full, 27 * Cfg::B_BOX_BYTES);
+    for (int tap = 0; tap < 27; ++tap) tma_load_3d_if(issue, wts + tap * Cfg::B_BOX_BYTES, &maps.b[0][0], w_full, 0, n0, tap);
+    int it = 0, j = 0;
+    for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++j) {
+      int w0, h0, d0, n;
+      tile_origin(t, w0, h0, d0, n);
+      const int hb = j % Cfg::HALO_BUFS;
+      mbar_wait(&halo_empty[hb], ((j / Cfg::HALO_BUFS) & 1) ^ 1);
+      mbar_expect_tx_if(issue, &halo_full[hb], Cfg::HALO_TX);
+      tma_load_5d_if(issue, halo + hb * Cfg::HALO_BYTES, &maps.a[0][0], &halo_full[hb], 0, w0 - 1, h0 - 1, d0 - 1, n);
+      if (p.ntaps[1] == 0) continue;
+      mbar_wait(r_free, (j & 1) ^ 1);   // the previous tile's store has read R
+      for (int kc = 0; kc < p.kchunks[1]; ++kc, ++it) {
+        const int s = it % Cfg::STAGES;
+        mbar_wait(&empty_bar[s], ((it / Cfg::STAGES) & 1) ^ 1);
+        mbar_expect_tx_if(issue, &full_bar[s], Cfg::A_BYTES + Cfg::B_BOX_BYTES);
+        uint8_t* sa = reg + s * Cfg::STAGE_BYTES;
+        tma_load_5d_if(issue, sa, &maps.a[1][0], &full_bar[s], kc * KC, w0, h0, d0, n);
+        tma_load_3d_if(issue, sa + Cfg::A_BYTES, &maps.b[1][0], &full_bar[s], kc * KC, n0, 0);
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumer warpgroup: wgmma, then the epilogue
+  constexpr uint32_t hi_d = desc_hi(Cfg::SBO, Cfg::LAYOUT);
+  constexpr uint32_t hi_halo = desc_hi(10 * Cfg::RB, Cfg::LAYOUT);   // see k_igemm_conv: 8-row groups are 10 halo rows apart
+  constexpr uint32_t HALF_M = (64 * KC * 2) >> 4;                    // ring A tile: row 64
+  constexpr uint32_t HALO_HALF = (80 * Cfg::RB) >> 4;                // halo: output rows 64-127 = h 8..15
+  const uint32_t w_lo0 = desc_lo(smem_u32(wts), 16);
+  const uint32_t halo_lo0 = desc_lo(smem_u32(halo), 16);
+  const uint32_t reg0 = smem_u32(reg);
+  const int row = threadIdx.x;
+  const int wl = row % 8, hl = row / 8;
+  const bool want_stats = (p.mode == 0) ? (p.stats != nullptr) : (p.bstats != nullptr);
+  double* stats_dst = (p.mode == 0) ? p.stats : p.bstats;
+  const int stats_ld = (p.mode == 0) ? p.stats_ld : p.coef_ld;
+  int it = 0, j = 0, coef_n = -1;
+  mbar_wait(w_full, 0);
+  for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++j) {
+    int w0, h0, d0, n;
+    tile_origin(t, w0, h0, d0, n);
+    const int w = w0 + wl, h = h0 + hl, d = d0;
+    const bool valid = (w < p.Wo) && (h < p.Ho) && (d < p.Do);
+    const bool edge = p.zero_last && (w == p.Wo - 1 || h == p.Ho - 1 || d == p.Do - 1);
+    const long long vox = (((long long)n * p.Do + d) * p.Ho + h) * p.Wo + w;
+    conv_epilogue_prefetch(p, n0, BN, vox, valid);   // -> L2 while the MMAs run
+
+    const int hb = j % Cfg::HALO_BUFS;
+    const uint32_t hlo = halo_lo0 + ((hb * Cfg::HALO_BYTES) >> 4);
+    float acc[2][BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+    mbar_wait(&halo_full[hb], (j / Cfg::HALO_BUFS) & 1);
+    wgmma_fence();
+#pragma unroll
+    for (int tap = 0; tap < 27; ++tap) {
+      const int kd = tap / 9, kh = (tap / 3) % 3, kw = tap % 3;
+      const uint32_t a_lo = hlo + (((kd * 180 + kh * 10 + kw) * Cfg::RB) >> 4);
+      const uint32_t b_lo = w_lo0 + ((tap * Cfg::B_BOX_BYTES) >> 4);
+#pragma unroll
+      for (int k = 0; k < KC / 16; ++k) {
+        const uint32_t accumulate = (tap > 0 || k > 0) ? 1u : 0u;
+        Wgmma<BN>::template mma<0, 0>(acc[0], desc_from(a_lo + 2 * k, hi_halo), desc_from(b_lo + 2 * k, hi_d), accumulate);
+        Wgmma<BN>::template mma<0, 0>(acc[1], desc_from(a_lo + HALO_HALF + 2 * k, hi_halo), desc_from(b_lo + 2 * k, hi_d), accumulate);
+      }
+    }
+    wgmma_commit();
+    // while the taps run: once the previous tile's store has read R, the producer may refill it with this tile's ring stages
+    if (j > 0 && threadIdx.x == 0) {
+      tma_store_wait_read0();
+      mbar_arrive(r_free);
+    }
+    int prev = -1;   // ring slot whose MMAs may still be reading it (-1: the halo box)
+    for (int kc = 0; kc < p.kchunks[1]; ++kc, ++it) {
+      const int s = it % Cfg::STAGES;
+      mbar_wait(&full_bar[s], (it / Cfg::STAGES) & 1);
+      const uint32_t a_lo = desc_lo(reg0 + s * Cfg::STAGE_BYTES, 16);
+      const uint32_t b_lo = desc_lo(reg0 + s * Cfg::STAGE_BYTES + Cfg::A_BYTES, 16);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < KC / 16; ++k) {
+        Wgmma<BN>::template mma<0, 0>(acc[0], desc_from(a_lo + 2 * k, hi_d), desc_from(b_lo + 2 * k, hi_d), 1u);
+        Wgmma<BN>::template mma<0, 0>(acc[1], desc_from(a_lo + HALF_M + 2 * k, hi_d), desc_from(b_lo + 2 * k, hi_d), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();   // everything before this chunk has retired: hand back the halo box or the previous ring slot
+      if (lane == 0) mbar_arrive(prev < 0 ? &halo_empty[hb] : &empty_bar[prev]);
+      prev = s;
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc[0]);
+    wgmma_fence_regs(acc[1]);
+    if (lane == 0) mbar_arrive(prev < 0 ? &halo_empty[hb] : &empty_bar[prev]);
+
+    // every warp's MMAs have retired (the ring lived in R) and the previous store has read R
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    if (p.mode == 1 && n != coef_n) {   // the previous epilogue's reads of s_coef ended before its last barrier
+      for (int c = threadIdx.x; c < BN; c += 128)
+        s_coef[c] = (n0 + c < p.Cout) ? p.coef[(long long)n * p.coef_ld + n0 + c] : make_float4(0.f, 0.f, 0.f, 0.f);
+      coef_n = n;
+    }
+#pragma unroll
+    for (int hm = 0; hm < 2; ++hm) {
+      const int r0 = hm * 64 + warp * 16 + (lane >> 2);
+#pragma unroll
+      for (int jj = 0; jj < BN / 8; ++jj) {
+        const int c = jj * 8 + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(s_acc + r0 * Cfg::ACC_LD + c) = make_float2(acc[hm][4 * jj], acc[hm][4 * jj + 1]);
+        *reinterpret_cast<float2*>(s_acc + (r0 + 8) * Cfg::ACC_LD + c) = make_float2(acc[hm][4 * jj + 2], acc[hm][4 * jj + 3]);
+      }
+    }
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    float4 acc_row[BN / 4];
+#pragma unroll
+    for (int i = 0; i < BN / 4; ++i) acc_row[i] = reinterpret_cast<const float4*>(s_acc + row * Cfg::ACC_LD)[i];
+    asm volatile("bar.sync 1, 128;" ::: "memory");   // the staging tile below overwrites the accumulator tile
+    conv_epilogue_tile<BN>(p, reinterpret_cast<const float*>(acc_row), warp, lane, n, n0, vox, valid, s_stats, s_coef, want_stats,
+                           edge, reg, row, false);
+    fence_proxy_async();
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    if (threadIdx.x == 0) {
+      tma_store_5d(&maps.o[0], reg, n0, w0, h0, d0, n);
+      tma_store_commit();
+    }
+    if (want_stats) {   // this tile's fp32 partials -> one fp64 atomic per channel; the slots restart from zero
+      for (int c = threadIdx.x; c < BN * 2; c += 128) {
+        const float v = s_stats[c] + s_stats[BN * 2 + c] + s_stats[2 * BN * 2 + c] + s_stats[3 * BN * 2 + c];
+        s_stats[c] = 0.f; s_stats[BN * 2 + c] = 0.f; s_stats[2 * BN * 2 + c] = 0.f; s_stats[3 * BN * 2 + c] = 0.f;
+        if (n0 + (c >> 1) < p.Cout) atomicAdd(&stats_dst[((long long)n * stats_ld + n0) * 2 + c], (double)v);
+      }
+    }
+  }
+  if (threadIdx.x == 0) tma_store_wait_all();   // the staging tile must outlive the bulk store
+}
+
 // ----------------------------------------------------------------------------------------------- host side
 static void pick_tile(int Wo, int Ho, int Do, int& tw, int& th, int& td) {
   tw = Wo >= 8 ? 8 : Wo >= 4 ? 4 : Wo >= 2 ? 2 : 1;
@@ -320,18 +547,27 @@ static void pick_tile(int Wo, int Ho, int Do, int& tw, int& th, int& td) {
   td = rem / th;
 }
 
+// The compile-time configuration of the kernel a (BN, KC, MODE) launch runs.
+template <int BN, int KC, int MODE>
+using ConvCfgOf = std::conditional_t<MODE == CONV_HALO_WS, HaloWsCfg<BN, KC>, ConvCfg<BN, KC, MODE>>;
+
 template <int BN, int KC, int MODE>
 static int launch_cfg(const ConvMaps& maps, const ConvArgs& args, dim3 grid, cudaStream_t st, const ConvClassMaps& cmaps) {
-  using Cfg = ConvCfg<BN, KC, MODE>;
+  using Cfg = ConvCfgOf<BN, KC, MODE>;
   static bool attr_set[64] = {false};
   int dev = 0;
   B200_CHECK_CUDA(cudaGetDevice(&dev));
   if (dev < 64 && !attr_set[dev]) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(k_igemm_conv<BN, KC, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES));
+    if constexpr (MODE == CONV_HALO_WS)
+      B200_CHECK_CUDA(cudaFuncSetAttribute(k_igemm_conv_halo_ws<BN, KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    else
+      B200_CHECK_CUDA(cudaFuncSetAttribute(k_igemm_conv<BN, KC, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_set[dev] = true;
   }
-  launch_pdl(k_igemm_conv<BN, KC, MODE>, grid, dim3(160), Cfg::SMEM_BYTES, st, maps, args, cmaps);
+  if constexpr (MODE == CONV_HALO_WS)
+    launch_pdl(k_igemm_conv_halo_ws<BN, KC>, grid, dim3(160), Cfg::SMEM_BYTES, st, maps, args);
+  else
+    launch_pdl(k_igemm_conv<BN, KC, MODE>, grid, dim3(160), Cfg::SMEM_BYTES, st, maps, args, cmaps);
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;
 }
@@ -358,13 +594,20 @@ static int conv_bn(const ConvOp& op) {
   return op.cls_mode && BN > 64 ? 64 : BN;   // class mode keeps its staging tile beside the accumulator tile (ConvCfg)
 }
 
+// Halo mode runs on the weight-stationary kernel wherever its configuration fits (BN <= 64 with KC <= 32; the 27 weight tiles
+// of KC = 64 or BN = 128 with KC = 32 take 221 KB), and on the ring kernel otherwise.
+template <int BN, int KC>
+constexpr int halo_mode() {
+  return HaloWsCfg<BN, KC>::FITS ? CONV_HALO_WS : CONV_HALO;
+}
+
 // Halo mode must not cost a configuration the second CTA per SM that per-tap tiles give it.  With KC = 64 and BN <= 32 the
 // halo box leaves room for fewer than four ring stages in half of the SM's shared memory; at one CTA per SM the 64 -> 32
 // channel convolutions of the C2 step (forward at 128^3, data gradient at 64^3) took 1.4x as long as on per-tap tiles at
 // two (H100 80GB HBM3, 400 W).  With a single K chunk per source the two modes accumulate in the same order.
 template <int BN, int KC>
 constexpr bool halo_keeps_occupancy() {
-  return ConvCfg<BN, KC, CONV_HALO>::BLOCKS_PER_SM >= ConvCfg<BN, KC, CONV_STREAM>::BLOCKS_PER_SM;
+  return ConvCfgOf<BN, KC, halo_mode<BN, KC>()>::BLOCKS_PER_SM >= ConvCfg<BN, KC, CONV_STREAM>::BLOCKS_PER_SM;
 }
 
 static bool halo_keeps_occupancy(int BN, int KC) {
@@ -406,7 +649,7 @@ static int with_conv_kernel(int kind, int BN, int KC, F&& f) {
     if (kind == CONV_KIND_CLASS1 || kind == CONV_KIND_CLASS2) {                                             \
       if constexpr (bn <= 64) return f(ConvKernel<bn, kc, CONV_CLASS>{});                                   \
     } else if (kind == CONV_KIND_HALO) {                                                                    \
-      if constexpr (halo_keeps_occupancy<bn, kc>()) return f(ConvKernel<bn, kc, CONV_HALO>{});              \
+      if constexpr (halo_keeps_occupancy<bn, kc>()) return f(ConvKernel<bn, kc, halo_mode<bn, kc>()>{});    \
     } else {                                                                                                \
       return f(ConvKernel<bn, kc, CONV_STREAM>{});                                                          \
     }                                                                                                       \
@@ -417,8 +660,9 @@ static int with_conv_kernel(int kind, int BN, int KC, F&& f) {
   return E_UNSUPPORTED;
 }
 
-int conv_route(const ConvOp& op, ConvRoute* r) {
+int conv_route(const ConvOp& op, int num_sms, ConvRoute* r) {
   memset(r, 0, sizeof(*r));
+  B200_REQUIRE(num_sms >= 1 && op.max_ctas >= 0, E_INVALID, "igemm_conv: num_sms=%d max_ctas=%d", num_sms, op.max_ctas);
   B200_REQUIRE(op.nsrc == 1 || op.nsrc == 2, E_INVALID, "igemm_conv: nsrc=%d", op.nsrc);
   B200_REQUIRE(op.cls_mode >= 0 && op.cls_mode <= 2, E_INVALID, "igemm_conv: cls_mode=%d", op.cls_mode);
   const Act& out = op.out;
@@ -458,7 +702,7 @@ int conv_route(const ConvOp& op, ConvRoute* r) {
   }
   const bool halo = conv_halo_eligible(op);
   r->kind = op.cls_mode == 1 ? CONV_KIND_CLASS1 : op.cls_mode == 2 ? CONV_KIND_CLASS2 : halo ? CONV_KIND_HALO : CONV_KIND_TAP;
-  if (halo) {   // one 8 x 16 output plane tile per CTA
+  if (halo) {   // 8 x 16 output plane tiles
     r->tw = 8; r->th = 16; r->td = 1;
   } else {
     pick_tile(gW, gH, gD, r->tw, r->th, r->td);
@@ -472,16 +716,23 @@ int conv_route(const ConvOp& op, ConvRoute* r) {
   r->grid[0] = (int)((long long)out.N * r->tiles_d * r->tiles_h * r->tiles_w);
   r->grid[1] = ceil_div(out.C, r->BN);
   r->grid[2] = 1;
-  return with_conv_kernel(r->kind, r->BN, r->KC, [r](auto k) {
-    using Cfg = ConvCfg<decltype(k)::BN, decltype(k)::KC, decltype(k)::MODE>;
+  return with_conv_kernel(r->kind, r->BN, r->KC, [&](auto k) {
+    using Cfg = ConvCfgOf<decltype(k)::BN, decltype(k)::KC, decltype(k)::MODE>;
     r->stages = Cfg::STAGES; r->blocks_per_sm = Cfg::BLOCKS_PER_SM; r->smem_bytes = Cfg::SMEM_BYTES;
+    if constexpr (decltype(k)::MODE == CONV_HALO_WS) {
+      // persistent CTAs: one wave (max_ctas, a diagnostics cap, makes small shapes walk several tiles per CTA)
+      int cap = Cfg::BLOCKS_PER_SM * num_sms / r->grid[1];
+      if (cap < 1) cap = 1;
+      if (op.max_ctas > 0 && op.max_ctas < cap) cap = op.max_ctas;
+      if (r->grid[0] > cap) r->grid[0] = cap;
+    }
     return (int)OK;
   });
 }
 
 int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
   ConvRoute r;
-  B200_TRY(conv_route(op, &r));
+  B200_TRY(conv_route(op, device_sms(), &r));
   const Act& out = op.out;
   const bool split = r.npass == 3, halo = r.kind == CONV_KIND_HALO, cls = op.cls_mode != 0;
   ConvArgs a;

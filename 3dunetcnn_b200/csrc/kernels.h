@@ -140,6 +140,7 @@ struct ConvOp {
   double* bstats;      // mode 1: [N][coef_ld][2] += (sum dz, sum dz*xhat)
   const float* bias;   // mode 0: optional per-channel bias
   int zero_last;       // mode 0: output voxels on the high boundary of each axis are forced to 0
+  int max_ctas;        // > 0: at most this many CTAs per N tile on the persistent halo kernel (diagnostics: several tiles per CTA)
   int cls_mode;        // 2: ConvTranspose3d(kernel = stride = 2) forward: src[0].x = input at half the output extent, src[0].w = the
                        // mode-4 pack [8][Cop][Cip]; class p = one tap.  1: data gradient of a 3x3x3 stride-2 padding-1 convolution WITHOUT zero insertion: src[0].x = dY (low
                        // resolution), src[0].w = the flipped data-gradient pack, out = dX at twice the extent; eight
@@ -159,8 +160,10 @@ struct ConvRoute {
   int grid[3];
   int stages, blocks_per_sm, smem_bytes;   // ConvCfg of the instantiation
 };
-int conv_route(const ConvOp& op, ConvRoute* r);   // validates the op: OK or the error launch_igemm_conv would return
+// on a device with num_sms SMs; validates the op: OK or the error launch_igemm_conv would return
+int conv_route(const ConvOp& op, int num_sms, ConvRoute* r);
 int launch_igemm_conv(const ConvOp& op, cudaStream_t st);
+int device_sms();   // SMs of the current device; 132 (an H100 SXM) without one
 bool conv_halo_eligible(const ConvOp& op);   // shape-only: does this convolution run in halo mode?
 
 // ---- tensor-core weight gradient (wgrad.cu):  dW[t][ci][co] += sum_v dy[v][co] * a[v*stride + t - pad][ci]

@@ -437,20 +437,12 @@ static void emit_conv_fwd(Plan& P, int ci, TRef a, int ci2, TRef a2, TRef res, T
 }
 
 // ---- backward op emitters
-static int plan_num_sms() {
-  int dev = 0, sms = 0;
-  if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && sms > 0)
-    return sms;
-  cudaGetLastError();   // planning on a host without a GPU: assume an H100 SXM
-  return 132;
-}
-
 static void size_wgrad_partials(Plan& P, const Act& a, const Act& dy, int ksz, int stride, int nopad, int Cip, int Cop) {
   if (!P.deterministic) return;
   WgradOp op;
   memset(&op, 0, sizeof(op));
   op.a = a; op.dy = dy; op.ksz = ksz; op.stride = stride; op.nopad = nopad; op.Cip = Cip; op.Cop = Cop;
-  const size_t need = wgrad_partial_bytes(op, plan_num_sms());
+  const size_t need = wgrad_partial_bytes(op, device_sms());
   if (need > P.wg_part_bytes) P.wg_part_bytes = need;
 }
 

@@ -356,11 +356,12 @@ int launch_wgrad_reduce(const float* part, int splits, long long elems, float* d
   return OK;
 }
 
-static int device_sms() {
+int device_sms() {
   int dev = 0, sms = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-    return 132;
-  return sms;
+  if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && sms > 0)
+    return sms;
+  cudaGetLastError();   // a host without a GPU (route queries, planning)
+  return 132;
 }
 
 size_t wgrad_partial_bytes(const WgradOp& op, int num_sms) {

@@ -38,7 +38,7 @@ class ConvDesc(C.Structure):
 class DiagExt(C.Structure):
     """``b200unet_diag_ext``: bias, zeroed high boundary and visible extents (include/b200unet_diag.h)."""
     _fields_ = [("bias", C.c_void_p), ("zero_last", C.c_int32), ("x_vis", (C.c_int32 * 3) * 2), ("a_vis", C.c_int32 * 3),
-                ("dy_vis", C.c_int32 * 3)]
+                ("dy_vis", C.c_int32 * 3), ("max_ctas", C.c_int32)]
 
 
 class ConvRoute(C.Structure):
@@ -330,9 +330,12 @@ def conv_desc(x: Act, w_hi, w_lo, ksz: int, stride: int, out: Act, cop: int, cip
     return d, keep
 
 
-def diag_ext(bias: Optional[torch.Tensor] = None, zero_last: bool = False, x_vis=None, a_vis=None, dy_vis=None) -> DiagExt:
-    """``b200unet_diag_ext``; each *_vis is a (d, h, w) triple (x_vis: one per source), 0 = the full extent"""
+def diag_ext(bias: Optional[torch.Tensor] = None, zero_last: bool = False, x_vis=None, a_vis=None, dy_vis=None,
+             max_ctas: int = 0) -> DiagExt:
+    """``b200unet_diag_ext``; each *_vis is a (d, h, w) triple (x_vis: one per source), 0 = the full extent; max_ctas > 0 caps
+    the CTAs per N tile of the persistent halo kernel"""
     e = DiagExt()
+    e.max_ctas = max_ctas
     e.bias = _p(bias)
     e.zero_last = int(bool(zero_last))
     for s, v in enumerate(x_vis or ()):

@@ -2,8 +2,9 @@
  *
  * They report which kernel a convolution or weight gradient runs on, and launch the operation with the options that only
  * the whole-network plans set otherwise (bias, zeroed boundary, visible extents, deterministic weight-gradient partial sums),
- * so that tests can hold every kernel route to a reference.  The route queries are host-only: they touch neither the device
- * nor the driver, and read the tensors' shapes and which of their pointers are NULL, never the data.  Same conventions and
+ * so that tests can hold every kernel route to a reference.  The route queries are host-only: they launch nothing, and read
+ * the tensors' shapes and which of their pointers are NULL, never the data.  The convolution route asks the runtime for the
+ * current device's SM count, which sizes the persistent halo kernel's grid.  Same conventions and
  * status codes as b200unet.h.
  */
 #ifndef B200UNET_DIAG_H_
@@ -24,6 +25,8 @@ typedef struct b200unet_diag_ext {
   int32_t x_vis[2][3];     /* conv: visible extents of each source */
   int32_t a_vis[3];        /* weight gradient: of the activation */
   int32_t dy_vis[3];       /* weight gradient and bias gradient: of dy */
+  int32_t max_ctas;        /* conv, halo kind on the persistent kernel: > 0 caps its CTAs per N tile (grid[0]), so that small
+                              shapes walk several voxel tiles per CTA */
 } b200unet_diag_ext;
 
 /* kernel kinds of b200unet_conv_route */
@@ -57,7 +60,8 @@ typedef struct b200unet_wgrad_route {
   int64_t part_bytes;             /* deterministic mode: splits * taps * cip * cop * 4, the partial-sum buffer it fills */
 } b200unet_wgrad_route;
 
-/* the route b200unet_conv3d / b200unet_diag_conv3d_ex take for this descriptor; an error when they would refuse it */
+/* the route b200unet_conv3d / b200unet_diag_conv3d_ex take for this descriptor on the current device (132 SMs without one); an
+ * error when they would refuse it */
 int b200unet_diag_conv3d_route(const b200unet_conv_desc* desc, const b200unet_diag_ext* ext, b200unet_conv_route* route);
 /* the route of b200unet_diag_wgrad_ex (deterministic = a partial buffer is passed) on a device with num_sms SMs */
 int b200unet_diag_wgrad_route(const b200unet_tensor* a, const b200unet_tensor* dy, int ksz, int stride, int cip, int cop,
