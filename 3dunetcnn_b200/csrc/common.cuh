@@ -82,6 +82,29 @@ static inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 }
 #endif
 
+// Opt Kernel in to `bytes` of dynamic shared memory, once per device: not a stream operation, so it stays out of CUDA-graph
+// captures after the first launch.  Keyed by the kernel itself (instantiations of one template share a signature).
+template <auto Kernel>
+static inline int set_max_dynamic_smem(int bytes) {
+  static bool done[64] = {};
+  int dev = 0;
+  B200_CHECK_CUDA(cudaGetDevice(&dev));
+  if (dev >= 64 || !done[dev]) {
+    B200_CHECK_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    if (dev < 64) done[dev] = true;
+  }
+  return OK;
+}
+
+// SMs of the current device; 132 (an H100 SXM) on a host without a GPU (route queries, planning).
+inline int device_sms() {
+  int dev = 0, sms = 0;
+  if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && sms > 0)
+    return sms;
+  cudaGetLastError();
+  return 132;
+}
+
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 static inline int round_up(int a, int b) { return ceil_div(a, b) * b; }
 

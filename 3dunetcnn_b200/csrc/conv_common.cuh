@@ -1,11 +1,47 @@
-// Shared pieces of the implicit-GEMM convolution kernel (igemm_conv.cu): argument block, TMA map bundle and the fused
-// epilogue.
+// Shared pieces of the implicit-GEMM convolution kernel (igemm_conv.cu) and the weight gradient (wgrad.cu): halo layout, tiling
+// policy, argument block, TMA map bundle and the fused epilogue.
 #pragma once
+#include <cstdlib>
 #include "kernels.h"
 #include "ptx.cuh"
 #include "tmap.h"
 
 namespace b200 {
+
+// Halo layout of the 3x3x3 stride-1 halo modes: an output tile of TW x TH x TD voxels reads ONE TMA box of BW x BH x BD source
+// voxels around it (its zero padding = TMA out-of-bounds fill), box row ((dz * BH) + hy) * BW + wx.  Output row r = h * TW + w of
+// tap (kd, kh, kw) reads box row tap_row + h * BW + w: each 8-row group (one h) is 8 consecutive box rows and the next group
+// starts GROUP_STRIDE rows further (the wgmma SBO).  Descriptors may start at any row inside the swizzled box: the swizzle is a
+// function of the absolute shared-memory address, for the TMA writes and for the wgmma reads alike.
+struct HaloTile {
+  static constexpr int TW = 8, TH = 16, TD = 1;
+  static constexpr int BW = TW + 2, BH = TH + 2, BD = TD + 2;
+  static constexpr int ROWS = BW * BH * BD;
+  static constexpr int GROUP_STRIDE = BW;
+  static constexpr int HALF_M = 64 / TW * BW;   // box rows from output row 0 to output row 64 (the second m64 half)
+  static_assert(TW == 8 && TW * TH == 128 && TD == 1, "one 128-row M tile of 8-row groups in one plane");
+  // tap = kd * 9 + kh * 3 + kw
+  __host__ __device__ static constexpr int tap_row(int tap) { return (tap / 9 * BH + tap / 3 % 3) * BW + tap % 3; }
+};
+
+// Channel buckets: K chunk (16 / 32 / 64) and N tile (16 / 32 / 64 / 128) for c channels.
+static inline int kc_bucket(int c) { return c > 32 ? 64 : c > 16 ? 32 : 16; }
+static inline int bn_bucket(int c) { return c > 64 ? 128 : kc_bucket(c); }
+
+// Per-tap voxel tile of 128 output voxels: as wide as W allows (<= 8), then <= 4 rows, the rest in depth.
+static inline void pick_tile(int Wo, int Ho, int Do, int& tw, int& th, int& td) {
+  tw = Wo >= 8 ? 8 : Wo >= 4 ? 4 : Wo >= 2 ? 2 : 1;
+  int rem = 128 / tw;
+  th = Ho >= 4 ? 4 : Ho >= 2 ? 2 : 1;
+  if (th > rem) th = rem;
+  td = rem / th;
+}
+
+// B200UNET_NO_HALO=1 keeps every convolution and weight gradient on per-tap tiles (A/B measurements).
+inline bool halo_disabled() {
+  static const bool off = getenv("B200UNET_NO_HALO") && atoi(getenv("B200UNET_NO_HALO")) != 0;
+  return off;
+}
 
 struct ConvMaps {
   CUtensorMap a[2][2];  // [source][hi/lo]

@@ -373,13 +373,7 @@ size_t head_mma_bwd_scratch_bytes(int n_out, int C) { return (size_t)kBwdSlots *
 
 template <int NT>
 static int launch_fwd_nt(const Act& x, const float* w, const float* bias, int n_out, int act_mode, float* logits, cudaStream_t st) {
-  static bool attr_set[64] = {};
-  int dev = 0;
-  B200_CHECK_CUDA(cudaGetDevice(&dev));
-  if (dev >= 64 || !attr_set[dev]) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(k_head_mma<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem(16 * NT)));
-    if (dev < 64) attr_set[dev] = true;
-  }
+  B200_TRY(set_max_dynamic_smem<k_head_mma<NT>>((int)fwd_smem(16 * NT)));
   const long long t = head_tiles(x);
   const int grid = (int)(t < 2 * 132 ? (t > 0 ? t : 1) : 2 * 132);
   k_head_mma<NT><<<grid, kThreads, fwd_smem(16 * NT), st>>>(x, w, bias, n_out, act_mode, logits);
@@ -390,13 +384,7 @@ static int launch_fwd_nt(const Act& x, const float* w, const float* bias, int n_
 template <int NT>
 static int launch_bwd_nt(const Act& x, const float* w, int n_out, const float* dlogits, const Act& dx, int want_dbias, float* part,
                          cudaStream_t st) {
-  static bool attr_set[64] = {};
-  int dev = 0;
-  B200_CHECK_CUDA(cudaGetDevice(&dev));
-  if (dev >= 64 || !attr_set[dev]) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(k_head_bwd_mma<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bwd_smem(16 * NT)));
-    if (dev < 64) attr_set[dev] = true;
-  }
+  B200_TRY(set_max_dynamic_smem<k_head_bwd_mma<NT>>((int)bwd_smem(16 * NT)));
   k_head_bwd_mma<NT><<<bwd_grid(x), kThreads, bwd_smem(16 * NT), st>>>(x, w, n_out, dlogits, dx, want_dbias, part);
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;

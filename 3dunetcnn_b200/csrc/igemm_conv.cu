@@ -18,26 +18,21 @@
 //           for the next GroupNorm (warp butterfly -> smem -> one double atomic per channel per CTA);
 //   mode 1: GroupNorm/ReLU backward: dz = dact * 1[A x + B > 0], per-channel (sum dz, sum dz*xhat).
 // Split-precision ("parity") mode runs three passes per K step: Ah*Wh, Al*Wh, Ah*Wl.
-#include <cstdlib>
 #include <type_traits>
 #include "conv_common.cuh"
 
 namespace b200 {
 
 // Kernel modes: per-tap streaming tiles, class mode (parity-class data gradient / k = s = 2 transposed convolution), and halo
-// mode: the 3x3x3 stride-1 source is loaded as ONE halo box (KC, 10, 18, 3) per K chunk for an 8 x 16 x 1 output tile, and the
-// 27 taps read it through shifted shared-memory descriptors (27x less activation traffic from L2 than per-tap boxes).
+// mode: the 3x3x3 stride-1 source, one K chunk wide, is loaded as ONE halo box around the output tile (HaloTile), and the 27
+// taps read it through shifted shared-memory descriptors (27x less activation traffic from L2 than per-tap boxes).
 // CONV_HALO_WS is halo mode on the persistent, weight-stationary kernel (k_igemm_conv_halo_ws) for the (BN, KC) whose 27 weight
 // tiles fit in shared memory beside the halo box; CONV_HALO runs the ring kernel below for the wider ones.
 enum ConvMode { CONV_STREAM = 0, CONV_CLASS = 1, CONV_HALO = 2, CONV_HALO_WS = 3 };
 
-// Shared memory: STAGES-deep TMA ring | fp32 accumulator tile [128][BN + 4] | (class mode) output staging | (halo mode) halo box
-// | aux.  Outside class mode the output staging tile reuses the ring: the CTA computes one tile, so every stage has been consumed
-// when the epilogue starts.  Class mode keeps the staging tile apart because the producer is already loading the next class.
-// BN <= 32 (<= 204 registers per thread) sizes the ring so that two CTAs share an SM (one CTA's epilogue overlaps the other's
-// MMAs) when that still leaves four stages; otherwise one CTA takes up to 227 KB.
-template <int BN, int KC, int MODE>
-struct ConvCfg {
+// Tile sizes and shared-memory limits both convolution kernels derive from (BN, KC).
+template <int BN, int KC>
+struct ConvTileCfg {
   static constexpr int A_BYTES = 128 * KC * 2;
   static constexpr int B_BOX_BYTES = BN * KC * 2;
   static constexpr int B_BYTES = B_BOX_BYTES < 1024 ? 1024 : B_BOX_BYTES;
@@ -45,25 +40,76 @@ struct ConvCfg {
   static constexpr int ACC_LD = BN + 4;                     // floats per accumulator row: 16-byte aligned, rows on staggered banks
   static constexpr int ACC_BYTES = 128 * ACC_LD * 4;
   static constexpr int AUX_BYTES = 1024 + 4 * BN * 2 * 4 + BN * 16;  // barriers | per-warp stats | coef
-  static constexpr int OUT_STAGING = 2 * 128 * BN * 2;    // hi + lo output tiles (class pairs: 256 rows of hi)
-  static constexpr int STG_BYTES = MODE == CONV_CLASS ? OUT_STAGING : 0;
   static constexpr int RB = KC * 2;                        // bytes per voxel row of an activation tile
-  static constexpr int HALO_TX = 540 * RB;                 // 10 x 18 x 3 voxels
-  static constexpr int HALO_BYTES = MODE == CONV_HALO ? (HALO_TX + 1023) / 1024 * 1024 : 0;
-  static constexpr int FIXED = ACC_BYTES + STG_BYTES + HALO_BYTES + AUX_BYTES + 1024;   // +1024 alignment slack
+  static constexpr int HALO_TX = HaloTile::ROWS * RB;
+  static constexpr int HALO_BOX_BYTES = (HALO_TX + 1023) / 1024 * 1024;
   static constexpr int SMEM_LIMIT = 232448;                // sm_90 opt-in dynamic shared memory per block
   static constexpr int TWO_PER_SM = 115712;                // 228 KB per SM, 1 KB reserved per block
-  static constexpr int MIN_BLOCKS = BN <= 32 ? 2 : 1;      // 2 x 160 threads x <= 204 registers fit the 64 K register file
-  static constexpr int STAGES_2 = MIN_BLOCKS == 2 ? (TWO_PER_SM - FIXED) / STAGE_BYTES : 0;
-  static constexpr int STAGES_RAW = STAGES_2 >= 4 ? STAGES_2 : (SMEM_LIMIT - FIXED) / STAGE_BYTES;
-  static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
-  static constexpr int BLOCKS_PER_SM = STAGES_2 >= 4 ? 2 : 1;
-  static constexpr int PIPE_BYTES = STAGES * STAGE_BYTES > OUT_STAGING ? STAGES * STAGE_BYTES : OUT_STAGING;
-  static constexpr int SMEM_BYTES = PIPE_BYTES + FIXED;
   static constexpr uint32_t LAYOUT = swizzle_for_row_bytes(KC * 2);
   static constexpr uint32_t SBO = 8 * KC * 2;
-  static_assert(STAGES >= 2 && SMEM_BYTES <= SMEM_LIMIT, "igemm_conv: configuration does not fit shared memory");
 };
+
+// Shared memory: STAGES-deep TMA ring | fp32 accumulator tile [128][BN + 4] | (class mode) output staging | (halo mode) halo box
+// | aux.  Outside class mode the output staging tile reuses the ring: the CTA computes one tile, so every stage has been consumed
+// when the epilogue starts.  Class mode keeps the staging tile apart because the producer is already loading the next class.
+// BN <= 32 (<= 204 registers per thread) sizes the ring so that two CTAs share an SM (one CTA's epilogue overlaps the other's
+// MMAs) when that still leaves four stages; otherwise one CTA takes up to 227 KB.
+template <int BN, int KC, int MODE>
+struct ConvCfg : ConvTileCfg<BN, KC> {
+  using Tile = ConvTileCfg<BN, KC>;
+  static constexpr int OUT_STAGING = 2 * 128 * BN * 2;    // hi + lo output tiles (class pairs: 256 rows of hi)
+  static constexpr int STG_BYTES = MODE == CONV_CLASS ? OUT_STAGING : 0;
+  static constexpr int HALO_BYTES = MODE == CONV_HALO ? Tile::HALO_BOX_BYTES : 0;
+  static constexpr int FIXED = Tile::ACC_BYTES + STG_BYTES + HALO_BYTES + Tile::AUX_BYTES + 1024;   // +1024 alignment slack
+  static constexpr int MIN_BLOCKS = BN <= 32 ? 2 : 1;      // 2 x 160 threads x <= 204 registers fit the 64 K register file
+  static constexpr int STAGES_2 = MIN_BLOCKS == 2 ? (Tile::TWO_PER_SM - FIXED) / Tile::STAGE_BYTES : 0;
+  static constexpr int STAGES_RAW = STAGES_2 >= 4 ? STAGES_2 : (Tile::SMEM_LIMIT - FIXED) / Tile::STAGE_BYTES;
+  static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
+  static constexpr int BLOCKS_PER_SM = STAGES_2 >= 4 ? 2 : 1;
+  static constexpr int PIPE_BYTES = STAGES * Tile::STAGE_BYTES > OUT_STAGING ? STAGES * Tile::STAGE_BYTES : OUT_STAGING;
+  static constexpr int SMEM_BYTES = PIPE_BYTES + FIXED;
+  static_assert(STAGES >= 2 && SMEM_BYTES <= Tile::SMEM_LIMIT, "igemm_conv: configuration does not fit shared memory");
+};
+
+// Accumulator fragments of the two m64 halves -> s_acc (row-major, ACC_LD floats per row), so that each thread drains one
+// output voxel row in the epilogue.
+template <int BN, int ACC_LD>
+__device__ __forceinline__ void store_acc(float* s_acc, const float (&acc)[2][BN / 2], int warp, int lane) {
+#pragma unroll
+  for (int hm = 0; hm < 2; ++hm) {
+    const int r0 = hm * 64 + warp * 16 + (lane >> 2);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = j * 8 + 2 * (lane & 3);
+      *reinterpret_cast<float2*>(s_acc + r0 * ACC_LD + c) = make_float2(acc[hm][4 * j], acc[hm][4 * j + 1]);
+      *reinterpret_cast<float2*>(s_acc + (r0 + 8) * ACC_LD + c) = make_float2(acc[hm][4 * j + 2], acc[hm][4 * j + 3]);
+    }
+  }
+}
+
+// Mode 1: the norm coefficients of sample n for the N tile at n0 -> s_coef (zero beyond Cout).
+template <int BN>
+__device__ __forceinline__ void load_coef(float4* s_coef, const ConvArgs& p, int n, int n0) {
+  for (int c = threadIdx.x; c < BN; c += 128)
+    s_coef[c] = (n0 + c < p.Cout) ? p.coef[(long long)n * p.coef_ld + n0 + c] : make_float4(0.f, 0.f, 0.f, 0.f);
+}
+
+// The epilogue warps' fp32 partial sums of sample n -> one fp64 atomic per channel statistic into dst [N][ld][2] (mode 0:
+// stats, mode 1: bstats); `restart` zeroes the slots for the next tile.
+template <int BN>
+__device__ __forceinline__ void flush_stats(float* s_stats, double* dst, int ld, int Cout, int n, int n0, bool restart) {
+  for (int c = threadIdx.x; c < BN * 2; c += 128) {
+    const float v = s_stats[c] + s_stats[BN * 2 + c] + s_stats[2 * BN * 2 + c] + s_stats[3 * BN * 2 + c];
+    if (restart) { s_stats[c] = 0.f; s_stats[BN * 2 + c] = 0.f; s_stats[2 * BN * 2 + c] = 0.f; s_stats[3 * BN * 2 + c] = 0.f; }
+    if (n0 + (c >> 1) < Cout) atomicAdd(&dst[((long long)n * ld + n0) * 2 + c], (double)v);
+  }
+}
+
+// Start (descriptor units) of the A operand of tap `tap` in the halo box whose descriptor starts at box_lo.
+template <int RB>
+__device__ __forceinline__ uint32_t halo_tap_lo(uint32_t box_lo, int tap) {
+  return box_lo + ((HaloTile::tap_row(tap) * RB) >> 4);
+}
 
 // Warps 0-3: one consumer warpgroup (wgmma issue, then the epilogue, one output voxel row per thread); warp 4: TMA producer.
 template <int BN, int KC, int MODE>
@@ -82,7 +128,6 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
   uint64_t* halo_full = empty_bar + Cfg::STAGES;
-  uint64_t* halo_empty = halo_full + 1;
   float* s_stats = reinterpret_cast<float*>(aux + 1024);             // [4 warps][BN][2]
   float4* s_coef = reinterpret_cast<float4*>(aux + 1024 + 4 * BN * 8);   // [BN]
 
@@ -102,17 +147,12 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
     tma_prefetch_desc(&maps.b[0][0]);
     for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 4); }
     mbar_init(halo_full, 1);
-    mbar_init(halo_empty, 4);
     fence_barrier_init();
   }
   pdl_wait();   // before the first global read (the coefficient table below); the barrier set-up above overlaps the previous kernel
   if (warp < 4) {
-    const int e = threadIdx.x;
-    for (int i = e; i < 4 * BN * 2; i += 128) s_stats[i] = 0.f;
-    if (p.mode == 1) {
-      for (int c = e; c < BN; c += 128)
-        s_coef[c] = (n0 + c < p.Cout) ? p.coef[(long long)n * p.coef_ld + n0 + c] : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
+    for (int i = threadIdx.x; i < 4 * BN * 2; i += 128) s_stats[i] = 0.f;
+    if (p.mode == 1) load_coef<BN>(s_coef, p, n, n0);
   }
   __syncthreads();
   pdl_launch_dependents();
@@ -134,18 +174,15 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
       if (nt == 0) continue;
       const int ks = p.ksz[src], pad = p.pad[src], sd = p.stride[src];
       if (MODE == CONV_HALO && src == 0) {
-        // one halo box per K chunk (its zero padding = TMA out-of-bounds fill), then the 27 taps' weight tiles
-        for (int kc = 0; kc < p.kchunks[0]; ++kc) {
-          mbar_wait(halo_empty, (kc & 1) ^ 1);
-          mbar_expect_tx_if(issue, halo_full, Cfg::HALO_TX);
-          tma_load_5d_if(issue, halo, &maps.a[0][0], halo_full, kc * KC, w0 - 1, h0 - 1, d0 - 1, n);
-          for (int tap = 0; tap < 27; ++tap) {
-            const int s = it % Cfg::STAGES;
-            mbar_wait(&empty_bar[s], ((it / Cfg::STAGES) & 1) ^ 1);
-            mbar_expect_tx_if(issue, &full_bar[s], Cfg::B_BOX_BYTES);
-            tma_load_3d_if(issue, smem + s * Cfg::STAGE_BYTES + Cfg::A_BYTES, &maps.b[0][0], &full_bar[s], kc * KC, n0, tap);
-            ++it;
-          }
+        // the halo box (one K chunk; its zero padding = TMA out-of-bounds fill), then the 27 taps' weight tiles
+        mbar_expect_tx_if(issue, halo_full, Cfg::HALO_TX);
+        tma_load_5d_if(issue, halo, &maps.a[0][0], halo_full, 0, w0 - 1, h0 - 1, d0 - 1, n);
+        for (int tap = 0; tap < 27; ++tap) {
+          const int s = it % Cfg::STAGES;
+          mbar_wait(&empty_bar[s], ((it / Cfg::STAGES) & 1) ^ 1);
+          mbar_expect_tx_if(issue, &full_bar[s], Cfg::B_BOX_BYTES);
+          tma_load_3d_if(issue, smem + s * Cfg::STAGE_BYTES + Cfg::A_BYTES, &maps.b[0][0], &full_bar[s], 0, n0, tap);
+          ++it;
         }
         continue;
       }
@@ -204,29 +241,22 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
   float acc[2][BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
-  // halo mode: the halo box holds rows ((dz * 18) + hy) * 10 + wx; output row r = h * 8 + w of tap (kd, kh, kw) reads halo row
-  // (kd * 18 + h + kh) * 10 + w + kw, so each 8-row group (one h) is 8 consecutive halo rows and the next group starts one halo
-  // row of 10 voxels further (SBO).  The descriptors start at arbitrary row offsets inside the swizzled box: the swizzle is a
-  // function of the absolute shared-memory address, for the TMA writes and for the wgmma reads alike.
-  constexpr uint32_t hi_halo = desc_hi(10 * Cfg::RB, Cfg::LAYOUT);
+  // halo mode: iterations 0..26 are the taps of source 0, read from the halo box (HaloTile)
+  constexpr uint32_t hi_halo = desc_hi(HaloTile::GROUP_STRIDE * Cfg::RB, Cfg::LAYOUT);
   const uint32_t halo_lo0 = desc_lo(smem_u32(halo), 16);
-  const int halo_iters = MODE == CONV_HALO ? 27 * p.kchunks[0] : 0;
+  if (MODE == CONV_HALO) mbar_wait(halo_full, 0);
   int it = 0;
   for (int cls = 0; cls < (p.cls_mode ? 8 : 1); ++cls) {
     const int n_it = p.cls_mode ? (int)p.cls_n[cls] * p.kchunks[0] * p.npass : total_iters;
     int prev = -1;   // ring slot whose MMAs may still be reading it
     for (int i = 0; i < n_it; ++i, ++it) {
       const int s = it % Cfg::STAGES;
-      const bool from_halo = i < halo_iters;
-      const int tap = i % 27;
-      if (from_halo && tap == 0) mbar_wait(halo_full, (i / 27) & 1);
       mbar_wait(&full_bar[s], (it / Cfg::STAGES) & 1);
       uint32_t a_lo = desc_lo(smem0 + s * Cfg::STAGE_BYTES, 16), a_hi = hi_d, a_half = HALF_M;
-      if (MODE == CONV_HALO && from_halo) {
-        const int kd = tap / 9, kh = (tap / 3) % 3, kw = tap % 3;
-        a_lo = halo_lo0 + (((kd * 180 + kh * 10 + kw) * Cfg::RB) >> 4);
+      if (MODE == CONV_HALO && i < 27) {
+        a_lo = halo_tap_lo<Cfg::RB>(halo_lo0, i);
         a_hi = hi_halo;
-        a_half = (80 * Cfg::RB) >> 4;   // rows 64-127 = h 8..15
+        a_half = (HaloTile::HALF_M * Cfg::RB) >> 4;
       }
       const uint32_t b_lo = desc_lo(smem0 + s * Cfg::STAGE_BYTES + Cfg::A_BYTES, 16);
       wgmma_fence();
@@ -237,43 +267,21 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
         Wgmma<BN>::template mma<0, 0>(acc[1], desc_from(a_lo + a_half + 2 * k, a_hi), desc_from(b_lo + 2 * k, hi_d), accumulate);
       }
       wgmma_commit();
-      if (from_halo && tap == 26) {
-        // last tap of a halo box: the producer can load the next chunk's box only once every MMA reading this one is done,
-        // and the next MMA needs that box -- so drain here instead of deferring the hand-back by one stage
-        wgmma_wait<0>();
-        if (lane == 0) {
-          if (prev >= 0) mbar_arrive(&empty_bar[prev]);
-          mbar_arrive(&empty_bar[s]);
-          mbar_arrive(halo_empty);
-        }
-        prev = -1;
-      } else {
-        wgmma_wait<1>();   // the previous stage's MMAs are complete: hand its slot back to the producer
-        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-        prev = s;
-      }
+      wgmma_wait<1>();   // the previous stage's MMAs are complete: hand its slot back to the producer
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = s;
     }
     wgmma_wait<0>();
     wgmma_fence_regs(acc[0]);
     wgmma_fence_regs(acc[1]);
     if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
 
-    // accumulator fragments -> s_acc (row-major), so that each thread drains one output voxel row below
     const bool pair = p.cls_pair != 0, pair_first = pair && (cls & 1) == 0, pair_second = pair && (cls & 1) == 1;
     if (cls > 0) {
       if (!pair_second && threadIdx.x == 0) tma_store_wait_read0();    // the previous stores have read the staging tile
       asm volatile("bar.sync 1, 128;" ::: "memory");                   // and every thread has read its s_acc row
     }
-#pragma unroll
-    for (int hm = 0; hm < 2; ++hm) {
-      const int r0 = hm * 64 + warp * 16 + (lane >> 2);
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int c = j * 8 + 2 * (lane & 3);
-        *reinterpret_cast<float2*>(s_acc + r0 * Cfg::ACC_LD + c) = make_float2(acc[hm][4 * j], acc[hm][4 * j + 1]);
-        *reinterpret_cast<float2*>(s_acc + (r0 + 8) * Cfg::ACC_LD + c) = make_float2(acc[hm][4 * j + 2], acc[hm][4 * j + 3]);
-      }
-    }
+    store_acc<BN, Cfg::ACC_LD>(s_acc, acc, warp, lane);
     asm volatile("bar.sync 1, 128;" ::: "memory");
 
     const long long vox = vox_of(cls);
@@ -304,12 +312,7 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
   }
   if (want_stats) {
     asm volatile("bar.sync 1, 128;" ::: "memory");
-    double* dst = (p.mode == 0) ? p.stats : p.bstats;
-    const int ld = (p.mode == 0) ? p.stats_ld : p.coef_ld;
-    for (int c = threadIdx.x; c < BN * 2; c += 128) {
-      const float v = s_stats[c] + s_stats[BN * 2 + c] + s_stats[2 * BN * 2 + c] + s_stats[3 * BN * 2 + c];
-      if (n0 + (c >> 1) < p.Cout) atomicAdd(&dst[((long long)n * ld + n0) * 2 + c], (double)v);
-    }
+    flush_stats<BN>(s_stats, (p.mode == 0) ? p.stats : p.bstats, (p.mode == 0) ? p.stats_ld : p.coef_ld, p.Cout, n, n0, false);
   }
   if (threadIdx.x == 0) tma_store_wait_all();   // the staging tile must outlive the bulk store
 }
@@ -326,30 +329,20 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
 // into registers before the staging tile overwrites it, and the producer refills the ring only once the previous tile's TMA store
 // has read the staging tile (r_free).  That is what lets BN 32 / KC 32 keep two CTAs per SM.
 template <int BN, int KC>
-struct HaloWsCfg {
-  static constexpr int A_BYTES = 128 * KC * 2;
-  static constexpr int B_BOX_BYTES = BN * KC * 2;
-  static constexpr int B_BYTES = B_BOX_BYTES < 1024 ? 1024 : B_BOX_BYTES;
+struct HaloWsCfg : ConvTileCfg<BN, KC> {
+  using Tile = ConvTileCfg<BN, KC>;
   static constexpr int STAGES = 2;                          // second-source ring
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int ACC_LD = BN + 4;
-  static constexpr int ACC_BYTES = 128 * ACC_LD * 4;        // > the 128 x BN bf16 staging tile
-  static constexpr int W_BYTES = (27 * B_BOX_BYTES + 1023) / 1024 * 1024;
-  static constexpr int R_RAW = STAGES * STAGE_BYTES > ACC_BYTES ? STAGES * STAGE_BYTES : ACC_BYTES;
+  static constexpr int W_BYTES = (27 * Tile::B_BOX_BYTES + 1023) / 1024 * 1024;
+  // ACC_BYTES > the 128 x BN bf16 staging tile
+  static constexpr int R_RAW = STAGES * Tile::STAGE_BYTES > Tile::ACC_BYTES ? STAGES * Tile::STAGE_BYTES : Tile::ACC_BYTES;
   static constexpr int R_BYTES = (R_RAW + 1023) / 1024 * 1024;
-  static constexpr int RB = KC * 2;
-  static constexpr int HALO_TX = 540 * RB;
-  static constexpr int HALO_BYTES = (HALO_TX + 1023) / 1024 * 1024;
-  static constexpr int AUX_BYTES = 1024 + 4 * BN * 2 * 4 + BN * 16;   // barriers | per-warp stats | coef
-  static constexpr int FIXED = W_BYTES + R_BYTES + AUX_BYTES + 1024;  // +1024 alignment slack
+  static constexpr int FIXED = W_BYTES + R_BYTES + Tile::AUX_BYTES + 1024;  // +1024 alignment slack
   static constexpr int BLOCKS_PER_SM = BN <= 32 ? 2 : 1;
-  static constexpr int BUDGET = BLOCKS_PER_SM == 2 ? ConvCfg<BN, KC, CONV_STREAM>::TWO_PER_SM : ConvCfg<BN, KC, CONV_STREAM>::SMEM_LIMIT;
-  static constexpr int HALO_BUFS = FIXED + 2 * HALO_BYTES <= BUDGET ? 2 : 1;
-  static constexpr int SMEM_BYTES = FIXED + HALO_BUFS * HALO_BYTES;
+  static constexpr int BUDGET = BLOCKS_PER_SM == 2 ? Tile::TWO_PER_SM : Tile::SMEM_LIMIT;
+  static constexpr int HALO_BUFS = FIXED + 2 * Tile::HALO_BOX_BYTES <= BUDGET ? 2 : 1;
+  static constexpr int SMEM_BYTES = FIXED + HALO_BUFS * Tile::HALO_BOX_BYTES;
   // BN <= 64: the accumulator row a thread holds in registers during the epilogue stays at <= 64 floats
   static constexpr bool FITS = BN <= 64 && SMEM_BYTES <= BUDGET;
-  static constexpr uint32_t LAYOUT = swizzle_for_row_bytes(KC * 2);
-  static constexpr uint32_t SBO = 8 * KC * 2;
 };
 
 template <int BN, int KC>
@@ -362,7 +355,7 @@ __global__ void __launch_bounds__(160, (HaloWsCfg<BN, KC>::BLOCKS_PER_SM)) k_ige
   uint8_t* wts = smem;
   uint8_t* reg = smem + Cfg::W_BYTES;
   uint8_t* halo = reg + Cfg::R_BYTES;
-  uint8_t* aux = halo + Cfg::HALO_BUFS * Cfg::HALO_BYTES;
+  uint8_t* aux = halo + Cfg::HALO_BUFS * Cfg::HALO_BOX_BYTES;
   uint64_t* w_full = reinterpret_cast<uint64_t*>(aux);
   uint64_t* halo_full = w_full + 1;               // [HALO_BUFS]
   uint64_t* halo_empty = halo_full + 2;           // [HALO_BUFS]
@@ -378,9 +371,9 @@ __global__ void __launch_bounds__(160, (HaloWsCfg<BN, KC>::BLOCKS_PER_SM)) k_ige
   const int ntiles = p.N * p.tiles_d * p.tiles_h * p.tiles_w;
   const int n0 = blockIdx.y * BN;
   auto tile_origin = [&](int t, int& w0, int& h0, int& d0, int& n) {
-    w0 = (t % p.tiles_w) * 8; t /= p.tiles_w;
-    h0 = (t % p.tiles_h) * 16; t /= p.tiles_h;
-    d0 = t % p.tiles_d;
+    w0 = (t % p.tiles_w) * HaloTile::TW; t /= p.tiles_w;
+    h0 = (t % p.tiles_h) * HaloTile::TH; t /= p.tiles_h;
+    d0 = (t % p.tiles_d) * HaloTile::TD;
     n = t / p.tiles_d;
   };
 
@@ -411,7 +404,7 @@ __global__ void __launch_bounds__(160, (HaloWsCfg<BN, KC>::BLOCKS_PER_SM)) k_ige
       const int hb = j % Cfg::HALO_BUFS;
       mbar_wait(&halo_empty[hb], ((j / Cfg::HALO_BUFS) & 1) ^ 1);
       mbar_expect_tx_if(issue, &halo_full[hb], Cfg::HALO_TX);
-      tma_load_5d_if(issue, halo + hb * Cfg::HALO_BYTES, &maps.a[0][0], &halo_full[hb], 0, w0 - 1, h0 - 1, d0 - 1, n);
+      tma_load_5d_if(issue, halo + hb * Cfg::HALO_BOX_BYTES, &maps.a[0][0], &halo_full[hb], 0, w0 - 1, h0 - 1, d0 - 1, n);
       if (p.ntaps[1] == 0) continue;
       mbar_wait(r_free, (j & 1) ^ 1);   // the previous tile's store has read R
       for (int kc = 0; kc < p.kchunks[1]; ++kc, ++it) {
@@ -428,14 +421,14 @@ __global__ void __launch_bounds__(160, (HaloWsCfg<BN, KC>::BLOCKS_PER_SM)) k_ige
 
   // -------------------------------------------------------------------- consumer warpgroup: wgmma, then the epilogue
   constexpr uint32_t hi_d = desc_hi(Cfg::SBO, Cfg::LAYOUT);
-  constexpr uint32_t hi_halo = desc_hi(10 * Cfg::RB, Cfg::LAYOUT);   // see k_igemm_conv: 8-row groups are 10 halo rows apart
-  constexpr uint32_t HALF_M = (64 * KC * 2) >> 4;                    // ring A tile: row 64
-  constexpr uint32_t HALO_HALF = (80 * Cfg::RB) >> 4;                // halo: output rows 64-127 = h 8..15
+  constexpr uint32_t hi_halo = desc_hi(HaloTile::GROUP_STRIDE * Cfg::RB, Cfg::LAYOUT);
+  constexpr uint32_t HALF_M = (64 * KC * 2) >> 4;                         // ring A tile: row 64
+  constexpr uint32_t HALO_HALF = (HaloTile::HALF_M * Cfg::RB) >> 4;      // halo: output rows 64-127
   const uint32_t w_lo0 = desc_lo(smem_u32(wts), 16);
   const uint32_t halo_lo0 = desc_lo(smem_u32(halo), 16);
   const uint32_t reg0 = smem_u32(reg);
   const int row = threadIdx.x;
-  const int wl = row % 8, hl = row / 8;
+  const int wl = row % HaloTile::TW, hl = row / HaloTile::TW;
   const bool want_stats = (p.mode == 0) ? (p.stats != nullptr) : (p.bstats != nullptr);
   double* stats_dst = (p.mode == 0) ? p.stats : p.bstats;
   const int stats_ld = (p.mode == 0) ? p.stats_ld : p.coef_ld;
@@ -451,7 +444,7 @@ __global__ void __launch_bounds__(160, (HaloWsCfg<BN, KC>::BLOCKS_PER_SM)) k_ige
     conv_epilogue_prefetch(p, n0, BN, vox, valid);   // -> L2 while the MMAs run
 
     const int hb = j % Cfg::HALO_BUFS;
-    const uint32_t hlo = halo_lo0 + ((hb * Cfg::HALO_BYTES) >> 4);
+    const uint32_t hlo = halo_lo0 + ((hb * Cfg::HALO_BOX_BYTES) >> 4);
     float acc[2][BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
@@ -459,8 +452,7 @@ __global__ void __launch_bounds__(160, (HaloWsCfg<BN, KC>::BLOCKS_PER_SM)) k_ige
     wgmma_fence();
 #pragma unroll
     for (int tap = 0; tap < 27; ++tap) {
-      const int kd = tap / 9, kh = (tap / 3) % 3, kw = tap % 3;
-      const uint32_t a_lo = hlo + (((kd * 180 + kh * 10 + kw) * Cfg::RB) >> 4);
+      const uint32_t a_lo = halo_tap_lo<Cfg::RB>(hlo, tap);
       const uint32_t b_lo = w_lo0 + ((tap * Cfg::B_BOX_BYTES) >> 4);
 #pragma unroll
       for (int k = 0; k < KC / 16; ++k) {
@@ -500,20 +492,10 @@ __global__ void __launch_bounds__(160, (HaloWsCfg<BN, KC>::BLOCKS_PER_SM)) k_ige
     // every warp's MMAs have retired (the ring lived in R) and the previous store has read R
     asm volatile("bar.sync 1, 128;" ::: "memory");
     if (p.mode == 1 && n != coef_n) {   // the previous epilogue's reads of s_coef ended before its last barrier
-      for (int c = threadIdx.x; c < BN; c += 128)
-        s_coef[c] = (n0 + c < p.Cout) ? p.coef[(long long)n * p.coef_ld + n0 + c] : make_float4(0.f, 0.f, 0.f, 0.f);
+      load_coef<BN>(s_coef, p, n, n0);
       coef_n = n;
     }
-#pragma unroll
-    for (int hm = 0; hm < 2; ++hm) {
-      const int r0 = hm * 64 + warp * 16 + (lane >> 2);
-#pragma unroll
-      for (int jj = 0; jj < BN / 8; ++jj) {
-        const int c = jj * 8 + 2 * (lane & 3);
-        *reinterpret_cast<float2*>(s_acc + r0 * Cfg::ACC_LD + c) = make_float2(acc[hm][4 * jj], acc[hm][4 * jj + 1]);
-        *reinterpret_cast<float2*>(s_acc + (r0 + 8) * Cfg::ACC_LD + c) = make_float2(acc[hm][4 * jj + 2], acc[hm][4 * jj + 3]);
-      }
-    }
+    store_acc<BN, Cfg::ACC_LD>(s_acc, acc, warp, lane);
     asm volatile("bar.sync 1, 128;" ::: "memory");
     float4 acc_row[BN / 4];
 #pragma unroll
@@ -527,26 +509,12 @@ __global__ void __launch_bounds__(160, (HaloWsCfg<BN, KC>::BLOCKS_PER_SM)) k_ige
       tma_store_5d(&maps.o[0], reg, n0, w0, h0, d0, n);
       tma_store_commit();
     }
-    if (want_stats) {   // this tile's fp32 partials -> one fp64 atomic per channel; the slots restart from zero
-      for (int c = threadIdx.x; c < BN * 2; c += 128) {
-        const float v = s_stats[c] + s_stats[BN * 2 + c] + s_stats[2 * BN * 2 + c] + s_stats[3 * BN * 2 + c];
-        s_stats[c] = 0.f; s_stats[BN * 2 + c] = 0.f; s_stats[2 * BN * 2 + c] = 0.f; s_stats[3 * BN * 2 + c] = 0.f;
-        if (n0 + (c >> 1) < p.Cout) atomicAdd(&stats_dst[((long long)n * stats_ld + n0) * 2 + c], (double)v);
-      }
-    }
+    if (want_stats) flush_stats<BN>(s_stats, stats_dst, stats_ld, p.Cout, n, n0, true);   // the slots restart from zero
   }
   if (threadIdx.x == 0) tma_store_wait_all();   // the staging tile must outlive the bulk store
 }
 
 // ----------------------------------------------------------------------------------------------- host side
-static void pick_tile(int Wo, int Ho, int Do, int& tw, int& th, int& td) {
-  tw = Wo >= 8 ? 8 : Wo >= 4 ? 4 : Wo >= 2 ? 2 : 1;
-  int rem = 128 / tw;
-  th = Ho >= 4 ? 4 : Ho >= 2 ? 2 : 1;
-  if (th > rem) th = rem;
-  td = rem / th;
-}
-
 // The compile-time configuration of the kernel a (BN, KC, MODE) launch runs.
 template <int BN, int KC, int MODE>
 using ConvCfgOf = std::conditional_t<MODE == CONV_HALO_WS, HaloWsCfg<BN, KC>, ConvCfg<BN, KC, MODE>>;
@@ -554,20 +522,13 @@ using ConvCfgOf = std::conditional_t<MODE == CONV_HALO_WS, HaloWsCfg<BN, KC>, Co
 template <int BN, int KC, int MODE>
 static int launch_cfg(const ConvMaps& maps, const ConvArgs& args, dim3 grid, cudaStream_t st, const ConvClassMaps& cmaps) {
   using Cfg = ConvCfgOf<BN, KC, MODE>;
-  static bool attr_set[64] = {false};
-  int dev = 0;
-  B200_CHECK_CUDA(cudaGetDevice(&dev));
-  if (dev < 64 && !attr_set[dev]) {
-    if constexpr (MODE == CONV_HALO_WS)
-      B200_CHECK_CUDA(cudaFuncSetAttribute(k_igemm_conv_halo_ws<BN, KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    else
-      B200_CHECK_CUDA(cudaFuncSetAttribute(k_igemm_conv<BN, KC, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    attr_set[dev] = true;
-  }
-  if constexpr (MODE == CONV_HALO_WS)
+  if constexpr (MODE == CONV_HALO_WS) {
+    B200_TRY((set_max_dynamic_smem<k_igemm_conv_halo_ws<BN, KC>>(Cfg::SMEM_BYTES)));
     launch_pdl(k_igemm_conv_halo_ws<BN, KC>, grid, dim3(160), Cfg::SMEM_BYTES, st, maps, args);
-  else
+  } else {
+    B200_TRY((set_max_dynamic_smem<k_igemm_conv<BN, KC, MODE>>(Cfg::SMEM_BYTES)));
     launch_pdl(k_igemm_conv<BN, KC, MODE>, grid, dim3(160), Cfg::SMEM_BYTES, st, maps, args, cmaps);
+  }
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;
 }
@@ -585,12 +546,11 @@ static int conv_kc(const ConvOp& op) {
   int k = 0;
   for (int s = 1; s < op.nsrc; ++s)
     if (op.src[s].ksz > op.src[k].ksz || (op.src[s].ksz == op.src[k].ksz && op.src[s].x.C > op.src[k].x.C)) k = s;
-  const int c = op.src[k].x.C;
-  return c > 32 ? 64 : c > 16 ? 32 : 16;
+  return kc_bucket(op.src[k].x.C);
 }
 
 static int conv_bn(const ConvOp& op) {
-  const int BN = op.out.C > 64 ? 128 : op.out.C > 32 ? 64 : op.out.C > 16 ? 32 : 16;
+  const int BN = bn_bucket(op.out.C);
   return op.cls_mode && BN > 64 ? 64 : BN;   // class mode keeps its staging tile beside the accumulator tile (ConvCfg)
 }
 
@@ -618,23 +578,17 @@ static bool halo_keeps_occupancy(int BN, int KC) {
   return false;
 }
 
-// Halo mode (see ConvMode) for 3x3x3 stride-1 convolutions (plus an optional fused 1x1x1 source) whose output planes fill the
-// 8 x 16 tile, in single-pass bf16, when it keeps the configuration's CTAs per SM.  Inputs wider than 64 channels take several
-// halo boxes per tile, drained one after the other;
-// they stay on per-tap tiles unless voxels * Cout >= B200UNET_HALO_WIDE_MIN (tests set it to 0 to reach that path with
-// oracle-sized shapes; off by default: the forward category of the C2 step was slower with them in halo mode on the H100).  B200UNET_NO_HALO=1 keeps every launch on the per-tap kernel (A/B measurements).
-bool conv_halo_eligible(const ConvOp& op) {
-  static const bool off = getenv("B200UNET_NO_HALO") && atoi(getenv("B200UNET_NO_HALO")) != 0;
-  if (off || op.cls_mode) return false;
+// Halo mode (see ConvMode) for 3x3x3 stride-1 convolutions with <= 64 input channels (plus an optional fused 1x1x1 source)
+// whose output planes fill the halo tile, in single-pass bf16, when it keeps the configuration's CTAs per SM.  Wider inputs
+// stay on per-tap tiles: several halo boxes per tile were slower in the forward convolutions of the C2 step on the H100.
+static bool conv_halo_eligible(const ConvOp& op) {
+  if (halo_disabled() || op.cls_mode) return false;
   const ConvSrc& c = op.src[0];
-  if (c.ksz != 3 || c.stride != 1 || c.nopad) return false;
+  if (c.ksz != 3 || c.stride != 1 || c.nopad || c.x.C > 64) return false;
   if (op.nsrc == 2 && (op.src[1].ksz != 1 || op.src[1].stride != 1)) return false;
   for (int s = 0; s < op.nsrc; ++s)
     if (op.src[s].x.lo || op.src[s].w_lo) return false;
-  long long wide_min = -1;
-  if (const char* e = getenv("B200UNET_HALO_WIDE_MIN")) wide_min = atoll(e);
-  if (c.x.C > 64 && (wide_min < 0 || (long long)op.out.N * op.out.D * op.out.H * op.out.W * op.out.C < wide_min)) return false;
-  return op.out.W >= 8 && op.out.H >= 16 && halo_keeps_occupancy(conv_bn(op), conv_kc(op));
+  return op.out.W >= HaloTile::TW && op.out.H >= HaloTile::TH && halo_keeps_occupancy(conv_bn(op), conv_kc(op));
 }
 
 template <int BN_, int KC_, int MODE_>
@@ -702,8 +656,8 @@ int conv_route(const ConvOp& op, int num_sms, ConvRoute* r) {
   }
   const bool halo = conv_halo_eligible(op);
   r->kind = op.cls_mode == 1 ? CONV_KIND_CLASS1 : op.cls_mode == 2 ? CONV_KIND_CLASS2 : halo ? CONV_KIND_HALO : CONV_KIND_TAP;
-  if (halo) {   // 8 x 16 output plane tiles
-    r->tw = 8; r->th = 16; r->td = 1;
+  if (halo) {
+    r->tw = HaloTile::TW; r->th = HaloTile::TH; r->td = HaloTile::TD;
   } else {
     pick_tile(gW, gH, gD, r->tw, r->th, r->td);
   }
@@ -711,6 +665,7 @@ int conv_route(const ConvOp& op, int num_sms, ConvRoute* r) {
   r->KC = conv_kc(op);
   r->BN = conv_bn(op);
   for (int s = 0; s < op.nsrc; ++s) r->kchunks[s] = ceil_div(op.src[s].x.C, r->KC);
+  B200_REQUIRE(!halo || r->kchunks[0] == 1, E_UNSUPPORTED, "igemm_conv: halo mode loads one K chunk of source 0 (%d)", r->kchunks[0]);
   r->npass = split ? 3 : 1;
   r->cls_pair = op.cls_mode && !split ? 1 : 0;
   r->grid[0] = (int)((long long)out.N * r->tiles_d * r->tiles_h * r->tiles_w);
@@ -750,19 +705,15 @@ int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
     a.ntaps[s] = c.ksz * c.ksz * c.ksz; a.ksz[s] = c.ksz; a.stride[s] = c.stride; a.pad[s] = c.nopad ? 0 : c.ksz / 2;
     a.kchunks[s] = r.kchunks[s];
     const int estride = cls ? 1 : c.stride;
-    B200_TRY(make_act_map(&maps.a[s][0], c.x.hi, c.x.N, c.x.D, c.x.H, c.x.W, c.x.C, c.x.ld, KC, a.tw, a.th, a.td,
-                          estride, swz, c.x.vD, c.x.vH, c.x.vW));
+    const bool box = halo && s == 0;   // halo mode: source 0 is one box around the output tile
+    B200_TRY(make_act_map(&maps.a[s][0], c.x.hi, c.x.N, c.x.D, c.x.H, c.x.W, c.x.C, c.x.ld, KC, box ? HaloTile::BW : a.tw,
+                          box ? HaloTile::BH : a.th, box ? HaloTile::BD : a.td, estride, swz, c.x.vD, c.x.vH, c.x.vW));
     B200_TRY(make_w_map(&maps.b[s][0], c.w_hi, a.ntaps[s], op.Cop, c.Cip, KC, BN, swz));
     if (split) {
       B200_TRY(make_act_map(&maps.a[s][1], c.x.lo, c.x.N, c.x.D, c.x.H, c.x.W, c.x.C, c.x.ld, KC, a.tw, a.th, a.td,
                             estride, swz, c.x.vD, c.x.vH, c.x.vW));
       B200_TRY(make_w_map(&maps.b[s][1], c.w_lo, a.ntaps[s], op.Cop, c.Cip, KC, BN, swz));
     }
-  }
-  if (halo) {
-    const ConvSrc& c = op.src[0];
-    B200_TRY(make_act_map(&maps.a[0][0], c.x.hi, c.x.N, c.x.D, c.x.H, c.x.W, c.x.C, c.x.ld, KC, 10, 18, 3, 1, swz, c.x.vD, c.x.vH,
-                          c.x.vW));
   }
   a.npass = r.npass;
   a.mode = op.mode;

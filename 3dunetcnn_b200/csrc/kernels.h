@@ -163,8 +163,6 @@ struct ConvRoute {
 // on a device with num_sms SMs; validates the op: OK or the error launch_igemm_conv would return
 int conv_route(const ConvOp& op, int num_sms, ConvRoute* r);
 int launch_igemm_conv(const ConvOp& op, cudaStream_t st);
-int device_sms();   // SMs of the current device; 132 (an H100 SXM) without one
-bool conv_halo_eligible(const ConvOp& op);   // shape-only: does this convolution run in halo mode?
 
 // ---- tensor-core weight gradient (wgrad.cu):  dW[t][ci][co] += sum_v dy[v][co] * a[v*stride + t - pad][ci]
 struct WgradOp {

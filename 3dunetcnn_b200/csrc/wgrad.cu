@@ -16,10 +16,7 @@
 // reduced into the fp32 gradient buffer with vector atomics.  Split-precision mode: passes (a_hi,dy_hi), (a_lo,dy_hi),
 // (a_hi,dy_lo).
 #include <algorithm>
-#include <cstdlib>
-#include "kernels.h"
-#include "ptx.cuh"
-#include "tmap.h"
+#include "conv_common.cuh"
 
 namespace b200 {
 
@@ -49,12 +46,11 @@ constexpr int WG_A_STAGES = 4;
 constexpr int WG_D_STAGES = 2;
 constexpr int WG_A_BYTES = 32768;
 
-// Halo mode (3x3x3 stride 1, 33..64 input channels, output planes filling an 8 x 16 tile, bf16): per voxel tile ONE TMA halo
-// box (64, 10, 18, 3) of the activation replaces the 27 per-tap boxes; the A operand of tap (kd, kh, kw) is the box read from
-// row kd * 180 + kh * 10 + kw with a K-group stride (SBO) of one 10-voxel halo row (the swizzle follows the absolute
-// shared-memory address, as for the convolution's halo mode).  Two halo buffers: the producer loads the next tile's box while
-// the MMAs of this one run.
-constexpr int WG_HALO_TX = 540 * 128;
+// Halo mode (3x3x3 stride 1, 33..64 input channels, output planes filling the halo tile, bf16): per voxel tile ONE TMA halo
+// box of 64 channels (HaloTile) replaces the 27 per-tap boxes; the A operand of a tap is the box read from the tap's row with a
+// K-group stride (SBO) of one halo row.  Two halo buffers: the producer loads the next tile's box while the MMAs of this one
+// run.
+constexpr int WG_HALO_TX = HaloTile::ROWS * 128;
 constexpr int WG_HALO_BYTES = (WG_HALO_TX + 1023) / 1024 * 1024;
 
 template <int CB, int BN, bool HALO = false>
@@ -181,7 +177,8 @@ __global__ void __launch_bounds__(160, 1) k_wgrad(const __grid_constant__ WgradM
       const uint32_t b_lo = desc_lo(d0s + sd * Cfg::D_STAGE, Cfg::LBO_B);
       if constexpr (HALO) {
         // M half hm of M tile q is unit 2q + hm = one tap of all 64 channels; K step k = output rows h = 2k, 2k + 1
-        constexpr uint32_t hi_h = desc_hi(10 * 128, GMMA_SW128);
+        constexpr uint32_t hi_h = desc_hi(HaloTile::GROUP_STRIDE * 128, GMMA_SW128);
+        constexpr uint32_t K_STEP = 2 * HaloTile::GROUP_STRIDE * (128 >> 4);   // descriptor offset of the next two output rows
         const int kbi = kb - kb0, hb = kbi & 1;
         mbar_wait(&a_full[hb], (kbi >> 1) & 1);
         const uint32_t h_lo = desc_lo(a0 + hb * WG_HALO_BYTES, 16);
@@ -193,14 +190,14 @@ __global__ void __launch_bounds__(160, 1) k_wgrad(const __grid_constant__ WgradM
             for (int hm = 0; hm < 2; ++hm) {
               int u = (q0 + qi) * 2 + hm;
               if (u >= p.units) u = p.units - 1;   // duplicate a valid unit; its rows are never written back
-              off[hm] = ((u / 9) * 180 + ((u / 3) % 3) * 10 + u % 3) * (128 >> 4);
+              off[hm] = HaloTile::tap_row(u) * (128 >> 4);
             }
             wgmma_fence();
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
               const uint64_t db = desc_from(b_lo + ((k * 2 * Cfg::SBO_B) >> 4), hi_b);
-              Wgmma<BN>::template mma<1, 1>(acc[qi][0], desc_from(h_lo + off[0] + k * 20 * (128 >> 4), hi_h), db, 1u);
-              Wgmma<BN>::template mma<1, 1>(acc[qi][1], desc_from(h_lo + off[1] + k * 20 * (128 >> 4), hi_h), db, 1u);
+              Wgmma<BN>::template mma<1, 1>(acc[qi][0], desc_from(h_lo + off[0] + k * K_STEP, hi_h), db, 1u);
+              Wgmma<BN>::template mma<1, 1>(acc[qi][1], desc_from(h_lo + off[1] + k * K_STEP, hi_h), db, 1u);
             }
             wgmma_commit();
           }
@@ -277,62 +274,49 @@ __global__ void __launch_bounds__(160, 1) k_wgrad(const __grid_constant__ WgradM
   }
 }
 
-static void pick_tile_w(int Wo, int Ho, int Do, int& tw, int& th, int& td) {
-  tw = Wo >= 8 ? 8 : Wo >= 4 ? 4 : Wo >= 2 ? 2 : 1;
-  int rem = 128 / tw;
-  th = Ho >= 4 ? 4 : Ho >= 2 ? 2 : 1;
-  if (th > rem) th = rem;
-  td = rem / th;
-}
-
 template <int CB, int BN, bool HALO>
 static int launch_wg(const WgradMaps& maps, const WgradArgs& a, dim3 grid, cudaStream_t st) {
   using Cfg = WgradCfg<CB, BN, HALO>;
-  static bool attr_set[64] = {false};   // once per device: not a stream operation, keep it out of CUDA-graph captures
-  int dev = 0;
-  B200_CHECK_CUDA(cudaGetDevice(&dev));
-  if (dev >= 64 || !attr_set[dev]) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(k_wgrad<CB, BN, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    if (dev < 64) attr_set[dev] = true;
-  }
+  B200_TRY((set_max_dynamic_smem<k_wgrad<CB, BN, HALO>>(Cfg::SMEM_BYTES)));
   launch_pdl(k_wgrad<CB, BN, HALO>, grid, dim3(160), Cfg::SMEM_BYTES, st, maps, a);
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;
 }
 
-// split-K factor of the streaming kernel for this shape (shared by the launcher and the deterministic-mode buffer sizing)
-// halo mode (see WG_HALO_TX); B200UNET_NO_HALO=1 keeps every launch on per-tap boxes (A/B measurements)
+// halo mode (see WG_HALO_TX)
 static bool wgrad_halo_eligible(const WgradOp& op) {
-  static const bool off = getenv("B200UNET_NO_HALO") && atoi(getenv("B200UNET_NO_HALO")) != 0;
   const Act& A = op.a;
   const Act& Y = op.dy;
-  return !off && op.ksz == 3 && op.stride == 1 && !op.nopad && !A.lo && !Y.lo && A.C > 32 && A.C <= 64 && Y.W >= 8 && Y.H >= 16 &&
-         A.D == Y.D && A.H == Y.H && A.W == Y.W;
+  return !halo_disabled() && op.ksz == 3 && op.stride == 1 && !op.nopad && !A.lo && !Y.lo && A.C > 32 && A.C <= 64 &&
+         Y.W >= HaloTile::TW && Y.H >= HaloTile::TH && A.D == Y.D && A.H == Y.H && A.W == Y.W;
 }
 
-static void wgrad_tile(bool halo, const WgradOp& op, int& tw, int& th, int& td) {
-  if (halo) { tw = 8; th = 16; td = 1; }
-  else pick_tile_w(op.dy.W, op.dy.H, op.dy.D, tw, th, td);
-}
-
-static int wgrad_stream_splits(const WgradOp& op, int num_sms, bool halo) {
+// The tiling fields of r for halo tiles or per-tap tiles: voxel tile, CB / BN, M tiles and their CTA groups, N tiles, voxel
+// tiles, the split-K factor and the partial-buffer bytes of deterministic mode.
+static void wgrad_tiling(const WgradOp& op, int num_sms, bool halo, WgradRoute* r) {
   const Act& A = op.a;
   const Act& Y = op.dy;
-  int tw, th, td;
-  wgrad_tile(halo, op, tw, th, td);
+  if (halo) {
+    r->tw = HaloTile::TW; r->th = HaloTile::TH; r->td = HaloTile::TD;
+  } else {
+    pick_tile(Y.W, Y.H, Y.D, r->tw, r->th, r->td);
+  }
   const int ntaps = op.ksz * op.ksz * op.ksz;
-  const int CB = A.C > 32 ? 64 : A.C > 16 ? 32 : 16;
-  const int BN = Y.C > 64 ? 128 : Y.C > 32 ? 64 : Y.C > 16 ? 32 : 16;
-  const int qtiles = ceil_div(ntaps * ceil_div(A.C, CB), 128 / CB);
-  int qt = 128 / BN;   // WgradCfg::QT
-  if (qt > qtiles) qt = qtiles;
-  const int groups = ceil_div(qtiles, qt);
-  const int cotiles = ceil_div(Y.C, BN);
-  const int kblocks = Y.N * ceil_div(Y.D, td) * ceil_div(Y.H, th) * ceil_div(Y.W, tw);
-  int splits = num_sms / (groups * cotiles);
-  if (splits < 1) splits = 1;
-  if (splits > kblocks) splits = kblocks;
-  return splits;
+  r->CB = kc_bucket(A.C);
+  r->BN = bn_bucket(Y.C);
+  r->nci = ceil_div(A.C, r->CB);
+  r->units = ntaps * r->nci;
+  r->qtiles = ceil_div(r->units, 128 / r->CB);
+  r->QT = 128 / r->BN;   // WgradCfg::QT
+  if (r->QT > r->qtiles) r->QT = r->qtiles;
+  r->groups = ceil_div(r->qtiles, r->QT);
+  r->QT = ceil_div(r->qtiles, r->groups);   // rebalance M tiles across groups
+  r->cotiles = ceil_div(Y.C, r->BN);
+  r->kblocks = Y.N * ceil_div(Y.D, r->td) * ceil_div(Y.H, r->th) * ceil_div(Y.W, r->tw);
+  r->splits = num_sms / (r->groups * r->cotiles);
+  if (r->splits < 1) r->splits = 1;
+  if (r->splits > r->kblocks) r->splits = r->kblocks;
+  r->part_bytes = (size_t)r->splits * ntaps * op.Cip * op.Cop * sizeof(float);
 }
 
 __global__ void k_wgrad_reduce(const float4* __restrict__ part, int splits, long long n4, float4* __restrict__ dw) {
@@ -356,19 +340,12 @@ int launch_wgrad_reduce(const float* part, int splits, long long elems, float* d
   return OK;
 }
 
-int device_sms() {
-  int dev = 0, sms = 0;
-  if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && sms > 0)
-    return sms;
-  cudaGetLastError();   // a host without a GPU (route queries, planning)
-  return 132;
-}
-
 size_t wgrad_partial_bytes(const WgradOp& op, int num_sms) {
-  const long long elems = (long long)op.ksz * op.ksz * op.ksz * op.Cip * op.Cop;
   // both tilings: a shape-only op (no lo pointers) cannot tell whether a split-precision launch will take halo mode
-  const int splits = std::max(wgrad_stream_splits(op, num_sms, false), wgrad_halo_eligible(op) ? wgrad_stream_splits(op, num_sms, true) : 0);
-  return (size_t)splits * elems * sizeof(float);
+  WgradRoute tap = {}, halo = {};
+  wgrad_tiling(op, num_sms, false, &tap);
+  if (wgrad_halo_eligible(op)) wgrad_tiling(op, num_sms, true, &halo);
+  return std::max(tap.part_bytes, halo.part_bytes);
 }
 
 template <int CB_, int BN_, bool HALO_>
@@ -423,22 +400,8 @@ int wgrad_route(const WgradOp& op, int num_sms, WgradRoute* r) {
   if (split) B200_REQUIRE(A.lo && Y.lo, E_INVALID, "wgrad: split mode needs lo parts on both operands");
   const bool halo = wgrad_halo_eligible(op);
   r->kind = halo ? WGRAD_KIND_HALO : WGRAD_KIND_TAP;
-  wgrad_tile(halo, op, r->tw, r->th, r->td);
-  const int ntaps = op.ksz * op.ksz * op.ksz;
-  r->CB = A.C > 32 ? 64 : A.C > 16 ? 32 : 16;
-  r->BN = Y.C > 64 ? 128 : Y.C > 32 ? 64 : Y.C > 16 ? 32 : 16;
-  r->nci = ceil_div(A.C, r->CB);
-  r->units = ntaps * r->nci;
-  r->qtiles = ceil_div(r->units, 128 / r->CB);
-  r->QT = 128 / r->BN;   // WgradCfg::QT
-  if (r->QT > r->qtiles) r->QT = r->qtiles;
-  r->groups = ceil_div(r->qtiles, r->QT);
-  r->QT = ceil_div(r->qtiles, r->groups);   // rebalance M tiles across groups
-  r->cotiles = ceil_div(Y.C, r->BN);
-  r->kblocks = Y.N * ceil_div(Y.D, r->td) * ceil_div(Y.H, r->th) * ceil_div(Y.W, r->tw);
-  r->splits = wgrad_stream_splits(op, num_sms, halo);
+  wgrad_tiling(op, num_sms, halo, r);
   r->npass = split ? 3 : 1;
-  r->part_bytes = (size_t)r->splits * ntaps * op.Cip * op.Cop * sizeof(float);
   return with_wgrad_kernel(*r, [](auto) { return (int)OK; });
 }
 
@@ -476,8 +439,9 @@ int launch_wgrad(const WgradOp& op, cudaStream_t st) {
     B200_REQUIRE(r.part_bytes <= op.part_bytes, E_INVALID, "wgrad: deterministic partial buffer too small (%d splits)", r.splits);
     if (op.part_splits) *op.part_splits = r.splits;
   }
-  if (halo)   // one (64, 10, 18, 3) box around the 8 x 16 x 1 voxel tile; the zero padding is TMA out-of-bounds fill
-    B200_TRY(make_act_map(&maps.a[0], A.hi, A.N, A.D, A.H, A.W, A.C, A.ld, 64, 10, 18, 3, 1, SWZ_128, A.vD, A.vH, A.vW));
+  if (halo)   // one 64-channel halo box around the voxel tile (HaloTile)
+    B200_TRY(make_act_map(&maps.a[0], A.hi, A.N, A.D, A.H, A.W, A.C, A.ld, 64, HaloTile::BW, HaloTile::BH, HaloTile::BD, 1, SWZ_128,
+                          A.vD, A.vH, A.vW));
   else
     B200_TRY(make_act_map(&maps.a[0], A.hi, A.N, A.D, A.H, A.W, A.C, A.ld, CB, a.tw, a.th, a.td, op.stride,
                           swz_for_bytes(CB * 2), A.vD, A.vH, A.vW));

@@ -8,14 +8,12 @@ against an fp64 reference after checking that it still takes its route.  The que
 so the sweep passes placeholder addresses.
 """
 import itertools
-import os
 from dataclasses import dataclass
 from typing import Tuple
 
 CHANNELS = (8, 16, 24, 32, 40, 64, 72, 128, 192, 256)
 SMALL_PLANE = (3, 5, 7)        # output extents (d, h, w): per-tap tiles only
 LARGE_PLANE = (2, 16, 8)       # output plane of at least 8 x 16: fills the halo tile
-WIDE_ENV = "B200UNET_HALO_WIDE_MIN"
 
 
 def kc_of(c: int) -> int:
@@ -50,8 +48,7 @@ class Addr:
 class ConvCase:
     """op: k3s1 | k3s2 | k1 (forward conv), class1 (data gradient of a k3s2 conv: source = dY at half the output extent) or
     class2 (ConvTranspose3d, kernel = stride = 2).  cin / cout: channels of source 0 / of the output view; cin2 > 0 adds a
-    fused 1x1x1 second source; dims: output extents (d, h, w); wide: B200UNET_HALO_WIDE_MIN=0.  The remaining fields are the
-    route it must take."""
+    fused 1x1x1 second source; dims: output extents (d, h, w).  The remaining fields are the route it must take."""
     kind: str
     bn: int
     kc: int
@@ -63,7 +60,6 @@ class ConvCase:
     cout: int
     dims: Tuple[int, int, int]
     cin2: int = 0
-    wide: bool = False
     kchunks: Tuple[int, int] = (1, 0)
 
     @property
@@ -113,36 +109,16 @@ def conv_query(L, op, cin, cout, dims, split=False, mode=0, cin2=0, n=2):
         return None
 
 
-def with_wide_env(wide, fn):
-    old = os.environ.get(WIDE_ENV)
-    if wide:
-        os.environ[WIDE_ENV] = "0"
-    else:
-        os.environ.pop(WIDE_ENV, None)
-    try:
-        return fn()
-    finally:
-        if old is None:
-            os.environ.pop(WIDE_ENV, None)
-        else:
-            os.environ[WIDE_ENV] = old
-
-
 def conv_sweep(L):
     """every (shape, options, route) of the sweep: yields (params dict, route dict)"""
     ops = {"k3s1": (SMALL_PLANE, LARGE_PLANE), "k3s2": (SMALL_PLANE, LARGE_PLANE), "k1": (SMALL_PLANE, LARGE_PLANE),
            "class1": ((4, 6, 8), (2, 32, 16)), "class2": ((4, 6, 8), (2, 32, 16))}
-    for wide in (False, True):
-        def run():
-            res = []
-            for op, planes in ops.items():
-                second = (0,) if op.startswith("class") else (0,) + CHANNELS
-                for dims, cin, cout, cin2, split, mode in itertools.product(planes, CHANNELS, CHANNELS, second, (False, True), (0, 1)):
-                    r = conv_query(L, op, cin, cout, dims, split, mode, cin2)
-                    if r is not None:
-                        res.append((dict(op=op, dims=dims, cin=cin, cout=cout, cin2=cin2, split=split, mode=mode, wide=wide), r))
-            return res
-        yield from with_wide_env(wide, run)
+    for op, planes in ops.items():
+        second = (0,) if op.startswith("class") else (0,) + CHANNELS
+        for dims, cin, cout, cin2, split, mode in itertools.product(planes, CHANNELS, CHANNELS, second, (False, True), (0, 1)):
+            r = conv_query(L, op, cin, cout, dims, split, mode, cin2)
+            if r is not None:
+                yield dict(op=op, dims=dims, cin=cin, cout=cout, cin2=cin2, split=split, mode=mode), r
 
 
 def route_key_of(params, r):
@@ -277,9 +253,9 @@ CONV_CASES = [
     _C("halo", 64, 32, False, 0, 2, "k3s1", 24, 40, H, cin2=40, kchunks=(1, 2)),
     _C("halo", 64, 32, False, 1, 1, "k3s1", 24, 40, H),
     _C("halo", 64, 32, False, 1, 2, "k3s1", 24, 40, H, cin2=16, kchunks=(1, 1)),
-    _C("halo", 64, 64, False, 0, 1, "k3s1", 136, 40, H, wide=True, kchunks=(3, 0)),
+    _C("halo", 64, 64, False, 0, 1, "k3s1", 64, 40, H),
     _C("halo", 64, 64, False, 0, 2, "k3s1", 40, 40, H, cin2=72, kchunks=(1, 2)),
-    _C("halo", 64, 64, False, 1, 1, "k3s1", 72, 40, H, wide=True, kchunks=(2, 0)),
+    _C("halo", 64, 64, False, 1, 1, "k3s1", 40, 40, H),
     _C("halo", 64, 64, False, 1, 2, "k3s1", 40, 40, H, cin2=24, kchunks=(1, 1)),
     _C("halo", 128, 16, False, 0, 1, "k3s1", 16, 200, H),
     _C("halo", 128, 16, False, 0, 2, "k3s1", 8, 200, H, cin2=64, kchunks=(1, 4)),
@@ -289,9 +265,9 @@ CONV_CASES = [
     _C("halo", 128, 32, False, 0, 2, "k3s1", 24, 200, H, cin2=40, kchunks=(1, 2)),
     _C("halo", 128, 32, False, 1, 1, "k3s1", 24, 200, H),
     _C("halo", 128, 32, False, 1, 2, "k3s1", 24, 200, H, cin2=16, kchunks=(1, 1)),
-    _C("halo", 128, 64, False, 0, 1, "k3s1", 136, 200, H, wide=True, kchunks=(3, 0)),
+    _C("halo", 128, 64, False, 0, 1, "k3s1", 64, 200, H),
     _C("halo", 128, 64, False, 0, 2, "k3s1", 40, 200, H, cin2=72, kchunks=(1, 2)),
-    _C("halo", 128, 64, False, 1, 1, "k3s1", 72, 200, H, wide=True, kchunks=(2, 0)),
+    _C("halo", 128, 64, False, 1, 1, "k3s1", 40, 200, H),
     _C("halo", 128, 64, False, 1, 2, "k3s1", 40, 200, H, cin2=24, kchunks=(1, 1)),
     _C("class1", 16, 16, False, 0, 1, "class1", 16, 8, CL),
     _C("class1", 16, 16, True, 0, 1, "class1", 8, 8, CL),

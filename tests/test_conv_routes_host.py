@@ -58,7 +58,7 @@ def test_every_reachable_conv_route_has_a_case(conv_sweep):
 
 @pytest.mark.parametrize("case", R.CONV_CASES, ids=lambda c: c.id)
 def test_conv_case_takes_its_route(L, case):
-    r = R.with_wide_env(case.wide, lambda: R.conv_query(L, case.op, case.cin, case.cout, case.dims, case.split, case.mode, case.cin2))
+    r = R.conv_query(L, case.op, case.cin, case.cout, case.dims, case.split, case.mode, case.cin2)
     assert r is not None, "the library refuses the case"
     assert (r["kind"], r["bn"], r["kc"]) == (case.kind, case.bn, case.kc)
     assert r["kchunks"] == case.kchunks
@@ -77,7 +77,7 @@ def test_conv_case_takes_its_route(L, case):
 
 def test_kc64_cases_walk_several_k_chunks_in_every_kind():
     kinds = {c.kind for c in R.CONV_CASES if c.kc == 64 and c.kchunks[0] > 1}
-    assert kinds == {"tap", "halo", "class1", "class2"}
+    assert kinds == {"tap", "class1", "class2"}           # halo mode loads one K chunk of its 3x3x3 source
     assert any(c.kind == "halo" and c.nsrc == 2 and c.kchunks[1] > 1 for c in R.CONV_CASES), "wide second source in halo mode"
     assert any(c.kind == "tap" and c.nsrc == 2 and c.kchunks[1] > 1 for c in R.CONV_CASES), "wide second source on per-tap tiles"
     assert any(c.kind == "halo" and c.mode == 1 and c.bn <= 32 for c in R.CONV_CASES), "mode 1 on the halo kernel at BN <= 32"
@@ -104,11 +104,24 @@ def test_halo_mode_never_costs_occupancy(L, conv_sweep):
     for p, r in conv_sweep:
         if r["kind"] != "halo":
             continue
-        tap = R.with_wide_env(p["wide"], lambda: R.conv_query(L, "k3s1", p["cin"], p["cout"], R.SMALL_PLANE, p["split"], p["mode"], p["cin2"]))
+        tap = R.conv_query(L, "k3s1", p["cin"], p["cout"], R.SMALL_PLANE, p["split"], p["mode"], p["cin2"])
         assert tap["kind"] == "tap" and (tap["bn"], tap["kc"]) == (r["bn"], r["kc"])
         assert r["blocks_per_sm"] >= tap["blocks_per_sm"], (p, r["blocks_per_sm"], tap["blocks_per_sm"])
         checked += 1
     assert checked > 0
+
+
+def test_halo_mode_reads_one_k_chunk_of_its_3x3x3_source(L, conv_sweep):
+    """the halo box holds one K chunk: every halo route of the sweep has kchunks[0] == 1, and a 3x3x3 source wider than 64
+    channels on a plane that fills the halo tile runs on per-tap tiles in both precisions"""
+    halo = [(p, r) for p, r in conv_sweep if r["kind"] == "halo"]
+    assert halo
+    for p, r in halo:
+        assert r["kchunks"][0] == 1, (p, r)
+    for cin in (72, 128, 256):
+        for split in (False, True):
+            r = R.conv_query(L, "k3s1", cin, 64, R.LARGE_PLANE, split)
+            assert r["kind"] == "tap" and r["kchunks"][0] > 1, (cin, split, r)
 
 
 def test_conv_configurations_fit_shared_memory(conv_sweep):

@@ -150,9 +150,9 @@ def run_mode0(L, case, gen, ext=None, edit_ref=None):
     stats = torch.zeros(n, C0 + case.cout + 8, 2, dtype=torch.float64, device=DEV)
     kw.update(res=res, scale=scale, stats=stats[:, C0:], stats_ld=C0 + case.cout + 8)
     x, whi, wlo, ksz, stride = args
-    route = R.with_wide_env(case.wide, lambda: L.conv3d_route(x, whi, wlo, ksz, stride, out, case.cout, case.cin, ext=ext, **kw))
+    route = L.conv3d_route(x, whi, wlo, ksz, stride, out, case.cout, case.cin, ext=ext, **kw)
     assert_route(route, case)
-    R.with_wide_env(case.wide, lambda: L.conv3d_ex(x, whi, wlo, ksz, stride, out, case.cout, case.cin, ext=ext, **kw))
+    L.conv3d_ex(x, whi, wlo, ksz, stride, out, case.cout, case.cin, ext=ext, **kw)
     torch.cuda.synchronize()
     s = scale.double().cpu()[:, :real_out, None, None, None]
     ref = (acc + resv) * s
@@ -192,9 +192,9 @@ def run_mode1(L, case, gen, slope):
     dz.hi.fill_(SENTINEL)
     kw.update(mode=1, gn_x=gx, coef=coef, coef_ld=case.cout, slope=slope, bstats=bst)
     x, whi, wlo, ksz, stride = args
-    route = R.with_wide_env(case.wide, lambda: L.conv3d_route(x, whi, wlo, ksz, stride, dz, case.cout, case.cin, **kw))
+    route = L.conv3d_route(x, whi, wlo, ksz, stride, dz, case.cout, case.cin, **kw)
     assert_route(route, case)
-    R.with_wide_env(case.wide, lambda: L.conv3d(x, whi, wlo, ksz, stride, dz, case.cout, case.cin, **kw))
+    L.conv3d(x, whi, wlo, ksz, stride, dz, case.cout, case.cin, **kw)
     torch.cuda.synchronize()
     xq = gxv.clone().requires_grad_(True)
     z = F.group_norm(xq, G, gamma.double().cpu(), beta.double().cpu(), 1e-5)

@@ -36,7 +36,7 @@ def _packed_to_torch(L, w, mode, split, cout, cin, ksz):
 
 
 # the forward shapes below that run on the halo kernel in bf16; (64, 32) has KC = 64 with BN = 32 and stays on per-tap tiles
-# (halo_keeps_occupancy), inputs wider than 64 channels unless B200UNET_HALO_WIDE_MIN allows them
+# (halo_keeps_occupancy), and so do inputs wider than 64 channels (the halo box holds one K chunk)
 HALO_FORWARD = {(32, 32, (8, 16, 16)), (8, 32, (16, 16, 16)), (24, 40, (6, 18, 12)), (32, 64, (5, 24, 20)), (16, 16, (1, 16, 8))}
 
 
@@ -78,11 +78,9 @@ def test_conv3d_forward(pkg, cin, cout, dims, ksz, stride, split):
     (128, 128, (4, 16, 8), "plain"), (256, 192, (2, 16, 16), "plain"), (96, 160, (6, 16, 8), "plain"),
     (128, 128, (5, 16, 16), "res"), (256, 256, (3, 16, 8), "res"),
 ])
-def test_conv3d_wide_inputs_on_halo_kernel(pkg, monkeypatch, cin, cout, dims, mode, split):
-    """Cin >= 128 in halo mode (bf16; several N tiles per voxel tile, 2-4 halo boxes per tile).  That dispatch is off by
-    default and enabled here through B200UNET_HALO_WIDE_MIN so that it stays correct.  Split precision runs on per-tap
-    tiles."""
-    monkeypatch.setenv("B200UNET_HALO_WIDE_MIN", "0")
+def test_conv3d_wide_inputs_on_large_planes_per_tap_tiles(pkg, cin, cout, dims, mode, split):
+    """Cin >= 96 on output planes that fill the halo tile: per-tap tiles in both precisions (several K chunks per tap, several
+    N tiles per voxel tile), with the statistics."""
     L = pkg.lib
     torch.manual_seed(cin * 3 + cout)
     n = 2
@@ -93,7 +91,7 @@ def test_conv3d_wide_inputs_on_halo_kernel(pkg, monkeypatch, cin, cout, dims, mo
     y = L.Act.empty(n, *dims, cop, split=split, zero=True)
     stats = torch.zeros(n, cop, 2, dtype=torch.float64, device=DEV)
     ref = F.conv3d(a.to_ncdhw(cin).double().cpu(), wq, padding=1)
-    assert L.conv3d_route(a, whi, wlo, 3, 1, y, cop, cip)["kind"] == ("tap" if split else "halo")
+    assert L.conv3d_route(a, whi, wlo, 3, 1, y, cop, cip)["kind"] == "tap"
     if mode == "res":
         assert cop == cout                                   # the shapes above need no channel padding
         r = L.Act.from_ncdhw(torch.randn(n, cout, *dims, device=DEV), split=split)
@@ -108,10 +106,9 @@ def test_conv3d_wide_inputs_on_halo_kernel(pkg, monkeypatch, cin, cout, dims, mo
 
 @pytest.mark.parametrize("split", [False, True])
 @pytest.mark.parametrize("ci,co,dims", [(128, 128, (4, 16, 8)), (192, 256, (2, 16, 16)), (128, 96, (5, 16, 8))])
-def test_conv3d_wide_inputs_on_halo_kernel_gn_backward_epilogue_on_fused_coefficients(pkg, monkeypatch, ci, co, dims, split):
-    """The same wide-input halo-mode dispatch with the mode-1 (GroupNorm/ReLU backward) epilogue: the data gradient of a
-    co -> ci ... convolution seen from its output side, i.e. K = co >= 128 input channels of the GEMM."""
-    monkeypatch.setenv("B200UNET_HALO_WIDE_MIN", "0")
+def test_conv3d_wide_inputs_on_large_planes_per_tap_tiles_gn_backward_epilogue(pkg, ci, co, dims, split):
+    """The same wide inputs on per-tap tiles with the mode-1 (GroupNorm/ReLU backward) epilogue: the data gradient of a
+    co -> ci ... convolution seen from its output side, i.e. K = co >= 96 input channels of the GEMM."""
     L = pkg.lib
     torch.manual_seed(ci + 2 * co)
     n, G = 2, 8
@@ -127,7 +124,7 @@ def test_conv3d_wide_inputs_on_halo_kernel_gn_backward_epilogue_on_fused_coeffic
     bst = torch.zeros(n, ci, 2, dtype=torch.float64, device=DEV)
     dz = L.Act.empty(n, *dims, ci, split=split)
     mode1 = dict(mode=1, gn_x=x, coef=coef, coef_ld=ci, bstats=bst)
-    assert L.conv3d_route(dy, wdh, wdl, 3, 1, dz, ci, co, **mode1)["kind"] == ("tap" if split else "halo")
+    assert L.conv3d_route(dy, wdh, wdl, 3, 1, dz, ci, co, **mode1)["kind"] == "tap"
     L.conv3d(dy, wdh, wdl, 3, 1, dz, ci, co, **mode1)
     xq = x.to_ncdhw(ci).double().cpu().requires_grad_(True)
     z = F.group_norm(xq, G, gamma.double().cpu(), beta.double().cpu(), 1e-5)
