@@ -85,7 +85,7 @@ using namespace b200;
 
 extern "C" {
 
-int b200unet_version(void) { return 101; }
+int b200unet_version(void) { return 102; }
 const char* b200unet_last_error(void) { return get_error(); }
 
 int b200unet_ncdhw_to_ndhwc(const float* x, int c_real, const b200unet_tensor* out, void* stream) {

@@ -53,7 +53,6 @@ struct RunCtx {
   struct Prof* prof;
   const char* label = nullptr;     // name of the op being launched (profiling only)
   bool skip_pack = false;          // the packed bf16 weights in the workspace are current (parameters unchanged since the last forward)
-  int part = -1;                   // backward only: -1 = the whole schedule; 0 / 1 = the part b200unet_plan_backward_part runs
   RunCtx(void* workspace, void* stream, struct Prof* p)
       : ws(reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~uintptr_t(1023))),
         st(reinterpret_cast<cudaStream_t>(stream)), prof(p) {}
@@ -146,11 +145,6 @@ struct b200unet_plan {
   size_t wg_part_off = 0, wg_part_bytes = 0;   // scratch shared by all weight-gradient launches (stream-ordered)
   float slope = 0.f;        // negative slope of the activation (0 = ReLU: UNet3D; 0.01 = LeakyReLU: DynUNet)
   bool infer = false;       // forward-only plan: no backward schedule / buffers, forward temporaries are recycled
-  // two-part backward (b200unet_plan_backward_part): part 0 = head, decoder and the deepest encoder level(s) -- most of the
-  // parameters -- whose gradients can be exchanged between ranks while part 1 (the shallow encoder levels) still runs
-  int bwd_split = -1;                 // index into bwd of the first op of part 1 (-1: one part)
-  std::vector<int> param_last_op;     // per parameter: index of the last backward op that contributes to its gradient
-  size_t unpack_split = 0;            // unpack jobs [0, unpack_split) belong to part 0
   std::vector<std::pair<size_t, std::pair<size_t, size_t>>> free_bufs;   // (bytes, (off_hi, off_lo)) of released buffers
 
   size_t alloc(size_t bytes) {
@@ -168,18 +162,6 @@ struct b200unet_plan {
 namespace b200 {
 
 typedef b200unet_plan Plan;
-
-// the backward op about to be pushed contributes to the gradient of parameter `pidx`
-static void touch(Plan& P, int pidx) {
-  if (pidx < 0) return;
-  if (P.param_last_op.size() < P.params.size()) P.param_last_op.resize(P.params.size(), -1);
-  P.param_last_op[pidx] = (int)P.bwd.size();
-}
-static int param_part(const Plan& P, int pidx) {
-  if (P.bwd_split < 0) return 0;
-  if (pidx < 0 || pidx >= (int)P.param_last_op.size() || P.param_last_op[pidx] < 0) return 1;   // unknown writer: final only at the end
-  return P.param_last_op[pidx] < P.bwd_split ? 0 : 1;
-}
 
 static int groups_for(int c, int norm_groups) { return (c < norm_groups || c % norm_groups) ? c : norm_groups; }
 
@@ -470,7 +452,6 @@ static int run_wgrad(Plan& P, RunCtx& cx, WgradOp& op) {
 static void emit_wgrad(Plan& P, int ci, TRef a, TRef dy) {
   P.macs[CAT_CONV_WGRAD] += conv_macs(P, ci, dy);
   size_wgrad_partials(P, shape_act(P, a), shape_act(P, dy), P.convs[ci].ksz, P.convs[ci].stride, 0, P.convs[ci].Cip, P.convs[ci].Cop);
-  touch(P, P.convs[ci].pw);
   push_op(P.bwd, "wgrad " + P.convs[ci].name + " " + shape_of(P, a) + " x " + shape_of(P, dy), [&P, ci, a, dy](RunCtx& cx) -> int {
     const ConvLayer& c = P.convs[ci];
     WgradOp op;
@@ -518,8 +499,6 @@ static void emit_dgrad(Plan& P, int ci, TRef dy, TRef out, int ni, TRef gn_x, TR
 }
 
 static void emit_gn_bwd_finalize(Plan& P, int ni) {
-  touch(P, P.norms[ni].pg);
-  touch(P, P.norms[ni].pb);
   push_op(P.bwd, "gn_bwd_finalize " + P.norms[ni].name, [&P, ni](RunCtx& cx) -> int {
     const NormLayer& n = P.norms[ni];
     LAUNCHED(cx, CAT_NORM, launch_gn_bwd_finalize(reinterpret_cast<double*>(cx.ws + P.bz_off + n.bstats),
@@ -531,8 +510,6 @@ static void emit_gn_bwd_finalize(Plan& P, int ni) {
 }
 
 static void emit_gn_bwd(Plan& P, int ni, TRef dz, TRef x, TRef add1, TRef dx, bool scale) {
-  touch(P, P.norms[ni].pg);
-  touch(P, P.norms[ni].pb);
   push_op(P.bwd, "gn_bwd " + P.norms[ni].name + " " + shape_of(P, x), [&P, ni, dz, x, add1, dx, scale](RunCtx& cx) -> int {
     const NormLayer& n = P.norms[ni];
     Act a1;
@@ -598,8 +575,6 @@ static TRef emit_head(Plan& P, TRef Xfinal, int w_param, int bias_param) {
   if (P.infer) return kNone;
   const Buf xb = P.bufs[Xfinal.buf];
   const TRef g = full(P, new_buf(P, xb.N, xb.D, xb.H, xb.W, Xfinal.c));
-  touch(P, w_param);
-  touch(P, bias_param);
   push_op(P.bwd, "head_bwd", [&P, Xfinal, g, bias_param](RunCtx& cx) -> int {
     float* scratch = reinterpret_cast<float*>(cx.ws + P.head_part_off);
     const bool fused_dbias = bias_param >= 0 && P.d.n_outputs > 8;
@@ -615,26 +590,11 @@ static TRef emit_head(Plan& P, TRef Xfinal, int w_param, int bias_param) {
   return g;
 }
 
-// Everything pushed so far is part 0 of a two-part backward.  The op pushed here unpacks the weight gradients of part 0
-// (accumulator -> torch layout) and runs only under b200unet_plan_backward_part(part = 0): the whole-schedule call unpacks
-// every job in its last op (emit_unpack_wgrads).
-static void emit_bwd_split(Plan& P) {
-  push_op(P.bwd, "unpack_wgrads (part 0)", [&P](RunCtx& cx) -> int {
-    if (cx.part != 0 || P.unpack_split == 0) return OK;
-    const PackJob* jobs = reinterpret_cast<const PackJob*>(cx.ws + P.jobs_off) + P.pack_jobs.size();
-    LAUNCHED(cx, CAT_PACK, launch_unpack_all(ptr_table(P, cx.grads), jobs, (int)P.unpack_split, cx.ws, cx.st));
-    return OK;
-  });
-  P.bwd_split = (int)P.bwd.size();
-}
-
 // last op of every backward: weight gradients, accumulator -> torch layout (one batched launch)
 static void emit_unpack_wgrads(Plan& P) {
   push_op(P.bwd, "unpack_wgrads", [&P](RunCtx& cx) -> int {
-    // run as part 1 of a two-part backward, the jobs of part 0 were unpacked at the split (emit_bwd_split)
-    const size_t first = cx.part == 1 ? P.unpack_split : 0;
-    const PackJob* jobs = reinterpret_cast<const PackJob*>(cx.ws + P.jobs_off) + P.pack_jobs.size() + first;
-    LAUNCHED(cx, CAT_PACK, launch_unpack_all(ptr_table(P, cx.grads), jobs, (int)(P.unpack_jobs.size() - first), cx.ws, cx.st));
+    const PackJob* jobs = reinterpret_cast<const PackJob*>(cx.ws + P.jobs_off) + P.pack_jobs.size();
+    LAUNCHED(cx, CAT_PACK, launch_unpack_all(ptr_table(P, cx.grads), jobs, (int)P.unpack_jobs.size(), cx.ws, cx.st));
     return OK;
   });
 }
@@ -883,7 +843,6 @@ static int build_unet3d(Plan& P) {
       // the padded boundary of the ConvT output is a constant: mask it out of dU (visible extent 2n-1 through TMA)
       TRef dUm = masked(dU);
       const int cup = s.cup;
-      touch(P, P.convs[cup].pb);
       push_op(P.bwd, "bias_grad " + P.convs[cup].name, [&P, dUm, cup](RunCtx& cx) -> int {
         LAUNCHED(cx, CAT_OTHER, launch_bias_grad(act_of(P, cx, dUm), cx.grads[P.convs[cup].pb], cx.st));
         return OK;
@@ -900,9 +859,6 @@ static int build_unet3d(Plan& P) {
     if (li > 0) {
       const int lj = li - 1;
       emit_wgrad(P, down[lj], skip[lj], g);
-      // head, decoder and the deepest encoder level are done: ~90 % of the parameters (C2: 21.4 M of 24.0 M) have their
-      // gradients, ~25 % of the backward time is still ahead
-      if (li == L - 1) emit_bwd_split(P);
       TRef gin = g;
       TRef gS = full(P, new_buf(P, N, Ds[lj], Hs[lj], Ws[lj], widths[lj]));
       // dropout scale belongs to the output of encoder block (0,0): that is this tensor iff level 0 has one block
@@ -948,9 +904,7 @@ static int finish_build(Plan& P) {
     if (c.up2) {   // accumulated with swapped roles as [T][pad(Co)][pad(Ci)] (see emit_wgrad_up2): reads back as [Ci][Co][T]
       u.mode = 0; u.Co = c.Ci; u.Ci = c.Co; u.Cop = c.Cip; u.Cip = c.Cop;
     }
-    // the jobs of part 0 of a two-part backward first (b200unet_plan_backward_part), the others behind them
-    if (param_part(P, c.pw) == 0 && P.bwd_split >= 0) P.unpack_jobs.insert(P.unpack_jobs.begin() + P.unpack_split++, u);
-    else P.unpack_jobs.push_back(u);
+    P.unpack_jobs.push_back(u);
   }
   P.jobs_off = P.alloc(sizeof(PackJob) * (P.pack_jobs.size() + P.unpack_jobs.size()));
   return OK;
@@ -1156,7 +1110,6 @@ static int build_dynunet(Plan& P) {
     const TRef Xlow = (lo == L - 1) ? enc[lo].out : dec[lo].out;
     P.macs[CAT_CONV_WGRAD] += (double)N * Ds[lo] * Hs[lo] * Ws[lo] * F[lo] * F[hi] * 8;
     size_wgrad_partials(P, shape_act(P, dU), shape_act(P, Xlow), 2, 2, 1, P.convs[ci].Cop, P.convs[ci].Cip);
-    touch(P, P.convs[ci].pw);
     push_op(P.bwd, "wgrad_up2 " + P.convs[ci].name, [&P, ci, Xlow, dU](RunCtx& cx) -> int {
       // dW[ci][co][t] = sum_j X[j][ci] dU[2j + t][co]: the weight gradient of the kernel-2 stride-2 convolution that maps the
       // FINE grid (dU, "input", channels co) to the COARSE grid (X, "output gradient", channels ci): accumulator [T][pad(Co)][pad(Ci)]
@@ -1192,8 +1145,6 @@ static int build_dynunet(Plan& P) {
     TRef g1 = (i == L - 1) ? g : dskip[i];
     TRef g2 = (i == L - 1) ? kNone : gdown;
     gdown = build_dyn_block_bwd(P, enc[i], g1, g2);
-    // decoder, bottleneck and (six-level nets) the level above it are done
-    if (i == (L >= 4 ? L - 2 : L - 1) && i > 0) emit_bwd_split(P);
   }
   emit_unpack_wgrads(P);
   return finish_build(P);
@@ -1286,26 +1237,14 @@ int b200unet_plan_forward(b200unet_plan* plan, const float* x, const float* cons
   return run_ops(*plan, plan->fwd, 0, plan->fwd.size(), cx, "plan_forward");
 }
 
-static int run_backward(b200unet_plan* plan, const float* dlogits, const float* const* params, float* const* grads, void* workspace,
-                        void* stream, int part) {
-  if (!plan || !dlogits || !params || !grads || !workspace) { set_error("plan_backward: null argument"); return E_INVALID; }
-  if (plan->infer) { set_error("plan_backward: this plan was created with inference_only=1 (no backward schedule)"); return E_INVALID; }
-  if (part >= 0 && (plan->bwd_split < 0 || part > 1)) {
-    set_error("plan_backward_part: part %d of a schedule with %d part(s)", part, plan->bwd_split < 0 ? 1 : 2);
-    return E_INVALID;
-  }
-  RunCtx cx(workspace, stream, plan->prof);
-  cx.params = params; cx.grads = grads; cx.dlogits = dlogits;
-  cx.part = part;
-  if (plan->have_drop) cx.drop = reinterpret_cast<float*>(cx.ws + plan->drop_off);
-  const size_t first = part == 1 ? (size_t)plan->bwd_split : 0;
-  const size_t last = part == 0 ? (size_t)plan->bwd_split : plan->bwd.size();
-  return run_ops(*plan, plan->bwd, first, last, cx, "plan_backward");
-}
-
 int b200unet_plan_backward(b200unet_plan* plan, const float* dlogits, const float* const* params, float* const* grads,
                            void* workspace, void* stream) {
-  return run_backward(plan, dlogits, params, grads, workspace, stream, -1);
+  if (!plan || !dlogits || !params || !grads || !workspace) { set_error("plan_backward: null argument"); return E_INVALID; }
+  if (plan->infer) { set_error("plan_backward: this plan was created with inference_only=1 (no backward schedule)"); return E_INVALID; }
+  RunCtx cx(workspace, stream, plan->prof);
+  cx.params = params; cx.grads = grads; cx.dlogits = dlogits;
+  if (plan->have_drop) cx.drop = reinterpret_cast<float*>(cx.ws + plan->drop_off);
+  return run_ops(*plan, plan->bwd, 0, plan->bwd.size(), cx, "plan_backward");
 }
 
 int b200unet_plan_input_grad(b200unet_plan* plan, float* dx, void* workspace, void* stream) {
@@ -1314,19 +1253,6 @@ int b200unet_plan_input_grad(b200unet_plan* plan, float* dx, void* workspace, vo
   RunCtx cx(workspace, stream, plan->prof);
   cx.dx = dx;
   return run_ops(*plan, plan->igrad, 0, plan->igrad.size(), cx, "plan_input_grad");
-}
-
-int b200unet_plan_backward_parts(const b200unet_plan* plan) { return (!plan || plan->infer) ? 0 : plan->bwd_split >= 0 ? 2 : 1; }
-
-int b200unet_plan_param_backward_part(const b200unet_plan* plan, int i) {
-  if (!plan || i < 0 || i >= (int)plan->params.size()) return -1;
-  return param_part(*plan, i);
-}
-
-int b200unet_plan_backward_part(b200unet_plan* plan, int part, const float* dlogits, const float* const* params, float* const* grads,
-                                void* workspace, void* stream) {
-  if (part < 0) { set_error("plan_backward_part: part %d", part); return E_INVALID; }
-  return run_backward(plan, dlogits, params, grads, workspace, stream, part);
 }
 
 int b200unet_plan_last_launches(const b200unet_plan* plan) { return plan ? plan->last_launches : 0; }

@@ -158,10 +158,6 @@ _SIGS = {
     "b200unet_plan_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                          C.c_void_p, C.c_void_p]),
     "b200unet_plan_input_grad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "b200unet_plan_backward_parts": (C.c_int, [C.c_void_p]),
-    "b200unet_plan_param_backward_part": (C.c_int, [C.c_void_p, C.c_int]),
-    "b200unet_plan_backward_part": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
-                                              C.c_void_p, C.c_void_p]),
     "b200unet_plan_last_launches": (C.c_int, [C.c_void_p]),
     "b200unet_plan_algorithmic_macs": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.c_int]),
     "b200unet_plan_profile_begin": (C.c_int, [C.c_void_p, C.c_int]),

@@ -71,16 +71,6 @@ class _Plan:
     def last_launches(self) -> int:
         return int(self.lib.b200unet_plan_last_launches(self.handle))
 
-    def backward_parts(self) -> int:
-        """2 when the backward schedule can run as two calls (``b200unet_plan_backward_part``), else 1 (0: forward-only plan)"""
-        return int(self.lib.b200unet_plan_backward_parts(self.handle))
-
-    def param_parts(self):
-        """per parameter (state-dict order): the backward part after which its gradient is final"""
-        if self.backward_parts() != 2:
-            return [0] * self.n_params
-        return [int(self.lib.b200unet_plan_param_backward_part(self.handle, i)) for i in range(self.n_params)]
-
     CATEGORIES = ("conv_fwd", "conv_dgrad", "conv_wgrad", "norm_act", "resample", "head", "weight_pack", "other")
 
     def algorithmic_macs(self):
@@ -170,18 +160,9 @@ class _UNetFunction(torch.autograd.Function):
         dlogits = dlogits.contiguous().float()
         dx = None
         with torch.cuda.device(dlogits.device):
-            grads, direct = model._grad_targets(params, plan)
-            # the input gradient reads what the whole backward leaves in the workspace: never deferred
-            if model._defer_backward_tail and direct and not need_dx and plan.backward_parts() == 2:
-                # two-part backward (train.GraphedTrainStep with a gradient exchange): part 0 -- head, decoder, deepest encoder
-                # level -- runs here; the caller runs the rest through finish_backward() after it has started the exchange of
-                # the gradients that are final now (model.flat_gradient_bucket_parts()[0])
-                _lib.check(plan.lib.b200unet_plan_backward_part(plan.handle, 0, dlogits.data_ptr(), _ptr_array(params), _ptr_array(grads),
-                                                                plan.workspace.data_ptr(), _lib.stream_ptr()), "plan_backward_part(0)")
-                model._backward_tail = (plan, dlogits, params, grads)
-            else:
-                _lib.check(plan.lib.b200unet_plan_backward(plan.handle, dlogits.data_ptr(), _ptr_array(params), _ptr_array(grads),
-                                                           plan.workspace.data_ptr(), _lib.stream_ptr()), "plan_backward")
+            grads, direct = model._grad_targets(params)
+            _lib.check(plan.lib.b200unet_plan_backward(plan.handle, dlogits.data_ptr(), _ptr_array(params), _ptr_array(grads),
+                                                       plan.workspace.data_ptr(), _lib.stream_ptr()), "plan_backward")
             model.launches_last_backward = plan.last_launches()
             if need_dx:
                 n, _, d, h, w = dlogits.shape
@@ -216,10 +197,6 @@ class _PlanModel(nn.Module):
         self._flat_grads = False
         self._grad_bucket: Optional[torch.Tensor] = None
         self._grad_views = None
-        self._bucket_split = None        # elements of the bucket that belong to part 0 of a two-part backward
-        self._param_parts = None         # per parameter: backward part after which its gradient is final (from the plan)
-        self._defer_backward_tail = False
-        self._backward_tail = None
         self._keys = []
         spec = self._param_spec_cpu()
         shapes = dict(spec)
@@ -253,61 +230,33 @@ class _PlanModel(nn.Module):
 
     # ------------------------------------------------------------------ gradient placement
     def use_flat_gradients(self, enabled: bool = True) -> None:
-        """Write the parameter gradients straight into views of ONE persistent flat fp32 bucket (the parameters whose gradients are final first:
-        ``flat_gradient_bucket_parts``) and
+        """Write the parameter gradients straight into views of ONE persistent flat fp32 bucket (state-dict order) and
         bind them as ``p.grad``: no per-step allocation, and the data-parallel exchange (``parallel.GradAllReduce``)
         all-reduces the bucket in place without copies.  Backward then returns no gradients to autograd for the
         parameters (hooks on them do not fire)."""
         self._flat_grads = bool(enabled)
         if not enabled:
-            self._grad_bucket = self._grad_views = self._bucket_split = None
+            self._grad_bucket = self._grad_views = None
 
     def flat_gradient_bucket(self) -> Optional[torch.Tensor]:
         return self._grad_bucket
 
-    def flat_gradient_bucket_parts(self):
-        """``(early, late)`` slices of the flat bucket: the gradients that are final after part 0 of a two-part backward (head,
-        decoder, deepest encoder level: ~90 % of the parameters) and the rest.  ``None`` before the first flat-gradient backward."""
-        if self._grad_bucket is None or self._bucket_split is None:
-            return None
-        return self._grad_bucket[:self._bucket_split], self._grad_bucket[self._bucket_split:]
-
-    def _bucket_views(self, params, plan=None):
+    def _bucket_views(self, params):
         if (self._grad_bucket is None or self._grad_bucket.device != params[0].device
                 or self._grad_bucket.numel() != sum(p.numel() for p in params)):
-            if self._param_parts is None:
-                # the schedule's split point is a property of the architecture, not of the input shape: any training plan tells
-                self._param_parts = plan.param_parts() if plan is not None else [0] * len(params)
             self._grad_bucket = torch.zeros(sum(p.numel() for p in params), dtype=torch.float32, device=params[0].device)
-            # bucket layout: the parameters of part 0 first (state-dict order within a part), so that each part is one
-            # contiguous slice for the exchange; the views stay in state-dict order
-            views, off = [None] * len(params), 0
-            for part in (0, 1):
-                for i, p in enumerate(params):
-                    if (self._param_parts[i] != 0) == bool(part):
-                        views[i] = self._grad_bucket[off:off + p.numel()].view_as(p)
-                        off += p.numel()
-                if part == 0:
-                    self._bucket_split = off
+            views, off = [], 0
+            for p in params:
+                views.append(self._grad_bucket[off:off + p.numel()].view_as(p))
+                off += p.numel()
             self._grad_views = views
         return self._grad_views
 
-    def finish_backward(self) -> None:
-        """Runs part 1 of a deferred two-part backward (see ``_UNetFunction.backward``) on the current stream."""
-        if self._backward_tail is None:
-            raise RuntimeError("finish_backward: no deferred backward is pending")
-        plan, dlogits, params, grads = self._backward_tail
-        self._backward_tail = None
-        with torch.cuda.device(dlogits.device):
-            _lib.check(plan.lib.b200unet_plan_backward_part(plan.handle, 1, dlogits.data_ptr(), _ptr_array(params), _ptr_array(grads),
-                                                            plan.workspace.data_ptr(), _lib.stream_ptr()), "plan_backward_part(1)")
-        self.launches_last_backward += plan.last_launches()
-
-    def _grad_targets(self, params, plan=None):
+    def _grad_targets(self, params):
         """(tensors the library writes the gradients into, whether they are already bound as ``.grad``)."""
         if not self._flat_grads:
             return [torch.empty_like(p) for p in params], False
-        views = self._bucket_views(params, plan)
+        views = self._bucket_views(params)
         live = self.ordered_parameters()
         if all(p.grad is None for p in live):                       # the usual step: zero_grad(set_to_none=True) ran
             for p, v in zip(live, views):

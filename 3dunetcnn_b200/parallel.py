@@ -34,8 +34,6 @@ class GradAllReduce:
         self.group = group
         self.flat = None
         self.model = model       # a UNet3D in flat-gradient mode: its bucket IS the exchange buffer (no copies)
-        self._side = None        # stream of the early part of an overlapped exchange (begin / finish)
-        self._begun = False
 
     def _reduce_mean(self, flat: torch.Tensor, world: int) -> None:
         if dist.get_backend(self.group) == "nccl":
@@ -43,58 +41,6 @@ class GradAllReduce:
         else:
             dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=self.group)
             flat.mul_(1.0 / world)
-
-    # ------------------------------------------------------------------ overlapped exchange (train.GraphedTrainStep)
-    @property
-    def supports_overlap(self) -> bool:
-        """begin()/finish() can split the exchange around the tail of backward: needs a flat-gradient model and >1 rank"""
-        return (self.model is not None and hasattr(self.model, "flat_gradient_bucket_parts")
-                and dist.is_available() and dist.is_initialized() and dist.get_world_size(self.group) > 1)
-
-    def _bound_parts(self):
-        parts = self.model.flat_gradient_bucket_parts() if self.model is not None and hasattr(self.model, "flat_gradient_bucket_parts") else None
-        if parts is None or parts[0].numel() == 0:
-            return None
-        bucket = self.model.flat_gradient_bucket()
-        lo, hi = bucket.data_ptr(), bucket.data_ptr() + bucket.numel() * 4
-        if not all(p.grad is not None and lo <= p.grad.data_ptr() < hi for p in self.params):
-            return None
-        return parts
-
-    def begin(self) -> None:
-        """Start the all-reduce of the early slice of the bucket (the gradients part 0 of the backward has finished) on a side
-        stream that waits for the work queued so far; the caller then queues the rest of the backward, then ``finish()``."""
-        self._begun = False
-        if not self.supports_overlap:
-            return
-        parts = self._bound_parts()
-        if parts is None:
-            return
-        world = dist.get_world_size(self.group)
-        early = parts[0]
-        if early.is_cuda:
-            if self._side is None or self._side.device != early.device:
-                self._side = torch.cuda.Stream(device=early.device)
-            self._side.wait_stream(torch.cuda.current_stream(early.device))
-            with torch.cuda.stream(self._side):
-                self._reduce_mean(early, world)
-        else:
-            self._reduce_mean(early, world)
-        self._begun = True
-
-    def finish(self) -> None:
-        """Reduce what ``begin()`` left (everything, if it did not start) and join the side stream."""
-        if not self._begun:
-            self()
-            return
-        self._begun = False
-        late = self.model.flat_gradient_bucket_parts()[1]
-        if late.is_cuda:
-            # collectives of one communicator are issued in the same order on every rank AND kept from overlapping each other:
-            # the late slice is reduced after the early one has completed
-            torch.cuda.current_stream(late.device).wait_stream(self._side)
-        if late.numel():
-            self._reduce_mean(late, dist.get_world_size(self.group))
 
     def broadcast_parameters(self, src: int = 0) -> None:
         if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(self.group) == 1:

@@ -5,7 +5,6 @@ _batch_loss), kept call-compatible so the reference's ``run_training`` can drive
 """
 from __future__ import annotations
 
-import os
 import time
 
 import torch
@@ -65,23 +64,12 @@ class GraphedTrainStep:
     graph's static input buffers (H2D lands in place, no staging copy) and the returned loss is the graph's static
     0-dim tensor (read it with ``.item()`` when needed).  The model runs in flat-gradient mode: every replay overwrites
     the ``.grad`` views of one persistent bucket, which ``grad_sync`` all-reduces in place.
-
-    ``split_backward`` (default off; ``B200UNET_OVERLAP_ALLREDUCE=1`` turns it on wherever ``grad_sync`` can overlap, i.e. a
-    ``parallel.GradAllReduce`` with more than one rank; the one-graph step stays the default): the step is captured as TWO graphs around the schedule's split point -- forward + loss +
-    backward of head / decoder / deepest encoder level, then the backward of the shallow encoder levels.  Between the two
-    replays ``grad_sync.begin()`` starts the all-reduce of the first ~90 % of the bucket on a side stream, so the exchange runs
-    under the second graph; ``grad_sync.finish()`` reduces the small remainder (SURVEY.md 8e: bucketed, overlapped exchange; the
-    reference's DataParallel reduces after the whole backward, unet3d/models/build.py:18-20).
     """
 
     def __init__(self, model, criterion, optimizer, images_shape, target_shape, target_dtype=torch.uint8, device=None,
-                 grad_sync=None, warmup: int = 2, capture_error_mode: str = "global", split_backward=None):
+                 grad_sync=None, warmup: int = 2, capture_error_mode: str = "global"):
         self.model, self.criterion, self.optimizer, self.grad_sync = model, criterion, optimizer, grad_sync
-        if split_backward is None:
-            split_backward = (grad_sync is not None and bool(getattr(grad_sync, "supports_overlap", False))
-                              and os.environ.get("B200UNET_OVERLAP_ALLREDUCE", "0") == "1")
-        self.split_backward = bool(split_backward)
-        self.graph_tail = None
+        self.graph_tail = None      # always None: bench.py reads it to report whether the exchange ran overlapped
         device = device or next(model.parameters()).device
         self.images = torch.zeros(tuple(images_shape), dtype=torch.float32, device=device)
         self.target = torch.zeros(tuple(target_shape), dtype=target_dtype, device=device)
@@ -115,22 +103,12 @@ class GraphedTrainStep:
         torch.cuda.synchronize(self.device)
         model._overwrite_grads = True
         self.graph = torch.cuda.CUDAGraph()
-        self.graph_tail = None
         try:
-            model._backward_tail = None
-            model._defer_backward_tail = self.split_backward
             with torch.cuda.graph(self.graph, capture_error_mode=self.capture_error_mode):
                 self.loss = self.criterion(model(self.images), self.target)
                 self.loss.backward()
-            model._defer_backward_tail = False
-            if model._backward_tail is not None:      # the schedule has a split point: the rest of backward is its own graph
-                self.graph_tail = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(self.graph_tail, pool=self.graph.pool(), capture_error_mode=self.capture_error_mode):
-                    model.finish_backward()
         except Exception as e:
-            model._defer_backward_tail = False
-            model._backward_tail = None
-            self.graph = self.graph_tail = None
+            self.graph = None
             self.loss = None
             raise RuntimeError(
                 "GraphedTrainStep: CUDA-graph capture of the training step failed (%s).  A loss (or any tensor with a grad_fn) of "
@@ -150,16 +128,7 @@ class GraphedTrainStep:
             for p, v in zip(params, self.model._grad_views):
                 if p.requires_grad:
                     p.grad = v
-        if self.graph_tail is not None:
-            overlap = self.grad_sync is not None and hasattr(self.grad_sync, "begin")
-            if overlap:
-                self.grad_sync.begin()      # all-reduce of the gradients that are final, on a side stream ...
-            self.graph_tail.replay()        # ... under the backward of the shallow encoder levels
-            if overlap:
-                self.grad_sync.finish()
-            elif self.grad_sync is not None:
-                self.grad_sync()
-        elif self.grad_sync is not None:
+        if self.grad_sync is not None:
             self.grad_sync()
         self.optimizer.step()
         return self.loss

@@ -248,18 +248,8 @@ int b200unet_plan_forward(b200unet_plan* plan, const float* x, const float* cons
 /* backward: dlogits NCDHW fp32 -> grads[i] (fp32, same shapes as params; overwritten). */
 int b200unet_plan_backward(b200unet_plan* plan, const float* dlogits, const float* const* params, float* const* grads,
                            void* workspace, void* stream);
-/* The same backward in two calls, so that a data-parallel caller can exchange the gradients that are already final while the
- * rest of the backward runs (the reference's DataParallel reduces every gradient after the whole backward:
- * unet3d/models/build.py:18-20).  backward_parts: 2 when the schedule has a split point (part 0 = head, decoder, deepest
- * encoder level(s): most of the parameters; part 1 = the shallow encoder levels), 1 otherwise, 0 for an inference_only plan.
- * param_backward_part(i): the part after which grads[i] is final.  backward_part(0) followed by backward_part(1) on the same
- * stream writes exactly what b200unet_plan_backward writes; both calls take the same pointers. */
-int b200unet_plan_backward_parts(const b200unet_plan* plan);
-int b200unet_plan_param_backward_part(const b200unet_plan* plan, int i);
-int b200unet_plan_backward_part(b200unet_plan* plan, int part, const float* dlogits, const float* const* params, float* const* grads,
-                                void* workspace, void* stream);
 /* input gradient of a plan created with input_grad = 1: dx = d(loss)/d(x), NCDHW fp32 [N][n_features][D][H][W], overwritten.
- * Runs after b200unet_plan_backward (or after backward_part(1)) on the same stream and workspace, before the next forward: it reads
+ * Runs after b200unet_plan_backward on the same stream and workspace, before the next forward: it reads
  * what that backward left in the workspace (the gradients reaching the first block, the packed input, the first norm's
  * coefficients).  UNet3D: GroupNorm(+ReLU) backward of encoder.layers.0.blocks.0.conv1.norm1 + the data gradient of the block's
  * 1x1x1 `sample` branch or its identity (myronenko.py:34-58); DynUNet: the data gradient of input_block.conv1.  The parameter

@@ -13,7 +13,6 @@ import torch
 
 HOST_ONLY = {"b200unet_version", "b200unet_last_error", "b200unet_plan_create", "b200unet_plan_destroy", "b200unet_plan_num_params",
              "b200unet_plan_param_info", "b200unet_plan_workspace_bytes", "b200unet_plan_last_launches", "b200unet_plan_algorithmic_macs",
-             "b200unet_plan_backward_parts", "b200unet_plan_param_backward_part",
              "b200unet_head_bwd_scratch_bytes"}
 
 
@@ -94,7 +93,7 @@ def test_unet3d_training_and_inference_calls(pkg, stubbed):
     crit(fake(model(x)), fake(torch.rand(1, 3, 16, 16, 16))).backward()
 
 
-def test_flat_gradient_bucket_binding(pkg, stubbed):
+def test_flat_gradient_bucket_binding_in_state_dict_order(pkg, stubbed):
     model = pkg.UNet3D(n_features=4, n_outputs=3, base_width=8)
     model.train()
     model.use_flat_gradients(True)
@@ -115,44 +114,12 @@ def test_flat_gradient_bucket_binding(pkg, stubbed):
     assert [p.grad.data_ptr() for p in model.parameters()] == first
     sync = pkg.parallel.GradAllReduce(model.parameters(), model=model)
     sync()                                   # no process group: a no-op that must not raise
-    # bucket layout: the parameters whose gradients part 0 of the two-part backward finishes (head, decoder, deepest encoder level)
-    # form the leading slice, state-dict order within each slice; the views themselves stay in state-dict order
-    early, late = model.flat_gradient_bucket_parts()
-    assert early.data_ptr() == bucket.data_ptr() and early.numel() + late.numel() == bucket.numel() and late.numel() > 0
-    plan = next(iter(model._plans.values()))
-    parts = plan.param_parts()
-    split = bucket.data_ptr() + 4 * early.numel()
-    offs = {0: [], 1: []}
-    for p, part in zip(model.ordered_parameters(), parts):
-        assert (p.grad.data_ptr() < split) == (part == 0)
-        offs[part].append(p.grad.data_ptr())
-    assert offs[0] == sorted(offs[0]) and offs[1] == sorted(offs[1])
-    assert not sync.supports_overlap and not sync._begun      # single process: begin() declines, finish() is the plain call
-    sync.begin()
-    sync.finish()
-
-
-def test_deferred_backward_tail_calls(pkg, stubbed):
-    """two-part backward marshalling: with the tail deferred the autograd backward issues part 0 only, finish_backward() part 1"""
-    model = pkg.UNet3D(n_features=4, n_outputs=3, base_width=8)
-    model.train()
-    model.use_flat_gradients(True)
-    x, _ = _batch()
-    model._defer_backward_tail = True
-    model(x).sum().backward()
-    model._defer_backward_tail = False
-    assert stubbed.count("b200unet_plan_backward_part") == 1 and stubbed.count("b200unet_plan_backward") == 0
-    assert model._backward_tail is not None
-    model.finish_backward()
-    assert stubbed.count("b200unet_plan_backward_part") == 2 and model._backward_tail is None
-    with pytest.raises(RuntimeError, match="no deferred backward"):
-        model.finish_backward()
-    # without the flat bucket the gradients go back through autograd: the backward cannot be deferred
-    model2 = pkg.UNet3D(n_features=4, n_outputs=3, base_width=8)
-    model2.train()
-    model2._defer_backward_tail = True
-    model2(x).sum().backward()
-    assert model2._backward_tail is None and stubbed.count("b200unet_plan_backward") == 1
+    # bucket layout: the .grad views tile the bucket contiguously, in state-dict order
+    off = bucket.data_ptr()
+    for p in model.ordered_parameters():
+        assert p.grad.data_ptr() == off
+        off += 4 * p.numel()
+    assert off == hi
 
 
 def test_dynunet_calls(pkg, stubbed):

@@ -176,7 +176,7 @@ def test_dynunet_split_precision_input_gradient_matches_unpinned_oracle(pkg, cin
     assert _cos(xd.grad.cpu().numpy(), x64.grad.numpy()) > 0.999
 
 
-def test_flat_gradients_with_a_deferred_tail_give_the_same_input_gradient(pkg):
+def test_flat_gradients_give_the_same_input_gradient(pkg):
     kw = dict(n_features=2, n_outputs=2, base_width=8)
     sd = make_state_dict(UNetConfig(**kw), seed=3)
     g = torch.Generator().manual_seed(5)
@@ -189,11 +189,8 @@ def test_flat_gradients_with_a_deferred_tail_give_the_same_input_gradient(pkg):
         model.train()
         if flat:
             model.use_flat_gradients(True)
-            model._defer_backward_tail = True                     # ignored while the input needs a gradient
         xi = x.clone().requires_grad_(True)
         pkg.DiceLoss(sigmoid=True)(model(xi), t).backward()
-        model._defer_backward_tail = False
-        assert model._backward_tail is None
         out[flat] = (xi.grad.clone(), [p.grad.clone() for p in model.ordered_parameters()])
     assert torch.equal(out[False][0], out[True][0])
     for a, b in zip(out[False][1], out[True][1]):

@@ -1,6 +1,6 @@
 """Many-class heads (9..128 outputs) on the GPU: the tensor-core head kernels through the C ABI against fp64 einsum, UNet3D
 in split precision against the reference's multi-class fixture (tests/golden/multiclass.npz), bf16 against torch's own bf16
-autocast, DynUNet with its bias, a cross-entropy step, and the existing machinery (launch count, two-part backward,
+autocast, DynUNet with its bias, a cross-entropy step, and the existing machinery (launch count,
 determinism, input-gradient plans, CUDA graphs, sliding windows, pre/post-processing) at 104 classes."""
 import os
 import sys
@@ -296,7 +296,7 @@ def test_104_outputs_take_the_launches_of_3_outputs(pkg):
 
 
 @pytest.mark.parametrize("precision", ["bf16", "split"])
-def test_two_part_and_deterministic_backward_at_104_outputs(pkg, precision):
+def test_deterministic_backward_repeats_bit_for_bit_at_104_outputs(pkg, precision):
     model = pkg.UNet3D(precision=precision, deterministic=True, dropout=0.0, **KW104).to(DEV)
     model.train()
     crit = pkg.DiceLoss(sigmoid=True)
@@ -314,11 +314,7 @@ def test_two_part_and_deterministic_backward_at_104_outputs(pkg, precision):
     for p in model.parameters():
         p.grad = None
     model.flat_gradient_bucket().fill_(float("nan"))
-    model._defer_backward_tail = True
     crit(model(x), t).backward()
-    model._defer_backward_tail = False
-    torch.cuda.synchronize()
-    model.finish_backward()
     torch.cuda.synchronize()
     assert torch.equal(model.flat_gradient_bucket(), whole)
 

@@ -165,29 +165,9 @@ def test_graphed_train_step_matches_eager(pkg):
     assert num / den < 1e-4
 
 
-class _RecordingSync:
-    """stands in for parallel.GradAllReduce on one GPU: records the call order and checks what is final at begin()"""
-    supports_overlap = True
-
-    def __init__(self, model):
-        self.model, self.calls, self.early_at_begin = model, [], None
-
-    def begin(self):
-        self.calls.append("begin")
-        torch.cuda.synchronize()
-        self.early_at_begin = self.model.flat_gradient_bucket_parts()[0].clone()
-
-    def finish(self):
-        self.calls.append("finish")
-
-    def __call__(self):
-        self.calls.append("call")
-
-
 @pytest.mark.parametrize("arch", ["unet3d", "dynunet"])
-def test_two_part_backward_is_the_whole_backward(pkg, arch):
-    """b200unet_plan_backward_part(0) + (1) must write bit for bit what b200unet_plan_backward writes (deterministic weight
-    gradients, so that bit equality is meaningful), and every gradient of the early bucket slice must be final after part 0."""
+def test_deterministic_backward_repeats_bit_for_bit(pkg, arch):
+    """A deterministic plan's backward writes the same flat gradient bucket bit for bit every time, and writes all of it."""
     torch.manual_seed(0)
     if arch == "unet3d":
         model = pkg.UNet3D(precision="bf16", deterministic=True, dropout=0.0, n_features=2, n_outputs=2, base_width=8).to(DEV)
@@ -206,60 +186,18 @@ def test_two_part_backward_is_the_whole_backward(pkg, arch):
     crit(model(x), t).backward()
     torch.cuda.synchronize()
     whole = model.flat_gradient_bucket().clone()
-    parts = model.flat_gradient_bucket_parts()
-    assert parts is not None and parts[0].numel() > parts[1].numel() > 0          # most parameters are final early
-    assert parts[0].numel() + parts[1].numel() == whole.numel()
     for p in model.parameters():
         p.grad = None
     crit(model(x), t).backward()
     torch.cuda.synchronize()
     assert torch.equal(model.flat_gradient_bucket(), whole), "a deterministic plan must repeat its gradients bit for bit"
-    # two parts; poison the bucket first so that a gradient nobody writes shows up
+    # poison the bucket first so that a gradient nobody writes shows up
     for p in model.parameters():
         p.grad = None
     model.flat_gradient_bucket().fill_(float("nan"))
-    model._defer_backward_tail = True
     crit(model(x), t).backward()
-    model._defer_backward_tail = False
     torch.cuda.synchronize()
-    assert model._backward_tail is not None
-    early = model.flat_gradient_bucket_parts()[0].clone()
-    assert torch.isnan(model.flat_gradient_bucket_parts()[1]).any()                  # part 1 has not run
-    model.finish_backward()
-    torch.cuda.synchronize()
-    assert torch.equal(early, whole[:early.numel()])                                  # final after part 0, bit for bit
     assert torch.equal(model.flat_gradient_bucket(), whole)
-    with pytest.raises(RuntimeError, match="no deferred backward"):
-        model.finish_backward()
-
-
-def test_graphed_train_step_split_backward_matches_single_graph(pkg):
-    """The two-graph step (forward + loss + part 0 | part 1, the exchange begun in between) must train exactly like the
-    one-graph step; begin() must see final early gradients; call order begin -> finish every step."""
-    sd = make_state_dict(UNetConfig(**KW), seed=3)
-    runs = {}
-    for mode in ("single", "split"):
-        torch.manual_seed(0)
-        model = pkg.UNet3D(precision="bf16", deterministic=True, dropout=0.0, **KW).to(DEV)
-        model.load_state_dict(sd)
-        crit = pkg.DiceLoss(sigmoid=True)
-        opt = torch.optim.Adam(model.parameters(), lr=1e-3)
-        sync = _RecordingSync(model) if mode == "split" else None
-        step = pkg.train.GraphedTrainStep(model, crit, opt, (2, 2, 16, 16, 16), (2, 2, 16, 16, 16), grad_sync=sync,
-                                          split_backward=(mode == "split"))
-        losses = []
-        for i in range(4):
-            x, t = _batch(100 + i)
-            losses.append(float(step(x.pin_memory(), t.pin_memory()).item()))
-            if sync is not None:
-                torch.cuda.synchronize()
-                assert torch.equal(sync.early_at_begin, model.flat_gradient_bucket_parts()[0])   # nothing touched it after begin()
-        if sync is not None:
-            assert step.graph_tail is not None and sync.calls == ["begin", "finish"] * 4
-        runs[mode] = (losses, [p.detach().clone() for p in model.ordered_parameters()])
-    assert runs["single"][0] == runs["split"][0]
-    for a, b in zip(runs["single"][1], runs["split"][1]):
-        assert torch.equal(a, b)
 
 
 def test_epoch_training_with_cuda_graph_and_short_last_batch(pkg):

@@ -206,15 +206,12 @@ def test_dynunet_input_gradient_calls(pkg, stubbed):
     assert x.grad.shape == x.shape
 
 
-def test_deferred_tail_is_not_used_when_the_input_needs_a_gradient(pkg, stubbed):
+def test_flat_gradients_with_an_input_gradient_calls(pkg, stubbed):
     model = pkg.UNet3D(n_features=4, n_outputs=3, base_width=8)
     model.train()
     model.use_flat_gradients(True)
-    model._defer_backward_tail = True
     x = _x()
     model(x).sum().backward()
-    model._defer_backward_tail = False
-    assert model._backward_tail is None and stubbed.count("b200unet_plan_backward_part") == 0
     assert stubbed.count("b200unet_plan_backward") == 1 and stubbed.count("b200unet_plan_input_grad") == 1
     assert x.grad is not None
 

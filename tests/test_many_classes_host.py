@@ -138,15 +138,6 @@ def test_head_scratch_bytes_by_path(pkg):
         assert lib.b200unet_head_bwd_scratch_bytes(n_out, c) == 132 * (n_out * c + n_out) * 4
 
 
-def test_two_part_backward_keeps_the_head_in_part_0(pkg):
-    net, plan = _unet_plan(pkg, 104, shape=(1, 4, 32, 32, 32))
-    lib = pkg.lib.load_library()
-    if lib.b200unet_plan_backward_parts(plan.handle) < 2:
-        pytest.skip("this plan has no split point")
-    idx = [k for k, _ in plan.param_spec()].index(HEAD)
-    assert lib.b200unet_plan_param_backward_part(plan.handle, idx) == 0
-
-
 # ------------------------------------------------------------------------------------------------ host layer (stub library)
 def test_104_output_unet3d_training_and_inference_calls(pkg, stubbed):
     model = pkg.UNet3D(n_features=4, n_outputs=104, base_width=8)
