@@ -14,7 +14,7 @@
 // A CTA owns QT = 128/BN M-tiles (accumulators in the registers of its consumer warpgroup) and a contiguous range of voxel
 // tiles (split-K); the dY tile of a voxel block is loaded once and reused by all of the CTA's M-tiles.  Partial sums are
 // reduced into the fp32 gradient buffer with vector atomics.  Split-precision mode: passes (a_hi,dy_hi), (a_lo,dy_hi),
-// (a_hi,dy_lo).
+// (a_hi,dy_lo).  3x3x3 stride-1 layers of at most 64 input channels run in halo mode instead (k_wgrad_halo, WgradHaloCfg).
 #include <algorithm>
 #include "conv_common.cuh"
 
@@ -46,24 +46,16 @@ constexpr int WG_A_STAGES = 4;
 constexpr int WG_D_STAGES = 2;
 constexpr int WG_A_BYTES = 32768;
 
-// Halo mode (3x3x3 stride 1, 33..64 input channels, output planes filling the halo tile, bf16): per voxel tile ONE TMA halo
-// box of 64 channels (HaloTile) replaces the 27 per-tap boxes; the A operand of a tap is the box read from the tap's row with a
-// K-group stride (SBO) of one halo row.  Two halo buffers: the producer loads the next tile's box while the MMAs of this one
-// run.
-constexpr int WG_HALO_TX = HaloTile::ROWS * 128;
-constexpr int WG_HALO_BYTES = (WG_HALO_TX + 1023) / 1024 * 1024;
-
-template <int CB, int BN, bool HALO = false>
+template <int CB, int BN>
 struct WgradCfg {
   static constexpr int CBN = BN < 64 ? BN : 64;
   static constexpr int BPM = 128 / CB;             // boxes per M tile
   static constexpr int BPN = BN / CBN;             // boxes per N tile
-  static constexpr int QT = 128 / BN;              // M tiles per CTA: QT * BN fp32 accumulator registers per thread
+  static constexpr int QT = 128 / BN;              // M tiles per consumer warpgroup: QT * BN fp32 accumulator registers per thread
   static constexpr int D_BYTES = BN * 128 * 2;
   static constexpr int D_STAGE = D_BYTES < 1024 ? 1024 : D_BYTES;
-  static constexpr int A_REGION = HALO ? 2 * WG_HALO_BYTES : WG_A_STAGES * WG_A_BYTES;
+  static constexpr int A_REGION = WG_A_STAGES * WG_A_BYTES;
   static constexpr int SMEM_BYTES = A_REGION + WG_D_STAGES * D_STAGE + 1024 + 1024;
-  static_assert(!HALO || CB == 64, "halo mode reads 64-channel rows");
   static_assert(SMEM_BYTES <= 232448, "wgrad: configuration does not fit shared memory");
   static constexpr uint32_t LAYOUT_A = swizzle_for_row_bytes(CB * 2);
   static constexpr uint32_t LAYOUT_B = swizzle_for_row_bytes(CBN * 2);
@@ -72,10 +64,24 @@ struct WgradCfg {
   static constexpr uint32_t HALF_M = 64 / CB * LBO_A;   // bytes from M row 0 to M row 64
 };
 
+// Halo mode (wgrad_halo_eligible): per voxel tile ONE TMA halo box of 64 channels (HaloTile; channels past the input's are the
+// TMA out-of-bounds zero fill) replaces the per-tap boxes.  Each m64 half of an M tile is one tap of all 64 channels, read from the
+// box at the tap's row with a K-group stride (SBO) of one halo row.  Two consumer warpgroups share every box and dY tile, each
+// with its own M tiles; two stages (box + dY tile): the producer loads the next voxel tile while the MMAs of this one run.
+template <int BN>
+struct WgradHaloCfg : WgradCfg<64, BN> {
+  static constexpr int ROWB = 128;                 // bytes per box row
+  static constexpr int BOX_TX = HaloTile::ROWS * ROWB;
+  static constexpr int BOX_BYTES = (BOX_TX + 1023) / 1024 * 1024;
+  static constexpr int STAGES = 2;
+  static constexpr int SMEM_BYTES = STAGES * (BOX_BYTES + WgradCfg<64, BN>::D_STAGE) + 1024 + 1024;
+  static_assert(SMEM_BYTES <= 232448, "wgrad: configuration does not fit shared memory");
+};
+
 // Warps 0-3: one consumer warpgroup (wgmma issue and the write-back); warp 4: TMA producer.
-template <int CB, int BN, bool HALO>
+template <int CB, int BN>
 __global__ void __launch_bounds__(160, 1) k_wgrad(const __grid_constant__ WgradMaps maps, const WgradArgs p) {
-  using Cfg = WgradCfg<CB, BN, HALO>;
+  using Cfg = WgradCfg<CB, BN>;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment by pointer arithmetic on the __shared__ array: an integer round trip loses the address space and every
   // shared-memory access below would compile to a generic LD.E / ST.E instead of LDS / STS
@@ -131,12 +137,6 @@ __global__ void __launch_bounds__(160, 1) k_wgrad(const __grid_constant__ WgradM
             tma_load_5d_if(issue, dst + bx * Cfg::LBO_B, &maps.dy[pass == 2], &d_full[s], co0 + bx * Cfg::CBN, w0, h0, d0, n);
           ++id;
         }
-        if constexpr (HALO) {   // a_full / a_empty [0..1] guard the two halo buffers
-          const int kbi = kb - kb0, hb = kbi & 1;
-          mbar_wait(&a_empty[hb], ((kbi >> 1) & 1) ^ 1);
-          mbar_expect_tx_if(issue, &a_full[hb], WG_HALO_TX);
-          tma_load_5d_if(issue, smem_a + hb * WG_HALO_BYTES, &maps.a[0], &a_full[hb], 0, w0 - 1, h0 - 1, d0 - 1, n);
-        } else {
         for (int q = q0; q < q1; ++q) {
           const int s = ia % WG_A_STAGES;
           const uint32_t ph = (ia / WG_A_STAGES) & 1;
@@ -153,7 +153,6 @@ __global__ void __launch_bounds__(160, 1) k_wgrad(const __grid_constant__ WgradM
                            w0 * p.stride + kw - pad, h0 * p.stride + kh - pad, d0 * p.stride + kd - pad, n);
           }
           ++ia;
-        }
         }
       }
     }
@@ -175,39 +174,6 @@ __global__ void __launch_bounds__(160, 1) k_wgrad(const __grid_constant__ WgradM
       const int sd = id % WG_D_STAGES;
       mbar_wait(&d_full[sd], (id / WG_D_STAGES) & 1);
       const uint32_t b_lo = desc_lo(d0s + sd * Cfg::D_STAGE, Cfg::LBO_B);
-      if constexpr (HALO) {
-        // M half hm of M tile q is unit 2q + hm = one tap of all 64 channels; K step k = output rows h = 2k, 2k + 1
-        constexpr uint32_t hi_h = desc_hi(HaloTile::GROUP_STRIDE * 128, GMMA_SW128);
-        constexpr uint32_t K_STEP = 2 * HaloTile::GROUP_STRIDE * (128 >> 4);   // descriptor offset of the next two output rows
-        const int kbi = kb - kb0, hb = kbi & 1;
-        mbar_wait(&a_full[hb], (kbi >> 1) & 1);
-        const uint32_t h_lo = desc_lo(a0 + hb * WG_HALO_BYTES, 16);
-#pragma unroll
-        for (int qi = 0; qi < Cfg::QT; ++qi) {
-          if (qi < nq) {
-            uint32_t off[2];
-#pragma unroll
-            for (int hm = 0; hm < 2; ++hm) {
-              int u = (q0 + qi) * 2 + hm;
-              if (u >= p.units) u = p.units - 1;   // duplicate a valid unit; its rows are never written back
-              off[hm] = HaloTile::tap_row(u) * (128 >> 4);
-            }
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              const uint64_t db = desc_from(b_lo + ((k * 2 * Cfg::SBO_B) >> 4), hi_b);
-              Wgmma<BN>::template mma<1, 1>(acc[qi][0], desc_from(h_lo + off[0] + k * K_STEP, hi_h), db, 1u);
-              Wgmma<BN>::template mma<1, 1>(acc[qi][1], desc_from(h_lo + off[1] + k * K_STEP, hi_h), db, 1u);
-            }
-            wgmma_commit();
-          }
-        }
-        wgmma_wait<0>();   // this tile's box and dY stage are read: hand both back (the other halo buffer is already loading)
-        if (lane == 0) {
-          mbar_arrive(&d_empty[sd]);
-          mbar_arrive(&a_empty[hb]);
-        }
-      } else {
 #pragma unroll
       for (int qi = 0; qi < Cfg::QT; ++qi) {
         if (qi < nq) {
@@ -231,7 +197,6 @@ __global__ void __launch_bounds__(160, 1) k_wgrad(const __grid_constant__ WgradM
           prev_d = qi == nq - 1 ? sd : -1;
           ++ia;
         }
-      }
       }
       ++id;
     }
@@ -274,21 +239,161 @@ __global__ void __launch_bounds__(160, 1) k_wgrad(const __grid_constant__ WgradM
   }
 }
 
+// Halo mode (WgradHaloCfg).  Warps 0-7: two consumer warpgroups, warpgroup g owning M tiles [q0 + g * qw, q0 + (g + 1) * qw) of
+// the CTA's p.qt with qw = ceil(p.qt / 2); warp 8: TMA producer.  M half hm of M tile q is tap 2q + hm; K step k = output rows
+// h = 2k, 2k + 1 of the voxel tile.
+template <int BN>
+__global__ void __launch_bounds__(288, 1) k_wgrad_halo(const __grid_constant__ WgradMaps maps, const WgradArgs p) {
+  using Cfg = WgradHaloCfg<BN>;
+  constexpr int S = Cfg::STAGES;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // (see k_wgrad)
+  uint8_t* smem_a = smem;
+  uint8_t* smem_d = smem + S * Cfg::BOX_BYTES;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem_d + S * Cfg::D_STAGE);   // stage s: box s and dY tile s
+  uint64_t* empty = full + S;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int split = blockIdx.x;
+  const int q0 = blockIdx.y * p.qt;
+  const int q1 = min(q0 + p.qt, p.qtiles);
+  const int co0 = blockIdx.z * BN;
+  const int kb0 = (int)((long long)p.kblocks * split / p.splits);
+  const int kb1 = (int)((long long)p.kblocks * (split + 1) / p.splits);
+
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&maps.a[0]);
+    tma_prefetch_desc(&maps.dy[0]);
+    for (int s = 0; s < S; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();                 // (see k_wgrad)
+  pdl_launch_dependents();
+
+  if (warp == 8) {
+    const uint32_t issue = elect_one() ? 1u : 0u;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      int t = kb;
+      const int wt = t % p.tiles_w; t /= p.tiles_w;
+      const int ht = t % p.tiles_h; t /= p.tiles_h;
+      const int dt = t % p.tiles_d;
+      const int n = t / p.tiles_d;
+      const int w0 = wt * p.tw, h0 = ht * p.th, d0 = dt * p.td;
+      const int kbi = kb - kb0, s = kbi % S;
+      mbar_wait(&empty[s], ((kbi / S) & 1) ^ 1);
+      mbar_expect_tx_if(issue, &full[s], Cfg::BOX_TX + Cfg::D_BYTES);
+#pragma unroll
+      for (int bx = 0; bx < Cfg::BPN; ++bx)
+        tma_load_5d_if(issue, smem_d + s * Cfg::D_STAGE + bx * Cfg::LBO_B, &maps.dy[0], &full[s], co0 + bx * Cfg::CBN, w0, h0, d0, n);
+      tma_load_5d_if(issue, smem_a + s * Cfg::BOX_BYTES, &maps.a[0], &full[s], 0, w0 - 1, h0 - 1, d0 - 1, n);
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumer warpgroups
+  const int wg = warp >> 2;
+  const int qw = (p.qt + 1) >> 1;
+  const int qa = q0 + wg * qw;
+  const int nq = min(qa + qw, q1) - qa;   // M tiles of this warpgroup (none in a last group with a single M tile)
+  constexpr uint32_t hi_a = desc_hi(HaloTile::GROUP_STRIDE * Cfg::ROWB, Cfg::LAYOUT_A);
+  constexpr uint32_t hi_b = desc_hi(Cfg::SBO_B, Cfg::LAYOUT_B);
+  constexpr uint32_t K_STEP = 2 * HaloTile::GROUP_STRIDE * Cfg::ROWB >> 4;   // descriptor offset of the next two output rows
+  // descriptor offsets of this warpgroup's M halves from the box start: the tap's first row
+  uint32_t off[Cfg::QT][2];
+#pragma unroll
+  for (int qi = 0; qi < Cfg::QT; ++qi)
+#pragma unroll
+    for (int hm = 0; hm < 2; ++hm) {
+      int u = 2 * (qa + qi) + hm;
+      if (u >= p.units) u = p.units - 1;   // duplicate a valid tap; its rows are never written back
+      off[qi][hm] = HaloTile::tap_row(u) * (Cfg::ROWB >> 4);
+    }
+  const uint32_t a0 = smem_u32(smem_a), d0s = smem_u32(smem_d);
+  float acc[Cfg::QT][2][BN / 2];
+#pragma unroll
+  for (int qi = 0; qi < Cfg::QT; ++qi)
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) { acc[qi][0][i] = 0.f; acc[qi][1][i] = 0.f; }
+  for (int kb = kb0; kb < kb1; ++kb) {
+    const int kbi = kb - kb0, s = kbi % S;
+    mbar_wait(&full[s], (kbi / S) & 1);
+    const uint32_t a_lo = desc_lo(a0 + s * Cfg::BOX_BYTES, 16);   // (LBO unused: an m64 half is one 128-byte swizzle atom)
+    const uint32_t b_lo = desc_lo(d0s + s * Cfg::D_STAGE, Cfg::LBO_B);
+#pragma unroll
+    for (int qi = 0; qi < Cfg::QT; ++qi) {
+      if (qi < nq) {
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          const uint64_t db = desc_from(b_lo + ((k * 2 * Cfg::SBO_B) >> 4), hi_b);
+          Wgmma<BN>::template mma<1, 1>(acc[qi][0], desc_from(a_lo + off[qi][0] + k * K_STEP, hi_a), db, 1u);
+          Wgmma<BN>::template mma<1, 1>(acc[qi][1], desc_from(a_lo + off[qi][1] + k * K_STEP, hi_a), db, 1u);
+        }
+        wgmma_commit();
+      }
+    }
+    wgmma_wait<0>();   // this stage's box and dY tile are read: hand them back (the other stage is already loading)
+    if (lane == 0) mbar_arrive(&empty[s]);
+  }
+#pragma unroll
+  for (int qi = 0; qi < Cfg::QT; ++qi) { wgmma_fence_regs(acc[qi][0]); wgmma_fence_regs(acc[qi][1]); }
+
+  // write-back straight from the fragments: row r of half hm of M tile q -> dw[2q + hm][r][co0 + c]
+  const bool has_work = kb1 > kb0;
+  float* const base = p.part ? p.part + (long long)split * p.part_stride : p.dw;
+#pragma unroll
+  for (int qi = 0; qi < Cfg::QT; ++qi) {
+    if (qi >= nq) continue;
+#pragma unroll
+    for (int hm = 0; hm < 2; ++hm) {
+#pragma unroll
+      for (int r8 = 0; r8 < 2; ++r8) {
+        const int row = (warp & 3) * 16 + (lane >> 2) + r8 * 8;
+        const int tap = 2 * (qa + qi) + hm, ci = row;
+        if (tap >= p.units || ci >= p.Ci || !(has_work || p.part)) continue;
+        float* dst = base + ((long long)tap * p.Cip + ci) * p.Cop;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int c = co0 + j * 8 + 2 * (lane & 3);
+          if (c < p.Cop) {   // (see k_wgrad)
+            const float2 v = make_float2(acc[qi][hm][4 * j + 2 * r8], acc[qi][hm][4 * j + 2 * r8 + 1]);
+            if (p.part) *reinterpret_cast<float2*>(dst + c) = has_work ? v : make_float2(0.f, 0.f);
+            else atomicAdd(reinterpret_cast<float2*>(dst + c), v);
+          }
+        }
+      }
+    }
+  }
+}
+
 template <int CB, int BN, bool HALO>
 static int launch_wg(const WgradMaps& maps, const WgradArgs& a, dim3 grid, cudaStream_t st) {
-  using Cfg = WgradCfg<CB, BN, HALO>;
-  B200_TRY((set_max_dynamic_smem<k_wgrad<CB, BN, HALO>>(Cfg::SMEM_BYTES)));
-  launch_pdl(k_wgrad<CB, BN, HALO>, grid, dim3(160), Cfg::SMEM_BYTES, st, maps, a);
+  if constexpr (HALO) {
+    static_assert(CB == 64, "halo mode loads 64-channel boxes");
+    using Cfg = WgradHaloCfg<BN>;
+    B200_TRY((set_max_dynamic_smem<k_wgrad_halo<BN>>(Cfg::SMEM_BYTES)));
+    launch_pdl(k_wgrad_halo<BN>, grid, dim3(288), Cfg::SMEM_BYTES, st, maps, a);
+  } else {
+    using Cfg = WgradCfg<CB, BN>;
+    B200_TRY((set_max_dynamic_smem<k_wgrad<CB, BN>>(Cfg::SMEM_BYTES)));
+    launch_pdl(k_wgrad<CB, BN>, grid, dim3(160), Cfg::SMEM_BYTES, st, maps, a);
+  }
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;
 }
 
-// halo mode (see WG_HALO_TX)
+// Halo mode (see WgradHaloCfg): 3x3x3 stride 1, bf16, output planes filling the 8 x 16 halo tile, 33..64 input channels -- and
+// 8..32 input channels when BN <= 32.  On per-tap tiles every M tile of a CTA re-loads 32 KB of activation boxes per voxel tile
+// for only BN columns of MMA, so at BN <= 32 those launches are bound by L2 -> shared-memory traffic; one 64-channel box per
+// voxel tile, zero-filled past the input's channels, removes that traffic at the price of MMAs on the zero channels.  At BN >= 64
+// the per-tap kernel is no longer bound by its A loads, and the 2-4x MMAs of the padded box would cost more than they save.
 static bool wgrad_halo_eligible(const WgradOp& op) {
   const Act& A = op.a;
   const Act& Y = op.dy;
-  return !halo_disabled() && op.ksz == 3 && op.stride == 1 && !op.nopad && !A.lo && !Y.lo && A.C > 32 && A.C <= 64 &&
-         Y.W >= HaloTile::TW && Y.H >= HaloTile::TH && A.D == Y.D && A.H == Y.H && A.W == Y.W;
+  return !halo_disabled() && op.ksz == 3 && op.stride == 1 && !op.nopad && !A.lo && !Y.lo && A.C <= 64 &&
+         (A.C > 32 || bn_bucket(Y.C) <= 32) && Y.W >= HaloTile::TW && Y.H >= HaloTile::TH && A.D == Y.D && A.H == Y.H &&
+         A.W == Y.W;
 }
 
 // The tiling fields of r for halo tiles or per-tap tiles: voxel tile, CB / BN, M tiles and their CTA groups, N tiles, voxel
@@ -302,12 +407,12 @@ static void wgrad_tiling(const WgradOp& op, int num_sms, bool halo, WgradRoute* 
     pick_tile(Y.W, Y.H, Y.D, r->tw, r->th, r->td);
   }
   const int ntaps = op.ksz * op.ksz * op.ksz;
-  r->CB = kc_bucket(A.C);
+  r->CB = halo ? 64 : kc_bucket(A.C);   // halo mode: one 64-channel box whatever the input's width
   r->BN = bn_bucket(Y.C);
   r->nci = ceil_div(A.C, r->CB);
   r->units = ntaps * r->nci;
   r->qtiles = ceil_div(r->units, 128 / r->CB);
-  r->QT = 128 / r->BN;   // WgradCfg::QT
+  r->QT = (halo ? 2 : 1) * (128 / r->BN);   // WgradCfg::QT per consumer warpgroup: one on per-tap tiles, two in halo mode
   if (r->QT > r->qtiles) r->QT = r->qtiles;
   r->groups = ceil_div(r->qtiles, r->QT);
   r->QT = ceil_div(r->qtiles, r->groups);   // rebalance M tiles across groups
