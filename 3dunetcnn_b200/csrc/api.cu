@@ -85,7 +85,7 @@ using namespace b200;
 
 extern "C" {
 
-int b200unet_version(void) { return 102; }
+int b200unet_version(void) { return 103; }
 const char* b200unet_last_error(void) { return get_error(); }
 
 int b200unet_ncdhw_to_ndhwc(const float* x, int c_real, const b200unet_tensor* out, void* stream) {
@@ -242,6 +242,17 @@ int b200unet_zscore(const float* x, int groups, int64_t spatial, int nonzero, do
 int b200unet_label_map(const float* p, int n_labels, int64_t spatial, const int32_t* labels, int act, float threshold,
                        int hierarchy, int sum_then_threshold, int16_t* out, void* stream) {
   return launch_label_map(p, n_labels, spatial, labels, act, threshold, hierarchy, sum_then_threshold, out, to_stream(stream));
+}
+
+size_t b200unet_augment_scratch_bytes(int n, int c, int64_t spatial) { return augment_scratch_bytes(n, c, spatial); }
+int b200unet_augment_resample(const float* image, const uint8_t* label, int n, int c, int l, int d, int h, int w, const float* affine,
+                              int padding, int nonzero, float* image_out, uint8_t* label_out, void* scratch, void* stream) {
+  return launch_augment_resample(image, label, n, c, l, d, h, w, affine, padding, nonzero, image_out, label_out, scratch,
+                                 to_stream(stream));
+}
+int b200unet_augment_intensity(float* image, int n, int c, int64_t spatial, int normalize, int nonzero, int channel_wise,
+                               const float* coef, void* scratch, void* stream) {
+  return launch_augment_intensity(image, n, c, spatial, normalize, nonzero, channel_wise, coef, scratch, to_stream(stream));
 }
 
 size_t b200unet_cc_scratch_bytes(int nvol, int d, int h, int w) { return cc_scratch_bytes(nvol, d, h, w); }

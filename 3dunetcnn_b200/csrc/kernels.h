@@ -106,6 +106,17 @@ int launch_zscore(const float* x, int groups, long long S, int nonzero, double* 
 int launch_label_map(const float* p, int L, long long S, const int32_t* labels, int act, float thr, int hierarchy,
                      int sum_then_threshold, int16_t* out, cudaStream_t st);
 
+// ---- random flips / rotation + z-score + scale / shift of a training batch (augment.cu)
+#define B200_AUG_MAX_CHANNELS 16
+// scratch: stats [N][C][3] fp64 (sum, sumsq, count), then the per-block partials of the resample pass; 0: the shape is rejected
+size_t augment_scratch_bytes(int N, int C, long long S);
+// affine: DEVICE [N][12] fp32 row-major 3x4 (output index (d, h, w) -> source index); padding 0 border, 1 zeros; L = 0: no label
+int launch_augment_resample(const float* img, const uint8_t* lab, int N, int C, int L, int D, int H, int W, const float* affine,
+                            int padding, int nonzero, float* img_out, uint8_t* lab_out, void* scratch, cudaStream_t st);
+// in place on the resampled image; coef: DEVICE [N][C][2] (a, b)
+int launch_augment_intensity(float* img, int N, int C, long long S, int normalize, int nonzero, int channel_wise, const float* coef,
+                             void* scratch, cudaStream_t st);
+
 // ---- connected components of binary masks (ccl.cu)
 size_t cc_scratch_bytes(int nvol, int d, int h, int w);   // 0: the shape is rejected
 int launch_cc_label(const uint8_t* mask, int nvol, int d, int h, int w, int connectivity, int32_t* labels, int32_t* counts,

@@ -144,6 +144,11 @@ _SIGS = {
     "b200unet_zscore": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200unet_label_map": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.POINTER(C.c_int32), C.c_int, C.c_float, C.c_int, C.c_int,
                                      C.c_void_p, C.c_void_p]),
+    "b200unet_augment_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int64]),
+    "b200unet_augment_resample": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int] * 6 + [C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200unet_augment_intensity": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                             C.c_void_p, C.c_void_p]),
     "b200unet_cc_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
     "b200unet_cc_label": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_void_p]),

@@ -142,12 +142,13 @@ class GraphedTrainStep:
 class DevicePrefetcher:
     """Iterates a loader of ``{"image", "label"}`` items one batch ahead: the next batch's host->device copies run on a
     side stream while the current step computes (the reference copies synchronously from pageable memory on the compute
-    stream: training_utils.py:89-91).  Pageable tensors still work, they just do not overlap."""
+    stream: training_utils.py:89-91).  Pageable tensors still work, they just do not overlap.  ``transform`` (optional, e.g.
+    an ``augment.Compose``) runs on each staged batch on the same side stream, after its copies."""
 
     _streams = {}    # one copy stream per device, kept across epochs (stream creation is not free)
 
-    def __init__(self, loader, device):
-        self.loader, self.device = loader, device
+    def __init__(self, loader, device, transform=None):
+        self.loader, self.device, self.transform = loader, device, transform
         key = torch.device(device).index if torch.device(device).index is not None else torch.cuda.current_device()
         if key not in DevicePrefetcher._streams:
             DevicePrefetcher._streams[key] = torch.cuda.Stream(device=device)
@@ -162,6 +163,8 @@ class DevicePrefetcher:
             for k in ("image", "label"):
                 t = item[k]
                 out[k] = t if t.is_cuda else t.to(self.device, non_blocking=True)
+            if self.transform is not None:
+                out = self.transform(out)
             ev = torch.cuda.Event()
             ev.record(self.stream)
         return out, ev
@@ -227,19 +230,23 @@ def _graphed_step_for(model, criterion, optimizer, images, target, grad_sync):
 
 def epoch_training(train_loader, model, criterion, optimizer, epoch, n_gpus=None, print_frequency=1,
                    print_gpu_memory=False, scaler=None, samples_per_epoch=None, iteration=1, grad_sync=None,
-                   use_cuda_graph=False):
+                   use_cuda_graph=False, device_transform=None):
     """training_utils.py:20-85.  ``grad_sync`` (optional callable) runs between backward and optimizer.step:
     the data-parallel gradient all-reduce of ``parallel.GradAllReduce``.  ``use_cuda_graph``: replay the step through
     ``GraphedTrainStep`` (kept on the model across epochs) for every batch of the first batch's shape; other shapes,
     e.g. a short last batch, run eagerly.  On a GPU the loader is read one batch ahead (``DevicePrefetcher``) and the
-    loss of step i is read back while step i+1 runs, so the only host syncs are one step behind the queue."""
+    loss of step i is read back while step i+1 runs, so the only host syncs are one step behind the queue.
+    ``device_transform`` (optional, e.g. the ``Compose`` of ``augment.build_device_transform``) runs on every staged training
+    batch on the prefetcher's copy stream, overlapping the running step; it keeps each batch's shapes and dtypes."""
     graphed = None
     batch_time = AverageMeter("Time", ":6.3f")
     data_time = AverageMeter("Data", ":6.3f")
     losses = AverageMeter("Loss", ":.4e")
     model.train()
     on_gpu = n_gpus is not None and torch.cuda.is_available() and next(model.parameters()).is_cuda
-    loader = DevicePrefetcher(train_loader, next(model.parameters()).device) if on_gpu else train_loader
+    if device_transform is not None and not on_gpu:
+        raise RuntimeError("epoch_training: device_transform needs the model on a CUDA device and n_gpus set")
+    loader = DevicePrefetcher(train_loader, next(model.parameters()).device, device_transform) if on_gpu else train_loader
     lag = _LaggedLoss() if on_gpu else None
     end = time.time()
     batch_size = 0

@@ -188,6 +188,27 @@ int b200unet_zscore(const float* x, int groups, int64_t spatial, int nonzero, do
 int b200unet_label_map(const float* p, int n_labels, int64_t spatial, const int32_t* labels, int act, float threshold,
                        int hierarchy, int sum_then_threshold, int16_t* out, void* stream);
 
+/* ---- random augmentation of a training batch (MONAI RandFlipd / RandRotated, NormalizeIntensityd, RandScaleIntensityd /
+ * RandShiftIntensityd as datasets/segmentation.py:72-94 chains them), two passes over the image.
+ *   scratch_bytes: from the shape alone (0 = rejected: 1..16 image channels, d*h*w < 2^31).  The scratch starts with stats
+ *                  [n][c][3] fp64 (sum, sumsq, count) of the resampled image, over the non-zero voxels when nonzero = 1.
+ *   resample:      image fp32 [n][c][d][h][w] -> image_out (trilinear), label uint8 [n][l][d][h][w] -> label_out (nearest, round
+ *                  half to even; l = 0: no label).  affine: DEVICE fp32 [n][3][4], output index (d, h, w, 1) -> source index.
+ *                  padding 0 = border (clamp the source coordinate to [0, size-1]), 1 = zeros; as grid_sample(align_corners=False)
+ *                  on index coordinates.  Corners of weight 0 are not read: an axis flip copies every value bit for bit.
+ *                  Writes the stats of image_out.
+ *   intensity:     in place on the resampled image, after resample with the same scratch: y = ((x - mean) / std) * a + b with
+ *                  coef DEVICE fp32 [n][c][2] = (a, b); statistics per (n, c) when channel_wise, else per n; std 0 -> 1;
+ *                  normalize = 0: y = x * a + b, and planes with (a, b) = (1, 0) stay untouched; nonzero = 1: zero voxels
+ *                  skip the z-score.  Any 4-byte aligned image pointer (16-byte aligned ones with d*h*w a multiple of 4 take
+ *                  vector loads).
+ * No floating-point atomics: bit-identical run to run. */
+size_t b200unet_augment_scratch_bytes(int n, int c, int64_t spatial);
+int b200unet_augment_resample(const float* image, const uint8_t* label, int n, int c, int l, int d, int h, int w, const float* affine,
+                              int padding, int nonzero, float* image_out, uint8_t* label_out, void* scratch, void* stream);
+int b200unet_augment_intensity(float* image, int n, int c, int64_t spatial, int normalize, int nonzero, int channel_wise,
+                               const float* coef, void* scratch, void* stream);
+
 /* ---- connected components of binary masks (the clean-up after the path: SimpleITK ConnectedComponent + RelabelComponent,
  * MONAI KeepLargestConnectedComponent).  mask uint8 [nvol][d][h][w], nonzero = foreground; each volume is labelled on its own;
  * d*h*w < 2^31.  connectivity in orthogonal hops: 1 = 6 face neighbours, 2 = 18 (+ edges), 3 = 26 (+ corners).
