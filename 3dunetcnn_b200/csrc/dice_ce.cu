@@ -5,11 +5,13 @@
 //         I = sum p*t, P = sum p (or p^2), T = sum t (or t^2), f = 1 - (2I + nr) / (P + T + dr)   [jaccard: 2(P + T - I)]
 //         include_background = 0 drops channel 0 after the activation; batch pools the sums over n; mean or sum of f
 //   CE:   on the raw logits.  C > 1: -sum_c t_c log_softmax(x)_c (a label map is its one-hot row); C == 1: BCEWithLogits(x, t).
-//         mean divides by N*S, sum sums.
+//         mean divides by N*S, sum sums.  lambda_ce = 0: no CE work at all, so logits of +-inf leave a sigmoid Dice finite
+//         (0 * the NaN of inf - inf would not be).
 // A label outside [0, C) is an all-zero target row: it adds nothing to I, T or CE and is never used as an index.
 //
 // Logits are NCDHW fp32, so every channel of a sample is a contiguous run of S floats.  Both passes stage a tile of kV voxels x
-// all C channels in shared memory (cp.async, one HBM read of the logits) and compute the per-voxel softmax statistics from it.
+// all C channels in shared memory (cp.async, one HBM read of the logits) and compute the per-voxel softmax statistics from it
+// when the CE term or a softmax needs them.
 //   forward:  thread v of the tile: max, sum of exponentials, CE term; then thread (c, slice) accumulates channel c's (I, P, T)
 //             over a slice of the tile's voxels in registers across the block's tiles.  Each block writes its partial sums to its
 //             own slot; k_dice_ce_reduce adds the slots in a fixed order in fp64 and k_dice_ce_finalize forms the loss and the
@@ -115,10 +117,11 @@ __device__ __forceinline__ Smem carve(unsigned char* base, int C, int kind) {
   return s;
 }
 
-// grid (grid_x, N).  part [N][C][slots][3] (I, P, T), ce_part [N][slots]
+// grid (grid_x, N).  part [N][C][slots][3] (I, P, T), ce_part [N][slots] (zero without with_ce)
 template <int TK, int ACT>
 __global__ void __launch_bounds__(kThreads) k_dice_ce_fwd(const float* __restrict__ x, const void* __restrict__ tgt, int C, long long S,
-                                                          int squared, double* __restrict__ part, double* __restrict__ ce_part) {
+                                                          int squared, int with_ce, double* __restrict__ part,
+                                                          double* __restrict__ ce_part) {
   extern __shared__ __align__(16) unsigned char smem[];
   const Smem sm = carve(smem, C, TK);
   const int n = blockIdx.y, tid = threadIdx.x, slots = gridDim.x;
@@ -131,7 +134,7 @@ __global__ void __launch_bounds__(kThreads) k_dice_ce_fwd(const float* __restric
     const int nv = (int)(S - s0 < kV ? S - s0 : kV);
     stage_tile<TK>(xn, tgt, n, C, S, s0, nv, sm.xs, sm.ts, sm.lab);
     // phase A: one voxel per thread -- softmax statistics and the CE term
-    if (tid < nv) {
+    if ((with_ce || ACT == A_SOFTMAX) && tid < nv) {
       const int v = tid;
       float ce;
       if (C == 1) {
@@ -259,17 +262,19 @@ __global__ void k_dice_ce_finalize(const double* __restrict__ sums, const double
       if (d.jaccard) den = 2.0 * (den - I);
       acc += 1.0 - (2.0 * I + d.smooth_nr) / (den + d.smooth_dr);
     }
-  double cet = 0;
-  for (int n = 0; n < N; ++n) cet += ce[n];
-  const double dice = d.reduction == 0 ? acc / terms : acc;
-  const double cel = d.reduction == 0 ? cet / ((double)N * S) : cet;
-  *loss = (float)(d.lambda_dice * dice + d.lambda_ce * cel);
+  double l = d.lambda_dice * (d.reduction == 0 ? acc / terms : acc);
+  if (d.lambda_ce != 0.f) {
+    double cet = 0;
+    for (int n = 0; n < N; ++n) cet += ce[n];
+    l += d.lambda_ce * (d.reduction == 0 ? cet / ((double)N * S) : cet);
+  }
+  *loss = (float)l;
 }
 
 // grid (grid_x, N); one voxel per thread
 template <int TK, int ACT>
 __global__ void __launch_bounds__(kThreads) k_dice_ce_bwd(const float* __restrict__ x, const void* __restrict__ tgt, int C, long long S,
-                                                          int squared, double ce_scale, const double* __restrict__ coef,
+                                                          int squared, int with_ce, double ce_scale, const double* __restrict__ coef,
                                                           const float* __restrict__ grad_out, float* __restrict__ dx) {
   extern __shared__ __align__(16) unsigned char smem[];
   const Smem sm = carve(smem, C, TK);
@@ -299,16 +304,18 @@ __global__ void __launch_bounds__(kThreads) k_dice_ce_bwd(const float* __restric
         *o = (ACT == A_SIGMOID ? g * p * (1.f - p) : g) + cg * (q - t);
       } else {
         const int l = TK < T_ONEHOT_U8 ? sm.lab[v] : -1;
-        float m = -INFINITY;
-        for (int k = 0; k < C; ++k) m = fmaxf(m, sm.xs[k * kP + v]);
-        float sum = 0.f, tsum = 0.f;
-        for (int k = 0; k < C; ++k) {
-          const float e = __expf(sm.xs[k * kP + v] - m);
-          sum += e;
-          if (ACT == A_SOFTMAX) sm.xs[k * kP + v] = e;
-          if (TK >= T_ONEHOT_U8) tsum += sm.ts[k * kP + v];
+        float m = -INFINITY, inv = 0.f, tsum = 0.f;
+        if (with_ce || ACT == A_SOFTMAX) {
+          for (int k = 0; k < C; ++k) m = fmaxf(m, sm.xs[k * kP + v]);
+          float sum = 0.f;
+          for (int k = 0; k < C; ++k) {
+            const float e = __expf(sm.xs[k * kP + v] - m);
+            sum += e;
+            if (ACT == A_SOFTMAX) sm.xs[k * kP + v] = e;
+            if (TK >= T_ONEHOT_U8) tsum += sm.ts[k * kP + v];
+          }
+          inv = 1.f / sum;
         }
-        const float inv = 1.f / sum;
         if (TK < T_ONEHOT_U8) tsum = l >= 0 ? 1.f : 0.f;
         if (ACT == A_SOFTMAX) {
           float s = 0.f;
@@ -326,11 +333,11 @@ __global__ void __launch_bounds__(kThreads) k_dice_ce_bwd(const float* __restric
         } else {
           for (int k = 0; k < C; ++k) {
             const float xv = sm.xs[k * kP + v];
-            const float q = __expf(xv - m) * inv;
             const float p = ACT == A_SIGMOID ? sigm(xv) : xv;
             const float t = TK >= T_ONEHOT_U8 ? sm.ts[k * kP + v] : (k == l ? 1.f : 0.f);
             const float g = a[k] * t + b[k] * (squared ? 2.f * p : 1.f);
-            o[(long long)k * S] = (ACT == A_SIGMOID ? g * p * (1.f - p) : g) + cg * (q * tsum - t);
+            const float dd = ACT == A_SIGMOID ? g * p * (1.f - p) : g;
+            o[(long long)k * S] = with_ce ? dd + cg * (__expf(xv - m) * inv * tsum - t) : dd;
           }
         }
       }
@@ -404,9 +411,10 @@ int launch_dice_ce_fwd(const DiceCEDesc& d, const float* logits, const void* tar
   const Scratch s = carve_scratch(scratch, sh);
   const size_t smem = tile_smem(sh.C, sh.kind);
   const dim3 grid(sh.slots, N);
-#define B200_FWD(tk, ac)                                                                                       \
-  B200_TRY(set_smem(k_dice_ce_fwd<tk, ac>, smem));                                                             \
-  k_dice_ce_fwd<tk, ac><<<grid, kThreads, smem, st>>>(logits, target, C, S, d.squared_pred, s.part, s.ce_part);
+  const int with_ce = d.lambda_ce != 0.f;
+#define B200_FWD(tk, ac)                                                                                                \
+  B200_TRY(set_smem(k_dice_ce_fwd<tk, ac>, smem));                                                                      \
+  k_dice_ce_fwd<tk, ac><<<grid, kThreads, smem, st>>>(logits, target, C, S, d.squared_pred, with_ce, s.part, s.ce_part);
   B200_DICE_CE_SWITCH(B200_FWD)
 #undef B200_FWD
   B200_CHECK_CUDA(cudaGetLastError());
@@ -425,10 +433,12 @@ int launch_dice_ce_bwd(const DiceCEDesc& d, const float* logits, const void* tar
   const Scratch s = carve_scratch(const_cast<void*>(scratch), sh);
   const size_t smem = tile_smem(sh.C, sh.kind);
   const dim3 grid(sh.slots, N);
+  const int with_ce = d.lambda_ce != 0.f;
   const double ce_scale = d.lambda_ce * (d.reduction == 0 ? 1.0 / ((double)N * S) : 1.0);
 #define B200_BWD(tk, ac)                                                                                                 \
   B200_TRY(set_smem(k_dice_ce_bwd<tk, ac>, smem));                                                                       \
-  k_dice_ce_bwd<tk, ac><<<grid, kThreads, smem, st>>>(logits, target, C, S, d.squared_pred, ce_scale, s.coef, grad_out, dlogits);
+  k_dice_ce_bwd<tk, ac><<<grid, kThreads, smem, st>>>(logits, target, C, S, d.squared_pred, with_ce, ce_scale, s.coef,   \
+                                                      grad_out, dlogits);
   B200_DICE_CE_SWITCH(B200_BWD)
 #undef B200_BWD
   B200_CHECK_CUDA(cudaGetLastError());

@@ -142,7 +142,8 @@ int b200unet_dice_bwd(const float* logits, const void* target, int n, int c, int
 /* ---- Dice + cross-entropy criterion (monai.losses.DiceCELoss): loss = lambda_dice * Dice(act(x), t) + lambda_ce * CE(x, t).
  * Dice is the formula above on p = act(x); include_background = 0 drops channel 0 after the activation.  CE is on the raw
  * logits: -sum_c t_c log_softmax(x)_c for c > 1 (a label map is its one-hot row), BCEWithLogits(x, t) for c == 1; mean
- * divides by n * spatial.  With c == 1 softmax is ignored and a uint8 label map is the target itself (int64: E_UNSUPPORTED).
+ * divides by n * spatial.  lambda_ce = 0 means the CE term is not evaluated, so logits of +-inf give a finite sigmoid Dice
+ * loss and gradient.  With c == 1 softmax is ignored and a uint8 label map is the target itself (int64: E_UNSUPPORTED).
  * A label outside [0, c) is an all-zero target row.  logits NCDHW fp32, 1 <= c <= 128.
  * scratch: b200unet_dice_ce_scratch_bytes() bytes (0 = the options or shape are rejected), written by fwd and read by bwd.
  * It starts with sums [n][c][3] fp64 (I, P, T) and ce [n] fp64 (the summed CE terms of each sample).  No floating-point

@@ -4,7 +4,7 @@ bit equality, a UNet3D training step on a label map, and CUDA-graph steps on lab
 import pytest
 import torch
 
-from oracle import UNetConfig, make_state_dict, unet3d_forward
+from oracle import UNetConfig, dice_loss, make_state_dict, unet3d_forward
 from oracle.dynunet_oracle import make_dynunet_state_dict
 from dice_ce_oracle import dice_ce_loss
 from test_dice_ce_host import X, T
@@ -116,6 +116,24 @@ def test_out_of_range_labels_are_all_zero_rows(pkg, dtype, bad):
         vo, go = _oracle(x, lab, **kw)
         assert abs(v - vo) <= 1e-5 * abs(vo)
         assert _rel(gr, go) <= 1e-4
+
+
+@pytest.mark.parametrize("c", [1, 3])
+@pytest.mark.parametrize("soft", [False, True])
+def test_dice_alone_stays_finite_at_infinite_logits(pkg, c, soft):
+    """lambda_ce = 0 evaluates no CE term: a sigmoid saturates at +-inf, so the loss and dlogits equal fp64 DiceLoss"""
+    g = torch.Generator().manual_seed(9)
+    x = torch.randn(2, c, 5, 6, 7, generator=g)
+    x.view(-1)[::7] = float("inf")
+    x.view(-1)[3::11] = -float("inf")
+    t = torch.rand(x.shape, generator=g) if soft else (torch.rand(x.shape, generator=g) > 0.5).to(torch.uint8)
+    for kw in (dict(), dict(squared_pred=True, batch=True), dict(jaccard=True, reduction="sum")):
+        v, gr = _run(pkg, x, t, sigmoid=True, lambda_ce=0.0, **kw)
+        xr = x.double().requires_grad_(True)
+        lr = dice_loss(xr, t, sigmoid=True, **kw)
+        lr.backward()
+        assert abs(v - float(lr)) <= 1e-5 * abs(float(lr)), (kw, v, float(lr))
+        assert bool(torch.isfinite(gr).all()) and _rel(gr, xr.grad) <= 1e-4, kw
 
 
 def test_bit_identical_run_to_run_at_104_classes(pkg):
