@@ -12,17 +12,21 @@ namespace b200 {
 // voxels around it (its zero padding = TMA out-of-bounds fill), box row ((dz * BH) + hy) * BW + wx.  Output row r = h * TW + w of
 // tap (kd, kh, kw) reads box row tap_row + h * BW + w: each 8-row group (one h) is 8 consecutive box rows and the next group
 // starts GROUP_STRIDE rows further (the wgmma SBO).  Descriptors may start at any row inside the swizzled box: the swizzle is a
-// function of the absolute shared-memory address, for the TMA writes and for the wgmma reads alike.
-struct HaloTile {
-  static constexpr int TW = 8, TH = 16, TD = 1;
+// function of the absolute shared-memory address, for the TMA writes and for the wgmma reads alike.  With TD output planes per
+// box, output plane z is its own 128-row M tile and reads the box from row z * PLANE on.
+template <int TD_>
+struct HaloBox {
+  static constexpr int TW = 8, TH = 16, TD = TD_;
   static constexpr int BW = TW + 2, BH = TH + 2, BD = TD + 2;
-  static constexpr int ROWS = BW * BH * BD;
+  static constexpr int PLANE = BW * BH;
+  static constexpr int ROWS = PLANE * BD;
   static constexpr int GROUP_STRIDE = BW;
   static constexpr int HALF_M = 64 / TW * BW;   // box rows from output row 0 to output row 64 (the second m64 half)
-  static_assert(TW == 8 && TW * TH == 128 && TD == 1, "one 128-row M tile of 8-row groups in one plane");
-  // tap = kd * 9 + kh * 3 + kw
+  static_assert(TW == 8 && TW * TH == 128 && TD >= 1, "one 128-row M tile of 8-row groups per output plane");
+  // tap = kd * 9 + kh * 3 + kw, of output plane 0
   __host__ __device__ static constexpr int tap_row(int tap) { return (tap / 9 * BH + tap / 3 % 3) * BW + tap % 3; }
 };
+using HaloTile = HaloBox<1>;
 
 // Channel buckets: K chunk (16 / 32 / 64) and N tile (16 / 32 / 64 / 128) for c channels.
 static inline int kc_bucket(int c) { return c > 32 ? 64 : c > 16 ? 32 : 16; }

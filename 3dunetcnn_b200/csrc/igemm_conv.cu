@@ -27,8 +27,9 @@ namespace b200 {
 // mode: the 3x3x3 stride-1 source, one K chunk wide, is loaded as ONE halo box around the output tile (HaloTile), and the 27
 // taps read it through shifted shared-memory descriptors (27x less activation traffic from L2 than per-tap boxes).
 // CONV_HALO_WS is halo mode on the persistent, weight-stationary kernel (k_igemm_conv_halo_ws) for the (BN, KC) whose 27 weight
-// tiles fit in shared memory beside the halo box; CONV_HALO runs the ring kernel below for the wider ones.
-enum ConvMode { CONV_STREAM = 0, CONV_CLASS = 1, CONV_HALO = 2, CONV_HALO_WS = 3 };
+// tiles fit in shared memory beside the halo box; CONV_HALO runs the ring kernel below for the wider ones.  CONV_HALO_PAIR
+// (k_igemm_conv_halo_pair) shares resident weights and one two-plane halo box between two consumer warpgroups.
+enum ConvMode { CONV_STREAM = 0, CONV_CLASS = 1, CONV_HALO = 2, CONV_HALO_WS = 3, CONV_HALO_PAIR = 4 };
 
 // Tile sizes and shared-memory limits both convolution kernels derive from (BN, KC).
 template <int BN, int KC>
@@ -87,18 +88,19 @@ __device__ __forceinline__ void store_acc(float* s_acc, const float (&acc)[2][BN
   }
 }
 
-// Mode 1: the norm coefficients of sample n for the N tile at n0 -> s_coef (zero beyond Cout).
+// Mode 1: the norm coefficients of sample n for the N tile at n0 -> s_coef (zero beyond Cout), by the 128 threads tid of one
+// consumer warpgroup.
 template <int BN>
-__device__ __forceinline__ void load_coef(float4* s_coef, const ConvArgs& p, int n, int n0) {
-  for (int c = threadIdx.x; c < BN; c += 128)
+__device__ __forceinline__ void load_coef(float4* s_coef, const ConvArgs& p, int n, int n0, int tid) {
+  for (int c = tid; c < BN; c += 128)
     s_coef[c] = (n0 + c < p.Cout) ? p.coef[(long long)n * p.coef_ld + n0 + c] : make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
 // The epilogue warps' fp32 partial sums of sample n -> one fp64 atomic per channel statistic into dst [N][ld][2] (mode 0:
-// stats, mode 1: bstats); `restart` zeroes the slots for the next tile.
+// stats, mode 1: bstats), by the 128 threads tid of the warpgroup that owns s_stats; `restart` zeroes the slots for the next tile.
 template <int BN>
-__device__ __forceinline__ void flush_stats(float* s_stats, double* dst, int ld, int Cout, int n, int n0, bool restart) {
-  for (int c = threadIdx.x; c < BN * 2; c += 128) {
+__device__ __forceinline__ void flush_stats(float* s_stats, double* dst, int ld, int Cout, int n, int n0, bool restart, int tid) {
+  for (int c = tid; c < BN * 2; c += 128) {
     const float v = s_stats[c] + s_stats[BN * 2 + c] + s_stats[2 * BN * 2 + c] + s_stats[3 * BN * 2 + c];
     if (restart) { s_stats[c] = 0.f; s_stats[BN * 2 + c] = 0.f; s_stats[2 * BN * 2 + c] = 0.f; s_stats[3 * BN * 2 + c] = 0.f; }
     if (n0 + (c >> 1) < Cout) atomicAdd(&dst[((long long)n * ld + n0) * 2 + c], (double)v);
@@ -152,7 +154,7 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
   pdl_wait();   // before the first global read (the coefficient table below); the barrier set-up above overlaps the previous kernel
   if (warp < 4) {
     for (int i = threadIdx.x; i < 4 * BN * 2; i += 128) s_stats[i] = 0.f;
-    if (p.mode == 1) load_coef<BN>(s_coef, p, n, n0);
+    if (p.mode == 1) load_coef<BN>(s_coef, p, n, n0, threadIdx.x);
   }
   __syncthreads();
   pdl_launch_dependents();
@@ -312,7 +314,8 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
   }
   if (want_stats) {
     asm volatile("bar.sync 1, 128;" ::: "memory");
-    flush_stats<BN>(s_stats, (p.mode == 0) ? p.stats : p.bstats, (p.mode == 0) ? p.stats_ld : p.coef_ld, p.Cout, n, n0, false);
+    flush_stats<BN>(s_stats, (p.mode == 0) ? p.stats : p.bstats, (p.mode == 0) ? p.stats_ld : p.coef_ld, p.Cout, n, n0, false,
+                    threadIdx.x);
   }
   if (threadIdx.x == 0) tma_store_wait_all();   // the staging tile must outlive the bulk store
 }
@@ -492,7 +495,7 @@ __global__ void __launch_bounds__(160, (HaloWsCfg<BN, KC>::BLOCKS_PER_SM)) k_ige
     // every warp's MMAs have retired (the ring lived in R) and the previous store has read R
     asm volatile("bar.sync 1, 128;" ::: "memory");
     if (p.mode == 1 && n != coef_n) {   // the previous epilogue's reads of s_coef ended before its last barrier
-      load_coef<BN>(s_coef, p, n, n0);
+      load_coef<BN>(s_coef, p, n, n0, threadIdx.x);
       coef_n = n;
     }
     store_acc<BN, Cfg::ACC_LD>(s_acc, acc, warp, lane);
@@ -509,20 +512,207 @@ __global__ void __launch_bounds__(160, (HaloWsCfg<BN, KC>::BLOCKS_PER_SM)) k_ige
       tma_store_5d(&maps.o[0], reg, n0, w0, h0, d0, n);
       tma_store_commit();
     }
-    if (want_stats) flush_stats<BN>(s_stats, stats_dst, stats_ld, p.Cout, n, n0, true);   // the slots restart from zero
+    if (want_stats) flush_stats<BN>(s_stats, stats_dst, stats_ld, p.Cout, n, n0, true, threadIdx.x);   // the slots restart from zero
   }
   if (threadIdx.x == 0) tma_store_wait_all();   // the staging tile must outlive the bulk store
+}
+
+// Two-plane halo mode, for the (BN, KC) whose 27 resident weight tiles take 27 x 2048 x 2 = 110,592 B: beside a halo box they
+// do not fit in half the SM's shared memory, so the weight-stationary kernel runs them at one CTA per SM (whose single warpgroup
+// leaves the tensor cores idle through its epilogue) and per-tap tiles reload every tap's box from L2.  Here one CTA per SM runs
+// two consumer warpgroups and a TMA producer warp.  A unit of work is two 8 x 16 x 1 output tiles in consecutive planes of one
+// sample; the producer loads ONE halo box (KC, 10, 18, 4) per unit, and warpgroup g computes output plane d0 + g from the box's
+// plane g on (HaloBox<2>), taps 0..26 with the k16 steps inside each, as the other kernels.  Both warpgroups' MMAs share the
+// resident weights; the next unit's box loads once both have retired theirs, under the two epilogues.  The epilogues take turns
+// on one region R (fp32 accumulator tile, then the bf16 staging tile): warpgroup 0 first, and R passes to the other warpgroup once
+// the TMA store has read it.
+// Shared memory: resident weights [27][BN][KC] | halo box | R | aux (barriers | per-warp stats of 8 warps | coef per warpgroup).
+template <int BN, int KC>
+struct HaloPairCfg : ConvTileCfg<BN, KC> {
+  using Tile = ConvTileCfg<BN, KC>;
+  using Box = HaloBox<2>;
+  static constexpr bool APPLIES = BN * KC == 2048 && BN <= 64;
+  static constexpr int STAGES = 2;                          // output tiles in flight per unit: one per consumer warpgroup
+  static constexpr int BLOCKS_PER_SM = 1;
+  static constexpr int W_BYTES = (27 * Tile::B_BOX_BYTES + 1023) / 1024 * 1024;
+  static constexpr int BOX_TX = Box::ROWS * Tile::RB;
+  static constexpr int BOX_BYTES = (BOX_TX + 1023) / 1024 * 1024;
+  static constexpr int ACC_R = (Tile::ACC_BYTES + 1023) / 1024 * 1024;   // > the 128 x BN bf16 staging tile
+  static constexpr int STG_BYTES = 128 * BN * 2;
+  static constexpr int AUX_BYTES = 1024 + 8 * BN * 2 * 4 + 2 * BN * 16;
+  static constexpr int FIXED = W_BYTES + BOX_BYTES + ACC_R + AUX_BYTES + 1024;   // +1024 alignment slack
+  // The staging tile follows the accumulator tile in R where it fits.  Otherwise it overwrites the accumulator tile, and each
+  // thread first copies its accumulator row into registers: 64 more registers per thread, which BN = 64 does not have at
+  // 288 threads (168 per thread).
+  static constexpr bool STG_APART = FIXED + STG_BYTES <= Tile::SMEM_LIMIT;
+  static constexpr int R_BYTES = ACC_R + (STG_APART ? STG_BYTES : 0);
+  static constexpr int SMEM_BYTES = FIXED + (STG_APART ? STG_BYTES : 0);
+  // (32, 64): 110,592 + 92,160 + 18,432 + 4,096 + 1,024 = 226,304 B, staging in the accumulator tile; (64, 32): 110,592 +
+  // 46,080 + 34,816 + 16,384 + 7,168 + 1,024 = 216,064 B.  A second region R (one per warpgroup) or a second box does not fit.
+  static_assert(!APPLIES || (SMEM_BYTES <= Tile::SMEM_LIMIT && (BN <= 32 || STG_APART) && SMEM_BYTES + R_BYTES > Tile::SMEM_LIMIT &&
+                             SMEM_BYTES + BOX_BYTES > Tile::SMEM_LIMIT),
+                "igemm_conv: two-plane halo layout");
+};
+
+template <int BN, int KC>
+__global__ void __launch_bounds__(288, 1) k_igemm_conv_halo_pair(const __grid_constant__ ConvMaps maps, const ConvArgs p) {
+  using Cfg = HaloPairCfg<BN, KC>;
+  using Box = typename Cfg::Box;
+  static_assert(Cfg::APPLIES, "igemm_conv: no two-plane halo configuration");
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* wts = smem;
+  uint8_t* box = smem + Cfg::W_BYTES;
+  uint8_t* reg = box + Cfg::BOX_BYTES;
+  uint8_t* aux = reg + Cfg::R_BYTES;
+  uint64_t* w_full = reinterpret_cast<uint64_t*>(aux);
+  uint64_t* box_full = w_full + 1;
+  uint64_t* box_empty = w_full + 2;
+  uint64_t* turn = w_full + 3;                    // [2]: warpgroup g may use R once turn[g] has completed its phase
+  float* s_stats_all = reinterpret_cast<float*>(aux + 1024);   // [8 warps][BN][2]
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int wg = warp >> 2;                       // consumer warpgroup (2: the producer warp)
+  const int tid = threadIdx.x & 127;
+  const int pairs_d = (p.tiles_d + 1) >> 1;
+  const int nunits = p.N * pairs_d * p.tiles_h * p.tiles_w;
+  const int n0 = blockIdx.y * BN;
+  auto unit_origin = [&](int u, int& w0, int& h0, int& d0, int& n) {
+    w0 = (u % p.tiles_w) * Box::TW; u /= p.tiles_w;
+    h0 = (u % p.tiles_h) * Box::TH; u /= p.tiles_h;
+    d0 = (u % pairs_d) * Box::TD;
+    n = u / pairs_d;
+  };
+
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&maps.a[0][0]);
+    tma_prefetch_desc(&maps.b[0][0]);
+    mbar_init(w_full, 1);
+    mbar_init(box_full, 1);
+    mbar_init(box_empty, 8);
+    mbar_init(&turn[0], 1);
+    mbar_init(&turn[1], 1);
+    fence_barrier_init();
+  }
+  pdl_wait();   // before the first global read; the barrier set-up above overlaps the previous kernel
+  if (warp < 8)
+    for (int i = threadIdx.x; i < 8 * BN * 2; i += 256) s_stats_all[i] = 0.f;
+  __syncthreads();
+  pdl_launch_dependents();
+
+  if (warp == 8) {
+    // ------------------------------------------------------------------ TMA producer (convergent, one lane issues)
+    const uint32_t issue = elect_one() ? 1u : 0u;
+    mbar_expect_tx_if(issue, w_full, 27 * Cfg::B_BOX_BYTES);
+    for (int tap = 0; tap < 27; ++tap) tma_load_3d_if(issue, wts + tap * Cfg::B_BOX_BYTES, &maps.b[0][0], w_full, 0, n0, tap);
+    int j = 0;
+    for (int u = blockIdx.x; u < nunits; u += gridDim.x, ++j) {
+      int w0, h0, d0, n;
+      unit_origin(u, w0, h0, d0, n);
+      mbar_wait(box_empty, (j & 1) ^ 1);   // both warpgroups' MMAs on the previous box have retired
+      mbar_expect_tx_if(issue, box_full, Cfg::BOX_TX);
+      tma_load_5d_if(issue, box, &maps.a[0][0], box_full, 0, w0 - 1, h0 - 1, d0 - 1, n);
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumer warpgroups: wgmma, then the epilogue
+  float* s_stats = s_stats_all + wg * 4 * BN * 2;                                        // [4 warps][BN][2]
+  float4* s_coef = reinterpret_cast<float4*>(aux + 1024 + 8 * BN * 8) + wg * BN;        // [BN]
+  float* s_acc = reinterpret_cast<float*>(reg);
+  uint8_t* stage = Cfg::STG_APART ? reg + Cfg::ACC_R : reg;
+  constexpr uint32_t hi_d = desc_hi(Cfg::SBO, Cfg::LAYOUT);
+  constexpr uint32_t hi_halo = desc_hi(Box::GROUP_STRIDE * Cfg::RB, Cfg::LAYOUT);
+  constexpr uint32_t HALO_HALF = (Box::HALF_M * Cfg::RB) >> 4;   // halo: output rows 64-127
+  const uint32_t w_lo0 = desc_lo(smem_u32(wts), 16);
+  const uint32_t plane_lo = desc_lo(smem_u32(box), 16) + ((wg * Box::PLANE * Cfg::RB) >> 4);   // this warpgroup's output plane
+  const int row = tid;
+  const int wl = row % Box::TW, hl = row / Box::TW;
+  const bool want_stats = (p.mode == 0) ? (p.stats != nullptr) : (p.bstats != nullptr);
+  double* stats_dst = (p.mode == 0) ? p.stats : p.bstats;
+  const int stats_ld = (p.mode == 0) ? p.stats_ld : p.coef_ld;
+  auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); };
+  int j = 0, coef_n = -1;
+  mbar_wait(w_full, 0);
+  for (int u = blockIdx.x; u < nunits; u += gridDim.x, ++j) {
+    int w0, h0, d0, n;
+    unit_origin(u, w0, h0, d0, n);
+    const int w = w0 + wl, h = h0 + hl, d = d0 + wg;   // an odd Do leaves the second plane of the last pair outside: masked
+    const bool valid = (w < p.Wo) && (h < p.Ho) && (d < p.Do);
+    const bool edge = p.zero_last && (w == p.Wo - 1 || h == p.Ho - 1 || d == p.Do - 1);
+    const long long vox = (((long long)n * p.Do + d) * p.Ho + h) * p.Wo + w;
+    conv_epilogue_prefetch(p, n0, BN, vox, valid);   // -> L2 while the MMAs run
+
+    float acc[2][BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+    mbar_wait(box_full, j & 1);
+    wgmma_fence();
+#pragma unroll
+    for (int tap = 0; tap < 27; ++tap) {
+      const uint32_t a_lo = halo_tap_lo<Cfg::RB>(plane_lo, tap);
+      const uint32_t b_lo = w_lo0 + ((tap * Cfg::B_BOX_BYTES) >> 4);
+#pragma unroll
+      for (int k = 0; k < KC / 16; ++k) {
+        const uint32_t accumulate = (tap > 0 || k > 0) ? 1u : 0u;
+        Wgmma<BN>::template mma<0, 0>(acc[0], desc_from(a_lo + 2 * k, hi_halo), desc_from(b_lo + 2 * k, hi_d), accumulate);
+        Wgmma<BN>::template mma<0, 0>(acc[1], desc_from(a_lo + HALO_HALF + 2 * k, hi_halo), desc_from(b_lo + 2 * k, hi_d), accumulate);
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc[0]);
+    wgmma_fence_regs(acc[1]);
+    if (lane == 0) mbar_arrive(box_empty);
+
+    // R: warpgroup 0 takes it first in every unit (its first wait passes on the fresh barrier), warpgroup 1 after it
+    mbar_wait(&turn[wg], (j & 1) ^ (wg == 0 ? 1 : 0));
+    if (p.mode == 1 && n != coef_n) {   // this warpgroup's previous epilogue read s_coef before its last barrier
+      load_coef<BN>(s_coef, p, n, n0, tid);
+      coef_n = n;
+    }
+    store_acc<BN, Cfg::ACC_LD>(s_acc, acc, warp & 3, lane);
+    wg_sync();
+    if constexpr (Cfg::STG_APART) {
+      conv_epilogue_tile<BN>(p, s_acc + row * Cfg::ACC_LD, warp & 3, lane, n, n0, vox, valid, s_stats, s_coef, want_stats, edge,
+                             stage, row, false);
+    } else {
+      float4 acc_row[BN / 4];
+#pragma unroll
+      for (int i = 0; i < BN / 4; ++i) acc_row[i] = reinterpret_cast<const float4*>(s_acc + row * Cfg::ACC_LD)[i];
+      wg_sync();   // the staging tile below overwrites the accumulator tile
+      conv_epilogue_tile<BN>(p, reinterpret_cast<const float*>(acc_row), warp & 3, lane, n, n0, vox, valid, s_stats, s_coef,
+                             want_stats, edge, stage, row, false);
+    }
+    fence_proxy_async();
+    wg_sync();
+    if (tid == 0) {
+      if (d < p.Do) {
+        tma_store_5d(&maps.o[0], stage, n0, w0, h0, d, n);
+        tma_store_commit();
+        tma_store_wait_read0();   // the store has read R: the other warpgroup may overwrite it
+      }
+      mbar_arrive(&turn[wg ^ 1]);
+    }
+    if (want_stats) flush_stats<BN>(s_stats, stats_dst, stats_ld, p.Cout, n, n0, true, tid);   // the slots restart from zero
+  }
+  if (tid == 0) tma_store_wait_all();
 }
 
 // ----------------------------------------------------------------------------------------------- host side
 // The compile-time configuration of the kernel a (BN, KC, MODE) launch runs.
 template <int BN, int KC, int MODE>
-using ConvCfgOf = std::conditional_t<MODE == CONV_HALO_WS, HaloWsCfg<BN, KC>, ConvCfg<BN, KC, MODE>>;
+using ConvCfgOf = std::conditional_t<MODE == CONV_HALO_WS, HaloWsCfg<BN, KC>,
+                                     std::conditional_t<MODE == CONV_HALO_PAIR, HaloPairCfg<BN, KC>, ConvCfg<BN, KC, MODE>>>;
 
 template <int BN, int KC, int MODE>
 static int launch_cfg(const ConvMaps& maps, const ConvArgs& args, dim3 grid, cudaStream_t st, const ConvClassMaps& cmaps) {
   using Cfg = ConvCfgOf<BN, KC, MODE>;
-  if constexpr (MODE == CONV_HALO_WS) {
+  if constexpr (MODE == CONV_HALO_PAIR) {
+    B200_TRY((set_max_dynamic_smem<k_igemm_conv_halo_pair<BN, KC>>(Cfg::SMEM_BYTES)));
+    launch_pdl(k_igemm_conv_halo_pair<BN, KC>, grid, dim3(288), Cfg::SMEM_BYTES, st, maps, args);
+  } else if constexpr (MODE == CONV_HALO_WS) {
     B200_TRY((set_max_dynamic_smem<k_igemm_conv_halo_ws<BN, KC>>(Cfg::SMEM_BYTES)));
     launch_pdl(k_igemm_conv_halo_ws<BN, KC>, grid, dim3(160), Cfg::SMEM_BYTES, st, maps, args);
   } else {
@@ -578,17 +768,35 @@ static bool halo_keeps_occupancy(int BN, int KC) {
   return false;
 }
 
+static bool halo_pair_applies(int BN, int KC) {
+#define B200_HALO_PAIR(bn, kc) \
+  if (BN == bn && KC == kc) return HaloPairCfg<bn, kc>::APPLIES;
+  B200_CONV_CONFIGS(B200_HALO_PAIR)
+#undef B200_HALO_PAIR
+  return false;
+}
+
+// Two-plane halo mode (k_igemm_conv_halo_pair) for a halo-eligible op of its (BN, KC) with one source, when its units of two
+// output planes give every SM at least one: below that, pairing the tiles would leave SMs idle that the per-tile kernels use.
+static bool conv_halo_pair(const ConvOp& op, int num_sms) {
+  if (op.nsrc != 1 || !halo_pair_applies(conv_bn(op), conv_kc(op))) return false;
+  const long long units = (long long)op.out.N * ceil_div(op.out.D, 2) * ceil_div(op.out.H, HaloTile::TH) * ceil_div(op.out.W, HaloTile::TW);
+  return units * ceil_div(op.out.C, conv_bn(op)) >= num_sms;
+}
+
 // Halo mode (see ConvMode) for 3x3x3 stride-1 convolutions with <= 64 input channels (plus an optional fused 1x1x1 source)
-// whose output planes fill the halo tile, in single-pass bf16, when it keeps the configuration's CTAs per SM.  Wider inputs
-// stay on per-tap tiles: several halo boxes per tile were slower in the forward convolutions of the C2 step on the H100.
-static bool conv_halo_eligible(const ConvOp& op) {
+// whose output planes fill the halo tile, in single-pass bf16, when it keeps the configuration's CTAs per SM or runs in
+// two-plane halo mode.  Wider inputs stay on per-tap tiles: several halo boxes per tile were slower in the forward convolutions
+// of the C2 step on the H100.
+static bool conv_halo_eligible(const ConvOp& op, int num_sms) {
   if (halo_disabled() || op.cls_mode) return false;
   const ConvSrc& c = op.src[0];
   if (c.ksz != 3 || c.stride != 1 || c.nopad || c.x.C > 64) return false;
   if (op.nsrc == 2 && (op.src[1].ksz != 1 || op.src[1].stride != 1)) return false;
   for (int s = 0; s < op.nsrc; ++s)
     if (op.src[s].x.lo || op.src[s].w_lo) return false;
-  return op.out.W >= HaloTile::TW && op.out.H >= HaloTile::TH && halo_keeps_occupancy(conv_bn(op), conv_kc(op));
+  return op.out.W >= HaloTile::TW && op.out.H >= HaloTile::TH &&
+         (halo_keeps_occupancy(conv_bn(op), conv_kc(op)) || conv_halo_pair(op, num_sms));
 }
 
 template <int BN_, int KC_, int MODE_>
@@ -604,7 +812,9 @@ static int with_conv_kernel(int kind, int BN, int KC, F&& f) {
       if constexpr (bn <= 64) return f(ConvKernel<bn, kc, CONV_CLASS>{});                                   \
     } else if (kind == CONV_KIND_HALO) {                                                                    \
       if constexpr (halo_keeps_occupancy<bn, kc>()) return f(ConvKernel<bn, kc, halo_mode<bn, kc>()>{});    \
-    } else {                                                                                                \
+    } else if (kind == CONV_KIND_HALO_PAIR) {                                                               \
+      if constexpr (HaloPairCfg<bn, kc>::APPLIES) return f(ConvKernel<bn, kc, CONV_HALO_PAIR>{});           \
+    } else {                                                                                              \
       return f(ConvKernel<bn, kc, CONV_STREAM>{});                                                          \
     }                                                                                                       \
   }
@@ -654,9 +864,14 @@ int conv_route(const ConvOp& op, int num_sms, ConvRoute* r) {
     B200_REQUIRE(op.gn_x && op.coef, E_INVALID, "igemm_conv: mode 1 needs gn_x and coef");
     B200_REQUIRE(op.gn_x->C == out.C, E_INVALID, "igemm_conv: gn_x channel mismatch");
   }
-  const bool halo = conv_halo_eligible(op);
-  r->kind = op.cls_mode == 1 ? CONV_KIND_CLASS1 : op.cls_mode == 2 ? CONV_KIND_CLASS2 : halo ? CONV_KIND_HALO : CONV_KIND_TAP;
-  if (halo) {
+  const bool halo = conv_halo_eligible(op, num_sms);
+  const bool pair = halo && conv_halo_pair(op, num_sms);
+  r->kind = op.cls_mode == 1 ? CONV_KIND_CLASS1
+          : op.cls_mode == 2 ? CONV_KIND_CLASS2
+          : pair             ? CONV_KIND_HALO_PAIR
+          : halo             ? CONV_KIND_HALO
+                             : CONV_KIND_TAP;
+  if (halo) {   // two-plane halo mode: the tile of one warpgroup (a unit of work is two tiles in consecutive planes)
     r->tw = HaloTile::TW; r->th = HaloTile::TH; r->td = HaloTile::TD;
   } else {
     pick_tile(gW, gH, gD, r->tw, r->th, r->td);
@@ -674,8 +889,9 @@ int conv_route(const ConvOp& op, int num_sms, ConvRoute* r) {
   return with_conv_kernel(r->kind, r->BN, r->KC, [&](auto k) {
     using Cfg = ConvCfgOf<decltype(k)::BN, decltype(k)::KC, decltype(k)::MODE>;
     r->stages = Cfg::STAGES; r->blocks_per_sm = Cfg::BLOCKS_PER_SM; r->smem_bytes = Cfg::SMEM_BYTES;
-    if constexpr (decltype(k)::MODE == CONV_HALO_WS) {
-      // persistent CTAs: one wave (max_ctas, a diagnostics cap, makes small shapes walk several tiles per CTA)
+    if constexpr (decltype(k)::MODE == CONV_HALO_WS || decltype(k)::MODE == CONV_HALO_PAIR) {
+      // persistent CTAs: one wave (max_ctas, a diagnostics cap, makes small shapes walk several tiles per CTA).  In two-plane
+      // mode conv_halo_pair has made sure that the wave has a unit for every CTA.
       int cap = Cfg::BLOCKS_PER_SM * num_sms / r->grid[1];
       if (cap < 1) cap = 1;
       if (op.max_ctas > 0 && op.max_ctas < cap) cap = op.max_ctas;
@@ -689,7 +905,8 @@ int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
   ConvRoute r;
   B200_TRY(conv_route(op, device_sms(), &r));
   const Act& out = op.out;
-  const bool split = r.npass == 3, halo = r.kind == CONV_KIND_HALO, cls = op.cls_mode != 0;
+  const bool pair = r.kind == CONV_KIND_HALO_PAIR;
+  const bool split = r.npass == 3, halo = r.kind == CONV_KIND_HALO || pair, cls = op.cls_mode != 0;
   ConvArgs a;
   memset(&a, 0, sizeof(a));
   ConvMaps maps;
@@ -705,9 +922,10 @@ int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
     a.ntaps[s] = c.ksz * c.ksz * c.ksz; a.ksz[s] = c.ksz; a.stride[s] = c.stride; a.pad[s] = c.nopad ? 0 : c.ksz / 2;
     a.kchunks[s] = r.kchunks[s];
     const int estride = cls ? 1 : c.stride;
-    const bool box = halo && s == 0;   // halo mode: source 0 is one box around the output tile
+    const bool box = halo && s == 0;   // halo mode: source 0 is one box around the output tile (two-plane mode: the pair of tiles)
     B200_TRY(make_act_map(&maps.a[s][0], c.x.hi, c.x.N, c.x.D, c.x.H, c.x.W, c.x.C, c.x.ld, KC, box ? HaloTile::BW : a.tw,
-                          box ? HaloTile::BH : a.th, box ? HaloTile::BD : a.td, estride, swz, c.x.vD, c.x.vH, c.x.vW));
+                          box ? HaloTile::BH : a.th, box ? (pair ? HaloBox<2>::BD : HaloTile::BD) : a.td, estride, swz, c.x.vD,
+                          c.x.vH, c.x.vW));
     B200_TRY(make_w_map(&maps.b[s][0], c.w_hi, a.ntaps[s], op.Cop, c.Cip, KC, BN, swz));
     if (split) {
       B200_TRY(make_act_map(&maps.a[s][1], c.x.lo, c.x.N, c.x.D, c.x.H, c.x.W, c.x.C, c.x.ld, KC, a.tw, a.th, a.td,

@@ -159,7 +159,7 @@ struct ConvOp {
 };
 
 // The kernel a convolution runs on, decided from the op alone (no device or driver call): launch_igemm_conv launches exactly this.
-enum ConvKind { CONV_KIND_TAP = 0, CONV_KIND_HALO = 1, CONV_KIND_CLASS1 = 2, CONV_KIND_CLASS2 = 3 };
+enum ConvKind { CONV_KIND_TAP = 0, CONV_KIND_HALO = 1, CONV_KIND_CLASS1 = 2, CONV_KIND_CLASS2 = 3, CONV_KIND_HALO_PAIR = 4 };
 struct ConvRoute {
   int kind;                 // ConvKind
   int BN, KC;

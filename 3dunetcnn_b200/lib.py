@@ -53,7 +53,7 @@ class WgradRoute(C.Structure):
                 ("tw", C.c_int32), ("th", C.c_int32), ("td", C.c_int32), ("part_bytes", C.c_int64)]
 
 
-CONV_KINDS = ("tap", "halo", "class1", "class2")     # b200unet_conv_route.kind
+CONV_KINDS = ("tap", "halo", "class1", "class2", "pair")     # b200unet_conv_route.kind
 WGRAD_KINDS = ("simt", "tap", "halo")               # b200unet_wgrad_route.kind
 
 

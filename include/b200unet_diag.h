@@ -34,6 +34,8 @@ typedef struct b200unet_diag_ext {
 #define B200UNET_CONV_HALO 1     /* one halo box per K chunk for an 8 x 16 x 1 output tile */
 #define B200UNET_CONV_CLASS1 2   /* parity classes: data gradient of a 3x3x3 stride-2 convolution */
 #define B200UNET_CONV_CLASS2 3   /* parity classes: ConvTranspose3d with kernel = stride = 2 */
+#define B200UNET_CONV_HALO_PAIR 4   /* one halo box for two 8 x 16 x 1 output tiles in consecutive planes, one per consumer
+                                       warpgroup; grid[0] counts CTAs, each walking units of two tiles */
 
 typedef struct b200unet_conv_route {
   int32_t kind;

@@ -18,9 +18,10 @@ SHAPES = [(8, 32, 128), (32, 32, 128), (64, 32, 128), (32, 64, 64), (64, 64, 64)
 # how many times each shape occurs in one C2 forward (for the weighted total)
 COUNT = {(8, 32, 128): 1, (32, 32, 128): 2, (64, 32, 128): 1, (32, 64, 64): 1, (64, 64, 64): 3, (128, 128, 64): 2,
          (64, 128, 32): 1, (128, 128, 32): 3, (256, 256, 32): 2, (128, 256, 16): 1, (256, 256, 16): 9}
-# the mode-1 data gradients (GroupNorm/ReLU backward epilogue) of the C2 step at 128^3 that run in halo mode: (Cin, Cout, r) of
+# the mode-1 data gradients (GroupNorm/ReLU backward epilogue) of the C2 step at 128^3 that run in halo mode, and the 64 -> 32
+# one of encoder level 1 at 64^3: (Cin, Cout, r) of
 # the data-gradient convolution, and how many times each occurs in one C2 backward
-DGRAD = {(32, 32, 128): 2, (32, 64, 128): 1, (32, 8, 128): 1}
+DGRAD = {(32, 32, 128): 2, (32, 64, 128): 1, (32, 8, 128): 1, (64, 32, 64): 1}
 
 
 def timeit(fn, reps):
