@@ -138,12 +138,17 @@ int b200unet_gn_bwd_finalize(const double* bstats, const float* coef, const floa
 int b200unet_gn_bwd(const b200unet_tensor* dz, const b200unet_tensor* x, const float* coef, const double* bstats,
                     const float* gamma, int c, int groups, float* dgamma, float* dbeta, const b200unet_tensor* add1,
                     const b200unet_tensor* add2, const b200unet_tensor* dx, void* stream) {
+  return b200unet_diag_gn_bwd(dz, x, coef, bstats, gamma, c, groups, dgamma, dbeta, add1, add2, dx, nullptr, stream);
+}
+int b200unet_diag_gn_bwd(const b200unet_tensor* dz, const b200unet_tensor* x, const float* coef, const double* bstats, const float* gamma,
+                         int c, int groups, float* dgamma, float* dbeta, const b200unet_tensor* add1, const b200unet_tensor* add2,
+                         const b200unet_tensor* dx, const float* scale, void* stream) {
   NOT_NULL(dz); NOT_NULL(x); NOT_NULL(coef); NOT_NULL(bstats); NOT_NULL(dx);
   Act a1, a2;
   if (add1) a1 = to_act(add1);
   if (add2) a2 = to_act(add2);
   return launch_gn_bwd(to_act(dz), to_act(x), coef, bstats, gamma, c, groups, (long long)x->d * x->h * x->w, dgamma, dbeta,
-                       add1 ? &a1 : nullptr, add2 ? &a2 : nullptr, to_act(dx), nullptr, to_stream(stream));
+                       add1 ? &a1 : nullptr, add2 ? &a2 : nullptr, to_act(dx), scale, to_stream(stream));
 }
 
 int b200unet_act_bwd(const b200unet_tensor* g1, const b200unet_tensor* g2, const b200unet_tensor* c, const float* coef, float slope,
@@ -327,11 +332,35 @@ int b200unet_diag_wgrad_ex(const b200unet_tensor* a, const b200unet_tensor* dy, 
   return launch_wgrad_reduce(part, n, (long long)ksz * ksz * ksz * cip * cop, dw, to_stream(stream));
 }
 
-int b200unet_diag_bias_grad(const b200unet_tensor* dy, const b200unet_diag_ext* ext, float* dbias, void* stream) {
-  NOT_NULL(dy); NOT_NULL(dbias);
+int b200unet_diag_bias_grad(const b200unet_tensor* dy, const b200unet_diag_ext* ext, float* scratch, float* dbias, void* stream) {
+  NOT_NULL(dy); NOT_NULL(scratch); NOT_NULL(dbias);
   Act y = to_act(dy);
   if (ext) set_vis(y, ext->dy_vis);
-  return launch_bias_grad(y, dbias, to_stream(stream));
+  return launch_bias_grad(y, dbias, scratch, to_stream(stream));
+}
+size_t b200unet_diag_bias_grad_scratch_bytes(int c) { return bias_grad_scratch_bytes(c); }
+
+int b200unet_diag_head_fwd(const b200unet_tensor* x, const float* w, const float* bias, int n_out, int act, float* logits, void* stream) {
+  NOT_NULL(x); NOT_NULL(w); NOT_NULL(logits);
+  return launch_head_fwd(to_act(x), w, n_out, act, logits, to_stream(stream), bias);
+}
+int b200unet_diag_head_dbias(const float* dlogits, int n, int n_out, int64_t spatial, float* scratch, float* dbias, void* stream) {
+  NOT_NULL(dlogits); NOT_NULL(scratch); NOT_NULL(dbias);
+  return launch_head_dbias(dlogits, n, n_out, spatial, dbias, to_stream(stream), scratch);
+}
+int b200unet_diag_input_pack(const float* x, int c, const b200unet_tensor* out, double* stats, int stats_ld, void* stream) {
+  NOT_NULL(x); NOT_NULL(out);
+  return launch_input_pack(x, c, to_act(out), stats, stats_ld, to_stream(stream));
+}
+int b200unet_diag_input_grad(const b200unet_tensor* dz, const b200unet_tensor* x, const float* coef, const float* coef2, int coef_ld,
+                             const b200unet_tensor* r, int c, float* dx, void* stream) {
+  NOT_NULL(r); NOT_NULL(dx);
+  Act a, b;
+  if (dz) {
+    NOT_NULL(x);
+    a = to_act(dz); b = to_act(x);
+  }
+  return launch_input_grad(dz ? &a : nullptr, dz ? &b : nullptr, coef, coef2, coef_ld, to_act(r), c, dx, to_stream(stream));
 }
 
 }  // extern "C"

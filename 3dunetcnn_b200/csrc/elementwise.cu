@@ -563,7 +563,7 @@ int launch_upsample2x_fwd(const Act& x, const Act& y, double* stats, int stats_l
                "upsample: output must be exactly 2x (got %dx%dx%d -> %dx%dx%d)", x.D, x.H, x.W, y.D, y.H, y.W);
   const int c8n = x.C / 8;
   const int threads = ew_threads_for(c8n);
-  B200_REQUIRE(threads <= 1024, E_UNSUPPORTED, "upsample: C=%d unsupported", x.C);
+  B200_REQUIRE(threads <= 256, E_UNSUPPORTED, "upsample: C=%d unsupported (at most 2048 channels)", x.C);
   const int vper = threads / c8n;
   const long long nblk = (long long)(x.D + 1) * (x.H + 1) * (x.W + 1);
   B200_REQUIRE(nblk < (1LL << 31), E_UNSUPPORTED, "upsample: volume too large");
@@ -889,7 +889,10 @@ int launch_head_bwd(const Act& x, const float* w, int n_out, const float* dlogit
 // ------------------------------------------------------------------------------------------------ bias gradient
 // dbias[c] = sum over the visible voxels (d < vD, h < vH, w < vW) of dy[v][c]   (ConvTranspose3d bias; the padded
 // boundary of its output is a constant and carries no gradient)
-__global__ void k_bias_grad(Act dy, float* __restrict__ dbias) {
+// No floating-point atomics, so that a deterministic plan repeats this gradient bit for bit: each block sums its threads'
+// partials in a fixed order into its slot of `part` [blocks][C] (as k_head_bwd does), then k_sum_slots adds the slots in order.
+constexpr int kBiasGradSlots = 592;
+__global__ void k_bias_grad(Act dy, float* __restrict__ part) {
   const int c8n = dy.C / 8;
   const int c8 = threadIdx.x % c8n;
   const int vslot = threadIdx.x / c8n, vper = blockDim.x / c8n;
@@ -906,23 +909,29 @@ __global__ void k_bias_grad(Act dy, float* __restrict__ dbias) {
 #pragma unroll
     for (int j = 0; j < 8; ++j) a[j] += g[j];
   }
-  extern __shared__ float sm[];
-  for (int i = threadIdx.x; i < dy.C; i += blockDim.x) sm[i] = 0.f;
-  __syncthreads();
+  extern __shared__ float s_tmp[];   // [blockDim.x][8]
 #pragma unroll
-  for (int j = 0; j < 8; ++j) atomicAdd(&sm[c8 * 8 + j], a[j]);
+  for (int j = 0; j < 8; ++j) s_tmp[threadIdx.x * 8 + j] = a[j];
   __syncthreads();
-  for (int i = threadIdx.x; i < dy.C; i += blockDim.x) atomicAdd(&dbias[i], sm[i]);
+  for (int i = threadIdx.x; i < dy.C; i += blockDim.x) {
+    float acc = 0.f;
+    for (int t = i >> 3; t < (int)blockDim.x; t += c8n) acc += s_tmp[t * 8 + (i & 7)];
+    part[(long long)blockIdx.x * dy.C + i] = acc;
+  }
 }
 
-int launch_bias_grad(const Act& dy, float* dbias, cudaStream_t st) {
+size_t bias_grad_scratch_bytes(int C) { return (size_t)kBiasGradSlots * C * sizeof(float); }
+
+int launch_bias_grad(const Act& dy, float* dbias, float* scratch, cudaStream_t st) {
   B200_REQUIRE(dy.C % 8 == 0, E_INVALID, "bias_grad: C=%d", dy.C);
-  B200_CHECK_CUDA(cudaMemsetAsync(dbias, 0, sizeof(float) * dy.C, st));
+  B200_REQUIRE(scratch != nullptr, E_INVALID, "bias_grad: needs bias_grad_scratch_bytes() of scratch");
   const int threads = ew_threads_for(dy.C / 8);
   B200_REQUIRE(threads <= 1024, E_UNSUPPORTED, "bias_grad: C=%d unsupported", dy.C);
   long long want = (dy.voxels() + threads / (dy.C / 8) - 1) / (threads / (dy.C / 8));
-  int blocks = (int)(want < 592 ? (want > 0 ? want : 1) : 592);
-  k_bias_grad<<<blocks, threads, dy.C * sizeof(float), st>>>(dy, dbias);
+  int blocks = (int)(want < kBiasGradSlots ? (want > 0 ? want : 1) : kBiasGradSlots);
+  k_bias_grad<<<blocks, threads, (size_t)threads * 8 * sizeof(float), st>>>(dy, scratch);
+  B200_CHECK_CUDA(cudaGetLastError());
+  k_sum_slots<<<dy.C, 128, 0, st>>>(scratch, blocks, dy.C, dbias);
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;
 }

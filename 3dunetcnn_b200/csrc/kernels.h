@@ -57,7 +57,9 @@ struct PackJob {
 };
 int launch_pack_all(const PtrTable& params, const PackJob* jobs_dev, int njobs, uint8_t* ws, bool split, cudaStream_t st);
 int launch_unpack_all(const PtrTable& grads, const PackJob* jobs_dev, int njobs, const uint8_t* ws, cudaStream_t st);
-int launch_bias_grad(const Act& dy, float* dbias, cudaStream_t st);   // dbias[c] = sum over the VISIBLE voxels of dy
+// dbias[c] = sum over the VISIBLE voxels of dy (overwritten), in a fixed order; scratch: bias_grad_scratch_bytes(dy.C)
+int launch_bias_grad(const Act& dy, float* dbias, float* scratch, cudaStream_t st);
+size_t bias_grad_scratch_bytes(int C);
 int launch_zero_insert(const Act& x, const Act& z, int od, int oh, int ow, cudaStream_t st);
 int launch_ncdhw_to_act(const float* x, int C, const Act& out, cudaStream_t st);
 int launch_act_to_ncdhw(const Act& in, int C, float* y, cudaStream_t st);

@@ -142,6 +142,7 @@ struct b200unet_plan {
   bool have_drop = false;
   bool deterministic = false;   // weight gradients: per-split partial sums + fixed-order reduction instead of fp32 atomics
   size_t head_part_off = 0;   // per-block partial sums of the head weight gradient (fixed-order reduction)
+  size_t head_part_bytes = 0;   // at least that, and the transposed-convolution bias gradients' partial sums (run after the head)
   size_t wg_part_off = 0, wg_part_bytes = 0;   // scratch shared by all weight-gradient launches (stream-ordered)
   float slope = 0.f;        // negative slope of the activation (0 = ReLU: UNet3D; 0.01 = LeakyReLU: DynUNet)
   bool infer = false;       // forward-only plan: no backward schedule / buffers, forward temporaries are recycled
@@ -843,8 +844,10 @@ static int build_unet3d(Plan& P) {
       // the padded boundary of the ConvT output is a constant: mask it out of dU (visible extent 2n-1 through TMA)
       TRef dUm = masked(dU);
       const int cup = s.cup;
+      P.head_part_bytes = std::max(P.head_part_bytes, bias_grad_scratch_bytes(out_w));
       push_op(P.bwd, "bias_grad " + P.convs[cup].name, [&P, dUm, cup](RunCtx& cx) -> int {
-        LAUNCHED(cx, CAT_OTHER, launch_bias_grad(act_of(P, cx, dUm), cx.grads[P.convs[cup].pb], cx.st));
+        LAUNCHED(cx, CAT_OTHER, launch_bias_grad(act_of(P, cx, dUm), cx.grads[P.convs[cup].pb],
+                                                 reinterpret_cast<float*>(cx.ws + P.head_part_off), cx.st));
         return OK;
       });
       emit_wgrad(P, cup, s.Z, dUm);                                   // dW[tap][ci][co] from the zero-inserted input
@@ -886,7 +889,7 @@ static int finish_build(Plan& P) {
   const int head_c = d.arch == 1 ? d.filters[0] : d.base_width;
   B200_REQUIRE(d.n_outputs <= 8 || head_c <= 64, E_UNSUPPORTED,
                "plan: more than 8 outputs need at most 64 channels into the head, got %d", head_c);
-  if (!P.infer) P.head_part_off = P.alloc(head_bwd_scratch_bytes(d.n_outputs, head_c));
+  if (!P.infer) P.head_part_off = P.alloc(std::max(P.head_part_bytes, head_bwd_scratch_bytes(d.n_outputs, head_c)));
   for (size_t i = 0; i < P.convs.size(); ++i)
     B200_REQUIRE(P.convs[i].pw >= 0, E_INVALID, "plan: internal: conv %d has no parameter", (int)i);
   for (const ConvLayer& c : P.convs) {

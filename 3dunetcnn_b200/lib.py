@@ -178,7 +178,16 @@ _DIAG_SIGS = {
     "b200unet_diag_wgrad_partial_bytes": (C.c_size_t, _WG_ARGS + [C.c_int]),
     "b200unet_diag_conv3d_ex": (C.c_int, [C.POINTER(ConvDesc), C.POINTER(DiagExt), C.c_void_p]),
     "b200unet_diag_wgrad_ex": (C.c_int, _WG_ARGS + [C.c_void_p, C.c_size_t, C.POINTER(C.c_int), C.c_void_p, C.c_void_p]),
-    "b200unet_diag_bias_grad": (C.c_int, [C.POINTER(Tensor5), C.POINTER(DiagExt), C.c_void_p, C.c_void_p]),
+    "b200unet_diag_bias_grad": (C.c_int, [C.POINTER(Tensor5), C.POINTER(DiagExt), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200unet_diag_bias_grad_scratch_bytes": (C.c_size_t, [C.c_int]),
+    "b200unet_diag_gn_bwd": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                       C.c_void_p, C.c_void_p, C.POINTER(Tensor5), C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p,
+                                       C.c_void_p]),
+    "b200unet_diag_head_fwd": (C.c_int, [C.POINTER(Tensor5), C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "b200unet_diag_head_dbias": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200unet_diag_input_pack": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(Tensor5), C.c_void_p, C.c_int, C.c_void_p]),
+    "b200unet_diag_input_grad": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_void_p, C.c_int, C.POINTER(Tensor5),
+                                           C.c_int, C.c_void_p, C.c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGS)
@@ -406,9 +415,39 @@ def wgrad_ex(a: Act, dy: Act, ksz: int, stride: int, cip: int, cop: int, dw: tor
 
 
 def bias_grad(dy: Act, dbias: torch.Tensor, ext: Optional[DiagExt] = None) -> None:
-    """dbias = sum of dy over its visible voxels (ext.dy_vis)"""
-    check(load_library().b200unet_diag_bias_grad(C.byref(dy.ct()), C.byref(ext) if ext is not None else None, dbias.data_ptr(),
-                                                 stream_ptr()), "diag_bias_grad")
+    """dbias = sum of dy over its visible voxels (ext.dy_vis), in a fixed order"""
+    lib = load_library()
+    scratch = torch.empty(int(lib.b200unet_diag_bias_grad_scratch_bytes(dy.c)), dtype=torch.uint8, device=dy.hi.device)
+    check(lib.b200unet_diag_bias_grad(C.byref(dy.ct()), C.byref(ext) if ext is not None else None, scratch.data_ptr(), dbias.data_ptr(),
+                                      stream_ptr()), "diag_bias_grad")
+
+
+def head_fwd_ex(x: Act, w: torch.Tensor, bias: Optional[torch.Tensor], n_out: int, act: int, logits: torch.Tensor) -> None:
+    """head_fwd with a per-output bias (None = none), as the plans run it"""
+    check(load_library().b200unet_diag_head_fwd(C.byref(x.ct()), w.data_ptr(), _p(bias), n_out, act, logits.data_ptr(), stream_ptr()),
+          "diag_head_fwd")
+
+
+def head_dbias(dlogits: torch.Tensor, dbias: torch.Tensor) -> None:
+    """dbias[o] = sum of dlogits [n][o][spatial...] over n and the voxels"""
+    n, n_out = dlogits.shape[:2]
+    scratch = torch.empty(128 * n_out, dtype=torch.float64, device=dlogits.device)
+    check(load_library().b200unet_diag_head_dbias(dlogits.data_ptr(), n, n_out, dlogits[0, 0].numel(), scratch.data_ptr(),
+                                                  dbias.data_ptr(), stream_ptr()), "diag_head_dbias")
+
+
+def input_pack(x: torch.Tensor, out: Act, stats: Optional[torch.Tensor] = None, stats_ld: int = 0) -> None:
+    """NCDHW fp32 x -> NDHWC out (8 or 16 channels, zero padded); stats [n][stats_ld][2] += fp64 (sum, sumsq) per channel"""
+    check(load_library().b200unet_diag_input_pack(x.data_ptr(), x.shape[1], C.byref(out.ct()), _p(stats), stats_ld, stream_ptr()),
+          "diag_input_pack")
+
+
+def input_grad(dz: Optional[Act], x: Optional[Act], coef, coef2, coef_ld: int, r: Act, c: int, dx: torch.Tensor) -> None:
+    """dx NCDHW fp32 = (A dz + E x + F) + r over c channels; dz None: dx = r"""
+    a = dz.ct() if dz is not None else None
+    b = x.ct() if x is not None else None
+    check(load_library().b200unet_diag_input_grad(C.byref(a) if a is not None else None, C.byref(b) if b is not None else None, _p(coef),
+                                                  _p(coef2), coef_ld, C.byref(r.ct()), c, dx.data_ptr(), stream_ptr()), "diag_input_grad")
 
 
 def conv3d_wgrad(a: Act, dy: Act, ksz: int, stride: int, cip: int, cop: int, dw: torch.Tensor) -> None:
@@ -433,13 +472,25 @@ def gn_bwd_finalize(bstats, coef, gamma, n, c, c_ld, groups, spatial, coef2, dga
 
 
 def gn_bwd(dz: Act, x: Act, coef, bstats, gamma, c, groups, dx: Act, dgamma=None, dbeta=None, add1: Optional[Act] = None,
-           add2: Optional[Act] = None) -> None:
-    """dx (+ add1 + add2) and dgamma / dbeta from the backward statistics bstats [n][x.c][2] = (sum dz, sum dz * xhat)"""
+           add2: Optional[Act] = None, scale: Optional[torch.Tensor] = None) -> None:
+    """dx (+ add1 + add2) [* scale [n][x.c]] and dgamma / dbeta from the backward statistics bstats [n][x.c][2] = (sum dz, sum dz * xhat);
+    the scale goes through the diagnostics entry point"""
     a1 = add1.ct() if add1 is not None else None
     a2 = add2.ct() if add2 is not None else None
-    check(load_library().b200unet_gn_bwd(C.byref(dz.ct()), C.byref(x.ct()), coef.data_ptr(), bstats.data_ptr(), _p(gamma), c,
-                                         groups, _p(dgamma), _p(dbeta), C.byref(a1) if a1 is not None else None,
-                                         C.byref(a2) if a2 is not None else None, C.byref(dx.ct()), stream_ptr()), "gn_bwd")
+    lib = load_library()
+    args = (C.byref(dz.ct()), C.byref(x.ct()), coef.data_ptr(), bstats.data_ptr(), _p(gamma), c, groups, _p(dgamma), _p(dbeta),
+            C.byref(a1) if a1 is not None else None, C.byref(a2) if a2 is not None else None, C.byref(dx.ct()))
+    if scale is None:
+        check(lib.b200unet_gn_bwd(*args, stream_ptr()), "gn_bwd")
+    else:
+        check(lib.b200unet_diag_gn_bwd(*args, scale.data_ptr(), stream_ptr()), "diag_gn_bwd")
+
+
+def act_bwd(g1: Act, g2: Optional[Act], c: Act, coef, slope: float, dz: Act, bstats, bstats_ld: int) -> None:
+    """dz = (g1 [+ g2]) * act'(A c + B); bstats [n][bstats_ld][2] += (sum dz, sum dz * xhat)"""
+    b = g2.ct() if g2 is not None else None
+    check(load_library().b200unet_act_bwd(C.byref(g1.ct()), C.byref(b) if b is not None else None, C.byref(c.ct()), coef.data_ptr(),
+                                          slope, C.byref(dz.ct()), bstats.data_ptr(), bstats_ld, stream_ptr()), "act_bwd")
 
 
 def upsample2x_fwd(x: Act, y: Act, stats=None, stats_ld=0) -> None:

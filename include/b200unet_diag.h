@@ -78,8 +78,25 @@ int b200unet_diag_conv3d_ex(const b200unet_conv_desc* desc, const b200unet_diag_
  * dw = their sum in a fixed order. */
 int b200unet_diag_wgrad_ex(const b200unet_tensor* a, const b200unet_tensor* dy, int ksz, int stride, int cip, int cop,
                            const b200unet_diag_ext* ext, float* part, size_t part_bytes, int* splits, float* dw, void* stream);
-/* dbias[c] = sum of dy over the visible voxels (overwritten) */
-int b200unet_diag_bias_grad(const b200unet_tensor* dy, const b200unet_diag_ext* ext, float* dbias, void* stream);
+/* dbias[c] = sum of dy over the visible voxels (overwritten), in a fixed order: per-block partial sums into scratch
+ * (b200unet_diag_bias_grad_scratch_bytes(dy->c) long), then their sum */
+int b200unet_diag_bias_grad(const b200unet_tensor* dy, const b200unet_diag_ext* ext, float* scratch, float* dbias, void* stream);
+size_t b200unet_diag_bias_grad_scratch_bytes(int c);
+/* b200unet_gn_bwd with the per-(n, c) dropout scale [n][x->c] the plans apply to dx (NULL = none) */
+int b200unet_diag_gn_bwd(const b200unet_tensor* dz, const b200unet_tensor* x, const float* coef, const double* bstats, const float* gamma,
+                         int c, int groups, float* dgamma, float* dbeta, const b200unet_tensor* add1, const b200unet_tensor* add2,
+                         const b200unet_tensor* dx, const float* scale, void* stream);
+/* the 1x1x1 head forward of b200unet_head_fwd with a per-output bias (NULL = none), as the plans run it */
+int b200unet_diag_head_fwd(const b200unet_tensor* x, const float* w, const float* bias, int n_out, int act, float* logits, void* stream);
+/* dbias[o] = sum of dlogits [n][n_out][spatial] over n and the voxels (overwritten), 1..32 outputs; scratch: 128 * n_out doubles */
+int b200unet_diag_head_dbias(const float* dlogits, int n, int n_out, int64_t spatial, float* scratch, float* dbias, void* stream);
+/* the network input NCDHW fp32 [n][c][out.d * out.h * out.w] -> NDHWC bf16 out (out->c = 8 or 16, the channels from c on stored
+ * as 0); stats != NULL: also += the fp64 (sum, sumsq) of each of the c channels, [n][stats_ld][2] */
+int b200unet_diag_input_pack(const float* x, int c, const b200unet_tensor* out, double* stats, int stats_ld, void* stream);
+/* the gradient of the network input, NCDHW fp32 [n][c][r.d * r.h * r.w]: dx = (A dz + E x + F) + r over its c <= 16 channels,
+ * A from coef [n][coef_ld][4], (E, F) from coef2 [n][coef_ld][2]; dz == NULL: dx = r (x, coef and coef2 are then unused) */
+int b200unet_diag_input_grad(const b200unet_tensor* dz, const b200unet_tensor* x, const float* coef, const float* coef2, int coef_ld,
+                             const b200unet_tensor* r, int c, float* dx, void* stream);
 
 #ifdef __cplusplus
 }

@@ -13,7 +13,7 @@ import torch
 
 HOST_ONLY = {"b200unet_version", "b200unet_last_error", "b200unet_plan_create", "b200unet_plan_destroy", "b200unet_plan_num_params",
              "b200unet_plan_param_info", "b200unet_plan_workspace_bytes", "b200unet_plan_last_launches", "b200unet_plan_algorithmic_macs",
-             "b200unet_head_bwd_scratch_bytes"}
+             "b200unet_head_bwd_scratch_bytes", "b200unet_diag_bias_grad_scratch_bytes"}
 
 
 class _FakeCuda(torch.Tensor):
@@ -180,3 +180,22 @@ def test_per_kernel_wrappers_marshal_fused_groupnorm(pkg, stubbed):
     L.head_bwd(b, torch.zeros(3, 16), 3, torch.zeros(1, 3, 4, 8, 8), b, torch.zeros(3, 16))
     L.pack_weights(torch.zeros(8, 16, 2, 2, 2), 4)
     assert {"b200unet_conv3d", "b200unet_gn_apply", "b200unet_gn_bwd", "b200unet_gn_bwd_finalize", "b200unet_head_bwd"} <= set(stubbed)
+
+
+def test_bandwidth_kernel_diagnostics_marshal(pkg, stubbed):
+    """the wrappers tests/test_gpu_bandwidth_kernels.py drives through include/b200unet_diag.h and the product header"""
+    L = pkg.lib
+    b = L.Act(torch.zeros(1, 4, 8, 8, 16, dtype=torch.bfloat16))
+    st = torch.zeros(1, 16, 2, dtype=torch.float64)
+    coef = torch.zeros(1, 16, 4)
+    L.gn_bwd(b, b, coef, st, None, 16, 8, b, add1=b, add2=b, scale=torch.ones(1, 16))
+    L.act_bwd(b, b, b, coef, 0.01, b, st, 16)
+    L.act_bwd(b, None, b, coef, 0.0, b, st, 16)
+    L.bias_grad(b, torch.zeros(16), ext=L.diag_ext(dy_vis=(3, 7, 7)))
+    L.head_fwd_ex(b, torch.zeros(3, 16), torch.zeros(3), 3, 2, torch.zeros(1, 3, 4, 8, 8))
+    L.head_dbias(torch.zeros(1, 3, 4, 8, 8), torch.zeros(3))
+    L.input_pack(torch.zeros(1, 4, 4, 8, 8), b, st, 16)
+    L.input_grad(b, b, coef, torch.zeros(1, 16, 2), 16, b, 4, torch.zeros(1, 4, 4, 8, 8))
+    L.input_grad(None, None, None, None, 0, b, 4, torch.zeros(1, 4, 4, 8, 8))
+    assert {"b200unet_diag_gn_bwd", "b200unet_act_bwd", "b200unet_diag_bias_grad", "b200unet_diag_head_fwd", "b200unet_diag_head_dbias",
+            "b200unet_diag_input_pack", "b200unet_diag_input_grad"} <= set(stubbed)

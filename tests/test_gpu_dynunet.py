@@ -107,36 +107,3 @@ def test_transposed_conv_k2s2_forward_dgrad_wgrad(pkg, ci, co, dims, split):
     L.conv3d_wgrad(dy, x, 2, 2, cop, cip, dw)
     got = dw[:, :co, :ci].double().cpu().reshape(2, 2, 2, co, ci).permute(4, 3, 0, 1, 2)
     assert _rel(got, wq.grad) < (2e-3 if not split else 5e-5)
-
-
-@pytest.mark.parametrize("split", [False, True])
-def test_activation_backward_kernel_on_fused_coefficients(pkg, split):
-    """dz = (g1 + g2) * LeakyReLU'(A c + B) with (sum dz, sum dz*xhat): through head-less plumbing = compare with autograd of
-    LeakyReLU(InstanceNorm(c)) for the statistics and the mask."""
-    import ctypes as C
-    L = pkg.lib
-    lib = L.load_library()
-    torch.manual_seed(3)
-    n, ch, dims = 2, 24, (6, 10, 8)
-    c = L.Act.from_ncdhw(torch.randn(n, ch, *dims, device=DEV) * 2 + 0.5, split=split)
-    g1 = L.Act.from_ncdhw(torch.randn(n, ch, *dims, device=DEV), split=split)
-    g2 = L.Act.from_ncdhw(torch.randn(n, ch, *dims, device=DEV), split=split)
-    gamma, beta = torch.randn(ch, device=DEV) * 0.3 + 1, torch.randn(ch, device=DEV) * 0.2
-    cv = c.value().double()
-    stats = torch.stack([cv.sum(dim=(1, 2, 3)), (cv * cv).sum(dim=(1, 2, 3))], dim=-1).contiguous()   # fp64 (sum, sumsq)
-    coef = torch.empty(n, ch, 4, device=DEV)
-    L.gn_apply(c, L.Act.empty(n, *dims, ch, split=split), stats, gamma, beta, ch, ch, coef, slope=0.01)   # G = C: instance norm
-    dz = L.Act.empty(n, *dims, ch, split=split)
-    bst = torch.zeros(n, ch, 2, dtype=torch.float64, device=DEV)
-    g2t = g2.ct()
-    L.check(lib.b200unet_act_bwd(C.byref(g1.ct()), C.byref(g2t), C.byref(c.ct()), coef.data_ptr(), C.c_float(0.01), C.byref(dz.ct()),
-                                 bst.data_ptr(), ch, L.stream_ptr()), "act_bwd")
-    cq = c.to_ncdhw(ch).double().cpu().requires_grad_(True)
-    z = F.instance_norm(cq, weight=gamma.double().cpu(), bias=beta.double().cpu(), eps=1e-5)
-    z.retain_grad()
-    F.leaky_relu(z, 0.01).backward((g1.to_ncdhw(ch) + g2.to_ncdhw(ch)).double().cpu())
-    assert _rel(dz.to_ncdhw(ch), z.grad) < (4e-3 if not split else 5e-5)
-    mu, rstd = coef[..., 2].double().cpu(), coef[..., 3].double().cpu()
-    xhat = (cq.detach() - mu[:, :, None, None, None]) * rstd[:, :, None, None, None]
-    b_ref = torch.stack([z.grad.sum(dim=(2, 3, 4)), (z.grad * xhat).sum(dim=(2, 3, 4))], dim=-1)
-    assert _rel(bst, b_ref) < 1e-4

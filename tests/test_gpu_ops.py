@@ -9,7 +9,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from oracle import conv3d_direct, dice_loss, group_norm, trilinear_upsample2x
+from oracle import conv3d_direct, dice_loss
 
 pytestmark = pytest.mark.gpu
 
@@ -325,111 +325,6 @@ def test_conv3d_weight_gradient(pkg, ci, co, dims, ksz, stride, split):
     wz = torch.zeros(co, ci, ksz, ksz, ksz, dtype=torch.float64, requires_grad=True)
     F.conv3d(a.to_ncdhw(ci).double().cpu(), wz, stride=stride, padding=pad).backward(dy.to_ncdhw(co).double().cpu())
     assert rel(out, wz.grad) < (1e-5 if not split else 5e-5)
-
-
-@pytest.mark.parametrize("split", [False, True])
-@pytest.mark.parametrize("C,G,dims", [(16, 8, (8, 12, 8)), (8, 8, (4, 4, 4)), (24, 24, (6, 4, 10)), (64, 8, (4, 4, 8)),
-                                      (4, 4, (5, 6, 7))])   # 4 real channels in an 8-channel view: the network's first norm
-def test_fused_groupnorm_relu_forward_backward(pkg, C, G, dims, split):
-    """The kernels every norm layer of the plans launches: statistics -> coefficients -> GroupNorm + ReLU in one launch, and
-    backward statistics -> dgamma, dbeta, dx in one launch; plus the first block's gn_bwd_finalize."""
-    L = pkg.lib
-    torch.manual_seed(C)
-    n = 2
-    S = dims[0] * dims[1] * dims[2]
-    x = L.Act.from_ncdhw(torch.randn(n, C, *dims, device=DEV) * 2 + 0.5, split=split)
-    Cv = x.c                                                 # view channels (C padded to 8): pitch of stats, coef, bstats
-    gamma, beta = torch.randn(C, device=DEV) * 0.3 + 1, torch.randn(C, device=DEV) * 0.2
-    stats = _channel_stats(x)
-    stats[:, C:] = 7.0                                       # padded channels: ignored
-    coef = torch.full((n, Cv, 4), float("nan"), device=DEV)  # every entry is written
-    y = L.Act.empty(n, *dims, Cv, split=split)
-    L.gn_apply(x, y, stats, gamma, beta, C, G, coef)
-    xv = x.to_ncdhw(C).double().cpu()
-    ref_np = np.maximum(group_norm(xv.numpy(), G, gamma.double().cpu().numpy(), beta.double().cpu().numpy()), 0)   # numpy oracle
-    assert rel(y.to_ncdhw(C), torch.from_numpy(ref_np)) < TOL_STORE[split]
-    xg = xv.reshape(n, G, -1)
-    mu_ref = xg.mean(-1).repeat_interleave(C // G, dim=1)
-    rstd_ref = (xg.var(-1, unbiased=False) + 1e-5).rsqrt().repeat_interleave(C // G, dim=1)
-    a_ref = gamma.double().cpu() * rstd_ref
-    assert rel(coef[:, :C, 2], mu_ref) < 1e-6 and rel(coef[:, :C, 3], rstd_ref) < 1e-6
-    assert rel(coef[:, :C, 0], a_ref) < 1e-6 and rel(coef[:, :C, 1], beta.double().cpu() - mu_ref * a_ref) < 1e-6
-    if Cv > C:
-        assert float(coef[:, C:].abs().max()) == 0.0 and float(y.value()[..., C:].abs().max()) == 0.0
-    # backward: dx = dL/dx given dz = dL/d(GN output)
-    dz = L.Act.from_ncdhw(torch.randn(n, C, *dims, device=DEV), split=split)
-    dzq = dz.to_ncdhw(C).double().cpu()
-    xq = xv.clone().requires_grad_(True)
-    g64, b64 = gamma.double().cpu().requires_grad_(True), beta.double().cpu().requires_grad_(True)
-    F.group_norm(xq, G, g64, b64, 1e-5).backward(dzq)
-    mu, rstd = coef[:, :C, 2].double().cpu(), coef[:, :C, 3].double().cpu()
-    xhat = (xv - mu[:, :, None, None, None]) * rstd[:, :, None, None, None]
-    bst = torch.zeros(n, Cv, 2, dtype=torch.float64)
-    bst[:, :C] = torch.stack([dzq.sum(dim=(2, 3, 4)), (dzq * xhat).sum(dim=(2, 3, 4))], dim=-1)
-    bst = bst.to(DEV)
-    add = L.Act.from_ncdhw(torch.randn(n, C, *dims, device=DEV), split=split)
-    dx = L.Act.empty(n, *dims, Cv, split=split)
-    dg, db = torch.full((C,), float("nan"), device=DEV), torch.full((C,), float("nan"), device=DEV)
-    L.gn_bwd(dz, x, coef, bst, gamma, C, G, dx, dg, db, add1=add)
-    assert rel(dx.to_ncdhw(C), xq.grad + add.to_ncdhw(C).double().cpu()) < TOL_STORE[split]
-    assert rel(dg, g64.grad) < 1e-5 and rel(db, b64.grad) < 1e-5
-    if Cv > C:
-        assert float(dx.value()[..., C:].abs().max()) == 0.0      # A = E = F = 0, and the padded add channels are zero
-    # the first block's norm: (E, F) of dx = A dz + E x + F for the input gradient, dgamma and dbeta
-    coef2 = torch.full((n, Cv, 2), float("nan"), device=DEV)
-    dg2, db2 = torch.empty(C, device=DEV), torch.empty(C, device=DEV)
-    L.gn_bwd_finalize(bst, coef, gamma, n, C, Cv, G, S, coef2, dg2, db2)
-    k, e = coef[:, :C].double().cpu(), coef2[:, :C].double().cpu()
-    dx2 = k[..., 0, None, None, None] * dzq + e[..., 0, None, None, None] * xv + e[..., 1, None, None, None]
-    assert rel(dx2, xq.grad) < TOL_STORE[True]
-    assert rel(dg2, g64.grad) < 1e-5 and rel(db2, b64.grad) < 1e-5
-    if Cv > C:
-        assert float(coef2[:, C:].abs().max()) == 0.0
-
-
-@pytest.mark.parametrize("split", [False, True])
-@pytest.mark.parametrize("dims", [(4, 6, 8), (3, 5, 7), (1, 2, 4), (2, 2, 6)])   # even extents: register-blocked adjoint; (2, ..): first == last block
-def test_trilinear_upsample_forward_backward(pkg, dims, split):
-    L = pkg.lib
-    torch.manual_seed(5)
-    n, C = 2, 16
-    x = L.Act.from_ncdhw(torch.randn(n, C, *dims, device=DEV), split=split)
-    od = [2 * s for s in dims]
-    cat = L.Act.empty(n, *od, 2 * C, split=split, zero=True)
-    stats = torch.zeros(n, 2 * C, 2, dtype=torch.float64, device=DEV)
-    L.upsample2x_fwd(x, cat.slice(0, C), stats, 2 * C)
-    ref = trilinear_upsample2x(x.to_ncdhw(C).double().cpu().numpy())                     # numpy oracle
-    got = cat.slice(0, C).to_ncdhw(C)
-    assert rel(got, torch.from_numpy(ref)) < TOL_STORE[split]
-    assert float(cat.hi[..., C:].float().abs().max()) == 0.0
-    gd = torch.from_numpy(ref)
-    s_ref = torch.stack([gd.sum(dim=(2, 3, 4)), (gd * gd).sum(dim=(2, 3, 4))], dim=-1)
-    assert rel(stats[:, :C], s_ref) < 1e-5
-    dy = L.Act.from_ncdhw(torch.randn(n, C, *od, device=DEV), split=split)
-    dx = L.Act.empty(n, *dims, C, split=split)
-    L.upsample2x_bwd(dy, dx)
-    xq = x.to_ncdhw(C).double().cpu().requires_grad_(True)
-    F.interpolate(xq, scale_factor=2, mode="trilinear", align_corners=False).backward(dy.to_ncdhw(C).double().cpu())
-    assert rel(dx.to_ncdhw(C), xq.grad) < TOL_STORE[split]
-
-
-@pytest.mark.parametrize("split", [False, True])
-def test_head_forward_backward(pkg, split):
-    L = pkg.lib
-    torch.manual_seed(6)
-    n, C, O, dims = 2, 32, 3, (6, 6, 10)
-    x = L.Act.from_ncdhw(torch.randn(n, C, *dims, device=DEV), split=split)
-    w = torch.randn(O, C, device=DEV) * 0.3
-    logits = torch.empty(n, O, *dims, device=DEV)
-    L.head_fwd(x, w, O, 0, logits)
-    xv = x.to_ncdhw(C).double().cpu()
-    assert rel(logits, torch.einsum("ncdhw,oc->nodhw", xv, w.double().cpu())) < 1e-6
-    dl = torch.randn(n, O, *dims, device=DEV)
-    dx = L.Act.empty(n, *dims, C, split=split)
-    dw = torch.empty(O, C, device=DEV)
-    L.head_bwd(x, w, O, dl, dx, dw)
-    assert rel(dx.to_ncdhw(C), torch.einsum("nodhw,oc->ncdhw", dl.double().cpu(), w.double().cpu())) < TOL_STORE[split]
-    assert rel(dw, torch.einsum("nodhw,ncdhw->oc", dl.double().cpu(), xv)) < 1e-5
 
 
 @pytest.mark.parametrize("kw", [dict(sigmoid=True), dict(sigmoid=True, squared_pred=True), dict(sigmoid=True, jaccard=True),

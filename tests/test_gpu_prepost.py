@@ -165,12 +165,14 @@ def test_graphed_train_step_matches_eager(pkg):
     assert num / den < 1e-4
 
 
-@pytest.mark.parametrize("arch", ["unet3d", "dynunet"])
+@pytest.mark.parametrize("arch", ["unet3d", "unet3d_convT", "dynunet"])
 def test_deterministic_backward_repeats_bit_for_bit(pkg, arch):
-    """A deterministic plan's backward writes the same flat gradient bucket bit for bit every time, and writes all of it."""
+    """A deterministic plan's backward writes the same flat gradient bucket bit for bit every time, and writes all of it (unet3d_convT:
+    the transposed-convolution up-sampling, whose bias gradient sums 32^3 voxels over a full grid of blocks)."""
     torch.manual_seed(0)
-    if arch == "unet3d":
-        model = pkg.UNet3D(precision="bf16", deterministic=True, dropout=0.0, n_features=2, n_outputs=2, base_width=8).to(DEV)
+    if arch.startswith("unet3d"):
+        model = pkg.UNet3D(precision="bf16", deterministic=True, dropout=0.0, n_features=2, n_outputs=2, base_width=8,
+                           use_transposed_convolutions=arch == "unet3d_convT").to(DEV)
         shape, tshape = (2, 2, 32, 32, 32), (2, 2, 32, 32, 32)
     else:
         model = pkg.DynUNet(spatial_dims=3, in_channels=2, out_channels=2, kernel_size=[[3, 3, 3]] * 4, strides=[[1, 1, 1]] + [[2, 2, 2]] * 3,
