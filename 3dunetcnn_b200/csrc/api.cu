@@ -85,7 +85,7 @@ using namespace b200;
 
 extern "C" {
 
-int b200unet_version(void) { return 103; }
+int b200unet_version(void) { return 104; }
 const char* b200unet_last_error(void) { return get_error(); }
 
 int b200unet_ncdhw_to_ndhwc(const float* x, int c_real, const b200unet_tensor* out, void* stream) {
@@ -258,6 +258,14 @@ int b200unet_augment_resample(const float* image, const uint8_t* label, int n, i
 int b200unet_augment_intensity(float* image, int n, int c, int64_t spatial, int normalize, int nonzero, int channel_wise,
                                const float* coef, void* scratch, void* stream) {
   return launch_augment_intensity(image, n, c, spatial, normalize, nonzero, channel_wise, coef, scratch, to_stream(stream));
+}
+
+int b200unet_resample_to_grid(const float* src, int c, int sd, int sh, int sw, const double affine[12], int mode, float* dst, int dd,
+                              int dh, int dw, void* stream) {
+  NOT_NULL(src); NOT_NULL(affine); NOT_NULL(dst);
+  IndexAffine m;
+  memcpy(m.m, affine, sizeof(m.m));
+  return launch_resample_to_grid(src, c, sd, sh, sw, m, mode, dst, dd, dh, dw, to_stream(stream));
 }
 
 size_t b200unet_cc_scratch_bytes(int nvol, int d, int h, int w) { return cc_scratch_bytes(nvol, d, h, w); }

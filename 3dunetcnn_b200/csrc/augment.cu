@@ -11,6 +11,7 @@
 // Padding follows torch.nn.functional.grid_sample(align_corners=False) on index coordinates: border clamps the source
 // coordinate to [0, size-1], zeros gives out-of-range corners weight 0 (labels 0); nearest rounds half to even.
 #include "kernels.h"
+#include "resample.cuh"
 
 namespace b200 {
 
@@ -36,18 +37,6 @@ struct AugDims {
   int D, H, W;
   long long S;
 };
-
-// fp32 source coordinate on one axis -> the two corner indices and the weight of the upper one (trilinear), corners outside
-// the volume flagged by ok0 / ok1 (zeros padding)
-__device__ __forceinline__ void aug_corners(float x, int n, int border, int& i0, int& i1, float& f, bool& ok0, bool& ok1) {
-  if (border) x = fminf(fmaxf(x, 0.f), (float)(n - 1));
-  const float fl = floorf(x);
-  f = x - fl;
-  i0 = (int)fl;
-  i1 = i0 + 1;
-  ok0 = i0 >= 0 && i0 < n;
-  ok1 = i1 >= 0 && i1 < n;
-}
 
 template <int CM>
 __global__ void __launch_bounds__(kAugThreads) k_aug_resample(const float* __restrict__ img, const uint8_t* __restrict__ lab,
@@ -81,39 +70,12 @@ __global__ void __launch_bounds__(kAugThreads) k_aug_resample(const float* __res
     const float sh = fmaf(m[4], fd, fmaf(m[5], fh, fmaf(m[6], fw, m[7])));
     const float sw = fmaf(m[8], fd, fmaf(m[9], fh, fmaf(m[10], fw, m[11])));
 
-    int d0, d1, h0, h1, w0, w1;
-    float ad, ah, aw;
-    bool od0, od1, oh0, oh1, ow0, ow1;
-    aug_corners(sd, g.D, border, d0, d1, ad, od0, od1);
-    aug_corners(sh, g.H, border, h0, h1, ah, oh0, oh1);
-    aug_corners(sw, g.W, border, w0, w1, aw, ow0, ow1);
-    // border: the upper corner of the last plane carries weight 0; read the last plane instead of past it
-    if (border) { d1 = min(d1, g.D - 1); h1 = min(h1, g.H - 1); w1 = min(w1, g.W - 1); od1 = oh1 = ow1 = true; }
-    const float bd = 1.f - ad, bh = 1.f - ah, bw = 1.f - aw;
-    const float wt[8] = {bd * bh * bw, bd * bh * aw, bd * ah * bw, bd * ah * aw,
-                         ad * bh * bw, ad * bh * aw, ad * ah * bw, ad * ah * aw};
-    // a corner counts when it lies inside the volume and has a non-zero weight: corners of weight 0 are not read, so a
-    // flip copies every value bit for bit (-0.0, inf and NaN included) and an inf beside a voxel does not leak into it
-    bool ok[8] = {od0 && oh0 && ow0, od0 && oh0 && ow1, od0 && oh1 && ow0, od0 && oh1 && ow1,
-                  od1 && oh0 && ow0, od1 && oh0 && ow1, od1 && oh1 && ow0, od1 && oh1 && ow1};
-    bool any = false;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) { ok[k] = ok[k] && wt[k] != 0.f; any = any || ok[k]; }
-    int off[8];   // within one plane: S < 2^31
-    {
-      const int dd[2] = {d0, d1}, hh[2] = {h0, h1}, ww[2] = {w0, w1};
-#pragma unroll
-      for (int k = 0; k < 8; ++k) off[k] = ok[k] ? (dd[k >> 2] * g.H + hh[(k >> 1) & 1]) * g.W + ww[k & 1] : 0;
-    }
+    const Trilinear t = trilinear_corners(sd, sh, sw, g.D, g.H, g.W, border);   // offsets within one plane: S < 2^31
 #pragma unroll
     for (int c = 0; c < CM; ++c) {
       if (c < C) {
-        const float* p = src + (long long)c * g.S;
-        float y = -0.f;                 // -0 + x == x for every x, so a single corner passes through unchanged
-#pragma unroll
-        for (int k = 0; k < 8; ++k)
-          if (ok[k]) y = fmaf(wt[k], __ldg(p + off[k]), y);
-        if (!any) y = 0.f;              // every corner outside the volume (zeros padding)
+        float y = trilinear_sample(src + (long long)c * g.S, t);
+        if (!t.any) y = 0.f;            // every corner outside the volume (zeros padding)
         dst[(long long)c * g.S + v] = y;
         if (!nonzero || y != 0.f) { s[c] += y; q[c] += (double)y * y; cnt[c] += 1u; }
       }

@@ -119,6 +119,13 @@ int launch_augment_resample(const float* img, const uint8_t* lab, int N, int C, 
 int launch_augment_intensity(float* img, int N, int C, long long S, int normalize, int nonzero, int channel_wise, const float* coef,
                              void* scratch, cudaStream_t st);
 
+// ---- resample a prediction onto the grid of its image file (resample.cu)
+// row-major 3x4 map of target index (d, h, w, 1) -> source index, passed by value
+struct IndexAffine { double m[12]; };
+// src fp32 [C][sd][sh][sw] -> dst fp32 [C][dd][dh][dw], 1 <= C <= B200_MAX_LABEL_CHANNELS; mode 0 trilinear, 1 nearest; border padding
+int launch_resample_to_grid(const float* src, int C, int sd, int sh, int sw, const IndexAffine& m, int mode, float* dst, int dd,
+                            int dh, int dw, cudaStream_t st);
+
 // ---- connected components of binary masks (ccl.cu)
 size_t cc_scratch_bytes(int nvol, int d, int h, int w);   // 0: the shape is rejected
 int launch_cc_label(const uint8_t* mask, int nvol, int d, int h, int w, int connectivity, int32_t* labels, int32_t* counts,

@@ -11,9 +11,11 @@ import ctypes as C
 import math
 from typing import Callable, List, Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import lib as _lib
+from . import prepost as _prepost
 
 
 def _scan_starts(size: int, roi: int, overlap: float) -> List[int]:
@@ -132,15 +134,45 @@ def _filename_of(x, index: int):
     return f[index] if isinstance(f, (list, tuple)) else f
 
 
+def _grid_meta_of(x, key: str, index: int, item_ndim: int) -> np.ndarray:
+    """``meta[key]`` of item ``index`` as fp64: batched by the collate function (a tensor or array with a leading batch axis),
+    a per-item sequence, or one value for every item (``item_ndim`` axes)"""
+    meta = x.meta
+    if key not in meta:
+        raise KeyError("volumetric_predictions(resample=True) needs meta[%r] of the input (LoadImageD records it when it loads "
+                       "the image; keep it through the transforms)" % key)
+    v = meta[key]
+    if isinstance(v, (list, tuple)) and len(v) and np.ndim(_numpy(v[0])) == item_ndim:
+        v = v[index]
+    v = _numpy(v)
+    return v[index] if v.ndim == item_ndim + 1 else v
+
+
+def _numpy(v) -> np.ndarray:
+    if isinstance(v, torch.Tensor):
+        return v.as_subclass(torch.Tensor).detach().cpu().double().numpy()
+    return np.asarray(v, dtype=np.float64)
+
+
 def volumetric_predictions(model, dataloader, prediction_dir, activation=None, resample=False, interpolation="trilinear",
                            inferer=None, writer: Optional[Callable] = None):
     """volumetric.py:131-177 without the NIfTI side: returns [(filename, prediction tensor)] and calls
-    ``writer(filename, tensor, prediction_dir)`` per item when given."""
+    ``writer(filename, tensor, prediction_dir)`` per item when given.
+
+    ``resample=True`` maps each activated prediction back onto the grid of the image file it came from, as the reference's
+    ``ResampleToMatch(mode=interpolation)`` against the re-loaded image: ``prepost.resample_to_match`` from the prediction's grid
+    (``meta["affine"]``, the input's affine after orientation, crop and resize) to the file's grid (``meta["original_affine"]``,
+    ``meta["spatial_shape"]``, as LoadImageD records them), so the prediction is fp32 ``[C, *spatial_shape]``.  The file is
+    not read again."""
+    if resample:
+        _prepost.resample_mode(interpolation)       # an unsupported mode fails before the model runs
     results = []
     with torch.no_grad():
         for item in dataloader:
             x = item["image"]
             filenames = [_filename_of(x, i) for i in range(x.shape[0])]
+            grids = [[_grid_meta_of(x, k, i, nd) for k, nd in (("affine", 2), ("original_affine", 2), ("spatial_shape", 1))]
+                     for i in range(x.shape[0])] if resample else None
             xd = x.to(next(model.parameters()).device)
             predictions = inferer(xd, model) if inferer is not None else model(xd)
             if activation == "sigmoid":
@@ -150,7 +182,10 @@ def volumetric_predictions(model, dataloader, prediction_dir, activation=None, r
             elif activation is not None:
                 predictions = getattr(torch, activation)(predictions)
             for i, fn in enumerate(filenames):
-                results.append((fn, predictions[i]))
+                p = predictions[i]
+                if resample:
+                    p = _prepost.resample_to_match(p, *grids[i], mode=interpolation)
+                results.append((fn, p))
                 if writer is not None:
-                    writer(fn, predictions[i], prediction_dir)
+                    writer(fn, p, prediction_dir)
     return results

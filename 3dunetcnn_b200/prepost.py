@@ -6,6 +6,7 @@ Mirrors (paths relative to /root/reference):
   * ``unet3d/datasets/segmentation.py:77-87``  ``normalization="zero_mean"`` -> ``monai.transforms.NormalizeIntensity``
   * ``examples/sppin/process.py:269-274``  SimpleITK ``ConnectedComponent`` + ``RelabelComponent`` -> ``connected_components``;
     ``monai.transforms.KeepLargestConnectedComponent`` -> ``keep_largest_connected_component``
+  * ``unet3d/predict/volumetric.py:135-137,168-170``  ``monai.transforms.ResampleToMatch`` -> ``resample_to_match``
 
 Same names, argument meaning and error behaviour; tensors live on the GPU and every voxel is touched by one
 hand-written kernel of libb200unet instead of a chain of boolean-mask torch ops on the host.  No CPU fallback.
@@ -15,6 +16,7 @@ from __future__ import annotations
 import ctypes as C
 from typing import Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import lib as _lib
@@ -227,3 +229,75 @@ def keep_largest_connected_component(img: torch.Tensor, applied_labels=None, is_
     else:
         out[0].masked_fill_(drop.any(0), 0)      # the label masks are disjoint
     return out
+
+
+# MONAI's resolves_modes maps every *linear mode to grid_sample's bilinear, which is trilinear on a volume
+_RESAMPLE_MODES = {"trilinear": 0, "bilinear": 0, "linear": 0, "nearest": 1}
+# An index-map entry within this distance of an integer is taken as that integer.  A crop, flip or axis permutation composed
+# from inexact voxel spacings (or from affines stored in fp32) then copies voxels exactly instead of blending in a 1e-12 share
+# of a neighbour, and two grids whose index map is the identity to this tolerance count as equal (the resample is skipped).
+INDEX_MAP_TOL = 1e-6
+
+
+def resample_mode(mode) -> int:
+    """the kernel's mode for an ``interpolation`` / ``mode`` argument: 0 trilinear, 1 nearest"""
+    if isinstance(mode, str) and mode in _RESAMPLE_MODES:
+        return _RESAMPLE_MODES[mode]
+    raise NotImplementedError("resample_to_match: mode %r is not implemented; use 'trilinear' (or 'bilinear' / 'linear', the same "
+                              "on a volume) or 'nearest'" % (mode,))
+
+
+def _affines(a, n: int, what: str):
+    """a [4, 4] affine shared by all n items, or one per item [n, 4, 4] -> list of n fp64 arrays"""
+    if isinstance(a, torch.Tensor):
+        a = _plain(a).detach().cpu().double().numpy()
+    a = np.asarray(a, dtype=np.float64)
+    if a.shape == (4, 4):
+        return [a] * n
+    if a.shape == (n, 4, 4):
+        return list(a)
+    raise ValueError("resample_to_match: %s must be a 4x4 affine or one per item [%d, 4, 4], got shape %s" % (what, n, a.shape))
+
+
+def index_map(src_affine, dst_affine) -> np.ndarray:
+    """fp64 3x4 map of a target voxel index (d, h, w, 1) to the source index: inv(src_affine) @ dst_affine, voxel centres on
+    integers (MONAI's spatial_resample with normalized=False).  Entries within INDEX_MAP_TOL of an integer are snapped to it."""
+    m = np.linalg.solve(np.asarray(src_affine, dtype=np.float64), np.asarray(dst_affine, dtype=np.float64))[:3]
+    r = np.rint(m)
+    return np.where(np.abs(m - r) <= INDEX_MAP_TOL, r, m)
+
+
+def resample_to_match(img: torch.Tensor, src_affine, dst_affine, dst_shape, mode: str = "trilinear") -> torch.Tensor:
+    """``monai.transforms.ResampleToMatch(mode)`` as volumetric.py:135-137,168-170 calls it, on the device: resample a channel-first
+    image ``[C, D, H, W]`` (or a batch ``[N, C, D, H, W]``) whose grid has the affine ``src_affine`` onto the grid of shape
+    ``dst_shape`` with the affine ``dst_affine`` (4x4 voxel-to-world; either may be one per item ``[N, 4, 4]``).  Returns fp32
+    ``[C, *dst_shape]`` (``[N, C, *dst_shape]``).  Parity unpinned: MONAI is absent from this image.
+
+    ``mode``: 'trilinear', 'bilinear' or 'linear' (all trilinear on a volume), or 'nearest' (round half to even, as
+    grid_sample); anything else raises ``NotImplementedError``.  Padding is MONAI's default, border: target voxels that map
+    outside the source take the nearest edge value (so outside a foreground crop the prediction's edge extends to the volume
+    boundary, as the reference writes it).  When the shapes are equal and ``index_map`` is the identity (affines equal to
+    INDEX_MAP_TOL) the image is copied unchanged.  One kernel per item, no CPU fallback."""
+    m = resample_mode(mode)
+    _need_cuda(img, "resample_to_match")
+    x = _plain(img)
+    if x.dim() not in (4, 5):
+        raise ValueError("resample_to_match: expected [C, D, H, W] or [N, C, D, H, W], got shape %s" % (tuple(x.shape),))
+    xs = (x if x.dim() == 5 else x[None]).contiguous().float()
+    n, c = xs.shape[:2]
+    src, dst = _affines(src_affine, n, "src_affine"), _affines(dst_affine, n, "dst_affine")
+    shape = tuple(int(s) for s in (dst_shape.tolist() if hasattr(dst_shape, "tolist") else dst_shape))
+    if len(shape) != 3 or min(shape) < 1:
+        raise ValueError("resample_to_match: dst_shape must be three positive extents, got %r" % (dst_shape,))
+    out = torch.empty((n, c) + shape, dtype=torch.float32, device=xs.device)
+    identity = np.eye(4)[:3]
+    lib = _lib.load_library()
+    with torch.cuda.device(xs.device):
+        for i in range(n):
+            a = index_map(src[i], dst[i])
+            if shape == tuple(xs.shape[2:]) and np.array_equal(a, identity):
+                out[i].copy_(xs[i])
+                continue
+            _lib.check(lib.b200unet_resample_to_grid(xs[i].data_ptr(), c, *xs.shape[2:], (C.c_double * 12)(*a.ravel().tolist()), m,
+                                                     out[i].data_ptr(), *shape, _lib.stream_ptr()), "resample_to_grid")
+    return out if x.dim() == 5 else out[0]

@@ -210,6 +210,15 @@ int b200unet_augment_resample(const float* image, const uint8_t* label, int n, i
 int b200unet_augment_intensity(float* image, int n, int c, int64_t spatial, int normalize, int nonzero, int channel_wise,
                                const float* coef, void* scratch, void* stream);
 
+/* ---- a prediction back onto the grid of its image file (monai.transforms.ResampleToMatch as predict/volumetric.py:135-137,
+ * 168-170 calls it): src fp32 [c][sd][sh][sw] -> dst fp32 [c][dd][dh][dw], 1 <= c <= 128, fewer than 2^31 voxels per channel.
+ * affine: HOST fp64 row-major 3x4, target index (d, h, w, 1) -> source index (inv(A_src) A_dst with voxel centres on integers),
+ * copied by value.  mode 0 = trilinear (fp64 coordinate, fp32 weights), 1 = nearest (round half to even).  Border padding:
+ * the source coordinate is clamped to [0, size-1].  Corners of weight 0 are not read: an identity, integer shift, flip or
+ * axis permutation copies every value bit for bit. */
+int b200unet_resample_to_grid(const float* src, int c, int sd, int sh, int sw, const double affine[12], int mode, float* dst, int dd,
+                              int dh, int dw, void* stream);
+
 /* ---- connected components of binary masks (the clean-up after the path: SimpleITK ConnectedComponent + RelabelComponent,
  * MONAI KeepLargestConnectedComponent).  mask uint8 [nvol][d][h][w], nonzero = foreground; each volume is labelled on its own;
  * d*h*w < 2^31.  connectivity in orthogonal hops: 1 = 6 face neighbours, 2 = 18 (+ edges), 3 = 26 (+ corners).
