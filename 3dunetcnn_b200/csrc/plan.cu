@@ -1021,7 +1021,6 @@ static int build_dynunet(Plan& P) {
   B200_REQUIRE(d.n_features >= 1 && d.n_features <= 16, E_UNSUPPORTED, "plan: in_channels=%d unsupported", d.n_features);
   B200_REQUIRE(d.n_outputs >= 1 && d.n_outputs <= B200_HEAD_MAX_OUTPUTS, E_UNSUPPORTED, "plan: out_channels=%d unsupported (1..%d)",
                d.n_outputs, B200_HEAD_MAX_OUTPUTS);
-  P.slope = d.act_slope;
   std::vector<int> F, Ds, Hs, Ws;
   {
     int D = d.depth, H = d.height, W = d.width;
@@ -1188,6 +1187,7 @@ int b200unet_plan_create(const b200unet_net_desc* desc, b200unet_plan** out) {
   P->infer = desc->inference_only != 0;
   P->deterministic = desc->deterministic != 0;
   P->input_grad = desc->input_grad != 0;
+  P->slope = desc->act_slope;
   if (P->input_grad && P->infer) {
     set_error("plan_create: input_grad=1 on an inference_only plan (the input gradient needs the backward schedule)");
     delete P;

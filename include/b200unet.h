@@ -250,7 +250,8 @@ typedef struct b200unet_net_desc {
                                  examples/brats2020/brats2020_config.json:2-107: n_levels = len(filters), kernel 3, strides
                                  1,2,2,..., transposed-conv upsampling kernel = stride = 2, InstanceNorm(affine) + LeakyReLU */
   int32_t filters[8];         /* arch 1: channels per level (multiples of 8) */
-  float act_slope;            /* arch 1: negative slope of the LeakyReLU (0.01) */
+  float act_slope;            /* both architectures: negative slope of the activation after each norm; 0 = the reference
+                                 UNet3D's ReLU, 0.01 = DynUNet's LeakyReLU */
   int32_t deterministic;      /* 1 = weight gradients without floating-point atomics: the split-K CTAs write per-split partial
                                  sums, a second kernel adds them in a fixed order (bit-identical gradients run to run) */
   int32_t inference_only;     /* 1 = forward-only plan (volumetric.py:131-150 runs under no_grad): no backward schedule, no

@@ -149,45 +149,48 @@ def make_state_dict(cfg: UNetConfig, seed: int = 0, dtype=torch.float32) -> Dict
 # --------------------------------------------------------------------------------------
 # forward restatement
 # --------------------------------------------------------------------------------------
-def _conv_block(sd, prefix, x, cfg: UNetConfig, stride=1):
+def _conv_block(sd, prefix, x, cfg: UNetConfig, stride=1, slope: float = 0.0):
     # myronenko.py:17-21  GN -> ReLU -> conv (bias-free, padding=k//2: resnet.py:12-17)
     cin = x.shape[1]
     x = F.group_norm(x, _groups(cin, cfg.norm_groups), sd[f"{prefix}.norm1.weight"], sd[f"{prefix}.norm1.bias"], eps=1e-5)
-    x = F.relu(x)
+    x = F.relu(x) if slope == 0.0 else F.leaky_relu(x, slope)
     return F.conv3d(x, sd[f"{prefix}.conv.weight"], None, stride=stride, padding=cfg.kernel_size // 2)
 
 
-def _res_block(sd, prefix, x, cfg: UNetConfig):
+def _res_block(sd, prefix, x, cfg: UNetConfig, slope: float = 0.0):
     # myronenko.py:47-58
     identity = x
-    y = _conv_block(sd, f"{prefix}.conv1", x, cfg)
-    y = _conv_block(sd, f"{prefix}.conv2", y, cfg)
+    y = _conv_block(sd, f"{prefix}.conv1", x, cfg, slope=slope)
+    y = _conv_block(sd, f"{prefix}.conv2", y, cfg, slope=slope)
     if f"{prefix}.sample.weight" in sd:
         identity = F.conv3d(identity, sd[f"{prefix}.sample.weight"])
     return y + identity
 
 
-def _layer(sd, prefix, x, n_blocks, cfg, dropout_mask=None):
+def _layer(sd, prefix, x, n_blocks, cfg, dropout_mask=None, slope: float = 0.0):
     # myronenko.py:75-80 ; Dropout3d after block 0 (level 0 of the encoder only, myronenko.py:97-100)
     for b in range(n_blocks):
-        x = _res_block(sd, f"{prefix}.blocks.{b}", x, cfg)
+        x = _res_block(sd, f"{prefix}.blocks.{b}", x, cfg, slope)
         if b == 0 and dropout_mask is not None:
             x = x * dropout_mask.to(x.dtype).view(x.shape[0], x.shape[1], 1, 1, 1)
     return x
 
 
 def unet3d_forward(sd: Dict[str, torch.Tensor], x: torch.Tensor, cfg: UNetConfig,
-                   dropout_mask: Optional[torch.Tensor] = None, return_intermediates: bool = False):
+                   dropout_mask: Optional[torch.Tensor] = None, return_intermediates: bool = False,
+                   slope: float = 0.0):
     """Reference ``UNet3D.forward`` (variational.py:81-87 -> unet.py:8-16 -> unet.py:27-44).
 
     ``dropout_mask``: optional (N, C0) tensor of per-channel scales (0 or 1/(1-p)) applied after
     block 0 of encoder level 0 -- Dropout3d semantics (SURVEY appendix C).  None == eval mode.
+    ``slope``: negative slope of the activation after each GroupNorm; 0 is the reference's ReLU.  Slope 1 makes
+    the network smooth, so its gradients can be compared at tight bounds (tests/plan_smooth_cases.py).
     """
     nlev = len(cfg.encoder_blocks)
     skips = []
     inter = {}
     for li, nb in enumerate(cfg.encoder_blocks):
-        x = _layer(sd, f"encoder.layers.{li}", x, nb, cfg, dropout_mask if li == 0 else None)
+        x = _layer(sd, f"encoder.layers.{li}", x, nb, cfg, dropout_mask if li == 0 else None, slope)
         skips.insert(0, x)  # unet.py:12
         if li != nlev - 1:
             x = F.conv3d(x, sd[f"encoder.downsampling_convolutions.{li}.weight"], None,
@@ -196,7 +199,7 @@ def unet3d_forward(sd: Dict[str, torch.Tensor], x: torch.Tensor, cfg: UNetConfig
     dblocks = cfg.dec_blocks()
     x = skips[0]
     for i in range(len(dblocks) - 1):
-        x = _layer(sd, f"decoder.layers.{i}", x, dblocks[i], cfg)          # unet.py:30
+        x = _layer(sd, f"decoder.layers.{i}", x, dblocks[i], cfg, slope=slope)  # unet.py:30
         if cfg.use_transposed_convolutions:
             x = F.conv_transpose3d(x, sd[f"decoder.upsampling_blocks.{i}.weight"],
                                    sd[f"decoder.upsampling_blocks.{i}.bias"],
@@ -211,7 +214,7 @@ def unet3d_forward(sd: Dict[str, torch.Tensor], x: torch.Tensor, cfg: UNetConfig
         dx = skip.shape[4] - x.shape[4]
         x = F.pad(x, [dx // 2, dx - dx // 2, dy // 2, dy - dy // 2, dz // 2, dz - dz // 2])  # unet.py:34-40
         x = torch.cat((x, skip), 1)                                                       # unet.py:42
-    x = _layer(sd, f"decoder.layers.{len(dblocks) - 1}", x, dblocks[-1], cfg)             # unet.py:43
+    x = _layer(sd, f"decoder.layers.{len(dblocks) - 1}", x, dblocks[-1], cfg, slope=slope)  # unet.py:43
     inter["decoder_out"] = x
     x = F.conv3d(x, sd["final_convolution.weight"])                                       # variational.py:84
     if cfg.activation == "sigmoid":
