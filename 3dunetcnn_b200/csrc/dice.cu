@@ -31,14 +31,15 @@ __device__ __forceinline__ double block_sum(double v, double* sh) {
   return r;
 }
 
-// grid (chunks, N*C); sums[(n*C+c)*3 + {0,1,2}] += (I, P, T)
+// grid (chunks, N*C); sums[(n*C+c)*3 + {0,1,2}] += (I, P, T).  vec: 4 voxels per load (uint8 targets only; the launcher
+// checks S % 4 and the alignment of both pointers)
 template <typename TT>
-__global__ void k_dice_sums(const float* __restrict__ x, const TT* __restrict__ t, long long S, DiceFlags f,
+__global__ void k_dice_sums(const float* __restrict__ x, const TT* __restrict__ t, long long S, int vec, DiceFlags f,
                             double* __restrict__ sums) {
   __shared__ double sh[32];
   const long long base = (long long)blockIdx.y * S;
   float aI = 0.f, aP = 0.f, aT = 0.f;
-  if ((S & 3) == 0 && sizeof(TT) == 1) {
+  if (vec && sizeof(TT) == 1) {
     const float4* x4 = reinterpret_cast<const float4*>(x + base);
     const uchar4* t4 = reinterpret_cast<const uchar4*>(t + base);
     const long long n4 = S >> 2;
@@ -156,8 +157,12 @@ int launch_dice_fwd(const float* logits, const uint8_t* target, int N, int C, lo
   int chunks = (int)(per < 1 ? 1 : per);
   int cap = (132 * 8 + N * C - 1) / (N * C);
   if (chunks > cap) chunks = cap < 1 ? 1 : cap;
-  if (flags & 64) k_dice_sums<float><<<dim3(chunks, N * C), 256, 0, st>>>(logits, reinterpret_cast<const float*>(target), S, f, sums);
-  else k_dice_sums<uint8_t><<<dim3(chunks, N * C), 256, 0, st>>>(logits, target, S, f, sums);
+  // float4 / uchar4 loads need S % 4 == 0 and 16- / 4-byte aligned pointers: a contiguous view at a storage offset (a slice
+  // of a wider tensor) may not be, and takes the scalar loop
+  const int vec = (S & 3) == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0 && (reinterpret_cast<uintptr_t>(target) & 3) == 0;
+  if (flags & 64)
+    k_dice_sums<float><<<dim3(chunks, N * C), 256, 0, st>>>(logits, reinterpret_cast<const float*>(target), S, 0, f, sums);
+  else k_dice_sums<uint8_t><<<dim3(chunks, N * C), 256, 0, st>>>(logits, target, S, vec, f, sums);
   B200_CHECK_CUDA(cudaGetLastError());
   k_dice_finalize<<<1, 32, 0, st>>>(sums, N, C, f, nr, dr, loss);
   B200_CHECK_CUDA(cudaGetLastError());
