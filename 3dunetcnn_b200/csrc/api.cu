@@ -85,7 +85,7 @@ using namespace b200;
 
 extern "C" {
 
-int b200unet_version(void) { return 104; }
+int b200unet_version(void) { return 105; }
 const char* b200unet_last_error(void) { return get_error(); }
 
 int b200unet_ncdhw_to_ndhwc(const float* x, int c_real, const b200unet_tensor* out, void* stream) {
@@ -258,6 +258,20 @@ int b200unet_augment_resample(const float* image, const uint8_t* label, int n, i
 int b200unet_augment_intensity(float* image, int n, int c, int64_t spatial, int normalize, int nonzero, int channel_wise,
                                const float* coef, void* scratch, void* stream) {
   return launch_augment_intensity(image, n, c, spatial, normalize, nonzero, channel_wise, coef, scratch, to_stream(stream));
+}
+static_assert(sizeof(AugSample) == 5 * sizeof(int64_t), "b200unet.h sample rows are five int64");
+size_t b200unet_foreground_scratch_bytes(int n, int c) { return foreground_scratch_bytes(n, c); }
+int b200unet_foreground_box(const int64_t* samples, int n, int c, int64_t max_spatial, int crop, const int64_t* ranks,
+                            const float* gamma, int margin, int allow_smaller, const double* affine, int d, int h, int w,
+                            float* affine_out, int32_t* box, int32_t* empty, float* threshold, void* scratch, void* stream) {
+  return launch_foreground_box(reinterpret_cast<const AugSample*>(samples), n, c, max_spatial, crop,
+                               reinterpret_cast<const long long*>(ranks), gamma, margin, allow_smaller, affine, d, h, w, affine_out,
+                               box, empty, threshold, scratch, to_stream(stream));
+}
+int b200unet_augment_resample_samples(const int64_t* samples, int n, int c, int l, int d, int h, int w, const float* affine,
+                                      int padding, int nonzero, float* image_out, uint8_t* label_out, void* scratch, void* stream) {
+  return launch_augment_resample_samples(reinterpret_cast<const AugSample*>(samples), n, c, l, d, h, w, affine, padding, nonzero,
+                                         image_out, label_out, scratch, to_stream(stream));
 }
 
 int b200unet_resample_to_grid(const float* src, int c, int sd, int sh, int sw, const double affine[12], int mode, float* dst, int dd,

@@ -4,7 +4,8 @@
 //
 //   k_aug_resample   pass 1: one thread per output voxel maps (d, h, w) through the sample's 3x4 index-space affine to a source
 //                    position and samples every image channel there (trilinear) and every label channel (nearest); the same
-//                    pass writes per-block fp64 (sum, sumsq, count) partials of the resampled image per (n, c)
+//                    pass writes per-block fp64 (sum, sumsq, count) partials of the resampled image per (n, c).  The source is
+//                    the batch itself on the output grid, or per sample a pointer and extents of its own (foreground.cu)
 //   k_aug_stats      fixed-order reduction of the partials -> stats [n][c][3]
 //   k_aug_apply      pass 2, in place: y = ((x - mean) / std) * a + b per (n, c)
 //
@@ -38,11 +39,14 @@ struct AugDims {
   long long S;
 };
 
+// g: the output grid.  samples == nullptr: sample n reads img / lab at n * C * g.S / n * L * g.S on the same grid; otherwise
+// samples[n] gives its own source pointers and extents (a batch of different sizes resampled onto one grid)
 template <int CM>
 __global__ void __launch_bounds__(kAugThreads) k_aug_resample(const float* __restrict__ img, const uint8_t* __restrict__ lab,
-                                                               int C, int L, AugDims g, const float* __restrict__ affine,
-                                                               int border, int nonzero, float* __restrict__ out,
-                                                               uint8_t* __restrict__ lout, double* __restrict__ part) {
+                                                               const AugSample* __restrict__ samples, int C, int L, AugDims g,
+                                                               const float* __restrict__ affine, int border, int nonzero,
+                                                               float* __restrict__ out, uint8_t* __restrict__ lout,
+                                                               double* __restrict__ part) {
   const int n = blockIdx.y;
   const int nb = gridDim.x;
   const long long per = (g.S + nb - 1) / nb;
@@ -51,7 +55,19 @@ __global__ void __launch_bounds__(kAugThreads) k_aug_resample(const float* __res
   float m[12];
 #pragma unroll
   for (int k = 0; k < 12; ++k) m[k] = __ldg(affine + n * 12 + k);
-  const float* src = img + (long long)n * C * g.S;
+  const float* src;
+  const uint8_t* lp;
+  int SD, SH, SW;
+  if (samples) {
+    const AugSample sm = samples[n];
+    src = sm.img; lp = sm.lab;
+    SD = (int)sm.d; SH = (int)sm.h; SW = (int)sm.w;
+  } else {
+    src = img + (long long)n * C * g.S;
+    lp = L > 0 ? lab + (long long)n * L * g.S : nullptr;
+    SD = g.D; SH = g.H; SW = g.W;
+  }
+  const long long SS = (long long)SD * SH * SW;     // source channel stride
   float* dst = out + (long long)n * C * g.S;
 
   double s[CM], q[CM];
@@ -70,11 +86,11 @@ __global__ void __launch_bounds__(kAugThreads) k_aug_resample(const float* __res
     const float sh = fmaf(m[4], fd, fmaf(m[5], fh, fmaf(m[6], fw, m[7])));
     const float sw = fmaf(m[8], fd, fmaf(m[9], fh, fmaf(m[10], fw, m[11])));
 
-    const Trilinear t = trilinear_corners(sd, sh, sw, g.D, g.H, g.W, border);   // offsets within one plane: S < 2^31
+    const Trilinear t = trilinear_corners(sd, sh, sw, SD, SH, SW, border);   // offsets within one plane: S < 2^31
 #pragma unroll
     for (int c = 0; c < CM; ++c) {
       if (c < C) {
-        float y = trilinear_sample(src + (long long)c * g.S, t);
+        float y = trilinear_sample(src + (long long)c * SS, t);
         if (!t.any) y = 0.f;            // every corner outside the volume (zeros padding)
         dst[(long long)c * g.S + v] = y;
         if (!nonzero || y != 0.f) { s[c] += y; q[c] += (double)y * y; cnt[c] += 1u; }
@@ -82,14 +98,13 @@ __global__ void __launch_bounds__(kAugThreads) k_aug_resample(const float* __res
     }
     if (L > 0) {
       // nearest: round half to even of the (clamped) coordinate, as grid_sample's nearest mode
-      const float rd = rintf(border ? fminf(fmaxf(sd, 0.f), (float)(g.D - 1)) : sd);
-      const float rh = rintf(border ? fminf(fmaxf(sh, 0.f), (float)(g.H - 1)) : sh);
-      const float rw = rintf(border ? fminf(fmaxf(sw, 0.f), (float)(g.W - 1)) : sw);
-      const bool in = rd >= 0.f && rd < (float)g.D && rh >= 0.f && rh < (float)g.H && rw >= 0.f && rw < (float)g.W;
-      const int o = in ? ((int)rd * g.H + (int)rh) * g.W + (int)rw : 0;
-      const uint8_t* lp = lab + (long long)n * L * g.S;
+      const float rd = rintf(border ? fminf(fmaxf(sd, 0.f), (float)(SD - 1)) : sd);
+      const float rh = rintf(border ? fminf(fmaxf(sh, 0.f), (float)(SH - 1)) : sh);
+      const float rw = rintf(border ? fminf(fmaxf(sw, 0.f), (float)(SW - 1)) : sw);
+      const bool in = rd >= 0.f && rd < (float)SD && rh >= 0.f && rh < (float)SH && rw >= 0.f && rw < (float)SW;
+      const int o = in ? ((int)rd * SH + (int)rh) * SW + (int)rw : 0;
       uint8_t* lo = lout + (long long)n * L * g.S;
-      for (int c = 0; c < L; ++c) lo[(long long)c * g.S + v] = in ? __ldg(lp + (long long)c * g.S + o) : (uint8_t)0;
+      for (int c = 0; c < L; ++c) lo[(long long)c * g.S + v] = in ? __ldg(lp + (long long)c * SS + o) : (uint8_t)0;
     }
   }
 
@@ -177,10 +192,11 @@ __global__ void __launch_bounds__(kAugThreads) k_aug_apply(float* __restrict__ x
   }
 }
 
-int launch_augment_resample(const float* img, const uint8_t* lab, int N, int C, int L, int D, int H, int W, const float* affine,
-                            int padding, int nonzero, float* img_out, uint8_t* lab_out, void* scratch, cudaStream_t st) {
-  B200_REQUIRE(img && img_out && affine && scratch, E_INVALID, "augment_resample: null argument");
-  B200_REQUIRE(L == 0 || (lab && lab_out), E_INVALID, "augment_resample: %d label channels but no label tensors", L);
+static int augment_resample(const float* img, const uint8_t* lab, const AugSample* samples, int N, int C, int L, int D, int H, int W,
+                            const float* affine, int padding, int nonzero, float* img_out, uint8_t* lab_out, void* scratch,
+                            cudaStream_t st) {
+  B200_REQUIRE(affine && img_out && scratch, E_INVALID, "augment_resample: null argument");
+  B200_REQUIRE(L == 0 || lab_out, E_INVALID, "augment_resample: %d label channels but no label output", L);
   B200_REQUIRE(N >= 1 && N <= 65535 && D >= 1 && H >= 1 && W >= 1 && L >= 0, E_INVALID,
                "augment_resample: bad shape n=%d l=%d %dx%dx%d", N, L, D, H, W);
   B200_REQUIRE(padding == 0 || padding == 1, E_UNSUPPORTED, "augment_resample: padding 0 (border) or 1 (zeros), got %d", padding);
@@ -191,12 +207,25 @@ int launch_augment_resample(const float* img, const uint8_t* lab, int N, int C, 
   double* part = reinterpret_cast<double*>(scratch) + (size_t)N * C * 3;
   const int border = padding == 0;
   if (C <= 4)
-    k_aug_resample<4><<<grid, kAugThreads, 0, st>>>(img, lab, C, L, g, affine, border, nonzero, img_out, lab_out, part);
+    k_aug_resample<4><<<grid, kAugThreads, 0, st>>>(img, lab, samples, C, L, g, affine, border, nonzero, img_out, lab_out, part);
   else
-    k_aug_resample<B200_AUG_MAX_CHANNELS><<<grid, kAugThreads, 0, st>>>(img, lab, C, L, g, affine, border, nonzero, img_out, lab_out,
-                                                                       part);
+    k_aug_resample<B200_AUG_MAX_CHANNELS><<<grid, kAugThreads, 0, st>>>(img, lab, samples, C, L, g, affine, border, nonzero, img_out,
+                                                                       lab_out, part);
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;
+}
+
+int launch_augment_resample(const float* img, const uint8_t* lab, int N, int C, int L, int D, int H, int W, const float* affine,
+                            int padding, int nonzero, float* img_out, uint8_t* lab_out, void* scratch, cudaStream_t st) {
+  B200_REQUIRE(img, E_INVALID, "augment_resample: null argument");
+  B200_REQUIRE(L == 0 || lab, E_INVALID, "augment_resample: %d label channels but no label tensors", L);
+  return augment_resample(img, lab, nullptr, N, C, L, D, H, W, affine, padding, nonzero, img_out, lab_out, scratch, st);
+}
+
+int launch_augment_resample_samples(const AugSample* samples, int N, int C, int L, int D, int H, int W, const float* affine,
+                                    int padding, int nonzero, float* img_out, uint8_t* lab_out, void* scratch, cudaStream_t st) {
+  B200_REQUIRE(samples, E_INVALID, "augment_resample_samples: null sample table");
+  return augment_resample(nullptr, nullptr, samples, N, C, L, D, H, W, affine, padding, nonzero, img_out, lab_out, scratch, st);
 }
 
 int launch_augment_intensity(float* img, int N, int C, long long S, int normalize, int nonzero, int channel_wise, const float* coef,

@@ -115,9 +115,29 @@ size_t augment_scratch_bytes(int N, int C, long long S);
 // affine: DEVICE [N][12] fp32 row-major 3x4 (output index (d, h, w) -> source index); padding 0 border, 1 zeros; L = 0: no label
 int launch_augment_resample(const float* img, const uint8_t* lab, int N, int C, int L, int D, int H, int W, const float* affine,
                             int padding, int nonzero, float* img_out, uint8_t* lab_out, void* scratch, cudaStream_t st);
+// one sample of a batch of different extents (DEVICE table, the layout of b200unet.h's sample rows): image [C][d][h][w] fp32,
+// label [L][d][h][w] uint8 (nullptr without a label)
+struct AugSample {
+  const float* img;
+  const uint8_t* lab;
+  long long d, h, w;
+};
+// as launch_augment_resample onto the (D, H, W) grid, sample n read from samples[n]
+int launch_augment_resample_samples(const AugSample* samples, int N, int C, int L, int D, int H, int W, const float* affine,
+                                    int padding, int nonzero, float* img_out, uint8_t* lab_out, void* scratch, cudaStream_t st);
 // in place on the resampled image; coef: DEVICE [N][C][2] (a, b)
 int launch_augment_intensity(float* img, int N, int C, long long S, int normalize, int nonzero, int channel_wise, const float* coef,
                              void* scratch, cudaStream_t st);
+
+// ---- foreground box of each sample + the composed crop / resize / augmentation affine (foreground.cu)
+// scratch: select histograms and state per (sample, channel), box accumulators per sample; 0: the shape is rejected
+size_t foreground_scratch_bytes(int N, int C);
+// crop = 0: the whole volume; ranks == nullptr: select x > 0; else x > thr with thr per (n, c) the linear interpolation
+// (weight gamma[n][c]) of the order statistics ranks[n][c][0..1], written to thr.  affine_in DEVICE fp64 [N][12] on the
+// (OD, OH, OW) grid -> affine_out fp32 [N][12] onto the sample's own grid; box int32 [N][3][2] (start, end), empty int32 [N]
+int launch_foreground_box(const AugSample* samples, int N, int C, long long max_spatial, int crop, const long long* ranks,
+                          const float* gamma, int margin, int allow_smaller, const double* affine_in, int OD, int OH, int OW,
+                          float* affine_out, int32_t* box, int32_t* empty, float* thr, void* scratch, cudaStream_t st);
 
 // ---- resample a prediction onto the grid of its image file (resample.cu)
 // row-major 3x4 map of target index (d, h, w, 1) -> source index, passed by value

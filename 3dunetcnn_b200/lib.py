@@ -149,6 +149,10 @@ _SIGS = {
                                             C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200unet_augment_intensity": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                              C.c_void_p, C.c_void_p]),
+    "b200unet_foreground_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "b200unet_foreground_box": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                          C.c_void_p, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 6),
+    "b200unet_augment_resample_samples": (C.c_int, [C.c_void_p] + [C.c_int] * 6 + [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 4),
     "b200unet_resample_to_grid": (C.c_int, [C.c_void_p] + [C.c_int] * 4 + [C.POINTER(C.c_double), C.c_int, C.c_void_p] + [C.c_int] * 3
                                   + [C.c_void_p]),
     "b200unet_cc_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),

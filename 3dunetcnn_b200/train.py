@@ -162,7 +162,10 @@ class DevicePrefetcher:
             out = dict(item)
             for k in ("image", "label"):
                 t = item[k]
-                out[k] = t if t.is_cuda else t.to(self.device, non_blocking=True)
+                if isinstance(t, (list, tuple)):      # augment.list_collate: samples of different sizes
+                    out[k] = [x if x.is_cuda else x.to(self.device, non_blocking=True) for x in t]
+                else:
+                    out[k] = t if t.is_cuda else t.to(self.device, non_blocking=True)
             if self.transform is not None:
                 out = self.transform(out)
             ev = torch.cuda.Event()
@@ -184,7 +187,8 @@ class DevicePrefetcher:
             main = torch.cuda.current_stream(self.device)
             main.wait_event(ev)
             for k in ("image", "label"):
-                cur[k].record_stream(main)
+                for t in (cur[k] if isinstance(cur[k], (list, tuple)) else (cur[k],)):
+                    t.record_stream(main)
             yield cur
 
 
@@ -237,7 +241,9 @@ def epoch_training(train_loader, model, criterion, optimizer, epoch, n_gpus=None
     e.g. a short last batch, run eagerly.  On a GPU the loader is read one batch ahead (``DevicePrefetcher``) and the
     loss of step i is read back while step i+1 runs, so the only host syncs are one step behind the queue.
     ``device_transform`` (optional, e.g. the ``Compose`` of ``augment.build_device_transform``) runs on every staged training
-    batch on the prefetcher's copy stream, overlapping the running step; it keeps each batch's shapes and dtypes."""
+    batch on the prefetcher's copy stream, overlapping the running step.  It keeps each batch's dtypes; one with a geometry
+    stage (``build_device_transform(..., geometry=True)``) changes its spatial shape: it takes the lists of different-size
+    samples a ``collate_fn=augment.list_collate`` loader yields and returns one batch at its ``spatial_size``."""
     graphed = None
     batch_time = AverageMeter("Time", ":6.3f")
     data_time = AverageMeter("Data", ":6.3f")

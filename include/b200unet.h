@@ -210,6 +210,29 @@ int b200unet_augment_resample(const float* image, const uint8_t* label, int n, i
 int b200unet_augment_intensity(float* image, int n, int c, int64_t spatial, int normalize, int nonzero, int channel_wise,
                                const float* coef, void* scratch, void* stream);
 
+/* ---- foreground crop + resize of a training batch of different extents, composed with the augmentation into the one resample
+ * above (MONAI CropForegroundD with the reference's percentile_threshold, then ResizeD, as datasets/segmentation.py:55-70 chains
+ * them lazily).  samples: DEVICE int64 [n][5] rows (image pointer, label pointer or 0, d, h, w): sample i is fp32
+ * [c][d][h][w] and uint8 [l][d][h][w], each fewer than 2^31 voxels per channel.
+ *   foreground_scratch_bytes: from (n, c) alone (0 = rejected: 1..16 channels, 1..65535 samples).
+ *   foreground_box: crop = 0 takes every whole volume; otherwise the mask is any_c(x_c > thr_c) with thr = 0 (ranks NULL,
+ *                  MONAI's default select_fn) or thr_c the linear interpolation, weight gamma DEVICE fp32 [n][c], between
+ *                  the order statistics of ranks DEVICE int64 [n][c][2] (np.percentile's two neighbours), written to
+ *                  threshold DEVICE fp32 [n][c] (NaN when the channel holds a NaN).  Box per axis [first - margin, last +
+ *                  margin + 1), clipped to the volume when allow_smaller; an empty mask takes the whole volume and sets
+ *                  empty[i] = 1.  box DEVICE int32 [n][3][2] (start, end).  affine DEVICE fp64 [n][3][4] (index space on the
+ *                  (d, h, w) output grid) -> affine_out DEVICE fp32 [n][3][4] onto the sample's own grid:
+ *                  box start + s * (A p) + (s - 1) / 2, s = box size / output size.  max_spatial: the largest d*h*w of the
+ *                  batch (sizes the grids).  Nothing is read back to the host.
+ *   augment_resample_samples: augment_resample onto the (d, h, w) output grid, sample i read from samples[i] at its own extents
+ *                  (affine_out above); the output, the scratch and augment_intensity are as for augment_resample. */
+size_t b200unet_foreground_scratch_bytes(int n, int c);
+int b200unet_foreground_box(const int64_t* samples, int n, int c, int64_t max_spatial, int crop, const int64_t* ranks,
+                            const float* gamma, int margin, int allow_smaller, const double* affine, int d, int h, int w,
+                            float* affine_out, int32_t* box, int32_t* empty, float* threshold, void* scratch, void* stream);
+int b200unet_augment_resample_samples(const int64_t* samples, int n, int c, int l, int d, int h, int w, const float* affine,
+                                      int padding, int nonzero, float* image_out, uint8_t* label_out, void* scratch, void* stream);
+
 /* ---- a prediction back onto the grid of its image file (monai.transforms.ResampleToMatch as predict/volumetric.py:135-137,
  * 168-170 calls it): src fp32 [c][sd][sh][sw] -> dst fp32 [c][dd][dh][dw], 1 <= c <= 128, fewer than 2^31 voxels per channel.
  * affine: HOST fp64 row-major 3x4, target index (d, h, w, 1) -> source index (inv(A_src) A_dst with voxel centres on integers),
