@@ -323,6 +323,7 @@ int b200unet_diag_wgrad_route(const b200unet_tensor* a, const b200unet_tensor* d
   route->groups = r.groups; route->cotiles = r.cotiles; route->kblocks = r.kblocks; route->splits = r.splits; route->npass = r.npass;
   route->tw = r.tw; route->th = r.th; route->td = r.td;
   route->part_bytes = (int64_t)r.part_bytes;
+  route->ctas = r.ctas;
   return OK;
 }
 

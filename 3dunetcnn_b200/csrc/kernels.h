@@ -214,7 +214,7 @@ struct WgradOp {
   int Cip;     // pitch of the [T][Cip][Cop] fp32 accumulator rows
   int Cop;
   float* dw;   // fp32 [T][Cip][Cop]; accumulated with atomics, caller zero-fills
-  // deterministic mode (optional): the split-K CTAs store their partial sums into part[split][T][Cip][Cop] instead of
+  // deterministic mode (optional): the split-K CTAs store their partial sums into slots part[slot][T][Cip][Cop] instead of
   // accumulating into dw with atomics; launch_wgrad_reduce then sums the slots in a fixed order.
   float* part;
   size_t part_bytes;
@@ -228,11 +228,12 @@ enum WgradKind { WGRAD_KIND_SIMT = 0, WGRAD_KIND_TAP = 1, WGRAD_KIND_HALO = 2 };
 struct WgradRoute {
   int kind;                 // WgradKind
   int ci8;                  // SIMT: input channels / 8
-  int CB, BN, QT;           // tensor-core kernels: channels per M box, N tile, M tiles per CTA
+  int CB, BN, QT;           // tensor-core kernels: channels per M box, N tile, M tiles per CTA (per work item)
   int nci, units, qtiles;   // CB chunks per tap, (tap, chunk) units, M tiles in total
   int groups, cotiles, kblocks, splits, npass;
   int tw, th, td;
   size_t part_bytes;        // deterministic mode: splits * T * Cip * Cop * 4, the partial buffer this launch fills
+  int ctas;                 // tensor-core kernels: CTAs of the launch
 };
 int wgrad_route(const WgradOp& op, int num_sms, WgradRoute* r);
 int launch_wgrad(const WgradOp& op, cudaStream_t st);              // dispatcher: SIMT register tile for narrow 1x1x1

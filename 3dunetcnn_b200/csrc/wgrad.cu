@@ -11,10 +11,14 @@
 //                        M tile, for Cin >= 128 one tap fills it - no padding waste for narrow layers.
 //   N side (BN columns) = output channels of dY, one or two boxes of min(BN,64) channels.
 //   K                   = the 128 voxels of a spatial tile, 8 steps of K=16 per tile, each two m64 wgmmas (the M halves).
-// A CTA owns QT = 128/BN M-tiles (accumulators in the registers of its consumer warpgroup) and a contiguous range of voxel
-// tiles (split-K); the dY tile of a voxel block is loaded once and reused by all of the CTA's M-tiles.  Partial sums are
-// reduced into the fp32 gradient buffer with vector atomics.  Split-precision mode: passes (a_hi,dy_hi), (a_lo,dy_hi),
-// (a_hi,dy_lo).  3x3x3 stride-1 layers of at most 64 input channels run in halo mode instead (k_wgrad_halo, WgradHaloCfg).
+// Work item = (group of up to 2 * 128/BN M tiles, N tile); iteration = (work item, voxel tile).  The per-tap kernel is
+// stream-K: `ctas` persistent CTAs take contiguous, equal (within one) ranges of the items x voxel tiles iterations, items
+// outer, and flush their register accumulators whenever the item changes and at the end of the range.  Two consumer
+// warpgroups share each dY tile, each with its own M tiles; an item with a single M tile splits its voxel tiles between them.
+// Partial sums are reduced into the fp32 gradient buffer with vector atomics, or stored into the slot of the CTA's rank among
+// the item's CTAs (deterministic mode).  Split-precision mode: passes (a_hi,dy_hi), (a_lo,dy_hi), (a_hi,dy_lo).  3x3x3
+// stride-1 layers of at most 64 input channels run in halo mode instead (k_wgrad_halo, WgradHaloCfg: grid of splits x M-tile
+// groups x N tiles).
 #include <algorithm>
 #include "conv_common.cuh"
 
@@ -33,16 +37,19 @@ struct WgradArgs {
   int nci;        // ci chunks per tap
   int units;      // ntaps * nci
   int qtiles;     // M-tiles in total
-  int qt;         // M-tiles per CTA
+  int qt;         // M-tiles per CTA (per-tap kernel: per work item)
   int kblocks;    // voxel tiles in total
-  int splits;
+  int splits;     // halo kernel: split-K CTAs per work item; per-tap kernel: partial slots per work item (deterministic mode)
+  int cotiles;    // N tiles
+  int items;      // per-tap kernel: work items, M-tile groups x cotiles
+  int ctas;       // per-tap kernel: persistent CTAs over the items x kblocks iterations
   int npass;
   float* dw;
   float* part;             // deterministic mode: per-split partial sums [splits][T][Cip][Cop] (plain stores) instead of atomics
   long long part_stride;   // elements per split
 };
 
-constexpr int WG_A_STAGES = 4;
+constexpr int WG_A_STAGES = 2;   // per consumer warpgroup
 constexpr int WG_D_STAGES = 2;
 constexpr int WG_A_BYTES = 32768;
 
@@ -54,7 +61,7 @@ struct WgradCfg {
   static constexpr int QT = 128 / BN;              // M tiles per consumer warpgroup: QT * BN fp32 accumulator registers per thread
   static constexpr int D_BYTES = BN * 128 * 2;
   static constexpr int D_STAGE = D_BYTES < 1024 ? 1024 : D_BYTES;
-  static constexpr int A_REGION = WG_A_STAGES * WG_A_BYTES;
+  static constexpr int A_REGION = 2 * WG_A_STAGES * WG_A_BYTES;   // one A ring per consumer warpgroup
   static constexpr int SMEM_BYTES = A_REGION + WG_D_STAGES * D_STAGE + 1024 + 1024;
   static_assert(SMEM_BYTES <= 232448, "wgrad: configuration does not fit shared memory");
   static constexpr uint32_t LAYOUT_A = swizzle_for_row_bytes(CB * 2);
@@ -78,36 +85,43 @@ struct WgradHaloCfg : WgradCfg<64, BN> {
   static_assert(SMEM_BYTES <= 232448, "wgrad: configuration does not fit shared memory");
 };
 
-// Warps 0-3: one consumer warpgroup (wgmma issue and the write-back); warp 4: TMA producer.
+// Stream-K partition of the per-tap kernel: CTA c of P runs iterations [c * T / P, (c + 1) * T / P) of the T = items x kblocks,
+// items outer.  The CTA that runs iteration x:
+__host__ __device__ inline int wgrad_sk_cta(long long x, long long T, int P) { return (int)(((x + 1) * P - 1) / T); }
+
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
+// Warps 0-7: two consumer warpgroups (wgmma issue and the write-back); warp 8: TMA producer.  Every CTA walks its stream-K
+// range as segments of one work item each.  An item of nq >= 2 M tiles gives warpgroup 0 its first ceil(nq / 2) M tiles and
+// warpgroup 1 the rest, and both read every dY tile.  An item of one M tile gives it to both: warpgroup g takes the segment's
+// voxel tiles kb with (kb - kb0) % 2 == g.  Each warpgroup has its own A ring; the dY ring is released by all eight warps.
 template <int CB, int BN>
-__global__ void __launch_bounds__(160, 1) k_wgrad(const __grid_constant__ WgradMaps maps, const WgradArgs p) {
+__global__ void __launch_bounds__(288, 1) k_wgrad(const __grid_constant__ WgradMaps maps, const WgradArgs p) {
   using Cfg = WgradCfg<CB, BN>;
+  constexpr int SA = WG_A_STAGES, SD = WG_D_STAGES;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment by pointer arithmetic on the __shared__ array: an integer round trip loses the address space and every
   // shared-memory access below would compile to a generic LD.E / ST.E instead of LDS / STS
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* smem_a = smem;
+  uint8_t* smem_a = smem;   // ring of warpgroup g: stages [g * SA, (g + 1) * SA)
   uint8_t* smem_d = smem + Cfg::A_REGION;
-  uint8_t* aux = smem_d + WG_D_STAGES * Cfg::D_STAGE;
+  uint8_t* aux = smem_d + SD * Cfg::D_STAGE;
   uint64_t* a_full = reinterpret_cast<uint64_t*>(aux);
-  uint64_t* a_empty = a_full + WG_A_STAGES;
-  uint64_t* d_full = a_empty + WG_A_STAGES;
-  uint64_t* d_empty = d_full + WG_D_STAGES;
+  uint64_t* a_empty = a_full + 2 * SA;
+  uint64_t* d_full = a_empty + 2 * SA;
+  uint64_t* d_empty = d_full + SD;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int split = blockIdx.x;
-  const int q0 = blockIdx.y * p.qt;
-  const int q1 = min(q0 + p.qt, p.qtiles);
-  const int nq = q1 - q0;
-  const int co0 = blockIdx.z * BN;
-  const int kb0 = (int)((long long)p.kblocks * split / p.splits);
-  const int kb1 = (int)((long long)p.kblocks * (split + 1) / p.splits);
+  const int T = p.items * p.kblocks;
+  const int it_begin = (int)((long long)T * blockIdx.x / p.ctas), it_end = (int)((long long)T * (blockIdx.x + 1) / p.ctas);
 
-  if (warp == 4 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&maps.a[0]);
     tma_prefetch_desc(&maps.dy[0]);
-    for (int s = 0; s < WG_A_STAGES; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 4); }
-    for (int s = 0; s < WG_D_STAGES; ++s) { mbar_init(&d_full[s], 1); mbar_init(&d_empty[s], 4); }
+    for (int s = 0; s < 2 * SA; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 4); }
+    for (int s = 0; s < SD; ++s) { mbar_init(&d_full[s], 1); mbar_init(&d_empty[s], 8); }
     fence_barrier_init();
   }
   __syncthreads();
@@ -115,53 +129,78 @@ __global__ void __launch_bounds__(160, 1) k_wgrad(const __grid_constant__ WgradM
   pdl_launch_dependents();
   const int pad = p.pad;
 
-  if (warp == 4) {
+  if (warp == 8) {
     const uint32_t issue = elect_one() ? 1u : 0u;
-    int ia = 0, id = 0;
-    for (int kb = kb0; kb < kb1; ++kb) {
-      int t = kb;
-      const int wt = t % p.tiles_w; t /= p.tiles_w;
-      const int ht = t % p.tiles_h; t /= p.tiles_h;
-      const int dt = t % p.tiles_d;
-      const int n = t / p.tiles_d;
-      const int w0 = wt * p.tw, h0 = ht * p.th, d0 = dt * p.td;
-      for (int pass = 0; pass < p.npass; ++pass) {
-        {
-          const int s = id % WG_D_STAGES;
-          const uint32_t ph = (id / WG_D_STAGES) & 1;
-          mbar_wait(&d_empty[s], ph ^ 1);
-          mbar_expect_tx_if(issue, &d_full[s], Cfg::D_BYTES);
-          uint8_t* dst = smem_d + s * Cfg::D_STAGE;
+    int ia0 = 0, ia1 = 0, id = 0;
+    for (int it = it_begin; it < it_end;) {
+      const int item = it / p.kblocks;
+      const int kb0 = it - item * p.kblocks;
+      const int kb1 = min(p.kblocks, kb0 + (it_end - it));
+      it += kb1 - kb0;
+      const int q0 = item / p.cotiles * p.qt, co0 = item % p.cotiles * BN;
+      const int nq = min(p.qt, p.qtiles - q0), n0 = (nq + 1) >> 1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        int t = kb;
+        const int wt = t % p.tiles_w; t /= p.tiles_w;
+        const int ht = t % p.tiles_h; t /= p.tiles_h;
+        const int dt = t % p.tiles_d;
+        const int n = t / p.tiles_d;
+        const int w0 = wt * p.tw, h0 = ht * p.th, d0 = dt * p.td;
+        const int own = (kb - kb0) & 1;   // single-M-tile item: the warpgroup that takes this voxel tile
+        for (int pass = 0; pass < p.npass; ++pass) {
+          {
+            const int s = id % SD;
+            const uint32_t ph = (id / SD) & 1;
+            mbar_wait(&d_empty[s], ph ^ 1);
+            mbar_expect_tx_if(issue, &d_full[s], Cfg::D_BYTES);
+            uint8_t* dst = smem_d + s * Cfg::D_STAGE;
 #pragma unroll
-          for (int bx = 0; bx < Cfg::BPN; ++bx)
-            tma_load_5d_if(issue, dst + bx * Cfg::LBO_B, &maps.dy[pass == 2], &d_full[s], co0 + bx * Cfg::CBN, w0, h0, d0, n);
-          ++id;
-        }
-        for (int q = q0; q < q1; ++q) {
-          const int s = ia % WG_A_STAGES;
-          const uint32_t ph = (ia / WG_A_STAGES) & 1;
-          mbar_wait(&a_empty[s], ph ^ 1);
-          mbar_expect_tx_if(issue, &a_full[s], WG_A_BYTES);
-          uint8_t* dst = smem_a + s * WG_A_BYTES;
-#pragma unroll
-          for (int bx = 0; bx < Cfg::BPM; ++bx) {
-            int u = q * Cfg::BPM + bx;
-            if (u >= p.units) u = p.units - 1;  // duplicate a valid unit; its rows are never written back
-            const int tap = u / p.nci, cic = u % p.nci;
-            const int kd = tap / (p.ksz * p.ksz), kh = (tap / p.ksz) % p.ksz, kw = tap % p.ksz;
-            tma_load_5d_if(issue, dst + bx * Cfg::LBO_A, &maps.a[pass == 1], &a_full[s], cic * CB,
-                           w0 * p.stride + kw - pad, h0 * p.stride + kh - pad, d0 * p.stride + kd - pad, n);
+            for (int bx = 0; bx < Cfg::BPN; ++bx)
+              tma_load_5d_if(issue, dst + bx * Cfg::LBO_B, &maps.dy[pass == 2], &d_full[s], co0 + bx * Cfg::CBN, w0, h0, d0, n);
+            ++id;
           }
-          ++ia;
+#pragma unroll
+          for (int qi = 0; qi < Cfg::QT; ++qi) {
+#pragma unroll
+            for (int g = 0; g < 2; ++g) {
+              int q;
+              if (nq == 1) {
+                if (qi != 0 || g != own) continue;
+                q = q0;
+              } else {
+                if (qi >= (g ? nq - n0 : n0)) continue;
+                q = q0 + g * n0 + qi;
+              }
+              int& ia = g ? ia1 : ia0;
+              const int s = g * SA + ia % SA;
+              const uint32_t ph = (ia / SA) & 1;
+              mbar_wait(&a_empty[s], ph ^ 1);
+              mbar_expect_tx_if(issue, &a_full[s], WG_A_BYTES);
+              uint8_t* dst = smem_a + s * WG_A_BYTES;
+#pragma unroll
+              for (int bx = 0; bx < Cfg::BPM; ++bx) {
+                int u = q * Cfg::BPM + bx;
+                if (u >= p.units) u = p.units - 1;  // duplicate a valid unit; its rows are never written back
+                const int tap = u / p.nci, cic = u % p.nci;
+                const int kd = tap / (p.ksz * p.ksz), kh = (tap / p.ksz) % p.ksz, kw = tap % p.ksz;
+                tma_load_5d_if(issue, dst + bx * Cfg::LBO_A, &maps.a[pass == 1], &a_full[s], cic * CB,
+                               w0 * p.stride + kw - pad, h0 * p.stride + kh - pad, d0 * p.stride + kd - pad, n);
+              }
+              ++ia;
+            }
+          }
         }
       }
     }
     return;
   }
 
-  // -------------------------------------------------------------------- consumer warpgroup
+  // -------------------------------------------------------------------- consumer warpgroups
+  const int wg = warp >> 2;
   constexpr uint32_t hi_a = desc_hi(Cfg::SBO_A, Cfg::LAYOUT_A), hi_b = desc_hi(Cfg::SBO_B, Cfg::LAYOUT_B);
-  const uint32_t a0 = smem_u32(smem_a), d0s = smem_u32(smem_d);
+  const uint32_t a0 = smem_u32(smem_a) + wg * SA * WG_A_BYTES, d0s = smem_u32(smem_d);
+  uint64_t* my_full = a_full + wg * SA;
+  uint64_t* my_empty = a_empty + wg * SA;
   float acc[Cfg::QT][2][BN / 2];
 #pragma unroll
   for (int qi = 0; qi < Cfg::QT; ++qi)
@@ -169,73 +208,120 @@ __global__ void __launch_bounds__(160, 1) k_wgrad(const __grid_constant__ WgradM
     for (int i = 0; i < BN / 2; ++i) { acc[qi][0][i] = 0.f; acc[qi][1][i] = 0.f; }
   int ia = 0, id = 0;
   int prev_a = -1, prev_d = -1;   // ring slots the previous wgmma group read: handed back once that group has retired
-  for (int kb = kb0; kb < kb1; ++kb) {
-    for (int pass = 0; pass < p.npass; ++pass) {
-      const int sd = id % WG_D_STAGES;
-      mbar_wait(&d_full[sd], (id / WG_D_STAGES) & 1);
-      const uint32_t b_lo = desc_lo(d0s + sd * Cfg::D_STAGE, Cfg::LBO_B);
+  for (int it = it_begin; it < it_end;) {
+    const int item = it / p.kblocks;
+    const int kb0 = it - item * p.kblocks;
+    const int kb1 = min(p.kblocks, kb0 + (it_end - it));
+    it += kb1 - kb0;
+    const int q0 = item / p.cotiles * p.qt, co0 = item % p.cotiles * BN;
+    const int nq = min(p.qt, p.qtiles - q0), n0 = (nq + 1) >> 1;
+    const int nt = nq == 1 ? 1 : wg ? nq - n0 : n0;   // M tiles of this warpgroup
+    const int qw = nq == 1 ? q0 : q0 + wg * n0;       // its first
+    for (int kb = kb0; kb < kb1; ++kb) {
+      const bool mine = nq > 1 || ((kb - kb0) & 1) == wg;
+      for (int pass = 0; pass < p.npass; ++pass) {
+        const int sd = id % SD;
+        mbar_wait(&d_full[sd], (id / SD) & 1);
+        ++id;
+        if (!mine) {   // the other warpgroup's voxel tile: retire this one's MMAs (the slots they hold gate the producer)
+          wgmma_wait<0>();
+          if (lane == 0) {
+            if (prev_a >= 0) mbar_arrive(&my_empty[prev_a]);
+            if (prev_d >= 0) mbar_arrive(&d_empty[prev_d]);
+            mbar_arrive(&d_empty[sd]);
+          }
+          prev_a = prev_d = -1;
+          continue;
+        }
+        const uint32_t b_lo = desc_lo(d0s + sd * Cfg::D_STAGE, Cfg::LBO_B);
+#pragma unroll
+        for (int qi = 0; qi < Cfg::QT; ++qi) {
+          if (qi < nt) {
+            const int sa = ia % SA;
+            mbar_wait(&my_full[sa], (ia / SA) & 1);
+            const uint32_t a_lo = desc_lo(a0 + sa * WG_A_BYTES, Cfg::LBO_A);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+              const uint64_t db = desc_from(b_lo + ((k * 2 * Cfg::SBO_B) >> 4), hi_b);
+              Wgmma<BN>::template mma<1, 1>(acc[qi][0], desc_from(a_lo + ((k * 2 * Cfg::SBO_A) >> 4), hi_a), db, 1u);
+              Wgmma<BN>::template mma<1, 1>(acc[qi][1], desc_from(a_lo + ((k * 2 * Cfg::SBO_A + Cfg::HALF_M) >> 4), hi_a), db, 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (lane == 0) {
+              if (prev_a >= 0) mbar_arrive(&my_empty[prev_a]);
+              if (prev_d >= 0) mbar_arrive(&d_empty[prev_d]);
+            }
+            prev_a = sa;
+            prev_d = qi == nt - 1 ? sd : -1;
+            ++ia;
+          }
+        }
+      }
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int qi = 0; qi < Cfg::QT; ++qi) { wgmma_fence_regs(acc[qi][0]); wgmma_fence_regs(acc[qi][1]); }
+    if (lane == 0) {
+      if (prev_a >= 0) mbar_arrive(&my_empty[prev_a]);
+      if (prev_d >= 0) mbar_arrive(&d_empty[prev_d]);
+    }
+    prev_a = prev_d = -1;
+
+    // flush the item's partial sum straight from the fragments: element (row r, column c) of M tile q -> [tap][ci][co0 + c]
+    // at element offset off.  Deterministic mode: slot = the CTA's rank among the CTAs of the item; the item's last CTA also
+    // zeroes the slots above its own, which no CTA of this item writes.
+    int slot = 0;
+    if (p.part) slot = (int)blockIdx.x - wgrad_sk_cta((long long)item * p.kblocks, T, p.ctas);
+    const bool zero_rest = p.part && kb1 == p.kblocks && (nq > 1 || wg == 0);
+    auto frags = [&](auto&& f) {
 #pragma unroll
       for (int qi = 0; qi < Cfg::QT; ++qi) {
-        if (qi < nq) {
-          const int sa = ia % WG_A_STAGES;
-          mbar_wait(&a_full[sa], (ia / WG_A_STAGES) & 1);
-          const uint32_t a_lo = desc_lo(a0 + sa * WG_A_BYTES, Cfg::LBO_A);
-          wgmma_fence();
+        if (qi >= nt) continue;
 #pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            const uint64_t db = desc_from(b_lo + ((k * 2 * Cfg::SBO_B) >> 4), hi_b);
-            Wgmma<BN>::template mma<1, 1>(acc[qi][0], desc_from(a_lo + ((k * 2 * Cfg::SBO_A) >> 4), hi_a), db, 1u);
-            Wgmma<BN>::template mma<1, 1>(acc[qi][1], desc_from(a_lo + ((k * 2 * Cfg::SBO_A + Cfg::HALF_M) >> 4), hi_a), db, 1u);
-          }
-          wgmma_commit();
-          wgmma_wait<1>();
-          if (lane == 0) {
-            if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
-            if (prev_d >= 0) mbar_arrive(&d_empty[prev_d]);
-          }
-          prev_a = sa;
-          prev_d = qi == nq - 1 ? sd : -1;
-          ++ia;
-        }
-      }
-      ++id;
-    }
-  }
-  wgmma_wait<0>();
+        for (int hm = 0; hm < 2; ++hm) {
 #pragma unroll
-  for (int qi = 0; qi < Cfg::QT; ++qi) { wgmma_fence_regs(acc[qi][0]); wgmma_fence_regs(acc[qi][1]); }
-  if (lane == 0) {
-    if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
-    if (prev_d >= 0) mbar_arrive(&d_empty[prev_d]);
-  }
-
-  // write-back straight from the fragments: element (row r, column c) -> dw[tap][ci][co0 + c]
-  const bool has_work = kb1 > kb0;
-  float* const base = p.part ? p.part + (long long)split * p.part_stride : p.dw;
+          for (int r8 = 0; r8 < 2; ++r8) {
+            const int row = hm * 64 + (warp & 3) * 16 + (lane >> 2) + r8 * 8;
+            const int u = (qw + qi) * Cfg::BPM + row / CB;
+            const int tap = u / p.nci, cic = u % p.nci;
+            const int ci = cic * CB + row % CB;
+            if (u >= p.units || ci >= p.Ci) continue;
+            const long long off = ((long long)tap * p.Cip + ci) * p.Cop;
 #pragma unroll
-  for (int qi = 0; qi < Cfg::QT; ++qi) {
-    if (qi >= nq) continue;
-#pragma unroll
-    for (int hm = 0; hm < 2; ++hm) {
-#pragma unroll
-      for (int r8 = 0; r8 < 2; ++r8) {
-        const int row = hm * 64 + warp * 16 + (lane >> 2) + r8 * 8;
-        const int u = (q0 + qi) * Cfg::BPM + row / CB;
-        const int tap = u / p.nci, cic = u % p.nci;
-        const int ci = cic * CB + row % CB;
-        if (u >= p.units || ci >= p.Ci || !(has_work || p.part)) continue;
-        float* dst = base + ((long long)tap * p.Cip + ci) * p.Cop;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int c = co0 + j * 8 + 2 * (lane & 3);
-          if (c < p.Cop) {   // Cop is a multiple of 4 and c is even: c + 1 < Cop as well
-            const float2 v = make_float2(acc[qi][hm][4 * j + 2 * r8], acc[qi][hm][4 * j + 2 * r8 + 1]);
-            if (p.part) *reinterpret_cast<float2*>(dst + c) = has_work ? v : make_float2(0.f, 0.f);   // every split writes its slot
-            else atomicAdd(reinterpret_cast<float2*>(dst + c), v);
+            for (int j = 0; j < BN / 8; ++j) {
+              const int c = co0 + j * 8 + 2 * (lane & 3);
+              if (c < p.Cop)   // Cop is a multiple of 4 and c is even: c + 1 < Cop as well
+                f(off + c, make_float2(acc[qi][hm][4 * j + 2 * r8], acc[qi][hm][4 * j + 2 * r8 + 1]));
+            }
           }
         }
       }
+    };
+    if (!p.part) {
+      frags([&](long long off, float2 v) { atomicAdd(reinterpret_cast<float2*>(p.dw + off), v); });
+    } else {
+      float* const base = p.part + slot * p.part_stride;
+      if (nq == 1) {   // both warpgroups hold a partial sum of the one M tile: warpgroup 1's, then warpgroup 0 adds its own
+        if (wg == 1) frags([&](long long off, float2 v) { *reinterpret_cast<float2*>(base + off) = v; });
+        named_bar_sync(1, 256);
+        if (wg == 0)
+          frags([&](long long off, float2 v) {
+            const float2 o = __ldcg(reinterpret_cast<const float2*>(base + off));
+            *reinterpret_cast<float2*>(base + off) = make_float2(o.x + v.x, o.y + v.y);
+          });
+      } else {
+        frags([&](long long off, float2 v) { *reinterpret_cast<float2*>(base + off) = v; });
+      }
+      if (zero_rest)
+        for (int s = slot + 1; s < p.splits; ++s)
+          frags([&](long long off, float2) { *reinterpret_cast<float2*>(p.part + s * p.part_stride + off) = make_float2(0.f, 0.f); });
     }
+#pragma unroll
+    for (int qi = 0; qi < Cfg::QT; ++qi)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) { acc[qi][0][i] = 0.f; acc[qi][1][i] = 0.f; }
   }
 }
 
@@ -377,7 +463,7 @@ static int launch_wg(const WgradMaps& maps, const WgradArgs& a, dim3 grid, cudaS
   } else {
     using Cfg = WgradCfg<CB, BN>;
     B200_TRY((set_max_dynamic_smem<k_wgrad<CB, BN>>(Cfg::SMEM_BYTES)));
-    launch_pdl(k_wgrad<CB, BN>, grid, dim3(160), Cfg::SMEM_BYTES, st, maps, a);
+    launch_pdl(k_wgrad<CB, BN>, grid, dim3(288), Cfg::SMEM_BYTES, st, maps, a);
   }
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;
@@ -396,8 +482,10 @@ static bool wgrad_halo_eligible(const WgradOp& op) {
          A.W == Y.W;
 }
 
-// The tiling fields of r for halo tiles or per-tap tiles: voxel tile, CB / BN, M tiles and their CTA groups, N tiles, voxel
-// tiles, the split-K factor and the partial-buffer bytes of deterministic mode.
+// The tiling fields of r for halo tiles or per-tap tiles: voxel tile, CB / BN, M tiles and their CTA groups (work items), N
+// tiles, voxel tiles, the CTAs, the split-K factor and the partial-buffer bytes of deterministic mode.  Halo tiles: a grid of
+// splits x groups x cotiles CTAs, each on one item and kblocks / splits voxel tiles.  Per-tap tiles: stream-K (k_wgrad) over
+// min(num_sms, T) CTAs, T = items x kblocks; splits = the most CTAs that share one item, the partial slots it needs.
 static void wgrad_tiling(const WgradOp& op, int num_sms, bool halo, WgradRoute* r) {
   const Act& A = op.a;
   const Act& Y = op.dy;
@@ -412,15 +500,26 @@ static void wgrad_tiling(const WgradOp& op, int num_sms, bool halo, WgradRoute* 
   r->nci = ceil_div(A.C, r->CB);
   r->units = ntaps * r->nci;
   r->qtiles = ceil_div(r->units, 128 / r->CB);
-  r->QT = (halo ? 2 : 1) * (128 / r->BN);   // WgradCfg::QT per consumer warpgroup: one on per-tap tiles, two in halo mode
+  r->QT = 2 * (128 / r->BN);   // two consumer warpgroups of WgradCfg::QT M tiles each
   if (r->QT > r->qtiles) r->QT = r->qtiles;
   r->groups = ceil_div(r->qtiles, r->QT);
   r->QT = ceil_div(r->qtiles, r->groups);   // rebalance M tiles across groups
   r->cotiles = ceil_div(Y.C, r->BN);
   r->kblocks = Y.N * ceil_div(Y.D, r->td) * ceil_div(Y.H, r->th) * ceil_div(Y.W, r->tw);
-  r->splits = num_sms / (r->groups * r->cotiles);
-  if (r->splits < 1) r->splits = 1;
-  if (r->splits > r->kblocks) r->splits = r->kblocks;
+  if (halo) {
+    r->splits = num_sms / (r->groups * r->cotiles);
+    if (r->splits < 1) r->splits = 1;
+    if (r->splits > r->kblocks) r->splits = r->kblocks;
+    r->ctas = r->splits * r->groups * r->cotiles;
+  } else {
+    const int items = r->groups * r->cotiles;
+    const long long T = (long long)items * r->kblocks;   // < 2^31: k_wgrad counts iterations in int
+    r->ctas = (int)std::min<long long>(num_sms, T);
+    r->splits = 1;
+    for (int i = 0; i < items; ++i)
+      r->splits = std::max(r->splits, wgrad_sk_cta((long long)(i + 1) * r->kblocks - 1, T, r->ctas) -
+                                          wgrad_sk_cta((long long)i * r->kblocks, T, r->ctas) + 1);
+  }
   r->part_bytes = (size_t)r->splits * ntaps * op.Cip * op.Cop * sizeof(float);
 }
 
@@ -506,6 +605,7 @@ int wgrad_route(const WgradOp& op, int num_sms, WgradRoute* r) {
   const bool halo = wgrad_halo_eligible(op);
   r->kind = halo ? WGRAD_KIND_HALO : WGRAD_KIND_TAP;
   wgrad_tiling(op, num_sms, halo, r);
+  B200_REQUIRE((long long)r->groups * r->cotiles * r->kblocks <= INT_MAX, E_UNSUPPORTED, "wgrad: too many voxel tiles");
   r->npass = split ? 3 : 1;
   return with_wgrad_kernel(*r, [](auto) { return (int)OK; });
 }
@@ -536,6 +636,9 @@ int launch_wgrad(const WgradOp& op, cudaStream_t st) {
   a.qt = r.QT;
   a.kblocks = r.kblocks;
   a.splits = r.splits;
+  a.cotiles = r.cotiles;
+  a.items = r.groups * r.cotiles;
+  a.ctas = r.ctas;
   a.npass = r.npass;
   a.dw = op.dw;
   if (op.part) {
@@ -558,7 +661,7 @@ int launch_wgrad(const WgradOp& op, cudaStream_t st) {
     B200_TRY(make_act_map(&maps.dy[1], Y.lo, Y.N, Y.D, Y.H, Y.W, Y.C, Y.ld, CBN, a.tw, a.th, a.td, 1,
                           swz_for_bytes(CBN * 2), Y.vD, Y.vH, Y.vW));
   }
-  const dim3 grid((unsigned)r.splits, (unsigned)r.groups, (unsigned)r.cotiles);
+  const dim3 grid = halo ? dim3((unsigned)r.splits, (unsigned)r.groups, (unsigned)r.cotiles) : dim3((unsigned)r.ctas);
   return with_wgrad_kernel(r, [&](auto k) {
     return launch_wg<decltype(k)::CB, decltype(k)::BN, decltype(k)::HALO>(maps, a, grid, st);
   });

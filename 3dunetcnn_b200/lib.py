@@ -50,7 +50,8 @@ class ConvRoute(C.Structure):
 class WgradRoute(C.Structure):
     _fields_ = [("kind", C.c_int32), ("ci8", C.c_int32), ("cb", C.c_int32), ("bn", C.c_int32), ("qt", C.c_int32),
                 ("groups", C.c_int32), ("cotiles", C.c_int32), ("kblocks", C.c_int32), ("splits", C.c_int32), ("npass", C.c_int32),
-                ("tw", C.c_int32), ("th", C.c_int32), ("td", C.c_int32), ("part_bytes", C.c_int64)]
+                ("tw", C.c_int32), ("th", C.c_int32), ("td", C.c_int32), ("part_bytes", C.c_int64),
+                ("ctas", C.c_int32)]
 
 
 CONV_KINDS = ("tap", "halo", "class1", "class2", "pair")     # b200unet_conv_route.kind

@@ -56,10 +56,13 @@ typedef struct b200unet_conv_route {
 typedef struct b200unet_wgrad_route {
   int32_t kind;
   int32_t ci8;                    /* SIMT: input channels / 8 */
-  int32_t cb, bn, qt;             /* input channels per M box, output channels per N tile, M tiles per CTA */
-  int32_t groups, cotiles, kblocks, splits, npass;
+  int32_t cb, bn, qt;             /* input channels per M box, output channels per N tile, M tiles per CTA (per work item) */
+  int32_t groups, cotiles, kblocks; /* M-tile groups (groups x cotiles work items), N tiles, voxel tiles */
+  int32_t splits;                 /* halo: CTAs per work item; per-tap: the most CTAs sharing one work item (partial slots) */
+  int32_t npass;
   int32_t tw, th, td;
   int64_t part_bytes;             /* deterministic mode: splits * taps * cip * cop * 4, the partial-sum buffer it fills */
+  int32_t ctas;                   /* tensor-core kinds: CTAs of the launch (per-tap: min(SMs, work items x voxel tiles)) */
 } b200unet_wgrad_route;
 
 /* the route b200unet_conv3d / b200unet_diag_conv3d_ex take for this descriptor on the current device (132 SMs without one); an
@@ -74,8 +77,8 @@ size_t b200unet_diag_wgrad_partial_bytes(const b200unet_tensor* a, const b200une
 
 int b200unet_diag_conv3d_ex(const b200unet_conv_desc* desc, const b200unet_diag_ext* ext, void* stream);
 /* dw fp32 [T][cip][cop].  part == NULL: dw += the gradient (atomics).  Otherwise the deterministic mode of the plans: the
- * split-K CTAs store partial sums into part (part_bytes long), *splits is set to their number, and a second kernel writes
- * dw = their sum in a fixed order. */
+ * split-K CTAs store partial sums into slots of part (part_bytes long), *splits is set to the number of slots, and a second
+ * kernel writes dw = their sum in a fixed order. */
 int b200unet_diag_wgrad_ex(const b200unet_tensor* a, const b200unet_tensor* dy, int ksz, int stride, int cip, int cop,
                            const b200unet_diag_ext* ext, float* part, size_t part_bytes, int* splits, float* dw, void* stream);
 /* dbias[c] = sum of dy over the visible voxels (overwritten), in a fixed order: per-block partial sums into scratch
