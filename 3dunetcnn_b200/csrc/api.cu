@@ -293,6 +293,22 @@ int b200unet_cc_sort_by_size(int32_t* labels, int nvol, int d, int h, int w, int
   return launch_cc_sort_by_size(labels, nvol, d, h, w, max_count, scratch, to_stream(stream));
 }
 
+static SurfaceMask to_surface_mask(const b200unet_surface_mask* m) {
+  SurfaceMask s;
+  s.data = m->data;
+  s.dtype = m->dtype;
+  for (int i = 0; i < 5; ++i) s.stride[i] = m->stride[i];
+  return s;
+}
+size_t b200unet_surface_scratch_bytes(int b, int c, int d, int h, int w) { return surface_scratch_bytes(b, c, d, h, w); }
+int b200unet_surface_distance(const b200unet_surface_mask* pred, const b200unet_surface_mask* gt, int b, int c, int d, int h, int w,
+                              const double* spacing, float q, int hd_dirs, int asd_dirs, const float* tau, float* hd, float* asd,
+                              float* nsd, void* scratch, void* stream) {
+  NOT_NULL(pred); NOT_NULL(gt); NOT_NULL(spacing); NOT_NULL(scratch);
+  return launch_surface_distance(to_surface_mask(pred), to_surface_mask(gt), b, c, d, h, w, spacing, q, hd_dirs, asd_dirs, tau, hd, asd,
+                                 nsd, scratch, to_stream(stream));
+}
+
 // ---- diagnostics (include/b200unet_diag.h)
 int b200unet_diag_conv3d_route(const b200unet_conv_desc* desc, const b200unet_diag_ext* ext, b200unet_conv_route* route) {
   NOT_NULL(desc); NOT_NULL(route);

@@ -152,6 +152,23 @@ int launch_cc_label(const uint8_t* mask, int nvol, int d, int h, int w, int conn
                     void* scratch, cudaStream_t st);
 int launch_cc_sort_by_size(int32_t* labels, int nvol, int d, int h, int w, int max_count, void* scratch, cudaStream_t st);
 
+// ---- boundary-distance scores of binary segmentations (surface.cu)
+#define B200_SURFACE_MAX_EXTENT 256   // per axis: site indices of the distance transform are uint8, offsets int16
+#define B200_SURFACE_MAX_PAIRS 4096   // (item, class) pairs per call
+// element (b, c, d, h, w) at data + b stride[0] + c stride[1] + d stride[2] + h stride[3] + w stride[4] (elements); foreground is
+// value == 1; dtype 0 = bool / uint8, 1 = fp32.  Field order of b200unet_surface_mask.
+struct SurfaceMask {
+  const void* data;
+  int dtype;
+  long long stride[5];
+};
+size_t surface_scratch_bytes(int nb, int nc, int d, int h, int w);   // 0: the shape is rejected
+// spacing DEVICE fp64 [nb][3]; q = 0: Hausdorff is the max, else the fp32 quantile q in (0, 1]; hd_dirs / asd_dirs 1 = pred -> gt,
+// 2 = both; tau DEVICE fp32 [nc] (surface Dice thresholds); hd, asd, nsd DEVICE fp32 [nb][nc] or nullptr
+int launch_surface_distance(const SurfaceMask& pred, const SurfaceMask& gt, int nb, int nc, int d, int h, int w, const double* spacing,
+                            float q, int hd_dirs, int asd_dirs, const float* tau, float* hd, float* asd, float* nsd, void* scratch,
+                            cudaStream_t st);
+
 // ---- tensor-core implicit-GEMM convolution (igemm_conv.cu)
 struct ConvSrc {
   Act x;               // A operand (NDHWC bf16, hi[/lo])

@@ -75,6 +75,10 @@ class NetDesc(C.Structure):
                 ("deterministic", C.c_int32), ("inference_only", C.c_int32), ("input_grad", C.c_int32)]
 
 
+class SurfaceMask(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("dtype", C.c_int32), ("stride", C.c_int64 * 5)]
+
+
 def build_library(force: bool = False, verbose: bool = False) -> str:
     """Compile libb200unet.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
     if os.environ.get("B200UNET_LIB"):
@@ -160,6 +164,9 @@ _SIGS = {
     "b200unet_cc_label": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_void_p]),
     "b200unet_cc_sort_by_size": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "b200unet_surface_scratch_bytes": (C.c_size_t, [C.c_int] * 5),
+    "b200unet_surface_distance": (C.c_int, [C.POINTER(SurfaceMask), C.POINTER(SurfaceMask)] + [C.c_int] * 5 + [C.c_void_p, C.c_float,
+                                            C.c_int, C.c_int] + [C.c_void_p] * 6),
     "b200unet_plan_create": (C.c_int, [C.POINTER(NetDesc), C.POINTER(C.c_void_p)]),
     "b200unet_plan_destroy": (None, [C.c_void_p]),
     "b200unet_plan_num_params": (C.c_int, [C.c_void_p]),
@@ -619,3 +626,30 @@ def dice_ce_bwd(desc: DiceCEDesc, logits, target, scratch, grad_out, dlogits) ->
     n, c, s = _nc_s(logits)
     check(load_library().b200unet_dice_ce_bwd(C.byref(desc), logits.data_ptr(), target.data_ptr(), n, c, s, scratch.data_ptr(),
                                               grad_out.data_ptr(), dlogits.data_ptr(), stream_ptr()), "dice_ce_bwd")
+
+
+def surface_scratch_bytes(b: int, c: int, d: int, h: int, w: int) -> int:
+    lib = load_library()
+    n = int(lib.b200unet_surface_scratch_bytes(b, c, d, h, w))
+    if n == 0:
+        msg = lib.b200unet_last_error()
+        raise RuntimeError("libb200unet surface_scratch_bytes rejected %d x %d x %d x %d x %d: %s" % (b, c, d, h, w,
+                                                                                                   msg.decode() if msg else "?"))
+    return n
+
+
+_SURFACE_DTYPES = {torch.bool: 0, torch.uint8: 0, torch.float32: 1}
+
+
+def surface_mask(t: torch.Tensor) -> SurfaceMask:
+    """[b, c, d, h, w] bool / uint8 / fp32 view, any strides"""
+    return SurfaceMask(t.data_ptr(), _SURFACE_DTYPES[t.dtype], (C.c_int64 * 5)(*t.stride()))
+
+
+def surface_distance(pred, gt, spacing, q: float, hd_dirs: int, asd_dirs: int, tau, hd, asd, nsd, scratch) -> None:
+    """pred, gt [b, c, d, h, w]; spacing fp64 [b, 3]; tau fp32 [c] or None; hd / asd / nsd fp32 [b, c] or None (not computed)"""
+    b, c, d, h, w = pred.shape
+    pm, gm = surface_mask(pred), surface_mask(gt)
+    check(load_library().b200unet_surface_distance(C.byref(pm), C.byref(gm), b, c, d, h, w, spacing.data_ptr(), q, hd_dirs, asd_dirs,
+                                                   _p(tau), _p(hd), _p(asd), _p(nsd), scratch.data_ptr(), stream_ptr()),
+          "surface_distance")

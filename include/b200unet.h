@@ -256,6 +256,30 @@ int b200unet_cc_label(const uint8_t* mask, int nvol, int d, int h, int w, int co
                       void* scratch, void* stream);
 int b200unet_cc_sort_by_size(int32_t* labels, int nvol, int d, int h, int w, int max_count, void* scratch, void* stream);
 
+/* ---- boundary-distance scores of binary segmentations (the scoring after the path: MONAI HausdorffDistanceMetric,
+ * SurfaceDistanceMetric, SurfaceDiceMetric on one-hot [b][c][d][h][w] masks, without scipy on the host).  A voxel is foreground
+ * iff its value is 1; edges = fg & ~erode(fg) with the 6-neighbour cross, outside the volume = background.  For each of the
+ * b x c (item, class) pairs the distances from every edge voxel of one mask to the nearest edge voxel of the other come from an
+ * exact Euclidean distance transform, sqrt(((dd s_d)^2 + (dh s_h)^2) + (dw s_w)^2) in fp64 rounded to fp32 as
+ * scipy.ndimage.distance_transform_edt computes it (bit for bit with unit spacing).  Extents 1..256 per axis, b x c <= 4096,
+ * else B200UNET_E_UNSUPPORTED.
+ *   surface_scratch_bytes: from the shape alone (0 = rejected).
+ *   surface_distance: spacing DEVICE fp64 [b][3] (d, h, w); q = 0: Hausdorff is the max distance, q in (0, 1]: torch.quantile(d, q)
+ *                  on the fp32 distances; hd_dirs / asd_dirs: 1 = pred -> gt only, 2 = both directions (HD: max of the two
+ *                  statistics; ASD: mean over both distance sets together, in fp64); nsd: (#{d_pg <= tau} + #{d_gp <= tau}) /
+ *                  (n_pg + n_gp) with tau DEVICE fp32 [c].  hd, asd, nsd: DEVICE fp32 [b][c], any of them NULL = not computed.
+ *                  Both masks empty: NaN; exactly one empty: HD = ASD = inf, NSD = 0.  Launches do not depend on b x c, nothing is
+ *                  read back to the host, no floating-point atomics: bit-identical run to run. */
+typedef struct b200unet_surface_mask {
+  const void* data;
+  int32_t dtype;        /* 0 bool / uint8, 1 fp32 */
+  int64_t stride[5];    /* elements, for (b, c, d, h, w) */
+} b200unet_surface_mask;
+size_t b200unet_surface_scratch_bytes(int b, int c, int d, int h, int w);
+int b200unet_surface_distance(const b200unet_surface_mask* pred, const b200unet_surface_mask* gt, int b, int c, int d, int h, int w,
+                              const double* spacing, float q, int hd_dirs, int asd_dirs, const float* tau, float* hd, float* asd,
+                              float* nsd, void* scratch, void* stream);
+
 /* ---- whole-network plan: UNet3D forward/backward (segmentation/unet.py:7-50, classification/myronenko.py,
  * classification/decoder.py:73-130, autoencoder/variational.py:37-87) as one schedule of the kernels above. */
 typedef struct b200unet_net_desc {
