@@ -85,7 +85,7 @@ using namespace b200;
 
 extern "C" {
 
-int b200unet_version(void) { return 105; }
+int b200unet_version(void) { return 106; }
 const char* b200unet_last_error(void) { return get_error(); }
 
 int b200unet_ncdhw_to_ndhwc(const float* x, int c_real, const b200unet_tensor* out, void* stream) {
@@ -184,25 +184,22 @@ int b200unet_head_bwd(const b200unet_tensor* x, const float* w, int n_out, const
   return launch_head_bwd(to_act(x), w, n_out, dlogits, to_act(dx), dw, to_stream(stream), scratch);
 }
 
-int b200unet_dice_fwd(const float* logits, const void* target, int n, int c, int64_t spatial, int flags,
-                      float smooth_nr, float smooth_dr, double* sums, float* loss, void* stream) {
-  NOT_NULL(logits); NOT_NULL(target); NOT_NULL(sums); NOT_NULL(loss);
-  return launch_dice_fwd(logits, reinterpret_cast<const uint8_t*>(target), n, c, spatial, flags, smooth_nr, smooth_dr, sums, loss, to_stream(stream));
-}
-int b200unet_dice_bwd(const float* logits, const void* target, int n, int c, int64_t spatial, int flags,
-                      float smooth_nr, float smooth_dr, const double* sums, const float* grad_out, float* dlogits,
-                      void* stream) {
-  NOT_NULL(logits); NOT_NULL(target); NOT_NULL(sums); NOT_NULL(grad_out); NOT_NULL(dlogits);
-  return launch_dice_bwd(logits, reinterpret_cast<const uint8_t*>(target), n, c, spatial, flags, smooth_nr, smooth_dr, sums, grad_out, dlogits,
-                         to_stream(stream));
-}
-
 static DiceCEDesc to_dice_ce(const b200unet_dice_ce_desc* d) {
   DiceCEDesc r;
   r.act = d->act; r.target_kind = d->target_kind; r.include_background = d->include_background; r.squared_pred = d->squared_pred;
   r.jaccard = d->jaccard; r.batch = d->batch; r.reduction = d->reduction;
   r.smooth_nr = d->smooth_nr; r.smooth_dr = d->smooth_dr; r.lambda_dice = d->lambda_dice; r.lambda_ce = d->lambda_ce;
   return r;
+}
+int b200unet_dice_fwd(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c, int64_t spatial,
+                      double* scratch, float* loss, void* stream) {
+  NOT_NULL(desc); NOT_NULL(logits); NOT_NULL(target); NOT_NULL(scratch); NOT_NULL(loss);
+  return launch_dice_fwd(to_dice_ce(desc), logits, target, n, c, spatial, scratch, loss, to_stream(stream));
+}
+int b200unet_dice_bwd(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c, int64_t spatial,
+                      const double* scratch, const float* grad_out, float* dlogits, void* stream) {
+  NOT_NULL(desc); NOT_NULL(logits); NOT_NULL(target); NOT_NULL(scratch); NOT_NULL(grad_out); NOT_NULL(dlogits);
+  return launch_dice_bwd(to_dice_ce(desc), logits, target, n, c, spatial, scratch, grad_out, dlogits, to_stream(stream));
 }
 size_t b200unet_dice_ce_scratch_bytes(const b200unet_dice_ce_desc* desc, int n, int c, int64_t spatial) {
   if (!desc) { set_error("%s: null argument desc", __func__); return 0; }

@@ -1,9 +1,10 @@
 // Fused Dice + cross-entropy criterion (monai.losses.DiceCELoss), forward and backward, on label-map or C-channel targets.
 //
 //   loss = lambda_dice * Dice(act(x), t) + lambda_ce * CE(x, t)
-//   Dice: the DiceLoss formula of dice.cu on p = act(x), act = softmax over channels, sigmoid or identity; per (n,c)
+//   Dice: the DiceLoss formula on p = act(x), act = softmax over channels, sigmoid or identity; per (n,c)
 //         I = sum p*t, P = sum p (or p^2), T = sum t (or t^2), f = 1 - (2I + nr) / (P + T + dr)   [jaccard: 2(P + T - I)]
-//         include_background = 0 drops channel 0 after the activation; batch pools the sums over n; mean or sum of f
+//         include_background = 0 drops channel 0 after the activation; batch pools the sums over n; mean or sum of f.
+//         The loss and the backward coefficients are formed by dice.cu's finalize, which DiceLoss shares.
 //   CE:   on the raw logits.  C > 1: -sum_c t_c log_softmax(x)_c (a label map is its one-hot row); C == 1: BCEWithLogits(x, t).
 //         mean divides by N*S, sum sums.  lambda_ce = 0: no CE work at all, so logits of +-inf leave a sigmoid Dice finite
 //         (0 * the NaN of inf - inf would not be).
@@ -14,7 +15,7 @@
 // when the CE term or a softmax needs them.
 //   forward:  thread v of the tile: max, sum of exponentials, CE term; then thread (c, slice) accumulates channel c's (I, P, T)
 //             over a slice of the tile's voxels in registers across the block's tiles.  Each block writes its partial sums to its
-//             own slot; k_dice_ce_reduce adds the slots in a fixed order in fp64 and k_dice_ce_finalize forms the loss and the
+//             own slot; k_dice_ce_reduce adds the slots in a fixed order in fp64 and launch_dice_finalize forms the loss and the
 //             backward coefficients.  No floating-point atomics: loss and dlogits are bit-identical run to run.
 //   backward: thread v of the tile: g_c = a_nc t_c + b_nc dP/dp_c from the coefficients, the activation Jacobian
 //             (softmax: p_c (g_c - sum_k p_k g_k)) and the CE gradient cg (q_c sum_k t_k - t_c); dlogits written coalesced.
@@ -32,9 +33,6 @@ constexpr int kP = kV + 1;          // row pitch (floats) of the staged [C][kV] 
 constexpr int kSMs = 132;           // H100 SXM; with the shared-memory size it fixes the forward grid, hence the slot count
 constexpr int kSmemPerSM = 228 * 1024;   // shared memory per SM; every resident block also takes kSmemReserved of it
 constexpr int kSmemReserved = 1024;
-
-enum TargetKind { T_LABEL_U8 = 0, T_LABEL_I64 = 1, T_ONEHOT_U8 = 2, T_SOFT_F32 = 3 };
-enum ActKind { A_NONE = 0, A_SIGMOID = 1, A_SOFTMAX = 2 };
 
 __device__ __forceinline__ void cp_async4(float* dst, const float* src, bool valid) {
   const unsigned d = static_cast<unsigned>(__cvta_generic_to_shared(dst));
@@ -224,53 +222,6 @@ __global__ void k_dice_ce_reduce(const double* __restrict__ part, const double* 
   }
 }
 
-__device__ __forceinline__ void pooled(const double* sums, int N, int C, int n, int c, int batch, double& I, double& P, double& T) {
-  if (batch) {
-    I = P = T = 0;
-    for (int m = 0; m < N; ++m) { I += sums[(m * C + c) * 3]; P += sums[(m * C + c) * 3 + 1]; T += sums[(m * C + c) * 3 + 2]; }
-  } else {
-    I = sums[(n * C + c) * 3]; P = sums[(n * C + c) * 3 + 1]; T = sums[(n * C + c) * 3 + 2];
-  }
-}
-
-// coef [N][C][2] = lambda_dice * w * (dF/dI, dF/dP) (dice.cu: k_dice_bwd), zero on a dropped background channel; the scalar loss
-__global__ void k_dice_ce_finalize(const double* __restrict__ sums, const double* __restrict__ ce, int N, int C, long long S, DiceCEDesc d,
-                                   double* __restrict__ coef, float* __restrict__ loss) {
-  const int c_lo = (!d.include_background && C > 1) ? 1 : 0;
-  const int terms = (d.batch ? 1 : N) * (C - c_lo);
-  const double w = d.lambda_dice * (d.reduction == 0 ? 1.0 / terms : 1.0);
-  for (int i = threadIdx.x; i < N * C; i += blockDim.x) {
-    const int n = i / C, c = i % C;
-    double I, P, T;
-    pooled(sums, N, C, n, c, d.batch, I, P, T);
-    double den = P + T;
-    if (d.jaccard) den = 2.0 * (den - I);
-    const double D = den + d.smooth_dr, num = 2.0 * I + d.smooth_nr;
-    double dFdI = -2.0 / D, dFdP = num / (D * D);
-    if (d.jaccard) { dFdI = -2.0 / D - 2.0 * num / (D * D); dFdP = 2.0 * num / (D * D); }
-    const double wc = c < c_lo ? 0.0 : w;
-    coef[i * 2] = wc * dFdI;
-    coef[i * 2 + 1] = wc * dFdP;
-  }
-  if (threadIdx.x != 0) return;
-  double acc = 0;
-  for (int n = 0; n < (d.batch ? 1 : N); ++n)
-    for (int c = c_lo; c < C; ++c) {
-      double I, P, T;
-      pooled(sums, N, C, n, c, d.batch, I, P, T);
-      double den = P + T;
-      if (d.jaccard) den = 2.0 * (den - I);
-      acc += 1.0 - (2.0 * I + d.smooth_nr) / (den + d.smooth_dr);
-    }
-  double l = d.lambda_dice * (d.reduction == 0 ? acc / terms : acc);
-  if (d.lambda_ce != 0.f) {
-    double cet = 0;
-    for (int n = 0; n < N; ++n) cet += ce[n];
-    l += d.lambda_ce * (d.reduction == 0 ? cet / ((double)N * S) : cet);
-  }
-  *loss = (float)l;
-}
-
 // grid (grid_x, N); one voxel per thread
 template <int TK, int ACT>
 __global__ void __launch_bounds__(kThreads) k_dice_ce_bwd(const float* __restrict__ x, const void* __restrict__ tgt, int C, long long S,
@@ -352,12 +303,8 @@ struct Shape {
 };
 
 int check_shape(const DiceCEDesc& d, int N, int C, long long S, Shape* sh) {
-  B200_REQUIRE(N > 0 && C > 0 && S > 0, E_INVALID, "dice_ce: empty input (n=%d c=%d spatial=%lld)", N, C, S);
+  B200_TRY(check_dice_desc(d, N, C, S, "dice_ce"));
   B200_REQUIRE(C <= 128, E_UNSUPPORTED, "dice_ce: %d channels (at most 128)", C);
-  B200_REQUIRE(d.act >= 0 && d.act <= 2, E_INVALID, "dice_ce: act=%d (0 none, 1 sigmoid, 2 softmax)", d.act);
-  B200_REQUIRE(d.target_kind >= 0 && d.target_kind <= 3, E_INVALID, "dice_ce: target_kind=%d", d.target_kind);
-  B200_REQUIRE(d.reduction == 0 || d.reduction == 1, E_INVALID, "dice_ce: reduction=%d (0 mean, 1 sum)", d.reduction);
-  B200_REQUIRE(d.lambda_dice >= 0.f && d.lambda_ce >= 0.f, E_INVALID, "dice_ce: negative lambda");
   sh->N = N; sh->C = C; sh->S = S; sh->kind = d.target_kind; sh->act = d.act;
   if (C == 1) {
     // one channel: softmax and the label-map expansion do not apply (MONAI ignores them); a uint8 map is the uint8 target itself
@@ -421,9 +368,7 @@ int launch_dice_ce_fwd(const DiceCEDesc& d, const float* logits, const void* tar
   const int warps = N * C + N;
   k_dice_ce_reduce<<<(warps + 7) / 8, 256, 0, st>>>(s.part, s.ce_part, N, C, sh.slots, s.sums, s.ce);
   B200_CHECK_CUDA(cudaGetLastError());
-  k_dice_ce_finalize<<<1, 128, 0, st>>>(s.sums, s.ce, N, C, S, d, s.coef, loss);
-  B200_CHECK_CUDA(cudaGetLastError());
-  return OK;
+  return launch_dice_finalize(d, s.sums, s.ce, N, C, S, s.coef, loss, st);
 }
 
 int launch_dice_ce_bwd(const DiceCEDesc& d, const float* logits, const void* target, int N, int C, long long S, const void* scratch,

@@ -68,23 +68,31 @@ int launch_act_to_ncdhw(const Act& in, int C, float* y, cudaStream_t st);
 int launch_input_grad(const Act* dz, const Act* x, const float* coef, const float* coef2, int coef_ld, const Act& r, int C, float* dx,
                       cudaStream_t st);
 
-// ---- Dice criterion (dice.cu)
-// flags: bit0 sigmoid, bit1 squared_pred, bit2 jaccard, bit3 batch, bit4 exclude background, bit5 reduction=sum,
-// bit6 target is fp32 (soft labels) instead of uint8
-int launch_dice_fwd(const float* logits, const uint8_t* target, int N, int C, long long S, int flags,
-                    float smooth_nr, float smooth_dr, double* sums, float* loss, cudaStream_t st);
-int launch_dice_bwd(const float* logits, const uint8_t* target, int N, int C, long long S, int flags,
-                    float smooth_nr, float smooth_dr, const double* sums, const float* grad_out, float* dlogits,
-                    cudaStream_t st);
-
-// ---- Dice + cross-entropy criterion (dice_ce.cu); the fields mirror b200unet_dice_ce_desc
+// ---- Dice criteria: the options of both; the fields mirror b200unet_dice_ce_desc
+enum TargetKind { T_LABEL_U8 = 0, T_LABEL_I64 = 1, T_ONEHOT_U8 = 2, T_SOFT_F32 = 3 };
+enum ActKind { A_NONE = 0, A_SIGMOID = 1, A_SOFTMAX = 2 };
 struct DiceCEDesc {
-  int act;               // 0 identity, 1 sigmoid, 2 softmax over channels
-  int target_kind;       // 0 uint8 label map [N][1][S], 1 int64 label map, 2 uint8 [N][C][S], 3 fp32 [N][C][S]
+  int act;               // ActKind: 0 identity, 1 sigmoid, 2 softmax over channels
+  int target_kind;       // TargetKind: 0 uint8 label map [N][1][S], 1 int64 label map, 2 uint8 [N][C][S], 3 fp32 [N][C][S]
   int include_background, squared_pred, jaccard, batch;
   int reduction;         // 0 mean, 1 sum
   float smooth_nr, smooth_dr, lambda_dice, lambda_ce;
 };
+// the checks both criteria make: a non-empty shape and in-range options ("who" prefixes the error message)
+int check_dice_desc(const DiceCEDesc& d, int N, int C, long long S, const char* who);
+// The loss and coef [N][C][2] (the backward's dF/dI, dF/dP per (n, c)) from sums [N][C][3] (I, P, T) in one single-block
+// launch; ce [N] (the summed CE terms of each sample) is read only when lambda_ce != 0 (dice.cu)
+int launch_dice_finalize(const DiceCEDesc& d, const double* sums, const double* ce, int N, int C, long long S, double* coef,
+                         float* loss, cudaStream_t st);
+
+// ---- DiceLoss (dice.cu): sigmoid or identity, uint8 or fp32 [N][C][S] target, lambda_ce == 0.  scratch: sums [N][C][3]
+// then coef [N][C][2], fp64
+int launch_dice_fwd(const DiceCEDesc& d, const float* logits, const void* target, int N, int C, long long S, double* scratch,
+                    float* loss, cudaStream_t st);
+int launch_dice_bwd(const DiceCEDesc& d, const float* logits, const void* target, int N, int C, long long S, const double* scratch,
+                    const float* grad_out, float* dlogits, cudaStream_t st);
+
+// ---- Dice + cross-entropy criterion (dice_ce.cu)
 size_t dice_ce_scratch_bytes(const DiceCEDesc& d, int N, int C, long long S);   // 0: the shape or options are rejected
 int launch_dice_ce_fwd(const DiceCEDesc& d, const float* logits, const void* target, int N, int C, long long S, void* scratch,
                        float* loss, cudaStream_t st);

@@ -59,7 +59,7 @@ WGRAD_KINDS = ("simt", "tap", "halo")               # b200unet_wgrad_route.kind
 
 
 class DiceCEDesc(C.Structure):
-    """``b200unet_dice_ce_desc``: options of the Dice + cross-entropy criterion."""
+    """``b200unet_dice_ce_desc``: options of both Dice criteria (DiceLoss and DiceCELoss)."""
     _fields_ = [("act", C.c_int32), ("target_kind", C.c_int32), ("include_background", C.c_int32), ("squared_pred", C.c_int32),
                 ("jaccard", C.c_int32), ("batch", C.c_int32), ("reduction", C.c_int32), ("smooth_nr", C.c_float),
                 ("smooth_dr", C.c_float), ("lambda_dice", C.c_float), ("lambda_ce", C.c_float)]
@@ -126,10 +126,10 @@ _SIGS = {
     "b200unet_head_bwd_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "b200unet_head_bwd": (C.c_int, [C.POINTER(Tensor5), C.c_void_p, C.c_int, C.c_void_p, C.POINTER(Tensor5),
                                     C.c_void_p, C.c_void_p, C.c_void_p]),
-    "b200unet_dice_fwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_float,
-                                    C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "b200unet_dice_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_float,
-                                    C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200unet_dice_fwd": (C.c_int, [C.POINTER(DiceCEDesc), C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p,
+                                    C.c_void_p, C.c_void_p]),
+    "b200unet_dice_bwd": (C.c_int, [C.POINTER(DiceCEDesc), C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200unet_dice_ce_scratch_bytes": (C.c_size_t, [C.POINTER(DiceCEDesc), C.c_int, C.c_int, C.c_int64]),
     "b200unet_dice_ce_fwd": (C.c_int, [C.POINTER(DiceCEDesc), C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p,
                                        C.c_void_p, C.c_void_p]),
@@ -533,29 +533,6 @@ def head_bwd(x: Act, w, n_out, dlogits, dx: Act, dw) -> None:
                                 dw.data_ptr(), scratch.data_ptr(), stream_ptr()), "head_bwd")
 
 
-def dice_flags(sigmoid=True, squared_pred=False, jaccard=False, batch=False, include_background=True,
-               reduction="mean", float_target=False) -> int:
-    if reduction not in ("mean", "sum"):
-        raise ValueError("fused Dice supports reduction 'mean' or 'sum', got %r" % (reduction,))
-    return (int(bool(sigmoid)) | (int(bool(squared_pred)) << 1) | (int(bool(jaccard)) << 2) | (int(bool(batch)) << 3)
-            | (int(not include_background) << 4) | (int(reduction == "sum") << 5) | (int(bool(float_target)) << 6))
-
-
-def dice_fwd(logits, target, flags, nr, dr, sums, loss) -> None:
-    n, c = logits.shape[:2]
-    s = logits[0, 0].numel()
-    check(load_library().b200unet_dice_fwd(logits.data_ptr(), target.data_ptr(), n, c, s, flags, nr, dr,
-                                           sums.data_ptr(), loss.data_ptr(), stream_ptr()), "dice_fwd")
-
-
-def dice_bwd(logits, target, flags, nr, dr, sums, grad_out, dlogits) -> None:
-    n, c = logits.shape[:2]
-    s = logits[0, 0].numel()
-    check(load_library().b200unet_dice_bwd(logits.data_ptr(), target.data_ptr(), n, c, s, flags, nr, dr,
-                                           sums.data_ptr(), grad_out.data_ptr(), dlogits.data_ptr(), stream_ptr()),
-          "dice_bwd")
-
-
 # b200unet_dice_ce_desc.target_kind of each target form
 DICE_CE_TARGETS = {"label_u8": 0, "label_i64": 1, "onehot_u8": 2, "soft_f32": 3}
 _DICE_CE_ACTS = {None: 0, "sigmoid": 1, "softmax": 2}
@@ -614,6 +591,18 @@ def cc_sort_by_size(labels, max_count, scratch) -> None:
     nvol, d, h, w = labels.shape
     check(load_library().b200unet_cc_sort_by_size(labels.data_ptr(), nvol, d, h, w, max_count, scratch.data_ptr(), stream_ptr()),
           "cc_sort_by_size")
+
+
+def dice_fwd(desc: DiceCEDesc, logits, target, scratch, loss) -> None:
+    n, c, s = _nc_s(logits)
+    check(load_library().b200unet_dice_fwd(C.byref(desc), logits.data_ptr(), target.data_ptr(), n, c, s, scratch.data_ptr(),
+                                           loss.data_ptr(), stream_ptr()), "dice_fwd")
+
+
+def dice_bwd(desc: DiceCEDesc, logits, target, scratch, grad_out, dlogits) -> None:
+    n, c, s = _nc_s(logits)
+    check(load_library().b200unet_dice_bwd(C.byref(desc), logits.data_ptr(), target.data_ptr(), n, c, s, scratch.data_ptr(),
+                                           grad_out.data_ptr(), dlogits.data_ptr(), stream_ptr()), "dice_bwd")
 
 
 def dice_ce_fwd(desc: DiceCEDesc, logits, target, scratch, loss) -> None:

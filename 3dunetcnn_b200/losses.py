@@ -18,25 +18,35 @@ from . import lib as _lib
 
 
 class _DiceFunction(torch.autograd.Function):
+    """Both criteria: ``fwd`` / ``bwd`` are the pair of entry points (``lib.dice_*`` or ``lib.dice_ce_*``) and ``scratch_len``
+    the fp64 scratch they share (the sums, the backward coefficients and any per-block partials; no host synchronisation)."""
+
     @staticmethod
-    def forward(ctx, logits, target, flags, nr, dr):
-        n, c = logits.shape[:2]
-        sums = torch.empty((n, c, 3), dtype=torch.float64, device=logits.device)
+    def forward(ctx, logits, target, desc, fwd, bwd, scratch_len):
+        scratch = torch.empty(scratch_len, dtype=torch.float64, device=logits.device)
         loss = torch.empty((), dtype=torch.float32, device=logits.device)
-        _lib.dice_fwd(logits, target, flags, nr, dr, sums, loss)
-        ctx.save_for_backward(logits, target, sums)
-        ctx.cfg = (flags, nr, dr)
+        fwd(desc, logits, target, scratch, loss)
+        ctx.save_for_backward(logits, target, scratch)
+        ctx.desc, ctx.bwd = desc, bwd
         return loss
 
     @staticmethod
     def backward(ctx, grad_out):
-        logits, target, sums = ctx.saved_tensors
-        flags, nr, dr = ctx.cfg
+        logits, target, scratch = ctx.saved_tensors
         dlogits = torch.empty_like(logits)
         g = grad_out.detach().float().contiguous()
         with torch.cuda.device(logits.device):
-            _lib.dice_bwd(logits, target, flags, nr, dr, sums, g, dlogits)
-        return dlogits, None, None, None, None
+            ctx.bwd(ctx.desc, logits, target, scratch, g, dlogits)
+        return dlogits, None, None, None, None, None
+
+
+def _prepare(name: str, output: torch.Tensor, target: torch.Tensor):
+    """(contiguous fp32 logits, target with bool as uint8), both plain CUDA tensors"""
+    if not output.is_cuda or not target.is_cuda:
+        raise RuntimeError("fused %s runs only on CUDA tensors (no CPU fallback)" % name)
+    out = output.as_subclass(torch.Tensor) if type(output) is not torch.Tensor else output
+    tgt = target.as_subclass(torch.Tensor) if type(target) is not torch.Tensor else target
+    return out.contiguous().float(), tgt.to(torch.uint8) if tgt.dtype == torch.bool else tgt
 
 
 class DiceLoss(nn.Module):
@@ -50,51 +60,25 @@ class DiceLoss(nn.Module):
             raise NotImplementedError("fused DiceLoss: softmax / to_onehot_y / other_act / weight are not implemented")
         if reduction not in ("mean", "sum"):
             raise NotImplementedError("fused DiceLoss: reduction=%r (only 'mean'/'sum')" % (reduction,))
-        self.flags = _lib.dice_flags(sigmoid=sigmoid, squared_pred=squared_pred, jaccard=jaccard, batch=batch,
-                                     include_background=include_background, reduction=reduction)
-        self.smooth_nr, self.smooth_dr = float(smooth_nr), float(smooth_dr)
+        self._opts = dict(act="sigmoid" if sigmoid else None, include_background=include_background, squared_pred=squared_pred,
+                          jaccard=jaccard, batch=batch, reduction=reduction, smooth_nr=smooth_nr, smooth_dr=smooth_dr,
+                          lambda_ce=0.0)
 
     def forward(self, output: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
-        if not output.is_cuda:
-            raise RuntimeError("fused DiceLoss runs only on CUDA tensors (no CPU fallback)")
         if output.shape != target.shape:
             raise AssertionError("ground truth has different shape (%s) from input (%s)" % (tuple(target.shape), tuple(output.shape)))
-        out = output.as_subclass(torch.Tensor) if type(output) is not torch.Tensor else output
-        tgt = target.as_subclass(torch.Tensor) if type(target) is not torch.Tensor else target
-        out = out.contiguous().float()
-        flags = self.flags
-        if tgt.dtype == torch.bool:
-            tgt = tgt.to(torch.uint8)
-        elif tgt.dtype != torch.uint8:
+        out, tgt = _prepare("DiceLoss", output, target)
+        kinds = _lib.DICE_CE_TARGETS
+        if tgt.dtype == torch.uint8:
+            kind = kinds["onehot_u8"]
+        else:
             # MONAI casts the target to float: soft / interpolated / label-smoothed targets are legal, so any non-uint8
             # target takes the kernels' fp32-target path instead of being truncated to 0/1
-            tgt = tgt.float()
-            flags |= 64
+            tgt, kind = tgt.float(), kinds["soft_f32"]
+        desc = _lib.dice_ce_desc(target_kind=kind, **self._opts)
+        n, c = out.shape[:2]
         with torch.cuda.device(out.device):
-            return _DiceFunction.apply(out, tgt.contiguous(), flags, self.smooth_nr, self.smooth_dr)
-
-
-class _DiceCEFunction(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, logits, target, desc):
-        n, c = logits.shape[:2]
-        # fp64 scratch: the per-block partial sums, their totals and the backward coefficients (no host synchronisation)
-        nbytes = _lib.dice_ce_scratch_bytes(desc, n, c, logits[0, 0].numel())
-        scratch = torch.empty(nbytes // 8, dtype=torch.float64, device=logits.device)
-        loss = torch.empty((), dtype=torch.float32, device=logits.device)
-        _lib.dice_ce_fwd(desc, logits, target, scratch, loss)
-        ctx.save_for_backward(logits, target, scratch)
-        ctx.desc = desc
-        return loss
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        logits, target, scratch = ctx.saved_tensors
-        dlogits = torch.empty_like(logits)
-        g = grad_out.detach().float().contiguous()
-        with torch.cuda.device(logits.device):
-            _lib.dice_ce_bwd(ctx.desc, logits, target, scratch, g, dlogits)
-        return dlogits, None, None
+            return _DiceFunction.apply(out, tgt.contiguous(), desc, _lib.dice_fwd, _lib.dice_bwd, n * c * 5)
 
 
 class DiceCELoss(nn.Module):
@@ -130,8 +114,6 @@ class DiceCELoss(nn.Module):
     def _target_kind(self, c: int, tgt: torch.Tensor):
         """(target as the kernels read it, b200unet_dice_ce_desc.target_kind)"""
         kinds = _lib.DICE_CE_TARGETS
-        if tgt.dtype == torch.bool:
-            tgt = tgt.to(torch.uint8)
         if c > 1 and tgt.shape[1] == 1:                     # label map
             if tgt.dtype == torch.uint8:
                 return tgt, kinds["label_u8"]
@@ -154,12 +136,10 @@ class DiceCELoss(nn.Module):
             raise ValueError("to_onehot_y=True needs a one-channel label map, got a %d-channel target" % tc)
         if c > 1 and not self.to_onehot_y and tc == 1:
             raise ValueError("a one-channel label map needs to_onehot_y=True (input has %d channels)" % c)
-        if not input.is_cuda or not target.is_cuda:
-            raise RuntimeError("fused DiceCELoss runs only on CUDA tensors (no CPU fallback)")
-        out = input.as_subclass(torch.Tensor) if type(input) is not torch.Tensor else input
-        tgt = target.as_subclass(torch.Tensor) if type(target) is not torch.Tensor else target
-        out = out.contiguous().float()
+        out, tgt = _prepare("DiceCELoss", input, target)
         tgt, kind = self._target_kind(c, tgt)
         desc = _lib.dice_ce_desc(target_kind=kind, **self._opts)
+        # fp64 scratch: the per-block partial sums, their totals and the backward coefficients
+        scratch_len = _lib.dice_ce_scratch_bytes(desc, out.shape[0], c, out[0, 0].numel()) // 8
         with torch.cuda.device(out.device):
-            return _DiceCEFunction.apply(out, tgt.contiguous(), desc)
+            return _DiceFunction.apply(out, tgt.contiguous(), desc, _lib.dice_ce_fwd, _lib.dice_ce_bwd, scratch_len)

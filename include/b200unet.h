@@ -129,25 +129,11 @@ size_t b200unet_head_bwd_scratch_bytes(int n_out, int c);
 int b200unet_head_bwd(const b200unet_tensor* x, const float* w, int n_out, const float* dlogits,
                       const b200unet_tensor* dx, float* dw, float* scratch, void* stream);
 
-/* ---- Dice criterion (monai.losses.DiceLoss as configured by script_utils.py:61-77).
- * flags: bit0 sigmoid, bit1 squared_pred, bit2 jaccard, bit3 batch, bit4 exclude background, bit5 reduction=sum,
- * bit6 `target` points to fp32 values (soft labels) instead of uint8.
- * sums: [N][C][3] doubles (I, P, T) written by fwd and consumed by bwd. */
-int b200unet_dice_fwd(const float* logits, const void* target, int n, int c, int64_t spatial, int flags,
-                      float smooth_nr, float smooth_dr, double* sums, float* loss, void* stream);
-int b200unet_dice_bwd(const float* logits, const void* target, int n, int c, int64_t spatial, int flags,
-                      float smooth_nr, float smooth_dr, const double* sums, const float* grad_out, float* dlogits,
-                      void* stream);
-
-/* ---- Dice + cross-entropy criterion (monai.losses.DiceCELoss): loss = lambda_dice * Dice(act(x), t) + lambda_ce * CE(x, t).
- * Dice is the formula above on p = act(x); include_background = 0 drops channel 0 after the activation.  CE is on the raw
- * logits: -sum_c t_c log_softmax(x)_c for c > 1 (a label map is its one-hot row), BCEWithLogits(x, t) for c == 1; mean
- * divides by n * spatial.  lambda_ce = 0 means the CE term is not evaluated, so logits of +-inf give a finite sigmoid Dice
- * loss and gradient.  With c == 1 softmax is ignored and a uint8 label map is the target itself (int64: E_UNSUPPORTED).
- * A label outside [0, c) is an all-zero target row.  logits NCDHW fp32, 1 <= c <= 128.
- * scratch: b200unet_dice_ce_scratch_bytes() bytes (0 = the options or shape are rejected), written by fwd and read by bwd.
- * It starts with sums [n][c][3] fp64 (I, P, T) and ce [n] fp64 (the summed CE terms of each sample).  No floating-point
- * atomics: the loss and dlogits are bit-identical run to run. */
+/* ---- Dice criteria (monai.losses.DiceLoss as configured by script_utils.py:61-77, and monai.losses.DiceCELoss).
+ * Both take their options in b200unet_dice_ce_desc.  loss = lambda_dice * Dice(act(x), t) + lambda_ce * CE(x, t), where per
+ * (n, c) I = sum p*t, P = sum p (or p^2), T = sum t (or t^2) on p = act(x) and f = 1 - (2I + smooth_nr) / (P + T + smooth_dr)
+ * [jaccard: denominator 2(P + T - I)]; batch pools I, P, T over n; Dice is the mean (or sum) of f; include_background = 0 drops
+ * channel 0 after the activation. */
 typedef struct b200unet_dice_ce_desc {
   int32_t act;                  /* 0 identity, 1 sigmoid, 2 softmax over channels */
   int32_t target_kind;          /* 0 uint8 label map [n][1][spatial], 1 int64 label map, 2 uint8 [n][c][spatial], 3 fp32 [n][c][spatial] */
@@ -155,6 +141,23 @@ typedef struct b200unet_dice_ce_desc {
   int32_t reduction;            /* 0 mean, 1 sum */
   float smooth_nr, smooth_dr, lambda_dice, lambda_ce;
 } b200unet_dice_ce_desc;
+
+/* DiceLoss: act 0 or 1 (softmax: E_UNSUPPORTED, b200unet_dice_ce_* runs it), target_kind 2 or 3 (label maps: E_UNSUPPORTED),
+ * lambda_ce 0 (else E_INVALID); any c >= 1.  logits NCDHW fp32.
+ * scratch: [n][c][3] fp64 sums (I, P, T) followed by [n][c][2] fp64 backward coefficients, written by fwd and read by bwd.
+ * The sums are added with fp64 atomics, so the loss may differ in its last bits from run to run. */
+int b200unet_dice_fwd(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c,
+                      int64_t spatial, double* scratch, float* loss, void* stream);
+int b200unet_dice_bwd(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c,
+                      int64_t spatial, const double* scratch, const float* grad_out, float* dlogits, void* stream);
+
+/* DiceCELoss: CE is on the raw logits: -sum_c t_c log_softmax(x)_c for c > 1 (a label map is its one-hot row),
+ * BCEWithLogits(x, t) for c == 1; mean divides by n * spatial.  lambda_ce = 0 means the CE term is not evaluated, so logits of +-inf give a finite sigmoid Dice
+ * loss and gradient.  With c == 1 softmax is ignored and a uint8 label map is the target itself (int64: E_UNSUPPORTED).
+ * A label outside [0, c) is an all-zero target row.  logits NCDHW fp32, 1 <= c <= 128.
+ * scratch: b200unet_dice_ce_scratch_bytes() bytes (0 = the options or shape are rejected), written by fwd and read by bwd.
+ * It starts with sums [n][c][3] fp64 (I, P, T) and ce [n] fp64 (the summed CE terms of each sample).  No floating-point
+ * atomics: the loss and dlogits are bit-identical run to run. */
 size_t b200unet_dice_ce_scratch_bytes(const b200unet_dice_ce_desc* desc, int n, int c, int64_t spatial);
 int b200unet_dice_ce_fwd(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c,
                          int64_t spatial, void* scratch, float* loss, void* stream);

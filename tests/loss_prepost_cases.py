@@ -47,7 +47,7 @@ def c_class(c):
 
 # ------------------------------------------------------------------------------------------------------------ dice.cu
 def dice_geometry(n, c, S, target, aligned=True):
-    """launch_dice_fwd (dice.cu:155-165) and k_dice_sums (:36-68): chunks per (n, c), whether the cap binds, the path, the
+    """launch_dice_fwd (dice.cu:171-190) and k_dice_sums (:34-67): chunks per (n, c), whether the cap binds, the path, the
     sweeps of a thread's grid-stride loop and the fp32 chain: the terms a thread adds into aI / aP / aT before the fp64 block
     sum (4 per vector iteration)"""
     chunks = max(cdiv(S, 1024), 1)

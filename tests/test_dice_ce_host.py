@@ -1,6 +1,8 @@
 """DiceCELoss without a GPU: the torch-op restatement against MONAI's published cases and hand-derived values, its closed-form
-gradient against fp64 autograd, the errors raised before any launch, and the marshalling of the three C-ABI calls."""
+gradient against fp64 autograd, the errors raised before any launch, and the marshalling of the three C-ABI calls; DiceLoss's
+marshalling of the same descriptor, and the options its entry points refuse."""
 import contextlib
+import ctypes as C
 import itertools
 import math
 
@@ -213,3 +215,48 @@ def test_scratch_size_depends_on_the_shape_alone(pkg):
         L.dice_ce_scratch_bytes(d, 2, 129, 1000)
     with pytest.raises(RuntimeError, match="int64"):
         L.dice_ce_scratch_bytes(L.dice_ce_desc(target_kind=1), 2, 1, 1000)
+
+
+@pytest.mark.parametrize("dtype, kind", [(torch.uint8, 2), (torch.bool, 2), (torch.float32, 3), (torch.float16, 3)])
+@pytest.mark.parametrize("opts, fields", [
+    (dict(sigmoid=True), dict(act=1, include_background=1, squared_pred=0, jaccard=0, batch=0, reduction=0,
+                              smooth_nr=1e-5, smooth_dr=1e-5)),
+    (dict(include_background=False, squared_pred=True, jaccard=True, batch=True, reduction="sum", smooth_nr=0.5, smooth_dr=2.0),
+     dict(act=0, include_background=0, squared_pred=1, jaccard=1, batch=1, reduction=1, smooth_nr=0.5, smooth_dr=2.0)),
+])
+def test_dice_calls_marshal(pkg, stubbed, dtype, kind, opts, fields):
+    """DiceLoss passes its options in the Dice + cross-entropy descriptor, with no CE term"""
+    x = torch.randn(2, 3, 6, 5, 7).as_subclass(_FakeCuda).requires_grad_(True)
+    t = torch.zeros(2, 3, 6, 5, 7).to(dtype).as_subclass(_FakeCuda)
+    pkg.DiceLoss(**opts)(x, t).backward()
+    assert [n for n, _ in stubbed] == ["b200unet_dice_fwd", "b200unet_dice_bwd"]
+    for _, args in stubbed:
+        desc = args[0]._obj
+        assert desc.target_kind == kind and desc.lambda_ce == 0.0 and desc.lambda_dice == 1.0
+        got = {k: getattr(desc, k) for k in fields}
+        assert got == pytest.approx(fields, rel=1e-7), got
+        assert args[3:6] == (2, 3, 6 * 5 * 7)
+    assert x.grad is not None and x.grad.shape == x.shape
+
+
+@pytest.mark.parametrize("field, value, status", [
+    ("act", 2, -2),                     # softmax: E_UNSUPPORTED
+    ("target_kind", 0, -2),             # uint8 label map: E_UNSUPPORTED
+    ("target_kind", 1, -2),             # int64 label map: E_UNSUPPORTED
+    ("lambda_ce", 0.5, -1),             # a CE term: E_INVALID
+])
+def test_dice_entry_points_reject_what_only_dice_ce_runs(pkg, field, value, status):
+    """b200unet_dice_fwd / _bwd refuse the options only b200unet_dice_ce_* implements, before any CUDA call"""
+    L = pkg.lib
+    lib = L.load_library()
+    d = L.dice_ce_desc(act="sigmoid", target_kind=L.DICE_CE_TARGETS["onehot_u8"], lambda_ce=0.0)
+    setattr(d, field, value)
+    n, c, s = 2, 3, 64
+    logits, target = torch.zeros(n, c, s), torch.zeros(n, c, s, dtype=torch.uint8)
+    scratch, loss, g, dlogits = torch.zeros(n * c * 5, dtype=torch.float64), torch.zeros(()), torch.ones(()), torch.zeros(n, c, s)
+    assert lib.b200unet_dice_fwd(C.byref(d), logits.data_ptr(), target.data_ptr(), n, c, s, scratch.data_ptr(), loss.data_ptr(),
+                                 None) == status
+    assert lib.b200unet_last_error().decode().startswith("dice: ")
+    assert lib.b200unet_dice_bwd(C.byref(d), logits.data_ptr(), target.data_ptr(), n, c, s, scratch.data_ptr(), g.data_ptr(),
+                                 dlogits.data_ptr(), None) == status
+    assert "b200unet_dice_ce_" in lib.b200unet_last_error().decode()
