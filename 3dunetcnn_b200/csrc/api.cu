@@ -380,6 +380,11 @@ int b200unet_diag_head_fwd(const b200unet_tensor* x, const float* w, const float
   NOT_NULL(x); NOT_NULL(w); NOT_NULL(logits);
   return launch_head_fwd(to_act(x), w, n_out, act, logits, to_stream(stream), bias);
 }
+int b200unet_diag_head_bwd(const b200unet_tensor* x, const float* w, int n_out, const float* dlogits, const b200unet_tensor* dx, float* dw,
+                           float* dbias, float* scratch, void* stream) {
+  NOT_NULL(x); NOT_NULL(w); NOT_NULL(dlogits); NOT_NULL(dx); NOT_NULL(dw); NOT_NULL(scratch);
+  return launch_head_bwd(to_act(x), w, n_out, dlogits, to_act(dx), dw, to_stream(stream), scratch, dbias);
+}
 int b200unet_diag_head_dbias(const float* dlogits, int n, int n_out, int64_t spatial, float* scratch, float* dbias, void* stream) {
   NOT_NULL(dlogits); NOT_NULL(scratch); NOT_NULL(dbias);
   return launch_head_dbias(dlogits, n, n_out, spatial, dbias, to_stream(stream), scratch);

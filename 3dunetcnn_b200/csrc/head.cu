@@ -204,7 +204,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_head_bwd_mma(Act x, const float
   const int warp = threadIdx.x >> 5, wg = threadIdx.x >> 7, wq = warp & 3, lane = threadIdx.x & 31;
   const long long S = (long long)x.D * x.H * x.W, total = x.voxels();
   const long long tiles = (total + kTile - 1) / kTile;
-  const bool vec = (S & 3) == 0;
+  // float4 loads need S % 4 == 0 (a voxel quad 4 q.. of a tile then stays in one sample) and a 16-byte aligned dlogits: a
+  // contiguous torch gradient may sit at any float offset of its storage
+  const bool vec = (S & 3) == 0 && (reinterpret_cast<uintptr_t>(dlogits) & 15) == 0;
   // float4 k of this thread: output o = 8 k + tid % 8, voxels 4 q .. 4 q + 3 of the tile with q = tid / 8 (four lanes read 64
   // contiguous bytes of one output; eight outputs share one 128-byte core-matrix column block in shared memory)
   const int oq = threadIdx.x & 7, q = threadIdx.x >> 3;
@@ -219,10 +221,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_head_bwd_mma(Act x, const float
       const long long v = v0 + 4 * q;
       r[k] = make_float4(0.f, 0.f, 0.f, 0.f);
       if (o < n_out && v < total) {
-        if (vec) {   // 4 voxels of one sample, 16-byte aligned
+        if (vec) {   // 4 voxels of one sample at a multiple of 4 floats from the aligned base
           const long long n = v / S;
           r[k] = __ldg(reinterpret_cast<const float4*>(dlogits + (n * n_out + o) * S + (v - n * S)));
-        } else {
+        } else {   // S % 4 != 0 or a misaligned dlogits: the same float4, one voxel at a time
           float e[4];
 #pragma unroll
           for (int j = 0; j < 4; ++j) {

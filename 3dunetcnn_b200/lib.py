@@ -198,6 +198,8 @@ _DIAG_SIGS = {
                                        C.c_void_p, C.c_void_p, C.POINTER(Tensor5), C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p,
                                        C.c_void_p]),
     "b200unet_diag_head_fwd": (C.c_int, [C.POINTER(Tensor5), C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "b200unet_diag_head_bwd": (C.c_int, [C.POINTER(Tensor5), C.c_void_p, C.c_int, C.c_void_p, C.POINTER(Tensor5), C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200unet_diag_head_dbias": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200unet_diag_input_pack": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(Tensor5), C.c_void_p, C.c_int, C.c_void_p]),
     "b200unet_diag_input_grad": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_void_p, C.c_int, C.POINTER(Tensor5),
@@ -440,6 +442,18 @@ def head_fwd_ex(x: Act, w: torch.Tensor, bias: Optional[torch.Tensor], n_out: in
     """head_fwd with a per-output bias (None = none), as the plans run it"""
     check(load_library().b200unet_diag_head_fwd(C.byref(x.ct()), w.data_ptr(), _p(bias), n_out, act, logits.data_ptr(), stream_ptr()),
           "diag_head_fwd")
+
+
+def head_bwd_ex(x: Act, w: torch.Tensor, n_out: int, dlogits: torch.Tensor, dx: Act, dw: torch.Tensor, dbias: Optional[torch.Tensor],
+                scratch: torch.Tensor) -> None:
+    """head_bwd with the fused bias gradient (None = none; 9..128 outputs only) into a caller-owned scratch of at least
+    b200unet_head_bwd_scratch_bytes(n_out, x.c) bytes, as the plans run it"""
+    check(load_library().b200unet_diag_head_bwd(C.byref(x.ct()), w.data_ptr(), n_out, dlogits.data_ptr(), C.byref(dx.ct()), dw.data_ptr(),
+                                                _p(dbias), scratch.data_ptr(), stream_ptr()), "diag_head_bwd")
+
+
+def head_bwd_scratch_bytes(n_out: int, c: int) -> int:
+    return int(load_library().b200unet_head_bwd_scratch_bytes(n_out, c))
 
 
 def head_dbias(dlogits: torch.Tensor, dbias: torch.Tensor) -> None:

@@ -91,6 +91,11 @@ int b200unet_diag_gn_bwd(const b200unet_tensor* dz, const b200unet_tensor* x, co
                          const b200unet_tensor* dx, const float* scale, void* stream);
 /* the 1x1x1 head forward of b200unet_head_fwd with a per-output bias (NULL = none), as the plans run it */
 int b200unet_diag_head_fwd(const b200unet_tensor* x, const float* w, const float* bias, int n_out, int act, float* logits, void* stream);
+/* b200unet_head_bwd with the fused bias gradient the plans take at 9..128 outputs: dbias[o] = sum of dlogits over n and the voxels
+ * (overwritten; NULL = none, which 1..8 outputs require).  scratch: b200unet_head_bwd_scratch_bytes(n_out, x->c), owned by the
+ * caller, so that a test can see which weight- and bias-gradient slots the tensor-core backward writes */
+int b200unet_diag_head_bwd(const b200unet_tensor* x, const float* w, int n_out, const float* dlogits, const b200unet_tensor* dx, float* dw,
+                           float* dbias, float* scratch, void* stream);
 /* dbias[o] = sum of dlogits [n][n_out][spatial] over n and the voxels (overwritten), 1..32 outputs; scratch: 128 * n_out doubles */
 int b200unet_diag_head_dbias(const float* dlogits, int n, int n_out, int64_t spatial, float* scratch, float* dbias, void* stream);
 /* the network input NCDHW fp32 [n][c][out.d * out.h * out.w] -> NDHWC bf16 out (out->c = 8 or 16, the channels from c on stored

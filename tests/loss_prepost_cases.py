@@ -205,6 +205,7 @@ def config_launches():
         128^3 patches): DiceLoss(sigmoid=True) on uint8 one-hot targets;
       - the golden recipes, and the many-class setups of tests/test_gpu_many_classes.py: the 24- and 104-output fixtures
         (1 x 32^3), the 104-output machinery (2 x 32^3 and 2 x 16^3) and the 128-output head shape (2 x 5 x 7 x 3);
+      - README's head table at the C2 size with 104 and 128 outputs: DiceLoss(sigmoid=True) on uint8 one-hot targets;
       - a DiceCELoss(softmax=True, to_onehot_y=True) step on a label map at 128^3, batch 2, 3 and 16 classes, uint8 and int64;
       - bench.py C5's tiled inference: one 256^3 volume, roi 128^3, overlap 0.25, sw_batch 3, one output channel;
       - the BraTS z-score: NormalizeIntensity(nonzero=True, channel_wise=True) on 4 channels at 128^3 and 240 x 240 x 155."""
@@ -217,6 +218,8 @@ def config_launches():
                                ("mc104-machinery", (2, 104, (32, 32, 32))), ("mc104-graph", (2, 104, (16, 16, 16))),
                                ("mc128-head", (2, 128, (5, 7, 3)))]:
         out.append((name, "dice", (n, c, vol(dims), "u8")))
+    for c in (104, 128):
+        out.append(("C2-%d" % c, "dice", (2, c, 128 ** 3, "u8")))
     for c in (3, 16):
         for kind in ("label_u8", "label_i64"):
             out.append(("dicece-label-c%d" % c, "dice_ce", (2, c, 128 ** 3, kind, "softmax", True)))
@@ -290,6 +293,9 @@ DICE_CASES = [
     _case("dice", 1, 104, 32 ** 3, "u8", key=("dice", "many", "capped", "multi-sweep", "vec", "u8")),               # mc104
     _case("dice", 2, 104, 32 ** 3, "u8", key=("dice", "many", "capped", "multi-sweep", "vec", "u8")),
     _case("dice", 2, 104, 64 ** 3, "u8", key=("dice", "many", "capped", "multi-sweep", "vec", "u8")),
+    # README's head table at the C2 size: 1368 (104 classes) and 1640 (128) terms in a thread's fp32 chains
+    _case("dice", 2, 104, 128 ** 3, "u8", key=("dice", "many", "capped", "multi-sweep", "vec", "u8")),              # C2-104
+    _case("dice", 2, 128, 128 ** 3, "u8", key=("dice", "many", "capped", "multi-sweep", "vec", "u8")),              # C2-128
     _case("dice", 2, 104, 16 ** 3, "u8", key=("dice", "many", "uncapped", "one-sweep", "vec", "u8")),
     _case("dice", 2, 128, 105, "u8", key=("dice", "many", "uncapped", "one-sweep", "scalar", "u8")),                # mc128 head
     _case("dice", 2, 128, 32 ** 3, "f32", key=("dice", "many", "capped", "multi-sweep", "scalar", "f32")),

@@ -194,8 +194,11 @@ def test_bandwidth_kernel_diagnostics_marshal(pkg, stubbed):
     L.bias_grad(b, torch.zeros(16), ext=L.diag_ext(dy_vis=(3, 7, 7)))
     L.head_fwd_ex(b, torch.zeros(3, 16), torch.zeros(3), 3, 2, torch.zeros(1, 3, 4, 8, 8))
     L.head_dbias(torch.zeros(1, 3, 4, 8, 8), torch.zeros(3))
+    scratch = torch.zeros(L.head_bwd_scratch_bytes(24, 16), dtype=torch.uint8)
+    L.head_bwd_ex(b, torch.zeros(24, 16), 24, torch.zeros(1, 24, 4, 8, 8), b, torch.zeros(24, 16), torch.zeros(24), scratch)
+    L.head_bwd_ex(b, torch.zeros(24, 16), 24, torch.zeros(1, 24, 4, 8, 8), b, torch.zeros(24, 16), None, scratch)
     L.input_pack(torch.zeros(1, 4, 4, 8, 8), b, st, 16)
     L.input_grad(b, b, coef, torch.zeros(1, 16, 2), 16, b, 4, torch.zeros(1, 4, 4, 8, 8))
     L.input_grad(None, None, None, None, 0, b, 4, torch.zeros(1, 4, 4, 8, 8))
     assert {"b200unet_diag_gn_bwd", "b200unet_act_bwd", "b200unet_diag_bias_grad", "b200unet_diag_head_fwd", "b200unet_diag_head_dbias",
-            "b200unet_diag_input_pack", "b200unet_diag_input_grad"} <= set(stubbed)
+            "b200unet_diag_head_bwd", "b200unet_diag_input_pack", "b200unet_diag_input_grad"} <= set(stubbed)

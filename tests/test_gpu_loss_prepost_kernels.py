@@ -253,6 +253,8 @@ def test_dice_loss_and_dlogits_match_fp64(pkg, case):
         assert err <= lim, "%s: loss %.10g ref %.10g bound %.3g" % (what, float(loss.detach()), ref, lim)
         note(case, "loss", err / lim)
         note(case, "dlogits", within(dx, rdx, dlim, what + " dlogits"))
+        # the C2-size rows hold 537 M logits: free this flag set's fp64 tensors (4.3 GB each) before the next one's
+        del loss, dx, rdx, dlim, x64, xq
 
 
 # ------------------------------------------------------------------------------------------------------ Dice + CE

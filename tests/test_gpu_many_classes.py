@@ -1,7 +1,8 @@
-"""Many-class heads (9..128 outputs) on the GPU: the tensor-core head kernels through the C ABI against fp64 einsum, UNet3D
-in split precision against the reference's multi-class fixture (tests/golden/multiclass.npz), bf16 against torch's own bf16
-autocast, DynUNet with its bias, a cross-entropy step, and the existing machinery (launch count,
-determinism, input-gradient plans, CUDA graphs, sliding windows, pre/post-processing) at 104 classes."""
+"""Many-class heads (9..128 outputs) on the GPU: the head's refusal of 129 outputs (tests/test_gpu_head_kernels.py holds the
+tensor-core head kernels to fp64), UNet3D in split precision against the reference's multi-class fixture
+(tests/golden/multiclass.npz), bf16 against torch's own bf16 autocast, DynUNet with its bias, a cross-entropy step, and the
+existing machinery (launch count, determinism, input-gradient plans, CUDA graphs, sliding windows, pre/post-processing) at
+104 classes."""
 import os
 import sys
 
@@ -46,81 +47,6 @@ def _act_in(pkg, shape, c, split, seed):
     lo = (v - hi.float()).to(torch.bfloat16) if split else None
     val = hi.double() + (lo.double() if split else 0)
     return pkg.lib.Act(hi.to(DEV).contiguous(), lo.to(DEV).contiguous() if split else None), val
-
-
-def _act_value(a):
-    return a.hi.double().cpu() + (a.lo.double().cpu() if a.lo is not None else 0)
-
-
-def _head_case(pkg, n_out, c, split, shape, act=0, seed=0):
-    L = pkg.lib
-    x, xv = _act_in(pkg, shape, c, split, seed)
-    g = torch.Generator().manual_seed(seed + 1)
-    w = (torch.randn(n_out, c, generator=g) / c ** 0.5)
-    logits = torch.empty((shape[0], n_out) + shape[1:], device=DEV)
-    L.head_fwd(x, w.to(DEV), n_out, act, logits)
-    ref = torch.einsum("ndhwc,oc->nodhw", xv, w.double())
-    if act == 1:
-        ref = torch.sigmoid(ref)
-    elif act == 2:
-        ref = torch.softmax(ref, dim=1)
-    return x, xv, w, logits, ref
-
-
-HEAD_SHAPES = [(n_out, c) for n_out in (9, 16, 24, 104, 128) for c in (8, 32, 48, 64)]
-
-
-@pytest.mark.parametrize("split", [False, True])
-@pytest.mark.parametrize("n_out,c", HEAD_SHAPES)
-def test_head_kernels_match_fp64_einsum(pkg, n_out, c, split):
-    shape = (2, 8, 9, 10)                                             # 1440 voxels: 12 tiles, the last one partial
-    x, xv, w, logits, ref = _head_case(pkg, n_out, c, split, shape)
-    tol = 2e-5 if split else 1e-2
-    assert _rel(logits, ref) < tol
-    # backward: dx = g w, dw = sum_v g x
-    L = pkg.lib
-    gl = torch.randn(logits.shape, generator=torch.Generator().manual_seed(7))
-    dx = L.Act.empty(*shape, c, split=split)
-    dw = torch.empty(n_out, c, device=DEV)
-    L.head_bwd(x, w.to(DEV), n_out, gl.to(DEV), dx, dw)
-    torch.cuda.synchronize()
-    ref_dx = torch.einsum("nodhw,oc->ndhwc", gl.double(), w.double())
-    ref_dw = torch.einsum("nodhw,ndhwc->oc", gl.double(), xv)
-    assert _rel(_act_value(dx), ref_dx) < (2e-5 if split else 1e-2)
-    assert _rel(dw, ref_dw) < (2e-5 if split else 1e-2)
-    # bit-identical on a second run
-    dx2 = L.Act.empty(*shape, c, split=split)
-    dw2 = torch.empty(n_out, c, device=DEV)
-    L.head_bwd(x, w.to(DEV), n_out, gl.to(DEV), dx2, dw2)
-    torch.cuda.synchronize()
-    assert torch.equal(dw, dw2) and torch.equal(dx.hi, dx2.hi)
-    assert not split or torch.equal(dx.lo, dx2.lo)
-
-
-@pytest.mark.parametrize("split", [False, True])
-@pytest.mark.parametrize("n_out", [9, 104])
-def test_head_kernels_odd_extents_straddle_samples(pkg, n_out, split):
-    shape = (2, 5, 7, 3)                                               # 105 voxels per sample: tiles straddle the samples
-    c = 32
-    x, xv, w, logits, ref = _head_case(pkg, n_out, c, split, shape, seed=3)
-    assert _rel(logits, ref) < (2e-5 if split else 1e-2)
-    L = pkg.lib
-    gl = torch.randn(logits.shape, generator=torch.Generator().manual_seed(8))
-    dx = L.Act.empty(*shape, c, split=split)
-    dw = torch.empty(n_out, c, device=DEV)
-    L.head_bwd(x, w.to(DEV), n_out, gl.to(DEV), dx, dw)
-    torch.cuda.synchronize()
-    assert _rel(_act_value(dx), torch.einsum("nodhw,oc->ndhwc", gl.double(), w.double())) < (2e-5 if split else 1e-2)
-    assert _rel(dw, torch.einsum("nodhw,ndhwc->oc", gl.double(), xv)) < (2e-5 if split else 1e-2)
-
-
-@pytest.mark.parametrize("act", [1, 2])
-@pytest.mark.parametrize("n_out", [9, 24, 128])
-def test_head_activation_epilogues(pkg, n_out, act):
-    _, _, _, logits, ref = _head_case(pkg, n_out, 32, True, (2, 5, 7, 3), act=act, seed=5)
-    assert float((logits.double().cpu() - ref).abs().max()) < 1e-5
-    if act == 2:                                                       # pad channels excluded from the softmax
-        assert float((logits.double().sum(dim=1) - 1).abs().max()) < 1e-5
 
 
 def test_head_refuses_129_outputs_with_the_limit(pkg):

@@ -67,6 +67,18 @@ def test_config_regimes_include_the_untested_geometry():
     assert ("zscore", "capped", "nonzero", "channel-wise") in keys                           # BraTS
 
 
+def test_many_class_dice_runs_at_the_c2_size():
+    """README's head table puts DiceLoss at 104 and 128 classes on 2 x 128^3: the table runs both shapes, so the longest
+    per-thread chains (4 x 342 and 4 x 410 terms) are held to the bound model"""
+    configs = {name: args for name, kernel, args in B.config_launches() if kernel == "dice"}
+    assert configs["C2-104"] == (2, 104, 128 ** 3, "u8") and configs["C2-128"] == (2, 128, 128 ** 3, "u8")
+    rows = {c.args[:4] for c in B.DICE_CASES if not c.opts}
+    for n, c, S, t in (configs["C2-104"], configs["C2-128"]):
+        assert (n, c, S, t) in rows
+    chains = [B.dice_geometry(*c.args)["chain"] for c in B.DICE_CASES]
+    assert max(chains) == 4 * 410 and 4 * 342 in chains
+
+
 def test_table_covers_every_target_form_activation_and_edge():
     """beyond the configurations: both Dice target forms and the misaligned views; every DiceCE target form, activation, CE on
     and off, one and several tiles, partial tiles and idle threads; tile batches that span samples and end partial"""
