@@ -37,6 +37,10 @@ size_t foreground_scratch_bytes(int N, int C) {
     set_error("foreground: 1..%d channels and 1..65535 samples (n=%d c=%d)", B200_AUG_MAX_CHANNELS, N, C);
     return 0;
   }
+  if (N * C > 65535) {   // k_fg_hist puts the planes on gridDim.y
+    set_error("foreground: n * c = %d planes, at most 65535 (n=%d c=%d)", N * C, N, C);
+    return 0;
+  }
   const int P = N * C;
   return fg_hist_bytes(P) + sizeof(FgPlane) * (size_t)P + sizeof(int) * 6 * (size_t)N;
 }

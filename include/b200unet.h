@@ -217,7 +217,7 @@ int b200unet_augment_intensity(float* image, int n, int c, int64_t spatial, int 
  * above (MONAI CropForegroundD with the reference's percentile_threshold, then ResizeD, as datasets/segmentation.py:55-70 chains
  * them lazily).  samples: DEVICE int64 [n][5] rows (image pointer, label pointer or 0, d, h, w): sample i is fp32
  * [c][d][h][w] and uint8 [l][d][h][w], each fewer than 2^31 voxels per channel.
- *   foreground_scratch_bytes: from (n, c) alone (0 = rejected: 1..16 channels, 1..65535 samples).
+ *   foreground_scratch_bytes: from (n, c) alone (0 = rejected: 1..16 channels, 1..65535 samples, n * c <= 65535).
  *   foreground_box: crop = 0 takes every whole volume; otherwise the mask is any_c(x_c > thr_c) with thr = 0 (ranks NULL,
  *                  MONAI's default select_fn) or thr_c the linear interpolation, weight gamma DEVICE fp32 [n][c], between
  *                  the order statistics of ranks DEVICE int64 [n][c][2] (np.percentile's two neighbours), written to
