@@ -46,13 +46,19 @@ int launch_unpack_wgrad(const float* g, int Co, int Ci, int Cop, int Cip, int T,
                         cudaStream_t st);
 // batched weight packing / gradient unpacking (one launch for the whole network)
 struct PtrTable { const void* p[256]; };
+// PackJob::mode, the `mode` of b200unet_pack_weights / b200unet_unpack_wgrad.  Conv3d weight [Co][Ci][T]:
+enum PackMode {
+  PACK_FWD = 0,          // forward [T][Cop][Cip]; unpack: [T][Cip][Cop] accumulator -> [Co][Ci][T]
+  PACK_DGRAD = 1,        // data-gradient [T][Cip][Cop], taps flipped
+  // ConvTranspose3d weight [Ci][Co][T] (the modes from PACK_T_FLIPPED on):
+  PACK_T_FLIPPED = 2,    // forward [T][Cop][Cip], taps flipped (the zero-inserted k3 s2 p1 layer); unpack: -> [Ci][Co][T] flipped
+  PACK_T_DGRAD = 3,      // data-gradient [T][Cip][Cop], unflipped
+  PACK_T_FWD = 4,        // forward [T][Cop][Cip], unflipped (kernel = stride ConvTranspose3d: out[2j+p] = x[j] w[p])
+};
 struct PackJob {
   int pidx;                 // index into the parameter / gradient pointer table
   int Co, Ci, Cop, Cip, T;
-  int mode;                 // 0 forward [T][Cop][Cip], 1 data-gradient [T][Cip][Cop] flipped; ConvTranspose3d weight
-                            // [Ci][Co][T]: 2 forward [T][Cop][Cip] flipped, 3 data-gradient [T][Cip][Cop] unflipped,
-                            // 4 forward [T][Cop][Cip] unflipped (kernel = stride ConvTranspose3d: out[2j+p] = x[j] w[p]);
-                            // unpack: 0 -> [Co][Ci][T], 2 -> [Ci][Co][T] flipped
+  int mode;                 // PackMode; unpack: PACK_FWD or PACK_T_FLIPPED
   long long off_hi, off_lo; // workspace byte offsets (unpack: off_hi = fp32 accumulator)
 };
 int launch_pack_all(const PtrTable& params, const PackJob* jobs_dev, int njobs, uint8_t* ws, bool split, cudaStream_t st);
@@ -207,7 +213,7 @@ struct ConvOp {
   int zero_last;       // mode 0: output voxels on the high boundary of each axis are forced to 0
   int max_ctas;        // > 0: at most this many CTAs per N tile on the persistent halo kernel (diagnostics: several tiles per CTA)
   int cls_mode;        // 2: ConvTranspose3d(kernel = stride = 2) forward: src[0].x = input at half the output extent, src[0].w = the
-                       // mode-4 pack [8][Cop][Cip]; class p = one tap.  1: data gradient of a 3x3x3 stride-2 padding-1 convolution WITHOUT zero insertion: src[0].x = dY (low
+                       // PACK_T_FWD pack [8][Cop][Cip]; class p = one tap.  1: data gradient of a 3x3x3 stride-2 padding-1 convolution WITHOUT zero insertion: src[0].x = dY (low
                        // resolution), src[0].w = the flipped data-gradient pack, out = dX at twice the extent; eight
                        // parity-class implicit GEMMs (27 tap products in total instead of 8 x 27) in one launch
 };

@@ -69,6 +69,14 @@ struct Prof {
   bool overflow = false;
 };
 
+enum LayerKind {
+  LAYER_CONV = 0,          // nn.Conv3d, weight [Co][Ci][T], padding ksz / 2
+  LAYER_CONVT_ZI,          // nn.ConvTranspose3d(k3, s2, p1) + bias parameter pb, weight [Ci][Co][T]: run as a stride-1 conv over
+                           // the zero-inserted input (ksz 3, stride 1), the high boundary of its output forced to 0
+  LAYER_CONVT_K2S2,        // ConvTranspose3d with kernel = stride = 2 (MONAI UnetUpBlock): ksz 2, stride 2, weight [Ci][Co][8], no padding
+};
+enum ConvDir { DIR_FWD = 0, DIR_DGRAD, DIR_WGRAD };
+
 struct ConvLayer {
   int pw;                  // parameter index
   int Co, Ci, Cop, Cip, ksz, stride, T;
@@ -76,11 +84,45 @@ struct ConvLayer {
   size_t wd_hi, wd_lo;     // packed data-grad weights [T][Cip][Cop]
   size_t dw;               // fp32 accumulator         [T][Cip][Cop]
   bool need_dgrad;
-  bool transposed;         // nn.ConvTranspose3d weight [Ci][Co][T] (+ bias parameter pb)
-  bool up2;                // ConvTranspose3d with kernel = stride = 2 (MONAI UnetUpBlock): T = 8, weight [Ci][Co][8], no padding
+  LayerKind kind;
   int pb;
   std::string name;        // state-dict key (profiling labels)
 };
+
+// How layer c runs in direction dir: everything the ops, the pack jobs and the MAC accounting take from its kind.
+struct ConvRole {
+  int stride;              // traversal stride on the A operand (the input; dgrad: the output gradient)
+  int nopad;               // 1: no padding
+  int cls_mode;            // ConvOp::cls_mode
+  bool bias;               // + bias parameter pb, the output's high boundary forced to 0 (ConvOp::zero_last)
+  int pack;                // PackMode of the weights the op reads; DIR_WGRAD: unpack mode of the accumulator
+  bool swap;               // the op sees the layer with Ci and Co exchanged: the data gradient, and the weight gradient of a
+                           // kernel = stride layer, which is that of the stride-2 convolution from the fine grid (dU, Co) to the
+                           // coarse grid (X, Ci): a = dU, dy = X, accumulator [T][Cop][Cip]
+  int macs_div;            // a transposed layer's output grid has 8x the voxels of its input
+};
+
+static ConvRole conv_role(const ConvLayer& c, ConvDir dir) {
+  const bool up = c.kind != LAYER_CONV, k2 = c.kind == LAYER_CONVT_K2S2;
+  ConvRole r = {};
+  r.nopad = k2 ? 1 : 0;
+  r.bias = dir == DIR_FWD && c.kind == LAYER_CONVT_ZI;
+  r.swap = dir == DIR_DGRAD || (dir == DIR_WGRAD && k2);
+  r.macs_div = up ? 8 : 1;
+  if (dir == DIR_FWD) {
+    r.stride = up ? 1 : c.stride;
+    r.cls_mode = k2 ? 2 : 0;
+    r.pack = k2 ? PACK_T_FWD : up ? PACK_T_FLIPPED : PACK_FWD;
+  } else if (dir == DIR_DGRAD) {   // a stride-2 convolution: parity-class mode over the un-inserted output gradient
+    r.stride = up ? 2 : 1;
+    r.cls_mode = !up && c.stride == 2 ? 1 : 0;
+    r.pack = up ? PACK_T_DGRAD : PACK_DGRAD;
+  } else {
+    r.stride = c.stride;
+    r.pack = c.kind == LAYER_CONVT_ZI ? PACK_T_FLIPPED : PACK_FWD;
+  }
+  return r;
+}
 
 struct NormLayer {
   int pg, pb;
@@ -298,7 +340,7 @@ static double* stats_ptr(const Plan& P, const RunCtx& cx, TRef t) {
   return reinterpret_cast<double*>(cx.ws + P.stats_off + b.stats_off) + (size_t)t.c0 * 2;
 }
 
-static int new_conv(Plan& P, const std::string& key, int Co, int Ci, int ksz, int stride, bool need_dgrad) {
+static int new_conv(Plan& P, const std::string& key, int Co, int Ci, int ksz, int stride, bool need_dgrad, LayerKind kind = LAYER_CONV) {
   ConvLayer c;
   c.pw = P.find_param(key);
   c.name = key;
@@ -306,8 +348,7 @@ static int new_conv(Plan& P, const std::string& key, int Co, int Ci, int ksz, in
   c.ksz = ksz; c.stride = stride; c.T = ksz * ksz * ksz;
   need_dgrad = need_dgrad && !P.infer;
   c.need_dgrad = need_dgrad;
-  c.transposed = false;
-  c.up2 = false;
+  c.kind = kind;
   c.pb = -1;
   size_t n = (size_t)c.T * c.Cop * c.Cip;
   c.wf_hi = P.alloc(n * 2);
@@ -367,68 +408,79 @@ static void emit_norm_fwd(Plan& P, int ni, TRef x, TRef y) {
   });
 }
 
-// A operand + packed weights of a convolution through layer c: its forward pack applied to x, or (dgrad) its data-gradient pack
-// applied to x = the gradient of its output.  A convolution reads its input at its stride and its output gradient at stride 1
-// (stride 2: parity-class mode); a transposed convolution reads its input at stride 1 (zero-inserted or parity-class mode) and
-// its output gradient at stride 2.
-static ConvSrc conv_src(const Plan& P, const RunCtx& cx, const ConvLayer& c, TRef x, bool dgrad) {
-  const bool up = c.transposed || c.up2;
+// A operand + packed weights of layer c in direction dir (DIR_FWD or DIR_DGRAD): its forward pack applied to x, or its
+// data-gradient pack applied to x = the gradient of its output
+static ConvSrc conv_src(const Plan& P, const RunCtx& cx, const ConvLayer& c, TRef x, ConvDir dir) {
+  const ConvRole r = conv_role(c, dir);
+  const bool dgrad = dir == DIR_DGRAD;
   ConvSrc s;
   memset(&s, 0, sizeof(s));
   s.x = act_of(P, cx, x);
   s.w_hi = reinterpret_cast<bf16*>(cx.ws + (dgrad ? c.wd_hi : c.wf_hi));
   s.w_lo = P.split ? reinterpret_cast<bf16*>(cx.ws + (dgrad ? c.wd_lo : c.wf_lo)) : nullptr;
   s.ksz = c.ksz;
-  s.nopad = c.up2 ? 1 : 0;
-  s.stride = up ? (dgrad ? 2 : 1) : (dgrad ? 1 : c.stride);
-  s.Cip = dgrad ? c.Cop : c.Cip;   // K extent of the data-gradient pack [T][Cip][Cop] = Cop
+  s.nopad = r.nopad;
+  s.stride = r.stride;
+  s.Cip = r.swap ? c.Cop : c.Cip;   // K extent: the data-gradient pack [T][Cip][Cop] has Cop
   return s;
 }
 
-// generic forward-weights conv:  out = (conv(a, W[ci]) [+ conv1x1(a2, W[ci2])] [+ res]) [* dropout]
-static double conv_macs(const Plan& P, int ci, TRef out_like) {
-  const ConvLayer& c = P.convs[ci];
-  const Buf& b = P.bufs[out_like.buf];
-  return (double)b.N * b.D * b.H * b.W * c.Co * c.Ci * c.T / (c.transposed ? 8.0 : 1.0);
+// the convolution through layer c in direction dir (DIR_FWD or DIR_DGRAD) from x to out, plain epilogue
+static ConvOp conv_op(const Plan& P, const RunCtx& cx, const ConvLayer& c, ConvDir dir, TRef x, TRef out) {
+  const ConvRole r = conv_role(c, dir);
+  ConvOp op;
+  memset(&op, 0, sizeof(op));
+  op.nsrc = 1;
+  op.src[0] = conv_src(P, cx, c, x, dir);
+  op.Cop = r.swap ? c.Cip : c.Cop;
+  op.out = act_of(P, cx, out);
+  op.cls_mode = r.cls_mode;
+  if (r.bias) { op.bias = cx.params[c.pb]; op.zero_last = 1; }
+  return op;
 }
 
+// the weight gradient of layer c from its input a and the gradient dy of its output (Acts of act_of, or of shape_act for sizing)
+static WgradOp wgrad_op(const ConvLayer& c, const Act& a, const Act& dy) {
+  const ConvRole r = conv_role(c, DIR_WGRAD);
+  WgradOp op;
+  memset(&op, 0, sizeof(op));
+  op.a = r.swap ? dy : a;
+  op.dy = r.swap ? a : dy;
+  op.ksz = c.ksz; op.stride = r.stride; op.nopad = r.nopad;
+  op.Cip = r.swap ? c.Cop : c.Cip;
+  op.Cop = r.swap ? c.Cip : c.Cop;
+  return op;
+}
+
+// algorithmic MACs of layer ci in direction dir; out_like is on the grid of the layer's output
+static double conv_macs(const Plan& P, int ci, ConvDir dir, TRef out_like) {
+  const ConvLayer& c = P.convs[ci];
+  const Buf& b = P.bufs[out_like.buf];
+  return (double)b.N * b.D * b.H * b.W * c.Co * c.Ci * c.T / (double)conv_role(c, dir).macs_div;
+}
+
+// generic forward-weights conv:  out = (conv(a, W[ci]) [+ conv1x1(a2, W[ci2])] [+ res]) [* dropout]
 static void emit_conv_fwd(Plan& P, int ci, TRef a, int ci2, TRef a2, TRef res, TRef out, bool stats, bool scale) {
   if (stats) need_stats(P, out.buf);
   const int cat = CAT_CONV_FWD;
-  P.macs[cat] += conv_macs(P, ci, out) + (ci2 >= 0 ? conv_macs(P, ci2, out) : 0.0);
+  P.macs[cat] += conv_macs(P, ci, DIR_FWD, out) + (ci2 >= 0 ? conv_macs(P, ci2, DIR_FWD, out) : 0.0);
   push_op(P.fwd, "conv_fwd " + P.convs[ci].name + " " + shape_of(P, a) + "->" + shape_of(P, out) + (ci2 >= 0 ? " +sample" : "") + (res.valid() ? " +res" : ""),
           [&P, ci, a, ci2, a2, res, out, stats, scale, cat](RunCtx& cx) -> int {
-    const ConvLayer& c = P.convs[ci];
-    ConvOp op;
-    memset(&op, 0, sizeof(op));
-    op.nsrc = 1;
-    op.src[0] = conv_src(P, cx, c, a, false);
-    op.Cop = c.Cop;
+    ConvOp op = conv_op(P, cx, P.convs[ci], DIR_FWD, a, out);
     if (ci2 >= 0) {
       op.nsrc = 2;
-      op.src[1] = conv_src(P, cx, P.convs[ci2], a2, false);
+      op.src[1] = conv_src(P, cx, P.convs[ci2], a2, DIR_FWD);
     }
-    op.out = act_of(P, cx, out);
     Act r;
     if (res.valid()) { r = act_of(P, cx, res); op.res = &r; }
     if (scale && cx.drop) op.scale = cx.drop;
     if (stats) { op.stats = stats_ptr(P, cx, out); op.stats_ld = P.bufs[out.buf].C; }
-    if (c.transposed) { op.bias = cx.params[c.pb]; op.zero_last = 1; }
     LAUNCHED(cx, cat, launch_igemm_conv(op, cx.st));
     return OK;
   });
 }
 
 // ---- backward op emitters
-static void size_wgrad_partials(Plan& P, const Act& a, const Act& dy, int ksz, int stride, int nopad, int Cip, int Cop) {
-  if (!P.deterministic) return;
-  WgradOp op;
-  memset(&op, 0, sizeof(op));
-  op.a = a; op.dy = dy; op.ksz = ksz; op.stride = stride; op.nopad = nopad; op.Cip = Cip; op.Cop = Cop;
-  const size_t need = wgrad_partial_bytes(op, device_sms());
-  if (need > P.wg_part_bytes) P.wg_part_bytes = need;
-}
-
 static Act shape_act(const Plan& P, TRef t) {
   const Buf& b = P.bufs[t.buf];
   return make_act(nullptr, nullptr, b.N, b.D, b.H, b.W, t.c, b.C);
@@ -450,37 +502,29 @@ static int run_wgrad(Plan& P, RunCtx& cx, WgradOp& op) {
   return OK;
 }
 
+// weight gradient of layer ci from its input a and the gradient dy of its output
 static void emit_wgrad(Plan& P, int ci, TRef a, TRef dy) {
-  P.macs[CAT_CONV_WGRAD] += conv_macs(P, ci, dy);
-  size_wgrad_partials(P, shape_act(P, a), shape_act(P, dy), P.convs[ci].ksz, P.convs[ci].stride, 0, P.convs[ci].Cip, P.convs[ci].Cop);
+  P.macs[CAT_CONV_WGRAD] += conv_macs(P, ci, DIR_WGRAD, dy);
+  if (P.deterministic)
+    P.wg_part_bytes = std::max(P.wg_part_bytes, wgrad_partial_bytes(wgrad_op(P.convs[ci], shape_act(P, a), shape_act(P, dy)), device_sms()));
   push_op(P.bwd, "wgrad " + P.convs[ci].name + " " + shape_of(P, a) + " x " + shape_of(P, dy), [&P, ci, a, dy](RunCtx& cx) -> int {
     const ConvLayer& c = P.convs[ci];
-    WgradOp op;
-  memset(&op, 0, sizeof(op));
-    op.a = act_of(P, cx, a);
-    op.dy = act_of(P, cx, dy);
-    op.ksz = c.ksz; op.stride = c.stride; op.nopad = 0; op.Cip = c.Cip; op.Cop = c.Cop;
+    WgradOp op = wgrad_op(c, act_of(P, cx, a), act_of(P, cx, dy));
     op.dw = reinterpret_cast<float*>(cx.ws + P.bz_off + c.dw);
     return run_wgrad(P, cx, op);
   });
 }
 
-// data gradient through conv `ci` (stride 1):  out = conv(dy, Wd)  with either the GN/ReLU backward epilogue
-// (ni >= 0, gn_x = raw input of the norm) or a plain epilogue (+res, *dropout scale).
-static void emit_dgrad(Plan& P, int ci, TRef dy, TRef out, int ni, TRef gn_x, TRef res, bool scale, double alg_macs,
-                       bool cls_mode = false, std::vector<OpFn>* list = nullptr) {
+// data gradient through layer ci:  out = conv(dy, Wd)  with either the GN/ReLU backward epilogue (ni >= 0, gn_x = raw input of
+// the norm) or a plain epilogue (+res, *dropout scale).  reads_input: the layer reads the network input, so its data gradient is
+// left out of the algorithmic MACs (b200unet_plan_algorithmic_macs).
+static void emit_dgrad(Plan& P, int ci, TRef dy, TRef out, int ni, TRef gn_x, TRef res, bool scale, bool reads_input = false,
+                       std::vector<OpFn>* list = nullptr) {
   const int cat = CAT_CONV_DGRAD;
-  P.macs[cat] += alg_macs;
+  if (!reads_input) P.macs[cat] += conv_macs(P, ci, DIR_DGRAD, dy);
   push_op(list ? *list : P.bwd, std::string(ni >= 0 ? "dgrad+gnrelu " : "dgrad ") + P.convs[ci].name + " " + shape_of(P, dy) + "->" + shape_of(P, out),
-          [&P, ci, dy, out, ni, gn_x, res, scale, cat, cls_mode](RunCtx& cx) -> int {
-    const ConvLayer& c = P.convs[ci];
-    ConvOp op;
-    memset(&op, 0, sizeof(op));
-    op.nsrc = 1;
-    op.cls_mode = cls_mode ? 1 : 0;
-    op.src[0] = conv_src(P, cx, c, dy, true);
-    op.Cop = c.Cip;   // rows of Wd = Cip
-    op.out = act_of(P, cx, out);
+          [&P, ci, dy, out, ni, gn_x, res, scale, cat](RunCtx& cx) -> int {
+    ConvOp op = conv_op(P, cx, P.convs[ci], DIR_DGRAD, dy, out);
     Act r, gx;
     if (res.valid()) { r = act_of(P, cx, res); op.res = &r; }
     if (scale && cx.drop) op.scale = cx.drop;
@@ -655,12 +699,12 @@ static TRef build_block_bwd(Plan& P, const BlockRec& r, TRef dOut) {
   emit_wgrad(P, r.c2, r.a2, dOut);
   if (r.cs >= 0) emit_wgrad(P, r.cs, r.X, dOut);
   TRef dz2 = full(P, new_buf(P, N, D, H, W, C));
-  emit_dgrad(P, r.c2, dOut, dz2, r.n2, r.y1, kNone, false, conv_macs(P, r.c2, dOut));
+  emit_dgrad(P, r.c2, dOut, dz2, r.n2, r.y1, kNone, false);
   TRef dy1 = full(P, new_buf(P, N, D, H, W, C));
   emit_gn_bwd(P, r.n2, dz2, r.y1, kNone, dy1, false);
   emit_wgrad(P, r.c1, r.a1, dy1);
   TRef dz1 = full(P, new_buf(P, N, D, H, W, r.X.c));
-  emit_dgrad(P, r.c1, dy1, dz1, r.n1, r.X, kNone, false, r.first ? 0.0 : conv_macs(P, r.c1, dy1));
+  emit_dgrad(P, r.c1, dy1, dz1, r.n1, r.X, kNone, false, /*reads_input=*/r.first);
   if (r.first) {   // no data gradient below the first block: only dgamma / dbeta of its first norm are needed
     emit_gn_bwd_finalize(P, r.n1);
     if (P.input_grad) {
@@ -668,7 +712,7 @@ static TRef build_block_bwd(Plan& P, const BlockRec& r, TRef dOut) {
       TRef res = dOut;
       if (r.cs >= 0) {
         res = full(P, new_buf(P, N, D, H, W, r.X.c));
-        emit_dgrad(P, r.cs, dOut, res, -1, kNone, kNone, false, 0.0, false, &P.igrad);
+        emit_dgrad(P, r.cs, dOut, res, -1, kNone, kNone, false, /*reads_input=*/true, &P.igrad);
       }
       emit_input_grad(P, r.n1, dz1, r.X, res);
     }
@@ -677,7 +721,7 @@ static TRef build_block_bwd(Plan& P, const BlockRec& r, TRef dOut) {
   TRef dX = full(P, new_buf(P, N, D, H, W, r.X.c));
   if (r.cs >= 0) {
     emit_gn_bwd(P, r.n1, dz1, r.X, kNone, dX, false);
-    emit_dgrad(P, r.cs, dOut, dX, -1, kNone, dX, r.scale_in, conv_macs(P, r.cs, dOut));  // dX = (conv1x1(dOut, Ws^T) + dX) [* scale]
+    emit_dgrad(P, r.cs, dOut, dX, -1, kNone, dX, r.scale_in);  // dX = (conv1x1(dOut, Ws^T) + dX) [* scale]
   } else {
     emit_gn_bwd(P, r.n1, dz1, r.X, dOut, dX, r.scale_in);
   }
@@ -685,6 +729,21 @@ static TRef build_block_bwd(Plan& P, const BlockRec& r, TRef dOut) {
 }
 
 static int finish_build(Plan& P);
+
+// spatial extents of each level (level 0: the input's), halved from one level to the next
+static int level_extents(const b200unet_net_desc& d, std::vector<int>& Ds, std::vector<int>& Hs, std::vector<int>& Ws) {
+  const int L = d.n_levels;
+  int D = d.depth, H = d.height, W = d.width;
+  for (int li = 0; li < L; ++li) {
+    Ds.push_back(D); Hs.push_back(H); Ws.push_back(W);
+    if (li + 1 < L)
+      B200_REQUIRE(D % 2 == 0 && H % 2 == 0 && W % 2 == 0 && D >= 2 && H >= 2 && W >= 2, E_UNSUPPORTED,
+                   "plan: level %d extent %dx%dx%d must be even (input %dx%dx%d not divisible by 2^%d)", li, D, H, W,
+                   d.depth, d.height, d.width, L - 1);
+    D /= 2; H /= 2; W /= 2;
+  }
+  return OK;
+}
 
 static int build_unet3d(Plan& P) {
   const b200unet_net_desc& d = P.d;
@@ -695,17 +754,8 @@ static int build_unet3d(Plan& P) {
   B200_REQUIRE(d.n_outputs >= 1 && d.n_outputs <= B200_HEAD_MAX_OUTPUTS, E_UNSUPPORTED, "plan: n_outputs=%d unsupported (1..%d)",
                d.n_outputs, B200_HEAD_MAX_OUTPUTS);
   std::vector<int> widths, Ds, Hs, Ws;
-  {
-    int w = d.base_width, D = d.depth, H = d.height, W = d.width;
-    for (int li = 0; li < L; ++li) {
-      widths.push_back(w); Ds.push_back(D); Hs.push_back(H); Ws.push_back(W);
-      if (li + 1 < L)
-        B200_REQUIRE(D % 2 == 0 && H % 2 == 0 && W % 2 == 0 && D >= 2 && H >= 2 && W >= 2, E_UNSUPPORTED,
-                     "plan: level %d extent %dx%dx%d must be even (input %dx%dx%d not divisible by 2^%d)", li, D, H, W,
-                     d.depth, d.height, d.width, L - 1);
-      w *= d.feature_dilation; D /= 2; H /= 2; W /= 2;
-    }
-  }
+  B200_TRY(level_extents(d, Ds, Hs, Ws));
+  for (int li = 0, w = d.base_width; li < L; ++li, w *= d.feature_dilation) widths.push_back(w);
   build_param_spec(P);
 
   // ---------------- forward
@@ -784,8 +834,7 @@ static int build_unet3d(Plan& P) {
       // ConvTranspose3d(k3, s2, p1) + bias, then F.pad(+1 high side) = zero-insert + 3x3x3 conv with the flipped
       // kernel over a 2n grid whose last plane/row/column is forced to 0 (decoder.py:101-102, unet.py:34-40)
       const std::string key = "decoder.upsampling_blocks." + std::to_string(i);
-      s.cup = new_conv(P, key + ".weight", out_w, in_w, 3, 1, true);
-      P.convs[s.cup].transposed = true;
+      s.cup = new_conv(P, key + ".weight", out_w, in_w, 3, 1, true, LAYER_CONVT_ZI);
       P.convs[s.cup].pb = P.find_param(key + ".bias");
       B200_REQUIRE(P.convs[s.cup].pb >= 0, E_INVALID, "plan: internal: missing bias for %s", key.c_str());
       s.Z = full(P, new_buf(P, N, 2 * xb.D, 2 * xb.H, 2 * xb.W, in_w));
@@ -839,7 +888,7 @@ static int build_unet3d(Plan& P) {
         return OK;
       });
       emit_wgrad(P, s.cpre, s.Xin, dP);
-      emit_dgrad(P, s.cpre, dP, gX, -1, kNone, kNone, false, conv_macs(P, s.cpre, dP));
+      emit_dgrad(P, s.cpre, dP, gX, -1, kNone, kNone, false);
     } else {
       // the padded boundary of the ConvT output is a constant: mask it out of dU (visible extent 2n-1 through TMA)
       TRef dUm = masked(dU);
@@ -851,7 +900,7 @@ static int build_unet3d(Plan& P) {
         return OK;
       });
       emit_wgrad(P, cup, s.Z, dUm);                                   // dW[tap][ci][co] from the zero-inserted input
-      emit_dgrad(P, cup, dUm, gX, -1, kNone, kNone, false, conv_macs(P, cup, dUm));   // stride-2 conv of dU: dX[i] = sum_k dU[2i+k-1] W[ci][co][k]
+      emit_dgrad(P, cup, dUm, gX, -1, kNone, kNone, false);   // stride-2 conv of dU: dX[i] = sum_k dU[2i+k-1] W[ci][co][k]
     }
     for (int b = d.decoder_blocks[i] - 1; b >= 0; --b) gX = build_block_bwd(P, dec[i][b], gX);
     g = gX;
@@ -862,13 +911,12 @@ static int build_unet3d(Plan& P) {
     if (li > 0) {
       const int lj = li - 1;
       emit_wgrad(P, down[lj], skip[lj], g);
-      TRef gin = g;
       TRef gS = full(P, new_buf(P, N, Ds[lj], Hs[lj], Ws[lj], widths[lj]));
       // dropout scale belongs to the output of encoder block (0,0): that is this tensor iff level 0 has one block
       const bool sc = (lj == 0 && d.encoder_blocks[0] == 1);
-      // eight parity-class implicit GEMMs over the un-inserted gradient (27 tap products instead of 8 x 27), TMA-stored
+      // parity-class mode: eight implicit GEMMs over the un-inserted gradient (27 tap products instead of 8 x 27), TMA-stored
       // into their interleaved positions
-      emit_dgrad(P, down[lj], gin, gS, -1, kNone, dskip_dec[lj], sc, conv_macs(P, down[lj], gin), /*cls_mode=*/true);
+      emit_dgrad(P, down[lj], g, gS, -1, kNone, dskip_dec[lj], sc);
       g = gS;
     }
   }
@@ -895,18 +943,17 @@ static int finish_build(Plan& P) {
   for (const ConvLayer& c : P.convs) {
     PackJob j;
     j.pidx = c.pw; j.Co = c.Co; j.Ci = c.Ci; j.Cop = c.Cop; j.Cip = c.Cip; j.T = c.T;
-    j.mode = c.up2 ? 4 : c.transposed ? 2 : 0; j.off_hi = (long long)c.wf_hi; j.off_lo = (long long)c.wf_lo;
+    j.mode = conv_role(c, DIR_FWD).pack; j.off_hi = (long long)c.wf_hi; j.off_lo = (long long)c.wf_lo;
     P.pack_jobs.push_back(j);
     if (c.need_dgrad) {
-      j.mode = (c.up2 || c.transposed) ? 3 : 1; j.off_hi = (long long)c.wd_hi; j.off_lo = (long long)c.wd_lo;
+      j.mode = conv_role(c, DIR_DGRAD).pack; j.off_hi = (long long)c.wd_hi; j.off_lo = (long long)c.wd_lo;
       P.pack_jobs.push_back(j);
     }
     if (P.infer) continue;
+    const ConvRole r = conv_role(c, DIR_WGRAD);
     PackJob u = j;
-    u.mode = c.transposed ? 2 : 0; u.off_hi = (long long)(P.bz_off + c.dw); u.off_lo = 0;
-    if (c.up2) {   // accumulated with swapped roles as [T][pad(Co)][pad(Ci)] (see emit_wgrad_up2): reads back as [Ci][Co][T]
-      u.mode = 0; u.Co = c.Ci; u.Ci = c.Co; u.Cop = c.Cip; u.Cip = c.Cop;
-    }
+    u.mode = r.pack; u.off_hi = (long long)(P.bz_off + c.dw); u.off_lo = 0;
+    if (r.swap) { std::swap(u.Co, u.Ci); std::swap(u.Cop, u.Cip); }   // accumulated as [T][Cop][Cip]: reads back as [Ci][Co][T]
     P.unpack_jobs.push_back(u);
   }
   P.jobs_off = P.alloc(sizeof(PackJob) * (P.pack_jobs.size() + P.unpack_jobs.size()));
@@ -995,7 +1042,7 @@ static TRef build_dyn_block_bwd(Plan& P, const DynBlock& r, TRef g1, TRef g2) {
   emit_gn_bwd(P, r.n2, dz2, r.c2, kNone, dc2, false);
   emit_wgrad(P, r.k2, r.a1, dc2);
   TRef dz1 = full(P, new_buf(P, N, D, H, W, C));
-  emit_dgrad(P, r.k2, dc2, dz1, r.n1, r.c1, kNone, false, conv_macs(P, r.k2, dc2));   // mode 1: masked by act'(norm1(c1)) + statistics
+  emit_dgrad(P, r.k2, dc2, dz1, r.n1, r.c1, kNone, false);   // mode 1: masked by act'(norm1(c1)) + statistics
   TRef dc1 = full(P, new_buf(P, N, D, H, W, C));
   emit_gn_bwd(P, r.n1, dz1, r.c1, kNone, dc1, false);
   emit_wgrad(P, r.k1, r.X, dc1);
@@ -1003,14 +1050,14 @@ static TRef build_dyn_block_bwd(Plan& P, const DynBlock& r, TRef g1, TRef g2) {
     if (P.input_grad) {
       const Buf& xb = P.bufs[r.X.buf];
       TRef dX = full(P, new_buf(P, N, xb.D, xb.H, xb.W, r.X.c));
-      emit_dgrad(P, r.k1, dc1, dX, -1, kNone, kNone, false, 0.0, r.stride == 2, &P.igrad);
+      emit_dgrad(P, r.k1, dc1, dX, -1, kNone, kNone, false, /*reads_input=*/true, &P.igrad);
       emit_input_grad(P, -1, kNone, kNone, dX);
     }
     return kNone;
   }
   const Buf& xb = P.bufs[r.X.buf];
   TRef dX = full(P, new_buf(P, N, xb.D, xb.H, xb.W, r.X.c));
-  emit_dgrad(P, r.k1, dc1, dX, -1, kNone, kNone, false, conv_macs(P, r.k1, dc1), /*cls_mode=*/r.stride == 2);
+  emit_dgrad(P, r.k1, dc1, dX, -1, kNone, kNone, false);
   return dX;
 }
 
@@ -1022,19 +1069,12 @@ static int build_dynunet(Plan& P) {
   B200_REQUIRE(d.n_outputs >= 1 && d.n_outputs <= B200_HEAD_MAX_OUTPUTS, E_UNSUPPORTED, "plan: out_channels=%d unsupported (1..%d)",
                d.n_outputs, B200_HEAD_MAX_OUTPUTS);
   std::vector<int> F, Ds, Hs, Ws;
-  {
-    int D = d.depth, H = d.height, W = d.width;
-    for (int i = 0; i < L; ++i) {
-      B200_REQUIRE(d.filters[i] >= 8 && d.filters[i] % 8 == 0, E_UNSUPPORTED, "plan: filters[%d]=%d must be a positive multiple of 8", i,
-                   d.filters[i]);
-      F.push_back(d.filters[i]); Ds.push_back(D); Hs.push_back(H); Ws.push_back(W);
-      if (i + 1 < L)
-        B200_REQUIRE(D % 2 == 0 && H % 2 == 0 && W % 2 == 0 && D >= 2 && H >= 2 && W >= 2, E_UNSUPPORTED,
-                     "plan: level %d extent %dx%dx%d must be even (input %dx%dx%d not divisible by 2^%d)", i, D, H, W, d.depth,
-                     d.height, d.width, L - 1);
-      D /= 2; H /= 2; W /= 2;
-    }
+  for (int i = 0; i < L; ++i) {
+    B200_REQUIRE(d.filters[i] >= 8 && d.filters[i] % 8 == 0, E_UNSUPPORTED, "plan: filters[%d]=%d must be a positive multiple of 8", i,
+                 d.filters[i]);
+    F.push_back(d.filters[i]);
   }
+  B200_TRY(level_extents(d, Ds, Hs, Ws));
   // ---- parameter spec in MONAI's registration order: input_block, downsamples, bottleneck, upsamples, output_block
   auto enc_name = [&](int i) -> std::string {
     return i == 0 ? "input_block" : i == L - 1 ? "bottleneck" : "downsamples." + std::to_string(i - 1);
@@ -1068,26 +1108,8 @@ static int build_dynunet(Plan& P) {
   for (int u = 0; u + 1 < L; ++u) {
     const int lo = L - 1 - u, hi = L - 2 - u;
     const std::string pre = "upsamples." + std::to_string(u);
-    up[hi] = new_conv(P, pre + ".transp_conv.conv.weight", F[hi], F[lo], 2, 2, true);
-    P.convs[up[hi]].up2 = true;
-    TRef U = slice(full(P, cat[hi]), 0, F[hi]);
-    {
-      const int ci = up[hi];
-      TRef Xin = X;
-      P.macs[CAT_CONV_FWD] += (double)N * Ds[lo] * Hs[lo] * Ws[lo] * F[lo] * F[hi] * 8;
-      push_op(P.fwd, "convT_k2s2 " + P.convs[ci].name + " " + shape_of(P, Xin) + "->" + shape_of(P, U), [&P, ci, Xin, U](RunCtx& cx) -> int {
-        const ConvLayer& c = P.convs[ci];
-        ConvOp op;
-        memset(&op, 0, sizeof(op));
-        op.nsrc = 1;
-        op.cls_mode = 2;
-        op.src[0] = conv_src(P, cx, c, Xin, false);
-        op.Cop = c.Cop;
-        op.out = act_of(P, cx, U);
-        LAUNCHED(cx, CAT_CONV_FWD, launch_igemm_conv(op, cx.st));
-        return OK;
-      });
-    }
+    up[hi] = new_conv(P, pre + ".transp_conv.conv.weight", F[hi], F[lo], 2, 2, true, LAYER_CONVT_K2S2);
+    emit_conv_fwd(P, up[hi], X, -1, kNone, kNone, slice(full(P, cat[hi]), 0, F[hi]), false, false);
     release_if_whole(P, X);
     TRef dest = full(P, new_buf(P, N, Ds[hi], Hs[hi], Ws[hi], F[hi]));
     dec[hi] = build_dyn_block_fwd(P, pre + ".conv_block", full(P, cat[hi]), 2 * F[hi], F[hi], 1, dest, false, /*x_dead=*/true);
@@ -1107,38 +1129,14 @@ static int build_dynunet(Plan& P) {
     TRef dCat = build_dyn_block_bwd(P, dec[hi], g, kNone);
     dskip[hi] = slice(dCat, F[hi], F[hi]);
     TRef dU = slice(dCat, 0, F[hi]);
-    const int ci = up[hi];
     // input of the transposed convolution: the activated output of the stage below (or of the bottleneck)
     const TRef Xlow = (lo == L - 1) ? enc[lo].out : dec[lo].out;
-    P.macs[CAT_CONV_WGRAD] += (double)N * Ds[lo] * Hs[lo] * Ws[lo] * F[lo] * F[hi] * 8;
-    size_wgrad_partials(P, shape_act(P, dU), shape_act(P, Xlow), 2, 2, 1, P.convs[ci].Cop, P.convs[ci].Cip);
-    push_op(P.bwd, "wgrad_up2 " + P.convs[ci].name, [&P, ci, Xlow, dU](RunCtx& cx) -> int {
-      // dW[ci][co][t] = sum_j X[j][ci] dU[2j + t][co]: the weight gradient of the kernel-2 stride-2 convolution that maps the
-      // FINE grid (dU, "input", channels co) to the COARSE grid (X, "output gradient", channels ci): accumulator [T][pad(Co)][pad(Ci)]
-      const ConvLayer& c = P.convs[ci];
-      WgradOp op;
-  memset(&op, 0, sizeof(op));
-      op.a = act_of(P, cx, dU);
-      op.dy = act_of(P, cx, Xlow);
-      op.ksz = 2; op.stride = 2; op.nopad = 1; op.Cip = c.Cop; op.Cop = c.Cip;
-      op.dw = reinterpret_cast<float*>(cx.ws + P.bz_off + c.dw);
-      return run_wgrad(P, cx, op);
-    });
+    // dW[ci][co][t] = sum_j X[j][ci] dU[2j + t][co]
+    emit_wgrad(P, up[hi], Xlow, dU);
     const Buf lb = P.bufs[Xlow.buf];
     TRef gX = full(P, new_buf(P, N, lb.D, lb.H, lb.W, F[lo]));
-    P.macs[CAT_CONV_DGRAD] += (double)N * Ds[lo] * Hs[lo] * Ws[lo] * F[lo] * F[hi] * 8;
-    push_op(P.bwd, "dgrad_up2 " + P.convs[ci].name, [&P, ci, dU, gX](RunCtx& cx) -> int {
-      // dX[j][ci] = sum_t sum_co dU[2j + t][co] W[ci][co][t]: a kernel-2 stride-2 unpadded convolution of dU with the mode-3 pack
-      const ConvLayer& c = P.convs[ci];
-      ConvOp op;
-      memset(&op, 0, sizeof(op));
-      op.nsrc = 1;
-      op.src[0] = conv_src(P, cx, c, dU, true);
-      op.Cop = c.Cip;
-      op.out = act_of(P, cx, gX);
-      LAUNCHED(cx, CAT_CONV_DGRAD, launch_igemm_conv(op, cx.st));
-      return OK;
-    });
+    // dX[j][ci] = sum_t sum_co dU[2j + t][co] W[ci][co][t]: a kernel-2 stride-2 unpadded convolution of dU
+    emit_dgrad(P, up[hi], dU, gX, -1, kNone, kNone, false);
     g = gX;
   }
   // g = gradient of the bottleneck output; encoder, bottom to top: skip gradient + gradient through the stride-2 conv below

@@ -20,9 +20,9 @@ template <int TC>
 __device__ __forceinline__ void pack_job_tiled(float (&tile)[PT][PT + 1][PTT], const PackJob& j, const float* __restrict__ w,
                                                bf16* __restrict__ hi, bf16* __restrict__ lo) {
   const int T = TC ? TC : j.T;
-  const bool tsrc = j.mode >= 2;                       // ConvTranspose3d weight [Ci][Co][T]
-  const bool flip = j.mode == 1 || j.mode == 2;
-  const bool co_inner = j.mode == 1 || j.mode == 3;    // data-gradient layout [T][Cip][Cop]
+  const bool tsrc = j.mode >= PACK_T_FLIPPED;                           // ConvTranspose3d weight [Ci][Co][T]
+  const bool flip = j.mode == PACK_DGRAD || j.mode == PACK_T_FLIPPED;
+  const bool co_inner = j.mode == PACK_DGRAD || j.mode == PACK_T_DGRAD;   // data-gradient layout [T][Cip][Cop]
   const int nco = (j.Cop + PT - 1) / PT, nci = (j.Cip + PT - 1) / PT;
   for (int tl = blockIdx.x; tl < nco * nci; tl += gridDim.x) {
     const int co0 = (tl / nci) * PT, ci0 = (tl % nci) * PT;
@@ -92,7 +92,7 @@ template <int TC>
 __device__ __forceinline__ void unpack_job_tiled(float (&tile)[PT][PT + 1][PTT], const PackJob& j, const float* __restrict__ g,
                                                  float* __restrict__ out) {
   const int T = TC ? TC : j.T;
-  const bool tdst = j.mode == 2;   // ConvTranspose3d gradient layout [Ci][Co][T], taps flipped back
+  const bool tdst = j.mode == PACK_T_FLIPPED;   // ConvTranspose3d gradient layout [Ci][Co][T], taps flipped back
   const int nco = (j.Co + PT - 1) / PT, nci = (j.Ci + PT - 1) / PT;
   for (int tl = blockIdx.x; tl < nco * nci; tl += gridDim.x) {
     const int co0 = (tl / nci) * PT, ci0 = (tl % nci) * PT;
@@ -163,7 +163,7 @@ static int check_pack_shape(const char* what, int Cop, int Cip, int T) {
 
 int launch_pack_weights(const float* w, int Co, int Ci, int Cop, int Cip, int T, int mode, bf16* hi, bf16* lo, cudaStream_t st) {
   B200_TRY(check_pack_shape("pack_weights", Cop, Cip, T));
-  B200_REQUIRE(mode >= 0 && mode <= 4, E_INVALID, "pack_weights: mode=%d", mode);
+  B200_REQUIRE(mode >= PACK_FWD && mode <= PACK_T_FWD, E_INVALID, "pack_weights: mode=%d", mode);
   const PackJob j = {0, Co, Ci, Cop, Cip, T, mode, 0, 0};
   k_pack_job_tiled<<<256, 256, 0, st>>>(j, w, hi, lo);
   B200_CHECK_CUDA(cudaGetLastError());
@@ -172,7 +172,7 @@ int launch_pack_weights(const float* w, int Co, int Ci, int Cop, int Cip, int T,
 
 int launch_unpack_wgrad(const float* g, int Co, int Ci, int Cop, int Cip, int T, int mode, float* out, cudaStream_t st) {
   B200_TRY(check_pack_shape("unpack_wgrad", Cop, Cip, T));
-  B200_REQUIRE(mode == 0 || mode == 2, E_INVALID, "unpack_wgrad: mode=%d (0 or 2)", mode);
+  B200_REQUIRE(mode == PACK_FWD || mode == PACK_T_FLIPPED, E_INVALID, "unpack_wgrad: mode=%d (0 or 2)", mode);
   const PackJob j = {0, Co, Ci, Cop, Cip, T, mode, 0, 0};
   k_unpack_job_tiled<<<256, 256, 0, st>>>(j, g, out);
   B200_CHECK_CUDA(cudaGetLastError());
