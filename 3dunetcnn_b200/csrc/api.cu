@@ -164,6 +164,13 @@ int b200unet_upsample2x_fwd(const b200unet_tensor* x, const b200unet_tensor* y, 
   NOT_NULL(x); NOT_NULL(y);
   return launch_upsample2x_fwd(to_act(x), to_act(y), stats, stats_ld, to_stream(stream));
 }
+int b200unet_upsample2x_add_fwd(const b200unet_tensor* x, const b200unet_tensor* add, const b200unet_tensor* y, double* stats,
+                                int stats_ld, void* stream) {
+  NOT_NULL(x); NOT_NULL(y);
+  Act a;
+  if (add) a = to_act(add);
+  return launch_upsample2x_fwd(to_act(x), to_act(y), stats, stats_ld, to_stream(stream), add ? &a : nullptr);
+}
 int b200unet_upsample2x_bwd(const b200unet_tensor* dy, const b200unet_tensor* dx, void* stream) {
   NOT_NULL(dy); NOT_NULL(dx);
   return launch_upsample2x_bwd(to_act(dy), to_act(dx), to_stream(stream));

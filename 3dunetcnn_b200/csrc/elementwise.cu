@@ -486,7 +486,10 @@ __device__ __forceinline__ void up_taps(int o, int n, int& i0, int& i1, float& w
 // Each thread produces a 2x2x2 block of outputs (o = 2k+1, 2k+2 per axis, k in [-1, n-1]) from the 2x2x2 block of
 // inputs (clamp(k), clamp(k+1)): 8 loads for 8 outputs instead of 8 loads per output.  grid (blocks, N); the 8-channel
 // chunk is constant per thread, so the per-channel statistics accumulate in registers.
-__global__ void __launch_bounds__(256) k_upsample2x_fwd(Act x, Act y, double* __restrict__ stats, int stats_ld) {
+// ADD: y = upsample(x) + add (SegResNet's additive skip), the statistics taken of the sum; one full-resolution write and
+// re-read fewer than an up-sampling followed by an add.
+template <bool ADD>
+__global__ void __launch_bounds__(256) k_upsample2x_fwd(Act x, Act y, double* __restrict__ stats, int stats_ld, Act add) {
   const int c8n = x.C / 8;
   extern __shared__ double smu[];  // [C][2], fp64: atomic order must not reach the fp32 coefficients
   if (stats) {
@@ -528,6 +531,12 @@ __global__ void __launch_bounds__(256) k_upsample2x_fwd(Act x, Act y, double* __
 #pragma unroll
         for (int j = 0; j < 8; ++j) r[j] = fmaf(wt, v[i][j], r[j]);
       }
+      if (ADD) {
+        float s[8];
+        load8(add.hi, add.lo, ((((long long)n * add.D + od) * add.H + oh) * add.W + ow) * add.ld + c8 * 8, s);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) r[j] += s[j];
+      }
       store8(y.hi, y.lo, ((((long long)n * y.D + od) * y.H + oh) * y.W + ow) * y.ld + c8 * 8, r);
 #pragma unroll
       for (int j = 0; j < 8; ++j) { a[j] += r[j]; b[j] = fmaf(r[j], r[j], b[j]); }
@@ -557,10 +566,14 @@ __global__ void __launch_bounds__(256) k_upsample2x_fwd(Act x, Act y, double* __
   }
 }
 
-int launch_upsample2x_fwd(const Act& x, const Act& y, double* stats, int stats_ld, cudaStream_t st) {
+int launch_upsample2x_fwd(const Act& x, const Act& y, double* stats, int stats_ld, cudaStream_t st, const Act* add) {
   B200_REQUIRE(x.C % 8 == 0 && y.C == x.C, E_INVALID, "upsample: channel mismatch");
   B200_REQUIRE(y.D == 2 * x.D && y.H == 2 * x.H && y.W == 2 * x.W, E_UNSUPPORTED,
                "upsample: output must be exactly 2x (got %dx%dx%d -> %dx%dx%d)", x.D, x.H, x.W, y.D, y.H, y.W);
+  if (add)
+    B200_REQUIRE(add->N == y.N && add->D == y.D && add->H == y.H && add->W == y.W && add->C == y.C && add->ld % 8 == 0, E_INVALID,
+                 "upsample: the addend must have the output's shape (%dx%dx%dx%dx%d, got %dx%dx%dx%dx%d)", y.N, y.D, y.H, y.W, y.C,
+                 add->N, add->D, add->H, add->W, add->C);
   const int c8n = x.C / 8;
   const int threads = ew_threads_for(c8n);
   B200_REQUIRE(threads <= 256, E_UNSUPPORTED, "upsample: C=%d unsupported (at most 2048 channels)", x.C);
@@ -570,7 +583,8 @@ int launch_upsample2x_fwd(const Act& x, const Act& y, double* stats, int stats_l
   long long want = (nblk + vper - 1) / vper;
   const long long cap = (132LL * 8 + x.N - 1) / x.N;
   const int blocks = (int)(want < cap ? (want > 0 ? want : 1) : cap);
-  k_upsample2x_fwd<<<dim3(blocks, x.N), threads, x.C * 2 * sizeof(double), st>>>(x, y, stats, stats_ld);
+  if (add) k_upsample2x_fwd<true><<<dim3(blocks, x.N), threads, x.C * 2 * sizeof(double), st>>>(x, y, stats, stats_ld, *add);
+  else k_upsample2x_fwd<false><<<dim3(blocks, x.N), threads, x.C * 2 * sizeof(double), st>>>(x, y, stats, stats_ld, Act());
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;
 }

@@ -16,7 +16,7 @@ int launch_gn_bwd(const Act& dz, const Act& x, const float* coef, const double* 
 // the same without dx (the first block's norm): dgamma, dbeta and (E, F) into coef2 [N][Cld][2] for launch_input_grad
 int launch_gn_bwd_finalize(const double* bstats, const float* coef, const float* gamma, int N, int C, int Cld, int G,
                            long long S, float* coef2, float* dgamma, float* dbeta, cudaStream_t st);
-int launch_upsample2x_fwd(const Act& x, const Act& y, double* stats, int stats_ld, cudaStream_t st);
+int launch_upsample2x_fwd(const Act& x, const Act& y, double* stats, int stats_ld, cudaStream_t st, const Act* add = nullptr);
 int launch_upsample2x_bwd(const Act& dy, const Act& dx, cudaStream_t st);
 // The 1x1x1 head takes 1..B200_HEAD_MAX_OUTPUTS outputs: 1..8 run the SIMT kernels below with fp32 weights, 9..128 the
 // tensor-core kernels of head.cu (launch_head_mma_*), chosen inside launch_head_fwd / launch_head_bwd from n_out alone.

@@ -645,18 +645,27 @@ static void emit_unpack_wgrads(Plan& P) {
 }
 
 // ------------------------------------------------------------------------------------------------ residual block
-static BlockRec build_block_fwd(Plan& P, const std::string& pre, TRef X, int cin_real, int C, TRef dest, bool want_stats,
+// state-dict keys of a pre-activation residual block: its two norms (prefixes of .weight / .bias), its two 3x3x3 convolutions
+// and the 1x1x1 `sample` convolution it has when it changes the width
+struct BlockKeys {
+  std::string n1, c1, n2, c2, sample;
+};
+static BlockKeys unet3d_block_keys(const std::string& pre) {   // classification/myronenko.py:34-58
+  return {pre + ".conv1.norm1", pre + ".conv1.conv.weight", pre + ".conv2.norm1", pre + ".conv2.conv.weight", pre + ".sample.weight"};
+}
+
+static BlockRec build_block_fwd(Plan& P, const BlockKeys& k, TRef X, int cin_real, int C, TRef dest, bool want_stats,
                                 bool first, bool scale_out, bool scale_in, bool x_dead) {
   const Buf& xb = P.bufs[X.buf];
   const int N = xb.N, D = xb.D, H = xb.H, W = xb.W;
   const long long S = (long long)D * H * W;
   BlockRec r;
   r.X = X; r.first = first; r.scale_out = scale_out; r.scale_in = scale_in;
-  r.n1 = new_norm(P, pre + ".conv1.norm1", cin_real, X.c, S);
-  r.c1 = new_conv(P, pre + ".conv1.conv.weight", C, cin_real, 3, 1, true);
-  r.n2 = new_norm(P, pre + ".conv2.norm1", C, C, S);
-  r.c2 = new_conv(P, pre + ".conv2.conv.weight", C, C, 3, 1, true);
-  r.cs = (cin_real != C) ? new_conv(P, pre + ".sample.weight", C, cin_real, 1, 1, !first || P.input_grad) : -1;
+  r.n1 = new_norm(P, k.n1, cin_real, X.c, S);
+  r.c1 = new_conv(P, k.c1, C, cin_real, 3, 1, true);
+  r.n2 = new_norm(P, k.n2, C, C, S);
+  r.c2 = new_conv(P, k.c2, C, C, 3, 1, true);
+  r.cs = (cin_real != C) ? new_conv(P, k.sample, C, cin_real, 1, 1, !first || P.input_grad) : -1;
   r.a1 = full(P, new_buf(P, N, D, H, W, X.c));
   r.y1 = full(P, new_buf(P, N, D, H, W, C));
   r.a2 = full(P, new_buf(P, N, D, H, W, C));
@@ -784,7 +793,7 @@ static int build_unet3d(Plan& P) {
       if (last && li + 1 < L) { dest = slice(full(P, cat[li]), C, C); want_stats = true; }
       else { dest = full(P, new_buf(P, N, Ds[li], Hs[li], Ws[li], C)); want_stats = true; }
       const bool first = (li == 0 && b == 0);
-      enc[li].push_back(build_block_fwd(P, "encoder.layers." + std::to_string(li) + ".blocks." + std::to_string(b), X,
+      enc[li].push_back(build_block_fwd(P, unet3d_block_keys("encoder.layers." + std::to_string(li) + ".blocks." + std::to_string(b)), X,
                                         cin_real, C, dest, want_stats, first, /*scale_out=*/first,
                                         /*scale_in=*/(li == 0 && b == 1), /*x_dead=*/true));
       X = dest;
@@ -807,7 +816,7 @@ static int build_unet3d(Plan& P) {
     const Buf xb = P.bufs[X.buf];
     for (int b = 0; b < d.decoder_blocks[i]; ++b) {
       TRef dest = full(P, new_buf(P, N, xb.D, xb.H, xb.W, in_w));
-      dec[i].push_back(build_block_fwd(P, "decoder.layers." + std::to_string(i) + ".blocks." + std::to_string(b), X, in_w,
+      dec[i].push_back(build_block_fwd(P, unet3d_block_keys("decoder.layers." + std::to_string(i) + ".blocks." + std::to_string(b)), X, in_w,
                                        in_w, dest, /*want_stats=*/b + 1 < d.decoder_blocks[i], false, false, false, true));
       X = dest;
     }
@@ -856,7 +865,7 @@ static int build_unet3d(Plan& P) {
     int cin = X.c;
     for (int b = 0; b < d.decoder_blocks[L - 1]; ++b) {
       TRef dest = full(P, new_buf(P, N, xb.D, xb.H, xb.W, d.base_width));
-      dec[L - 1].push_back(build_block_fwd(P, "decoder.layers." + std::to_string(L - 1) + ".blocks." + std::to_string(b), X,
+      dec[L - 1].push_back(build_block_fwd(P, unet3d_block_keys("decoder.layers." + std::to_string(L - 1) + ".blocks." + std::to_string(b)), X,
                                            cin, d.base_width, dest, b + 1 < d.decoder_blocks[L - 1], false, false, false, true));
       X = dest;
       cin = d.base_width;
@@ -1150,7 +1159,188 @@ static int build_dynunet(Plan& P) {
   return finish_build(P);
 }
 
-static int build(Plan& P) { return P.d.arch == 1 ? build_dynunet(P) : build_unet3d(P); }
+// ================================================================================================ SegResNet (MONAI)
+// MONAI's SegResNet (Myronenko's BraTS 2018 network), absent from this image like DynUNet: restated from its public definition
+// (monai/networks/nets/segresnet.py, monai/networks/blocks/segresnet_block.py) -- parity unpinned, see oracle/segresnet_oracle.py.
+//   conv(ci, co, k = 3, s = 1, bias = False):  Conv3d, padding k // 2;  F = init_filters, L = len(blocks_down)
+//   ResBlock(C):   y = conv2(act(norm2(conv1(act(norm1(x)))))) + x,  GroupNorm(num_groups, C) affine eps 1e-5, C -> C 3x3x3 convs
+//   forward:       x = convInit(x) [-> Dropout3d(dropout_prob)];  level i: x = pre_conv_i(x) (Identity at i = 0, else conv(F 2^(i-1),
+//                  F 2^i, 3, stride 2)), then blocks_down[i] x ResBlock(F 2^i); down_x[i] = x.  Up stage i = 0..L-2, C = F 2^(L-2-i):
+//                  x = upsample2x(conv1x1(2C -> C)(x)) + down_x[L-2-i], then blocks_up[i] x ResBlock(C).
+//                  Head: conv_final = GroupNorm(F) -> act -> conv(F, out_channels, 1, bias = True).
+//   state dict (registration order): convInit.conv.weight; down_layers.{i}.0.conv.weight (i > 0), down_layers.{i}.{1..}.<ResBlock>;
+//                  up_layers.{i}.{0..}.<ResBlock>; up_samples.{i}.0.conv.weight [C, 2C, 1, 1, 1]; conv_final.0.weight / .bias,
+//                  conv_final.2.conv.weight / .bias.  <ResBlock> = norm1.weight, norm1.bias, norm2.weight, norm2.bias,
+//                  conv1.conv.weight, conv2.conv.weight.
+// Schedule: every op is one the UNet3D / DynUNet plans already run, except the up-sampling, which adds the skip in the same pass
+// (launch_upsample2x_fwd with an addend) and takes the statistics of the sum for the next ResBlock's norm1.
+static BlockKeys segres_block_keys(const std::string& pre) {
+  return {pre + ".norm1", pre + ".conv1.conv.weight", pre + ".norm2", pre + ".conv2.conv.weight", pre + ".sample"};
+}
+
+static void add_segres_block_params(Plan& P, const std::string& pre, int C) {
+  add_param(P, pre + ".norm1.weight", {C});
+  add_param(P, pre + ".norm1.bias", {C});
+  add_param(P, pre + ".norm2.weight", {C});
+  add_param(P, pre + ".norm2.bias", {C});
+  add_param(P, pre + ".conv1.conv.weight", {C, C, 3, 3, 3});
+  add_param(P, pre + ".conv2.conv.weight", {C, C, 3, 3, 3});
+}
+
+static int build_segresnet(Plan& P) {
+  const b200unet_net_desc& d = P.d;
+  const int L = d.n_levels, N = d.batch, F = d.base_width;
+  B200_REQUIRE(L >= 2 && L <= 8, E_UNSUPPORTED, "plan: SegResNet with %d levels unsupported (2..8)", L);
+  B200_REQUIRE(F >= 8 && F % 8 == 0, E_UNSUPPORTED, "plan: init_filters=%d must be a positive multiple of 8", F);
+  B200_REQUIRE(F << (L - 1) <= 1024, E_UNSUPPORTED, "plan: SegResNet widths up to %d channels unsupported (the norms take at most 1024)",
+               F << (L - 1));
+  B200_REQUIRE(d.norm_groups >= 1 && F % d.norm_groups == 0, E_UNSUPPORTED, "plan: num_groups=%d must divide init_filters=%d",
+               d.norm_groups, F);
+  B200_REQUIRE(d.n_features >= 1 && d.n_features <= 16, E_UNSUPPORTED, "plan: in_channels=%d unsupported", d.n_features);
+  B200_REQUIRE(d.n_outputs >= 1 && d.n_outputs <= B200_HEAD_MAX_OUTPUTS, E_UNSUPPORTED, "plan: out_channels=%d unsupported (1..%d)",
+               d.n_outputs, B200_HEAD_MAX_OUTPUTS);
+  for (int i = 0; i < L; ++i)
+    B200_REQUIRE(d.encoder_blocks[i] >= 1, E_UNSUPPORTED, "plan: blocks_down[%d]=%d must be at least 1", i, d.encoder_blocks[i]);
+  for (int i = 0; i + 1 < L; ++i)
+    B200_REQUIRE(d.decoder_blocks[i] >= 1, E_UNSUPPORTED, "plan: blocks_up[%d]=%d must be at least 1", i, d.decoder_blocks[i]);
+  std::vector<int> Wd, Ds, Hs, Ws;
+  for (int i = 0; i < L; ++i) Wd.push_back(F << i);
+  B200_TRY(level_extents(d, Ds, Hs, Ws));
+  auto down_name = [](int i, int j) { return "down_layers." + std::to_string(i) + "." + std::to_string(j); };
+  auto up_name = [](int i, int j) { return "up_layers." + std::to_string(i) + "." + std::to_string(j); };
+  auto up_conv_name = [](int i) { return "up_samples." + std::to_string(i) + ".0.conv.weight"; };
+
+  // ---- parameter spec in MONAI's registration order
+  add_param(P, "convInit.conv.weight", {F, d.n_features, 3, 3, 3});
+  for (int i = 0; i < L; ++i) {
+    if (i > 0) add_param(P, down_name(i, 0) + ".conv.weight", {Wd[i], Wd[i - 1], 3, 3, 3});
+    for (int b = 1; b <= d.encoder_blocks[i]; ++b) add_segres_block_params(P, down_name(i, b), Wd[i]);
+  }
+  for (int i = 0; i + 1 < L; ++i)
+    for (int b = 0; b < d.decoder_blocks[i]; ++b) add_segres_block_params(P, up_name(i, b), Wd[L - 2 - i]);
+  for (int i = 0; i + 1 < L; ++i) add_param(P, up_conv_name(i), {Wd[L - 2 - i], 2 * Wd[L - 2 - i], 1, 1, 1});
+  add_param(P, "conv_final.0.weight", {F});
+  add_param(P, "conv_final.0.bias", {F});
+  add_param(P, "conv_final.2.conv.weight", {d.n_outputs, F, 1, 1, 1});
+  add_param(P, "conv_final.2.conv.bias", {d.n_outputs});
+
+  // ---- forward
+  const int Cp_in = round_up(d.n_features, 8);
+  const int b_in = new_buf(P, N, Ds[0], Hs[0], Ws[0], Cp_in);
+  emit_prologue(P, b_in, /*with_input_stats=*/false);
+  // convInit, Dropout3d through the epilogue's per-(n, c) scale; the statistics are those of the scaled output
+  const int cinit = new_conv(P, "convInit.conv.weight", F, d.n_features, 3, 1, P.input_grad);
+  TRef X = full(P, new_buf(P, N, Ds[0], Hs[0], Ws[0], F));
+  emit_conv_fwd(P, cinit, full(P, b_in), -1, kNone, kNone, X, true, /*scale=*/true);
+  release_buf(P, b_in);
+  std::vector<std::vector<BlockRec>> enc(L), dec(L);
+  std::vector<int> pre(L, -1);
+  std::vector<TRef> down_x(L);
+  for (int i = 0; i < L; ++i) {
+    if (i > 0) {   // stride-2 convolution of the previous level's output, which stays live as the skip
+      pre[i] = new_conv(P, down_name(i, 0) + ".conv.weight", Wd[i], Wd[i - 1], 3, 2, true);
+      TRef Y = full(P, new_buf(P, N, Ds[i], Hs[i], Ws[i], Wd[i]));
+      emit_conv_fwd(P, pre[i], X, -1, kNone, kNone, Y, true, false);
+      X = Y;
+    }
+    const int nb = d.encoder_blocks[i];
+    for (int b = 0; b < nb; ++b) {
+      // the level output feeds a convolution, not a norm: no statistics
+      TRef dest = full(P, new_buf(P, N, Ds[i], Hs[i], Ws[i], Wd[i]));
+      enc[i].push_back(build_block_fwd(P, segres_block_keys(down_name(i, b + 1)), X, Wd[i], Wd[i], dest, /*want_stats=*/b + 1 < nb,
+                                       false, false, /*scale_in=*/i == 0 && b == 0, /*x_dead=*/true));
+      X = dest;
+    }
+    down_x[i] = X;
+  }
+  std::vector<int> upc(L, -1);
+  std::vector<TRef> up_in(L), up_p(L), up_y(L);
+  for (int i = 0; i + 1 < L; ++i) {
+    const int j = L - 2 - i, C = Wd[j];
+    upc[i] = new_conv(P, up_conv_name(i), C, 2 * C, 1, 1, true);
+    up_in[i] = X;
+    up_p[i] = full(P, new_buf(P, N, Ds[j + 1], Hs[j + 1], Ws[j + 1], C));
+    emit_conv_fwd(P, upc[i], X, -1, kNone, kNone, up_p[i], false, false);
+    release_if_whole(P, X);
+    up_y[i] = full(P, new_buf(P, N, Ds[j], Hs[j], Ws[j], C));
+    need_stats(P, up_y[i].buf);
+    const TRef Pin = up_p[i], Sk = down_x[j], Y = up_y[i];
+    push_op(P.fwd, "upsample2x_fwd+skip " + shape_of(P, Pin), [&P, Pin, Sk, Y](RunCtx& cx) -> int {
+      const Act sk = act_of(P, cx, Sk);
+      LAUNCHED(cx, CAT_RESAMPLE, launch_upsample2x_fwd(act_of(P, cx, Pin), act_of(P, cx, Y), stats_ptr(P, cx, Y), P.bufs[Y.buf].C, cx.st, &sk));
+      return OK;
+    });
+    release_buf(P, up_p[i].buf);
+    release_if_whole(P, down_x[j]);
+    X = up_y[i];
+    const int nb = d.decoder_blocks[i];
+    for (int b = 0; b < nb; ++b) {
+      // the last stage's output feeds the head's GroupNorm; the other stages' feed a 1x1x1 convolution
+      TRef dest = full(P, new_buf(P, N, Ds[j], Hs[j], Ws[j], C));
+      dec[i].push_back(build_block_fwd(P, segres_block_keys(up_name(i, b)), X, C, C, dest, /*want_stats=*/b + 1 < nb || j == 0,
+                                       false, false, false, /*x_dead=*/true));
+      X = dest;
+    }
+  }
+  // head: GroupNorm + act into a buffer, then the biased 1x1x1 head
+  const int nf = new_norm(P, "conv_final.0", F, F, (long long)Ds[0] * Hs[0] * Ws[0]);
+  const TRef A = full(P, new_buf(P, N, Ds[0], Hs[0], Ws[0], F));
+  emit_norm_fwd(P, nf, X, A);
+  release_if_whole(P, X);
+  if (!P.infer) {
+    B200_REQUIRE(d.activation == 0, E_UNSUPPORTED, "plan: activation inside the model is inference-only; train on logits");
+    emit_bwd_memset(P);
+  }
+  TRef g = emit_head(P, A, P.find_param("conv_final.2.conv.weight"), P.find_param("conv_final.2.conv.bias"));
+  if (P.infer) return finish_build(P);
+
+  // ---- backward
+  {
+    TRef dz = full(P, new_buf(P, N, Ds[0], Hs[0], Ws[0], F));
+    emit_act_bwd(P, nf, g, kNone, X, dz);
+    TRef dX = full(P, new_buf(P, N, Ds[0], Hs[0], Ws[0], F));
+    emit_gn_bwd(P, nf, dz, X, kNone, dX, false);
+    g = dX;
+  }
+  std::vector<TRef> dskip(L, kNone);
+  for (int i = L - 2; i >= 0; --i) {   // up stages, top to bottom
+    const int j = L - 2 - i, C = Wd[j];
+    for (int b = d.decoder_blocks[i] - 1; b >= 0; --b) g = build_block_bwd(P, dec[i][b], g);
+    // d(up(p) + skip): unchanged to the skip, through the adjoint of the up-sampling to the 1x1x1 convolution
+    dskip[j] = g;
+    TRef dP = full(P, new_buf(P, N, Ds[j + 1], Hs[j + 1], Ws[j + 1], C));
+    push_op(P.bwd, "upsample2x_bwd " + shape_of(P, dP), [&P, g, dP](RunCtx& cx) -> int {
+      LAUNCHED(cx, CAT_RESAMPLE, launch_upsample2x_bwd(act_of(P, cx, g), act_of(P, cx, dP), cx.st));
+      return OK;
+    });
+    emit_wgrad(P, upc[i], up_in[i], dP);
+    TRef gX = full(P, new_buf(P, N, Ds[j + 1], Hs[j + 1], Ws[j + 1], 2 * C));
+    emit_dgrad(P, upc[i], dP, gX, -1, kNone, kNone, false);
+    g = gX;
+  }
+  // g = gradient of the bottom level's output; encoder, bottom to top
+  for (int i = L - 1; i >= 0; --i) {
+    for (int b = d.encoder_blocks[i] - 1; b >= 0; --b) g = build_block_bwd(P, enc[i][b], g);
+    if (i > 0) {
+      // the level below's output gets the parity-class data gradient of this level's stride-2 convolution + its skip gradient
+      emit_wgrad(P, pre[i], down_x[i - 1], g);
+      TRef gS = full(P, new_buf(P, N, Ds[i - 1], Hs[i - 1], Ws[i - 1], Wd[i - 1]));
+      emit_dgrad(P, pre[i], g, gS, -1, kNone, dskip[i - 1], false);
+      g = gS;
+    }
+  }
+  // g = gradient of convInit's output (the first ResBlock applied the dropout scale to it)
+  emit_wgrad(P, cinit, full(P, b_in), g);
+  if (P.input_grad) {
+    TRef dX = full(P, new_buf(P, N, Ds[0], Hs[0], Ws[0], Cp_in));
+    emit_dgrad(P, cinit, g, dX, -1, kNone, kNone, false, /*reads_input=*/true, &P.igrad);
+    emit_input_grad(P, -1, kNone, kNone, dX);
+  }
+  emit_unpack_wgrads(P);
+  return finish_build(P);
+}
+
+static int build(Plan& P) { return P.d.arch == 2 ? build_segresnet(P) : P.d.arch == 1 ? build_dynunet(P) : build_unet3d(P); }
 
 // runs ops [first, last) of a schedule.  B200UNET_CAPTURE_DEBUG=1: after every op, check whether it invalidated an ongoing
 // CUDA-graph capture of the stream, and name it if so.

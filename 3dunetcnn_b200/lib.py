@@ -120,6 +120,8 @@ _SIGS = {
     "b200unet_gn_bwd": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                   C.c_void_p, C.c_void_p, C.POINTER(Tensor5), C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p]),
     "b200unet_upsample2x_fwd": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_int, C.c_void_p]),
+    "b200unet_upsample2x_add_fwd": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_int,
+                                              C.c_void_p]),
     "b200unet_upsample2x_bwd": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p]),
     "b200unet_zero_insert": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "b200unet_head_fwd": (C.c_int, [C.POINTER(Tensor5), C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
@@ -521,9 +523,14 @@ def act_bwd(g1: Act, g2: Optional[Act], c: Act, coef, slope: float, dz: Act, bst
                                           slope, C.byref(dz.ct()), bstats.data_ptr(), bstats_ld, stream_ptr()), "act_bwd")
 
 
-def upsample2x_fwd(x: Act, y: Act, stats=None, stats_ld=0) -> None:
-    check(load_library().b200unet_upsample2x_fwd(C.byref(x.ct()), C.byref(y.ct()), _p(stats), stats_ld, stream_ptr()),
-          "upsample2x_fwd")
+def upsample2x_fwd(x: Act, y: Act, stats=None, stats_ld=0, add: Optional[Act] = None) -> None:
+    """y = trilinear x2 of x (+ add, of y's shape), with the per-channel (sum, sumsq) of y into stats when given"""
+    if add is None:
+        check(load_library().b200unet_upsample2x_fwd(C.byref(x.ct()), C.byref(y.ct()), _p(stats), stats_ld, stream_ptr()),
+              "upsample2x_fwd")
+        return
+    check(load_library().b200unet_upsample2x_add_fwd(C.byref(x.ct()), C.byref(add.ct()), C.byref(y.ct()), _p(stats), stats_ld,
+                                                     stream_ptr()), "upsample2x_add_fwd")
 
 
 def upsample2x_bwd(dy: Act, dx: Act) -> None:

@@ -210,6 +210,23 @@ class _PlanModel(nn.Module):
         sd = dict(self.named_parameters())
         return [sd[k] for k in self._keys]
 
+    # ------------------------------------------------------------------ Dropout3d on the first feature map
+    dropout_p = 0.0          # subclasses with a Dropout3d set it and dropout_width (the channels it drops)
+    dropout_width = 0
+
+    def set_dropout_scale(self, scale: Optional[torch.Tensor]) -> None:
+        """Testing hook: force the (N, C0) Dropout3d channel scale used by the next training forwards."""
+        self._forced_dropout_scale = scale
+
+    def _dropout_scale(self, xp: torch.Tensor) -> Optional[torch.Tensor]:
+        """(N, dropout_width) per-channel Dropout3d scale of a training forward (keep / (1 - p), or the forced one); None in eval"""
+        if not (self.training and self.dropout_p > 0):
+            return None
+        if self._forced_dropout_scale is not None:
+            return self._forced_dropout_scale.to(device=xp.device, dtype=torch.float32).contiguous()
+        keep = (torch.rand((xp.shape[0], self.dropout_width), device=xp.device) >= self.dropout_p)
+        return keep.float() / (1.0 - self.dropout_p)
+
     # ------------------------------------------------------------------ plan cache
     def _plan_for(self, x: torch.Tensor, inference_only: bool = False, input_grad: bool = False) -> _Plan:
         n, _, d, h, w = x.shape
@@ -421,22 +438,11 @@ class UNet3D(_PlanModel):
         nd.batch, nd.depth, nd.height, nd.width = n, d, h, w
         return nd
 
-    def set_dropout_scale(self, scale: Optional[torch.Tensor]) -> None:
-        """Testing hook: force the (N, C0) Dropout3d channel scale used by the next training forwards."""
-        self._forced_dropout_scale = scale
-
     # ------------------------------------------------------------------ forward
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         xp = self._check_input(x, self.n_features)
         params = self.ordered_parameters()
-        drop = None
-        if self.training and self.dropout_p > 0:
-            if self._forced_dropout_scale is not None:
-                drop = self._forced_dropout_scale.to(device=xp.device, dtype=torch.float32).contiguous()
-            else:
-                keep = (torch.rand((xp.shape[0], self.base_width), device=xp.device) >= self.dropout_p)
-                drop = keep.float() / (1.0 - self.dropout_p)
-        return _UNetFunction.apply(self, xp, drop, *self._needs_backward(params, xp), *params)
+        return _UNetFunction.apply(self, xp, self._dropout_scale(xp), *self._needs_backward(params, xp), *params)
 
 
 class AutocastUNet(UNet3D):
@@ -569,8 +575,138 @@ class DynUNet(_PlanModel):
         return _UNetFunction.apply(self, xp, None, *self._needs_backward(params, xp), *params)
 
 
+def _name_and_args(v, what):
+    """MONAI's layer spelling: "name" or ("name", {kwargs}) -> (lower-case name, kwargs)"""
+    if isinstance(v, str):
+        return v.lower(), {}
+    if isinstance(v, (tuple, list)) and len(v) == 2 and isinstance(v[0], str) and isinstance(v[1], dict):
+        return v[0].lower(), dict(v[1])
+    if isinstance(v, (tuple, list)) and len(v) == 1 and isinstance(v[0], str):
+        return v[0].lower(), {}
+    raise NotImplementedError("B200 SegResNet: %s=%r (a name or a (name, kwargs) pair)" % (what, v))
+
+
+class SegResNet(_PlanModel):
+    """Drop-in for ``monai.networks.nets.SegResNet`` (Myronenko's BraTS 2018 network), which the reference builds by name
+    through the ``from monai.networks.nets import *`` in unet3d/models/pytorch/__init__.py:1.
+
+    MONAI's kwargs; implemented: ``spatial_dims=3``, ``init_filters`` a multiple of 8, GroupNorm (``norm=("GROUP",
+    {"num_groups": G})``, ``"group"``, or the legacy ``norm_name="group"`` + ``num_groups``), ReLU or LeakyReLU, ``dropout_prob``
+    (Dropout3d on convInit's output), ``use_conv_final=True``, ``upsample_mode="nontrainable"`` (trilinear x2); anything else
+    raises.  State-dict keys and order are MONAI's (convInit / down_layers / up_layers / up_samples / conv_final), so MONAI
+    checkpoints load with ``strict=True`` (parity with MONAI itself is unpinned: it is absent from this image)."""
+
+    def __init__(self, spatial_dims=3, init_filters=8, in_channels=1, out_channels=2, dropout_prob=None,
+                 act=("RELU", {"inplace": True}), norm=("GROUP", {"num_groups": 8}), norm_name="", num_groups=8,
+                 use_conv_final=True, blocks_down=(1, 2, 2, 4), blocks_up=(1, 1, 1), upsample_mode="nontrainable",
+                 precision: Optional[str] = None, deterministic: Optional[bool] = None):
+        super().__init__()
+        if spatial_dims != 3:
+            raise NotImplementedError("B200 SegResNet: spatial_dims=%r (only 3)" % (spatial_dims,))
+        mode = str(getattr(upsample_mode, "value", upsample_mode)).lower()
+        if mode != "nontrainable":
+            raise NotImplementedError("B200 SegResNet: upsample_mode=%r (only 'nontrainable': trilinear x2)" % (upsample_mode,))
+        if not use_conv_final:
+            raise NotImplementedError("B200 SegResNet: use_conv_final=False (the plan always runs the head)")
+        if norm_name:                                       # MONAI's deprecated spelling
+            if str(norm_name).lower() != "group":
+                raise NotImplementedError("B200 SegResNet: norm_name=%r (only 'group')" % (norm_name,))
+            norm = ("group", {"num_groups": num_groups})
+        norm_type, norm_kw = _name_and_args(norm, "norm")
+        if norm_type != "group":
+            raise NotImplementedError("B200 SegResNet: norm=%r (only GROUP)" % (norm,))
+        groups = int(norm_kw.pop("num_groups", num_groups))
+        if float(norm_kw.pop("eps", 1e-5)) != 1e-5 or not norm_kw.pop("affine", True) or norm_kw:
+            raise NotImplementedError("B200 SegResNet: GroupNorm options %r (only num_groups, eps 1e-5, affine)" % (norm,))
+        act_type, act_kw = _name_and_args(act, "act")
+        act_kw.pop("inplace", None)
+        if act_type == "relu" and not act_kw:
+            slope = 0.0
+        elif act_type == "leakyrelu" and set(act_kw) <= {"negative_slope"}:
+            slope = float(act_kw.get("negative_slope", 0.01))
+        else:
+            raise NotImplementedError("B200 SegResNet: act=%r (only relu / leakyrelu)" % (act,))
+        blocks_down, blocks_up = [int(b) for b in blocks_down], [int(b) for b in blocks_up]
+        if any(b < 1 for b in blocks_down + blocks_up):
+            raise NotImplementedError("B200 SegResNet: blocks_down=%r blocks_up=%r (every stage needs a block)" % (blocks_down, blocks_up))
+        if len(blocks_up) != len(blocks_down) - 1:
+            raise NotImplementedError("B200 SegResNet: len(blocks_up) must be len(blocks_down) - 1 (got %d, %d)"
+                                      % (len(blocks_up), len(blocks_down)))
+        if not 2 <= len(blocks_down) <= 8:
+            raise NotImplementedError("B200 SegResNet: 2..8 levels")
+        init_filters = int(init_filters)
+        if groups < 1 or init_filters % groups:
+            raise ValueError("num_channels must be divisible by num_groups (init_filters=%d, num_groups=%d)" % (init_filters, groups))
+        self.spatial_dims = 3
+        self.init_filters, self.in_channels, self.out_channels = init_filters, int(in_channels), int(out_channels)
+        self.n_features, self.n_outputs = self.in_channels, self.out_channels
+        self.blocks_down, self.blocks_up = blocks_down, blocks_up
+        self.num_groups = groups
+        self.act_slope = slope
+        self.dropout_prob = dropout_prob
+        self.dropout_p = float(dropout_prob) if dropout_prob is not None else 0.0
+        self.dropout_width = init_filters
+        self._setup(precision, deterministic)
+
+    def _param_spec_cpu(self):
+        F_, L = self.init_filters, len(self.blocks_down)
+        spec = [("convInit.conv.weight", (F_, self.in_channels, 3, 3, 3))]
+
+        def block(prefix, c):
+            for n in ("norm1", "norm2"):
+                spec.append((prefix + "." + n + ".weight", (c,)))
+                spec.append((prefix + "." + n + ".bias", (c,)))
+            spec.append((prefix + ".conv1.conv.weight", (c, c, 3, 3, 3)))
+            spec.append((prefix + ".conv2.conv.weight", (c, c, 3, 3, 3)))
+        for i, nb in enumerate(self.blocks_down):
+            if i > 0:
+                spec.append(("down_layers.%d.0.conv.weight" % i, (F_ << i, F_ << (i - 1), 3, 3, 3)))
+            for b in range(1, nb + 1):
+                block("down_layers.%d.%d" % (i, b), F_ << i)
+        for i, nb in enumerate(self.blocks_up):
+            for b in range(nb):
+                block("up_layers.%d.%d" % (i, b), F_ << (L - 2 - i))
+        for i in range(L - 1):
+            c = F_ << (L - 2 - i)
+            spec.append(("up_samples.%d.0.conv.weight" % i, (c, 2 * c, 1, 1, 1)))
+        spec += [("conv_final.0.weight", (F_,)), ("conv_final.0.bias", (F_,)),
+                 ("conv_final.2.conv.weight", (self.out_channels, F_, 1, 1, 1)), ("conv_final.2.conv.bias", (self.out_channels,))]
+        return spec
+
+    @staticmethod
+    def _init_tensor(key, t, shapes):
+        """torch's default init (MONAI's SegResNet adds none): Conv3d weight and bias U(+-1/sqrt(fan_in)); GroupNorm 1 / 0"""
+        if t.dim() == 1 and (".norm" in key or key.startswith("conv_final.0.")):
+            (nn.init.ones_ if key.endswith("weight") else nn.init.zeros_)(t)
+        else:
+            wshape = shapes[key[:-5] + ".weight"] if key.endswith(".bias") else tuple(t.shape)
+            bound = 1.0 / math.sqrt(wshape[1] * wshape[2] * wshape[3] * wshape[4])
+            nn.init.uniform_(t, -bound, bound)
+
+    def _net_desc(self, n, d, h, w) -> _lib.NetDesc:
+        nd = _lib.NetDesc()
+        nd.arch = 2
+        nd.n_features, nd.n_outputs, nd.base_width = self.in_channels, self.out_channels, self.init_filters
+        nd.n_levels = len(self.blocks_down)
+        for i, b in enumerate(self.blocks_down):
+            nd.encoder_blocks[i] = b
+        for i, b in enumerate(self.blocks_up):
+            nd.decoder_blocks[i] = b
+        nd.norm_groups = self.num_groups
+        nd.act_slope = self.act_slope
+        nd.activation = 0
+        nd.split_precision = int(self.precision == "split")
+        nd.batch, nd.depth, nd.height, nd.width = n, d, h, w
+        return nd
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        xp = self._check_input(x, self.in_channels)
+        params = self.ordered_parameters()
+        return _UNetFunction.apply(self, xp, self._dropout_scale(xp), *self._needs_backward(params, xp), *params)
+
+
 _MODELS = {"UNet3D": UNet3D, "AutocastUNet": AutocastUNet, "AutoImplantUNet": AutoImplantUNet,
-           "B200UNet3D": UNet3D, "DynUNet": DynUNet}
+           "B200UNet3D": UNet3D, "DynUNet": DynUNet, "SegResNet": SegResNet}
 
 
 def fetch_model_by_name(model_name, *args, **kwargs):

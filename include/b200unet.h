@@ -112,9 +112,13 @@ int b200unet_gn_bwd_finalize(const double* bstats, const float* coef, const floa
 int b200unet_act_bwd(const b200unet_tensor* g1, const b200unet_tensor* g2, const b200unet_tensor* c, const float* coef, float slope,
                      const b200unet_tensor* dz, double* bstats, int bstats_ld, void* stream);
 
-/* ---- F.interpolate(scale_factor=2, mode="trilinear", align_corners=False) (decoder.py:105-106), fwd + adjoint */
+/* ---- F.interpolate(scale_factor=2, mode="trilinear", align_corners=False) (decoder.py:105-106), fwd + adjoint.
+ * add_fwd: y = upsample(x) + add in one pass (MONAI SegResNet's `up(x) + skip`), add of y's shape (NULL = upsample_fwd); the
+ * statistics are those of y.  The gradient of the sum reaches add unchanged and x through upsample2x_bwd. */
 int b200unet_upsample2x_fwd(const b200unet_tensor* x, const b200unet_tensor* y, double* stats, int stats_ld,
                             void* stream);
+int b200unet_upsample2x_add_fwd(const b200unet_tensor* x, const b200unet_tensor* add, const b200unet_tensor* y, double* stats,
+                                int stats_ld, void* stream);
 int b200unet_upsample2x_bwd(const b200unet_tensor* dy, const b200unet_tensor* dx, void* stream);
 int b200unet_zero_insert(const b200unet_tensor* x, const b200unet_tensor* z, int od, int oh, int ow, void* stream);
 
@@ -298,10 +302,17 @@ typedef struct b200unet_net_desc {
   int32_t batch, depth, height, width;
   int32_t arch;               /* 0 = the reference's UNet3D (above); 1 = MONAI DynUNet blocks as trained by
                                  examples/brats2020/brats2020_config.json:2-107: n_levels = len(filters), kernel 3, strides
-                                 1,2,2,..., transposed-conv upsampling kernel = stride = 2, InstanceNorm(affine) + LeakyReLU */
+                                 1,2,2,..., transposed-conv upsampling kernel = stride = 2, InstanceNorm(affine) + LeakyReLU;
+                                 2 = MONAI SegResNet (GroupNorm pre-activation residual blocks, stride-2 3x3x3 down-sampling,
+                                 1x1x1 conv + trilinear x2 + additive skip, GroupNorm + act + biased 1x1x1 head) with
+                                 base_width = init_filters (a multiple of 8), n_levels = len(blocks_down), encoder_blocks =
+                                 blocks_down, decoder_blocks = blocks_up (n_levels - 1 entries, all >= 1), norm_groups =
+                                 num_groups (dividing init_filters); Dropout3d(dropout_prob) on convInit's output through
+                                 dropout_scale [N][init_filters].  Rejected with B200UNET_E_UNSUPPORTED: extents not even at
+                                 every level above the last, widths above 1024, more than 8 outputs from more than 64 channels */
   int32_t filters[8];         /* arch 1: channels per level (multiples of 8) */
-  float act_slope;            /* both architectures: negative slope of the activation after each norm; 0 = the reference
-                                 UNet3D's ReLU, 0.01 = DynUNet's LeakyReLU */
+  float act_slope;            /* every architecture: negative slope of the activation after each norm; 0 = the reference
+                                 UNet3D's (and SegResNet's default) ReLU, 0.01 = DynUNet's LeakyReLU */
   int32_t deterministic;      /* 1 = weight gradients without floating-point atomics: the split-K CTAs write per-split partial
                                  sums, a second kernel adds them in a fixed order (bit-identical gradients run to run) */
   int32_t inference_only;     /* 1 = forward-only plan (volumetric.py:131-150 runs under no_grad): no backward schedule, no
@@ -315,7 +326,7 @@ typedef struct b200unet_plan b200unet_plan;
 
 int b200unet_plan_create(const b200unet_net_desc* desc, b200unet_plan** out);
 void b200unet_plan_destroy(b200unet_plan* plan);
-/* number of parameter tensors, in reference state_dict order (SURVEY.md appendix B) */
+/* number of parameter tensors, in reference state_dict order (SURVEY.md appendix B; arch 1 and 2: MONAI's registration order) */
 int b200unet_plan_num_params(const b200unet_plan* plan);
 /* shape (up to 5 dims, zero padded) and state_dict key of parameter i */
 int b200unet_plan_param_info(const b200unet_plan* plan, int i, int64_t shape[5], char* key, int key_cap);
@@ -334,7 +345,8 @@ int b200unet_plan_backward(b200unet_plan* plan, const float* dlogits, const floa
  * Runs after b200unet_plan_backward on the same stream and workspace, before the next forward: it reads
  * what that backward left in the workspace (the gradients reaching the first block, the packed input, the first norm's
  * coefficients).  UNet3D: GroupNorm(+ReLU) backward of encoder.layers.0.blocks.0.conv1.norm1 + the data gradient of the block's
- * 1x1x1 `sample` branch or its identity (myronenko.py:34-58); DynUNet: the data gradient of input_block.conv1.  The parameter
+ * 1x1x1 `sample` branch or its identity (myronenko.py:34-58); DynUNet: the data gradient of input_block.conv1; SegResNet: that of
+ * convInit.  The parameter
  * gradients come from the backward alone: this call writes nothing but dx. */
 int b200unet_plan_input_grad(b200unet_plan* plan, float* dx, void* workspace, void* stream);
 /* number of kernels the last forward / backward / input-gradient call launched (for bench.py's gpu_launches) */
