@@ -175,6 +175,7 @@ struct b200unet_plan {
   size_t bz_off = 0, bz_bytes = 0;        // zeroed at the start of every backward (bstats + dw accumulators)
   int last_launches = 0;
   int head_param = -1;
+  int head_c = 0;           // channels into the head
   std::vector<PackJob> pack_jobs, unpack_jobs;   // batched weight (un)packing tables (host copies)
   size_t jobs_off = 0;                           // device copy: pack jobs then unpack jobs
   const void* jobs_uploaded_for = nullptr;       // workspace base the table was last uploaded into
@@ -244,7 +245,7 @@ static void dec_widths(const b200unet_net_desc& d, int depth, int* in_w, int* ou
   *out_w = o;
 }
 
-static void build_param_spec(Plan& P) {
+static void unet3d_param_spec(Plan& P) {
   const b200unet_net_desc& d = P.d;
   const int L = d.n_levels;
   int cin = d.n_features;
@@ -361,12 +362,13 @@ static int new_conv(Plan& P, const std::string& key, int Co, int Ci, int ksz, in
   return (int)P.convs.size() - 1;
 }
 
-static int new_norm(Plan& P, const std::string& prefix, int C, int Cld, long long S) {
+// a norm with G groups over C channels (instance norm: G = C)
+static int new_norm(Plan& P, const std::string& prefix, int C, int Cld, long long S, int G) {
   NormLayer n;
   n.name = prefix;
   n.pg = P.find_param(prefix + ".weight");
   n.pb = P.find_param(prefix + ".bias");
-  n.C = C; n.Cld = Cld; n.G = groups_for(C, P.d.norm_groups); n.S = S;
+  n.C = C; n.Cld = Cld; n.G = G; n.S = S;
   n.coef = P.alloc((size_t)P.d.batch * Cld * 4 * sizeof(float));
   n.coef2 = P.infer ? 0 : P.alloc((size_t)P.d.batch * Cld * 2 * sizeof(float));
   n.bstats = P.bz_bytes;
@@ -480,6 +482,19 @@ static void emit_conv_fwd(Plan& P, int ci, TRef a, int ci2, TRef a2, TRef res, T
   });
 }
 
+// out = trilinear x2 up-sampling of in [+ skip, in the same pass], and the statistics of out for the norm that reads it
+static void emit_upsample2x_fwd(Plan& P, TRef in, TRef out, TRef skip) {
+  need_stats(P, out.buf);
+  push_op(P.fwd, std::string(skip.valid() ? "upsample2x_fwd+skip " : "upsample2x_fwd ") + shape_of(P, in),
+          [&P, in, out, skip](RunCtx& cx) -> int {
+    Act sk;
+    if (skip.valid()) sk = act_of(P, cx, skip);
+    LAUNCHED(cx, CAT_RESAMPLE, launch_upsample2x_fwd(act_of(P, cx, in), act_of(P, cx, out), stats_ptr(P, cx, out), P.bufs[out.buf].C, cx.st,
+                                                     skip.valid() ? &sk : nullptr));
+    return OK;
+  });
+}
+
 // ---- backward op emitters
 static Act shape_act(const Plan& P, TRef t) {
   const Buf& b = P.bufs[t.buf];
@@ -568,6 +583,33 @@ static void emit_gn_bwd(Plan& P, int ni, TRef dz, TRef x, TRef add1, TRef dx, bo
   });
 }
 
+// returns the gradient of norm ni's input x from the gradient g1 (+ g2) of its activated output: the activation's backward
+// (which also takes the norm's backward statistics), then the norm's
+static TRef emit_act_norm_bwd(Plan& P, int ni, TRef x, TRef g1, TRef g2) {
+  const Buf xb = P.bufs[x.buf];
+  const TRef dz = full(P, new_buf(P, xb.N, xb.D, xb.H, xb.W, x.c));
+  push_op(P.bwd, "act_bwd " + P.norms[ni].name + " " + shape_of(P, x), [&P, ni, g1, g2, x, dz](RunCtx& cx) -> int {
+    const NormLayer& n = P.norms[ni];
+    Act a2;
+    if (g2.valid()) a2 = act_of(P, cx, g2);
+    LAUNCHED(cx, CAT_NORM, launch_act_bwd(act_of(P, cx, g1), g2.valid() ? &a2 : nullptr, act_of(P, cx, x),
+                                          reinterpret_cast<float*>(cx.ws + n.coef), P.slope, act_of(P, cx, dz),
+                                          reinterpret_cast<double*>(cx.ws + P.bz_off + n.bstats), n.Cld, cx.st));
+    return OK;
+  });
+  const TRef dx = full(P, new_buf(P, xb.N, xb.D, xb.H, xb.W, x.c));
+  emit_gn_bwd(P, ni, dz, x, kNone, dx, false);
+  return dx;
+}
+
+// dx = the adjoint of the trilinear x2 up-sampling applied to dy
+static void emit_upsample2x_bwd(Plan& P, TRef dy, TRef dx) {
+  push_op(P.bwd, "upsample2x_bwd " + shape_of(P, dx), [&P, dy, dx](RunCtx& cx) -> int {
+    LAUNCHED(cx, CAT_RESAMPLE, launch_upsample2x_bwd(act_of(P, cx, dy), act_of(P, cx, dx), cx.st));
+    return OK;
+  });
+}
+
 // the per-parameter pointers (cx.params or cx.grads) as the batched (un)packing kernels take them
 static PtrTable ptr_table(const Plan& P, const float* const* p) {
   PtrTable tbl;
@@ -577,8 +619,11 @@ static PtrTable ptr_table(const Plan& P, const float* const* p) {
 }
 
 // First op of every forward: zero the statistics arena, upload the job tables into a new workspace, pack all weights (one
-// launch) and pack the network input (with_input_stats: and its channel statistics, for a GroupNorm that reads it).
-static void emit_prologue(Plan& P, int b_in, bool with_input_stats) {
+// launch) and pack the network input (with_input_stats: and its channel statistics, for a GroupNorm that reads it).  Returns
+// the packed input, its channels padded to a multiple of 8.
+static TRef emit_prologue(Plan& P, bool with_input_stats) {
+  const b200unet_net_desc& d = P.d;
+  const int b_in = new_buf(P, d.batch, d.depth, d.height, d.width, round_up(d.n_features, 8));
   if (with_input_stats) need_stats(P, b_in);
   push_op(P.fwd, "pack_weights+input_pack", [&P, b_in, with_input_stats](RunCtx& cx) -> int {
     B200_CHECK_CUDA(cudaMemsetAsync(cx.ws + P.stats_off, 0, P.stats_bytes, cx.st));
@@ -597,29 +642,34 @@ static void emit_prologue(Plan& P, int b_in, bool with_input_stats) {
                                                  P.bufs[b_in].C, cx.st));
     return OK;
   });
+  return full(P, b_in);
 }
 
-// first op of every backward: zero the backward statistics and the weight-gradient accumulators
-static void emit_bwd_memset(Plan& P) {
-  push_op(P.bwd, "memset", [&P](RunCtx& cx) -> int {
-    B200_CHECK_CUDA(cudaMemsetAsync(cx.ws + P.bz_off, 0, P.bz_bytes, cx.st));
-    return OK;
-  });
-}
-
-// The 1x1x1 head (bias_param >= 0: with a bias).  Training plans also get its backward op; returns the gradient of Xfinal
-// (kNone in a forward-only plan).  launch_head_fwd / launch_head_bwd pick the kernels from n_outputs; above 8 outputs the
-// bias gradient comes out of the same backward pass instead of launch_head_dbias.
-static TRef emit_head(Plan& P, TRef Xfinal, int w_param, int bias_param) {
+// The 1x1x1 head (bias_param >= 0: with a bias).  Training plans also get the first op of the backward and the head's backward
+// op; *dX = the gradient of Xfinal (kNone in a forward-only plan).  launch_head_fwd / launch_head_bwd pick the kernels from
+// n_outputs; above 8 outputs the bias gradient comes out of the same backward pass instead of launch_head_dbias.
+static int emit_head(Plan& P, TRef Xfinal, int w_param, int bias_param, TRef* dX) {
+  if (!P.infer) {
+    // UNet3D's constructor is the one that takes the activation kinds, so its message names them
+    B200_REQUIRE(P.d.activation == 0, E_UNSUPPORTED, "plan: activation inside the model%s is inference-only; train on logits",
+                 P.d.arch == 0 ? " (sigmoid/softmax)" : "");
+    push_op(P.bwd, "memset", [&P](RunCtx& cx) -> int {   // zero the backward statistics and the weight-gradient accumulators
+      B200_CHECK_CUDA(cudaMemsetAsync(cx.ws + P.bz_off, 0, P.bz_bytes, cx.st));
+      return OK;
+    });
+  }
   P.head_param = w_param;
+  P.head_c = Xfinal.c;
   push_op(P.fwd, "head_fwd", [&P, Xfinal, bias_param](RunCtx& cx) -> int {
     LAUNCHED(cx, CAT_HEAD, launch_head_fwd(act_of(P, cx, Xfinal), cx.params[P.head_param], P.d.n_outputs, P.d.activation, cx.logits, cx.st,
                                            bias_param >= 0 ? cx.params[bias_param] : nullptr));
     return OK;
   });
-  if (P.infer) return kNone;
+  *dX = kNone;
+  if (P.infer) return OK;
   const Buf xb = P.bufs[Xfinal.buf];
   const TRef g = full(P, new_buf(P, xb.N, xb.D, xb.H, xb.W, Xfinal.c));
+  *dX = g;
   push_op(P.bwd, "head_bwd", [&P, Xfinal, g, bias_param](RunCtx& cx) -> int {
     float* scratch = reinterpret_cast<float*>(cx.ws + P.head_part_off);
     const bool fused_dbias = bias_param >= 0 && P.d.n_outputs > 8;
@@ -632,7 +682,7 @@ static TRef emit_head(Plan& P, TRef Xfinal, int w_param, int bias_param) {
     }
     return OK;
   });
-  return g;
+  return OK;
 }
 
 // last op of every backward: weight gradients, accumulator -> torch layout (one batched launch)
@@ -661,9 +711,9 @@ static BlockRec build_block_fwd(Plan& P, const BlockKeys& k, TRef X, int cin_rea
   const long long S = (long long)D * H * W;
   BlockRec r;
   r.X = X; r.first = first; r.scale_out = scale_out; r.scale_in = scale_in;
-  r.n1 = new_norm(P, k.n1, cin_real, X.c, S);
+  r.n1 = new_norm(P, k.n1, cin_real, X.c, S, groups_for(cin_real, P.d.norm_groups));
   r.c1 = new_conv(P, k.c1, C, cin_real, 3, 1, true);
-  r.n2 = new_norm(P, k.n2, C, C, S);
+  r.n2 = new_norm(P, k.n2, C, C, S, groups_for(C, P.d.norm_groups));
   r.c2 = new_conv(P, k.c2, C, C, 3, 1, true);
   r.cs = (cin_real != C) ? new_conv(P, k.sample, C, cin_real, 1, 1, !first || P.input_grad) : -1;
   r.a1 = full(P, new_buf(P, N, D, H, W, X.c));
@@ -700,6 +750,26 @@ static void emit_input_grad(Plan& P, int ni, TRef dz, TRef x, TRef r) {
   });
 }
 
+// input_grad plans: the data gradient of layer ci, which reads the packed network input x, from the gradient dy of its output,
+// then d(loss)/d(x) from it (ni, dz: see emit_input_grad)
+static void emit_input_dgrad(Plan& P, int ci, TRef dy, TRef x, int ni, TRef dz) {
+  const Buf xb = P.bufs[x.buf];
+  const TRef r = full(P, new_buf(P, xb.N, xb.D, xb.H, xb.W, x.c));
+  emit_dgrad(P, ci, dy, r, -1, kNone, kNone, false, /*reads_input=*/true, &P.igrad);
+  emit_input_grad(P, ni, dz, x, r);
+}
+
+// backward through an encoder's stride-2 convolution ci from the gradient dy of its output: its weight gradient; returns the
+// gradient of its input x (also a skip) = the parity-class data gradient + dskip [* the Dropout3d scale].  Parity-class mode:
+// eight implicit GEMMs over the un-inserted gradient (27 tap products instead of 8 x 27), TMA-stored into their interleaved positions.
+static TRef emit_down_bwd(Plan& P, int ci, TRef x, TRef dy, TRef dskip, bool scale) {
+  emit_wgrad(P, ci, x, dy);
+  const Buf xb = P.bufs[x.buf];
+  const TRef dx = full(P, new_buf(P, xb.N, xb.D, xb.H, xb.W, x.c));
+  emit_dgrad(P, ci, dy, dx, -1, kNone, dskip, scale);
+  return dx;
+}
+
 // returns the TRef of dX (kNone for the first block of the network)
 static TRef build_block_bwd(Plan& P, const BlockRec& r, TRef dOut) {
   const Buf& xb = P.bufs[r.X.buf];
@@ -718,12 +788,8 @@ static TRef build_block_bwd(Plan& P, const BlockRec& r, TRef dOut) {
     emit_gn_bwd_finalize(P, r.n1);
     if (P.input_grad) {
       // dOut already carries the Dropout3d scale of this block's output (applied by whoever produced it): not applied again
-      TRef res = dOut;
-      if (r.cs >= 0) {
-        res = full(P, new_buf(P, N, D, H, W, r.X.c));
-        emit_dgrad(P, r.cs, dOut, res, -1, kNone, kNone, false, /*reads_input=*/true, &P.igrad);
-      }
-      emit_input_grad(P, r.n1, dz1, r.X, res);
+      if (r.cs >= 0) emit_input_dgrad(P, r.cs, dOut, r.X, r.n1, dz1);
+      else emit_input_grad(P, r.n1, dz1, r.X, dOut);
     }
     return kNone;
   }
@@ -765,13 +831,10 @@ static int build_unet3d(Plan& P) {
   std::vector<int> widths, Ds, Hs, Ws;
   B200_TRY(level_extents(d, Ds, Hs, Ws));
   for (int li = 0, w = d.base_width; li < L; ++li, w *= d.feature_dilation) widths.push_back(w);
-  build_param_spec(P);
+  unet3d_param_spec(P);
 
   // ---------------- forward
-  const int Cp_in = round_up(d.n_features, 8);
-  const int b_in = new_buf(P, N, Ds[0], Hs[0], Ws[0], Cp_in);
-  emit_prologue(P, b_in, /*with_input_stats=*/true);
-
+  TRef X = emit_prologue(P, /*with_input_stats=*/true);
   std::vector<std::vector<BlockRec>> enc(L), dec(L);
   std::vector<int> cat(L, -1), down(L, -1);
   std::vector<TRef> skip(L), down_out(L);
@@ -780,7 +843,6 @@ static int build_unet3d(Plan& P) {
     cat[li] = new_buf(P, N, Ds[li], Hs[li], Ws[li], 2 * widths[li]);
     need_stats(P, cat[li]);
   }
-  TRef X = full(P, b_in);
   int cin_real = d.n_features;
   for (int li = 0; li < L; ++li) {
     const int C = widths[li];
@@ -832,12 +894,7 @@ static int build_unet3d(Plan& P) {
       s.P = full(P, new_buf(P, N, xb.D, xb.H, xb.W, out_w));
       emit_conv_fwd(P, s.cpre, X, -1, kNone, kNone, s.P, false, false);
       release_if_whole(P, X);
-      TRef Pin = s.P, U = s.U;
-      push_op(P.fwd, "upsample2x_fwd " + shape_of(P, Pin), [&P, Pin, U](RunCtx& cx) -> int {
-        LAUNCHED(cx, CAT_RESAMPLE, launch_upsample2x_fwd(act_of(P, cx, Pin), act_of(P, cx, U), stats_ptr(P, cx, U), P.bufs[U.buf].C,
-                                           cx.st));
-        return OK;
-      });
+      emit_upsample2x_fwd(P, s.P, s.U, kNone);
       release_buf(P, s.P.buf);
     } else {
       // ConvTranspose3d(k3, s2, p1) + bias, then F.pad(+1 high side) = zero-insert + 3x3x3 conv with the flipped
@@ -871,15 +928,11 @@ static int build_unet3d(Plan& P) {
       cin = d.base_width;
     }
   }
-  if (!P.infer) {
-    B200_REQUIRE(d.activation == 0, E_UNSUPPORTED,
-                 "plan: activation inside the model (sigmoid/softmax) is inference-only; train on logits");
-    emit_bwd_memset(P);
-  }
-  TRef g = emit_head(P, X, P.find_param("final_convolution.weight"), -1);
+  TRef g;
+  B200_TRY(emit_head(P, X, P.find_param("final_convolution.weight"), -1, &g));
+  if (P.infer) return finish_build(P);
 
-  // ---------------- backward (training plans only)
-  if (!P.infer) {
+  // ---------------- backward
   for (int b = d.decoder_blocks[L - 1] - 1; b >= 0; --b) g = build_block_bwd(P, dec[L - 1][b], g);
   std::vector<TRef> dskip_dec(L, kNone);
   for (int i = L - 2; i >= 0; --i) {
@@ -892,10 +945,7 @@ static int build_unet3d(Plan& P) {
     TRef gX = full(P, new_buf(P, N, xb.D, xb.H, xb.W, s.Xin.c));
     if (s.cup < 0) {
       TRef dP = full(P, new_buf(P, N, xb.D, xb.H, xb.W, out_w));
-      push_op(P.bwd, "upsample2x_bwd " + shape_of(P, dP), [&P, dU, dP](RunCtx& cx) -> int {
-        LAUNCHED(cx, CAT_RESAMPLE, launch_upsample2x_bwd(act_of(P, cx, dU), act_of(P, cx, dP), cx.st));
-        return OK;
-      });
+      emit_upsample2x_bwd(P, dU, dP);
       emit_wgrad(P, s.cpre, s.Xin, dP);
       emit_dgrad(P, s.cpre, dP, gX, -1, kNone, kNone, false);
     } else {
@@ -919,18 +969,11 @@ static int build_unet3d(Plan& P) {
     for (int b = d.encoder_blocks[li] - 1; b >= 0; --b) g = build_block_bwd(P, enc[li][b], g);
     if (li > 0) {
       const int lj = li - 1;
-      emit_wgrad(P, down[lj], skip[lj], g);
-      TRef gS = full(P, new_buf(P, N, Ds[lj], Hs[lj], Ws[lj], widths[lj]));
       // dropout scale belongs to the output of encoder block (0,0): that is this tensor iff level 0 has one block
-      const bool sc = (lj == 0 && d.encoder_blocks[0] == 1);
-      // parity-class mode: eight implicit GEMMs over the un-inserted gradient (27 tap products instead of 8 x 27), TMA-stored
-      // into their interleaved positions
-      emit_dgrad(P, down[lj], g, gS, -1, kNone, dskip_dec[lj], sc);
-      g = gS;
+      g = emit_down_bwd(P, down[lj], skip[lj], g, dskip_dec[lj], /*scale=*/lj == 0 && d.encoder_blocks[0] == 1);
     }
   }
   emit_unpack_wgrads(P);
-  }  // !P.infer
   return finish_build(P);
 }
 
@@ -943,10 +986,9 @@ static int finish_build(Plan& P) {
   P.stats_off = P.alloc(P.stats_bytes);
   P.bz_off = P.alloc(P.bz_bytes);
   if (P.wg_part_bytes) P.wg_part_off = P.alloc(P.wg_part_bytes);
-  const int head_c = d.arch == 1 ? d.filters[0] : d.base_width;
-  B200_REQUIRE(d.n_outputs <= 8 || head_c <= 64, E_UNSUPPORTED,
-               "plan: more than 8 outputs need at most 64 channels into the head, got %d", head_c);
-  if (!P.infer) P.head_part_off = P.alloc(std::max(P.head_part_bytes, head_bwd_scratch_bytes(d.n_outputs, head_c)));
+  B200_REQUIRE(d.n_outputs <= 8 || P.head_c <= 64, E_UNSUPPORTED,
+               "plan: more than 8 outputs need at most 64 channels into the head, got %d", P.head_c);
+  if (!P.infer) P.head_part_off = P.alloc(std::max(P.head_part_bytes, head_bwd_scratch_bytes(d.n_outputs, P.head_c)));
   for (size_t i = 0; i < P.convs.size(); ++i)
     B200_REQUIRE(P.convs[i].pw >= 0, E_INVALID, "plan: internal: conv %d has no parameter", (int)i);
   for (const ConvLayer& c : P.convs) {
@@ -997,10 +1039,25 @@ static void add_dyn_block_params(Plan& P, const std::string& pre, int cin, int c
   add_param(P, pre + ".norm2.bias", {cout});
 }
 
-static int new_norm_keys(Plan& P, const std::string& prefix, int C, long long S) {
-  const int ni = new_norm(P, prefix, C, C, S);
-  P.norms[ni].G = C;   // instance norm: one group per channel
-  return ni;
+// module name of encoder level i of an L-level DynUNet
+static std::string dyn_enc_name(int L, int i) {
+  return i == 0 ? "input_block" : i == L - 1 ? "bottleneck" : "downsamples." + std::to_string(i - 1);
+}
+
+// in MONAI's registration order: input_block, downsamples, bottleneck, upsamples, output_block
+static void dynunet_param_spec(Plan& P) {
+  const b200unet_net_desc& d = P.d;
+  const int L = d.n_levels;
+  const int* F = d.filters;
+  for (int i = 0; i < L; ++i) add_dyn_block_params(P, dyn_enc_name(L, i), i == 0 ? d.n_features : F[i - 1], F[i]);
+  for (int u = 0; u + 1 < L; ++u) {      // upsamples[u] maps level L-1-u -> L-2-u
+    const int lo = L - 1 - u, hi = L - 2 - u;
+    const std::string pre = "upsamples." + std::to_string(u);
+    add_param(P, pre + ".transp_conv.conv.weight", {F[lo], F[hi], 2, 2, 2});
+    add_dyn_block_params(P, pre + ".conv_block", 2 * F[hi], F[hi]);
+  }
+  add_param(P, "output_block.conv.conv.weight", {d.n_outputs, F[0], 1, 1, 1});
+  add_param(P, "output_block.conv.conv.bias", {d.n_outputs});
 }
 
 static DynBlock build_dyn_block_fwd(Plan& P, const std::string& pre, TRef X, int cin_real, int C, int stride, TRef dest, bool first,
@@ -1012,8 +1069,8 @@ static DynBlock build_dyn_block_fwd(Plan& P, const std::string& pre, TRef X, int
   r.X = X; r.stride = stride; r.first = first;
   r.k1 = new_conv(P, pre + ".conv1.conv.weight", C, cin_real, 3, stride, !first || P.input_grad);
   r.k2 = new_conv(P, pre + ".conv2.conv.weight", C, C, 3, 1, true);
-  r.n1 = new_norm_keys(P, pre + ".norm1", C, S);
-  r.n2 = new_norm_keys(P, pre + ".norm2", C, S);
+  r.n1 = new_norm(P, pre + ".norm1", C, C, S, C);
+  r.n2 = new_norm(P, pre + ".norm2", C, C, S, C);
   r.c1 = full(P, new_buf(P, N, D, H, W, C));
   emit_conv_fwd(P, r.k1, X, -1, kNone, kNone, r.c1, true, false);
   if (x_dead) release_if_whole(P, X);
@@ -1029,26 +1086,11 @@ static DynBlock build_dyn_block_fwd(Plan& P, const std::string& pre, TRef X, int
   return r;
 }
 
-static void emit_act_bwd(Plan& P, int ni, TRef g1, TRef g2, TRef c, TRef dz) {
-  push_op(P.bwd, "act_bwd " + P.norms[ni].name + " " + shape_of(P, c), [&P, ni, g1, g2, c, dz](RunCtx& cx) -> int {
-    const NormLayer& n = P.norms[ni];
-    Act a2;
-    if (g2.valid()) a2 = act_of(P, cx, g2);
-    LAUNCHED(cx, CAT_NORM, launch_act_bwd(act_of(P, cx, g1), g2.valid() ? &a2 : nullptr, act_of(P, cx, c),
-                                          reinterpret_cast<float*>(cx.ws + n.coef), P.slope, act_of(P, cx, dz),
-                                          reinterpret_cast<double*>(cx.ws + P.bz_off + n.bstats), n.Cld, cx.st));
-    return OK;
-  });
-}
-
 // gradient of the block output arrives as g1 (+ g2); returns dX (kNone for the first block)
 static TRef build_dyn_block_bwd(Plan& P, const DynBlock& r, TRef g1, TRef g2) {
   const Buf& cb = P.bufs[r.c1.buf];
   const int N = cb.N, D = cb.D, H = cb.H, W = cb.W, C = r.c1.c;
-  TRef dz2 = full(P, new_buf(P, N, D, H, W, C));
-  emit_act_bwd(P, r.n2, g1, g2, r.c2, dz2);
-  TRef dc2 = full(P, new_buf(P, N, D, H, W, C));
-  emit_gn_bwd(P, r.n2, dz2, r.c2, kNone, dc2, false);
+  TRef dc2 = emit_act_norm_bwd(P, r.n2, r.c2, g1, g2);
   emit_wgrad(P, r.k2, r.a1, dc2);
   TRef dz1 = full(P, new_buf(P, N, D, H, W, C));
   emit_dgrad(P, r.k2, dc2, dz1, r.n1, r.c1, kNone, false);   // mode 1: masked by act'(norm1(c1)) + statistics
@@ -1056,12 +1098,7 @@ static TRef build_dyn_block_bwd(Plan& P, const DynBlock& r, TRef g1, TRef g2) {
   emit_gn_bwd(P, r.n1, dz1, r.c1, kNone, dc1, false);
   emit_wgrad(P, r.k1, r.X, dc1);
   if (r.first) {
-    if (P.input_grad) {
-      const Buf& xb = P.bufs[r.X.buf];
-      TRef dX = full(P, new_buf(P, N, xb.D, xb.H, xb.W, r.X.c));
-      emit_dgrad(P, r.k1, dc1, dX, -1, kNone, kNone, false, /*reads_input=*/true, &P.igrad);
-      emit_input_grad(P, -1, kNone, kNone, dX);
-    }
+    if (P.input_grad) emit_input_dgrad(P, r.k1, dc1, r.X, -1, kNone);
     return kNone;
   }
   const Buf& xb = P.bufs[r.X.buf];
@@ -1084,33 +1121,18 @@ static int build_dynunet(Plan& P) {
     F.push_back(d.filters[i]);
   }
   B200_TRY(level_extents(d, Ds, Hs, Ws));
-  // ---- parameter spec in MONAI's registration order: input_block, downsamples, bottleneck, upsamples, output_block
-  auto enc_name = [&](int i) -> std::string {
-    return i == 0 ? "input_block" : i == L - 1 ? "bottleneck" : "downsamples." + std::to_string(i - 1);
-  };
-  for (int i = 0; i < L; ++i) add_dyn_block_params(P, enc_name(i), i == 0 ? d.n_features : F[i - 1], F[i]);
-  for (int u = 0; u + 1 < L; ++u) {      // upsamples[u] maps level L-1-u -> L-2-u
-    const int lo = L - 1 - u, hi = L - 2 - u;
-    const std::string pre = "upsamples." + std::to_string(u);
-    add_param(P, pre + ".transp_conv.conv.weight", {F[lo], F[hi], 2, 2, 2});
-    add_dyn_block_params(P, pre + ".conv_block", 2 * F[hi], F[hi]);
-  }
-  add_param(P, "output_block.conv.conv.weight", {d.n_outputs, F[0], 1, 1, 1});
-  add_param(P, "output_block.conv.conv.bias", {d.n_outputs});
+  dynunet_param_spec(P);
 
   // ---- forward
-  const int Cp_in = round_up(d.n_features, 8);
-  const int b_in = new_buf(P, N, Ds[0], Hs[0], Ws[0], Cp_in);
-  emit_prologue(P, b_in, /*with_input_stats=*/false);
+  TRef X = emit_prologue(P, /*with_input_stats=*/false);
   std::vector<int> cat(L, -1);
   for (int i = 0; i + 1 < L; ++i) cat[i] = new_buf(P, N, Ds[i], Hs[i], Ws[i], 2 * F[i]);
   std::vector<DynBlock> enc(L), dec(L);
   std::vector<int> up(L, -1);
-  TRef X = full(P, b_in);
   int cin_real = d.n_features;
   for (int i = 0; i < L; ++i) {
     TRef dest = (i + 1 < L) ? slice(full(P, cat[i]), F[i], F[i]) : full(P, new_buf(P, N, Ds[i], Hs[i], Ws[i], F[i]));
-    enc[i] = build_dyn_block_fwd(P, enc_name(i), X, cin_real, F[i], i == 0 ? 1 : 2, dest, i == 0, /*x_dead=*/i == 0);
+    enc[i] = build_dyn_block_fwd(P, dyn_enc_name(L, i), X, cin_real, F[i], i == 0 ? 1 : 2, dest, i == 0, /*x_dead=*/i == 0);
     X = dest;
     cin_real = F[i];
   }
@@ -1124,11 +1146,8 @@ static int build_dynunet(Plan& P) {
     dec[hi] = build_dyn_block_fwd(P, pre + ".conv_block", full(P, cat[hi]), 2 * F[hi], F[hi], 1, dest, false, /*x_dead=*/true);
     X = dest;
   }
-  if (!P.infer) {
-    B200_REQUIRE(d.activation == 0, E_UNSUPPORTED, "plan: activation inside the model is inference-only; train on logits");
-    emit_bwd_memset(P);
-  }
-  TRef g = emit_head(P, X, P.find_param("output_block.conv.conv.weight"), P.find_param("output_block.conv.conv.bias"));
+  TRef g;
+  B200_TRY(emit_head(P, X, P.find_param("output_block.conv.conv.weight"), P.find_param("output_block.conv.conv.bias"), &g));
   if (P.infer) return finish_build(P);
 
   // ---- backward
@@ -1187,6 +1206,30 @@ static void add_segres_block_params(Plan& P, const std::string& pre, int C) {
   add_param(P, pre + ".conv2.conv.weight", {C, C, 3, 3, 3});
 }
 
+static std::string down_name(int i, int j) { return "down_layers." + std::to_string(i) + "." + std::to_string(j); }
+static std::string up_name(int i, int j) { return "up_layers." + std::to_string(i) + "." + std::to_string(j); }
+static std::string up_conv_name(int i) { return "up_samples." + std::to_string(i) + ".0.conv.weight"; }
+
+// in MONAI's registration order
+static void segresnet_param_spec(Plan& P) {
+  const b200unet_net_desc& d = P.d;
+  const int L = d.n_levels, F = d.base_width;
+  std::vector<int> Wd;
+  for (int i = 0; i < L; ++i) Wd.push_back(F << i);
+  add_param(P, "convInit.conv.weight", {F, d.n_features, 3, 3, 3});
+  for (int i = 0; i < L; ++i) {
+    if (i > 0) add_param(P, down_name(i, 0) + ".conv.weight", {Wd[i], Wd[i - 1], 3, 3, 3});
+    for (int b = 1; b <= d.encoder_blocks[i]; ++b) add_segres_block_params(P, down_name(i, b), Wd[i]);
+  }
+  for (int i = 0; i + 1 < L; ++i)
+    for (int b = 0; b < d.decoder_blocks[i]; ++b) add_segres_block_params(P, up_name(i, b), Wd[L - 2 - i]);
+  for (int i = 0; i + 1 < L; ++i) add_param(P, up_conv_name(i), {Wd[L - 2 - i], 2 * Wd[L - 2 - i], 1, 1, 1});
+  add_param(P, "conv_final.0.weight", {F});
+  add_param(P, "conv_final.0.bias", {F});
+  add_param(P, "conv_final.2.conv.weight", {d.n_outputs, F, 1, 1, 1});
+  add_param(P, "conv_final.2.conv.bias", {d.n_outputs});
+}
+
 static int build_segresnet(Plan& P) {
   const b200unet_net_desc& d = P.d;
   const int L = d.n_levels, N = d.batch, F = d.base_width;
@@ -1206,33 +1249,15 @@ static int build_segresnet(Plan& P) {
   std::vector<int> Wd, Ds, Hs, Ws;
   for (int i = 0; i < L; ++i) Wd.push_back(F << i);
   B200_TRY(level_extents(d, Ds, Hs, Ws));
-  auto down_name = [](int i, int j) { return "down_layers." + std::to_string(i) + "." + std::to_string(j); };
-  auto up_name = [](int i, int j) { return "up_layers." + std::to_string(i) + "." + std::to_string(j); };
-  auto up_conv_name = [](int i) { return "up_samples." + std::to_string(i) + ".0.conv.weight"; };
-
-  // ---- parameter spec in MONAI's registration order
-  add_param(P, "convInit.conv.weight", {F, d.n_features, 3, 3, 3});
-  for (int i = 0; i < L; ++i) {
-    if (i > 0) add_param(P, down_name(i, 0) + ".conv.weight", {Wd[i], Wd[i - 1], 3, 3, 3});
-    for (int b = 1; b <= d.encoder_blocks[i]; ++b) add_segres_block_params(P, down_name(i, b), Wd[i]);
-  }
-  for (int i = 0; i + 1 < L; ++i)
-    for (int b = 0; b < d.decoder_blocks[i]; ++b) add_segres_block_params(P, up_name(i, b), Wd[L - 2 - i]);
-  for (int i = 0; i + 1 < L; ++i) add_param(P, up_conv_name(i), {Wd[L - 2 - i], 2 * Wd[L - 2 - i], 1, 1, 1});
-  add_param(P, "conv_final.0.weight", {F});
-  add_param(P, "conv_final.0.bias", {F});
-  add_param(P, "conv_final.2.conv.weight", {d.n_outputs, F, 1, 1, 1});
-  add_param(P, "conv_final.2.conv.bias", {d.n_outputs});
+  segresnet_param_spec(P);
 
   // ---- forward
-  const int Cp_in = round_up(d.n_features, 8);
-  const int b_in = new_buf(P, N, Ds[0], Hs[0], Ws[0], Cp_in);
-  emit_prologue(P, b_in, /*with_input_stats=*/false);
+  const TRef in = emit_prologue(P, /*with_input_stats=*/false);
   // convInit, Dropout3d through the epilogue's per-(n, c) scale; the statistics are those of the scaled output
   const int cinit = new_conv(P, "convInit.conv.weight", F, d.n_features, 3, 1, P.input_grad);
   TRef X = full(P, new_buf(P, N, Ds[0], Hs[0], Ws[0], F));
-  emit_conv_fwd(P, cinit, full(P, b_in), -1, kNone, kNone, X, true, /*scale=*/true);
-  release_buf(P, b_in);
+  emit_conv_fwd(P, cinit, in, -1, kNone, kNone, X, true, /*scale=*/true);
+  release_buf(P, in.buf);
   std::vector<std::vector<BlockRec>> enc(L), dec(L);
   std::vector<int> pre(L, -1);
   std::vector<TRef> down_x(L);
@@ -1263,13 +1288,7 @@ static int build_segresnet(Plan& P) {
     emit_conv_fwd(P, upc[i], X, -1, kNone, kNone, up_p[i], false, false);
     release_if_whole(P, X);
     up_y[i] = full(P, new_buf(P, N, Ds[j], Hs[j], Ws[j], C));
-    need_stats(P, up_y[i].buf);
-    const TRef Pin = up_p[i], Sk = down_x[j], Y = up_y[i];
-    push_op(P.fwd, "upsample2x_fwd+skip " + shape_of(P, Pin), [&P, Pin, Sk, Y](RunCtx& cx) -> int {
-      const Act sk = act_of(P, cx, Sk);
-      LAUNCHED(cx, CAT_RESAMPLE, launch_upsample2x_fwd(act_of(P, cx, Pin), act_of(P, cx, Y), stats_ptr(P, cx, Y), P.bufs[Y.buf].C, cx.st, &sk));
-      return OK;
-    });
+    emit_upsample2x_fwd(P, up_p[i], up_y[i], down_x[j]);
     release_buf(P, up_p[i].buf);
     release_if_whole(P, down_x[j]);
     X = up_y[i];
@@ -1283,25 +1302,16 @@ static int build_segresnet(Plan& P) {
     }
   }
   // head: GroupNorm + act into a buffer, then the biased 1x1x1 head
-  const int nf = new_norm(P, "conv_final.0", F, F, (long long)Ds[0] * Hs[0] * Ws[0]);
+  const int nf = new_norm(P, "conv_final.0", F, F, (long long)Ds[0] * Hs[0] * Ws[0], groups_for(F, d.norm_groups));
   const TRef A = full(P, new_buf(P, N, Ds[0], Hs[0], Ws[0], F));
   emit_norm_fwd(P, nf, X, A);
   release_if_whole(P, X);
-  if (!P.infer) {
-    B200_REQUIRE(d.activation == 0, E_UNSUPPORTED, "plan: activation inside the model is inference-only; train on logits");
-    emit_bwd_memset(P);
-  }
-  TRef g = emit_head(P, A, P.find_param("conv_final.2.conv.weight"), P.find_param("conv_final.2.conv.bias"));
+  TRef g;
+  B200_TRY(emit_head(P, A, P.find_param("conv_final.2.conv.weight"), P.find_param("conv_final.2.conv.bias"), &g));
   if (P.infer) return finish_build(P);
 
   // ---- backward
-  {
-    TRef dz = full(P, new_buf(P, N, Ds[0], Hs[0], Ws[0], F));
-    emit_act_bwd(P, nf, g, kNone, X, dz);
-    TRef dX = full(P, new_buf(P, N, Ds[0], Hs[0], Ws[0], F));
-    emit_gn_bwd(P, nf, dz, X, kNone, dX, false);
-    g = dX;
-  }
+  g = emit_act_norm_bwd(P, nf, X, g, kNone);
   std::vector<TRef> dskip(L, kNone);
   for (int i = L - 2; i >= 0; --i) {   // up stages, top to bottom
     const int j = L - 2 - i, C = Wd[j];
@@ -1309,10 +1319,7 @@ static int build_segresnet(Plan& P) {
     // d(up(p) + skip): unchanged to the skip, through the adjoint of the up-sampling to the 1x1x1 convolution
     dskip[j] = g;
     TRef dP = full(P, new_buf(P, N, Ds[j + 1], Hs[j + 1], Ws[j + 1], C));
-    push_op(P.bwd, "upsample2x_bwd " + shape_of(P, dP), [&P, g, dP](RunCtx& cx) -> int {
-      LAUNCHED(cx, CAT_RESAMPLE, launch_upsample2x_bwd(act_of(P, cx, g), act_of(P, cx, dP), cx.st));
-      return OK;
-    });
+    emit_upsample2x_bwd(P, g, dP);
     emit_wgrad(P, upc[i], up_in[i], dP);
     TRef gX = full(P, new_buf(P, N, Ds[j + 1], Hs[j + 1], Ws[j + 1], 2 * C));
     emit_dgrad(P, upc[i], dP, gX, -1, kNone, kNone, false);
@@ -1321,21 +1328,11 @@ static int build_segresnet(Plan& P) {
   // g = gradient of the bottom level's output; encoder, bottom to top
   for (int i = L - 1; i >= 0; --i) {
     for (int b = d.encoder_blocks[i] - 1; b >= 0; --b) g = build_block_bwd(P, enc[i][b], g);
-    if (i > 0) {
-      // the level below's output gets the parity-class data gradient of this level's stride-2 convolution + its skip gradient
-      emit_wgrad(P, pre[i], down_x[i - 1], g);
-      TRef gS = full(P, new_buf(P, N, Ds[i - 1], Hs[i - 1], Ws[i - 1], Wd[i - 1]));
-      emit_dgrad(P, pre[i], g, gS, -1, kNone, dskip[i - 1], false);
-      g = gS;
-    }
+    if (i > 0) g = emit_down_bwd(P, pre[i], down_x[i - 1], g, dskip[i - 1], false);
   }
   // g = gradient of convInit's output (the first ResBlock applied the dropout scale to it)
-  emit_wgrad(P, cinit, full(P, b_in), g);
-  if (P.input_grad) {
-    TRef dX = full(P, new_buf(P, N, Ds[0], Hs[0], Ws[0], Cp_in));
-    emit_dgrad(P, cinit, g, dX, -1, kNone, kNone, false, /*reads_input=*/true, &P.igrad);
-    emit_input_grad(P, -1, kNone, kNone, dX);
-  }
+  emit_wgrad(P, cinit, in, g);
+  if (P.input_grad) emit_input_dgrad(P, cinit, g, in, -1, kNone);
   emit_unpack_wgrads(P);
   return finish_build(P);
 }

@@ -177,8 +177,9 @@ class _UNetFunction(torch.autograd.Function):
 
 class _PlanModel(nn.Module):
     """Shared machinery of the plan-backed models: canonical fp32 parameters under the reference's state-dict keys, a
-    cache of whole-network plans keyed by input shape, gradient placement.  Subclasses provide ``_param_spec_cpu`` (ordered
-    (key, shape) list), ``_net_desc`` (the library's network descriptor) and ``_init_tensor``."""
+    cache of whole-network plans keyed by input shape, gradient placement, the forward.  Subclasses provide
+    ``_param_spec_cpu`` (ordered (key, shape) list), ``n_features`` / ``n_outputs``, their architecture's fields of
+    ``_net_desc``, and ``_is_norm_key`` (the parameters ``_init_tensor`` sets to 1 / 0) or their own ``_init_tensor``."""
 
     def _setup(self, precision: Optional[str], deterministic: Optional[bool] = None) -> None:
         # deterministic: weight gradients reduced without floating-point atomics (per-split partial sums + fixed-order sum):
@@ -206,6 +207,15 @@ class _PlanModel(nn.Module):
             _register(self, key, nn.Parameter(t))
             self._keys.append(key)
 
+    def _init_tensor(self, key, t, shapes):
+        """torch's default init: Conv3d weight and bias U(+-1/sqrt(fan_in)); GroupNorm weight 1, bias 0"""
+        if self._is_norm_key(key):
+            (nn.init.ones_ if key.endswith("weight") else nn.init.zeros_)(t)
+        else:
+            wshape = shapes[key[:-5] + ".weight"] if key.endswith(".bias") else tuple(t.shape)
+            bound = 1.0 / math.sqrt(wshape[1] * wshape[2] * wshape[3] * wshape[4])   # fan_in = weight.size(1) * k^3
+            nn.init.uniform_(t, -bound, bound)
+
     def ordered_parameters(self):
         sd = dict(self.named_parameters())
         return [sd[k] for k in self._keys]
@@ -226,6 +236,15 @@ class _PlanModel(nn.Module):
             return self._forced_dropout_scale.to(device=xp.device, dtype=torch.float32).contiguous()
         keep = (torch.rand((xp.shape[0], self.dropout_width), device=xp.device) >= self.dropout_p)
         return keep.float() / (1.0 - self.dropout_p)
+
+    # ------------------------------------------------------------------ library descriptor
+    def _net_desc(self, n, d, h, w) -> _lib.NetDesc:
+        """the fields every architecture sets; subclasses add their own (the struct zero-fills the rest)"""
+        nd = _lib.NetDesc()
+        nd.n_features, nd.n_outputs = self.n_features, self.n_outputs
+        nd.split_precision = int(self.precision == "split")
+        nd.batch, nd.depth, nd.height, nd.width = n, d, h, w
+        return nd
 
     # ------------------------------------------------------------------ plan cache
     def _plan_for(self, x: torch.Tensor, inference_only: bool = False, input_grad: bool = False) -> _Plan:
@@ -296,13 +315,13 @@ class _PlanModel(nn.Module):
         need_dx = bool(torch.is_grad_enabled() and x.requires_grad)
         return bool(need_dx or (torch.is_grad_enabled() and any(p.requires_grad for p in params))), need_dx
 
-    def _check_input(self, x: torch.Tensor, n_in: int) -> torch.Tensor:
+    def _check_input(self, x: torch.Tensor) -> torch.Tensor:
         if not isinstance(x, torch.Tensor) or x.dim() != 5:
             raise ValueError("%s expects a 5-D tensor [N, C, D, H, W]" % type(self).__name__)
         if not x.is_cuda:
             raise RuntimeError("B200 %s runs only on CUDA tensors (no CPU fallback); got device %s" % (type(self).__name__, x.device))
-        if x.shape[1] != n_in:
-            raise ValueError("expected %d input channels, got %d" % (n_in, x.shape[1]))
+        if x.shape[1] != self.n_features:
+            raise ValueError("expected %d input channels, got %d" % (self.n_features, x.shape[1]))
         # MetaTensor -> plain view; as_subclass, contiguous and float stay on the autograd graph, so the input gradient
         # reaches the caller's tensor
         xp = x.as_subclass(torch.Tensor) if type(x) is not torch.Tensor else x
@@ -311,6 +330,11 @@ class _PlanModel(nn.Module):
         if params[0].device != xp.device:
             raise RuntimeError("model parameters are on %s but the input is on %s" % (params[0].device, xp.device))
         return xp
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        xp = self._check_input(x)
+        params = self.ordered_parameters()
+        return _UNetFunction.apply(self, xp, self._dropout_scale(xp), *self._needs_backward(params, xp), *params)
 
 
 class UNet3D(_PlanModel):
@@ -359,17 +383,8 @@ class UNet3D(_PlanModel):
         self._setup(precision, deterministic)                    # parameters under the reference's keys (SURVEY appendix B)
 
     @staticmethod
-    def _init_tensor(key, t, shapes):
-        """default torch init of the reference's modules (Conv3d: U(+-1/sqrt(fan_in)); GroupNorm: 1 / 0)"""
-        if key.endswith("norm1.weight"):
-            nn.init.ones_(t)
-        elif key.endswith("norm1.bias"):
-            nn.init.zeros_(t)
-        else:
-            wshape = shapes[key[:-5] + ".weight"] if key.endswith(".bias") else tuple(t.shape)
-            fan_in = wshape[1] * wshape[2] * wshape[3] * wshape[4]   # torch default: weight.size(1) * k^3
-            bound = 1.0 / math.sqrt(fan_in)
-            nn.init.uniform_(t, -bound, bound)
+    def _is_norm_key(key):
+        return key.endswith(("norm1.weight", "norm1.bias"))
 
     # ------------------------------------------------------------------ spec (pure python twin of plan.cu's)
     def _dec_widths(self, depth: int) -> Tuple[int, int]:
@@ -423,8 +438,8 @@ class UNet3D(_PlanModel):
 
     # ------------------------------------------------------------------ library descriptor
     def _net_desc(self, n, d, h, w) -> _lib.NetDesc:
-        nd = _lib.NetDesc()
-        nd.n_features, nd.n_outputs, nd.base_width = self.n_features, self.n_outputs, self.base_width
+        nd = super()._net_desc(n, d, h, w)
+        nd.base_width = self.base_width
         nd.n_levels = len(self.encoder_blocks)
         for i, b in enumerate(self.encoder_blocks):
             nd.encoder_blocks[i] = b
@@ -434,15 +449,7 @@ class UNet3D(_PlanModel):
         nd.norm_groups = self.norm_groups
         nd.use_transposed_convolutions = int(self.use_transposed_convolutions)
         nd.activation = _ACT[self.activation_name]
-        nd.split_precision = int(self.precision == "split")
-        nd.batch, nd.depth, nd.height, nd.width = n, d, h, w
         return nd
-
-    # ------------------------------------------------------------------ forward
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        xp = self._check_input(x, self.n_features)
-        params = self.ordered_parameters()
-        return _UNetFunction.apply(self, xp, self._dropout_scale(xp), *self._needs_backward(params, xp), *params)
 
 
 class AutocastUNet(UNet3D):
@@ -557,22 +564,13 @@ class DynUNet(_PlanModel):
             nn.init.kaiming_normal_(t, a=0.01)
 
     def _net_desc(self, n, d, h, w) -> _lib.NetDesc:
-        nd = _lib.NetDesc()
+        nd = super()._net_desc(n, d, h, w)
         nd.arch = 1
-        nd.n_features, nd.n_outputs = self.in_channels, self.out_channels
         nd.n_levels = len(self.filters)
         for i, f in enumerate(self.filters):
             nd.filters[i] = f
         nd.act_slope = self.act_slope
-        nd.activation = 0
-        nd.split_precision = int(self.precision == "split")
-        nd.batch, nd.depth, nd.height, nd.width = n, d, h, w
         return nd
-
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        xp = self._check_input(x, self.in_channels)
-        params = self.ordered_parameters()
-        return _UNetFunction.apply(self, xp, None, *self._needs_backward(params, xp), *params)
 
 
 def _name_and_args(v, what):
@@ -674,19 +672,13 @@ class SegResNet(_PlanModel):
         return spec
 
     @staticmethod
-    def _init_tensor(key, t, shapes):
-        """torch's default init (MONAI's SegResNet adds none): Conv3d weight and bias U(+-1/sqrt(fan_in)); GroupNorm 1 / 0"""
-        if t.dim() == 1 and (".norm" in key or key.startswith("conv_final.0.")):
-            (nn.init.ones_ if key.endswith("weight") else nn.init.zeros_)(t)
-        else:
-            wshape = shapes[key[:-5] + ".weight"] if key.endswith(".bias") else tuple(t.shape)
-            bound = 1.0 / math.sqrt(wshape[1] * wshape[2] * wshape[3] * wshape[4])
-            nn.init.uniform_(t, -bound, bound)
+    def _is_norm_key(key):   # MONAI's SegResNet adds no init of its own
+        return ".norm" in key or key.startswith("conv_final.0.")
 
     def _net_desc(self, n, d, h, w) -> _lib.NetDesc:
-        nd = _lib.NetDesc()
+        nd = super()._net_desc(n, d, h, w)
         nd.arch = 2
-        nd.n_features, nd.n_outputs, nd.base_width = self.in_channels, self.out_channels, self.init_filters
+        nd.base_width = self.init_filters
         nd.n_levels = len(self.blocks_down)
         for i, b in enumerate(self.blocks_down):
             nd.encoder_blocks[i] = b
@@ -694,15 +686,7 @@ class SegResNet(_PlanModel):
             nd.decoder_blocks[i] = b
         nd.norm_groups = self.num_groups
         nd.act_slope = self.act_slope
-        nd.activation = 0
-        nd.split_precision = int(self.precision == "split")
-        nd.batch, nd.depth, nd.height, nd.width = n, d, h, w
         return nd
-
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        xp = self._check_input(x, self.in_channels)
-        params = self.ordered_parameters()
-        return _UNetFunction.apply(self, xp, self._dropout_scale(xp), *self._needs_backward(params, xp), *params)
 
 
 _MODELS = {"UNet3D": UNet3D, "AutocastUNet": AutocastUNet, "AutoImplantUNet": AutoImplantUNet,
