@@ -92,7 +92,9 @@ def config_launches():
         of 4, forward only;
       - DynUNet with 14 outputs and a bias (2 x 32^3, filters[0] = 16);
       - the plan-smooth rows unet_24out_bw16 (UNet3D, 16 channels, 1 x 32^3) and dyn_24out_dx (DynUNet with its bias,
-        filters[0] = 16, 1 x 32^3).
+        filters[0] = 16, 1 x 32^3);
+      - SegResNet's three_level_24out case of tests/segresnet_cases.py (biased head, init_filters 8, 1 x 24 x 32 x 40), in bf16
+        and in split precision.
     args: fwd (n_out, c, n, dims, act, bias, precision); bwd (n_out, c, n, dims, dbias, precision)."""
     out = []
 
@@ -113,6 +115,8 @@ def config_launches():
     train("dynunet-14-bias", 14, 16, 2, (32, 32, 32), True, "split")
     train("plan-smooth-unet_24out_bw16", 24, 16, 1, (32, 32, 32), False, "split")
     train("plan-smooth-dyn_24out_dx", 24, 16, 1, (32, 32, 32), True, "split")
+    for precision in ("bf16", "split"):
+        train("segresnet-three_level_24out-%s" % precision, 24, 8, 1, (24, 32, 40), True, precision)
     return out
 
 
@@ -223,6 +227,9 @@ CONFIG_CASES = (
         _c(14, 16, 2, (32, 32, 32), "split", GEO_32_2, bias=True, positive=True),     # DynUNet with a bias
         _c(24, 16, 1, (32, 32, 32), "split", GEO_32_1),                               # plan-smooth unet_24out_bw16
         _c(24, 16, 1, (32, 32, 32), "split", GEO_32_1, bias=True),                    # plan-smooth dyn_24out_dx
+        # SegResNet three_level_24out: 1 x 24 x 32 x 40, 240 tiles (one per forward CTA; 1 or 2 per backward slot)
+        _c(24, 8, 1, (24, 32, 40), "bf16", GEO_32_1, bias=True),
+        _c(24, 8, 1, (24, 32, 40), "split", GEO_32_1, bias=True),
     ])
 
 # Beyond the configurations, per NT 1..8: n_out at both ends of its 16-block (16k + 1, 16k + 16; 9 for NT 1), both

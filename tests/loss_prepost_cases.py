@@ -201,8 +201,9 @@ GOLDEN = {   # tests/golden/recipe.py CASES: (n_outputs, input shape); every one
 
 def config_launches():
     """(config, kernel, args) of every criterion / pre- / post-processing launch of the configurations:
-      - bench.py C2 (batch 2, 3 outputs, 128^3) and C3 (160 x 192 x 128) and the BraTS config (3 sigmoid outputs, batch 2 of
-        128^3 patches): DiceLoss(sigmoid=True) on uint8 one-hot targets;
+      - bench.py C2 (batch 2, 3 outputs, 128^3) and C3 (160 x 192 x 128), the BraTS config (3 sigmoid outputs, batch 2 of
+        128^3 patches) and the BraTS SegResNet recipe (3 sigmoid outputs, 1 x 224 x 224 x 144): DiceLoss(sigmoid=True) on uint8
+        one-hot targets;
       - the golden recipes, and the many-class setups of tests/test_gpu_many_classes.py: the 24- and 104-output fixtures
         (1 x 32^3), the 104-output machinery (2 x 32^3 and 2 x 16^3) and the 128-output head shape (2 x 5 x 7 x 3);
       - README's head table at the C2 size with 104 and 128 outputs: DiceLoss(sigmoid=True) on uint8 one-hot targets;
@@ -210,7 +211,8 @@ def config_launches():
       - bench.py C5's tiled inference: one 256^3 volume, roi 128^3, overlap 0.25, sw_batch 3, one output channel;
       - the BraTS z-score: NormalizeIntensity(nonzero=True, channel_wise=True) on 4 channels at 128^3 and 240 x 240 x 155."""
     out = []
-    for name, (n, c, dims) in [("C2", (2, 3, (128, 128, 128))), ("C3", (2, 3, (160, 192, 128))), ("brats", (2, 3, (128, 128, 128)))]:
+    for name, (n, c, dims) in [("C2", (2, 3, (128, 128, 128))), ("C3", (2, 3, (160, 192, 128))), ("brats", (2, 3, (128, 128, 128))),
+                               ("brats-segresnet", (1, 3, (224, 224, 144)))]:
         out.append((name, "dice", (n, c, vol(dims), "u8")))
     for name, (c, shape) in GOLDEN.items():
         out.append(("golden-" + name, "dice", (shape[0], c, vol(shape[2:]), "u8")))

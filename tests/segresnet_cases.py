@@ -46,11 +46,16 @@ class Case:
 MONAI_DEFAULTS = dict()
 BRATS = dict(init_filters=16, in_channels=4, out_channels=3, dropout_prob=0.2, blocks_down=[1, 2, 2, 4], blocks_up=[1, 1, 1])
 THREE_LEVEL = dict(in_channels=2, out_channels=24, blocks_down=(2, 1, 2), blocks_up=(1, 2), norm_name="group", num_groups=4)
+# widths 24 .. 192 (3 to 24 chunks of 8 channels: no shuffle pattern), 3 channels per group, 12 input channels packed into two
+# 8-channel chunks, and level extents down to 3 x 5 x 4
+NPOW2 = dict(init_filters=24, in_channels=12, out_channels=5, dropout_prob=0.2, norm=("GROUP", {"num_groups": 8}))
 RELU_CASES = [
     Case("monai_defaults", MONAI_DEFAULTS, (1, 1, 32, 32, 32), seed=1),
     Case("brats_recipe", BRATS, (2, 4, 32, 32, 48), dropout=True, seed=2),
     Case("three_level_24out", THREE_LEVEL, (1, 2, 24, 32, 40), seed=3),
+    Case("npow2_f24_in12", NPOW2, (2, 12, 24, 40, 32), dropout=True, seed=5),
 ]
+NPOW2_CASE = RELU_CASES[3]
 SMOOTH_CASE = Case("smooth_brats_dx", dict(BRATS, init_filters=8, act=("leakyrelu", {"negative_slope": 1.0})), (2, 4, 32, 32, 32),
                    dropout=True, seed=4)
 
@@ -180,6 +185,51 @@ def route_table(L, split, n=1, in_channels=4, init_filters=16, dims=(224, 224, 1
     for label, op, ci, co, ext, mode in conv_layers(n, in_channels, init_filters, dims):
         r = conv_query(L, op, ci, co, ext, split, mode, n=n)
         out[label] = None if r is None else (r["kind"], r["bn"], r["kc"])
+    return out
+
+
+def wgrad_layers(in_channels, init_filters, dims, blocks_down=(1, 2, 2, 4)):
+    """(label, op, ci, co, dy extents) of every weight gradient of a SegResNet training plan (plan.cu: build_segresnet; one
+    entry per distinct shape): convInit from the packed input, the two 3x3x3 convolutions of every ResBlock, the stride-2
+    convolution into each lower level and the 1x1x1 convolution of each decoder stage"""
+    L = len(blocks_down)
+    ext = [tuple(d >> k for d in dims) for k in range(L)]
+    W = [init_filters << k for k in range(L)]
+    out = [("convInit", "k3s1", 8 if in_channels <= 8 else 16, W[0], ext[0])]
+    for i in range(L):
+        out.append(("ResBlock L%d" % i, "k3s1", W[i], W[i], ext[i]))
+        if i > 0:
+            out.append(("down_layers.%d.0" % i, "k3s2", W[i - 1], W[i], ext[i]))
+    for j in range(L - 1):
+        out.append(("up_samples.%d.0" % (L - 2 - j), "k1", 2 * W[j], W[j], ext[j + 1]))
+    return out
+
+
+# the weight-gradient routes of the BraTS recipe (batch 1, 4 x 224 x 224 x 144, init_filters 16) on a 132-SM H100: (kind, K
+# chunk, BN) per precision
+BRATS_WGRAD_ROUTES = {
+    "bf16": {
+        "convInit": ("halo", 64, 16), "ResBlock L0": ("halo", 64, 16), "ResBlock L1": ("halo", 64, 32),
+        "down_layers.1.0": ("tap", 16, 32), "ResBlock L2": ("halo", 64, 64), "down_layers.2.0": ("tap", 32, 64),
+        "ResBlock L3": ("tap", 64, 128), "down_layers.3.0": ("tap", 64, 128),
+        "up_samples.2.0": ("tap", 32, 16), "up_samples.1.0": ("tap", 64, 32), "up_samples.0.0": ("tap", 64, 64),
+    },
+    "split": {   # no halo mode for hi + lo operands: the per-tap kernel, K chunks of the input width
+        "convInit": ("tap", 16, 16), "ResBlock L0": ("tap", 16, 16), "ResBlock L1": ("tap", 32, 32),
+        "down_layers.1.0": ("tap", 16, 32), "ResBlock L2": ("tap", 64, 64), "down_layers.2.0": ("tap", 32, 64),
+        "ResBlock L3": ("tap", 64, 128), "down_layers.3.0": ("tap", 64, 128),
+        "up_samples.2.0": ("tap", 32, 16), "up_samples.1.0": ("tap", 64, 32), "up_samples.0.0": ("tap", 64, 64),
+    },
+}
+
+
+def wgrad_route_table(L, split, n=1, in_channels=4, init_filters=16, dims=(224, 224, 144), num_sms=132):
+    """{label: (kind, K chunk, BN)} from the library's weight-gradient route query"""
+    from conv_route_cases import wgrad_query
+    out = {}
+    for label, op, ci, co, ext in wgrad_layers(in_channels, init_filters, dims):
+        r = wgrad_query(L, op, ci, co, ext, split, num_sms=num_sms, n=n)
+        out[label] = None if r is None else (r["kind"], r["cb"], r["bn"])
     return out
 
 

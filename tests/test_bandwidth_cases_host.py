@@ -20,6 +20,12 @@ def test_launch_rule_restatement():
     assert B.upsample_bwd_kernel(False, (2, 4, 6)) == "blk"
     assert B.upsample_bwd_kernel(True, (2, 4, 6)) == B.upsample_bwd_kernel(False, (1, 4, 6)) == B.upsample_bwd_kernel(False, (3, 4, 6)) == "gather"
     assert B.bias_grad_geometry(2, 32, (128, 128, 128))[:3] == (592, 256, True)
+    # SIMT head forward at the BraTS SegResNet size: 7,225,344 voxels over 2112 blocks of 256 threads, 13.4 sweeps
+    assert B.head_fwd_geometry(1, 16, (224, 224, 144)) == (2112, 256, True, True)
+    # head_dbias: 128 blocks per output; 220.5 sweeps of 32,768 voxels at 224 x 224 x 144, 64 exact ones at 128^3
+    assert B.head_dbias_geometry(1, (224, 224, 144)) == (128, 256, True, True)
+    assert B.head_dbias_geometry(2, (128, 128, 128)) == (128, 256, True, False)
+    assert B.head_dbias_geometry(2, (24, 40, 32))[:3] == (120, 256, False)
 
 
 @pytest.mark.parametrize("case", B.CASES, ids=lambda c: c.id)
@@ -37,7 +43,8 @@ def test_plan_regimes_include_the_capped_grids():
     """the benchmark-size plans run every keyed kernel with a clamped grid, so the table must hold capped cases of each"""
     keys = B.plan_keys()
     capped = {k[0] for k in keys if k[2] == "capped"}
-    assert capped >= {"gn", "act_bwd", "up_fwd", "up_bwd_blk", "up_bwd_gather", "bias_grad", "head_bwd"}
+    assert capped >= {"gn", "act_bwd", "up_fwd", "up_add", "up_bwd_blk", "up_bwd_gather", "bias_grad", "head_bwd", "head_fwd",
+                      "head_dbias"}
     assert ("up_fwd", "npow2", "capped", "tail", "bf16", "view") in keys          # C5: widths 48 .. 768
     assert any(k[0] == "gn" and k[1] == "wide" for k in keys)                     # C5 and BraTS: more than 256 channels
 
@@ -45,5 +52,17 @@ def test_plan_regimes_include_the_capped_grids():
 def test_case_ids_are_unique_and_each_kernel_has_both_precisions():
     ids = collections.Counter(c.id for c in B.CASES)
     assert max(ids.values()) == 1
-    for kernel in {c.kernel for c in B.CASES}:
+    for kernel in {c.kernel for c in B.CASES} - {"head_dbias"}:     # k_head_dbias reads only the fp32 dlogits
         assert {c.split for c in B.CASES if c.kernel == kernel} == {False, True}, kernel
+    assert {c.key[4] for c in B.CASES if c.kernel == "head_dbias"} == {"fp32"}
+
+
+def test_gn_cases_hold_every_backward_variant_of_the_plans():
+    """the regime key does not carry what k_gn_bwd adds and scales, so the variants the training plans hand it are checked here:
+    each has a case in both precisions, and SegResNet's residual addend + Dropout3d scale also with a whole-buffer addend"""
+    variants = B.plan_gn_bwd_variants()
+    assert set(variants) == {"plain", "add1", "add1+scale"}
+    assert any(name.startswith("brats-segresnet") for name in variants["add1+scale"])
+    for v in variants:
+        assert {c.split for c in B.GN_CASES if c.opt["bwd"] == v} == {False, True}, v
+    assert {c.split for c in B.GN_CASES if c.opt["bwd"] == "add1+scale" and c.opt.get("whole")} == {False, True}

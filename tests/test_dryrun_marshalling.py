@@ -202,3 +202,41 @@ def test_bandwidth_kernel_diagnostics_marshal(pkg, stubbed):
     L.input_grad(None, None, None, None, 0, b, 4, torch.zeros(1, 4, 4, 8, 8))
     assert {"b200unet_diag_gn_bwd", "b200unet_act_bwd", "b200unet_diag_bias_grad", "b200unet_diag_head_fwd", "b200unet_diag_head_dbias",
             "b200unet_diag_head_bwd", "b200unet_diag_input_pack", "b200unet_diag_input_grad"} <= set(stubbed)
+
+
+def test_segresnet_calls(pkg, stubbed):
+    """SegResNet reaches the library as arch 2 with blocks_down / blocks_up on the levels, and its training forward hands over the
+    (N, init_filters) Dropout3d scale; eval and no-dropout forwards hand over none"""
+    L = pkg.lib
+    model = pkg.SegResNet(init_filters=8, in_channels=4, out_channels=3, dropout_prob=0.2, blocks_down=(1, 2, 3), blocks_up=(2, 1),
+                          norm=("GROUP", {"num_groups": 4}), act=("leakyrelu", {"negative_slope": 0.1}))
+    d = model._net_desc(1, 16, 16, 16)
+    assert (d.arch, d.n_levels, d.base_width, d.norm_groups, d.n_features, d.n_outputs) == (2, 3, 8, 4, 4, 3)
+    assert list(d.encoder_blocks)[:4] == [1, 2, 3, 0] and list(d.decoder_blocks)[:3] == [2, 1, 0]
+    assert d.act_slope == pytest.approx(0.1)
+    drops = []
+    fwd = L._lib.b200unet_plan_forward
+
+    def record(*args):
+        drops.append(args[3])
+        return fwd(*args)
+    L._lib.b200unet_plan_forward = record
+    x, t = _batch()
+    model.train()
+    scale = fake(torch.full((1, 8), 1.25))
+    model.set_dropout_scale(scale)
+    pkg.DiceLoss(sigmoid=True)(fake(model(x)), t).backward()
+    assert all(p.grad is not None and p.grad.shape == p.shape for p in model.parameters())
+    assert stubbed.count("b200unet_plan_forward") == 1 and stubbed.count("b200unet_plan_backward") == 1
+    assert drops == [scale.data_ptr()]
+    model.set_dropout_scale(None)
+    model(x).sum().backward()                       # a random keep / (1 - p) scale of its own
+    assert drops[-1] not in (None, 0, scale.data_ptr())
+    model.eval()
+    with torch.no_grad():
+        assert model(x).shape == (1, 3, 16, 16, 16)
+    assert drops[-1] is None
+    plain = pkg.SegResNet(init_filters=8, in_channels=4, out_channels=3, blocks_down=(1, 1), blocks_up=(1,))
+    plain.train()
+    plain(x).sum().backward()
+    assert drops[-1] is None

@@ -1,7 +1,7 @@
 """The bandwidth-bound kernels of csrc/elementwise.cu against fp64, element by element, at the launch geometries the plans give
 them (tests/bandwidth_cases.py): GroupNorm apply / backward / finalize, the activation backward, the x2 up-sampling forward and
-backward, the transposed-convolution bias gradient and the 1..8-output head, plus zero insertion, input packing, the input
-gradient and the layout converters.
+backward, the fused up-sampling + skip-add, the transposed-convolution bias gradient and the 1..8-output head (forward, backward
+and bias gradient), plus zero insertion, input packing, the input gradient and the layout converters.
 
 Inputs are built in torch and rounded to bf16 there (hi, or hi + lo); the reference reads the exact fp64 value each one stores.
 Outputs are read straight from their hi / lo tensors, never through the library's converters, and are views at channel 8 of
@@ -83,14 +83,15 @@ def untouched(buf, c):
 
 
 def check(got, ref, absb, r, a, what, mask=None):
-    """|got - ref| <= r |ref| + a * absb at every element (of mask); names the worst element"""
+    """|got - ref| <= r |ref| + a * absb at every element (of mask); names the worst element.  A NaN (an output the kernel never
+    wrote keeps the NaN it was filled with) is out of bounds."""
     err = (got - ref).abs()
     lim = r * ref.abs() + a * absb + 1e-300
-    bad = err > lim
+    bad = ~(err <= lim)
     if mask is not None:
         bad &= mask
     if bool(bad.any()):
-        worst = int(((err - lim) * bad).flatten().argmax())
+        worst = int(torch.where(bad, (err - lim).nan_to_num(float("inf")), -1.0).flatten().argmax())
         idx = tuple(int(i) for i in torch.unravel_index(torch.tensor(worst), got.shape))
         pytest.fail("%s: %d of %d elements out of bounds; worst at %s: got %.10g ref %.10g bound %.3g"
                     % (what, int(bad.sum()), bad.numel(), idx, float(got[idx]), float(ref[idx]), float(lim[idx])))
@@ -184,21 +185,22 @@ def test_groupnorm_apply_backward_finalize(L, case):
     # from the exact mu and rstd, the statistics from the stored fp32 ones; dbeta does not depend on them)
     check(dg2.double(), bst[:, :real, 1].sum(0), bst[:, :real, 1].abs().sum(0), 2 * U, 2.0 ** -40, "dgamma (finalize)")
     check(db2.double(), bq.grad, bst[:, :real, 0].abs().sum(0), 2 * U, 2.0 ** -40, "dbeta (finalize)")
-    # dx = (A dz + E x + F (+ add1) (+ add2)) * scale: against autograd of torch's group_norm
+    # dx = (A dz + E x + F (+ add1) (+ add2)) * scale: against autograd of torch's group_norm; add1 is a channel slice, or a whole
+    # buffer as SegResNet's ResBlocks hand over their output gradient
     ref = torch.zeros(n, *dims, c, dtype=f64, device=DEV)
     ref[..., :real] = ndhwc(xq.grad)
     absb = (A32 * dzv).abs()
     absb[..., :real] += (k2[:, None, None, None, :real, 0] * xr).abs() + k2[:, None, None, None, :real, 1].abs()
     kw = {}
     if "add1" in variant:
-        a1, a1v = rand_in(L, n, c, dims, split, gen, c_view=c + 8, c0=8)
+        a1, a1v = rand_in(L, n, c, dims, split, gen) if o.get("whole") else rand_in(L, n, c, dims, split, gen, c_view=c + 8, c0=8)
         kw["add1"] = a1
         ref, absb = ref + a1v, absb + a1v.abs()
     if "add2" in variant:
         a2, a2v = rand_in(L, n, c, dims, split, gen)
         kw["add2"] = a2
         ref, absb = ref + a2v, absb + a2v.abs()
-    if variant == "scale":
+    if "scale" in variant:
         kw["scale"] = torch.tensor([0.0, 0.8, 1.25], device=DEV)[torch.randint(0, 3, (n, c), generator=gen, device=DEV)]
         s = kw["scale"].double()[:, None, None, None, :]
         ref, absb = ref * s, absb * s
@@ -324,13 +326,44 @@ def test_upsample_forward_refuses_more_than_2048_channels(L):
         L.upsample2x_fwd(x, y)
 
 
+def check_upsample_skip_add(L, n, c, dims, split, gen):
+    """y = trilinear x2 of p + skip into a whole buffer, and the per-channel (sum, sumsq) of y"""
+    od = tuple(2 * d for d in dims)
+    p, pv = rand_in(L, n, c, dims, split, gen, shift=0.25)
+    s, sv = rand_in(L, n, c, od, split, gen)
+    y = L.Act.empty(n, *od, c, split=split)
+    stats = torch.zeros(n, c, 2, dtype=f64, device=DEV)
+    L.upsample2x_fwd(p, y, stats, c, add=s)
+    torch.cuda.synchronize()
+    ref = _up(pv) + sv
+    absb = _up(pv.abs()) + sv.abs()
+    check(got_of(y), ref, absb, R_STORE[split], 10 * U, "y")
+    # statistics: the fp32 values before storage, summed in chains of 8 per 2 x 2 x 2 block
+    blocks, threads, _, _ = B.upsample_fwd_geometry(n, c, dims)
+    nblk = (dims[0] + 1) * (dims[1] + 1) * (dims[2] + 1)
+    chain = 8 * -(-nblk // (blocks * (threads // (c // 8)))) + 6      # 8 outputs per 2 x 2 x 2 block, then the shuffles
+    e = 10 * U * absb
+    s1, s2 = chan_sums(ref), chan_sums(ref * ref)
+    b1 = chan_sums(e) + chain * U * chan_sums(absb)
+    b2 = chan_sums(2 * ref.abs() * e + e * e) + chain * U * chan_sums(ref * ref)
+    assert bool(((stats[..., 0] - s1).abs() <= b1).all()), "per-channel sums"
+    assert bool(((stats[..., 1] - s2).abs() <= b2).all()), "per-channel sums of squares"
+
+
+@pytest.mark.parametrize("case", B.UP_ADD_CASES, ids=lambda c: c.id)
+def test_upsample_skip_add_forward_and_statistics(L, case):
+    """the fused x2 up-sampling + skip-add of SegResNet's decoder, with the statistics of the sum, in every regime of the plans"""
+    check_upsample_skip_add(L, case.n, case.c, case.dims, case.split, gen_of(case.id))
+
+
 @pytest.mark.parametrize("case", B.UP_BWD_CASES, ids=lambda c: c.id)
 def test_upsample_backward_from_concat_gradient(L, case):
-    """dx = the adjoint of the x2 up-sampling, reading dy as channels [0, C) of a 2C-channel concat gradient as the plans do"""
+    """dx = the adjoint of the x2 up-sampling, reading dy as channels [0, C) of a 2C-channel concat gradient as the UNet3D plans
+    do (case.view), or from a whole C-channel buffer as SegResNet's decoder does"""
     n, c, dims, split = case.n, case.c, case.dims, case.split
     gen = gen_of(case.id)
     od = tuple(2 * d for d in dims)
-    dy, dyv = rand_in(L, n, c, od, split, gen, c_view=2 * c)
+    dy, dyv = rand_in(L, n, c, od, split, gen, c_view=2 * c if case.view else None)
     dxbuf, dx = out_view(L, n, dims, c, split)
     L.upsample2x_bwd(dy, dx)
     torch.cuda.synchronize()
@@ -393,6 +426,42 @@ def test_head_backward(L, case):
     check(dw.double(), ref, torch.einsum("ndhwo,ndhwc->oc", dlv.abs(), xv.abs()), 0.0, chain * U, "dw")
 
 
+@pytest.mark.parametrize("case", B.HEAD_FWD_CASES, ids=lambda c: c.id)
+def test_head_forward_at_plan_geometries(L, case):
+    """logits = w x (+ b) of the SIMT head at the plans' grids, clamped ones with a partial last sweep included"""
+    n, c, dims, split, no = case.n, case.c, case.dims, case.split, case.opt["o"]
+    gen = gen_of(case.id)
+    x, xv = rand_in(L, n, c, dims, split, gen)
+    w = torch.randn(no, c, generator=gen, device=DEV) * 0.3
+    bias = torch.randn(no, generator=gen, device=DEV)
+    for b in (None, bias):
+        zref = ndhwc_to_out(xv @ w.double().t() + (b.double() if b is not None else 0))
+        zabs = ndhwc_to_out(xv.abs() @ w.double().abs().t() + (b.double().abs() if b is not None else 0))
+        logits = torch.full((n, no, *dims), float("nan"), device=DEV)
+        L.head_fwd_ex(x, w, b, no, 0, logits)
+        torch.cuda.synchronize()
+        check(logits.double(), zref, zabs, 0.0, (c + 2) * U, "logits (bias %s)" % (b is not None))
+
+
+def head_dbias_chain(dims):
+    """values a thread of k_head_dbias adds in fp32 per sample (its sweeps), plus one"""
+    blocks, threads, _, _ = B.head_dbias_geometry(1, dims)
+    return -(-B.vol(dims) // (blocks * threads)) + 1
+
+
+@pytest.mark.parametrize("case", B.HEAD_DBIAS_CASES, ids=lambda c: c.id)
+def test_head_bias_gradient_at_plan_geometries(L, case):
+    """dbias = the sum of dlogits over samples and voxels, at the plans' grids: 128 blocks per output and hundreds of sweeps at
+    224 x 224 x 144, a partial last sweep, one sample and several"""
+    n, dims, no = case.n, case.dims, case.opt["o"]
+    dl = torch.randn(n, no, *dims, generator=gen_of(case.id), device=DEV) + 0.5
+    db = torch.full((no,), float("nan"), device=DEV)
+    L.head_dbias(dl, db)
+    torch.cuda.synchronize()
+    d = dl.double()
+    check(db.double(), d.sum(dim=(0, 2, 3, 4)), d.abs().sum(dim=(0, 2, 3, 4)), U, head_dbias_chain(dims) * U, "head dbias")
+
+
 @pytest.mark.parametrize("c", [8, 24, 32, 48, 64])
 @pytest.mark.parametrize("n_out", range(1, 9))
 def test_head_forward_bias_and_epilogues(L, n_out, c):
@@ -425,10 +494,8 @@ def test_head_forward_bias_and_epilogues(L, n_out, c):
     db = torch.full((n_out,), float("nan"), device=DEV)
     L.head_dbias(dl, db)
     torch.cuda.synchronize()
-    S = B.vol(dims)
-    chain = -(-S // (max(1, min(-(-S // 256), 128)) * 256)) + 1
     d = dl.double()
-    check(db.double(), d.sum(dim=(0, 2, 3, 4)), d.abs().sum(dim=(0, 2, 3, 4)), U, chain * U, "head dbias")
+    check(db.double(), d.sum(dim=(0, 2, 3, 4)), d.abs().sum(dim=(0, 2, 3, 4)), U, head_dbias_chain(dims) * U, "head dbias")
 
 
 def ndhwc_to_out(v):

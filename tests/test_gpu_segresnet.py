@@ -6,12 +6,11 @@ import zlib
 
 import pytest
 import torch
-import torch.nn.functional as F
 
-import bandwidth_cases as B
 import segresnet_cases as S
 from oracle import sliding_window_inference
 from oracle.segresnet_oracle import segresnet_forward
+from test_gpu_bandwidth_kernels import check_upsample_skip_add
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -74,14 +73,22 @@ def test_segresnet_smooth_network_tight_bounds(pkg, input_grad):
         assert S.rel_l2(x.grad, ref["dx"]) < b["grad"]
 
 
-def test_segresnet_bf16_mode_dice_bound(pkg):
-    case = S.RELU_CASES[1]
+def _check_bf16_dice_bound(pkg, case):
     ref = S.reference(case)
     m, x, t = _model(pkg, case, precision="bf16")
     out, loss = _step(pkg, m, x, t)
     assert abs(float(loss) - float(ref["loss"])) < S.BF16_DICE
     assert S.rel_l2(out, ref["logits"]) < S.BF16_LOGITS
     assert all(torch.isfinite(p.grad).all() for p in m.parameters())
+
+
+def test_segresnet_bf16_mode_dice_bound(pkg):
+    _check_bf16_dice_bound(pkg, S.RELU_CASES[1])
+
+
+def test_segresnet_npow2_widths_bf16_mode_dice_bound(pkg):
+    """widths 24 .. 192, 3 channels per group, 12 input channels, 5 outputs, a forced dropout scale"""
+    _check_bf16_dice_bound(pkg, S.NPOW2_CASE)
 
 
 def test_segresnet_input_gradient_matches_oracle(pkg):
@@ -143,48 +150,13 @@ def test_segresnet_sliding_window_inference(pkg):
 
 
 # ------------------------------------------------------------------------------------------------ fused up-sample + skip-add
-U = 2.0 ** -24
-R_STORE = {False: 2.0 ** -8, True: 2.0 ** -16}
-
-
-def _act(L, v, split):
-    hi = v.bfloat16()
-    lo = (v - hi.float()).bfloat16() if split else None
-    return L.Act(hi.contiguous(), lo.contiguous() if split else None), hi.double() + (lo.double() if split else 0)
-
-
 @pytest.mark.parametrize("split", [False, True], ids=["bf16", "split"])
 @pytest.mark.parametrize("geom", S.upskip_geometries(), ids=lambda g: "n%d-c%d-%s" % (g[0], g[1], "x".join(map(str, g[2]))))
 def test_upsample_skip_add_forward_and_statistics(pkg, geom, split):
-    """y = trilinear x2 of p + skip and the per-channel (sum, sumsq) of y, at the SegResNet plans' launch geometries"""
-    L = pkg.lib
-    n, c, dims = geom
+    """y = trilinear x2 of p + skip and the per-channel (sum, sumsq) of y, at the SegResNet plans' launch geometries (the bounds:
+    tests/test_gpu_bandwidth_kernels.py, whose cases cover every regime of these launches)"""
     gen = torch.Generator(device=DEV).manual_seed(zlib.crc32(repr(geom).encode()))
-    od = tuple(2 * d for d in dims)
-    p, pv = _act(L, torch.randn(n, *dims, c, generator=gen, device=DEV) + 0.25, split)
-    s, sv = _act(L, torch.randn(n, *od, c, generator=gen, device=DEV), split)
-    y = L.Act.empty(n, *od, c, split=split)
-    stats = torch.zeros(n, c, 2, dtype=torch.float64, device=DEV)
-    L.upsample2x_fwd(p, y, stats, c, add=s)
-    torch.cuda.synchronize()
-
-    def up(v):
-        return F.interpolate(v.permute(0, 4, 1, 2, 3), scale_factor=2, mode="trilinear", align_corners=False).permute(0, 2, 3, 4, 1)
-    ref = up(pv) + sv
-    absb = up(pv.abs()) + sv.abs()
-    got = y.hi.double() + (y.lo.double() if split else 0)
-    err, lim = (got - ref).abs(), R_STORE[split] * ref.abs() + 10 * U * absb + 1e-300
-    assert bool((err <= lim).all()), "y: %d elements out of bounds" % int((err > lim).sum())
-    # statistics: the fp32 values before storage, summed in chains of 8 per 2 x 2 x 2 block
-    blocks, threads, _, _ = B.upsample_fwd_geometry(n, c, dims)
-    nblk = (dims[0] + 1) * (dims[1] + 1) * (dims[2] + 1)
-    chain = 8 * -(-nblk // (blocks * (threads // (c // 8)))) + 6      # 8 outputs per 2 x 2 x 2 block, then the shuffles
-    e = 10 * U * absb
-    s1, s2 = ref.sum(dim=(1, 2, 3)), (ref * ref).sum(dim=(1, 2, 3))
-    b1 = e.sum(dim=(1, 2, 3)) + chain * U * absb.sum(dim=(1, 2, 3))
-    b2 = (2 * ref.abs() * e + e * e).sum(dim=(1, 2, 3)) + chain * U * (ref * ref).sum(dim=(1, 2, 3))
-    assert bool(((stats[..., 0] - s1).abs() <= b1).all()), "per-channel sums"
-    assert bool(((stats[..., 1] - s2).abs() <= b2).all()), "per-channel sums of squares"
+    check_upsample_skip_add(pkg.lib, *geom, split, gen)
 
 
 def test_upsample_skip_add_rejects_a_mismatched_addend(pkg):

@@ -32,6 +32,17 @@ def test_state_dict_and_plan_spec(pkg, kw):
     m.load_state_dict(make_segresnet_state_dict(**S.spec_kw(kw)), strict=True)
 
 
+def test_npow2_case_plan_spec(pkg):
+    """the non-power-of-two case of the GPU tests: its plan builds at the case's shape with the oracle's spec, 12 input channels
+    packed into 16"""
+    case = S.NPOW2_CASE
+    m = pkg.SegResNet(**case.kw)
+    spec = segresnet_state_dict_spec(**S.spec_kw(case.kw))
+    assert [(k, tuple(v.shape)) for k, v in m.state_dict().items()] == spec
+    assert (m.num_groups, m.dropout_width) == (8, 24)
+    assert _plan(pkg, m, case.shape[0], case.shape[2:]).param_spec() == spec
+
+
 def test_monai_defaults_and_init(pkg):
     m = pkg.SegResNet()
     assert (m.init_filters, m.in_channels, m.out_channels, m.blocks_down, m.blocks_up, m.num_groups) == (8, 1, 2, [1, 2, 2, 4], [1, 1, 1], 8)
@@ -172,8 +183,17 @@ def test_relu_split_bounds_sit_above_the_noise_floor():
         assert floor["logits"] <= S.RELU_BOUNDS["logits"] / 4 and floor["loss"] <= S.RELU_BOUNDS["loss"] / 4, (case.id, floor["logits"])
 
 
+def _bf16_floor_below_bounds(case):
+    floor = S.noise_floor(case, 2.0 ** -8, runs=1, input_grad=False)
+    assert floor["loss"] * float(S.reference(case)["loss"]) <= S.BF16_DICE
+    assert floor["logits"] <= S.BF16_LOGITS
+
+
 def test_bf16_dice_bound_sits_above_the_noise_floor():
     """bf16 storage (eps 2^-8) moves the sigmoid Dice of the bf16 case by less than its bound"""
-    floor = S.noise_floor(S.RELU_CASES[1], 2.0 ** -8, runs=1, input_grad=False)
-    assert floor["loss"] * float(S.reference(S.RELU_CASES[1])["loss"]) <= S.BF16_DICE
-    assert floor["logits"] <= S.BF16_LOGITS
+    _bf16_floor_below_bounds(S.RELU_CASES[1])
+
+
+def test_npow2_bf16_dice_bound_sits_above_the_noise_floor():
+    """the same for the non-power-of-two widths of tests/test_gpu_segresnet.py's second bf16 run"""
+    _bf16_floor_below_bounds(S.NPOW2_CASE)

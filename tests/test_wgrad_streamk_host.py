@@ -1,6 +1,6 @@
 """The stream-K partition of the per-tap weight gradient (wgrad.cu: wgrad_tiling, k_wgrad), restated in Python and held to the
-library's route query over the weight-gradient launch shapes of the C2 and C3 UNet3D plans and the BraTS DynUNet plan, on 114
-and 132 SMs.  A work item is (M-tile group, N tile); an iteration is (work item, voxel tile), items outer.  CTA c of P runs
+library's route query over the weight-gradient launch shapes of the C2 and C3 UNet3D plans, the BraTS DynUNet plan and the BraTS
+SegResNet recipe (batch 1 at 224 x 224 x 144, batch 2 at 128^3), on 114 and 132 SMs.  A work item is (M-tile group, N tile); an iteration is (work item, voxel tile), items outer.  CTA c of P runs
 iterations [c * T / P, (c + 1) * T / P): every iteration once, per-CTA work within one voxel tile, and in deterministic mode
 each CTA stores into the slot of its rank among the CTAs of its item, below the route's split count."""
 import math
@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 import conv_route_cases as R
+import segresnet_cases as S
 
 
 def pick_tile(w, h, d):
@@ -65,7 +66,14 @@ def dynunet_wgrads(dims, filters=(64, 96, 128, 192, 256, 384)):
     return out
 
 
-PLANS = {"C2": unet3d_wgrads((128, 128, 128)), "C3": unet3d_wgrads((160, 192, 128)), "brats-dynunet": dynunet_wgrads((128, 128, 128))}
+def segresnet_wgrads(dims, in_channels=4, init_filters=16):
+    """the BraTS SegResNet recipe (segresnet_cases.wgrad_layers)"""
+    return [(op, ci, co, ext) for _, op, ci, co, ext in S.wgrad_layers(in_channels, init_filters, dims)]
+
+
+PLANS = {"C2": unet3d_wgrads((128, 128, 128)), "C3": unet3d_wgrads((160, 192, 128)), "brats-dynunet": dynunet_wgrads((128, 128, 128)),
+         "brats-segresnet": segresnet_wgrads((224, 224, 144)), "brats-segresnet-128": segresnet_wgrads((128, 128, 128))}
+BATCH = {"brats-segresnet": 1}          # every other plan trains at batch 2
 CASES = sorted({(plan, *shape) for plan, shapes in PLANS.items() for shape in shapes})
 
 
@@ -108,14 +116,15 @@ def restate(op, ci, co, dims, num_sms, n=2):
 @pytest.mark.parametrize("num_sms", [114, 132])
 @pytest.mark.parametrize("plan,op,ci,co,dims", CASES, ids=lambda v: str(v))
 def test_streamk_partition(L, plan, op, ci, co, dims, num_sms):
+    n = BATCH.get(plan, 2)
     for split in (False, True):
-        r = R.wgrad_query(L, op, ci, co, dims, split, num_sms=num_sms)
+        r = R.wgrad_query(L, op, ci, co, dims, split, num_sms=num_sms, n=n)
         assert r is not None, (op, ci, co, dims)
         if r["kind"] != "tap":
             continue
-        fields, ranges, first, T, kblocks = restate(op, ci, co, dims, num_sms)
+        fields, ranges, first, T, kblocks = restate(op, ci, co, dims, num_sms, n=n)
         assert {k: r[k] for k in fields} == fields
-        assert R.wgrad_query(L, op, ci, co, dims, split, deterministic=True, num_sms=num_sms) == r
+        assert R.wgrad_query(L, op, ci, co, dims, split, deterministic=True, num_sms=num_sms, n=n) == r
         # every CTA of the machine works unless there are fewer iterations
         assert r["ctas"] == min(num_sms, T)
         # every (item, voxel tile) exactly once: the ranges tile [0, T) in order
@@ -142,3 +151,13 @@ def test_wide_c2_launches_fill_every_sm(L):
     for op, ci, co, dims in wide:
         r = R.wgrad_query(L, op, ci, co, dims)
         assert r["kind"] == "tap" and r["ctas"] == 132, (op, ci, co, dims, r)
+
+
+@pytest.mark.parametrize("precision", ["bf16", "split"])
+def test_segresnet_brats_wgrad_routes(L, precision):
+    """the weight-gradient route of every SegResNet layer of the BraTS recipe on a 132-SM H100 (the table the at-size GPU test
+    asserts), and the per-tap ones split over every SM"""
+    assert S.wgrad_route_table(L, precision == "split") == S.BRATS_WGRAD_ROUTES[precision]
+    for _, op, ci, co, ext in S.wgrad_layers(4, 16, (224, 224, 144)):
+        r = R.wgrad_query(L, op, ci, co, ext, precision == "split", n=1)
+        assert r["ctas"] == 132, (op, ci, co, ext, r)
