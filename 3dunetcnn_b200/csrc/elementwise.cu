@@ -581,7 +581,10 @@ int launch_upsample2x_fwd(const Act& x, const Act& y, double* stats, int stats_l
   const long long nblk = (long long)(x.D + 1) * (x.H + 1) * (x.W + 1);
   B200_REQUIRE(nblk < (1LL << 31), E_UNSUPPORTED, "upsample: volume too large");
   long long want = (nblk + vper - 1) / vper;
-  const long long cap = (132LL * 8 + x.N - 1) / x.N;
+  // at most 4 blocks per SM for EACH sample, whatever the batch (the grid of a batch of two is unchanged): the blocks' fp32
+  // partial sums of the statistics then cover the same voxels at every batch size, so a sample's statistics, and its outputs,
+  // do not depend on what else is in the batch
+  const long long cap = 132LL * 4;
   const int blocks = (int)(want < cap ? (want > 0 ? want : 1) : cap);
   if (add) k_upsample2x_fwd<true><<<dim3(blocks, x.N), threads, x.C * 2 * sizeof(double), st>>>(x, y, stats, stats_ld, *add);
   else k_upsample2x_fwd<false><<<dim3(blocks, x.N), threads, x.C * 2 * sizeof(double), st>>>(x, y, stats, stats_ld, Act());

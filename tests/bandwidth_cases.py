@@ -71,12 +71,13 @@ def act_bwd_geometry(n, c, dims):
 
 
 def upsample_fwd_geometry(n, c, xdims):
-    """k_upsample2x_fwd (launch_upsample2x_fwd, :564-572): one thread per 2 x 2 x 2 output block, (D+1)(H+1)(W+1) blocks"""
+    """k_upsample2x_fwd (launch_upsample2x_fwd): one thread per 2 x 2 x 2 output block, (D+1)(H+1)(W+1) blocks, at most 4 blocks
+    per SM for each sample whatever the batch"""
     c8n = c // 8
     threads = ew_threads_for(c8n)
     vper = threads // c8n
     nblk = (xdims[0] + 1) * (xdims[1] + 1) * (xdims[2] + 1)
-    blocks, capped = _clamp((nblk + vper - 1) // vper, (SMS * 8 + n - 1) // n)
+    blocks, capped = _clamp((nblk + vper - 1) // vper, SMS * 4)
     return blocks, threads, capped, nblk % (blocks * vper) != 0
 
 

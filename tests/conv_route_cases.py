@@ -88,6 +88,8 @@ def conv_geometry(op, cin, dims):
         return (d // 2, h // 2, w // 2), 3, 1, 1
     if op == "class2":
         return (d // 2, h // 2, w // 2), 2, 2, 2
+    if op == "k2s2":   # unpadded kernel = stride 2 (the data gradient of a kernel-2 transposed convolution)
+        return (2 * d, 2 * h, 2 * w), 2, 2, 0
     raise ValueError(op)
 
 
@@ -306,6 +308,30 @@ CONV_CASES = [
     _C("class2", 64, 64, False, 0, 1, "class2", 72, 72, CL, kchunks=(2, 0)),
     _C("class2", 64, 64, True, 0, 1, "class2", 40, 40, CL),
 ]
+
+# Deep K loops: the route key leaves out how many K chunks a launch walks, and the cases above walk at most four (256 channels
+# of KC 16, 136 of KC 64).  The C5 network's 384- and 768-channel layers walk 6 and 12 chunks of 64 channels, the BraTS DynUNet's
+# up to 6; these cases walk 6, 7, 12 and 13 (392 and 776 channels: a partial last chunk), in both precisions and both epilogues,
+# on the second source too, and through the parity-class kernels.  test_conv_routes_host.py requires a case here or above that
+# walks at least as many chunks as any layer of the configurations the repository restates.
+DEEP_K_CASES = [
+    _C("tap", 64, 64, False, 0, 1, "k3s1", 776, 40, P, kchunks=(13, 0)),
+    _C("tap", 128, 64, False, 0, 1, "k3s1", 384, 200, P, kchunks=(6, 0)),
+    _C("tap", 64, 64, False, 0, 2, "k3s1", 384, 40, P, cin2=776, kchunks=(6, 13)),
+    _C("tap", 64, 64, True, 0, 1, "k3s1", 768, 40, P, kchunks=(12, 0)),
+    _C("tap", 64, 64, True, 0, 2, "k3s1", 392, 40, P, cin2=392, kchunks=(7, 7)),
+    _C("tap", 64, 64, False, 1, 1, "k3s1", 768, 40, P, kchunks=(12, 0)),
+    _C("tap", 64, 64, True, 1, 1, "k3s1", 392, 40, P, kchunks=(7, 0)),
+    _C("class1", 64, 64, False, 0, 1, "class1", 392, 72, CL, kchunks=(7, 0)),
+    _C("class1", 64, 64, True, 0, 1, "class1", 392, 40, CL, kchunks=(7, 0)),
+    _C("class2", 64, 64, False, 0, 1, "class2", 392, 72, CL, kchunks=(7, 0)),
+    _C("class2", 64, 64, True, 0, 1, "class2", 392, 40, CL, kchunks=(7, 0)),
+]
+
+
+def deep_k_id(case):
+    return "%s-cin%d%s" % (case.id, case.cin, "+%d" % case.cin2 if case.cin2 else "")
+
 
 # (kind, BN, KC) combinations B200_CONV_CONFIGS instantiates for no reachable launch, and why
 CONV_UNREACHABLE = {

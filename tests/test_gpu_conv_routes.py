@@ -1,5 +1,5 @@
-"""Every kernel route of the convolution and the weight gradient (tests/conv_route_cases.py) against an fp64 reference, element by
-element.  Each case first checks through the host query that it still takes its route, then launches it on inputs the
+"""Every kernel route of the convolution and the weight gradient (tests/conv_route_cases.py), and the deep K loops of the wide
+layers, against an fp64 reference, element by element.  Each case first checks through the host query that it still takes its route, then launches it on inputs the
 reference reads exactly (bf16 hi, or hi + lo, as stored), and bounds every element by
 
     |got - ref| <= r * |ref| + a * (|x| conv |w|)
@@ -219,6 +219,17 @@ def run_mode1(L, case, gen, slope):
 @pytest.mark.parametrize("case", R.CONV_CASES, ids=lambda c: c.id)
 def test_conv_route_matches_fp64(L, case):
     gen = torch.Generator().manual_seed(zlib.crc32(case.id.encode()))
+    if case.mode == 0:
+        run_mode0(L, case, gen)
+    else:
+        for slope in (0.0, 0.01):
+            run_mode1(L, case, gen, slope)
+
+
+@pytest.mark.parametrize("case", R.DEEP_K_CASES, ids=R.deep_k_id)
+def test_deep_k_conv_matches_fp64(L, case):
+    """6 to 13 K chunks of 64 channels per source (tests/conv_route_cases.py: DEEP_K_CASES), at the bounds above"""
+    gen = torch.Generator().manual_seed(zlib.crc32(R.deep_k_id(case).encode()))
     if case.mode == 0:
         run_mode0(L, case, gen)
     else:
