@@ -10,13 +10,14 @@ A regime key is (kernel, c8n class, capped, tail, precision, view):
   - view: the operand the plan hands over is a channel slice of a wider buffer.
 The SIMT head's forward keys the class of its input width, and its bias gradient (k_head_dbias, which reads only the fp32
 dlogits) keys "one-sample" / "batch" in the class slot and "fp32" as its precision.
-The functions below restate the launch code, so that a host test (tests/test_bandwidth_cases_host.py) derives the keys of the
-C2, C3 and C5 benchmark plans, the BraTS DynUNet and SegResNet plans, the SegResNet plan cases and the golden configurations, and
-requires a case for every one of them; tests/test_gpu_bandwidth_kernels.py runs the cases against fp64.  Line numbers refer to
-3dunetcnn_b200/csrc/elementwise.cu.
+The functions below restate the launch code, so that a host test (tests/test_bandwidth_cases_host.py) derives the keys of every
+plan configuration of tests/plan_launches.py and requires a case for every one of them; tests/test_gpu_bandwidth_kernels.py runs
+the cases against fp64.  Line numbers refer to 3dunetcnn_b200/csrc/elementwise.cu.
 """
 from dataclasses import dataclass, field
 from typing import Tuple
+
+import plan_launches as PL
 
 SMS = 132
 
@@ -164,170 +165,38 @@ def regime_key(kernel, n, c, dims, split, view):
 
 
 # ------------------------------------------------------------------------------------------------------ plan shapes
-def _half(dims, k):
-    return tuple(d >> k for d in dims)
+KERNELS = ("gn", "act_bwd", "up_fwd", "up_add", "up_bwd", "bias_grad", "head_fwd", "head_bwd", "head_dbias")
 
 
-def unet3d_launches(n, n_features, base_width, dims, encoder_blocks=(1, 2, 2, 4), decoder_blocks=None, convT=False, train=True):
-    """(kernel, n, c, dims, view[, GroupNorm backward variant]) of every launch of the bandwidth kernels in a UNet3D plan (plan.cu:
-    build_unet3d_plan).  The widths double per level; each residual block normalises its input and its first convolution's output;
-    a decoder stage runs its blocks at the width it receives, then a 1x1x1 convolution to the next width and the x2 up-sampling into
-    the low half of the concat buffer (or, with transposed convolutions, the zero insertion whose backward runs bias_grad on that
-    half).  The head has no bias.  The variant (training plans) is what build_block_bwd hands k_gn_bwd: "plain", "add1" (the
-    block's output gradient as the residual addend, when the block keeps its width) or "add1+scale" (and the Dropout3d scale); the
-    network's first norm runs no k_gn_bwd (None)."""
-    L = len(encoder_blocks)
-    decoder_blocks = list(decoder_blocks) if decoder_blocks is not None else list(encoder_blocks)
-    widths = [base_width * 2 ** k for k in range(L)]
-    ext = [_half(dims, k) for k in range(L)]
-    out = []
-
-    def block(cin, c, k, first=False, scale_in=False):
-        v1 = None if first else "plain" if cin != c else "add1+scale" if scale_in else "add1"
-        out.append(("gn", n, cin, ext[k], False, v1 if train else None))
-        out.append(("gn", n, c, ext[k], False, "plain" if train else None))
-    cin = 8 if n_features <= 8 else 16
-    for k in range(L):
-        for b in range(encoder_blocks[k]):
-            block(cin, widths[k], k, first=k == 0 and b == 0, scale_in=k == 0 and b == 1)
-            cin = widths[k]
-    for i in range(L - 1):
-        depth = L - 1 - i
-        for _ in range(decoder_blocks[i]):
-            block(cin, cin, depth)
-        out_w = widths[depth - 1]
-        if convT:
-            if train:
-                out.append(("bias_grad", n, out_w, ext[depth - 1], True))
-        else:
-            out.append(("up_fwd", n, out_w, ext[depth], True))
-            if train:
-                out.append(("up_bwd", n, out_w, ext[depth], True))
-        cin = 2 * out_w
-    for _ in range(decoder_blocks[L - 1]):
-        block(cin, base_width, 0)
-        cin = base_width
-    out.append(("head_fwd", n, base_width, dims, False))
-    if train:
-        out.append(("head_bwd", n, base_width, dims, False))
-    return out
-
-
-def dynunet_launches(n, filters, dims, train=True):
-    """DynUNet with post-activation blocks (conv -> InstanceNorm -> LeakyReLU, twice per block) and strides 1, 2, 2, ...: every norm
-    at level k has filters[k] channels; the backward runs act_bwd on each and k_gn_bwd without addend or scale (plan.cu:
-    build_dyn_block_bwd).  The head has a bias."""
-    out = []
-    L = len(filters)
-    for k in range(L):
-        per_level = 4 if k < L - 1 else 2     # encoder and decoder block, two norms each; the bottleneck has one block
-        for _ in range(per_level):
-            out.append(("gn", n, filters[k], _half(dims, k), False, "plain" if train else None))
-            if train:
-                out.append(("act_bwd", n, filters[k], _half(dims, k), False))
-    out.append(("head_fwd", n, filters[0], dims, False))
-    if train:
-        out.append(("head_bwd", n, filters[0], dims, False))
-        out.append(("head_dbias", n, filters[0], dims, False))
-    return out
-
-
-def segresnet_launches(n, F, dims, blocks_down=(1, 2, 2, 4), blocks_up=(1, 1, 1), train=True, dropout=True):
-    """SegResNet (plan.cu: build_segresnet): level i has F << i channels; every ResBlock normalises its input and its first
-    convolution's output, both whole buffers, and in the backward hands its output gradient to the first norm's k_gn_bwd as the
-    residual addend (the first encoder block also the Dropout3d scale of convInit's output, when dropout is on).  A decoder stage
-    runs the 1x1x1 convolution to C channels at the lower level's extents, then the fused x2 up-sampling + skip-add (up_add, a
-    whole C-channel output), its blocks, and in the backward the up-sampling's adjoint from the whole C-channel gradient.  The
-    head normalises F channels (act_bwd on it alone) and runs the biased 1x1x1 convolution."""
-    L = len(blocks_down)
-    ext = [_half(dims, k) for k in range(L)]
-    out = []
-
-    def block(c, k, scale_in=False):
-        out.append(("gn", n, c, ext[k], False, ("add1+scale" if scale_in else "add1") if train else None))
-        out.append(("gn", n, c, ext[k], False, "plain" if train else None))
-    for i in range(L):
-        for b in range(blocks_down[i]):
-            block(F << i, i, scale_in=dropout and i == 0 and b == 0)
-    for i in range(L - 1):
-        j = L - 2 - i
-        out.append(("up_add", n, F << j, ext[j + 1], False))
-        for _ in range(blocks_up[i]):
-            block(F << j, j)
-        if train:
-            out.append(("up_bwd", n, F << j, ext[j + 1], False))
-    out.append(("gn", n, F, dims, False, "plain" if train else None))
-    out.append(("head_fwd", n, F, dims, False))
-    if train:
-        out.append(("act_bwd", n, F, dims, False))
-        out.append(("head_bwd", n, F, dims, False))
-        out.append(("head_dbias", n, F, dims, False))
-    return out
-
-
-def _segresnet_case_launches(case):
-    """segresnet_launches of a tests/segresnet_cases.py plan case"""
-    bd, bu = case.blocks
-    return segresnet_launches(case.shape[0], case.kw.get("init_filters", 8), case.shape[2:], bd, bu,
-                              dropout=case.dropout or case.kw.get("dropout_prob", 0.0) > 0)
-
-
-# The configurations whose shapes the GPU cases must cover: the benchmark's C2 (4 channels, 128^3, width 32, batch 2; also with
-# transposed convolutions), C3 (160 x 192 x 128), C5 (1 channel, 5 levels [1, 2, 2, 4, 4], width 48, forward of 3 tiles of 128^3),
-# the BraTS DynUNet (examples/brats2020/brats2020_config.json: filters 64 .. 384, six levels; a 128^3 patch, batch 2), the BraTS
-# SegResNet recipe (init_filters 16, blocks_down [1, 2, 2, 4], blocks_up [1, 1, 1], dropout 0.2: training at 1 x 224 x 224 x 144
-# and 2 x 128^3, the two shapes tools/segresnet_bench.py times, and its forward-only plan), the SegResNet plan cases of
-# tests/segresnet_cases.py and the golden configurations of tests/golden/recipe.py.  Training plans run in both precisions.
 def plan_launches_by_config():
-    import segresnet_cases as SC
-    brats = dict(blocks_down=(1, 2, 2, 4), blocks_up=(1, 1, 1))
-    tr = [
-        ("C2", unet3d_launches(2, 4, 32, (128, 128, 128))),
-        ("C2-convT", unet3d_launches(2, 4, 32, (128, 128, 128), convT=True)),
-        ("C3", unet3d_launches(2, 4, 32, (160, 192, 128))),
-        ("brats-dynunet", dynunet_launches(2, [64, 96, 128, 192, 256, 384], (128, 128, 128))),
-        ("brats-segresnet", segresnet_launches(1, 16, (224, 224, 144), **brats)),
-        ("brats-segresnet-128", segresnet_launches(2, 16, (128, 128, 128), **brats)),
-        ("brats-segresnet-infer", segresnet_launches(1, 16, (224, 224, 144), train=False, **brats)),
-        ("golden-c1-32", unet3d_launches(1, 4, 8, (32, 32, 32))),
-        ("golden-c1-64", unet3d_launches(1, 4, 8, (64, 64, 64))),
-        ("golden-bw16", unet3d_launches(2, 4, 16, (32, 32, 32))),
-        ("golden-convT", unet3d_launches(1, 4, 8, (32, 32, 32), convT=True)),
-        ("golden-c5like", unet3d_launches(1, 1, 8, (32, 32, 32), encoder_blocks=(1, 2, 2, 4, 4), decoder_blocks=(1, 1, 1, 1, 1))),
-        ("golden-nonpow2", unet3d_launches(1, 4, 8, (24, 32, 40))),
-    ]
-    tr += [("segresnet-" + c.id, _segresnet_case_launches(c)) for c in SC.RELU_CASES + [SC.SMOOTH_CASE, SC.NPOW2_CASE]]
-    infer = [("C5", unet3d_launches(3, 1, 48, (128, 128, 128), encoder_blocks=(1, 2, 2, 4, 4), decoder_blocks=(1, 1, 1, 1, 1),
-                                    train=False))]
+    """(training plans, forward-only plans): [(config, [launch of a keyed kernel, ...]), ...] over every configuration of
+    tests/plan_launches.py"""
+    tr, infer = [], []
+    for c in PL.CONFIGS:
+        (tr if c.train else infer).append((c.name, [l for l in c.launches() if l.kernel in KERNELS]))
     return tr, infer
 
 
-def plan_launches():
-    tr, infer = plan_launches_by_config()
-    for name, launches in tr:
-        for split in (False, True):
-            for kernel, n, c, dims, view in (l[:5] for l in launches):
-                yield name, (kernel, n, c, dims, split, view)
-    for name, launches in infer:
-        for kernel, n, c, dims, view in (l[:5] for l in launches):
-            yield name, (kernel, n, c, dims, False, view)
-
-
 def plan_gn_bwd_variants():
-    """{k_gn_bwd variant: [config, ...]} over the training plans above (the regime key does not carry the variant)"""
+    """{k_gn_bwd variant: [config, ...]} over the training plans (the regime key does not carry the variant)"""
     out = {}
     for name, launches in plan_launches_by_config()[0]:
         for l in launches:
-            if l[0] == "gn" and l[5] is not None and name not in out.setdefault(l[5], []):
-                out[l[5]].append(name)
+            if l.variant is not None and name not in out.setdefault(l.variant, []):
+                out[l.variant].append(name)
     return out
 
 
 def plan_keys():
-    """{regime key: [(config, launch), ...]} over every plan above"""
+    """{regime key: [(config, launch), ...]} over every plan; training plans run in both precisions"""
     keys = {}
-    for name, (kernel, n, c, dims, split, view) in plan_launches():
-        keys.setdefault(regime_key(kernel, n, c, dims, split, view), []).append((name, (n, c, dims)))
+    tr, infer = plan_launches_by_config()
+    for plans, precisions in ((tr, (False, True)), (infer, (False,))):
+        for name, launches in plans:
+            for split in precisions:
+                for l in launches:
+                    key = regime_key(l.kernel, l.n, PL.pad8(l.c), l.dims, split, l.view)
+                    keys.setdefault(key, []).append((name, (l.n, PL.pad8(l.c), l.dims)))
     return keys
 
 

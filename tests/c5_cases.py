@@ -1,10 +1,10 @@
 """The C5 inference network (bench.py: 1 channel, 5 levels [1, 2, 2, 4, 4], base_width 48, three 128^3 tiles per forward) and
-the convolution launches of the UNet3D plans, restated from plan.cu: build_unet3d.
+the route of every forward convolution of its forward-only plan on a 132-SM H100, ``C5_ROUTES``, asserted by
+tests/test_conv_routes_host.py and tests/test_gpu_c5_size.py through the library's route query (include/b200unet_diag.h)."""
+import re
 
-``unet3d_conv_layers`` lists every convolution launch of a UNet3D plan with its route-query arguments; ``C5_ROUTES`` is the
-route of every forward convolution of the C5 forward-only plan on a 132-SM H100, asserted by tests/test_conv_routes_host.py and
-tests/test_gpu_c5_size.py through the library's route query (include/b200unet_diag.h)."""
 import bench
+import plan_launches as P
 
 C5 = dict(bench.CONFIGS["C5"]["model"])
 C5_BATCH = bench.CONFIGS["C5"]["sw_batch"]
@@ -13,69 +13,15 @@ C5_VOLUME = tuple(bench.CONFIGS["C5"]["volume"])
 C5_OVERLAP = bench.CONFIGS["C5"]["overlap"]
 
 
-def unet3d_conv_layers(n_features, base_width, dims, encoder_blocks=(1, 2, 2, 4), decoder_blocks=None, train=False):
-    """(label, op, cin, cout, output extents, epilogue mode, cin2) of every convolution launch of a UNet3D plan with trilinear
-    up-sampling (plan.cu: build_unet3d).  cin is the channel count of the source view (the packed input has its channels padded to
-    a multiple of 8), cin2 that of a fused 1x1x1 second source.
-
-    Forward: per residual block conv1 (3x3x3) and conv2 (3x3x3), which adds the block's `sample` 1x1x1 convolution of the block
-    input as its second source when the width changes (otherwise the input as a residual); the stride-2 downsampling convolution
-    of every level but the last; per decoder stage the blocks at the width the stage receives (the deeper stages read the 2C-channel
-    concat buffer), then the `pre_upsampling_blocks` 1x1x1 convolution to the next width.  Training plans add the data gradients
-    (build_block_bwd, emit_down_bwd): conv2 and conv1 through the GroupNorm + ReLU backward epilogue (mode 1), the sample
-    convolution's, the stride-2 convolution's on parity classes and the pre-up-sampling convolution's."""
-    L = len(encoder_blocks)
-    decoder_blocks = list(decoder_blocks) if decoder_blocks is not None else [1] * L
-    widths = [base_width << k for k in range(L)]
-    ext = [tuple(d >> k for d in dims) for k in range(L)]
-    out = []
-
-    def block(pre, xc, cin_real, C, k):
-        sample = xc if cin_real != C else 0
-        out.append((pre + ".conv1", "k3s1", xc, C, ext[k], 0, 0))
-        out.append((pre + ".conv2" + ("+sample" if sample else ""), "k3s1", C, C, ext[k], 0, sample))
-        if train:
-            out.append((pre + ".conv2.dgrad", "k3s1", C, C, ext[k], 1, 0))
-            out.append((pre + ".conv1.dgrad", "k3s1", C, xc, ext[k], 1, 0))
-            if sample and pre != "encoder.layers.0.blocks.0":
-                out.append((pre + ".sample.dgrad", "k1", C, xc, ext[k], 0, 0))
-
-    xc, cin_real = (n_features + 7) // 8 * 8, n_features
-    for k in range(L):
-        for b in range(encoder_blocks[k]):
-            block("encoder.layers.%d.blocks.%d" % (k, b), xc, cin_real, widths[k], k)
-            xc = cin_real = widths[k]
-        if k + 1 < L:
-            out.append(("encoder.downsampling_convolutions.%d" % k, "k3s2", widths[k], widths[k], ext[k + 1], 0, 0))
-            if train:
-                out.append(("encoder.downsampling_convolutions.%d.dgrad" % k, "class1", widths[k], widths[k], ext[k], 0, 0))
-    for i in range(L - 1):
-        depth = L - 1 - i
-        in_w = widths[depth] if depth == L - 1 else 2 * widths[depth]
-        for b in range(decoder_blocks[i]):
-            block("decoder.layers.%d.blocks.%d" % (i, b), in_w, in_w, in_w, depth)
-        out.append(("decoder.pre_upsampling_blocks.%d" % i, "k1", in_w, widths[depth - 1], ext[depth], 0, 0))
-        if train:
-            out.append(("decoder.pre_upsampling_blocks.%d.dgrad" % i, "k1", widths[depth - 1], in_w, ext[depth], 0, 0))
-    xc = 2 * base_width
-    for b in range(decoder_blocks[L - 1]):
-        block("decoder.layers.%d.blocks.%d" % (L - 1, b), xc, xc, base_width, 0)
-        xc = base_width
-    return out
-
-
-def conv_layers():
-    """the forward convolutions of the C5 forward-only plan: batch 3 (sw_batch) of 128^3 tiles"""
-    return unet3d_conv_layers(C5["n_features"], C5["base_width"], C5_ROI, C5["encoder_blocks"])
-
-
 def route_table(L, split):
-    """{label: (kind, BN, KC, kchunks)} of the C5 forward from the library's route query"""
-    from conv_route_cases import conv_query
+    """{label: (kind, BN, KC, kchunks)} of the C5 forward (tests/plan_launches.py) from the library's route query; a label is the
+    layer's state-dict name, with "+sample" when the launch adds the block's sample convolution"""
     out = {}
-    for label, op, ci, co, ext, mode, ci2 in conv_layers():
-        r = conv_query(L, op, ci, co, ext, split, mode, ci2, n=C5_BATCH)
-        out[label] = None if r is None else (r["kind"], r["bn"], r["kc"], r["kchunks"])
+    for l in P.BY_NAME["C5"].launches():
+        if l.kernel == "fwd":
+            r = P.conv_route(L, l, split)
+            out[re.sub(r"(\.conv)?\.weight$", "", l.key) + ("+sample" if l.key2 else "")] = \
+                None if r is None else (r["kind"], r["bn"], r["kc"], r["kchunks"])
     return out
 
 

@@ -29,6 +29,8 @@ import math
 from dataclasses import dataclass, field
 from typing import Tuple
 
+import plan_launches as PL
+
 SMS = 132
 U = 2.0 ** -24             # fp32 unit roundoff
 
@@ -192,20 +194,14 @@ def zscore_key(c, dims, nonzero, channel_wise):
 
 
 # ------------------------------------------------------------------------------------------------------ configurations
-GOLDEN = {   # tests/golden/recipe.py CASES: (n_outputs, input shape); every one trains on DiceLoss(sigmoid=True), uint8 one-hot
-    "c1_bw8_32": (3, (1, 4, 32, 32, 32)), "c1_bw8_64": (3, (1, 4, 64, 64, 64)), "bw16_n2_32": (3, (2, 4, 32, 32, 32)),
-    "bw8_convT_32": (3, (1, 4, 32, 32, 32)), "c5like_1ch_5lev_32": (1, (1, 1, 32, 32, 32)),
-    "bw8_nonpow2_24x32x40": (3, (1, 4, 24, 32, 40)),
-}
-
-
 def config_launches():
     """(config, kernel, args) of every criterion / pre- / post-processing launch of the configurations:
       - bench.py C2 (batch 2, 3 outputs, 128^3) and C3 (160 x 192 x 128), the BraTS config (3 sigmoid outputs, batch 2 of
         128^3 patches) and the BraTS SegResNet recipe (3 sigmoid outputs, 1 x 224 x 224 x 144): DiceLoss(sigmoid=True) on uint8
         one-hot targets;
-      - the golden recipes, and the many-class setups of tests/test_gpu_many_classes.py: the 24- and 104-output fixtures
-        (1 x 32^3), the 104-output machinery (2 x 32^3 and 2 x 16^3) and the 128-output head shape (2 x 5 x 7 x 3);
+      - the golden recipes (tests/plan_launches.py), and the many-class setups of tests/test_gpu_many_classes.py: the 24- and
+        104-output fixtures (1 x 32^3), the 104-output machinery (2 x 32^3 and 2 x 16^3) and the 128-output head shape
+        (2 x 5 x 7 x 3);
       - README's head table at the C2 size with 104 and 128 outputs: DiceLoss(sigmoid=True) on uint8 one-hot targets;
       - a DiceCELoss(softmax=True, to_onehot_y=True) step on a label map at 128^3, batch 2, 3 and 16 classes, uint8 and int64;
       - bench.py C5's tiled inference: one 256^3 volume, roi 128^3, overlap 0.25, sw_batch 3, one output channel;
@@ -214,8 +210,9 @@ def config_launches():
     for name, (n, c, dims) in [("C2", (2, 3, (128, 128, 128))), ("C3", (2, 3, (160, 192, 128))), ("brats", (2, 3, (128, 128, 128))),
                                ("brats-segresnet", (1, 3, (224, 224, 144)))]:
         out.append((name, "dice", (n, c, vol(dims), "u8")))
-    for name, (c, shape) in GOLDEN.items():
-        out.append(("golden-" + name, "dice", (shape[0], c, vol(shape[2:]), "u8")))
+    for c in PL.CONFIGS:
+        if c.name.startswith("golden-"):          # every one trains on DiceLoss(sigmoid=True), uint8 one-hot
+            out.append((c.name, "dice", (c.n, c.kw["n_outputs"], vol(c.dims), "u8")))
     for name, (n, c, dims) in [("mc24", (1, 24, (32, 32, 32))), ("mc104", (1, 104, (32, 32, 32))),
                                ("mc104-machinery", (2, 104, (32, 32, 32))), ("mc104-graph", (2, 104, (16, 16, 16))),
                                ("mc128-head", (2, 128, (5, 7, 3)))]:

@@ -138,24 +138,20 @@ def noise_floor(case: Case, eps: float, runs: int = 2, input_grad: bool = True) 
 
 
 # ------------------------------------------------------------------------------------------------ conv routes
-def conv_layers(n, in_channels, init_filters, dims, levels=4):
-    """(label, op, cin, cout, output extents, epilogue mode) of every convolution launch of a SegResNet training plan with
-    input_grad (plan.cu: build_segresnet): forward ops, and the data gradients (mode 1: the GroupNorm + act backward epilogue of
-    the ResBlock convolutions)"""
-    ext = [tuple(d >> k for d in dims) for k in range(levels)]
-    W = [init_filters << k for k in range(levels)]
-    cp = 8 if in_channels <= 8 else 16
-    out = [("convInit", "k3s1", cp, W[0], ext[0], 0), ("convInit.dgrad", "k3s1", W[0], cp, ext[0], 0)]
-    for i in range(levels):
-        out.append(("ResBlock L%d" % i, "k3s1", W[i], W[i], ext[i], 0))
-        out.append(("ResBlock L%d.dgrad" % i, "k3s1", W[i], W[i], ext[i], 1))
-        if i > 0:
-            out.append(("down_layers.%d.0" % i, "k3s2", W[i - 1], W[i], ext[i], 0))
-            out.append(("down_layers.%d.0.dgrad" % i, "class1", W[i], W[i - 1], ext[i - 1], 0))
-    for j in range(levels - 1):
-        i = levels - 2 - j
-        out.append(("up_samples.%d.0" % i, "k1", 2 * W[j], W[j], ext[j + 1], 0))
-        out.append(("up_samples.%d.0.dgrad" % i, "k1", W[j], 2 * W[j], ext[j + 1], 0))
+def _brats_table(kernels, route, fields):
+    """{label: fields of route(launch)} over the BraTS recipe's convolutions of the given kernels (tests/plan_launches.py:
+    brats-segresnet).  A label is the layer's state-dict name, with ".dgrad" for a data gradient; the ResBlock convolutions of a
+    level share one, "ResBlock L<level>", and must take the same route."""
+    import plan_launches as P
+    out = {}
+    for l in P.BY_NAME["brats-segresnet"].launches():
+        if l.kernel in kernels:
+            name = l.key[:-len(".conv.weight")]
+            if name.endswith((".conv1", ".conv2")):
+                name = "ResBlock L%d" % ((l.co // BRATS["init_filters"]).bit_length() - 1)
+            r = route(l)
+            label, r = name + (".dgrad" if l.kernel == "dgrad" else ""), None if r is None else tuple(r[f] for f in fields)
+            assert out.setdefault(label, r) == r, (label, out[label], r)
     return out
 
 
@@ -178,31 +174,10 @@ BRATS_ROUTES = {
 BRATS_ROUTES["split"] = {k: (("tap" if v[0] == "halo" else v[0]),) + v[1:] for k, v in BRATS_ROUTES["bf16"].items()}
 
 
-def route_table(L, split, n=1, in_channels=4, init_filters=16, dims=(224, 224, 144)):
+def route_table(L, split):
     """{label: (kind, BN, KC)} from the library's route query (include/b200unet_diag.h)"""
-    from conv_route_cases import conv_query
-    out = {}
-    for label, op, ci, co, ext, mode in conv_layers(n, in_channels, init_filters, dims):
-        r = conv_query(L, op, ci, co, ext, split, mode, n=n)
-        out[label] = None if r is None else (r["kind"], r["bn"], r["kc"])
-    return out
-
-
-def wgrad_layers(in_channels, init_filters, dims, blocks_down=(1, 2, 2, 4)):
-    """(label, op, ci, co, dy extents) of every weight gradient of a SegResNet training plan (plan.cu: build_segresnet; one
-    entry per distinct shape): convInit from the packed input, the two 3x3x3 convolutions of every ResBlock, the stride-2
-    convolution into each lower level and the 1x1x1 convolution of each decoder stage"""
-    L = len(blocks_down)
-    ext = [tuple(d >> k for d in dims) for k in range(L)]
-    W = [init_filters << k for k in range(L)]
-    out = [("convInit", "k3s1", 8 if in_channels <= 8 else 16, W[0], ext[0])]
-    for i in range(L):
-        out.append(("ResBlock L%d" % i, "k3s1", W[i], W[i], ext[i]))
-        if i > 0:
-            out.append(("down_layers.%d.0" % i, "k3s2", W[i - 1], W[i], ext[i]))
-    for j in range(L - 1):
-        out.append(("up_samples.%d.0" % (L - 2 - j), "k1", 2 * W[j], W[j], ext[j + 1]))
-    return out
+    from plan_launches import conv_route
+    return _brats_table(("fwd", "dgrad"), lambda l: conv_route(L, l, split), ("kind", "bn", "kc"))
 
 
 # the weight-gradient routes of the BraTS recipe (batch 1, 4 x 224 x 224 x 144, init_filters 16) on a 132-SM H100: (kind, K
@@ -223,25 +198,19 @@ BRATS_WGRAD_ROUTES = {
 }
 
 
-def wgrad_route_table(L, split, n=1, in_channels=4, init_filters=16, dims=(224, 224, 144), num_sms=132):
+def wgrad_route_table(L, split):
     """{label: (kind, K chunk, BN)} from the library's weight-gradient route query"""
-    from conv_route_cases import wgrad_query
-    out = {}
-    for label, op, ci, co, ext in wgrad_layers(in_channels, init_filters, dims):
-        r = wgrad_query(L, op, ci, co, ext, split, num_sms=num_sms, n=n)
-        out[label] = None if r is None else (r["kind"], r["cb"], r["bn"])
-    return out
+    from plan_launches import wgrad_route
+    return _brats_table(("wgrad",), lambda l: wgrad_route(L, l, split), ("kind", "cb", "bn"))
 
 
 # ------------------------------------------------------------------------------------------------ fused up-sampling kernel
 def upskip_geometries():
-    """(n, C, low-resolution extents) of every up-sample + skip launch of the plans the tests and tools/segresnet_bench.py run"""
-    plans = [(1, 16, (224, 224, 144)), (2, 16, (128, 128, 128))]
-    plans += [(c.shape[0], c.kw.get("init_filters", 8), c.shape[2:]) for c in RELU_CASES + [SMOOTH_CASE]]
+    """(n, C, low-resolution extents) of every up-sample + skip launch of the SegResNet configurations of tests/plan_launches.py"""
+    import plan_launches as P
     out = []
-    for (n, f, dims), case_levels in zip(plans, [4, 4] + [len(c.kw.get("blocks_down", (1, 2, 2, 4))) for c in RELU_CASES + [SMOOTH_CASE]]):
-        for j in range(case_levels - 1):
-            g = (n, f << j, tuple(d >> (j + 1) for d in dims))
-            if g not in out:
-                out.append(g)
+    for c in P.CONFIGS:
+        for l in c.launches():
+            if l.kernel == "up_add" and (l.n, l.c, l.dims) not in out:
+                out.append((l.n, l.c, l.dims))
     return out

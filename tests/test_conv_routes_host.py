@@ -10,6 +10,7 @@ import re
 import pytest
 
 import conv_route_cases as R
+import plan_launches as P
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "3dunetcnn_b200", "csrc")
@@ -91,100 +92,35 @@ def test_deep_k_case_takes_its_route(L, case):
     assert case.key in {c.key for c in R.CONV_CASES}, "a deep-K case of a route without a case in CONV_CASES"
 
 
-def _dynunet_conv_layers(in_channels, filters, dims):
-    """(label, op, cin, cout, output extents, mode, cin2) of every convolution launch of a DynUNet training plan (plan.cu:
-    build_dynunet): per level a block of a 3x3x3 convolution (stride 2 below level 0) and a 3x3x3 one; per decoder stage the
-    kernel-2 transposed convolution (parity class 2) into the low half of the concat buffer and a block reading all of it.
-    Backward (build_dyn_block_bwd): conv2's data gradient through the norm + act epilogue (mode 1), conv1's (parity class 1 for
-    stride 2; none for the first block), and the transposed convolution's as a kernel-2 stride-2 convolution."""
-    L = len(filters)
-    ext = [tuple(d >> k for d in dims) for k in range(L)]
-    out = []
-    for i in range(L):
-        xc = (in_channels + 7) // 8 * 8 if i == 0 else filters[i - 1]
-        out += [("enc%d.conv1" % i, "k3s1" if i == 0 else "k3s2", xc, filters[i], ext[i], 0, 0),
-                ("enc%d.conv2" % i, "k3s1", filters[i], filters[i], ext[i], 0, 0),
-                ("enc%d.conv2.dgrad" % i, "k3s1", filters[i], filters[i], ext[i], 1, 0)]
-        if i > 0:
-            out.append(("enc%d.conv1.dgrad" % i, "class1", filters[i], filters[i - 1], ext[i - 1], 0, 0))
-    for hi in range(L - 1):
-        f = filters[hi]
-        out += [("up%d" % hi, "class2", filters[hi + 1], f, ext[hi], 0, 0),
-                ("up%d.dgrad" % hi, "k2s2", f, filters[hi + 1], ext[hi + 1], 0, 0),
-                ("dec%d.conv1" % hi, "k3s1", 2 * f, f, ext[hi], 0, 0), ("dec%d.conv2" % hi, "k3s1", f, f, ext[hi], 0, 0),
-                ("dec%d.conv2.dgrad" % hi, "k3s1", f, f, ext[hi], 1, 0), ("dec%d.conv1.dgrad" % hi, "k3s1", f, 2 * f, ext[hi], 0, 0)]
-    return out
-
-
-def _restated_conv_layers():
-    """(config, n, precisions, layers) of the configurations the tests restate: the benchmark's C2 and C3 training steps (batch 2)
-    and C5 forward, the BraTS DynUNet (examples/brats2020/brats2020_config.json) and the SegResNet recipes"""
-    import c5_cases
-    import segresnet_cases as S
-    both = (False, True)
-    out = [("C2", 2, both, c5_cases.unet3d_conv_layers(4, 32, (128, 128, 128), train=True)),
-           ("C3", 2, both, c5_cases.unet3d_conv_layers(4, 32, (160, 192, 128), train=True)),
-           ("C5", c5_cases.C5_BATCH, both, c5_cases.conv_layers()),
-           ("brats-dynunet", 2, both, _dynunet_conv_layers(4, [64, 96, 128, 192, 256, 384], (128, 128, 128))),
-           ("brats-segresnet", 1, both, [l + (0,) for l in S.conv_layers(1, 4, 16, (224, 224, 144))])]
-    for c in S.RELU_CASES + [S.SMOOTH_CASE]:
-        layers = S.conv_layers(c.shape[0], c.kw.get("in_channels", 1), c.kw.get("init_filters", 8), c.shape[2:], len(c.blocks[0]))
-        out.append(("segresnet-" + c.id, c.shape[0], both, [l + (0,) for l in layers]))
-    return out
+# the configurations of tests/plan_launches.py whose K loops need fp64 cases: the benchmark's C2 and C3 training steps and C5
+# forward, the BraTS DynUNet and the SegResNet recipes
+DEEP_K_CONFIGS = ["C2", "C3", "C5", "brats-dynunet", "brats-segresnet"] + [c.name for c in P.CONFIGS
+                                                                          if c.name.startswith("segresnet-")]
 
 
 def test_deep_k_loops_of_the_restated_configurations_have_fp64_cases(L):
-    """for each (kind, KC, precision, mode) the largest K-chunk count, per source, that a layer of C2, C3, C5, the BraTS DynUNet or
-    the SegResNet recipes walks must be walked by a case the GPU tests run against fp64 (CONV_CASES + DEEP_K_CASES)"""
+    """for each (kind, KC, precision, mode) the largest K-chunk count, per source, that a layer of the DEEP_K_CONFIGS walks in
+    either precision must be walked by a case the GPU tests run against fp64 (CONV_CASES + DEEP_K_CASES)"""
     have = {}
     for c in R.CONV_CASES + R.DEEP_K_CASES:
         k = (c.kind, c.kc, "split" if c.split else "bf16", c.mode)
         have[k] = tuple(max(a, b) for a, b in zip(have.get(k, (0, 0)), c.kchunks))
     need = {}
-    for config, n, precisions, layers in _restated_conv_layers():
-        for label, op, ci, co, ext, mode, ci2 in layers:
-            for split in precisions:
-                r = R.conv_query(L, op, ci, co, ext, split, mode, ci2, n=n)
-                assert r is not None, (config, label, split)
-                k = (r["kind"], r["kc"], "split" if split else "bf16", mode)
+    for config in DEEP_K_CONFIGS:
+        for l in P.BY_NAME[config].launches():
+            if l.kernel not in ("fwd", "dgrad"):
+                continue
+            for split in (False, True):
+                r = P.conv_route(L, l, split)
+                assert r is not None, (config, l, split)
+                k = (r["kind"], r["kc"], "split" if split else "bf16", l.mode)
                 for s in (0, 1):
                     if r["kchunks"][s] > need.get((k, s), (1, None))[0]:
-                        need[(k, s)] = (r["kchunks"][s], "%s %s" % (config, label))
+                        need[(k, s)] = (r["kchunks"][s], "%s %s %s" % (config, l.kernel, l.key))
     assert max(v[0] for v in need.values()) == 12          # the C5 network's 768-channel layers
     short = ["%s source %d: %d K chunks (%s), the cases walk %d" % (k, s, m, where, have.get(k, (0, 0))[s])
              for (k, s), (m, where) in sorted(need.items()) if have.get(k, (0, 0))[s] < m]
     assert not short, "K loops deeper than any fp64 case walks:\n  " + "\n  ".join(short)
-
-
-@pytest.mark.parametrize("n,n_features,dims,blocks,train", [(2, 4, (128, 128, 128), (1, 2, 2, 4), True),
-                                                             (2, 4, (160, 192, 128), (1, 2, 2, 4), True),
-                                                             (3, 1, (128, 128, 128), (1, 2, 2, 4, 4), False)],
-                         ids=["C2", "C3", "C5"])
-def test_unet3d_conv_layers_are_the_plans(pkg, n, n_features, dims, blocks, train):
-    """the restated launches of c5_cases.unet3d_conv_layers carry exactly the convolution MACs the plan itself counts, forward and
-    data gradient (plan.cu: conv_macs; a data-gradient MAC is its layer's forward MAC, and the first block's conv1 data gradient,
-    which feeds only its norm's dgamma / dbeta, is not counted)"""
-    import c5_cases
-    import torch
-    width = 48 if n_features == 1 else 32
-    m = pkg.UNet3D(n_features=n_features, n_outputs=1, base_width=width, encoder_blocks=list(blocks))
-    desc = m._net_desc(n, *dims)
-    desc.inference_only = int(not train)
-    macs = pkg.models._Plan(desc, torch.device("cpu")).algorithmic_macs()
-    fwd = dgrad = 0.0
-    for label, op, ci, co, ext, mode, ci2 in c5_cases.unet3d_conv_layers(n_features, width, dims, blocks, train=train):
-        first = label.startswith("encoder.layers.0.blocks.0.")
-        vox = n * ext[0] * ext[1] * ext[2]
-        if label.endswith(".dgrad"):
-            if label == "encoder.layers.0.blocks.0.conv1.dgrad":
-                continue
-            co = n_features if first and co == 8 else co
-            dgrad += (vox // 8 if op == "class1" else vox) * ci * co * (1 if op == "k1" else 27)
-        else:
-            if first:      # the packed input's padding channels carry no MACs
-                ci, ci2 = (n_features, 0) if label.endswith("conv1") else (ci, n_features)
-            fwd +=vox * co * (ci * (1 if op == "k1" else 27) + ci2)
-    assert (macs["conv_fwd"], macs["conv_dgrad"]) == (fwd, dgrad)
 
 
 def test_c5_routes(L):

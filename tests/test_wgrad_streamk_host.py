@@ -1,14 +1,16 @@
 """The stream-K partition of the per-tap weight gradient (wgrad.cu: wgrad_tiling, k_wgrad), restated in Python and held to the
-library's route query over the weight-gradient launch shapes of the C2 and C3 UNet3D plans, the BraTS DynUNet plan and the BraTS
-SegResNet recipe (batch 1 at 224 x 224 x 144, batch 2 at 128^3), on 114 and 132 SMs.  A work item is (M-tile group, N tile); an iteration is (work item, voxel tile), items outer.  CTA c of P runs
-iterations [c * T / P, (c + 1) * T / P): every iteration once, per-CTA work within one voxel tile, and in deterministic mode
-each CTA stores into the slot of its rank among the CTAs of its item, below the route's split count."""
+library's route query over the weight-gradient launch shapes (tests/plan_launches.py) of the C2 and C3 UNet3D plans, the BraTS
+DynUNet plan and the BraTS SegResNet recipe (batch 1 at 224 x 224 x 144, batch 2 at 128^3), on 114 and 132 SMs.  A work item
+is (M-tile group, N tile); an iteration is (work item, voxel tile), items outer.  CTA c of P runs iterations
+[c * T / P, (c + 1) * T / P): every iteration once, per-CTA work within one voxel tile, and in deterministic mode each CTA stores
+into the slot of its rank among the CTAs of its item, below the route's split count."""
 import math
 
 import numpy as np
 import pytest
 
 import conv_route_cases as R
+import plan_launches as P
 import segresnet_cases as S
 
 
@@ -29,52 +31,9 @@ def bn_bucket(c):
     return 128 if c > 64 else kc_bucket(c)
 
 
-def unet3d_wgrads(dims, widths=(32, 64, 128, 256), encoder_blocks=(1, 2, 2, 4)):
-    """(op, ci, co, dy extents) of the weight gradients of a UNet3D plan: residual blocks of two 3x3x3 convolutions with a 1x1x1
-    sample convolution where the width changes, a 3x3x3 stride-2 convolution between encoder levels, and per decoder level
-    its blocks, a 1x1x1 convolution to the next width and the concat with the skip"""
-    ext = [tuple(d >> k for d in dims) for k in range(len(widths))]
-    out, cin = [], 8
-    for k, c in enumerate(widths):
-        if k:
-            out.append(("k3s2", widths[k - 1], widths[k - 1], ext[k]))
-        for _ in range(encoder_blocks[k]):
-            out += [("k3s1", cin, c, ext[k]), ("k3s1", c, c, ext[k])]
-            if cin != c:
-                out.append(("k1", cin, c, ext[k]))
-            cin = c
-    for depth in range(len(widths) - 1, 0, -1):
-        out += [("k3s1", cin, cin, ext[depth]), ("k3s1", cin, cin, ext[depth])]
-        out.append(("k1", cin, widths[depth - 1], ext[depth]))
-        cin = 2 * widths[depth - 1]
-    out += [("k3s1", cin, widths[0], ext[0]), ("k3s1", widths[0], widths[0], ext[0]), ("k1", cin, widths[0], ext[0])]
-    return out
-
-
-def dynunet_wgrads(dims, filters=(64, 96, 128, 192, 256, 384)):
-    """the BraTS DynUNet (filters 64 .. 384, strides 1, 2, 2, ...): two 3x3x3 convolutions per block, the first of a level at
-    stride 2, and per decoder level a kernel-2 stride-2 transposed convolution and a block on the concat"""
-    out, cin = [], 8
-    for k, f in enumerate(filters):
-        e = tuple(d >> k for d in dims)
-        out += [("k3s2" if k else "k3s1", cin, f, e), ("k3s1", f, f, e)]
-        cin = f
-    for k in range(len(filters) - 2, -1, -1):
-        e = tuple(d >> k for d in dims)
-        out += [("k2s2", filters[k], filters[k + 1], tuple(x >> 1 for x in e)), ("k3s1", 2 * filters[k], filters[k], e),
-                ("k3s1", filters[k], filters[k], e)]
-    return out
-
-
-def segresnet_wgrads(dims, in_channels=4, init_filters=16):
-    """the BraTS SegResNet recipe (segresnet_cases.wgrad_layers)"""
-    return [(op, ci, co, ext) for _, op, ci, co, ext in S.wgrad_layers(in_channels, init_filters, dims)]
-
-
-PLANS = {"C2": unet3d_wgrads((128, 128, 128)), "C3": unet3d_wgrads((160, 192, 128)), "brats-dynunet": dynunet_wgrads((128, 128, 128)),
-         "brats-segresnet": segresnet_wgrads((224, 224, 144)), "brats-segresnet-128": segresnet_wgrads((128, 128, 128))}
-BATCH = {"brats-segresnet": 1}          # every other plan trains at batch 2
-CASES = sorted({(plan, *shape) for plan, shapes in PLANS.items() for shape in shapes})
+CONFIGS = ("C2", "C3", "brats-dynunet", "brats-segresnet", "brats-segresnet-128")
+CASES = sorted({(c, l.op, P.pad8(l.c), P.pad8(l.co), l.dims) for c in CONFIGS for l in P.BY_NAME[c].launches()
+                if l.kernel == "wgrad"})
 
 
 @pytest.fixture(scope="module")
@@ -116,7 +75,7 @@ def restate(op, ci, co, dims, num_sms, n=2):
 @pytest.mark.parametrize("num_sms", [114, 132])
 @pytest.mark.parametrize("plan,op,ci,co,dims", CASES, ids=lambda v: str(v))
 def test_streamk_partition(L, plan, op, ci, co, dims, num_sms):
-    n = BATCH.get(plan, 2)
+    n = P.BY_NAME[plan].n
     for split in (False, True):
         r = R.wgrad_query(L, op, ci, co, dims, split, num_sms=num_sms, n=n)
         assert r is not None, (op, ci, co, dims)
@@ -146,7 +105,7 @@ def test_streamk_partition(L, plan, op, ci, co, dims, num_sms):
 
 def test_wide_c2_launches_fill_every_sm(L):
     """the 3x3x3 launches of more than 64 input channels ran on 108 of 132 SMs before stream-K"""
-    wide = [s for s in PLANS["C2"] if s[0] in ("k3s1", "k3s2") and s[1] > 64]
+    wide = [s[1:] for s in CASES if s[0] == "C2" and s[1] in ("k3s1", "k3s2") and s[2] > 64]
     assert len({s for s in wide}) >= 5
     for op, ci, co, dims in wide:
         r = R.wgrad_query(L, op, ci, co, dims)
@@ -158,6 +117,7 @@ def test_segresnet_brats_wgrad_routes(L, precision):
     """the weight-gradient route of every SegResNet layer of the BraTS recipe on a 132-SM H100 (the table the at-size GPU test
     asserts), and the per-tap ones split over every SM"""
     assert S.wgrad_route_table(L, precision == "split") == S.BRATS_WGRAD_ROUTES[precision]
-    for _, op, ci, co, ext in S.wgrad_layers(4, 16, (224, 224, 144)):
-        r = R.wgrad_query(L, op, ci, co, ext, precision == "split", n=1)
-        assert r["ctas"] == 132, (op, ci, co, ext, r)
+    for l in P.BY_NAME["brats-segresnet"].launches():
+        if l.kernel == "wgrad":
+            r = P.wgrad_route(L, l, precision == "split")
+            assert r["ctas"] == 132, (l, r)
