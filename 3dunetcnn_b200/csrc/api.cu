@@ -196,6 +196,9 @@ static DiceCEDesc to_dice_ce(const b200unet_dice_ce_desc* d) {
   r.act = d->act; r.target_kind = d->target_kind; r.include_background = d->include_background; r.squared_pred = d->squared_pred;
   r.jaccard = d->jaccard; r.batch = d->batch; r.reduction = d->reduction;
   r.smooth_nr = d->smooth_nr; r.smooth_dr = d->smooth_dr; r.lambda_dice = d->lambda_dice; r.lambda_ce = d->lambda_ce;
+  r.overlap = d->overlap; r.tversky_alpha = d->tversky_alpha; r.tversky_beta = d->tversky_beta; r.w_type = d->w_type;
+  r.voxel_term = d->voxel_term; r.focal_softmax = d->focal_softmax; r.focal_gamma = d->focal_gamma; r.focal_alpha = d->focal_alpha;
+  r.focal_use_alpha = d->focal_use_alpha; r.class_weight = d->class_weight;
   return r;
 }
 int b200unet_dice_fwd(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c, int64_t spatial,

@@ -82,43 +82,118 @@ __device__ __forceinline__ void pooled(const double* sums, int N, int C, int n, 
   }
 }
 
-// coef [N][C][2] = lambda_dice * w * (dF/dI, dF/dP), zero on a dropped background channel; the scalar loss.
+// f of one (n, c) pair (Dice, Jaccard or Tversky) and its (dF/dI, dF/dP):
 //   F = 1 - (2I+nr)/(Den+dr);  plain: Den = P+T  ->  dF/dI = -2/D', dF/dP = (2I+nr)/D'^2
 //   jaccard: Den = 2(P+T-I)    ->  dF/dI = -2/D' - 2(2I+nr)/D'^2 , dF/dP = 2(2I+nr)/D'^2          (D' = Den + dr)
-// The backward kernels form dL/dx = g * [ coef_I * t + coef_P * dP/dp ] * dp/dx.  ce [N] is read only when lambda_ce != 0.
+//   Tversky: F = 1 - (I+nr)/D', D' = I + a(P-I) + b(T-I) + dr  ->  dF/dI = -1/D' + (I+nr)(1-a-b)/D'^2, dF/dP = a(I+nr)/D'^2
+__device__ __forceinline__ double overlap_f(const DiceCEDesc& d, double I, double P, double T, double& dFdI, double& dFdP) {
+  if (d.overlap == O_TVERSKY) {
+    const double a = d.tversky_alpha, b = d.tversky_beta;
+    const double D = I + a * (P - I) + b * (T - I) + d.smooth_dr, num = I + d.smooth_nr;
+    dFdI = -1.0 / D + num * (1.0 - a - b) / (D * D);
+    dFdP = a * num / (D * D);
+    return 1.0 - num / D;
+  }
+  double den = P + T;
+  if (d.jaccard) den = 2.0 * (den - I);
+  const double D = den + d.smooth_dr, num = 2.0 * I + d.smooth_nr;
+  dFdI = -2.0 / D; dFdP = num / (D * D);
+  if (d.jaccard) { dFdI = -2.0 / D - 2.0 * num / (D * D); dFdP = 2.0 * num / (D * D); }
+  return 1.0 - (2.0 * I + d.smooth_nr) / (den + d.smooth_dr);
+}
+
+// generalized Dice weight of a class with target sum T (inf when T == 0 and the weight is not uniform)
+__device__ __forceinline__ double gdice_weight(double T, int w_type) {
+  return w_type == W_SQUARE ? 1.0 / (T * T) : w_type == W_SIMPLE ? 1.0 / T : 1.0;
+}
+
+// Generalized Dice of group g (sample g, or every sample with batch): the largest finite weight, which replaces the infinite
+// ones, and A = 2 sum_c w_c I_c + nr, B = sum_c w_c (P_c + T_c) + dr over the kept channels
+__device__ void gdice_group(const double* sums, int N, int C, int g, int c_lo, const DiceCEDesc& d, double* out) {
+  double wmax = 0;
+  for (int c = c_lo; c < C; ++c) {
+    double I, P, T;
+    pooled(sums, N, C, g, c, d.batch, I, P, T);
+    const double w = gdice_weight(T, d.w_type);
+    if (!isinf(w)) wmax = fmax(wmax, w);
+  }
+  double A = 0, B = 0;
+  for (int c = c_lo; c < C; ++c) {
+    double I, P, T;
+    pooled(sums, N, C, g, c, d.batch, I, P, T);
+    double w = gdice_weight(T, d.w_type);
+    if (isinf(w)) w = wmax;
+    A += w * I;
+    B += w * (P + T);
+  }
+  out[0] = 2.0 * A + d.smooth_nr;
+  out[1] = B + d.smooth_dr;
+  out[2] = wmax;
+}
+
+// coef [N][C][2] = lambda_dice * w * (dF/dI, dF/dP), zero on a dropped background channel and everywhere when lambda_dice = 0;
+// the scalar loss.  The backward kernels form dL/dx = g * [ coef_I * t + coef_P * dP/dp ] * dp/dx.  ce [N] is read only when
+// lambda_ce != 0.  Generalized Dice couples a group's classes through A and B: f = 1 - A/B, dF/dI_c = -2 w_c / B,
+// dF/dP_c = A w_c / B^2; the groups are formed 128 at a time, then their pairs' coefficients.
 __global__ void k_dice_finalize(const double* __restrict__ sums, const double* __restrict__ ce, int N, int C, long long S, DiceCEDesc d,
                                 double* __restrict__ coef, float* __restrict__ loss) {
   const int c_lo = (!d.include_background && C > 1) ? 1 : 0;
-  const int terms = (d.batch ? 1 : N) * (C - c_lo);
-  const double w = d.lambda_dice * (d.reduction == 0 ? 1.0 / terms : 1.0);
-  for (int i = threadIdx.x; i < N * C; i += blockDim.x) {
-    const int n = i / C, c = i % C;
-    double I, P, T;
-    pooled(sums, N, C, n, c, d.batch, I, P, T);
-    double den = P + T;
-    if (d.jaccard) den = 2.0 * (den - I);
-    const double D = den + d.smooth_dr, num = 2.0 * I + d.smooth_nr;
-    double dFdI = -2.0 / D, dFdP = num / (D * D);
-    if (d.jaccard) { dFdI = -2.0 / D - 2.0 * num / (D * D); dFdP = 2.0 * num / (D * D); }
-    const double wc = c < c_lo ? 0.0 : w;
-    coef[i * 2] = wc * dFdI;
-    coef[i * 2 + 1] = wc * dFdP;
+  double acc = 0;
+  if (d.lambda_dice == 0.f) {
+    for (int i = threadIdx.x; i < N * C; i += blockDim.x) coef[i * 2] = coef[i * 2 + 1] = 0.0;
+  } else if (d.overlap == O_GDICE) {
+    __shared__ double grp[128][3];
+    const int G = d.batch ? 1 : N;
+    const double w = d.lambda_dice * (d.reduction == 0 ? 1.0 / G : 1.0);
+    for (int g0 = 0; g0 < G; g0 += 128) {
+      const int ng = min(128, G - g0);
+      if ((int)threadIdx.x < ng) gdice_group(sums, N, C, g0 + threadIdx.x, c_lo, d, grp[threadIdx.x]);
+      __syncthreads();
+      const int n0 = d.batch ? 0 : g0, rows = d.batch ? N : ng;
+      for (int i = threadIdx.x; i < rows * C; i += blockDim.x) {
+        const int n = n0 + i / C, c = i % C;
+        const double* q = grp[d.batch ? 0 : n - g0];
+        double I, P, T;
+        pooled(sums, N, C, n, c, d.batch, I, P, T);
+        double wc = gdice_weight(T, d.w_type);
+        if (isinf(wc)) wc = q[2];
+        if (c < c_lo) wc = 0.0;
+        coef[((long long)n * C + c) * 2] = w * (-2.0 * wc / q[1]);
+        coef[((long long)n * C + c) * 2 + 1] = w * (q[0] * wc / (q[1] * q[1]));
+      }
+      if (threadIdx.x == 0)
+        for (int g = 0; g < ng; ++g) acc += 1.0 - grp[g][0] / grp[g][1];
+      __syncthreads();
+    }
+    if (threadIdx.x != 0) return;
+    acc = d.lambda_dice * (d.reduction == 0 ? acc / G : acc);
+  } else {
+    const int terms = (d.batch ? 1 : N) * (C - c_lo);
+    const double w = d.lambda_dice * (d.reduction == 0 ? 1.0 / terms : 1.0);
+    for (int i = threadIdx.x; i < N * C; i += blockDim.x) {
+      const int n = i / C, c = i % C;
+      double I, P, T, dFdI, dFdP;
+      pooled(sums, N, C, n, c, d.batch, I, P, T);
+      overlap_f(d, I, P, T, dFdI, dFdP);
+      const double wc = c < c_lo ? 0.0 : w;
+      coef[i * 2] = wc * dFdI;
+      coef[i * 2 + 1] = wc * dFdP;
+    }
+    if (threadIdx.x != 0) return;
+    for (int n = 0; n < (d.batch ? 1 : N); ++n)
+      for (int c = c_lo; c < C; ++c) {
+        double I, P, T, dFdI, dFdP;
+        pooled(sums, N, C, n, c, d.batch, I, P, T);
+        acc += overlap_f(d, I, P, T, dFdI, dFdP);
+      }
+    acc = d.lambda_dice * (d.reduction == 0 ? acc / terms : acc);
   }
   if (threadIdx.x != 0) return;
-  double acc = 0;
-  for (int n = 0; n < (d.batch ? 1 : N); ++n)
-    for (int c = c_lo; c < C; ++c) {
-      double I, P, T;
-      pooled(sums, N, C, n, c, d.batch, I, P, T);
-      double den = P + T;
-      if (d.jaccard) den = 2.0 * (den - I);
-      acc += 1.0 - (2.0 * I + d.smooth_nr) / (den + d.smooth_dr);
-    }
-  double l = d.lambda_dice * (d.reduction == 0 ? acc / terms : acc);
+  double l = acc;
   if (d.lambda_ce != 0.f) {
     double cet = 0;
     for (int n = 0; n < N; ++n) cet += ce[n];
-    l += d.lambda_ce * (d.reduction == 0 ? cet / ((double)N * S) : cet);
+    l += d.lambda_ce * (cet / voxel_divisor(d, N, C, S));
   }
   *loss = (float)l;
 }
@@ -148,6 +223,12 @@ int check_dice_desc(const DiceCEDesc& d, int N, int C, long long S, const char* 
   B200_REQUIRE(d.target_kind >= 0 && d.target_kind <= 3, E_INVALID, "%s: target_kind=%d", who, d.target_kind);
   B200_REQUIRE(d.reduction == 0 || d.reduction == 1, E_INVALID, "%s: reduction=%d (0 mean, 1 sum)", who, d.reduction);
   B200_REQUIRE(d.lambda_dice >= 0.f && d.lambda_ce >= 0.f, E_INVALID, "%s: negative lambda", who);
+  B200_REQUIRE(d.overlap >= 0 && d.overlap <= 2, E_INVALID, "%s: overlap=%d (0 Dice, 1 Tversky, 2 generalized Dice)", who, d.overlap);
+  B200_REQUIRE(d.overlap == O_DICE || (!d.squared_pred && !d.jaccard), E_INVALID,
+               "%s: squared_pred / jaccard apply to the Dice overlap only (overlap=%d)", who, d.overlap);
+  B200_REQUIRE(d.w_type >= 0 && d.w_type <= 2, E_INVALID, "%s: w_type=%d (0 square, 1 simple, 2 uniform)", who, d.w_type);
+  B200_REQUIRE(d.voxel_term == V_CE || d.voxel_term == V_FOCAL, E_INVALID, "%s: voxel_term=%d (0 CE, 1 focal)", who, d.voxel_term);
+  B200_REQUIRE(d.focal_gamma >= 0.f, E_INVALID, "%s: focal_gamma=%g (>= 0)", who, d.focal_gamma);
   return OK;
 }
 
@@ -164,6 +245,9 @@ static int check_dice(const DiceCEDesc& d, int N, int C, long long S) {
   B200_REQUIRE(d.target_kind == T_ONEHOT_U8 || d.target_kind == T_SOFT_F32, E_UNSUPPORTED,
                "dice: target_kind=%d (a label map goes to b200unet_dice_ce_*; here 2 uint8 or 3 fp32 [n][c][spatial])", d.target_kind);
   B200_REQUIRE(d.lambda_ce == 0.f, E_INVALID, "dice: lambda_ce=%g (the CE term is computed by b200unet_dice_ce_*)", d.lambda_ce);
+  B200_REQUIRE(d.overlap == O_DICE && d.voxel_term == V_CE && !d.focal_softmax && !d.focal_use_alpha && !d.class_weight,
+               E_UNSUPPORTED, "dice: overlap=%d voxel_term=%d (Tversky, generalized Dice and the focal term run on b200unet_dice_ce_*)",
+               d.overlap, d.voxel_term);
   return OK;
 }
 

@@ -8,6 +8,11 @@
 //   CE:   on the raw logits.  C > 1: -sum_c t_c log_softmax(x)_c (a label map is its one-hot row); C == 1: BCEWithLogits(x, t).
 //         mean divides by N*S, sum sums.  lambda_ce = 0: no CE work at all, so logits of +-inf leave a sigmoid Dice finite
 //         (0 * the NaN of inf - inf would not be).
+//   The same kernels run monai.losses.TverskyLoss and GeneralizedDiceLoss (another overlap f of the same sums, formed by the
+//   finalize) and FocalLoss / DiceFocalLoss: the focal term takes CE's place, scaled by lambda_ce, on the channels
+//   include_background keeps.  Sigmoid form per element, softmax form over the kept channels -- under include_background = 0
+//   a softmax Dice takes its softmax over all C channels and the focal term over 1..C-1, so a voxel then needs both sums of
+//   exponentials.  The focal term leaves the raw logits in the staged tile (a softmax Dice recomputes exp(x - max)).
 // A label outside [0, C) is an all-zero target row: it adds nothing to I, T or CE and is never used as an index.
 //
 // Logits are NCDHW fp32, so every channel of a sample is a contiguous run of S floats.  Both passes stage a tile of kV voxels x
@@ -21,6 +26,8 @@
 //             (softmax: p_c (g_c - sum_k p_k g_k)) and the CE gradient cg (q_c sum_k t_k - t_c); dlogits written coalesced.
 // HBM bytes: forward N*S*(4C + b_t), backward N*S*(8C + b_t), b_t = target bytes per voxel (1 / 8 for uint8 / int64 label maps,
 // C / 4C for uint8 / fp32 C-channel targets).
+#include <type_traits>
+
 #include "kernels.h"
 
 namespace b200 {
@@ -41,6 +48,70 @@ __device__ __forceinline__ void cp_async4(float* dst, const float* src, bool val
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 __device__ __forceinline__ float sigm(float x) { return 1.f / (1.f + __expf(-x)); }
+
+// The per-voxel term of a launch (uniform): none (lambda_ce = 0), CE, or focal in either form
+enum VoxKind { VX_NONE = 0, VX_CE = 1, VX_FOCAL_SIG = 2, VX_FOCAL_SMX = 3 };
+struct Vox {
+  int kind;          // VoxKind
+  int lo;            // focal: first kept channel (1 when include_background = 0 drops channel 0 of a C > 1 input)
+  float gamma, alpha;
+  int use_alpha;
+  const float* w;    // focal: [C - lo] class factors or nullptr
+};
+
+// focal class factor of channel c (the softmax form's alpha folded in); 0 on a dropped channel
+__device__ __forceinline__ float focal_class_factor(const Vox& vx, int c) {
+  if (c < vx.lo) return 0.f;
+  float w = vx.w ? __ldg(vx.w + c - vx.lo) : 1.f;
+  if (vx.kind == VX_FOCAL_SMX && vx.use_alpha) w *= c == vx.lo ? 1.f - vx.alpha : vx.alpha;
+  return w;
+}
+
+// (1 - p)^gamma with 0^0 = 1
+__device__ __forceinline__ float pow_gamma(float omp, float gamma) {
+  return gamma == 0.f ? 1.f : (omp > 0.f ? __expf(gamma * __logf(omp)) : 0.f);
+}
+
+// focal, sigmoid form, of one element: a (x - x t - logsigmoid(x)) exp(gamma logsigmoid(-x (2t - 1))), a = w times the alpha
+// factor; *dfdx (when asked) = a E [(sigmoid(x) - t) - gamma s l0 sigmoid(x s)], s = 2t - 1.  BIN: t is 0 or 1 (uint8 targets), so both
+// softplus terms share log1p(exp(-|x|)).
+template <bool BIN>
+__device__ __forceinline__ float focal_sig(float x, float t, float w, const Vox& vx, float* dfdx) {
+  const float e = __expf(-fabsf(x));
+  const float L = log1pf(e);
+  const float l0 = x * (1.f - t) + fmaxf(-x, 0.f) + L;          // x - x t + softplus(-x)
+  const float s = 2.f * t - 1.f, z = x * s;                      // logsigmoid(-z) = -softplus(z)
+  const float spz = fmaxf(z, 0.f) + (BIN ? L : log1pf(__expf(-fabsf(z))));
+  const float E = vx.gamma == 0.f ? 1.f : __expf(-vx.gamma * spz);
+  const float a = vx.use_alpha ? w * (t * vx.alpha + (1.f - t) * (1.f - vx.alpha)) : w;
+  if (dfdx) {
+    const float r = 1.f / (1.f + e);
+    const float sx = x >= 0.f ? r : e * r, sxn = x >= 0.f ? e * r : r;   // sigmoid(x), sigmoid(-x)
+    const float sz = BIN ? (t > 0.5f ? sx : sxn) : sigm(z);
+    *dfdx = a * E * ((sx - t) - vx.gamma * s * l0 * sz);
+  }
+  return a * l0 * E;
+}
+
+// focal, softmax form, of one kept channel with log-probability ls: -a t (1 - p)^gamma ls, and *u = d/d ls =
+// -a t [(1 - p)^gamma - gamma (1 - p)^(gamma - 1) p ls]
+__device__ __forceinline__ float focal_smx(float ls, float t, float a, float gamma, float* u) {
+  const float omp = -expm1f(ls);
+  const float pw = pow_gamma(omp, gamma);
+  if (u) {
+    const float d = (gamma == 0.f || omp <= 0.f) ? 0.f : gamma * pw / omp * __expf(ls) * ls;
+    *u = -a * t * (pw - d);
+  }
+  return -a * t * pw * ls;
+}
+
+// log of the sum of exponentials over channels 1..C-1 of voxel v (the focal softmax when channel 0 is dropped)
+__device__ __forceinline__ float lse_from1(const float* xs, int C, int v) {
+  float m = -INFINITY, sum = 0.f;
+  for (int k = 1; k < C; ++k) m = fmaxf(m, xs[k * kP + v]);
+  for (int k = 1; k < C; ++k) sum += __expf(xs[k * kP + v] - m);
+  return m + logf(sum);
+}
 
 __device__ __forceinline__ double warp_sum(double v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -115,10 +186,11 @@ __device__ __forceinline__ Smem carve(unsigned char* base, int C, int kind) {
   return s;
 }
 
-// grid (grid_x, N).  part [N][C][slots][3] (I, P, T), ce_part [N][slots] (zero without with_ce)
+// grid (grid_x, N).  part [N][C][slots][3] (I, P, T; zero without with_dice), ce_part [N][slots] (the per-voxel term; zero
+// without one)
 template <int TK, int ACT>
 __global__ void __launch_bounds__(kThreads) k_dice_ce_fwd(const float* __restrict__ x, const void* __restrict__ tgt, int C, long long S,
-                                                          int squared, int with_ce, double* __restrict__ part,
+                                                          int squared, int with_dice, Vox vx, double* __restrict__ part,
                                                           double* __restrict__ ce_part) {
   extern __shared__ __align__(16) unsigned char smem[];
   const Smem sm = carve(smem, C, TK);
@@ -126,48 +198,81 @@ __global__ void __launch_bounds__(kThreads) k_dice_ce_fwd(const float* __restric
   const float* xn = x + (long long)n * C * S;
   const long long tiles = (S + kV - 1) / kV;
   const int K = kThreads / C, c = tid % C, slice = tid / C;   // phase B: thread (c, slice) walks voxels slice, slice + K, ...
+  // the reduction buffer is free until the end: the focal class factors, and each voxel's maximum when a focal term keeps the
+  // raw logits in the tile under a softmax Dice
+  const bool keep = vx.kind >= VX_FOCAL_SIG;
+  float* mrow = reinterpret_cast<float*>(sm.red);
+  float* fw = mrow + kV;
+  if (keep)
+    for (int k = tid; k < C; k += kThreads) fw[k] = focal_class_factor(vx, k);
   double aI = 0, aP = 0, aT = 0, ace = 0;
   for (long long tile = blockIdx.x; tile < tiles; tile += slots) {
     const long long s0 = tile * kV;
     const int nv = (int)(S - s0 < kV ? S - s0 : kV);
     stage_tile<TK>(xn, tgt, n, C, S, s0, nv, sm.xs, sm.ts, sm.lab);
-    // phase A: one voxel per thread -- softmax statistics and the CE term
-    if ((with_ce || ACT == A_SOFTMAX) && tid < nv) {
+    // phase A: one voxel per thread -- softmax statistics and the CE or focal term
+    if ((vx.kind != VX_NONE || ACT == A_SOFTMAX) && tid < nv) {
       const int v = tid;
-      float ce;
+      float ce = 0.f;
       if (C == 1) {
         const float xv = sm.xs[v], t = sm.ts[v];
-        ce = fmaxf(xv, 0.f) - xv * t + log1pf(__expf(-fabsf(xv)));
+        if (vx.kind <= VX_CE) ce = fmaxf(xv, 0.f) - xv * t + log1pf(__expf(-fabsf(xv)));
+        else if (vx.kind == VX_FOCAL_SIG) ce = focal_sig<TK != T_SOFT_F32>(xv, t, fw[0], vx, nullptr);
+        // the softmax form over one channel: log_softmax = 0, no term
       } else {
-        float m = -INFINITY;
-        for (int k = 0; k < C; ++k) m = fmaxf(m, sm.xs[k * kP + v]);
         const int l = TK < T_ONEHOT_U8 ? sm.lab[v] : -1;
-        const float xl = l >= 0 ? sm.xs[l * kP + v] : 0.f;
-        float sum = 0.f, tx = 0.f, tsum = 0.f;
-        for (int k = 0; k < C; ++k) {
-          const float xv = sm.xs[k * kP + v];
-          const float e = __expf(xv - m);
-          sum += e;
-          if (ACT == A_SOFTMAX) sm.xs[k * kP + v] = e;
-          if (TK >= T_ONEHOT_U8) {
-            const float t = sm.ts[k * kP + v];
-            tx += t * xv;
-            tsum += t;
+        if (vx.kind != VX_FOCAL_SIG || ACT == A_SOFTMAX) {
+          float m = -INFINITY;
+          for (int k = 0; k < C; ++k) m = fmaxf(m, sm.xs[k * kP + v]);
+          const float xl = l >= 0 ? sm.xs[l * kP + v] : 0.f;
+          float sum = 0.f, tx = 0.f, tsum = 0.f;
+          for (int k = 0; k < C; ++k) {
+            const float xv = sm.xs[k * kP + v];
+            const float e = __expf(xv - m);
+            sum += e;
+            if (ACT == A_SOFTMAX && !keep) sm.xs[k * kP + v] = e;
+            if (TK >= T_ONEHOT_U8) {
+              const float t = sm.ts[k * kP + v];
+              tx += t * xv;
+              tsum += t;
+            }
+          }
+          const float lse = m + logf(sum);
+          if (ACT == A_SOFTMAX) {
+            sm.inv[v] = 1.f / sum;
+            if (keep) mrow[v] = m;
+          }
+          if (vx.kind <= VX_CE) {
+            ce = TK >= T_ONEHOT_U8 ? lse * tsum - tx : (l >= 0 ? lse - xl : 0.f);
+          } else if (vx.kind == VX_FOCAL_SMX) {
+            const float lsf = vx.lo ? lse_from1(sm.xs, C, v) : lse;
+            if (TK < T_ONEHOT_U8) {
+              if (l >= vx.lo) ce = focal_smx(xl - lsf, 1.f, fw[l], vx.gamma, nullptr);
+            } else {
+              for (int k = vx.lo; k < C; ++k) {
+                const float t = sm.ts[k * kP + v];
+                if (t != 0.f) ce += focal_smx(sm.xs[k * kP + v] - lsf, t, fw[k], vx.gamma, nullptr);
+              }
+            }
           }
         }
-        const float lse = m + logf(sum);
-        if (ACT == A_SOFTMAX) sm.inv[v] = 1.f / sum;
-        ce = TK >= T_ONEHOT_U8 ? lse * tsum - tx : (l >= 0 ? lse - xl : 0.f);
+        if (vx.kind == VX_FOCAL_SIG)
+          for (int k = vx.lo; k < C; ++k) {
+            const float t = TK >= T_ONEHOT_U8 ? sm.ts[k * kP + v] : (k == l ? 1.f : 0.f);
+            ce += focal_sig<TK != T_SOFT_F32>(sm.xs[k * kP + v], t, fw[k], vx, nullptr);
+          }
       }
       ace += ce;
     }
     __syncthreads();
-    // phase B: channel c's Dice sums over this thread's slice of the tile
-    if (slice < K) {
+    // phase B: channel c's Dice sums over this thread's slice of the tile.  KEEP (the tile holds raw logits) is a uniform
+    // branch outside the loop, so the CE path's loop stays as it was
+    auto phase_b = [&](auto keep_c) {
+      constexpr bool KEEP = decltype(keep_c)::value;
       float I[2] = {0.f, 0.f}, P[2] = {0.f, 0.f}, T[2] = {0.f, 0.f};   // two interleaved chains: voxels v and v + K
       auto acc = [&](int v, int j) {
         const float r = sm.xs[c * kP + v];
-        const float p = ACT == A_SOFTMAX ? r * sm.inv[v] : ACT == A_SIGMOID ? sigm(r) : r;
+        const float p = ACT == A_SOFTMAX ? (KEEP ? __expf(r - mrow[v]) : r) * sm.inv[v] : ACT == A_SIGMOID ? sigm(r) : r;
         const float t = TK >= T_ONEHOT_U8 ? sm.ts[c * kP + v] : (sm.lab[v] == c ? 1.f : 0.f);
         I[j] += p * t;
         P[j] += squared ? p * p : p;
@@ -177,6 +282,10 @@ __global__ void __launch_bounds__(kThreads) k_dice_ce_fwd(const float* __restric
       for (; v + K < nv; v += 2 * K) { acc(v, 0); acc(v + K, 1); }
       if (v < nv) acc(v, 0);
       aI += I[0] + I[1]; aP += P[0] + P[1]; aT += T[0] + T[1];
+    };
+    if (with_dice && slice < K) {
+      if (keep) phase_b(std::true_type());
+      else phase_b(std::false_type());
     }
     __syncthreads();
   }
@@ -222,20 +331,25 @@ __global__ void k_dice_ce_reduce(const double* __restrict__ part, const double* 
   }
 }
 
-// grid (grid_x, N); one voxel per thread
+// grid (grid_x, N); one voxel per thread.  At most 64 registers (8 blocks per SM), as before the focal term: uncapped, the focal
+// paths take 72 and spill in three instantiations
 template <int TK, int ACT>
-__global__ void __launch_bounds__(kThreads) k_dice_ce_bwd(const float* __restrict__ x, const void* __restrict__ tgt, int C, long long S,
-                                                          int squared, int with_ce, double ce_scale, const double* __restrict__ coef,
+__global__ void __launch_bounds__(kThreads, 8) k_dice_ce_bwd(const float* __restrict__ x, const void* __restrict__ tgt, int C, long long S,
+                                                          int squared, Vox vx, double ce_scale, const double* __restrict__ coef,
                                                           const float* __restrict__ grad_out, float* __restrict__ dx) {
+  constexpr bool BIN = TK != T_SOFT_F32;   // label maps and uint8 one-hot targets hold 0 or 1
   extern __shared__ __align__(16) unsigned char smem[];
   const Smem sm = carve(smem, C, TK);
   float* a = reinterpret_cast<float*>(sm.red);      // [C] dF/dI and [C] dF/dP coefficients of sample n, times grad_out
   float* b = a + C;
+  float* fw = b + C;                                // [C] focal class factors
   const int n = blockIdx.y, v = threadIdx.x;
   const float go = *grad_out;
+  const bool keep = vx.kind >= VX_FOCAL_SIG;        // the focal term reads the raw logits: the tile keeps them
   for (int c = v; c < C; c += kThreads) {
     a[c] = (float)(coef[((long long)n * C + c) * 2] * go);
     b[c] = (float)(coef[((long long)n * C + c) * 2 + 1] * go);
+    if (keep) fw[c] = focal_class_factor(vx, c);
   }
   const float cg = (float)(ce_scale * go);
   const float* xn = x + (long long)n * C * S;
@@ -244,7 +358,7 @@ __global__ void __launch_bounds__(kThreads) k_dice_ce_bwd(const float* __restric
   for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
     const long long s0 = tile * kV;
     const int nv = (int)(S - s0 < kV ? S - s0 : kV);
-    stage_tile<TK>(xn, tgt, n, C, S, s0, nv, sm.xs, sm.ts, sm.lab);   // its barrier also publishes a / b
+    stage_tile<TK>(xn, tgt, n, C, S, s0, nv, sm.xs, sm.ts, sm.lab);   // its barrier also publishes a / b / fw
     if (v < nv) {
       float* o = dxn + s0 + v;
       if (C == 1) {
@@ -252,45 +366,90 @@ __global__ void __launch_bounds__(kThreads) k_dice_ce_bwd(const float* __restric
         const float q = sigm(xv);
         const float p = ACT == A_SIGMOID ? q : xv;
         const float g = a[0] * t + b[0] * (squared ? 2.f * p : 1.f);
-        *o = (ACT == A_SIGMOID ? g * p * (1.f - p) : g) + cg * (q - t);
+        const float dd = ACT == A_SIGMOID ? g * p * (1.f - p) : g;
+        if (vx.kind <= VX_CE) {
+          *o = dd + cg * (q - t);
+        } else {
+          float df = 0.f;                                   // the softmax form over one channel has no term
+          if (vx.kind == VX_FOCAL_SIG) focal_sig<BIN>(xv, t, fw[0], vx, &df);
+          *o = dd + cg * df;
+        }
       } else {
         const int l = TK < T_ONEHOT_U8 ? sm.lab[v] : -1;
-        float m = -INFINITY, inv = 0.f, tsum = 0.f;
-        if (with_ce || ACT == A_SOFTMAX) {
+        float m = -INFINITY, inv = 0.f, tsum = 0.f, lsf = 0.f;
+        if (vx.kind == VX_CE || vx.kind == VX_FOCAL_SMX || ACT == A_SOFTMAX) {
           for (int k = 0; k < C; ++k) m = fmaxf(m, sm.xs[k * kP + v]);
           float sum = 0.f;
           for (int k = 0; k < C; ++k) {
             const float e = __expf(sm.xs[k * kP + v] - m);
             sum += e;
-            if (ACT == A_SOFTMAX) sm.xs[k * kP + v] = e;
+            if (ACT == A_SOFTMAX && !keep) sm.xs[k * kP + v] = e;
             if (TK >= T_ONEHOT_U8) tsum += sm.ts[k * kP + v];
           }
           inv = 1.f / sum;
+          if (vx.kind == VX_FOCAL_SMX) lsf = vx.lo ? lse_from1(sm.xs, C, v) : m + logf(sum);
         }
         if (TK < T_ONEHOT_U8) tsum = l >= 0 ? 1.f : 0.f;
-        if (ACT == A_SOFTMAX) {
-          float s = 0.f;
-          for (int k = 0; k < C; ++k) {
-            const float p = sm.xs[k * kP + v] * inv;
-            const float t = TK >= T_ONEHOT_U8 ? sm.ts[k * kP + v] : (k == l ? 1.f : 0.f);
-            s += p * (a[k] * t + b[k] * (squared ? 2.f * p : 1.f));
-          }
-          for (int k = 0; k < C; ++k) {
-            const float p = sm.xs[k * kP + v] * inv;
-            const float t = TK >= T_ONEHOT_U8 ? sm.ts[k * kP + v] : (k == l ? 1.f : 0.f);
-            const float g = a[k] * t + b[k] * (squared ? 2.f * p : 1.f);
-            o[(long long)k * S] = p * (g - s) + cg * (p * tsum - t);
-          }
-        } else {
-          for (int k = 0; k < C; ++k) {
-            const float xv = sm.xs[k * kP + v];
-            const float p = ACT == A_SIGMOID ? sigm(xv) : xv;
-            const float t = TK >= T_ONEHOT_U8 ? sm.ts[k * kP + v] : (k == l ? 1.f : 0.f);
-            const float g = a[k] * t + b[k] * (squared ? 2.f * p : 1.f);
-            const float dd = ACT == A_SIGMOID ? g * p * (1.f - p) : g;
-            o[(long long)k * S] = with_ce ? dd + cg * (__expf(xv - m) * inv * tsum - t) : dd;
+        // softmax focal: U = sum_c u_c over the kept channels; dx_j gains u_j - p'_j U
+        float U = 0.f;
+        if (vx.kind == VX_FOCAL_SMX) {
+          if (TK < T_ONEHOT_U8) {
+            if (l >= vx.lo) focal_smx(sm.xs[l * kP + v] - lsf, 1.f, fw[l], vx.gamma, &U);
+          } else {
+            for (int k = vx.lo; k < C; ++k) {
+              const float t = sm.ts[k * kP + v];
+              float u = 0.f;
+              if (t != 0.f) focal_smx(sm.xs[k * kP + v] - lsf, t, fw[k], vx.gamma, &u);
+              U += u;
+            }
           }
         }
+        // the focal term's derivative by the raw logit xv of channel k
+        auto focal_grad = [&](int k, float xv, float t) -> float {
+          if (vx.kind == VX_FOCAL_SIG) {
+            float df = 0.f;
+            if (k >= vx.lo) focal_sig<BIN>(xv, t, fw[k], vx, &df);
+            return df;
+          }
+          if (k < vx.lo) return 0.f;
+          const float ls = xv - lsf;
+          float u = 0.f;
+          if (TK < T_ONEHOT_U8) u = k == l ? U : 0.f;
+          else if (t != 0.f) focal_smx(ls, t, fw[k], vx.gamma, &u);
+          return u - __expf(ls) * U;
+        };
+        // FOCAL: the focal term, and the tile holds raw logits.  A uniform branch outside the loops, so the CE path's loops stay
+        // as they were
+        auto out_loops = [&](auto focal_c) {
+          constexpr bool FOCAL = decltype(focal_c)::value;
+          if (ACT == A_SOFTMAX) {
+            float s = 0.f;
+            for (int k = 0; k < C; ++k) {
+              const float p = (FOCAL ? __expf(sm.xs[k * kP + v] - m) : sm.xs[k * kP + v]) * inv;
+              const float t = TK >= T_ONEHOT_U8 ? sm.ts[k * kP + v] : (k == l ? 1.f : 0.f);
+              s += p * (a[k] * t + b[k] * (squared ? 2.f * p : 1.f));
+            }
+            for (int k = 0; k < C; ++k) {
+              const float r = sm.xs[k * kP + v];
+              const float p = (FOCAL ? __expf(r - m) : r) * inv;
+              const float t = TK >= T_ONEHOT_U8 ? sm.ts[k * kP + v] : (k == l ? 1.f : 0.f);
+              const float g = a[k] * t + b[k] * (squared ? 2.f * p : 1.f);
+              o[(long long)k * S] = FOCAL ? p * (g - s) + cg * focal_grad(k, r, t) : p * (g - s) + cg * (p * tsum - t);
+            }
+          } else {
+            for (int k = 0; k < C; ++k) {
+              const float xv = sm.xs[k * kP + v];
+              const float p = ACT == A_SIGMOID ? sigm(xv) : xv;
+              const float t = TK >= T_ONEHOT_U8 ? sm.ts[k * kP + v] : (k == l ? 1.f : 0.f);
+              const float g = a[k] * t + b[k] * (squared ? 2.f * p : 1.f);
+              const float dd = ACT == A_SIGMOID ? g * p * (1.f - p) : g;
+              o[(long long)k * S] = FOCAL ? dd + cg * focal_grad(k, xv, t)
+                                          : vx.kind == VX_CE ? dd + cg * (__expf(xv - m) * inv * tsum - t) : dd;
+            }
+          }
+        };
+        if (keep) out_loops(std::true_type());
+        else out_loops(std::false_type());
       }
     }
     __syncthreads();
@@ -314,6 +473,15 @@ int check_shape(const DiceCEDesc& d, int N, int C, long long S, Shape* sh) {
   }
   sh->slots = grid_x(N, C, S, sh->kind);
   return OK;
+}
+
+// the per-voxel term of a launch: none when lambda_ce = 0
+Vox vox_of(const DiceCEDesc& d, int C) {
+  Vox v;
+  v.kind = d.lambda_ce == 0.f ? VX_NONE : d.voxel_term == V_CE ? VX_CE : d.focal_softmax ? VX_FOCAL_SMX : VX_FOCAL_SIG;
+  v.lo = (!d.include_background && C > 1) ? 1 : 0;
+  v.gamma = d.focal_gamma; v.alpha = d.focal_alpha; v.use_alpha = d.focal_use_alpha; v.w = d.class_weight;
+  return v;
 }
 
 struct Scratch {
@@ -358,10 +526,11 @@ int launch_dice_ce_fwd(const DiceCEDesc& d, const float* logits, const void* tar
   const Scratch s = carve_scratch(scratch, sh);
   const size_t smem = tile_smem(sh.C, sh.kind);
   const dim3 grid(sh.slots, N);
-  const int with_ce = d.lambda_ce != 0.f;
+  const Vox vx = vox_of(d, C);
 #define B200_FWD(tk, ac)                                                                                                \
   B200_TRY(set_smem(k_dice_ce_fwd<tk, ac>, smem));                                                                      \
-  k_dice_ce_fwd<tk, ac><<<grid, kThreads, smem, st>>>(logits, target, C, S, d.squared_pred, with_ce, s.part, s.ce_part);
+  k_dice_ce_fwd<tk, ac><<<grid, kThreads, smem, st>>>(logits, target, C, S, d.squared_pred, d.lambda_dice != 0.f, vx, s.part,  \
+                                                      s.ce_part);
   B200_DICE_CE_SWITCH(B200_FWD)
 #undef B200_FWD
   B200_CHECK_CUDA(cudaGetLastError());
@@ -378,11 +547,11 @@ int launch_dice_ce_bwd(const DiceCEDesc& d, const float* logits, const void* tar
   const Scratch s = carve_scratch(const_cast<void*>(scratch), sh);
   const size_t smem = tile_smem(sh.C, sh.kind);
   const dim3 grid(sh.slots, N);
-  const int with_ce = d.lambda_ce != 0.f;
-  const double ce_scale = d.lambda_ce * (d.reduction == 0 ? 1.0 / ((double)N * S) : 1.0);
+  const Vox vx = vox_of(d, C);
+  const double ce_scale = d.lambda_ce * (1.0 / voxel_divisor(d, N, C, S));
 #define B200_BWD(tk, ac)                                                                                                 \
   B200_TRY(set_smem(k_dice_ce_bwd<tk, ac>, smem));                                                                       \
-  k_dice_ce_bwd<tk, ac><<<grid, kThreads, smem, st>>>(logits, target, C, S, d.squared_pred, with_ce, ce_scale, s.coef,   \
+  k_dice_ce_bwd<tk, ac><<<grid, kThreads, smem, st>>>(logits, target, C, S, d.squared_pred, vx, ce_scale, s.coef,        \
                                                       grad_out, dlogits);
   B200_DICE_CE_SWITCH(B200_BWD)
 #undef B200_BWD

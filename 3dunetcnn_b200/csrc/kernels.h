@@ -77,17 +77,36 @@ int launch_input_grad(const Act* dz, const Act* x, const float* coef, const floa
 // ---- Dice criteria: the options of both; the fields mirror b200unet_dice_ce_desc
 enum TargetKind { T_LABEL_U8 = 0, T_LABEL_I64 = 1, T_ONEHOT_U8 = 2, T_SOFT_F32 = 3 };
 enum ActKind { A_NONE = 0, A_SIGMOID = 1, A_SOFTMAX = 2 };
+enum OverlapKind { O_DICE = 0, O_TVERSKY = 1, O_GDICE = 2 };
+enum GDiceWeight { W_SQUARE = 0, W_SIMPLE = 1, W_UNIFORM = 2 };
+enum VoxelTerm { V_CE = 0, V_FOCAL = 1 };
 struct DiceCEDesc {
   int act;               // ActKind: 0 identity, 1 sigmoid, 2 softmax over channels
   int target_kind;       // TargetKind: 0 uint8 label map [N][1][S], 1 int64 label map, 2 uint8 [N][C][S], 3 fp32 [N][C][S]
   int include_background, squared_pred, jaccard, batch;
   int reduction;         // 0 mean, 1 sum
   float smooth_nr, smooth_dr, lambda_dice, lambda_ce;
+  // a zeroed tail is the Dice overlap with the CE term
+  int overlap;           // OverlapKind
+  float tversky_alpha, tversky_beta;
+  int w_type;            // GDiceWeight
+  int voxel_term;        // VoxelTerm, scaled by lambda_ce
+  int focal_softmax;     // focal: 0 sigmoid form, 1 softmax form over the kept channels
+  float focal_gamma, focal_alpha;
+  int focal_use_alpha;
+  const float* class_weight;   // focal: DEVICE fp32 [C'] (C' = channels kept), nullptr = none
 };
 // the checks both criteria make: a non-empty shape and in-range options ("who" prefixes the error message)
 int check_dice_desc(const DiceCEDesc& d, int N, int C, long long S, const char* who);
+// The per-voxel term's total is divided by this: CE: N*S (mean) or 1 (sum); focal: N*C'*S (mean) or S (sum, MONAI's
+// FocalLoss averages over the voxels before it sums over samples and classes)
+__host__ __device__ inline double voxel_divisor(const DiceCEDesc& d, int N, int C, long long S) {
+  if (d.voxel_term == V_CE) return d.reduction == 0 ? (double)N * S : 1.0;
+  const int kept = (!d.include_background && C > 1) ? C - 1 : C;
+  return d.reduction == 0 ? (double)N * kept * S : (double)S;
+}
 // The loss and coef [N][C][2] (the backward's dF/dI, dF/dP per (n, c)) from sums [N][C][3] (I, P, T) in one single-block
-// launch; ce [N] (the summed CE terms of each sample) is read only when lambda_ce != 0 (dice.cu)
+// launch; ce [N] (the summed per-voxel terms of each sample) is read only when lambda_ce != 0 (dice.cu)
 int launch_dice_finalize(const DiceCEDesc& d, const double* sums, const double* ce, int N, int C, long long S, double* coef,
                          float* loss, cudaStream_t st);
 

@@ -59,10 +59,14 @@ WGRAD_KINDS = ("simt", "tap", "halo")               # b200unet_wgrad_route.kind
 
 
 class DiceCEDesc(C.Structure):
-    """``b200unet_dice_ce_desc``: options of both Dice criteria (DiceLoss and DiceCELoss)."""
+    """``b200unet_dice_ce_desc``: options of every fused criterion (DiceLoss, DiceCELoss, TverskyLoss, GeneralizedDiceLoss,
+    FocalLoss, DiceFocalLoss)."""
     _fields_ = [("act", C.c_int32), ("target_kind", C.c_int32), ("include_background", C.c_int32), ("squared_pred", C.c_int32),
                 ("jaccard", C.c_int32), ("batch", C.c_int32), ("reduction", C.c_int32), ("smooth_nr", C.c_float),
-                ("smooth_dr", C.c_float), ("lambda_dice", C.c_float), ("lambda_ce", C.c_float)]
+                ("smooth_dr", C.c_float), ("lambda_dice", C.c_float), ("lambda_ce", C.c_float),
+                ("overlap", C.c_int32), ("tversky_alpha", C.c_float), ("tversky_beta", C.c_float), ("w_type", C.c_int32),
+                ("voxel_term", C.c_int32), ("focal_softmax", C.c_int32), ("focal_gamma", C.c_float), ("focal_alpha", C.c_float),
+                ("focal_use_alpha", C.c_int32), ("class_weight", C.c_void_p)]
 
 
 class NetDesc(C.Structure):
@@ -559,8 +563,17 @@ DICE_CE_TARGETS = {"label_u8": 0, "label_i64": 1, "onehot_u8": 2, "soft_f32": 3}
 _DICE_CE_ACTS = {None: 0, "sigmoid": 1, "softmax": 2}
 
 
+# b200unet_dice_ce_desc.overlap, .w_type and .voxel_term
+DICE_CE_OVERLAPS = {"dice": 0, "tversky": 1, "generalized_dice": 2}
+GDICE_WEIGHTS = {"square": 0, "simple": 1, "uniform": 2}
+DICE_CE_VOXEL_TERMS = {"ce": 0, "focal": 1}
+
+
 def dice_ce_desc(act=None, target_kind=0, include_background=True, squared_pred=False, jaccard=False, batch=False,
-                 reduction="mean", smooth_nr=1e-5, smooth_dr=1e-5, lambda_dice=1.0, lambda_ce=1.0) -> DiceCEDesc:
+                 reduction="mean", smooth_nr=1e-5, smooth_dr=1e-5, lambda_dice=1.0, lambda_ce=1.0, overlap="dice",
+                 tversky_alpha=0.5, tversky_beta=0.5, w_type="square", voxel_term="ce", focal_softmax=False, focal_gamma=2.0,
+                 focal_alpha=None, class_weight=None) -> DiceCEDesc:
+    """``class_weight``: a CUDA fp32 tensor of the focal term's per-class factors, or None; the caller keeps it alive"""
     if reduction not in ("mean", "sum"):
         raise ValueError("fused DiceCE supports reduction 'mean' or 'sum', got %r" % (reduction,))
     d = DiceCEDesc()
@@ -568,6 +581,14 @@ def dice_ce_desc(act=None, target_kind=0, include_background=True, squared_pred=
     d.include_background, d.squared_pred, d.jaccard, d.batch = (int(bool(v)) for v in (include_background, squared_pred, jaccard, batch))
     d.reduction = int(reduction == "sum")
     d.smooth_nr, d.smooth_dr, d.lambda_dice, d.lambda_ce = float(smooth_nr), float(smooth_dr), float(lambda_dice), float(lambda_ce)
+    d.overlap, d.w_type, d.voxel_term = DICE_CE_OVERLAPS[overlap], GDICE_WEIGHTS[w_type], DICE_CE_VOXEL_TERMS[voxel_term]
+    if overlap == "tversky":
+        d.tversky_alpha, d.tversky_beta = float(tversky_alpha), float(tversky_beta)
+    if voxel_term == "focal":
+        d.focal_softmax, d.focal_gamma = int(bool(focal_softmax)), float(focal_gamma)
+        d.focal_use_alpha = int(focal_alpha is not None)
+        d.focal_alpha = float(focal_alpha) if focal_alpha is not None else 0.0
+        d.class_weight = class_weight.data_ptr() if class_weight is not None else None
     return d
 
 

@@ -144,10 +144,27 @@ typedef struct b200unet_dice_ce_desc {
   int32_t include_background, squared_pred, jaccard, batch;
   int32_t reduction;            /* 0 mean, 1 sum */
   float smooth_nr, smooth_dr, lambda_dice, lambda_ce;
+  /* Everything below is the dice_ce entry points' alone; zeroed, it is the Dice overlap with the CE term above. */
+  int32_t overlap;              /* 0 Dice; 1 Tversky (monai.losses.TverskyLoss): f = 1 - (I + smooth_nr) / (I + tversky_alpha (P - I)
+                                   + tversky_beta (T - I) + smooth_dr); 2 generalized Dice (GeneralizedDiceLoss): per sample (once
+                                   with batch) f = 1 - (2 sum_c w_c I_c + smooth_nr) / (sum_c w_c (P_c + T_c) + smooth_dr), w_c from
+                                   T_c by w_type, an infinite weight replaced by the largest finite one of the sample (of all, with
+                                   batch); squared_pred and jaccard 0 for both */
+  float tversky_alpha, tversky_beta;
+  int32_t w_type;               /* generalized Dice: 0 1/T^2, 1 1/T, 2 uniform */
+  int32_t voxel_term;           /* the term lambda_ce scales: 0 CE, 1 focal (monai.losses.FocalLoss) on the channels include_background
+                                   keeps; mean divides its total by n * c' * spatial, sum by spatial (MONAI averages over the voxels) */
+  int32_t focal_softmax;        /* 0 sigmoid form, per element (x - x t - logsigmoid(x)) exp(gamma logsigmoid(-x (2t - 1)));
+                                   1 softmax form -(1 - exp(ls))^gamma ls t, ls = log_softmax over the kept channels */
+  float focal_gamma;            /* >= 0 */
+  float focal_alpha;            /* with focal_use_alpha: sigmoid t alpha + (1 - t)(1 - alpha), softmax 1 - alpha on the first kept
+                                   channel and alpha on the others */
+  int32_t focal_use_alpha;
+  const float* class_weight;    /* focal: DEVICE fp32 [c'] per-class factors, NULL = none */
 } b200unet_dice_ce_desc;
 
 /* DiceLoss: act 0 or 1 (softmax: E_UNSUPPORTED, b200unet_dice_ce_* runs it), target_kind 2 or 3 (label maps: E_UNSUPPORTED),
- * lambda_ce 0 (else E_INVALID); any c >= 1.  logits NCDHW fp32.
+ * lambda_ce 0 (else E_INVALID), overlap and voxel_term 0 (else E_UNSUPPORTED); any c >= 1.  logits NCDHW fp32.
  * scratch: [n][c][3] fp64 sums (I, P, T) followed by [n][c][2] fp64 backward coefficients, written by fwd and read by bwd.
  * The sums are added with fp64 atomics, so the loss may differ in its last bits from run to run. */
 int b200unet_dice_fwd(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c,
@@ -156,8 +173,9 @@ int b200unet_dice_bwd(const b200unet_dice_ce_desc* desc, const float* logits, co
                       int64_t spatial, const double* scratch, const float* grad_out, float* dlogits, void* stream);
 
 /* DiceCELoss: CE is on the raw logits: -sum_c t_c log_softmax(x)_c for c > 1 (a label map is its one-hot row),
- * BCEWithLogits(x, t) for c == 1; mean divides by n * spatial.  lambda_ce = 0 means the CE term is not evaluated, so logits of +-inf give a finite sigmoid Dice
- * loss and gradient.  With c == 1 softmax is ignored and a uint8 label map is the target itself (int64: E_UNSUPPORTED).
+ * BCEWithLogits(x, t) for c == 1; mean divides by n * spatial.  lambda_ce = 0 means the CE (or focal) term is not evaluated, so logits of +-inf give a finite sigmoid Dice
+ * loss and gradient; lambda_dice = 0 likewise skips the overlap sums.  The same entry points run TverskyLoss, GeneralizedDiceLoss,
+ * FocalLoss and DiceFocalLoss through the descriptor's tail.  With c == 1 softmax is ignored and a uint8 label map is the target itself (int64: E_UNSUPPORTED).
  * A label outside [0, c) is an all-zero target row.  logits NCDHW fp32, 1 <= c <= 128.
  * scratch: b200unet_dice_ce_scratch_bytes() bytes (0 = the options or shape are rejected), written by fwd and read by bwd.
  * It starts with sums [n][c][3] fp64 (I, P, T) and ce [n] fp64 (the summed CE terms of each sample).  No floating-point
