@@ -57,6 +57,7 @@ static int to_conv_op(const b200unet_conv_desc* d, const b200unet_diag_ext* ext,
     op.bias = ext->bias;
     op.zero_last = ext->zero_last;
     op.max_ctas = ext->max_ctas;
+    op.tile128 = ext->tile128;
     for (int s = 0; s < d->nsrc; ++s) {
       op.src[s].x.vD = ext->x_vis[s][0]; op.src[s].x.vH = ext->x_vis[s][1]; op.src[s].x.vW = ext->x_vis[s][2];
     }
@@ -329,6 +330,7 @@ int b200unet_diag_conv3d_route(const b200unet_conv_desc* desc, const b200unet_di
   route->tw = r.tw; route->th = r.th; route->td = r.td;
   for (int i = 0; i < 3; ++i) route->grid[i] = r.grid[i];
   route->stages = r.stages; route->blocks_per_sm = r.blocks_per_sm; route->smem_bytes = r.smem_bytes;
+  route->wgs = r.wgs;
   return OK;
 }
 

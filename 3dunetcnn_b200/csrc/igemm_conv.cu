@@ -28,8 +28,9 @@ namespace b200 {
 // taps read it through shifted shared-memory descriptors (27x less activation traffic from L2 than per-tap boxes).
 // CONV_HALO_WS is halo mode on the persistent, weight-stationary kernel (k_igemm_conv_halo_ws) for the (BN, KC) whose 27 weight
 // tiles fit in shared memory beside the halo box; CONV_HALO runs the ring kernel below for the wider ones.  CONV_HALO_PAIR
-// (k_igemm_conv_halo_pair) shares resident weights and one two-plane halo box between two consumer warpgroups.
-enum ConvMode { CONV_STREAM = 0, CONV_CLASS = 1, CONV_HALO = 2, CONV_HALO_WS = 3, CONV_HALO_PAIR = 4 };
+// (k_igemm_conv_halo_pair) shares resident weights and one two-plane halo box between two consumer warpgroups.  CONV_WIDE
+// (k_igemm_conv_wide) runs per-tap tiles of 256 voxels on two consumer warpgroups that share each weight tile.
+enum ConvMode { CONV_STREAM = 0, CONV_CLASS = 1, CONV_HALO = 2, CONV_HALO_WS = 3, CONV_HALO_PAIR = 4, CONV_WIDE = 5 };
 
 // Tile sizes and shared-memory limits both convolution kernels derive from (BN, KC).
 template <int BN, int KC>
@@ -318,6 +319,185 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
                     threadIdx.x);
   }
   if (threadIdx.x == 0) tma_store_wait_all();   // the staging tile must outlive the bulk store
+}
+
+// Wide per-tap mode (CONV_WIDE) for BN = 128: a 256-voxel tile, the 128-voxel tile of the kernel above doubled in depth.  Every
+// tap of a 128-channel tile is 1 M MACs per K chunk, fed by a 16 KB activation box and a 16 KB weight box from L2; here one ring
+// stage holds the activation box of 256 voxels and ONE weight box, and two consumer warpgroups issue their MMAs from it, warpgroup
+// g on rows 128 g .. 128 g + 127 (output planes d0 + g td / 2 ..): 48 KB per 2 M MACs instead of 32 KB per 1 M.  The producer
+// loop is the kernel above's (taps, K chunks, passes, then the second source); a stage goes back to it once both warpgroups'
+// MMAs have retired it (eight warp arrivals).  Every output row sees the MMA order of the 128-voxel kernel, so the stored output
+// is the same bit for bit, and each warpgroup flushes its own per-channel statistics as a 128-voxel CTA does.
+// 384 threads: warpgroups 0 and 1 consume, warp 8 of warpgroup 2 produces.  setmaxnreg moves the registers the producer
+// warpgroup does not need to the consumers (40 / 232 per thread), whose 128-float accumulator the 168 of an even split cannot
+// hold next to the epilogue.
+// Shared memory: STAGES-deep ring [A 256 x KC | B 128 x KC] | bf16 output staging (64 KB) | aux (barriers | per-warp stats of 8
+// warps | coef).  Once both warpgroups have retired their last MMAs the ring is drained and holds their two fp32 accumulator tiles
+// [128][BN + 4], so that the two epilogues run side by side.  In bf16 the staging region holds both warpgroups' hi tiles; in
+// split precision it holds the hi + lo tiles of one, and warpgroup 1 writes them once warpgroup 0's TMA store has read its own.
+template <int KC>
+struct WideCfg : ConvTileCfg<128, KC> {
+  using Tile = ConvTileCfg<128, KC>;
+  static constexpr int BN = 128;
+  static constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= the 64 K register file
+  static constexpr int A_BYTES = 2 * Tile::A_BYTES;
+  static constexpr int STAGE_BYTES = A_BYTES + Tile::B_BYTES;
+  static constexpr int OUT_TILE = 128 * BN * 2;           // one bf16 output tile of a warpgroup
+  static constexpr int STG_BYTES = 2 * OUT_TILE;
+  static constexpr int AUX_BYTES = 1024 + 8 * BN * 2 * 4 + BN * 16;
+  static constexpr int FIXED = STG_BYTES + AUX_BYTES + 1024;   // +1024 alignment slack
+  static constexpr int STAGES_RAW = (Tile::SMEM_LIMIT - FIXED) / STAGE_BYTES;
+  static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
+  static constexpr int BLOCKS_PER_SM = 1;
+  static constexpr int PIPE_BYTES = STAGES * STAGE_BYTES > 2 * Tile::ACC_BYTES ? STAGES * STAGE_BYTES : 2 * Tile::ACC_BYTES;
+  static constexpr int SMEM_BYTES = PIPE_BYTES + FIXED;
+  // KC 64: 3 x 49,152 (>= 2 x 67,584) + 65,536 + 11,264 + 1,024 = 225,280 B
+  static_assert(STAGES >= 3 && SMEM_BYTES <= Tile::SMEM_LIMIT && 128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= 65536,
+                "igemm_conv: wide per-tap configuration");
+};
+
+template <int KC>
+__global__ void __launch_bounds__(384, 1) k_igemm_conv_wide(const __grid_constant__ ConvMaps maps, const ConvArgs p) {
+  using Cfg = WideCfg<KC>;
+  constexpr int BN = Cfg::BN;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* stg = smem + Cfg::PIPE_BYTES;
+  uint8_t* aux = stg + Cfg::STG_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);
+  uint64_t* empty_bar = full_bar + Cfg::STAGES;
+  float* s_stats_all = reinterpret_cast<float*>(aux + 1024);               // [8 warps][BN][2]
+  float4* s_coef = reinterpret_cast<float4*>(aux + 1024 + 8 * BN * 8);     // [BN]
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int wg = warp >> 2;                       // consumer warpgroup (2: the producer)
+  const int tid = threadIdx.x & 127;
+
+  int t = blockIdx.x;
+  const int wt = t % p.tiles_w; t /= p.tiles_w;
+  const int ht = t % p.tiles_h; t /= p.tiles_h;
+  const int dt = t % p.tiles_d;
+  const int n = t / p.tiles_d;
+  const int w0 = wt * p.tw, h0 = ht * p.th, d0 = dt * p.td;
+  const int n0 = blockIdx.y * BN;
+
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&maps.a[0][0]);
+    tma_prefetch_desc(&maps.b[0][0]);
+    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
+    fence_barrier_init();
+  }
+  pdl_wait();   // before the first global read (the coefficient table below); the barrier set-up above overlaps the previous kernel
+  if (wg < 2) {
+    for (int i = threadIdx.x; i < 8 * BN * 2; i += 256) s_stats_all[i] = 0.f;
+    if (p.mode == 1 && wg == 0) load_coef<BN>(s_coef, p, n, n0, tid);
+  }
+  __syncthreads();
+  pdl_launch_dependents();
+
+  const int total_iters = (p.ntaps[0] * p.kchunks[0] + p.ntaps[1] * p.kchunks[1]) * p.npass;
+  if (wg == 2) {
+    // ------------------------------------------------------------------ TMA producer (warp 8 convergent, one lane issues)
+    setmaxnreg_dec<Cfg::PRODUCER_REGS>();
+    if (warp != 8) return;
+    const uint32_t issue = elect_one() ? 1u : 0u;
+    int it = 0;
+    for (int src = 0; src < 2; ++src) {
+      const int nt = p.ntaps[src];
+      const int ks = p.ksz[src], pad = p.pad[src], sd = p.stride[src];
+      for (int tap = 0; tap < nt; ++tap) {
+        const int kd = tap / (ks * ks), kh = (tap / ks) % ks, kw = tap % ks;
+        const int cw = w0 * sd + kw - pad, ch = h0 * sd + kh - pad, cd = d0 * sd + kd - pad;
+        for (int kc = 0; kc < p.kchunks[src]; ++kc) {
+          for (int pass = 0; pass < p.npass; ++pass) {
+            const int s = it % Cfg::STAGES;
+            mbar_wait(&empty_bar[s], ((it / Cfg::STAGES) & 1) ^ 1);
+            mbar_expect_tx_if(issue, &full_bar[s], Cfg::A_BYTES + Cfg::B_BOX_BYTES);
+            uint8_t* sa = smem + s * Cfg::STAGE_BYTES;
+            tma_load_5d_if(issue, sa, &maps.a[src][pass == 1], &full_bar[s], kc * KC, cw, ch, cd, n);
+            tma_load_3d_if(issue, sa + Cfg::A_BYTES, &maps.b[src][pass == 2], &full_bar[s], kc * KC, n0, tap);
+            ++it;
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumer warpgroups: wgmma, then the epilogue
+  setmaxnreg_inc<Cfg::CONSUMER_REGS>();
+  constexpr uint32_t hi_d = desc_hi(Cfg::SBO, Cfg::LAYOUT);
+  constexpr uint32_t HALF_M = (64 * KC * 2) >> 4;   // descriptor offset of A row 64 of this warpgroup's rows
+  const uint32_t a_wg = desc_lo(smem_u32(smem) + wg * Cfg::Tile::A_BYTES, 16);
+  const uint32_t b_lo0 = desc_lo(smem_u32(smem) + Cfg::A_BYTES, 16);
+  const int row = wg * 128 + tid;
+  const int wl = row % p.tw, hl = (row / p.tw) % p.th, dl = row / (p.tw * p.th);
+  const int w = w0 + wl, h = h0 + hl, d = d0 + dl;
+  const int dw0 = d0 + wg * (p.td >> 1);   // this warpgroup's first output plane
+  const bool valid = (w < p.Wo) && (h < p.Ho) && (d < p.Do);
+  const bool want_stats = (p.mode == 0) ? (p.stats != nullptr) : (p.bstats != nullptr);
+  const bool edge = p.zero_last && (w == p.Wo - 1 || h == p.Ho - 1 || d == p.Do - 1);
+  const bool split = p.out_lo != nullptr;
+  float* s_stats = s_stats_all + wg * 4 * BN * 2;   // [4 warps][BN][2]
+  float* s_acc = reinterpret_cast<float*>(smem + wg * Cfg::ACC_BYTES);   // in the drained ring
+  uint8_t* stage = stg + (split ? 0 : wg * Cfg::OUT_TILE);
+  const long long vox = (((long long)n * p.Do + d) * p.Ho + h) * p.Wo + w;
+  conv_epilogue_prefetch(p, n0, BN, vox, valid);   // -> L2 while the MMAs run
+  auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); };
+
+  float acc[2][BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+  int prev = -1;   // ring slot whose MMAs may still be reading it
+  for (int it = 0; it < total_iters; ++it) {
+    const int s = it % Cfg::STAGES;
+    mbar_wait(&full_bar[s], (it / Cfg::STAGES) & 1);
+    const uint32_t a_lo = a_wg + ((s * Cfg::STAGE_BYTES) >> 4);
+    const uint32_t b_lo = b_lo0 + ((s * Cfg::STAGE_BYTES) >> 4);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < KC / 16; ++k) {
+      const uint32_t accumulate = (it > 0 || k > 0) ? 1u : 0u;
+      Wgmma<BN>::template mma<0, 0>(acc[0], desc_from(a_lo + 2 * k, hi_d), desc_from(b_lo + 2 * k, hi_d), accumulate);
+      Wgmma<BN>::template mma<0, 0>(acc[1], desc_from(a_lo + HALF_M + 2 * k, hi_d), desc_from(b_lo + 2 * k, hi_d), accumulate);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();   // the previous stage's MMAs are complete: hand its slot back to the producer
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+    prev = s;
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc[0]);
+  wgmma_fence_regs(acc[1]);
+  if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+
+  asm volatile("bar.sync 3, 256;" ::: "memory");   // both warpgroups' MMAs have retired: the ring is free
+  store_acc<BN, Cfg::ACC_LD>(s_acc, acc, warp & 3, lane);
+  wg_sync();
+  if (split && wg == 1) asm volatile("bar.sync 4, 256;" ::: "memory");   // warpgroup 0's store has read the staging tiles
+  conv_epilogue_tile<BN>(p, s_acc + tid * Cfg::ACC_LD, warp & 3, lane, n, n0, vox, valid, s_stats, s_coef, want_stats, edge, stage,
+                         tid, split);
+  fence_proxy_async();
+  wg_sync();
+  if (tid == 0 && dw0 < p.Do) {
+#pragma unroll
+    for (int cb = 0; cb < BN / 64; ++cb) {
+      if (n0 + cb * 64 < p.Cout) {
+        tma_store_5d(&maps.o[0], stage + cb * 128 * 64 * 2, n0 + cb * 64, w0, h0, dw0, n);
+        if (split) tma_store_5d(&maps.o[1], stage + 128 * BN * 2 + cb * 128 * 64 * 2, n0 + cb * 64, w0, h0, dw0, n);
+      }
+    }
+    tma_store_commit();
+  }
+  if (split && wg == 0) {
+    if (tid == 0) tma_store_wait_read0();
+    wg_sync();
+    asm volatile("bar.arrive 4, 256;" ::: "memory");
+  }
+  if (want_stats)
+    flush_stats<BN>(s_stats, (p.mode == 0) ? p.stats : p.bstats, (p.mode == 0) ? p.stats_ld : p.coef_ld, p.Cout, n, n0, false, tid);
+  if (tid == 0) tma_store_wait_all();   // the staging tile must outlive the bulk store
 }
 
 // Persistent, weight-stationary halo mode.  With one CTA per 8 x 16 x 1 tile, every CTA fetched all 27 weight tiles through the
@@ -703,13 +883,17 @@ __global__ void __launch_bounds__(288, 1) k_igemm_conv_halo_pair(const __grid_co
 // ----------------------------------------------------------------------------------------------- host side
 // The compile-time configuration of the kernel a (BN, KC, MODE) launch runs.
 template <int BN, int KC, int MODE>
-using ConvCfgOf = std::conditional_t<MODE == CONV_HALO_WS, HaloWsCfg<BN, KC>,
-                                     std::conditional_t<MODE == CONV_HALO_PAIR, HaloPairCfg<BN, KC>, ConvCfg<BN, KC, MODE>>>;
+using ConvCfgOf = std::conditional_t<
+    MODE == CONV_HALO_WS, HaloWsCfg<BN, KC>,
+    std::conditional_t<MODE == CONV_HALO_PAIR, HaloPairCfg<BN, KC>, std::conditional_t<MODE == CONV_WIDE, WideCfg<KC>, ConvCfg<BN, KC, MODE>>>>;
 
 template <int BN, int KC, int MODE>
 static int launch_cfg(const ConvMaps& maps, const ConvArgs& args, dim3 grid, cudaStream_t st, const ConvClassMaps& cmaps) {
   using Cfg = ConvCfgOf<BN, KC, MODE>;
-  if constexpr (MODE == CONV_HALO_PAIR) {
+  if constexpr (MODE == CONV_WIDE) {
+    B200_TRY((set_max_dynamic_smem<k_igemm_conv_wide<KC>>(Cfg::SMEM_BYTES)));
+    launch_pdl(k_igemm_conv_wide<KC>, grid, dim3(384), Cfg::SMEM_BYTES, st, maps, args);
+  } else if constexpr (MODE == CONV_HALO_PAIR) {
     B200_TRY((set_max_dynamic_smem<k_igemm_conv_halo_pair<BN, KC>>(Cfg::SMEM_BYTES)));
     launch_pdl(k_igemm_conv_halo_pair<BN, KC>, grid, dim3(288), Cfg::SMEM_BYTES, st, maps, args);
   } else if constexpr (MODE == CONV_HALO_WS) {
@@ -799,13 +983,21 @@ static bool conv_halo_eligible(const ConvOp& op, int num_sms) {
          (halo_keeps_occupancy(conv_bn(op), conv_kc(op)) || conv_halo_pair(op, num_sms));
 }
 
+// The 256-voxel per-tap tile (k_igemm_conv_wide) for a BN = 128 launch whose CTAs of that tile still give every SM one: below
+// that, halving the CTAs would leave SMs idle that the 128-voxel tiles use (at C2 the 16^3 launches, 64 x 2 CTAs of 128 voxels).
+// tiles_hw: the (h, w) tiles of a sample, td: the depth of the 128-voxel tile.
+static bool conv_wide(const ConvOp& op, int BN, int gD, int tiles_hw, int td, int num_sms) {
+  if (BN != 128 || op.tile128) return false;
+  return (long long)op.out.N * ceil_div(gD, 2 * td) * tiles_hw * ceil_div(op.out.C, BN) >= num_sms;
+}
+
 template <int BN_, int KC_, int MODE_>
 struct ConvKernel { static constexpr int BN = BN_, KC = KC_, MODE = MODE_; };
 
-// f(ConvKernel<BN, KC, MODE>{}) for the instantiated kernel of (kind, BN, KC): the one selection conv_route reports and
-// launch_igemm_conv launches.  E_UNSUPPORTED when no such kernel is instantiated.
+// f(ConvKernel<BN, KC, MODE>{}) for the instantiated kernel of (kind, BN, KC) with wgs consumer warpgroups: the one selection
+// conv_route reports and launch_igemm_conv launches.  E_UNSUPPORTED when no such kernel is instantiated.
 template <class F>
-static int with_conv_kernel(int kind, int BN, int KC, F&& f) {
+static int with_conv_kernel(int kind, int BN, int KC, int wgs, F&& f) {
 #define B200_CONV_CASE(bn, kc)                                                                              \
   if (BN == bn && KC == kc) {                                                                               \
     if (kind == CONV_KIND_CLASS1 || kind == CONV_KIND_CLASS2) {                                             \
@@ -814,13 +1006,15 @@ static int with_conv_kernel(int kind, int BN, int KC, F&& f) {
       if constexpr (halo_keeps_occupancy<bn, kc>()) return f(ConvKernel<bn, kc, halo_mode<bn, kc>()>{});    \
     } else if (kind == CONV_KIND_HALO_PAIR) {                                                               \
       if constexpr (HaloPairCfg<bn, kc>::APPLIES) return f(ConvKernel<bn, kc, CONV_HALO_PAIR>{});           \
-    } else {                                                                                              \
+    } else if (wgs == 2) {                                                                                  \
+      if constexpr (bn == 128) return f(ConvKernel<bn, kc, CONV_WIDE>{});                                   \
+    } else {                                                                                                \
       return f(ConvKernel<bn, kc, CONV_STREAM>{});                                                          \
     }                                                                                                       \
   }
   B200_CONV_CONFIGS(B200_CONV_CASE)
 #undef B200_CONV_CASE
-  set_error("igemm_conv: no kernel for BN=%d KC=%d (kind %d)", BN, KC, kind);
+  set_error("igemm_conv: no kernel for BN=%d KC=%d (kind %d, %d consumer warpgroups)", BN, KC, kind, wgs);
   return E_UNSUPPORTED;
 }
 
@@ -876,9 +1070,14 @@ int conv_route(const ConvOp& op, int num_sms, ConvRoute* r) {
   } else {
     pick_tile(gW, gH, gD, r->tw, r->th, r->td);
   }
-  r->tiles_w = ceil_div(gW, r->tw); r->tiles_h = ceil_div(gH, r->th); r->tiles_d = ceil_div(gD, r->td);
   r->KC = conv_kc(op);
   r->BN = conv_bn(op);
+  r->wgs = pair ? 2 : 1;
+  if (r->kind == CONV_KIND_TAP && conv_wide(op, r->BN, gD, ceil_div(gH, r->th) * ceil_div(gW, r->tw), r->td, num_sms)) {
+    r->td *= 2;
+    r->wgs = 2;
+  }
+  r->tiles_w = ceil_div(gW, r->tw); r->tiles_h = ceil_div(gH, r->th); r->tiles_d = ceil_div(gD, r->td);
   for (int s = 0; s < op.nsrc; ++s) r->kchunks[s] = ceil_div(op.src[s].x.C, r->KC);
   B200_REQUIRE(!halo || r->kchunks[0] == 1, E_UNSUPPORTED, "igemm_conv: halo mode loads one K chunk of source 0 (%d)", r->kchunks[0]);
   r->npass = split ? 3 : 1;
@@ -886,7 +1085,7 @@ int conv_route(const ConvOp& op, int num_sms, ConvRoute* r) {
   r->grid[0] = (int)((long long)out.N * r->tiles_d * r->tiles_h * r->tiles_w);
   r->grid[1] = ceil_div(out.C, r->BN);
   r->grid[2] = 1;
-  return with_conv_kernel(r->kind, r->BN, r->KC, [&](auto k) {
+  return with_conv_kernel(r->kind, r->BN, r->KC, r->wgs, [&](auto k) {
     using Cfg = ConvCfgOf<decltype(k)::BN, decltype(k)::KC, decltype(k)::MODE>;
     r->stages = Cfg::STAGES; r->blocks_per_sm = Cfg::BLOCKS_PER_SM; r->smem_bytes = Cfg::SMEM_BYTES;
     if constexpr (decltype(k)::MODE == CONV_HALO_WS || decltype(k)::MODE == CONV_HALO_PAIR) {
@@ -907,6 +1106,7 @@ int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
   const Act& out = op.out;
   const bool pair = r.kind == CONV_KIND_HALO_PAIR;
   const bool split = r.npass == 3, halo = r.kind == CONV_KIND_HALO || pair, cls = op.cls_mode != 0;
+  const bool wide = r.kind == CONV_KIND_TAP && r.wgs == 2;
   ConvArgs a;
   memset(&a, 0, sizeof(a));
   ConvMaps maps;
@@ -975,10 +1175,11 @@ int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
     maps.o[0] = cmaps.oc[0][0];   // keeps the (unused) plain output descriptor valid
   } else {
     const int cbo = BN < 64 ? BN : 64;
-    B200_TRY(make_act_map(&maps.o[0], out.hi, out.N, out.D, out.H, out.W, out.C, out.ld, cbo, a.tw, a.th, a.td, 1,
+    const int otd = wide ? a.td / 2 : a.td;   // the 256-voxel tile: each warpgroup stores its half
+    B200_TRY(make_act_map(&maps.o[0], out.hi, out.N, out.D, out.H, out.W, out.C, out.ld, cbo, a.tw, a.th, otd, 1,
                           swz_for_bytes(cbo * 2)));
     if (split)
-      B200_TRY(make_act_map(&maps.o[1], out.lo, out.N, out.D, out.H, out.W, out.C, out.ld, cbo, a.tw, a.th, a.td, 1,
+      B200_TRY(make_act_map(&maps.o[1], out.lo, out.N, out.D, out.H, out.W, out.C, out.ld, cbo, a.tw, a.th, otd, 1,
                             swz_for_bytes(cbo * 2)));
   }
   if (op.res) {
@@ -993,7 +1194,7 @@ int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
     a.slope = op.slope; a.bstats = op.bstats;
   }
   const dim3 grid((unsigned)r.grid[0], (unsigned)r.grid[1], (unsigned)r.grid[2]);
-  return with_conv_kernel(r.kind, BN, KC, [&](auto k) {
+  return with_conv_kernel(r.kind, BN, KC, r.wgs, [&](auto k) {
     return launch_cfg<decltype(k)::BN, decltype(k)::KC, decltype(k)::MODE>(maps, a, grid, st, cmaps);
   });
 }

@@ -231,6 +231,7 @@ struct ConvOp {
   const float* bias;   // mode 0: optional per-channel bias
   int zero_last;       // mode 0: output voxels on the high boundary of each axis are forced to 0
   int max_ctas;        // > 0: at most this many CTAs per N tile on the persistent halo kernel (diagnostics: several tiles per CTA)
+  int tile128;         // != 0: per-tap tiles stay at 128 voxels where 256 would be taken (diagnostics: the one-warpgroup reference)
   int cls_mode;        // 2: ConvTranspose3d(kernel = stride = 2) forward: src[0].x = input at half the output extent, src[0].w = the
                        // PACK_T_FWD pack [8][Cop][Cip]; class p = one tap.  1: data gradient of a 3x3x3 stride-2 padding-1 convolution WITHOUT zero insertion: src[0].x = dY (low
                        // resolution), src[0].w = the flipped data-gradient pack, out = dX at twice the extent; eight
@@ -249,6 +250,7 @@ struct ConvRoute {
   int tiles_w, tiles_h, tiles_d;
   int grid[3];
   int stages, blocks_per_sm, smem_bytes;   // ConvCfg of the instantiation
+  int wgs;                  // consumer warpgroups per CTA (2: the 256-voxel per-tap tile and the two-plane halo mode)
 };
 // on a device with num_sms SMs; validates the op: OK or the error launch_igemm_conv would return
 int conv_route(const ConvOp& op, int num_sms, ConvRoute* r);

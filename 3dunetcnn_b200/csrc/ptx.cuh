@@ -130,6 +130,13 @@ __device__ __forceinline__ void tma_load_3d_if(uint32_t issue, void* smem_dst, c
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
+// ----------------------------------------------------------------------------- register reallocation between warpgroups
+// executed by all four warps of a warpgroup: its threads' register limit drops to / rises to N (a multiple of 8, 24..256)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ----------------------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
 // D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 operands from shared memory (descriptors), fp32 accumulator in the registers of
 // the four warps of a warpgroup.  Thread t of the warpgroup (warp w = t / 32, lane l) holds, for every 8-column block i,

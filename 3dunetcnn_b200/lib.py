@@ -38,13 +38,13 @@ class ConvDesc(C.Structure):
 class DiagExt(C.Structure):
     """``b200unet_diag_ext``: bias, zeroed high boundary and visible extents (include/b200unet_diag.h)."""
     _fields_ = [("bias", C.c_void_p), ("zero_last", C.c_int32), ("x_vis", (C.c_int32 * 3) * 2), ("a_vis", C.c_int32 * 3),
-                ("dy_vis", C.c_int32 * 3), ("max_ctas", C.c_int32)]
+                ("dy_vis", C.c_int32 * 3), ("max_ctas", C.c_int32), ("tile128", C.c_int32)]
 
 
 class ConvRoute(C.Structure):
     _fields_ = [("kind", C.c_int32), ("bn", C.c_int32), ("kc", C.c_int32), ("kchunks", C.c_int32 * 2), ("npass", C.c_int32),
                 ("cls_pair", C.c_int32), ("tw", C.c_int32), ("th", C.c_int32), ("td", C.c_int32), ("grid", C.c_int32 * 3),
-                ("stages", C.c_int32), ("blocks_per_sm", C.c_int32), ("smem_bytes", C.c_int32)]
+                ("stages", C.c_int32), ("blocks_per_sm", C.c_int32), ("smem_bytes", C.c_int32), ("wgs", C.c_int32)]
 
 
 class WgradRoute(C.Structure):
@@ -363,11 +363,12 @@ def conv_desc(x: Act, w_hi, w_lo, ksz: int, stride: int, out: Act, cop: int, cip
 
 
 def diag_ext(bias: Optional[torch.Tensor] = None, zero_last: bool = False, x_vis=None, a_vis=None, dy_vis=None,
-             max_ctas: int = 0) -> DiagExt:
+             max_ctas: int = 0, tile128: bool = False) -> DiagExt:
     """``b200unet_diag_ext``; each *_vis is a (d, h, w) triple (x_vis: one per source), 0 = the full extent; max_ctas > 0 caps
-    the CTAs per N tile of the persistent halo kernel"""
+    the CTAs per N tile of the persistent halo kernel; tile128 keeps per-tap launches on 128-voxel tiles"""
     e = DiagExt()
     e.max_ctas = max_ctas
+    e.tile128 = int(bool(tile128))
     e.bias = _p(bias)
     e.zero_last = int(bool(zero_last))
     for s, v in enumerate(x_vis or ()):

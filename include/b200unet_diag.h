@@ -27,6 +27,8 @@ typedef struct b200unet_diag_ext {
   int32_t dy_vis[3];       /* weight gradient and bias gradient: of dy */
   int32_t max_ctas;        /* conv, halo kind on the persistent kernel: > 0 caps its CTAs per N tile (grid[0]), so that small
                               shapes walk several voxel tiles per CTA */
+  int32_t tile128;         /* conv, tap kind: != 0 keeps the 128-voxel tile of one consumer warpgroup where the route would take
+                              the 256-voxel tile of two (same MMA order per output row: the bf16 output is the same bit for bit) */
 } b200unet_diag_ext;
 
 /* kernel kinds of b200unet_conv_route */
@@ -43,9 +45,11 @@ typedef struct b200unet_conv_route {
   int32_t kchunks[2];             /* K chunks of each source */
   int32_t npass;                  /* 1 bf16, 3 split precision */
   int32_t cls_pair;               /* class mode in bf16: the two W-parity classes share one store */
-  int32_t tw, th, td;             /* output voxel tile (class mode: of one parity class) */
+  int32_t tw, th, td;             /* output voxel tile of a CTA (class mode: of one parity class) */
   int32_t grid[3];
   int32_t stages, blocks_per_sm, smem_bytes;   /* of the kernel's compile-time configuration */
+  int32_t wgs;                    /* consumer warpgroups per CTA: 2 for per-tap tiles of 256 voxels (each warpgroup computes the
+                                     half at d0 and d0 + td / 2) and for the two-plane halo kind, 1 otherwise */
 } b200unet_conv_route;
 
 /* kernel kinds of b200unet_wgrad_route */
