@@ -54,23 +54,41 @@ struct ConvTileCfg {
 // Shared memory: STAGES-deep TMA ring | fp32 accumulator tile [128][BN + 4] | (class mode) output staging | (halo mode) halo box
 // | aux.  Outside class mode the output staging tile reuses the ring: the CTA computes one tile, so every stage has been consumed
 // when the epilogue starts.  Class mode keeps the staging tile apart because the producer is already loading the next class.
-// BN <= 32 (<= 204 registers per thread) sizes the ring so that two CTAs share an SM (one CTA's epilogue overlaps the other's
-// MMAs) when that still leaves four stages; otherwise one CTA takes up to 227 KB.
+// BN <= 32 (<= 168 registers per thread, MIN_BLOCKS) sizes the ring so that two CTAs share an SM (one CTA's epilogue overlaps
+// the other's MMAs) when that still leaves four stages; otherwise one CTA takes up to 227 KB.
+//
+// Weight-only ring (W_RING: halo mode with BN = 64, the 64 -> 64 channel layers): a tap stage fills only its weight box, so the
+// ring holds W_STAGES weight boxes, and everything else lives in the halo box region, which nothing reads once the taps have
+// retired (the grid is not persistent).  In turn it holds the halo box; the A tiles of the fused 1x1x1 second source, A tile s
+// beside weight slot s, loaded once every warp's tap MMAs have retired (box_free); then the fp32 accumulator tile and the
+// output staging tile.  (64, 64): 4 x 8,192 + 69,632 + 4,096 + 1,024 = 107,520 B, so two CTAs share an SM and one CTA's
+// epilogue and second-source stall run under the other's MMAs.  (16, 64) and (32, 64) would fit as well, but their halo
+// launches run on the two-plane kernel or stay on per-tap tiles, which already run them two per SM.
 template <int BN, int KC, int MODE>
 struct ConvCfg : ConvTileCfg<BN, KC> {
   using Tile = ConvTileCfg<BN, KC>;
   static constexpr int OUT_STAGING = 2 * 128 * BN * 2;    // hi + lo output tiles (class pairs: 256 rows of hi)
+  static constexpr int ACC_R = (Tile::ACC_BYTES + 1023) / 1024 * 1024;
+  static constexpr int W_STAGES = 4;
+  static constexpr bool W_RING = MODE == CONV_HALO && BN == 64 && W_STAGES * Tile::A_BYTES <= Tile::HALO_BOX_BYTES &&
+                                 ACC_R + OUT_STAGING <= Tile::HALO_BOX_BYTES &&
+                                 W_STAGES * Tile::B_BYTES + Tile::HALO_BOX_BYTES + Tile::AUX_BYTES + 1024 <= Tile::TWO_PER_SM;
+  static constexpr int STAGE_BYTES = W_RING ? Tile::B_BYTES : Tile::STAGE_BYTES;
+  static constexpr int B_OFF = W_RING ? 0 : Tile::A_BYTES;   // weight box within a ring stage
   static constexpr int STG_BYTES = MODE == CONV_CLASS ? OUT_STAGING : 0;
   static constexpr int HALO_BYTES = MODE == CONV_HALO ? Tile::HALO_BOX_BYTES : 0;
-  static constexpr int FIXED = Tile::ACC_BYTES + STG_BYTES + HALO_BYTES + Tile::AUX_BYTES + 1024;   // +1024 alignment slack
-  static constexpr int MIN_BLOCKS = BN <= 32 ? 2 : 1;      // 2 x 160 threads x <= 204 registers fit the 64 K register file
-  static constexpr int STAGES_2 = MIN_BLOCKS == 2 ? (Tile::TWO_PER_SM - FIXED) / Tile::STAGE_BYTES : 0;
-  static constexpr int STAGES_RAW = STAGES_2 >= 4 ? STAGES_2 : (Tile::SMEM_LIMIT - FIXED) / Tile::STAGE_BYTES;
+  static constexpr int FIXED = (W_RING ? 0 : Tile::ACC_BYTES) + STG_BYTES + HALO_BYTES + Tile::AUX_BYTES + 1024;   // +1024 alignment slack
+  // 2 x 160 threads fit the 64 K register file at <= 168 registers per thread (each SM sub-partition's 16 K registers hold
+  // three of the ten warps)
+  static constexpr int MIN_BLOCKS = BN <= 32 || W_RING ? 2 : 1;
+  static constexpr int STAGES_2 = MIN_BLOCKS == 2 ? (Tile::TWO_PER_SM - FIXED) / STAGE_BYTES : 0;
+  static constexpr int STAGES_RAW = W_RING ? W_STAGES : STAGES_2 >= 4 ? STAGES_2 : (Tile::SMEM_LIMIT - FIXED) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
   static constexpr int BLOCKS_PER_SM = STAGES_2 >= 4 ? 2 : 1;
-  static constexpr int PIPE_BYTES = STAGES * Tile::STAGE_BYTES > OUT_STAGING ? STAGES * Tile::STAGE_BYTES : OUT_STAGING;
+  static constexpr int PIPE_BYTES = W_RING || STAGES * STAGE_BYTES > OUT_STAGING ? STAGES * STAGE_BYTES : OUT_STAGING;
   static constexpr int SMEM_BYTES = PIPE_BYTES + FIXED;
   static_assert(STAGES >= 2 && SMEM_BYTES <= Tile::SMEM_LIMIT, "igemm_conv: configuration does not fit shared memory");
+  static_assert(!W_RING || (BLOCKS_PER_SM == 2 && SMEM_BYTES <= Tile::TWO_PER_SM), "igemm_conv: weight-only halo ring");
 };
 
 // Accumulator fragments of the two m64 halves -> s_acc (row-major, ACC_LD floats per row), so that each thread drains one
@@ -124,13 +142,14 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
   // 1024-byte alignment by pointer arithmetic on the __shared__ array: an integer round trip loses the address space and every
   // shared-memory access below would compile to a generic LD.E / ST.E instead of LDS / STS
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  float* s_acc = reinterpret_cast<float*>(smem + Cfg::PIPE_BYTES);
-  uint8_t* stage_out = MODE == CONV_CLASS ? smem + Cfg::PIPE_BYTES + Cfg::ACC_BYTES : smem;
-  uint8_t* halo = smem + Cfg::PIPE_BYTES + Cfg::ACC_BYTES + Cfg::STG_BYTES;
+  uint8_t* halo = smem + Cfg::PIPE_BYTES + (Cfg::W_RING ? 0 : Cfg::ACC_BYTES) + Cfg::STG_BYTES;
+  float* s_acc = reinterpret_cast<float*>(Cfg::W_RING ? halo : smem + Cfg::PIPE_BYTES);
+  uint8_t* stage_out = Cfg::W_RING ? halo + Cfg::ACC_R : MODE == CONV_CLASS ? smem + Cfg::PIPE_BYTES + Cfg::ACC_BYTES : smem;
   uint8_t* aux = halo + Cfg::HALO_BYTES;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
   uint64_t* halo_full = empty_bar + Cfg::STAGES;
+  uint64_t* box_free = halo_full + 1;   // W_RING: every warp's tap MMAs have retired, the box region takes second-source A tiles
   float* s_stats = reinterpret_cast<float*>(aux + 1024);             // [4 warps][BN][2]
   float4* s_coef = reinterpret_cast<float4*>(aux + 1024 + 4 * BN * 8);   // [BN]
 
@@ -150,6 +169,7 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
     tma_prefetch_desc(&maps.b[0][0]);
     for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 4); }
     mbar_init(halo_full, 1);
+    mbar_init(box_free, 4);
     fence_barrier_init();
   }
   pdl_wait();   // before the first global read (the coefficient table below); the barrier set-up above overlaps the previous kernel
@@ -161,9 +181,11 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
   pdl_launch_dependents();
 
   // class mode: ONE CTA computes all eight parity classes of its voxel tile (27 tap products walked class by class, each class
-  // drained by the epilogue before the next one starts).  One CTA per class would spend most of its life in set-up.
+  // drained by the epilogue before the next one starts).  One CTA per class would spend most of its life in set-up.  Only the
+  // class-mode instances compile its code: the others keep those registers.
+  const bool cls_mode = MODE == CONV_CLASS && p.cls_mode != 0;
   int total_iters = (p.ntaps[0] * p.kchunks[0] + p.ntaps[1] * p.kchunks[1]) * p.npass;
-  if (p.cls_mode) {
+  if (cls_mode) {
     total_iters = 0;
     for (int c = 0; c < 8; ++c) total_iters += (int)p.cls_n[c] * p.kchunks[0] * p.npass;
   }
@@ -184,16 +206,17 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
           const int s = it % Cfg::STAGES;
           mbar_wait(&empty_bar[s], ((it / Cfg::STAGES) & 1) ^ 1);
           mbar_expect_tx_if(issue, &full_bar[s], Cfg::B_BOX_BYTES);
-          tma_load_3d_if(issue, smem + s * Cfg::STAGE_BYTES + Cfg::A_BYTES, &maps.b[0][0], &full_bar[s], 0, n0, tap);
+          tma_load_3d_if(issue, smem + s * Cfg::STAGE_BYTES + Cfg::B_OFF, &maps.b[0][0], &full_bar[s], 0, n0, tap);
           ++it;
         }
         continue;
       }
-      for (int cls = 0; cls < (p.cls_mode ? 8 : 1); ++cls) {
-        const int ntap_loop = p.cls_mode ? (int)p.cls_n[cls] : nt;
+      if (Cfg::W_RING) mbar_wait(box_free, 0);   // the second source's A tiles overwrite the halo box
+      for (int cls = 0; cls < (cls_mode ? 8 : 1); ++cls) {
+        const int ntap_loop = cls_mode ? (int)p.cls_n[cls] : nt;
         for (int ti = 0; ti < ntap_loop; ++ti) {
           int tap = ti, cw, ch, cd;
-          if (p.cls_mode) {   // class tap list: source voxel j + delta, packed-weight tap index
+          if (cls_mode) {   // class tap list: source voxel j + delta, packed-weight tap index
             const int e = p.cls_tap[cls][ti];
             tap = e & 31;
             cw = w0 + ((e >> 5) & 1); ch = h0 + ((e >> 6) & 1); cd = d0 + ((e >> 7) & 1);
@@ -207,9 +230,9 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
               const uint32_t ph = (it / Cfg::STAGES) & 1;
               mbar_wait(&empty_bar[s], ph ^ 1);
               mbar_expect_tx_if(issue, &full_bar[s], Cfg::A_BYTES + Cfg::B_BOX_BYTES);
-              uint8_t* sa = smem + s * Cfg::STAGE_BYTES;
+              uint8_t* sa = Cfg::W_RING ? halo + s * Cfg::A_BYTES : smem + s * Cfg::STAGE_BYTES;
               tma_load_5d_if(issue, sa, &maps.a[src][pass == 1], &full_bar[s], kc * KC, cw, ch, cd, n);
-              tma_load_3d_if(issue, sa + Cfg::A_BYTES, &maps.b[src][pass == 2], &full_bar[s], kc * KC, n0, tap);
+              tma_load_3d_if(issue, smem + s * Cfg::STAGE_BYTES + Cfg::B_OFF, &maps.b[src][pass == 2], &full_bar[s], kc * KC, n0, tap);
               ++it;
             }
           }
@@ -235,11 +258,11 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
   constexpr int SROWS_BOX = 128 * CBO * 2;
   // side inputs (residual) are indexed in the OUTPUT tensor: in class mode that is voxel 2j + p of a 2x grid
   auto vox_of = [&](int cls) -> long long {
-    return p.cls_mode
+    return cls_mode
         ? (((long long)n * (2 * p.Do) + 2 * d + ((cls >> 2) & 1)) * (2 * p.Ho) + 2 * h + ((cls >> 1) & 1)) * (2 * p.Wo) + 2 * w + (cls & 1)
         : (((long long)n * p.Do + d) * p.Ho + h) * p.Wo + w;
   };
-  for (int cls = 0; cls < (p.cls_mode ? 8 : 1); ++cls) conv_epilogue_prefetch(p, n0, BN, vox_of(cls), valid);   // -> L2 while the MMAs run
+  for (int cls = 0; cls < (cls_mode ? 8 : 1); ++cls) conv_epilogue_prefetch(p, n0, BN, vox_of(cls), valid);   // -> L2 while the MMAs run
 
   float acc[2][BN / 2];
 #pragma unroll
@@ -249,19 +272,20 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
   const uint32_t halo_lo0 = desc_lo(smem_u32(halo), 16);
   if (MODE == CONV_HALO) mbar_wait(halo_full, 0);
   int it = 0;
-  for (int cls = 0; cls < (p.cls_mode ? 8 : 1); ++cls) {
-    const int n_it = p.cls_mode ? (int)p.cls_n[cls] * p.kchunks[0] * p.npass : total_iters;
+  for (int cls = 0; cls < (cls_mode ? 8 : 1); ++cls) {
+    const int n_it = cls_mode ? (int)p.cls_n[cls] * p.kchunks[0] * p.npass : total_iters;
     int prev = -1;   // ring slot whose MMAs may still be reading it
     for (int i = 0; i < n_it; ++i, ++it) {
       const int s = it % Cfg::STAGES;
       mbar_wait(&full_bar[s], (it / Cfg::STAGES) & 1);
-      uint32_t a_lo = desc_lo(smem0 + s * Cfg::STAGE_BYTES, 16), a_hi = hi_d, a_half = HALF_M;
+      uint32_t a_lo = Cfg::W_RING ? halo_lo0 + ((s * Cfg::A_BYTES) >> 4) : desc_lo(smem0 + s * Cfg::STAGE_BYTES, 16);
+      uint32_t a_hi = hi_d, a_half = HALF_M;
       if (MODE == CONV_HALO && i < 27) {
         a_lo = halo_tap_lo<Cfg::RB>(halo_lo0, i);
         a_hi = hi_halo;
         a_half = (HaloTile::HALF_M * Cfg::RB) >> 4;
       }
-      const uint32_t b_lo = desc_lo(smem0 + s * Cfg::STAGE_BYTES + Cfg::A_BYTES, 16);
+      const uint32_t b_lo = desc_lo(smem0 + s * Cfg::STAGE_BYTES + Cfg::B_OFF, 16);
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < KC / 16; ++k) {
@@ -273,13 +297,18 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
       wgmma_wait<1>();   // the previous stage's MMAs are complete: hand its slot back to the producer
       if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
       prev = s;
+      if (Cfg::W_RING && i == 26 && n_it > 27) {   // the last tap: the second source's A tiles may overwrite the box once it retires
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(box_free);
+      }
     }
     wgmma_wait<0>();
     wgmma_fence_regs(acc[0]);
     wgmma_fence_regs(acc[1]);
     if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+    if (Cfg::W_RING) asm volatile("bar.sync 1, 128;" ::: "memory");   // every warp's MMAs have retired: the box region is free
 
-    const bool pair = p.cls_pair != 0, pair_first = pair && (cls & 1) == 0, pair_second = pair && (cls & 1) == 1;
+    const bool pair = MODE == CONV_CLASS && p.cls_pair != 0, pair_first = pair && (cls & 1) == 0, pair_second = pair && (cls & 1) == 1;
     if (cls > 0) {
       if (!pair_second && threadIdx.x == 0) tma_store_wait_read0();    // the previous stores have read the staging tile
       asm volatile("bar.sync 1, 128;" ::: "memory");                   // and every thread has read its s_acc row
@@ -300,8 +329,8 @@ __global__ void __launch_bounds__(160, (ConvCfg<BN, KC, MODE>::MIN_BLOCKS)) k_ig
       if (pair) {
         tma_store_5d(&cmaps.oc[cls & 6][0], stage_out, n0, 2 * w0, h0, d0, n);
       } else {
-        const CUtensorMap* mo_hi = p.cls_mode ? &cmaps.oc[cls][0] : &maps.o[0];
-        const CUtensorMap* mo_lo = p.cls_mode ? &cmaps.oc[cls][1] : &maps.o[1];
+        const CUtensorMap* mo_hi = cls_mode ? &cmaps.oc[cls][0] : &maps.o[0];
+        const CUtensorMap* mo_lo = cls_mode ? &cmaps.oc[cls][1] : &maps.o[1];
 #pragma unroll
         for (int cb = 0; cb < BN / CBO; ++cb) {
           if (n0 + cb * CBO < p.Cout) {
