@@ -317,6 +317,20 @@ int b200unet_surface_distance(const b200unet_surface_mask* pred, const b200unet_
                                  nsd, scratch, to_stream(stream));
 }
 
+static OverlapOperand to_overlap_operand(const b200unet_overlap_operand* o) {
+  OverlapOperand r;
+  r.data = o->data;
+  r.kind = o->kind;
+  r.dtype = o->dtype;
+  r.thr = o->threshold;
+  return r;
+}
+int b200unet_overlap_counts(const b200unet_overlap_operand* pred, const b200unet_overlap_operand* gt, int b, int c, int d, int h,
+                            int w, int64_t* counts, void* stream) {
+  NOT_NULL(pred); NOT_NULL(gt); NOT_NULL(counts);
+  return launch_overlap_counts(to_overlap_operand(pred), to_overlap_operand(gt), b, c, d, h, w, counts, to_stream(stream));
+}
+
 // ---- diagnostics (include/b200unet_diag.h)
 int b200unet_diag_conv3d_route(const b200unet_conv_desc* desc, const b200unet_diag_ext* ext, b200unet_conv_route* route) {
   NOT_NULL(desc); NOT_NULL(route);

@@ -202,6 +202,23 @@ int launch_surface_distance(const SurfaceMask& pred, const SurfaceMask& gt, int 
                             float q, int hd_dirs, int asd_dirs, const float* tau, float* hd, float* asd, float* nsd, void* scratch,
                             cudaStream_t st);
 
+// ---- overlap counts of segmentations: P, G, I per (item, class) (overlap.cu)
+#define B200_OVERLAP_MAX_CLASSES 128
+#define B200_OVERLAP_MAX_ITEMS 65535   // items per call: the grid's y extent
+// kind and dtype of b200unet_overlap_operand; field order of that struct
+enum OverlapOperandKind { OV_KIND_ONEHOT = 0, OV_KIND_LABEL = 1, OV_KIND_THRESHOLD = 2, OV_KIND_ARGMAX = 3 };
+enum OverlapDtype { OV_DTYPE_U8 = 0, OV_DTYPE_I64 = 1, OV_DTYPE_F32 = 2 };
+// the (kind, dtype) pairs the kernel reads
+enum OverlapForm { OV_ONEHOT_U8 = 0, OV_ONEHOT_F32 = 1, OV_LABEL_U8 = 2, OV_LABEL_I64 = 3, OV_THRESH_F32 = 4, OV_ARGMAX_F32 = 5 };
+struct OverlapOperand {
+  const void* data;
+  int kind, dtype;
+  float thr;
+};
+// counts DEVICE int64 [B][C][3] = (P, G, I), overwritten
+int launch_overlap_counts(const OverlapOperand& pred, const OverlapOperand& gt, int B, int C, int D, int H, int W, int64_t* counts,
+                          cudaStream_t st);
+
 // ---- tensor-core implicit-GEMM convolution (igemm_conv.cu)
 struct ConvSrc {
   Act x;               // A operand (NDHWC bf16, hi[/lo])

@@ -83,6 +83,10 @@ class SurfaceMask(C.Structure):
     _fields_ = [("data", C.c_void_p), ("dtype", C.c_int32), ("stride", C.c_int64 * 5)]
 
 
+class OverlapOperand(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("kind", C.c_int32), ("dtype", C.c_int32), ("threshold", C.c_float)]
+
+
 def build_library(force: bool = False, verbose: bool = False) -> str:
     """Compile libb200unet.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
     if os.environ.get("B200UNET_LIB"):
@@ -173,6 +177,8 @@ _SIGS = {
     "b200unet_surface_scratch_bytes": (C.c_size_t, [C.c_int] * 5),
     "b200unet_surface_distance": (C.c_int, [C.POINTER(SurfaceMask), C.POINTER(SurfaceMask)] + [C.c_int] * 5 + [C.c_void_p, C.c_float,
                                             C.c_int, C.c_int] + [C.c_void_p] * 6),
+    "b200unet_overlap_counts": (C.c_int, [C.POINTER(OverlapOperand), C.POINTER(OverlapOperand)] + [C.c_int] * 5
+                                + [C.c_void_p, C.c_void_p]),
     "b200unet_plan_create": (C.c_int, [C.POINTER(NetDesc), C.POINTER(C.c_void_p)]),
     "b200unet_plan_destroy": (None, [C.c_void_p]),
     "b200unet_plan_num_params": (C.c_int, [C.c_void_p]),
@@ -685,3 +691,17 @@ def surface_distance(pred, gt, spacing, q: float, hd_dirs: int, asd_dirs: int, t
     check(load_library().b200unet_surface_distance(C.byref(pm), C.byref(gm), b, c, d, h, w, spacing.data_ptr(), q, hd_dirs, asd_dirs,
                                                    _p(tau), _p(hd), _p(asd), _p(nsd), scratch.data_ptr(), stream_ptr()),
           "surface_distance")
+
+
+OVERLAP_KINDS = {"onehot": 0, "label": 1, "threshold": 2, "argmax": 3}
+OVERLAP_DTYPES = {torch.bool: 0, torch.uint8: 0, torch.int64: 1, torch.float32: 2}
+
+
+def overlap_counts(pred, pred_kind: str, gt, gt_kind: str, c: int, counts, threshold: float = 0.0) -> None:
+    """pred, gt contiguous [b, c or 1, d, h, w] read as ``pred_kind`` / ``gt_kind`` (OVERLAP_KINDS); counts int64 [b, c, 3]
+    (P, G, I), overwritten"""
+    b, _, d, h, w = pred.shape
+    po = OverlapOperand(pred.data_ptr(), OVERLAP_KINDS[pred_kind], OVERLAP_DTYPES.get(pred.dtype, -1), threshold)
+    go = OverlapOperand(gt.data_ptr(), OVERLAP_KINDS[gt_kind], OVERLAP_DTYPES.get(gt.dtype, -1), 0.0)
+    check(load_library().b200unet_overlap_counts(C.byref(po), C.byref(go), b, c, d, h, w, counts.data_ptr(), stream_ptr()),
+          "overlap_counts")

@@ -22,6 +22,26 @@ Restated semantics:
 Limits: 3-D images only (other spatial ranks raise NotImplementedError), 1..256 voxels per axis and at most 4096 (item, class)
 pairs per call (RuntimeError from the library beyond them).  Euclidean distances only; ``use_subvoxels`` is not implemented.
 Lists of [C, D, H, W] tensors are stacked into one batch (one copy).  No CPU fallback.
+
+Overlap scores, as MONAI computes them (``monai/metrics/meandice.py``, ``meaniou.py`` and ``confusion_matrix.py`` of MONAI 1.3+):
+``DiceHelper`` / ``compute_dice`` / ``DiceMetric``, ``compute_iou`` / ``MeanIoU`` and ``get_confusion_matrix`` /
+``compute_confusion_matrix_metric`` / ``ConfusionMatrixMetric``.  One call of libb200unet counts, for every (item, class) pair,
+P (predicted voxels), G (target voxels) and I (both) in one pass over the inputs, straight from one-hot masks, label maps or
+fp32 logits: no activated, thresholded or one-hot copy of the batch is made.  Each score is a few torch ops on those [B, C]
+counts on the device; nothing is read back to the host.
+
+Restated semantics:
+  * ``sigmoid=True`` thresholds ``sigmoid(x) > 0.5`` as the compare ``x >= SIGMOID_ABOVE_HALF``, the smallest fp32 whose
+    torch.sigmoid on the device is above 0.5 (``x > 0`` differs: the sigmoid of a tiny positive x rounds to 0.5); without
+    ``activate`` the values themselves are compared, ``x > 0.5``.  ``softmax=True`` takes the argmax (ties: the lowest channel, as torch.argmax);
+  * a label outside [0, C) belongs to no class, in either operand; ``include_background=False`` drops channel 0 after counting.
+Deliberate differences from MONAI:
+  * a one-hot operand counts its nonzero voxels, so a soft fp32 target is read as binary, where MONAI sums its values (and a
+    one-channel input counts nonzero voxels where MONAI compares with 1); ConfusionMatrixMetric does not warn about
+    non-binary inputs;
+  * the counts are exact integers, where MONAI's fp32 sums stop being exact above 2^24 voxels per pair.
+Limits: 3-D images only; 1..128 classes and at most 65535 items per call; label maps uint8 or int64, logits fp32, one-hot masks
+bool, uint8 or fp32.  ``GeneralizedDiceScore`` is not provided.
 """
 from __future__ import annotations
 
@@ -34,7 +54,9 @@ from . import lib as _lib
 from .prepost import _need_cuda, _plain
 
 __all__ = ["compute_hausdorff_distance", "compute_average_surface_distance", "compute_surface_dice", "prepare_spacing",
-           "compute_surface_metrics", "do_metric_reduction", "HausdorffDistanceMetric", "SurfaceDistanceMetric", "SurfaceDiceMetric"]
+           "compute_surface_metrics", "do_metric_reduction", "HausdorffDistanceMetric", "SurfaceDistanceMetric", "SurfaceDiceMetric",
+           "SIGMOID_ABOVE_HALF", "DiceHelper", "compute_dice", "DiceMetric", "compute_iou", "MeanIoU", "get_confusion_matrix",
+           "check_confusion_matrix_metric_name", "compute_confusion_matrix_metric", "ConfusionMatrixMetric"]
 
 _REDUCTIONS = ("none", "mean", "sum", "mean_batch", "sum_batch", "mean_channel", "sum_channel")
 
@@ -288,3 +310,266 @@ class SurfaceDiceMetric(_CumulativeSurfaceMetric):
 
     def _compute(self, y_pred, y, spacing):
         return compute_surface_dice(y_pred, y, self.class_thresholds, self.include_background, self.distance_metric, spacing)
+
+
+# ---------------------------------------------------------------------------------------------------------- overlap scores
+# The smallest fp32 x whose torch.sigmoid(x) on a CUDA tensor is above 0.5 (8.262958e-08).  Below it the device's expf(-x) returns
+# 1.0, 1 + exp(-x) is 2 and the sigmoid exactly 0.5.  torch's CPU sigmoid crosses 0.5 higher, at 0x33C00001 (8.940697e-08): its exp
+# returns 1 - 2^-24 in between, and 1 + (1 - 2^-24) rounds to 2.  The metrics run on CUDA tensors, so the device's value is taken.
+SIGMOID_ABOVE_HALF = float(np.uint32(0x33B17218).view(np.float32))
+_ABOVE_HALF = float(np.nextafter(np.float32(0.5), np.float32(1.0)))     # x > 0.5 on values that are already probabilities
+_ONEHOT_DTYPES = (torch.bool, torch.uint8, torch.float32)
+_LABEL_DTYPES = (torch.bool, torch.uint8, torch.int64)
+
+
+def _overlap_counts(y_pred, y, n: int, pred_kind: str, threshold: float = 0.0):
+    """(P, G, I), int64 [B, n] each, from one pass.  y_pred is read as ``pred_kind``; y [B, 1] with n > 1 is a label map, else
+    a one-hot [B, n]."""
+    y_pred, y = _as_batch(y_pred, "y_pred"), _as_batch(y, "y")
+    if y_pred.dim() < 3:
+        raise ValueError(f"y_pred should have at least 3 dimensions (batch, channel, spatial), got {y_pred.dim()}.")
+    if y_pred.dim() != 5 or y.dim() != 5:
+        raise NotImplementedError("overlap metrics are implemented for 3-D images [B, C, D, H, W] only (got %d and %d spatial dims)"
+                                  % (y_pred.dim() - 2, y.dim() - 2))
+    if y_pred.shape[0] != y.shape[0] or y_pred.shape[2:] != y.shape[2:]:
+        raise ValueError(f"y_pred and y should have the same batch and spatial shape, got {tuple(y_pred.shape)} and {tuple(y.shape)}.")
+    gt_kind = "label" if y.shape[1] == 1 and n > 1 else "onehot"
+    if not 1 <= n <= 128:
+        raise ValueError("%d classes; 1..128 are supported" % n)
+    for name, t, kind in (("y_pred", y_pred, pred_kind), ("y", y, gt_kind)):
+        want = 1 if kind == "label" else n
+        if t.shape[1] != want:
+            raise ValueError("%s: %d channels; %s input of %d classes has %d" % (name, t.shape[1], kind, n, want))
+        dtypes = {"onehot": _ONEHOT_DTYPES, "label": _LABEL_DTYPES}.get(kind, (torch.float32,))
+        if t.dtype not in dtypes:
+            raise TypeError("%s: dtype %s; a %s input is %s" % (name, t.dtype, kind, " or ".join(str(d) for d in dtypes)))
+    _need_cuda(y_pred, "overlap metrics")
+    _need_cuda(y, "overlap metrics")
+    if y_pred.device != y.device:
+        raise ValueError("y_pred and y are on different devices (%s, %s)" % (y_pred.device, y.device))
+    counts = torch.empty((y_pred.shape[0], n, 3), dtype=torch.int64, device=y_pred.device)
+    with torch.cuda.device(y_pred.device):
+        _lib.overlap_counts(y_pred.contiguous(), pred_kind, y.contiguous(), gt_kind, n, counts, threshold)
+    return counts.unbind(-1)
+
+
+def _overlap_score(num: torch.Tensor, den: torch.Tensor, G: torch.Tensor, P: torch.Tensor, ignore_empty: bool) -> torch.Tensor:
+    """num / den in fp32 where the target is not empty; otherwise nan (ignore_empty), 1 when both masks are empty, else 0"""
+    if ignore_empty:
+        empty = torch.full_like(num, float("nan"), dtype=torch.float32)
+    else:
+        empty = ((G + P) == 0).float()
+    return torch.where(G > 0, num.float() / den.float(), empty)
+
+
+def _drop_background(counts, include_background: bool):
+    return counts if include_background or counts[0].shape[1] == 1 else tuple(t[:, 1:] for t in counts)
+
+
+class DiceHelper:
+    """MONAI ``DiceHelper``: which input form each flag selects, then the Dice of every (item, class) pair and the reduction.
+    ``sigmoid`` thresholds at 0.5 (applying the sigmoid only with ``activate``), ``softmax`` takes the argmax over the channels; a
+    one-channel ``y_pred`` with ``num_classes > 1`` is a label map.  Returns (f, not_nans) with ``get_not_nans``."""
+
+    def __init__(self, include_background: Optional[bool] = None, sigmoid: bool = False, softmax: Optional[bool] = None,
+                 activate: bool = False, get_not_nans: bool = True, reduction: str = "mean_batch", ignore_empty: bool = True,
+                 num_classes: Optional[int] = None):
+        self.sigmoid = sigmoid
+        self.reduction = reduction
+        self.get_not_nans = get_not_nans
+        self.include_background = sigmoid if include_background is None else include_background
+        self.softmax = not sigmoid if softmax is None else softmax
+        self.activate = activate
+        self.ignore_empty = ignore_empty
+        self.num_classes = num_classes
+
+    def counts(self, y_pred, y):
+        """(P, G, I) int64 [B, C'] of the classes scored"""
+        y_pred = _as_batch(y_pred, "y_pred")
+        if y_pred.dim() < 3:
+            raise ValueError(f"y_pred should have at least 3 dimensions (batch, channel, spatial), got {y_pred.dim()}.")
+        argmax, threshold = self.softmax, self.sigmoid
+        n = y_pred.shape[1] if self.num_classes is None else self.num_classes
+        if self.num_classes is not None and y_pred.shape[1] == 1 and n > 1:
+            argmax = threshold = False
+        kind, thr = ("label" if y_pred.shape[1] == 1 and n > 1 else "onehot"), 0.0
+        if argmax and n > 1:
+            kind = "argmax"
+        elif threshold and y_pred.dtype == torch.float32:
+            kind, thr = "threshold", SIGMOID_ABOVE_HALF if self.activate else _ABOVE_HALF
+        # a bool / uint8 y_pred is above 0.5, or has a sigmoid above 0.5, exactly where it is nonzero: the one-hot reading
+        return _drop_background(_overlap_counts(y_pred, y, n, kind, thr), self.include_background)
+
+    def __call__(self, y_pred, y):
+        P, G, I = self.counts(y_pred, y)
+        f, not_nans = do_metric_reduction(_overlap_score(2 * I, G + P, G, P, self.ignore_empty), self.reduction)
+        return (f, not_nans) if self.get_not_nans else f
+
+
+def compute_dice(y_pred, y, include_background: bool = True, ignore_empty: bool = True, num_classes: Optional[int] = None):
+    """MONAI ``compute_dice``: fp32 [B, C'].  ``y_pred`` one-hot [B, C] (nonzero = class) or a label map [B, 1] with
+    ``num_classes``; ``y`` one-hot or a label map."""
+    return DiceHelper(include_background=include_background, reduction="none", get_not_nans=False, softmax=False,
+                      ignore_empty=ignore_empty, num_classes=num_classes)(y_pred, y)
+
+
+class _CumulativeOverlapMetric(_CumulativeSurfaceMetric):
+    """The cumulative base without the surface metrics' spacing argument"""
+
+    def __call__(self, y_pred, y):
+        return super().__call__(y_pred, y)
+
+
+class DiceMetric(_CumulativeOverlapMetric):
+    """MONAI ``DiceMetric`` on the device.  ``return_with_label``: True or a list of names turns the aggregate into a dict of
+    rounded floats per class (read back to the host, as MONAI does)."""
+
+    def __init__(self, include_background: bool = True, reduction: str = "mean", get_not_nans: bool = False, ignore_empty: bool = True,
+                 num_classes: Optional[int] = None, return_with_label=False):
+        super().__init__(reduction, get_not_nans)
+        self.include_background, self.ignore_empty, self.num_classes = include_background, ignore_empty, num_classes
+        self.return_with_label = return_with_label
+
+    def _compute(self, y_pred, y, spacing):
+        return compute_dice(y_pred, y, self.include_background, self.ignore_empty, self.num_classes)
+
+    def aggregate(self, reduction: Optional[str] = None):
+        data = self.get_buffer()
+        if not isinstance(data, torch.Tensor):
+            raise ValueError("the data to aggregate must be PyTorch Tensor.")
+        f, not_nans = do_metric_reduction(data, reduction or self.reduction)
+        if self.return_with_label:
+            if isinstance(self.return_with_label, bool):
+                first = 0 if self.include_background else 1
+                f = {f"label_{i + first}": round(v.item(), 4) for i, v in enumerate(f)}
+            else:
+                f = {key: round(v.item(), 4) for key, v in zip(self.return_with_label, f)}
+        return (f, not_nans) if self.get_not_nans else f
+
+
+def _same_shape_counts(y_pred, y, include_background: bool):
+    y_pred, y = _as_batch(y_pred, "y_pred"), _as_batch(y, "y")
+    if y.shape != y_pred.shape:
+        raise ValueError(f"y_pred and y should have same shapes, got {y_pred.shape} and {y.shape}.")
+    if y_pred.dim() < 3:
+        raise ValueError(f"y_pred should have at least 3 dimensions (batch, channel, spatial), got {y_pred.dim()}.")
+    return _drop_background(_overlap_counts(y_pred, y, y_pred.shape[1], "onehot"), include_background), y_pred.shape[2:].numel()
+
+
+def compute_iou(y_pred, y, include_background: bool = True, ignore_empty: bool = True) -> torch.Tensor:
+    """MONAI ``compute_iou``: fp32 [B, C'] of one-hot inputs of the same shape (nonzero = class)."""
+    (P, G, I), _ = _same_shape_counts(y_pred, y, include_background)
+    return _overlap_score(I, G + P - I, G, P, ignore_empty)
+
+
+class MeanIoU(_CumulativeOverlapMetric):
+    """MONAI ``MeanIoU`` on the device."""
+
+    def __init__(self, include_background: bool = True, reduction: str = "mean", get_not_nans: bool = False, ignore_empty: bool = True):
+        super().__init__(reduction, get_not_nans)
+        self.include_background, self.ignore_empty = include_background, ignore_empty
+
+    def _compute(self, y_pred, y, spacing):
+        return compute_iou(y_pred, y, self.include_background, self.ignore_empty)
+
+
+def get_confusion_matrix(y_pred, y, include_background: bool = True) -> torch.Tensor:
+    """MONAI ``get_confusion_matrix``: fp32 [B, C', 4] = (tp, fp, tn, fn) of one-hot inputs of the same shape, each the exact
+    count rounded once to fp32."""
+    (P, G, I), S = _same_shape_counts(y_pred, y, include_background)
+    return torch.stack([I, P - I, S - P - G + I, G - I], dim=-1).float()
+
+
+_CM_NAMES = {
+    "tpr": ("sensitivity", "recall", "hit_rate", "true_positive_rate", "tpr"),
+    "tnr": ("specificity", "selectivity", "true_negative_rate", "tnr"),
+    "ppv": ("precision", "positive_predictive_value", "ppv"),
+    "npv": ("negative_predictive_value", "npv"),
+    "fnr": ("miss_rate", "false_negative_rate", "fnr"),
+    "fpr": ("fall_out", "false_positive_rate", "fpr"),
+    "fdr": ("false_discovery_rate", "fdr"),
+    "for": ("false_omission_rate", "for"),
+    "pt": ("prevalence_threshold", "pt"),
+    "ts": ("threat_score", "critical_success_index", "ts", "csi"),
+    "acc": ("accuracy", "acc"),
+    "ba": ("balanced_accuracy", "ba"),
+    "f1": ("f1_score", "f1"),
+    "mcc": ("matthews_correlation_coefficient", "mcc"),
+    "fm": ("fowlkes_mallows_index", "fm"),
+    "bm": ("informedness", "bookmaker_informedness", "bm", "youden_index", "youden"),
+    "mk": ("markedness", "deltap", "mk"),
+}
+
+
+def check_confusion_matrix_metric_name(metric_name: str) -> str:
+    """MONAI's names and aliases -> the short name; spaces count as underscores, case is ignored"""
+    name = metric_name.replace(" ", "_").lower()
+    for short, aliases in _CM_NAMES.items():
+        if name in aliases:
+            return short
+    raise NotImplementedError("the metric is not implemented.")
+
+
+def compute_confusion_matrix_metric(metric_name: str, confusion_matrix: torch.Tensor) -> torch.Tensor:
+    """MONAI ``compute_confusion_matrix_metric`` on [..., 4] (tp, fp, tn, fn): nan where a denominator is 0."""
+    metric = check_confusion_matrix_metric_name(metric_name)
+    if confusion_matrix.dim() == 1:
+        confusion_matrix = confusion_matrix.unsqueeze(dim=0)
+    if confusion_matrix.shape[-1] != 4:
+        raise ValueError("the size of the last dimension of confusion_matrix should be 4.")
+    tp, fp, tn, fn = confusion_matrix.unbind(-1)
+    p, n = tp + fn, fp + tn
+    nan = torch.tensor(float("nan"), device=confusion_matrix.device)
+
+    def ratio(a, b):
+        return torch.where(b > 0, a / b, nan)
+
+    if metric in ("pt", "ba", "bm"):
+        tpr, tnr = ratio(tp, p), ratio(tn, n)
+        if metric == "pt":
+            num, den = torch.sqrt(tpr * (1.0 - tnr)) + tnr - 1.0, tpr + tnr - 1.0
+        else:
+            return (tpr + tnr) / 2.0 if metric == "ba" else tpr + tnr - 1.0
+    elif metric == "fm":
+        return torch.sqrt(ratio(tp, tp + fp) * ratio(tp, p))
+    elif metric == "mk":
+        return ratio(tp, tp + fp) + ratio(tn, tn + fn) - 1.0
+    elif metric == "mcc":
+        num, den = tp * tn - fp * fn, torch.sqrt((tp + fp) * (tp + fn) * (tn + fp) * (tn + fn))
+    else:
+        num, den = {"tpr": (tp, p), "tnr": (tn, n), "ppv": (tp, tp + fp), "npv": (tn, tn + fn), "fnr": (fn, p), "fpr": (fp, n),
+                    "fdr": (fp, fp + tp), "for": (fn, fn + tn), "ts": (tp, tp + fn + fp), "acc": (tp + tn, p + n),
+                    "f1": (tp * 2.0, tp * 2.0 + fn + fp)}[metric]
+    return torch.where(den != 0, num / den, nan)
+
+
+class ConfusionMatrixMetric(_CumulativeOverlapMetric):
+    """MONAI ``ConfusionMatrixMetric`` on the device.  The buffer holds [B, C', 4] matrices; ``aggregate`` returns one result per
+    name: with ``compute_sample`` the metric of each sample, then the reduction; otherwise the reduction of the matrices, then the
+    metric."""
+
+    def __init__(self, include_background: bool = True, metric_name="hit_rate", compute_sample: bool = False, reduction: str = "mean",
+                 get_not_nans: bool = False):
+        super().__init__(reduction, get_not_nans)
+        self.include_background = include_background
+        self.metric_name = (metric_name,) if isinstance(metric_name, str) else tuple(metric_name)
+        for name in self.metric_name:
+            check_confusion_matrix_metric_name(name)
+        self.compute_sample = compute_sample
+
+    def _compute(self, y_pred, y, spacing):
+        return get_confusion_matrix(y_pred, y, self.include_background)
+
+    def aggregate(self, compute_sample: bool = False, reduction: Optional[str] = None):
+        data = self.get_buffer()
+        if not isinstance(data, torch.Tensor):
+            raise ValueError("the data to aggregate must be PyTorch Tensor.")
+        results = []
+        for name in self.metric_name:
+            if compute_sample or self.compute_sample:
+                f, not_nans = do_metric_reduction(compute_confusion_matrix_metric(name, data), reduction or self.reduction)
+            else:
+                f, not_nans = do_metric_reduction(data, reduction or self.reduction)
+                f = compute_confusion_matrix_metric(name, f)
+            results.append((f, not_nans) if self.get_not_nans else f)
+        return results

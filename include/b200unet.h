@@ -305,6 +305,26 @@ int b200unet_surface_distance(const b200unet_surface_mask* pred, const b200unet_
                               const double* spacing, float q, int hd_dirs, int asd_dirs, const float* tau, float* hd, float* asd,
                               float* nsd, void* scratch, void* stream);
 
+/* ---- overlap counts of segmentations (the scoring after the path: MONAI DiceMetric, MeanIoU, ConfusionMatrixMetric), in one
+ * pass over the batch.  For every (item, class) pair, counts[b][cls] = (P, G, I): voxels predicted as cls, voxels whose target is
+ * cls, voxels that are both.  For binary masks tp = I, fp = P - I, fn = G - I and tn = d*h*w - P - G + I.  An operand is read as:
+ *   kind 0 one-hot     [b][c][d][h][w], dtype 0 (bool / uint8) or 2 (fp32): class cls iff the value is nonzero;
+ *   kind 1 label map   [b][1][d][h][w], dtype 0 (uint8) or 1 (int64): the class is the value; a value outside [0, c) is no class;
+ *   kind 2 threshold   [b][c][d][h][w], dtype 2: class cls iff the value is >= threshold (prediction only);
+ *   kind 3 argmax      [b][c][d][h][w], dtype 2: the class is the first channel of the largest value, NaN counting as the
+ *                      largest, as torch.argmax (prediction only).
+ * Operands are contiguous.  1 <= c <= 128, 1 <= b <= 65535, d*h*w < 2^31, else B200UNET_E_UNSUPPORTED; another kind / dtype pair:
+ * B200UNET_E_UNSUPPORTED.  counts: DEVICE int64 [b][c][3], overwritten; exact integers, bit-identical run to run.  Nothing is
+ * read back to the host: the call can be captured in a CUDA graph. */
+typedef struct b200unet_overlap_operand {
+  const void* data;
+  int32_t kind;         /* 0 one-hot, 1 label map, 2 threshold, 3 argmax */
+  int32_t dtype;        /* 0 bool / uint8, 1 int64, 2 fp32 */
+  float threshold;      /* kind 2 */
+} b200unet_overlap_operand;
+int b200unet_overlap_counts(const b200unet_overlap_operand* pred, const b200unet_overlap_operand* gt, int b, int c, int d, int h,
+                            int w, int64_t* counts, void* stream);
+
 /* ---- whole-network plan: UNet3D forward/backward (segmentation/unet.py:7-50, classification/myronenko.py,
  * classification/decoder.py:73-130, autoencoder/variational.py:37-87) as one schedule of the kernels above. */
 typedef struct b200unet_net_desc {
