@@ -160,6 +160,34 @@ int b200unet_act_bwd(const b200unet_tensor* g1, const b200unet_tensor* g2, const
   return launch_act_bwd(to_act(g1), g2 ? &a2 : nullptr, to_act(c), coef, slope, to_act(dz), bstats, bstats_ld, to_stream(stream));
 }
 
+int b200unet_prelu_apply(const b200unet_tensor* x, const b200unet_tensor* y, const double* stats, const float* gamma,
+                         const float* beta, int c, int groups, float eps, const float* slope, const b200unet_tensor* add, float* coef,
+                         void* stream) {
+  NOT_NULL(x); NOT_NULL(y); NOT_NULL(stats); NOT_NULL(coef); NOT_NULL(slope);
+  Act a;
+  if (add) a = to_act(add);
+  return launch_gn_apply(to_act(x), to_act(y), stats, gamma, beta, c, groups, (long long)x->d * x->h * x->w, eps, coef, 0.f,
+                         to_stream(stream), slope, add ? &a : nullptr);
+}
+size_t b200unet_prelu_bwd_scratch_bytes(const b200unet_tensor* c) { return c ? act_bwd_slope_scratch_bytes(to_act(c)) : 0; }
+int b200unet_prelu_bwd(const b200unet_tensor* g1, const b200unet_tensor* g2, const b200unet_tensor* c, const float* coef,
+                       const float* slope, const b200unet_tensor* dz, double* bstats, int bstats_ld, const b200unet_tensor* gsum,
+                       float* dslope, float* scratch, void* stream) {
+  NOT_NULL(g1); NOT_NULL(c); NOT_NULL(coef); NOT_NULL(slope); NOT_NULL(dz); NOT_NULL(bstats); NOT_NULL(dslope); NOT_NULL(scratch);
+  Act a2, gs;
+  if (g2) a2 = to_act(g2);
+  if (gsum) gs = to_act(gsum);
+  return launch_act_bwd(to_act(g1), g2 ? &a2 : nullptr, to_act(c), coef, 0.f, to_act(dz), bstats, bstats_ld, to_stream(stream), slope,
+                        dslope, scratch, gsum ? &gs : nullptr);
+}
+int b200unet_logits_unpack(const b200unet_tensor* in, const b200unet_tensor* add, const float* bias, int c_real, float* logits,
+                           void* stream) {
+  NOT_NULL(in); NOT_NULL(logits);
+  Act a;
+  if (add) a = to_act(add);
+  return launch_logits_unpack(to_act(in), add ? &a : nullptr, bias, c_real, logits, to_stream(stream));
+}
+
 int b200unet_upsample2x_fwd(const b200unet_tensor* x, const b200unet_tensor* y, double* stats, int stats_ld,
                             void* stream) {
   NOT_NULL(x); NOT_NULL(y);

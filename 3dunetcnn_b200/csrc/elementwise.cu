@@ -87,9 +87,14 @@ int launch_input_pack(const float* x, int C, const Act& out, double* stats, int 
 struct GnFin {
   const double* stats; const float* gamma; const float* beta; int C; int G; double S; float eps; float4* coef_out;
 };
-__global__ void __launch_bounds__(256) k_gn_apply(Act x, Act y, float slope, GnFin f) {
+// EXT (MONAI UNet's Convolution / ResidualUnit): the slope is read from slope_dev (a learnable PReLU parameter, so a captured
+// CUDA graph sees each optimizer step's value) when it is set, and y = act(z) + add when add.hi is set (the residual unit's
+// `conv(x) + residual(x)` after the activation, the addend read as hi + lo).  EXT = false is the plain launch.
+template <bool EXT>
+__global__ void __launch_bounds__(256) k_gn_apply(Act x, Act y, float slope, GnFin f, const float* __restrict__ slope_dev, Act add) {
   pdl_wait();                 // launched through launch_pdl: the producer of x / of the statistics has completed past this line
   pdl_launch_dependents();
+  if (EXT && slope_dev) slope = *slope_dev;
   const int c8n = x.C / 8;
   const int n = blockIdx.y;
   const long long S = (long long)x.D * x.H * x.W;
@@ -139,6 +144,13 @@ __global__ void __launch_bounds__(256) k_gn_apply(Act x, Act y, float slope, GnF
       v0[j] = z0 > 0.f ? z0 : z0 * slope;
       v1[j] = z1 > 0.f ? z1 : z1 * slope;
     }
+    if (EXT && add.hi) {
+      float a0[8], a1[8];
+      load8(add.hi, add.lo, (base + s) * add.ld + c8 * 8, a0);
+      load8(add.hi, add.lo, (base + s + stride) * add.ld + c8 * 8, a1);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) { v0[j] += a0[j]; v1[j] += a1[j]; }
+    }
     store8(y.hi, y.lo, (base + s) * y.ld + c8 * 8, v0);
     store8(y.hi, y.lo, (base + s + stride) * y.ld + c8 * 8, v1);
   }
@@ -149,6 +161,12 @@ __global__ void __launch_bounds__(256) k_gn_apply(Act x, Act y, float slope, GnF
     for (int j = 0; j < 8; ++j) {
       const float z0 = fmaf(ka[j], v0[j], kb[j]);
       v0[j] = z0 > 0.f ? z0 : z0 * slope;
+    }
+    if (EXT && add.hi) {
+      float a0[8];
+      load8(add.hi, add.lo, (base + s) * add.ld + c8 * 8, a0);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v0[j] += a0[j];
     }
     store8(y.hi, y.lo, (base + s) * y.ld + c8 * 8, v0);
   }
@@ -182,8 +200,10 @@ static void gn_launch_dims(const Act& x, dim3& grid, dim3& block) {
 
 // statistics -> coefficients -> y = act(A x + B) in one launch; coef [N][x.C] float4 is written for the backward pass
 int launch_gn_apply(const Act& x, const Act& y, const double* stats, const float* gamma, const float* beta, int C, int G,
-                    long long S, float eps, float* coef, float slope, cudaStream_t st) {
+                    long long S, float eps, float* coef, float slope, cudaStream_t st, const float* slope_dev, const Act* add) {
   B200_REQUIRE(x.C % 8 == 0 && y.C == x.C, E_INVALID, "gn_apply: C=%d/%d", x.C, y.C);
+  B200_REQUIRE(!add || (add->C == x.C && add->N == x.N && add->D == x.D && add->H == x.H && add->W == x.W), E_INVALID,
+               "gn_apply: addend shape mismatch");
   B200_REQUIRE(G > 0 && C % G == 0 && C <= x.C, E_INVALID, "gn_apply: C=%d G=%d", C, G);
   B200_REQUIRE(x.C <= 1024, E_UNSUPPORTED, "gn_apply: C <= 1024 supported (got %d)", x.C);
   GnFin f;
@@ -191,7 +211,9 @@ int launch_gn_apply(const Act& x, const Act& y, const double* stats, const float
   f.coef_out = reinterpret_cast<float4*>(coef);
   dim3 grid, block;
   gn_launch_dims(x, grid, block);
-  launch_pdl(k_gn_apply, grid, block, 0, st, x, y, slope, f);
+  const Act none = make_act(nullptr, nullptr, 0, 0, 0, 0, 0, 0);
+  if (slope_dev || add) launch_pdl(k_gn_apply<true>, grid, block, 0, st, x, y, slope, f, slope_dev, add ? *add : none);
+  else launch_pdl(k_gn_apply<false>, grid, block, 0, st, x, y, slope, f, (const float*)nullptr, none);
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;
 }
@@ -359,14 +381,24 @@ int launch_gn_bwd(const Act& dz, const Act& x, const float* coef, const double* 
   return OK;
 }
 
+__global__ void __launch_bounds__(128) k_sum_slots(const float* __restrict__ part, int slots, int n, float* __restrict__ out);
+
 // ------------------------------------------------------------------------------------------------ activation backward (+ statistics)
 // Post-activation blocks (conv -> norm -> act: MONAI UnetBasicBlock, the model examples/brats2020/brats2020_config.json
 // trains): the gradient arriving at a block output is that of the ACTIVATED tensor a = act(A c + B), c = the
 // convolution output.   dz = (g1 [+ g2]) * act'(A c + B);   bstats[n][ch] += (sum dz, sum dz * xhat),  xhat = (c - mu) rstd
 // which is exactly what the GroupNorm backward (k_gn_bwd) consumes.  Same thread <-> channel-chunk mapping as k_gn_apply.
+// EXT (PReLU, MONAI UNet): the slope is read from slope_dev when it is set; dslope_part[n][blockIdx.x] = the block's sum of
+// z * g over z <= 0 (dL/da of the PReLU slope a, g = g1 + g2), reduced in a fixed order (warp shuffles, then the warps in turn)
+// so that launch_act_bwd's fixed-order slot sum repeats it bit for bit; gsum.hi set: gsum = g1 + g2 (the output gradient a
+// residual branch takes as well).
+template <bool EXT>
 __global__ void __launch_bounds__(256) k_act_bwd(Act g1, Act g2, Act c, const float4* __restrict__ coef, float slope, Act dz,
-                                                 double* __restrict__ bstats, int bstats_ld) {
+                                                 double* __restrict__ bstats, int bstats_ld, const float* __restrict__ slope_dev,
+                                                 float* __restrict__ dslope_part, Act gsum) {
   extern __shared__ double smb[];   // [C][2]
+  if (EXT && slope_dev) slope = *slope_dev;
+  float sa = 0.f;
   for (int i = threadIdx.x; i < c.C * 2; i += blockDim.x) smb[i] = 0.0;
   __syncthreads();
   const int c8n = c.C / 8;
@@ -392,9 +424,11 @@ __global__ void __launch_bounds__(256) k_act_bwd(Act g1, Act g2, Act c, const fl
 #pragma unroll
       for (int j = 0; j < 8; ++j) g[j] += h[j];
     }
+    if (EXT && gsum.hi) store8(gsum.hi, gsum.lo, (base + s) * gsum.ld + c8 * 8, g);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const float z = fmaf(ka[j], x[j], kb[j]);
+      if (EXT && z < 0.f) sa = fmaf(z, g[j], sa);
       const float d = z > 0.f ? g[j] : g[j] * slope;
       g[j] = d;
       s1[j] += d;
@@ -409,23 +443,65 @@ __global__ void __launch_bounds__(256) k_act_bwd(Act g1, Act g2, Act c, const fl
   }
   __syncthreads();
   for (int i = threadIdx.x; i < c.C * 2; i += blockDim.x) atomicAdd(&bstats[(long long)n * bstats_ld * 2 + i], smb[i]);
+  if (EXT && dslope_part) {
+    // fixed order over blockDim threads, which need not be a multiple of 32 (ew_threads_for: 252 threads at C = 72): lane l
+    // of warp 0 adds the threads l, l + 32, ..., then lane 0 adds the 32 lanes
+    __shared__ float s_sa[256];
+    s_sa[threadIdx.x] = sa;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+      float t = 0.f;
+      for (int i = threadIdx.x; i < (int)blockDim.x; i += 32) t += s_sa[i];
+      s_sa[threadIdx.x] = t;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float t = 0.f;
+      for (int i = 0; i < 32 && i < (int)blockDim.x; ++i) t += s_sa[i];
+      dslope_part[(long long)n * gridDim.x + blockIdx.x] = t;
+    }
+  }
 }
 
-int launch_act_bwd(const Act& g1, const Act* g2, const Act& c, const float* coef, float slope, const Act& dz, double* bstats,
-                   int bstats_ld, cudaStream_t st) {
-  B200_REQUIRE(c.C % 8 == 0 && g1.C == c.C && dz.C == c.C && (!g2 || g2->C == c.C), E_INVALID, "act_bwd: channel mismatch");
-  B200_REQUIRE(coef && bstats, E_INVALID, "act_bwd: null argument");
+// grid of k_act_bwd: (blocks, N)
+static int act_bwd_blocks(const Act& c, int threads) {
   const int c8n = c.C / 8;
-  const int threads = ew_threads_for(c8n);
-  B200_REQUIRE(threads <= 256, E_UNSUPPORTED, "act_bwd: C=%d unsupported", c.C);
   const long long S = (long long)c.D * c.H * c.W;
   const int vper = threads / c8n;
   long long want = (S + vper - 1) / vper;
   const long long cap = (132LL * 4 + c.N - 1) / c.N;
-  const int blocks = (int)(want < cap ? (want > 0 ? want : 1) : cap);
+  return (int)(want < cap ? (want > 0 ? want : 1) : cap);
+}
+
+size_t act_bwd_slope_scratch_bytes(const Act& c) {
+  return (size_t)act_bwd_blocks(c, ew_threads_for(c.C / 8)) * c.N * sizeof(float);
+}
+
+int launch_act_bwd(const Act& g1, const Act* g2, const Act& c, const float* coef, float slope, const Act& dz, double* bstats,
+                   int bstats_ld, cudaStream_t st, const float* slope_dev, float* dslope, float* scratch, const Act* gsum) {
+  B200_REQUIRE(c.C % 8 == 0 && g1.C == c.C && dz.C == c.C && (!g2 || g2->C == c.C), E_INVALID, "act_bwd: channel mismatch");
+  B200_REQUIRE(coef && bstats, E_INVALID, "act_bwd: null argument");
+  B200_REQUIRE(!dslope || scratch, E_INVALID, "act_bwd: the slope gradient needs act_bwd_slope_scratch_bytes() of scratch");
+  B200_REQUIRE(!gsum || gsum->C == c.C, E_INVALID, "act_bwd: gsum channel mismatch");
+  const int c8n = c.C / 8;
+  const int threads = ew_threads_for(c8n);
+  B200_REQUIRE(threads <= 256, E_UNSUPPORTED, "act_bwd: C=%d unsupported", c.C);
+  const int blocks = act_bwd_blocks(c, threads);
   Act none = make_act(nullptr, nullptr, 0, 0, 0, 0, 0, 0);
-  k_act_bwd<<<dim3(blocks, c.N), threads, c.C * 2 * sizeof(double), st>>>(g1, g2 ? *g2 : none, c, reinterpret_cast<const float4*>(coef),
-                                                                          slope, dz, bstats, bstats_ld);
+  const size_t smem = c.C * 2 * sizeof(double);
+  if (slope_dev || dslope || gsum) {
+    k_act_bwd<true><<<dim3(blocks, c.N), threads, smem, st>>>(g1, g2 ? *g2 : none, c, reinterpret_cast<const float4*>(coef), slope, dz,
+                                                              bstats, bstats_ld, slope_dev, dslope ? scratch : nullptr,
+                                                              gsum ? *gsum : none);
+    B200_CHECK_CUDA(cudaGetLastError());
+    if (dslope) {
+      k_sum_slots<<<1, 128, 0, st>>>(scratch, blocks * c.N, 1, dslope);
+      B200_CHECK_CUDA(cudaGetLastError());
+    }
+    return OK;
+  }
+  k_act_bwd<false><<<dim3(blocks, c.N), threads, smem, st>>>(g1, g2 ? *g2 : none, c, reinterpret_cast<const float4*>(coef), slope, dz,
+                                                             bstats, bstats_ld, nullptr, nullptr, none);
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;
 }
@@ -939,8 +1015,10 @@ __global__ void k_bias_grad(Act dy, float* __restrict__ part) {
 
 size_t bias_grad_scratch_bytes(int C) { return (size_t)kBiasGradSlots * C * sizeof(float); }
 
-int launch_bias_grad(const Act& dy, float* dbias, float* scratch, cudaStream_t st) {
+int launch_bias_grad(const Act& dy, float* dbias, float* scratch, cudaStream_t st, int c_real) {
   B200_REQUIRE(dy.C % 8 == 0, E_INVALID, "bias_grad: C=%d", dy.C);
+  if (c_real <= 0) c_real = dy.C;
+  B200_REQUIRE(c_real <= dy.C, E_INVALID, "bias_grad: %d real channels of %d", c_real, dy.C);
   B200_REQUIRE(scratch != nullptr, E_INVALID, "bias_grad: needs bias_grad_scratch_bytes() of scratch");
   const int threads = ew_threads_for(dy.C / 8);
   B200_REQUIRE(threads <= 1024, E_UNSUPPORTED, "bias_grad: C=%d unsupported", dy.C);
@@ -948,7 +1026,7 @@ int launch_bias_grad(const Act& dy, float* dbias, float* scratch, cudaStream_t s
   int blocks = (int)(want < kBiasGradSlots ? (want > 0 ? want : 1) : kBiasGradSlots);
   k_bias_grad<<<blocks, threads, (size_t)threads * 8 * sizeof(float), st>>>(dy, scratch);
   B200_CHECK_CUDA(cudaGetLastError());
-  k_sum_slots<<<dy.C, 128, 0, st>>>(scratch, blocks, dy.C, dbias);
+  k_sum_slots<<<c_real, 128, 0, st>>>(scratch, blocks, dy.C, dbias);
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;
 }
@@ -1077,6 +1155,46 @@ int launch_input_grad(const Act* dz, const Act* x, const float* coef, const floa
   B200_REQUIRE(tiles < (1LL << 31) && r.N <= 65535, E_UNSUPPORTED, "input_grad: extent too large");
   k_input_grad<<<dim3((unsigned)tiles, r.N), 256, 0, st>>>(dz ? *dz : none, dz ? *x : none, reinterpret_cast<const float4*>(coef),
                                                          reinterpret_cast<const float2*>(coef2), coef_ld, r, C, dx);
+  B200_CHECK_CUDA(cudaGetLastError());
+  return OK;
+}
+
+// ------------------------------------------------------------------------------------------------ logits of a network whose last layer is a conv
+// y[n][c][s] = in[v][c] + bias[c] (+ add[v][c]) over the C real channels: the conv result (hi + lo: the plans store the last
+// conv's fp32 accumulators as a hi/lo pair in both precisions, so the logits carry no bf16 rounding of their own), its bias in
+// fp32, and MONAI UNet's identity residual `conv(y) + y` of the top residual unit.  Same thread <-> (voxel, 8-channel chunk) walk as k_act_to_ncdhw.
+__global__ void k_logits_unpack(Act in, Act add, const float* __restrict__ bias, int C, float* __restrict__ y) {
+  const long long S = (long long)in.D * in.H * in.W;
+  const int c8n = in.C / 8;
+  const long long total = in.N * S * c8n;
+  for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
+    const int c8 = (int)(t % c8n);
+    const long long vox = t / c8n;
+    const int n = (int)(vox / S);
+    const long long s = vox % S;
+    float v[8];
+    load8(in.hi, in.lo, vox * in.ld + c8 * 8, v);
+    if (add.hi) {
+      float a[8];
+      load8(add.hi, add.lo, vox * add.ld + c8 * 8, a);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) { const int c = c8 * 8 + j; v[j] = (v[j] + (bias && c < C ? bias[c] : 0.f)) + a[j]; }
+    } else if (bias) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) { const int c = c8 * 8 + j; if (c < C) v[j] += bias[c]; }
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { int c = c8 * 8 + j; if (c < C) y[((long long)n * C + c) * S + s] = v[j]; }
+  }
+}
+
+int launch_logits_unpack(const Act& in, const Act* add, const float* bias, int C, float* y, cudaStream_t st) {
+  B200_REQUIRE(in.C % 8 == 0 && C >= 1 && C <= in.C, E_INVALID, "logits_unpack: %d channels of a %d-channel view", C, in.C);
+  B200_REQUIRE(!add || (add->C == in.C && add->N == in.N && add->D == in.D && add->H == in.H && add->W == in.W), E_INVALID,
+               "logits_unpack: addend shape mismatch");
+  const Act none = make_act(nullptr, nullptr, 0, 0, 0, 0, 0, 0);
+  long long total = in.voxels() * (in.C / 8);
+  k_logits_unpack<<<ew_blocks(total, 256), 256, 0, st>>>(in, add ? *add : none, bias, C, y);
   B200_CHECK_CUDA(cudaGetLastError());
   return OK;
 }

@@ -1008,6 +1008,7 @@ static bool conv_halo_eligible(const ConvOp& op, int num_sms) {
   if (op.nsrc == 2 && (op.src[1].ksz != 1 || op.src[1].stride != 1)) return false;
   for (int s = 0; s < op.nsrc; ++s)
     if (op.src[s].x.lo || op.src[s].w_lo) return false;
+  if (op.out.lo) return false;   // the halo kernels store hi only; a lo output of a bf16 op runs per-tap (the epilogue splits)
   return op.out.W >= HaloTile::TW && op.out.H >= HaloTile::TH &&
          (halo_keeps_occupancy(conv_bn(op), conv_kc(op)) || conv_halo_pair(op, num_sms));
 }
@@ -1207,7 +1208,7 @@ int launch_igemm_conv(const ConvOp& op, cudaStream_t st) {
     const int otd = wide ? a.td / 2 : a.td;   // the 256-voxel tile: each warpgroup stores its half
     B200_TRY(make_act_map(&maps.o[0], out.hi, out.N, out.D, out.H, out.W, out.C, out.ld, cbo, a.tw, a.th, otd, 1,
                           swz_for_bytes(cbo * 2)));
-    if (split)
+    if (split || out.lo)   // bf16 operands with a lo output: the fp32 accumulators stored as hi + lo (MONAI UNet's logits)
       B200_TRY(make_act_map(&maps.o[1], out.lo, out.N, out.D, out.H, out.W, out.C, out.ld, cbo, a.tw, a.th, otd, 1,
                             swz_for_bytes(cbo * 2)));
   }

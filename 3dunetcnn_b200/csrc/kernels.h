@@ -7,8 +7,11 @@ namespace b200 {
 // ---- bandwidth-bound kernels (elementwise.cu)
 int launch_input_pack(const float* x, int C, const Act& out, double* stats, int stats_ld, cudaStream_t st);
 // GroupNorm(+ReLU / LeakyReLU) forward: statistics -> coefficients (coef [N][x.C][4], written) -> y; x.C <= 1024
+// slope_dev (optional): the negative slope is read from this device scalar (a learnable PReLU) instead of `slope`;
+// add (optional, y's shape): y = act(A x + B) + add, the addend read as hi + lo
 int launch_gn_apply(const Act& x, const Act& y, const double* stats, const float* gamma, const float* beta, int C, int G,
-                    long long S, float eps, float* coef, float slope, cudaStream_t st);
+                    long long S, float eps, float* coef, float slope, cudaStream_t st, const float* slope_dev = nullptr,
+                    const Act* add = nullptr);
 // GroupNorm backward: backward statistics -> (E, F), dgamma, dbeta -> dx; x.C <= 1024
 int launch_gn_bwd(const Act& dz, const Act& x, const float* coef, const double* bstats, const float* gamma, int C, int G,
                   long long S, float* dgamma, float* dbeta, const Act* add1, const Act* add2, const Act& dx,
@@ -25,8 +28,14 @@ int launch_head_fwd(const Act& x, const float* w, int n_out, int act_mode, float
                     const float* bias = nullptr);
 int launch_head_dbias(const float* dlogits, int N, int NO, long long S, float* dbias, cudaStream_t st, float* scratch);
 // post-activation blocks: dz = (g1 [+ g2]) * act'(A c + B), bstats += (sum dz, sum dz*xhat)
+// PReLU (optional): slope_dev as in launch_gn_apply; dslope (with scratch of act_bwd_slope_scratch_bytes(c)) = sum over z <= 0
+// of z * (g1 [+ g2]), written, bit-identical run to run (per-block partials + a fixed-order sum); gsum = g1 [+ g2]
 int launch_act_bwd(const Act& g1, const Act* g2, const Act& c, const float* coef, float slope, const Act& dz, double* bstats,
-                   int bstats_ld, cudaStream_t st);
+                   int bstats_ld, cudaStream_t st, const float* slope_dev = nullptr, float* dslope = nullptr,
+                   float* scratch = nullptr, const Act* gsum = nullptr);
+size_t act_bwd_slope_scratch_bytes(const Act& c);
+// fp32 NCDHW logits [N][C][S] = in (+ bias[c]) (+ add) over the C real channels of the padded conv result `in`
+int launch_logits_unpack(const Act& in, const Act* add, const float* bias, int C, float* y, cudaStream_t st);
 // scratch: head_bwd_scratch_bytes(n_out, C) (per-block partial sums).  dbias (more than 8 outputs only; launch_head_dbias
 // serves 1..8): also write the bias gradient from the same pass.
 int launch_head_bwd(const Act& x, const float* w, int n_out, const float* dlogits, const Act& dx, float* dw,
@@ -63,8 +72,9 @@ struct PackJob {
 };
 int launch_pack_all(const PtrTable& params, const PackJob* jobs_dev, int njobs, uint8_t* ws, bool split, cudaStream_t st);
 int launch_unpack_all(const PtrTable& grads, const PackJob* jobs_dev, int njobs, const uint8_t* ws, cudaStream_t st);
-// dbias[c] = sum over the VISIBLE voxels of dy (overwritten), in a fixed order; scratch: bias_grad_scratch_bytes(dy.C)
-int launch_bias_grad(const Act& dy, float* dbias, float* scratch, cudaStream_t st);
+// dbias[c] = sum over the VISIBLE voxels of dy (overwritten), in a fixed order, for the first c_real channels (<= 0: all
+// dy.C); scratch: bias_grad_scratch_bytes(dy.C)
+int launch_bias_grad(const Act& dy, float* dbias, float* scratch, cudaStream_t st, int c_real = 0);
 size_t bias_grad_scratch_bytes(int C);
 int launch_zero_insert(const Act& x, const Act& z, int od, int oh, int ow, cudaStream_t st);
 int launch_ncdhw_to_act(const float* x, int C, const Act& out, cudaStream_t st);

@@ -29,6 +29,7 @@ struct Buf {
   size_t off_hi, off_lo;
   int N, D, H, W, C;
   long long stats_off;  // offset (bytes) of [N][C][2] doubles in the stats arena, or -1
+  bool force_lo;        // a lo plane in bf16 plans too (MONAI UNet's logits: the last conv's accumulators as hi + lo)
 };
 
 struct TRef {
@@ -74,6 +75,8 @@ enum LayerKind {
   LAYER_CONVT_ZI,          // nn.ConvTranspose3d(k3, s2, p1) + bias parameter pb, weight [Ci][Co][T]: run as a stride-1 conv over
                            // the zero-inserted input (ksz 3, stride 1), the high boundary of its output forced to 0
   LAYER_CONVT_K2S2,        // ConvTranspose3d with kernel = stride = 2 (MONAI UnetUpBlock): ksz 2, stride 2, weight [Ci][Co][8], no padding
+  LAYER_CONVT_OP1,         // nn.ConvTranspose3d(k3, s2, p1, output_padding 1) (MONAI UNet's up layers): LAYER_CONVT_ZI with the high
+                           // boundary kept (the 2n grid is the op's own output), bias parameter pb optional
 };
 enum ConvDir { DIR_FWD = 0, DIR_DGRAD, DIR_WGRAD };
 
@@ -86,6 +89,7 @@ struct ConvLayer {
   bool need_dgrad;
   LayerKind kind;
   int pb;
+  size_t bias_pad;         // != 0: workspace copy of the bias padded to Cop with zeros (the epilogue reads Cop entries)
   std::string name;        // state-dict key (profiling labels)
 };
 
@@ -94,7 +98,8 @@ struct ConvRole {
   int stride;              // traversal stride on the A operand (the input; dgrad: the output gradient)
   int nopad;               // 1: no padding
   int cls_mode;            // ConvOp::cls_mode
-  bool bias;               // + bias parameter pb, the output's high boundary forced to 0 (ConvOp::zero_last)
+  bool bias;               // + bias parameter pb when the layer has one
+  bool zero_last;          // the output's high boundary forced to 0 (ConvOp::zero_last)
   int pack;                // PackMode of the weights the op reads; DIR_WGRAD: unpack mode of the accumulator
   bool swap;               // the op sees the layer with Ci and Co exchanged: the data gradient, and the weight gradient of a
                            // kernel = stride layer, which is that of the stride-2 convolution from the fine grid (dU, Co) to the
@@ -106,7 +111,8 @@ static ConvRole conv_role(const ConvLayer& c, ConvDir dir) {
   const bool up = c.kind != LAYER_CONV, k2 = c.kind == LAYER_CONVT_K2S2;
   ConvRole r = {};
   r.nopad = k2 ? 1 : 0;
-  r.bias = dir == DIR_FWD && c.kind == LAYER_CONVT_ZI;
+  r.bias = dir == DIR_FWD && !k2;
+  r.zero_last = dir == DIR_FWD && c.kind == LAYER_CONVT_ZI;
   r.swap = dir == DIR_DGRAD || (dir == DIR_WGRAD && k2);
   r.macs_div = up ? 8 : 1;
   if (dir == DIR_FWD) {
@@ -119,13 +125,14 @@ static ConvRole conv_role(const ConvLayer& c, ConvDir dir) {
     r.pack = up ? PACK_T_DGRAD : PACK_DGRAD;
   } else {
     r.stride = c.stride;
-    r.pack = c.kind == LAYER_CONVT_ZI ? PACK_T_FLIPPED : PACK_FWD;
+    r.pack = (c.kind == LAYER_CONVT_ZI || c.kind == LAYER_CONVT_OP1) ? PACK_T_FLIPPED : PACK_FWD;
   }
   return r;
 }
 
 struct NormLayer {
-  int pg, pb;
+  int pg, pb;              // affine parameters (-1: none)
+  int pa;                  // PReLU slope parameter (-1: the plan's fixed slope)
   int C, Cld, G;
   long long S;
   size_t coef, coef2, bstats;
@@ -190,6 +197,7 @@ struct b200unet_plan {
   float slope = 0.f;        // negative slope of the activation (0 = ReLU: UNet3D; 0.01 = LeakyReLU: DynUNet)
   bool infer = false;       // forward-only plan: no backward schedule / buffers, forward temporaries are recycled
   std::vector<std::pair<size_t, std::pair<size_t, size_t>>> free_bufs;   // (bytes, (off_hi, off_lo)) of released buffers
+  std::vector<int> bias_pad_convs;   // convolutions whose bias the prologue copies into a zero-padded workspace slot
 
   size_t alloc(size_t bytes) {
     size_t off = (cur + 1023) & ~size_t(1023);
@@ -282,11 +290,11 @@ static void unet3d_param_spec(Plan& P) {
 }
 
 // ------------------------------------------------------------------------------------------------ builders
-static int new_buf(Plan& P, int N, int D, int H, int W, int C) {
+static int new_buf(Plan& P, int N, int D, int H, int W, int C, bool force_lo = false) {
   Buf b;
   size_t bytes = (size_t)N * D * H * W * C * sizeof(bf16);
   bool reused = false;
-  for (size_t i = 0; i < P.free_bufs.size(); ++i)
+  for (size_t i = 0; i < P.free_bufs.size() && !(force_lo && !P.split); ++i)
     if (P.free_bufs[i].first == bytes) {   // forward-only plans: take a released buffer of the same size
       b.off_hi = P.free_bufs[i].second.first;
       b.off_lo = P.free_bufs[i].second.second;
@@ -296,8 +304,9 @@ static int new_buf(Plan& P, int N, int D, int H, int W, int C) {
     }
   if (!reused) {
     b.off_hi = P.alloc(bytes);
-    b.off_lo = P.split ? P.alloc(bytes) : 0;
+    b.off_lo = (P.split || force_lo) ? P.alloc(bytes) : 0;
   }
+  b.force_lo = force_lo;
   b.N = N; b.D = D; b.H = H; b.W = W; b.C = C;
   b.stats_off = -1;
   P.bufs.push_back(b);
@@ -324,7 +333,7 @@ static void release_if_whole(Plan& P, TRef t) {
 static Act act_of(const Plan& P, const RunCtx& cx, TRef t) {
   const Buf& b = P.bufs[t.buf];
   bf16* hi = reinterpret_cast<bf16*>(cx.ws + b.off_hi) + t.c0;
-  bf16* lo = P.split ? reinterpret_cast<bf16*>(cx.ws + b.off_lo) + t.c0 : nullptr;
+  bf16* lo = (P.split || b.force_lo) ? reinterpret_cast<bf16*>(cx.ws + b.off_lo) + t.c0 : nullptr;
   Act a = make_act(hi, lo, b.N, b.D, b.H, b.W, t.c, b.C);
   if (t.vis_m1) { a.vD = b.D - 1; a.vH = b.H - 1; a.vW = b.W - 1; }
   return a;
@@ -351,6 +360,7 @@ static int new_conv(Plan& P, const std::string& key, int Co, int Ci, int ksz, in
   c.need_dgrad = need_dgrad;
   c.kind = kind;
   c.pb = -1;
+  c.bias_pad = 0;
   size_t n = (size_t)c.T * c.Cop * c.Cip;
   c.wf_hi = P.alloc(n * 2);
   c.wf_lo = P.split ? P.alloc(n * 2) : 0;
@@ -368,6 +378,7 @@ static int new_norm(Plan& P, const std::string& prefix, int C, int Cld, long lon
   n.name = prefix;
   n.pg = P.find_param(prefix + ".weight");
   n.pb = P.find_param(prefix + ".bias");
+  n.pa = -1;
   n.C = C; n.Cld = Cld; n.G = G; n.S = S;
   n.coef = P.alloc((size_t)P.d.batch * Cld * 4 * sizeof(float));
   n.coef2 = P.infer ? 0 : P.alloc((size_t)P.d.batch * Cld * 2 * sizeof(float));
@@ -393,19 +404,26 @@ static inline void prof_mark(RunCtx& cx, int cat, bool end) {
 }
 #define LAUNCHED(cx, cat, expr) do { prof_mark(cx, cat, false); B200_TRY(expr); prof_mark(cx, cat, true); (cx).launches++; } while (0)
 
+// the pointer of parameter (or gradient) i, nullptr for i < 0 (a norm without affine parameters)
+static inline const float* pptr(const float* const* p, int i) { return i >= 0 ? p[i] : nullptr; }
+static inline float* pptr(float* const* p, int i) { return i >= 0 ? p[i] : nullptr; }
+
 static std::string shape_of(const Plan& P, TRef t) {
   const Buf& b = P.bufs[t.buf];
   return std::to_string(t.c) + "ch@" + std::to_string(b.D) + "x" + std::to_string(b.H) + "x" + std::to_string(b.W);
 }
 
 // ---- forward op emitters (weight packing is batched: see emit_prologue)
-static void emit_norm_fwd(Plan& P, int ni, TRef x, TRef y) {
-  push_op(P.fwd, "gn_apply " + P.norms[ni].name + " " + shape_of(P, x), [&P, ni, x, y](RunCtx& cx) -> int {
+// add (optional): y = act(norm(x)) + add, the output of a MONAI ResidualUnit
+static void emit_norm_fwd(Plan& P, int ni, TRef x, TRef y, TRef add = kNone) {
+  push_op(P.fwd, "gn_apply " + P.norms[ni].name + " " + shape_of(P, x) + (add.valid() ? " +res" : ""), [&P, ni, x, y, add](RunCtx& cx) -> int {
     const NormLayer& n = P.norms[ni];
+    Act a;
+    if (add.valid()) a = act_of(P, cx, add);
     // statistics -> coefficients -> normalise + ReLU in one launch (the coefficients are kept for the backward pass)
-    LAUNCHED(cx, CAT_NORM, launch_gn_apply(act_of(P, cx, x), act_of(P, cx, y), stats_ptr(P, cx, x), cx.params[n.pg],
-                                           cx.params[n.pb], n.C, n.G, n.S, 1e-5f, reinterpret_cast<float*>(cx.ws + n.coef),
-                                           P.slope, cx.st));
+    LAUNCHED(cx, CAT_NORM, launch_gn_apply(act_of(P, cx, x), act_of(P, cx, y), stats_ptr(P, cx, x), pptr(cx.params, n.pg),
+                                           pptr(cx.params, n.pb), n.C, n.G, n.S, 1e-5f, reinterpret_cast<float*>(cx.ws + n.coef),
+                                           P.slope, cx.st, pptr(cx.params, n.pa), add.valid() ? &a : nullptr));
     return OK;
   });
 }
@@ -437,7 +455,10 @@ static ConvOp conv_op(const Plan& P, const RunCtx& cx, const ConvLayer& c, ConvD
   op.Cop = r.swap ? c.Cip : c.Cop;
   op.out = act_of(P, cx, out);
   op.cls_mode = r.cls_mode;
-  if (r.bias) { op.bias = cx.params[c.pb]; op.zero_last = 1; }
+  if (r.bias && c.pb >= 0) {
+    op.bias = c.bias_pad ? reinterpret_cast<const float*>(cx.ws + c.bias_pad) : cx.params[c.pb];
+    op.zero_last = r.zero_last;
+  }
   return op;
 }
 
@@ -562,9 +583,9 @@ static void emit_gn_bwd_finalize(Plan& P, int ni) {
   push_op(P.bwd, "gn_bwd_finalize " + P.norms[ni].name, [&P, ni](RunCtx& cx) -> int {
     const NormLayer& n = P.norms[ni];
     LAUNCHED(cx, CAT_NORM, launch_gn_bwd_finalize(reinterpret_cast<double*>(cx.ws + P.bz_off + n.bstats),
-                                        reinterpret_cast<float*>(cx.ws + n.coef), cx.params[n.pg], P.d.batch, n.C, n.Cld,
-                                        n.G, n.S, reinterpret_cast<float*>(cx.ws + n.coef2), cx.grads[n.pg],
-                                        cx.grads[n.pb], cx.st));
+                                        reinterpret_cast<float*>(cx.ws + n.coef), pptr(cx.params, n.pg), P.d.batch, n.C, n.Cld,
+                                        n.G, n.S, reinterpret_cast<float*>(cx.ws + n.coef2), pptr(cx.grads, n.pg),
+                                        pptr(cx.grads, n.pb), cx.st));
     return OK;
   });
 }
@@ -576,25 +597,30 @@ static void emit_gn_bwd(Plan& P, int ni, TRef dz, TRef x, TRef add1, TRef dx, bo
     if (add1.valid()) a1 = act_of(P, cx, add1);
     // finalize fused: (E, F), dgamma, dbeta are derived from the backward statistics inside the kernel
     LAUNCHED(cx, CAT_NORM, launch_gn_bwd(act_of(P, cx, dz), act_of(P, cx, x), reinterpret_cast<float*>(cx.ws + n.coef),
-                                         reinterpret_cast<double*>(cx.ws + P.bz_off + n.bstats), cx.params[n.pg], n.C, n.G,
-                                         n.S, cx.grads[n.pg], cx.grads[n.pb], add1.valid() ? &a1 : nullptr, nullptr,
+                                         reinterpret_cast<double*>(cx.ws + P.bz_off + n.bstats), pptr(cx.params, n.pg), n.C, n.G,
+                                         n.S, pptr(cx.grads, n.pg), pptr(cx.grads, n.pb), add1.valid() ? &a1 : nullptr, nullptr,
                                          act_of(P, cx, dx), (scale && cx.drop) ? cx.drop : nullptr, cx.st));
     return OK;
   });
 }
 
 // returns the gradient of norm ni's input x from the gradient g1 (+ g2) of its activated output: the activation's backward
-// (which also takes the norm's backward statistics), then the norm's
-static TRef emit_act_norm_bwd(Plan& P, int ni, TRef x, TRef g1, TRef g2) {
+// (which also takes the norm's backward statistics and, for a PReLU, the slope's gradient), then the norm's.  gsum (optional):
+// also store g1 + g2 there, for a residual branch that takes the same gradient.
+static TRef emit_act_norm_bwd(Plan& P, int ni, TRef x, TRef g1, TRef g2, TRef gsum = kNone) {
   const Buf xb = P.bufs[x.buf];
   const TRef dz = full(P, new_buf(P, xb.N, xb.D, xb.H, xb.W, x.c));
-  push_op(P.bwd, "act_bwd " + P.norms[ni].name + " " + shape_of(P, x), [&P, ni, g1, g2, x, dz](RunCtx& cx) -> int {
+  if (P.norms[ni].pa >= 0) P.head_part_bytes = std::max(P.head_part_bytes, act_bwd_slope_scratch_bytes(shape_act(P, x)));
+  push_op(P.bwd, "act_bwd " + P.norms[ni].name + " " + shape_of(P, x), [&P, ni, g1, g2, x, dz, gsum](RunCtx& cx) -> int {
     const NormLayer& n = P.norms[ni];
-    Act a2;
+    Act a2, gs;
     if (g2.valid()) a2 = act_of(P, cx, g2);
+    if (gsum.valid()) gs = act_of(P, cx, gsum);
     LAUNCHED(cx, CAT_NORM, launch_act_bwd(act_of(P, cx, g1), g2.valid() ? &a2 : nullptr, act_of(P, cx, x),
                                           reinterpret_cast<float*>(cx.ws + n.coef), P.slope, act_of(P, cx, dz),
-                                          reinterpret_cast<double*>(cx.ws + P.bz_off + n.bstats), n.Cld, cx.st));
+                                          reinterpret_cast<double*>(cx.ws + P.bz_off + n.bstats), n.Cld, cx.st, pptr(cx.params, n.pa),
+                                          pptr(cx.grads, n.pa), reinterpret_cast<float*>(cx.ws + P.head_part_off),
+                                          gsum.valid() ? &gs : nullptr));
     return OK;
   });
   const TRef dx = full(P, new_buf(P, xb.N, xb.D, xb.H, xb.W, x.c));
@@ -637,6 +663,11 @@ static TRef emit_prologue(Plan& P, bool with_input_stats) {
     if (!cx.skip_pack)
       LAUNCHED(cx, CAT_PACK, launch_pack_all(ptr_table(P, cx.params), reinterpret_cast<const PackJob*>(cx.ws + P.jobs_off),
                                              (int)P.pack_jobs.size(), cx.ws, P.split, cx.st));
+    for (int ci : P.bias_pad_convs) {   // zero-padded bias copies (layers whose output width is not a multiple of 8)
+      const ConvLayer& c = P.convs[ci];
+      B200_CHECK_CUDA(cudaMemsetAsync(cx.ws + c.bias_pad, 0, sizeof(float) * c.Cop, cx.st));
+      B200_CHECK_CUDA(cudaMemcpyAsync(cx.ws + c.bias_pad, cx.params[c.pb], sizeof(float) * c.Co, cudaMemcpyDeviceToDevice, cx.st));
+    }
     TRef t = full(P, b_in);
     LAUNCHED(cx, CAT_RESAMPLE, launch_input_pack(cx.x, P.d.n_features, act_of(P, cx, t), with_input_stats ? stats_ptr(P, cx, t) : nullptr,
                                                  P.bufs[b_in].C, cx.st));
@@ -1337,7 +1368,331 @@ static int build_segresnet(Plan& P) {
   return finish_build(P);
 }
 
-static int build(Plan& P) { return P.d.arch == 2 ? build_segresnet(P) : P.d.arch == 1 ? build_dynunet(P) : build_unet3d(P); }
+static int build_unet(Plan& P);
+
+static int build(Plan& P) {
+  return P.d.arch == 3 ? build_unet(P) : P.d.arch == 2 ? build_segresnet(P) : P.d.arch == 1 ? build_dynunet(P) : build_unet3d(P);
+}
+
+// ================================================================================================ UNet (MONAI)
+// MONAI's UNet (monai/networks/nets/unet.py with monai/networks/blocks/convolutions.py Convolution / ResidualUnit), absent
+// from this image like DynUNet: restated from its public definition -- parity unpinned, see oracle/unet_oracle.py.
+//   Convolution(ci, co, stride):  conv k3 (transposed: k3 s2 p1 output_padding 1) [+ bias] -> InstanceNorm3d(co) [affine] -> act
+//                                 (PReLU with one learnable slope, ReLU or LeakyReLU); conv_only: the conv alone
+//   ResidualUnit(ci, co, stride, subunits r):  conv.unit0 (strided) .. conv.unit{r-1}, then + residual(x): a k3 conv with the
+//                                 stride when it is 2, a 1x1x1 conv when only the width changes, else the identity (a bias iff bias)
+//   level i (channels c = F[i]):  Sequential(down_i: inc -> c stride 2, SkipConnection(sub_i) = cat([x, sub_i(x)]), up_i: upc -> outc)
+//                                 sub_i = level i + 1 (outc = c), or at the bottom the stride-1 down layer c -> F[L-1];
+//                                 up_i = Convolution(transposed) [ + ResidualUnit(outc, outc, 1, last_conv_only = top) ]
+//   the top up layer is conv_only without residual units, and its residual unit's one conv with them: logits = conv(y) + y.
+// Schedule: cat_i (the SkipConnection output at level i + 1) holds [down_i output | sub_i output]; each Convolution is the conv
+// (bias in its epilogue, before the statistics) + one fused norm-apply (+ PReLU slope read on the device, + the residual addend);
+// the logits conv stores its fp32 accumulators as a hi/lo pair in both precisions (a per-tap launch whose epilogue splits them),
+// which launch_logits_unpack turns into fp32 NCDHW logits with the bias and the identity residual.
+struct UConv {           // one Convolution
+  int k = -1, ni = -1;   // conv layer, norm (-1: conv_only)
+  TRef in = kNone;       // conv input (transposed: the input before zero insertion)
+  TRef z = kNone;        // transposed: the zero-inserted input the conv reads
+  TRef c = kNone;        // raw conv output (conv_only: the logits buffer)
+  int pb = -1;           // bias parameter
+};
+struct ULayer {          // a down / bottom layer (ResidualUnit or Convolution) or an up layer
+  TRef X = kNone;
+  std::vector<UConv> u;
+  int res = -1;          // residual conv (-1: identity, or no residual unit)
+  TRef R = kNone;        // residual conv output
+  bool first = false;    // reads the network input
+  TRef y = kNone;        // up layer with residual units: output of the transposed Convolution
+};
+
+static std::string unet_prefix(int level) {
+  std::string p = "model.";
+  for (int i = 0; i < level; ++i) p += "1.submodule.";
+  return p;
+}
+
+static void add_unet_conv_params(Plan& P, const std::string& pre, int ci, int co, bool transposed, bool conv_only) {
+  const b200unet_net_desc& d = P.d;
+  if (transposed) add_param(P, pre + ".conv.weight", {ci, co, 3, 3, 3});
+  else add_param(P, pre + ".conv.weight", {co, ci, 3, 3, 3});
+  if (d.conv_bias) add_param(P, pre + ".conv.bias", {co});
+  if (conv_only) return;
+  if (d.norm_affine) { add_param(P, pre + ".adn.N.weight", {co}); add_param(P, pre + ".adn.N.bias", {co}); }
+  if (d.act_kind == 1) add_param(P, pre + ".adn.A.weight", {1});
+}
+
+static void add_unet_down_params(Plan& P, const std::string& pre, int ci, int co, int stride) {
+  const int r = P.d.num_res_units;
+  if (r == 0) { add_unet_conv_params(P, pre, ci, co, false, false); return; }
+  for (int u = 0; u < r; ++u) add_unet_conv_params(P, pre + ".conv.unit" + std::to_string(u), u == 0 ? ci : co, co, false, false);
+  if (stride != 1 || ci != co) {
+    const int k = stride != 1 ? 3 : 1;
+    add_param(P, pre + ".residual.weight", {co, ci, k, k, k});
+    if (P.d.conv_bias) add_param(P, pre + ".residual.bias", {co});
+  }
+}
+
+static void add_unet_up_params(Plan& P, const std::string& pre, int upc, int outc, bool top) {
+  if (P.d.num_res_units == 0) { add_unet_conv_params(P, pre, upc, outc, true, top); return; }
+  add_unet_conv_params(P, pre + ".0", upc, outc, true, false);
+  add_unet_conv_params(P, pre + ".1.conv.unit0", outc, outc, false, top);
+}
+
+// MONAI's registration order: level i's down layer, its submodule (level i + 1, or the bottom layer), its up layer
+static void unet_param_spec_level(Plan& P, int i) {
+  const b200unet_net_desc& d = P.d;
+  const int L = d.n_levels;
+  const int* F = d.filters;
+  const std::string pre = unet_prefix(i);
+  const int inc = i == 0 ? d.n_features : F[i - 1], outc = i == 0 ? d.n_outputs : F[i - 1];
+  add_unet_down_params(P, pre + "0", inc, F[i], 2);
+  if (i + 2 < L) unet_param_spec_level(P, i + 1);
+  else add_unet_down_params(P, pre + "1.submodule", F[i], F[L - 1], 1);
+  add_unet_up_params(P, pre + "2", i + 2 < L ? 2 * F[i] : F[i] + F[L - 1], outc, i == 0);
+}
+static void unet_param_spec(Plan& P) { unet_param_spec_level(P, 0); }
+
+// dbias = the per-channel sum of dy over its first c_real channels (fixed order)
+static void emit_bias_grad(Plan& P, int pb, TRef dy, int c_real) {
+  P.head_part_bytes = std::max(P.head_part_bytes, bias_grad_scratch_bytes(dy.c));
+  push_op(P.bwd, "bias_grad " + P.params[pb].key, [&P, pb, dy, c_real](RunCtx& cx) -> int {
+    LAUNCHED(cx, CAT_OTHER, launch_bias_grad(act_of(P, cx, dy), cx.grads[pb], reinterpret_cast<float*>(cx.ws + P.head_part_off), cx.st,
+                                             c_real));
+    return OK;
+  });
+}
+
+// forward of one Convolution from X (ci real channels) into dest (+ add after the activation); conv_only: dest receives the raw
+// conv result (no bias: launch_logits_unpack adds it).  first: X is the packed network input.
+static UConv unet_conv_fwd(Plan& P, const std::string& pre, TRef X, int ci, int co, int stride, bool transposed, bool conv_only,
+                           TRef dest, TRef add, bool first) {
+  UConv u;
+  u.in = X;
+  const Buf xb = P.bufs[X.buf];
+  const int N = xb.N, D = transposed ? 2 * xb.D : xb.D / stride, H = transposed ? 2 * xb.H : xb.H / stride,
+            W = transposed ? 2 * xb.W : xb.W / stride;
+  u.k = new_conv(P, pre + ".conv.weight", co, ci, 3, transposed ? 1 : stride, !first || P.input_grad,
+                 transposed ? LAYER_CONVT_OP1 : LAYER_CONV);
+  u.pb = P.find_param(pre + ".conv.bias");
+  ConvLayer& c = P.convs[u.k];
+  if (!conv_only) {
+    c.pb = u.pb;
+    if (c.pb >= 0 && c.Co % 8) { c.bias_pad = P.alloc(sizeof(float) * c.Cop); P.bias_pad_convs.push_back(u.k); }
+  }
+  TRef src = X;
+  if (transposed) {
+    u.z = full(P, new_buf(P, N, D, H, W, X.c));
+    const TRef Xi = X, Z = u.z;
+    push_op(P.fwd, "zero_insert " + shape_of(P, Z), [&P, Xi, Z](RunCtx& cx) -> int {
+      LAUNCHED(cx, CAT_RESAMPLE, launch_zero_insert(act_of(P, cx, Xi), act_of(P, cx, Z), 0, 0, 0, cx.st));
+      return OK;
+    });
+    src = u.z;
+  }
+  if (conv_only) {
+    u.c = dest;
+    emit_conv_fwd(P, u.k, src, -1, kNone, kNone, dest, false, false);
+    if (transposed) release_buf(P, u.z.buf);
+    return u;
+  }
+  u.c = full(P, new_buf(P, N, D, H, W, P.convs[u.k].Cop));
+  emit_conv_fwd(P, u.k, src, -1, kNone, kNone, u.c, true, false);
+  if (transposed) release_buf(P, u.z.buf);
+  u.ni = new_norm(P, pre + ".adn.N", co, u.c.c, (long long)D * H * W, co);
+  P.norms[u.ni].pa = P.find_param(pre + ".adn.A.weight");
+  emit_norm_fwd(P, u.ni, u.c, dest, add);
+  release_buf(P, u.c.buf);
+  return u;
+}
+
+static ULayer unet_down_fwd(Plan& P, const std::string& pre, TRef X, int ci, int co, int stride, TRef dest, bool first) {
+  const int r = P.d.num_res_units;
+  ULayer l;
+  l.X = X; l.first = first;
+  if (r == 0) {
+    l.u.push_back(unet_conv_fwd(P, pre, X, ci, co, stride, false, false, dest, kNone, first));
+    return l;
+  }
+  const Buf xb = P.bufs[X.buf];
+  const int N = xb.N, D = xb.D / stride, H = xb.H / stride, W = xb.W / stride;
+  TRef R = X;
+  if (stride != 1 || ci != co) {
+    const int k = stride != 1 ? 3 : 1;
+    l.res = new_conv(P, pre + ".residual.weight", co, ci, k, stride, !first || P.input_grad);
+    P.convs[l.res].pb = P.find_param(pre + ".residual.bias");
+    l.R = R = full(P, new_buf(P, N, D, H, W, co));
+    emit_conv_fwd(P, l.res, X, -1, kNone, kNone, R, false, false);
+  }
+  TRef a = X;
+  int cin = ci;
+  for (int u = 0; u < r; ++u) {
+    const bool last = u + 1 == r;
+    const TRef out = last ? dest : full(P, new_buf(P, N, D, H, W, co));
+    l.u.push_back(unet_conv_fwd(P, pre + ".conv.unit" + std::to_string(u), a, cin, co, u == 0 ? stride : 1, false, false, out,
+                                last ? R : kNone, first && u == 0));
+    if (u > 0) release_buf(P, a.buf);
+    a = out;
+    cin = co;
+  }
+  if (l.res >= 0) release_buf(P, l.R.buf);
+  return l;
+}
+
+static ULayer unet_up_fwd(Plan& P, const std::string& pre, TRef X, int upc, int outc, bool top, TRef dest) {
+  ULayer l;
+  l.X = X;
+  if (P.d.num_res_units == 0) {
+    l.u.push_back(unet_conv_fwd(P, pre, X, upc, outc, 2, true, top, dest, kNone, false));
+    return l;
+  }
+  const Buf xb = P.bufs[X.buf];
+  l.y = full(P, new_buf(P, xb.N, 2 * xb.D, 2 * xb.H, 2 * xb.W, round_up(outc, 8)));
+  l.u.push_back(unet_conv_fwd(P, pre + ".0", X, upc, outc, 2, true, false, l.y, kNone, false));
+  l.u.push_back(unet_conv_fwd(P, pre + ".1.conv.unit0", l.y, outc, outc, 1, false, top, dest, top ? kNone : l.y, false));
+  if (!top) release_buf(P, l.y.buf);
+  return l;
+}
+
+// backward of one Convolution from the gradient dc of its raw conv output: bias and weight gradients; returns the data gradient
+// of its input (into dx when valid, else a new buffer) + res (optional), or kNone when want_dx is false
+static TRef unet_conv_bwd_from_dc(Plan& P, const UConv& u, TRef dc, bool want_dx, TRef res, TRef dx = kNone) {
+  if (u.pb >= 0 && u.ni >= 0) emit_bias_grad(P, u.pb, dc, P.convs[u.k].Co);
+  emit_wgrad(P, u.k, u.z.valid() ? u.z : u.in, dc);
+  if (!want_dx) return kNone;
+  if (!dx.valid()) {
+    const Buf xb = P.bufs[u.in.buf];
+    dx = full(P, new_buf(P, xb.N, xb.D, xb.H, xb.W, u.in.c));
+  }
+  emit_dgrad(P, u.k, dc, dx, -1, kNone, res, false);
+  return dx;
+}
+
+// down / bottom layer: gradient g1 (+ g2) of its output; returns the gradient of its input (kNone for the first layer, whose
+// input-gradient ops go to the input_grad list)
+static TRef unet_down_bwd(Plan& P, const ULayer& l, TRef g1, TRef g2) {
+  const int r = (int)l.u.size();
+  const bool resunit = P.d.num_res_units > 0;
+  TRef G = g1;
+  TRef gsum = kNone;
+  if (resunit && g2.valid()) {   // the residual branch takes the same gradient: materialise g1 + g2 in the act backward
+    const Buf gb = P.bufs[l.u[r - 1].c.buf];
+    G = gsum = full(P, new_buf(P, gb.N, gb.D, gb.H, gb.W, g1.c));
+  }
+  TRef dc = emit_act_norm_bwd(P, l.u[r - 1].ni, l.u[r - 1].c, g1, g2, gsum);
+  if (l.res >= 0) {
+    emit_wgrad(P, l.res, l.X, G);
+    if (P.convs[l.res].pb >= 0) emit_bias_grad(P, P.convs[l.res].pb, G, P.convs[l.res].Co);
+  }
+  for (int u = r - 1; u > 0; --u) {
+    const TRef da = unet_conv_bwd_from_dc(P, l.u[u], dc, true, kNone);
+    dc = emit_act_norm_bwd(P, l.u[u - 1].ni, l.u[u - 1].c, da, kNone);
+  }
+  const UConv& u0 = l.u[0];
+  if (l.first) {
+    unet_conv_bwd_from_dc(P, u0, dc, false, kNone);
+    if (!P.input_grad) return kNone;
+    if (!resunit) { emit_input_dgrad(P, u0.k, dc, l.X, -1, kNone); return kNone; }
+    const Buf xb = P.bufs[l.X.buf];
+    const TRef rb = full(P, new_buf(P, xb.N, xb.D, xb.H, xb.W, l.X.c));
+    TRef add = G;
+    if (l.res >= 0) { emit_dgrad(P, l.res, G, rb, -1, kNone, kNone, false, true, &P.igrad); add = rb; }
+    emit_dgrad(P, u0.k, dc, rb, -1, kNone, add, false, true, &P.igrad);
+    emit_input_grad(P, -1, kNone, l.X, rb);
+    return kNone;
+  }
+  if (!resunit) return unet_conv_bwd_from_dc(P, u0, dc, true, kNone);
+  TRef add = G;
+  if (l.res >= 0) {
+    const Buf xb = P.bufs[l.X.buf];
+    add = full(P, new_buf(P, xb.N, xb.D, xb.H, xb.W, l.X.c));
+    emit_dgrad(P, l.res, G, add, -1, kNone, kNone, false);
+  }
+  return unet_conv_bwd_from_dc(P, u0, dc, true, add);
+}
+
+// up layer: gradient G of its output (top: of the padded logits); returns the gradient of its input (the whole cat buffer)
+static TRef unet_up_bwd(Plan& P, const ULayer& l, TRef G) {
+  if (l.u.size() == 1) {
+    const UConv& u = l.u[0];
+    const TRef dc = u.ni >= 0 ? emit_act_norm_bwd(P, u.ni, u.c, G, kNone) : G;
+    return unet_conv_bwd_from_dc(P, u, dc, true, kNone);
+  }
+  const UConv& u1 = l.u[1];
+  const TRef dc1 = u1.ni >= 0 ? emit_act_norm_bwd(P, u1.ni, u1.c, G, kNone) : G;
+  const TRef dy = unet_conv_bwd_from_dc(P, u1, dc1, true, /*identity residual*/ G);
+  const UConv& u0 = l.u[0];
+  return unet_conv_bwd_from_dc(P, u0, emit_act_norm_bwd(P, u0.ni, u0.c, dy, kNone), true, kNone);
+}
+
+static int build_unet(Plan& P) {
+  const b200unet_net_desc& d = P.d;
+  const int L = d.n_levels, N = d.batch;
+  B200_REQUIRE(L >= 2 && L <= 8, E_UNSUPPORTED, "plan: UNet with %d levels unsupported (len(channels) 2..8)", L);
+  B200_REQUIRE(d.n_features >= 1 && d.n_features <= 16, E_UNSUPPORTED, "plan: in_channels=%d unsupported (1..16)", d.n_features);
+  B200_REQUIRE(d.n_outputs >= 1 && d.n_outputs <= 16, E_UNSUPPORTED, "plan: out_channels=%d unsupported (1..16)", d.n_outputs);
+  B200_REQUIRE(d.num_res_units >= 0, E_UNSUPPORTED, "plan: num_res_units=%d unsupported", d.num_res_units);
+  B200_REQUIRE(d.act_kind == 0 || d.act_kind == 1, E_UNSUPPORTED, "plan: act_kind=%d unsupported (0 fixed slope, 1 PReLU)", d.act_kind);
+  B200_REQUIRE(d.activation == 0, E_UNSUPPORTED, "plan: UNet has no output activation (activation=%d)", d.activation);
+  for (int i = 0; i < L; ++i)
+    B200_REQUIRE(d.filters[i] >= 8 && d.filters[i] % 8 == 0 && d.filters[i] <= 1024, E_UNSUPPORTED,
+                 "plan: channels[%d]=%d must be a multiple of 8 up to 1024", i, d.filters[i]);
+  std::vector<int> F(d.filters, d.filters + L), Ds, Hs, Ws;
+  B200_TRY(level_extents(d, Ds, Hs, Ws));
+  unet_param_spec(P);
+
+  // ---- forward: down layers, bottom, up layers (the recursion's execution order)
+  const TRef in = emit_prologue(P, /*with_input_stats=*/false);
+  std::vector<int> cat(L - 1);
+  for (int i = 0; i + 1 < L; ++i) cat[i] = new_buf(P, N, Ds[i + 1], Hs[i + 1], Ws[i + 1], F[i] + (i + 2 < L ? F[i] : F[L - 1]));
+  std::vector<ULayer> down(L - 1), up(L - 1);
+  for (int i = 0; i + 1 < L; ++i) {
+    const TRef X = i == 0 ? in : slice(full(P, cat[i - 1]), 0, F[i - 1]);
+    down[i] = unet_down_fwd(P, unet_prefix(i) + "0", X, i == 0 ? d.n_features : F[i - 1], F[i], 2, slice(full(P, cat[i]), 0, F[i]),
+                            i == 0);
+    if (i == 0) release_buf(P, in.buf);
+  }
+  const ULayer bottom = unet_down_fwd(P, unet_prefix(L - 2) + "1.submodule", slice(full(P, cat[L - 2]), 0, F[L - 2]), F[L - 2], F[L - 1],
+                                      1, slice(full(P, cat[L - 2]), F[L - 2], F[L - 1]), false);
+  const TRef logits = full(P, new_buf(P, N, Ds[0], Hs[0], Ws[0], round_up(d.n_outputs, 8), /*force_lo=*/true));
+  for (int i = L - 2; i >= 0; --i) {
+    const TRef dest = i == 0 ? logits : slice(full(P, cat[i - 1]), F[i - 1], F[i - 1]);
+    up[i] = unet_up_fwd(P, unet_prefix(i) + "2", full(P, cat[i]), P.bufs[cat[i]].C, i == 0 ? d.n_outputs : F[i - 1], i == 0, dest);
+    release_buf(P, cat[i]);
+  }
+  const UConv& last = up[0].u.back();
+  const TRef yres = d.num_res_units > 0 ? up[0].y : kNone;
+  const int pbl = last.pb;
+  push_op(P.fwd, "logits_unpack " + shape_of(P, logits), [&P, logits, yres, pbl](RunCtx& cx) -> int {
+    Act a;
+    if (yres.valid()) a = act_of(P, cx, yres);
+    LAUNCHED(cx, CAT_HEAD, launch_logits_unpack(act_of(P, cx, logits), yres.valid() ? &a : nullptr, pptr(cx.params, pbl), P.d.n_outputs,
+                                                cx.logits, cx.st));
+    return OK;
+  });
+  if (P.infer) return finish_build(P);
+
+  // ---- backward
+  push_op(P.bwd, "memset", [&P](RunCtx& cx) -> int {   // zero the backward statistics and the weight-gradient accumulators
+    B200_CHECK_CUDA(cudaMemsetAsync(cx.ws + P.bz_off, 0, P.bz_bytes, cx.st));
+    return OK;
+  });
+  const TRef gL = full(P, new_buf(P, N, Ds[0], Hs[0], Ws[0], logits.c));
+  push_op(P.bwd, "dlogits_pack " + shape_of(P, gL), [&P, gL](RunCtx& cx) -> int {
+    LAUNCHED(cx, CAT_HEAD, launch_ncdhw_to_act(cx.dlogits, P.d.n_outputs, act_of(P, cx, gL), cx.st));
+    return OK;
+  });
+  if (pbl >= 0) emit_bias_grad(P, pbl, gL, d.n_outputs);
+  std::vector<TRef> dcat(L - 1);
+  TRef g = gL;
+  for (int i = 0; i + 1 < L; ++i) {
+    dcat[i] = unet_up_bwd(P, up[i], g);
+    if (i + 2 < L) g = slice(dcat[i], F[i], F[i]);
+  }
+  TRef gdown = unet_down_bwd(P, bottom, slice(dcat[L - 2], F[L - 2], F[L - 1]), kNone);
+  for (int i = L - 2; i >= 0; --i) gdown = unet_down_bwd(P, down[i], slice(dcat[i], 0, F[i]), gdown);
+  emit_unpack_wgrads(P);
+  return finish_build(P);
+}
 
 // runs ops [first, last) of a schedule.  B200UNET_CAPTURE_DEBUG=1: after every op, check whether it invalidated an ongoing
 // CUDA-graph capture of the stream, and name it if so.

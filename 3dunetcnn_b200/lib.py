@@ -76,7 +76,8 @@ class NetDesc(C.Structure):
                 ("use_transposed_convolutions", C.c_int32), ("activation", C.c_int32),
                 ("split_precision", C.c_int32), ("batch", C.c_int32), ("depth", C.c_int32), ("height", C.c_int32),
                 ("width", C.c_int32), ("arch", C.c_int32), ("filters", C.c_int32 * 8), ("act_slope", C.c_float),
-                ("deterministic", C.c_int32), ("inference_only", C.c_int32), ("input_grad", C.c_int32)]
+                ("deterministic", C.c_int32), ("inference_only", C.c_int32), ("input_grad", C.c_int32),
+                ("num_res_units", C.c_int32), ("act_kind", C.c_int32), ("norm_affine", C.c_int32), ("conv_bias", C.c_int32)]
 
 
 class SurfaceMask(C.Structure):
@@ -147,6 +148,12 @@ _SIGS = {
                                        C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200unet_act_bwd": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_float,
                                    C.POINTER(Tensor5), C.c_void_p, C.c_int, C.c_void_p]),
+    "b200unet_prelu_apply": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                       C.c_float, C.c_void_p, C.POINTER(Tensor5), C.c_void_p, C.c_void_p]),
+    "b200unet_prelu_bwd_scratch_bytes": (C.c_size_t, [C.POINTER(Tensor5)]),
+    "b200unet_prelu_bwd": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_void_p,
+                                     C.POINTER(Tensor5), C.c_void_p, C.c_int, C.POINTER(Tensor5), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200unet_logits_unpack": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "b200unet_tiles_gather": (C.c_int, [C.c_void_p] + [C.c_int] * 5 + [C.POINTER(C.c_int32), C.c_int, C.c_int, C.c_int, C.c_int,
                                         C.c_void_p, C.c_void_p]),
     "b200unet_tiles_scatter": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.c_int, C.c_int, C.c_int, C.c_int,
@@ -532,6 +539,40 @@ def act_bwd(g1: Act, g2: Optional[Act], c: Act, coef, slope: float, dz: Act, bst
     b = g2.ct() if g2 is not None else None
     check(load_library().b200unet_act_bwd(C.byref(g1.ct()), C.byref(b) if b is not None else None, C.byref(c.ct()), coef.data_ptr(),
                                           slope, C.byref(dz.ct()), bstats.data_ptr(), bstats_ld, stream_ptr()), "act_bwd")
+
+
+def _opt(a: Optional[Act]):
+    """(keep-alive, pointer) of an optional view"""
+    t = a.ct() if a is not None else None
+    return t, (C.byref(t) if t is not None else None)
+
+
+def prelu_apply(x: Act, y: Act, stats, gamma, beta, c, groups, coef, slope: torch.Tensor, add: Optional[Act] = None,
+                eps=1e-5) -> None:
+    """y = PReLU(GroupNorm(x)) (+ add) with the slope read from the device scalar ``slope``; writes coef [n][x.c][4]"""
+    _, pa = _opt(add)
+    check(load_library().b200unet_prelu_apply(C.byref(x.ct()), C.byref(y.ct()), stats.data_ptr(), _p(gamma), _p(beta), c, groups, eps,
+                                              slope.data_ptr(), pa, coef.data_ptr(), stream_ptr()), "prelu_apply")
+
+
+def prelu_bwd(g1: Act, g2: Optional[Act], c: Act, coef, slope: torch.Tensor, dz: Act, bstats, bstats_ld: int, dslope: torch.Tensor,
+              gsum: Optional[Act] = None) -> None:
+    """act_bwd with the device slope; dslope[0] = sum over z <= 0 of z * (g1 [+ g2]); gsum = g1 [+ g2] when given"""
+    lib = load_library()
+    t = c.ct()
+    scratch = torch.empty(int(lib.b200unet_prelu_bwd_scratch_bytes(C.byref(t))), dtype=torch.uint8, device=c.hi.device)
+    _, p2 = _opt(g2)
+    _, pg = _opt(gsum)
+    check(lib.b200unet_prelu_bwd(C.byref(g1.ct()), p2, C.byref(t), coef.data_ptr(), slope.data_ptr(), C.byref(dz.ct()),
+                                 bstats.data_ptr(), bstats_ld, pg, dslope.data_ptr(), scratch.data_ptr(), stream_ptr()), "prelu_bwd")
+
+
+def logits_unpack(x: Act, c_real: int, bias: Optional[torch.Tensor] = None, add: Optional[Act] = None) -> torch.Tensor:
+    """NCDHW fp32 [n][c_real] = x (+ bias) (+ add) from the padded conv result x (hi + lo)"""
+    y = torch.empty((x.n, c_real, x.d, x.h, x.w), dtype=torch.float32, device=x.hi.device)
+    _, pa = _opt(add)
+    check(load_library().b200unet_logits_unpack(C.byref(x.ct()), pa, _p(bias), c_real, y.data_ptr(), stream_ptr()), "logits_unpack")
+    return y
 
 
 def upsample2x_fwd(x: Act, y: Act, stats=None, stats_ld=0, add: Optional[Act] = None) -> None:

@@ -689,8 +689,168 @@ class SegResNet(_PlanModel):
         return nd
 
 
+def _layer_spec(v, what):
+    """MONAI's Act / Norm spelling (an enum member, "name" or ("name", {kwargs})) -> (lower-case name, kwargs)"""
+    if isinstance(v, (tuple, list)) and len(v) == 2 and isinstance(v[1], dict):
+        name, kw = v[0], dict(v[1])
+    elif isinstance(v, (tuple, list)) and len(v) == 1:
+        name, kw = v[0], {}
+    else:
+        name, kw = v, {}
+    name = getattr(name, "value", name)
+    if not isinstance(name, str):
+        raise NotImplementedError("B200 UNet: %s=%r (a name or a (name, kwargs) pair)" % (what, v))
+    return name.lower(), kw
+
+
+class UNet(_PlanModel):
+    """Drop-in for ``monai.networks.nets.UNet`` (the network of MONAI's 3D segmentation tutorials), which the reference builds
+    by name through the ``from monai.networks.nets import *`` in unet3d/models/pytorch/__init__.py:1.
+
+    MONAI's kwargs; implemented: ``spatial_dims=3``, every stride 2, ``kernel_size=3``, ``up_kernel_size=3``, 2..8 levels of
+    ``channels`` that are multiples of 8 up to 1024, ``in_channels`` and ``out_channels`` 1..16, any ``num_res_units``, ``bias``,
+    ``act`` PReLU (one parameter), ReLU or LeakyReLU, ``norm`` instance (affine or not), ``dropout`` 0 / None and
+    ``adn_ordering="NDA"``.  Anything else raises NotImplementedError (BatchNorm needs running statistics the plans do not keep
+    yet).  State-dict keys and order are MONAI's (model.0 / model.1.submodule... / model.2), so MONAI checkpoints load with
+    ``strict=True`` (parity with MONAI itself is unpinned: it is absent from this image)."""
+
+    def __init__(self, spatial_dims=3, in_channels=1, out_channels=2, channels=(16, 32, 64, 128, 256), strides=(2, 2, 2, 2),
+                 kernel_size=3, up_kernel_size=3, num_res_units=0, act="PRELU", norm="INSTANCE", dropout=0.0, bias=True,
+                 adn_ordering="NDA", precision: Optional[str] = None, deterministic: Optional[bool] = None):
+        super().__init__()
+        channels, strides = list(channels), list(strides)
+        if len(channels) < 2:
+            raise ValueError("the length of `channels` should be no less than 2.")
+        if len(strides) < len(channels) - 1:
+            raise ValueError("the length of `strides` should equal to `len(channels) - 1`.")
+        strides = strides[:len(channels) - 1]   # MONAI warns and ignores the extra strides
+        if spatial_dims != 3:
+            raise NotImplementedError("B200 UNet: spatial_dims=%r (only 3)" % (spatial_dims,))
+
+        def all_two(v):
+            return all((e == 2 if isinstance(e, int) else list(e) == [2, 2, 2]) for e in v)
+        if not all_two(strides):
+            raise NotImplementedError("B200 UNet: strides=%r (only stride 2 at every level)" % (strides,))
+        for name, k in (("kernel_size", kernel_size), ("up_kernel_size", up_kernel_size)):
+            if not (k == 3 or (not isinstance(k, int) and list(k) == [3, 3, 3])):
+                raise NotImplementedError("B200 UNet: %s=%r (only 3)" % (name, k))
+        if not 2 <= len(channels) <= 8:
+            raise NotImplementedError("B200 UNet: %d levels (2..8)" % len(channels))
+        if any(c % 8 or c < 8 or c > 1024 for c in channels):
+            raise NotImplementedError("B200 UNet: channels=%r (multiples of 8 up to 1024)" % (channels,))
+        if not 1 <= in_channels <= 16 or not 1 <= out_channels <= 16:
+            raise NotImplementedError("B200 UNet: in_channels=%r out_channels=%r (1..16 each)" % (in_channels, out_channels))
+        if int(num_res_units) < 0:
+            raise NotImplementedError("B200 UNet: num_res_units=%r" % (num_res_units,))
+        if dropout not in (None, 0, 0.0):
+            raise NotImplementedError("B200 UNet: dropout=%r (only 0 / None)" % (dropout,))
+        if str(adn_ordering).upper() != "NDA":
+            raise NotImplementedError("B200 UNet: adn_ordering=%r (only 'NDA')" % (adn_ordering,))
+        norm_type, norm_kw = _layer_spec(norm, "norm")
+        if norm_type != "instance":
+            raise NotImplementedError("B200 UNet: norm=%r (only instance norm; BatchNorm is not implemented yet)" % (norm,))
+        affine = bool(norm_kw.pop("affine", False))
+        if float(norm_kw.pop("eps", 1e-5)) != 1e-5 or norm_kw.pop("track_running_stats", False) or norm_kw:
+            raise NotImplementedError("B200 UNet: norm options %r (only affine, eps 1e-5)" % (norm,))
+        act_type, act_kw = _layer_spec(act, "act")
+        act_kw.pop("inplace", None)
+        self.prelu_init = 0.25
+        if act_type == "prelu":
+            if int(act_kw.pop("num_parameters", 1)) != 1:
+                raise NotImplementedError("B200 UNet: act=%r (per-channel PReLU is not implemented)" % (act,))
+            self.prelu_init = float(act_kw.pop("init", 0.25))
+            act_kind, slope = 1, 0.0
+        elif act_type == "relu":
+            act_kind, slope = 0, 0.0
+        elif act_type == "leakyrelu":
+            act_kind, slope = 0, float(act_kw.pop("negative_slope", 0.01))
+        else:
+            raise NotImplementedError("B200 UNet: act=%r (only prelu / relu / leakyrelu)" % (act,))
+        if act_kw:
+            raise NotImplementedError("B200 UNet: act options %r" % (act,))
+        self.spatial_dims = 3
+        self.in_channels, self.out_channels = int(in_channels), int(out_channels)
+        self.n_features, self.n_outputs = self.in_channels, self.out_channels
+        self.channels, self.strides = [int(c) for c in channels], strides
+        self.num_res_units = int(num_res_units)
+        self.act_kind, self.act_slope = act_kind, slope
+        self.norm_affine = affine
+        self.bias = bool(bias)
+        self._setup(precision, deterministic)
+
+    def _param_spec_cpu(self):
+        ch, L, r = self.channels, len(self.channels), self.num_res_units
+        spec = []
+
+        def conv(pre, ci, co, transposed=False, conv_only=False):
+            spec.append((pre + ".conv.weight", (ci, co, 3, 3, 3) if transposed else (co, ci, 3, 3, 3)))
+            if self.bias:
+                spec.append((pre + ".conv.bias", (co,)))
+            if conv_only:
+                return
+            if self.norm_affine:
+                spec.extend([(pre + ".adn.N.weight", (co,)), (pre + ".adn.N.bias", (co,))])
+            if self.act_kind == 1:
+                spec.append((pre + ".adn.A.weight", (1,)))
+
+        def down(pre, ci, co, stride):
+            if r == 0:
+                return conv(pre, ci, co)
+            for u in range(r):
+                conv("%s.conv.unit%d" % (pre, u), ci if u == 0 else co, co)
+            if stride != 1 or ci != co:
+                k = 3 if stride != 1 else 1
+                spec.append((pre + ".residual.weight", (co, ci, k, k, k)))
+                if self.bias:
+                    spec.append((pre + ".residual.bias", (co,)))
+
+        def level(i):
+            pre = "model." + "1.submodule." * i
+            inc = self.in_channels if i == 0 else ch[i - 1]
+            outc = self.out_channels if i == 0 else ch[i - 1]
+            down(pre + "0", inc, ch[i], 2)
+            if i + 2 < L:
+                level(i + 1)
+                upc = 2 * ch[i]
+            else:
+                down(pre + "1.submodule", ch[i], ch[L - 1], 1)
+                upc = ch[i] + ch[L - 1]
+            if r == 0:
+                conv(pre + "2", upc, outc, transposed=True, conv_only=i == 0)
+            else:
+                conv(pre + "2.0", upc, outc, transposed=True)
+                conv(pre + "2.1.conv.unit0", outc, outc, conv_only=i == 0)
+        level(0)
+        return spec
+
+    def _init_tensor(self, key, t, shapes):
+        """torch's defaults: conv weights and biases U(+-1/sqrt(fan_in)) (a transposed conv's fan_in is weight.size(1) * k^3 as
+        well), InstanceNorm affine 1 / 0, PReLU at its init (0.25 unless act gives one)"""
+        if key.endswith(".adn.A.weight"):
+            nn.init.constant_(t, self.prelu_init)
+        else:
+            super()._init_tensor(key, t, shapes)
+
+    @staticmethod
+    def _is_norm_key(key):
+        return ".adn.N." in key
+
+    def _net_desc(self, n, d, h, w) -> _lib.NetDesc:
+        nd = super()._net_desc(n, d, h, w)
+        nd.arch = 3
+        nd.n_levels = len(self.channels)
+        for i, c in enumerate(self.channels):
+            nd.filters[i] = c
+        nd.act_slope = self.act_slope
+        nd.num_res_units = self.num_res_units
+        nd.act_kind = self.act_kind
+        nd.norm_affine = int(self.norm_affine)
+        nd.conv_bias = int(self.bias)
+        return nd
+
+
 _MODELS = {"UNet3D": UNet3D, "AutocastUNet": AutocastUNet, "AutoImplantUNet": AutoImplantUNet,
-           "B200UNet3D": UNet3D, "DynUNet": DynUNet, "SegResNet": SegResNet}
+           "B200UNet3D": UNet3D, "DynUNet": DynUNet, "SegResNet": SegResNet, "UNet": UNet}
 
 
 def fetch_model_by_name(model_name, *args, **kwargs):

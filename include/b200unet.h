@@ -112,6 +112,29 @@ int b200unet_gn_bwd_finalize(const double* bstats, const float* coef, const floa
 int b200unet_act_bwd(const b200unet_tensor* g1, const b200unet_tensor* g2, const b200unet_tensor* c, const float* coef, float slope,
                      const b200unet_tensor* dz, double* bstats, int bstats_ld, void* stream);
 
+/* ---- MONAI UNet's learnable PReLU (nn.PReLU(num_parameters=1)) after an instance norm, the slope read from the DEVICE fp32
+ * scalar `slope` (the parameter itself, so a captured CUDA graph sees every optimizer step's value).
+ *   prelu_apply:   gn_apply with act(z) = z > 0 ? z : slope[0] * z, then y = act(z) + add (add: y's shape or NULL; MONAI's
+ *                  ResidualUnit output conv(x) + residual(x), the addend read as hi + lo and the sum stored as y's hi [+ lo]).
+ *   prelu_bwd:     act_bwd with the same slope; also dslope[0] = sum over z <= 0 of z * (g1 [+ g2]) (written), z = A c + B the
+ *                  normalised, affine-applied pre-activation, from per-block partial sums added in a fixed order: bit-identical run
+ *                  to run.  scratch: prelu_bwd_scratch_bytes(c).  gsum (optional, c's shape): gsum = g1 [+ g2], the gradient
+ *                  a residual branch takes as well. */
+int b200unet_prelu_apply(const b200unet_tensor* x, const b200unet_tensor* y, const double* stats, const float* gamma,
+                         const float* beta, int c, int groups, float eps, const float* slope, const b200unet_tensor* add, float* coef,
+                         void* stream);
+size_t b200unet_prelu_bwd_scratch_bytes(const b200unet_tensor* c);
+int b200unet_prelu_bwd(const b200unet_tensor* g1, const b200unet_tensor* g2, const b200unet_tensor* c, const float* coef,
+                       const float* slope, const b200unet_tensor* dz, double* bstats, int bstats_ld, const b200unet_tensor* gsum,
+                       float* dslope, float* scratch, void* stream);
+
+/* ---- logits of a network whose last layer is a convolution (MONAI UNet): logits NCDHW fp32 [n][c_real][d][h][w] =
+ * in + bias (+ add) over the first c_real channels of the padded conv result `in` (read as hi + lo); bias DEVICE fp32 [c_real]
+ * or NULL; add (in's shape) or NULL: the top residual unit's identity branch, logits = conv(y) + bias + y.  The matching
+ * backward pack of dlogits into the padded NDHWC layout is b200unet_ncdhw_to_ndhwc. */
+int b200unet_logits_unpack(const b200unet_tensor* in, const b200unet_tensor* add, const float* bias, int c_real, float* logits,
+                           void* stream);
+
 /* ---- F.interpolate(scale_factor=2, mode="trilinear", align_corners=False) (decoder.py:105-106), fwd + adjoint.
  * add_fwd: y = upsample(x) + add in one pass (MONAI SegResNet's `up(x) + skip`), add of y's shape (NULL = upsample_fwd); the
  * statistics are those of y.  The gradient of the sum reaches add unchanged and x through upsample2x_bwd. */
@@ -358,13 +381,22 @@ typedef struct b200unet_net_desc {
   int32_t input_grad;         /* 1 = the plan can also produce d(loss)/d(x) (b200unet_plan_input_grad): saliency maps, adversarial
                                  training, cascades whose input comes from a differentiable stage.  Costs the forward only the data-
                                  gradient weight packs of the first block's convolutions.  Rejected with inference_only = 1. */
+  /* arch 3 = MONAI UNet (monai/networks/nets/unet.py): n_levels = len(channels) (2..8), filters = channels (multiples of 8 up
+   * to 1024), every stride 2, kernel_size = up_kernel_size = 3, InstanceNorm3d (eps 1e-5) and the activation after every conv
+   * but the last; n_features = in_channels 1..16, n_outputs = out_channels 1..16, activation 0.  The fields below are arch 3's
+   * alone (zero elsewhere). */
+  int32_t num_res_units;      /* 0: Convolution layers; r > 0: ResidualUnit(subunits = r) down layers and up layers followed by a
+                                 one-subunit ResidualUnit */
+  int32_t act_kind;           /* 0: act_slope (0 ReLU, else LeakyReLU); 1: PReLU with one learnable slope per layer (adn.A.weight) */
+  int32_t norm_affine;        /* 1: the instance norms have a weight and a bias (adn.N.weight / .bias) */
+  int32_t conv_bias;          /* 1: every convolution has a bias (MONAI's bias=True) */
 } b200unet_net_desc;
 
 typedef struct b200unet_plan b200unet_plan;
 
 int b200unet_plan_create(const b200unet_net_desc* desc, b200unet_plan** out);
 void b200unet_plan_destroy(b200unet_plan* plan);
-/* number of parameter tensors, in reference state_dict order (SURVEY.md appendix B; arch 1 and 2: MONAI's registration order) */
+/* number of parameter tensors, in reference state_dict order (SURVEY.md appendix B; arch 1, 2 and 3: MONAI's registration order) */
 int b200unet_plan_num_params(const b200unet_plan* plan);
 /* shape (up to 5 dims, zero padded) and state_dict key of parameter i */
 int b200unet_plan_param_info(const b200unet_plan* plan, int i, int64_t shape[5], char* key, int key_cap);
