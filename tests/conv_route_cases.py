@@ -93,11 +93,12 @@ def conv_geometry(op, cin, dims):
     raise ValueError(op)
 
 
-def conv_query(L, op, cin, cout, dims, split=False, mode=0, cin2=0, n=2):
-    """route of a convolution of this shape (host-only); None when the library refuses the combination"""
+def conv_query(L, op, cin, cout, dims, split=False, mode=0, cin2=0, n=2, lo_out=False):
+    """route of a convolution of this shape (host-only); None when the library refuses the combination.  The output has a lo
+    plane in split precision, and with lo_out also for bf16 operands (the fp32 accumulators stored as hi + lo)."""
     sdims, ksz, stride, cls = conv_geometry(op, cin, dims)
     x = ShapeAct(L, n, *sdims, cin, split)
-    out = ShapeAct(L, n, *dims, cout, split)
+    out = ShapeAct(L, n, *dims, cout, split or lo_out)
     w = Addr()
     wl = Addr() if split else None
     kw = dict(cls_mode=cls, mode=mode)

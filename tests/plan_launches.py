@@ -34,6 +34,7 @@ class Launch:
     macs_div: int = 1            # conv_role's macs_div, for a transposed layer launched over its output grid
     view: bool = False           # bandwidth kernels: the up-sampling's full-resolution operand is a channel slice of a concat
     variant: Optional[str] = None   # gn of a training plan: what k_gn_bwd adds and scales ("plain", "add1", "add1+scale")
+    lo_out: bool = False         # conv: the output has a lo plane in bf16 plans too (plan.cu: new_buf's force_lo)
 
     def macs(self):
         """the algorithmic MACs the plan counts for a convolution (plan.cu: conv_macs): on the grid of the layer's output (data
@@ -49,7 +50,7 @@ def pad8(c):
 
 def conv_route(L, l, split):
     """the library's route of a forward or data-gradient launch (conv_route_cases.conv_query)"""
-    return R.conv_query(L, l.op, pad8(l.c), pad8(l.co), l.dims, split, l.mode, pad8(l.c2), n=l.n)
+    return R.conv_query(L, l.op, pad8(l.c), pad8(l.co), l.dims, split, l.mode, pad8(l.c2), n=l.n, lo_out=l.lo_out)
 
 
 def wgrad_route(L, l, split):

@@ -1,5 +1,5 @@
-"""Every kernel route of the convolution and the weight gradient (tests/conv_route_cases.py), and the deep K loops of the wide
-layers, against an fp64 reference, element by element.  Each case first checks through the host query that it still takes its route, then launches it on inputs the
+"""Every kernel route of the convolution and the weight gradient (tests/conv_route_cases.py), the deep K loops of the wide
+layers, and the bf16 convolution with a hi + lo output (MONAI UNet's logits), against an fp64 reference, element by element.  Each case first checks through the host query that it still takes its route, then launches it on inputs the
 reference reads exactly (bf16 hi, or hi + lo, as stored), and bounds every element by
 
     |got - ref| <= r * |ref| + a * (|x| conv |w|)
@@ -235,6 +235,59 @@ def test_deep_k_conv_matches_fp64(L, case):
     else:
         for slope in (0.0, 0.01):
             run_mode1(L, case, gen, slope)
+
+
+# ------------------------------------------------------------------------------------------ bf16 operands, hi + lo output
+# The conv that writes MONAI UNet's logits reads bf16 operands and stores its fp32 accumulators as hi + lo (plan.cu: new_buf's
+# force_lo): (source channels, output view, real outputs, output extents, transposed).  The k3s1 convs of the residual-unit top
+# layer, and the conv-only transposed top layer (zero-inserted grid, mode-2 flipped pack), on planes that fill the halo tile.
+LO_OUT_CASES = [(8, 8, 2, R.H, False), (32, 8, 2, R.H, False), (32, 8, 2, (4, 18, 10), True)]
+
+
+def bf16_ulp(hi):
+    """the spacing of bf16 values at |hi| (hi != 0)"""
+    return torch.ldexp(torch.ones_like(hi), torch.frexp(hi)[1] - 8)
+
+
+@pytest.mark.parametrize("cin,cout,real_out,dims,transposed", LO_OUT_CASES,
+                         ids=["k3s1-%dto%d%s" % (c[0], c[2], "-transposed" if c[4] else "") for c in LO_OUT_CASES])
+def test_bf16_conv_with_lo_output_matches_fp64(L, cin, cout, real_out, dims, transposed):
+    """hi + lo at the fp32 accumulation bound, not a bf16 one; hi the bf16 rounding of hi + lo; the padded output channels
+    zero in both planes; per-tap tiles, where the same conv without the lo plane runs on halo tiles"""
+    n = 2
+    gen = torch.Generator().manual_seed(cin + 1000 * transposed)
+    if transposed:     # ConvTranspose3d(k3, s2, p1, output_padding 1): zero insertion, then a k3 s1 conv with the mode-2 pack
+        xs, xv = rand_act(L, n, cin, tuple(e // 2 for e in dims), False, gen)
+        x = L.Act.empty(n, *dims, cin)
+        L.zero_insert(xs, x)
+        w = (torch.randn(cin, real_out, 3, 3, 3, generator=gen) / (cin * 27) ** 0.5).bfloat16().float()
+        whi = L.pack_weights(w.to(DEV), 2, cop=cout, cip=cin)[0]
+        acc = F.conv_transpose3d(xv, w.double(), stride=2, padding=1, output_padding=1)
+        absacc = F.conv_transpose3d(xv.abs(), w.double().abs(), stride=2, padding=1, output_padding=1)
+    else:
+        x, xv = rand_act(L, n, cin, dims, False, gen)
+        w = (torch.randn(real_out, cin, 3, 3, 3, generator=gen) / (cin * 27) ** 0.5).bfloat16().float()
+        whi = L.pack_weights(w.to(DEV), 0, cop=cout)[0]
+        acc = F.conv3d(xv, w.double(), padding=1)
+        absacc = F.conv3d(xv.abs(), w.double().abs(), padding=1)
+    y = L.Act.empty(n, *dims, cout, split=True)
+    y.hi.fill_(SENTINEL)
+    y.lo.fill_(SENTINEL / 256)
+    assert L.conv3d_route(x, whi, None, 3, 1, L.Act(y.hi), cout, cin)["kind"] == "halo"
+    r = L.conv3d_route(x, whi, None, 3, 1, y, cout, cin)
+    assert (r["kind"], r["npass"]) == ("tap", 1), r
+    L.conv3d(x, whi, None, 3, 1, y, cout, cin)
+    torch.cuda.synchronize()
+    check_elements(view_value(y)[:, :real_out], acc, A_ACC * absacc, R_STORE[True], "hi + lo")
+    assert not y.hi[..., real_out:].any() and not y.lo[..., real_out:].any(), "padded output channels"
+    hi, lo = y.hi[..., :real_out].float(), y.lo[..., :real_out].float()
+    nz = hi != 0
+    assert not lo[~nz].any(), "lo beside a zero hi"
+    half = 0.5 * bf16_ulp(hi[nz])
+    assert bool((lo[nz].abs() <= half).all()), "|lo| above half a bf16 ulp of hi"
+    # hi + lo is exact in fp32; it rounds back to hi except at a tie (|lo| exactly half an ulp), where hi may be the odd neighbour
+    back = (hi + lo).bfloat16().float()
+    assert bool(((back == hi) | (lo.abs() == 0.5 * bf16_ulp(hi.masked_fill(~nz, 1.0)))).all()), "hi is not bf16(hi + lo)"
 
 
 # -------------------------------------------------------------------------------------------------- plan-only conv options
