@@ -227,7 +227,7 @@ static DiceCEDesc to_dice_ce(const b200unet_dice_ce_desc* d) {
   r.smooth_nr = d->smooth_nr; r.smooth_dr = d->smooth_dr; r.lambda_dice = d->lambda_dice; r.lambda_ce = d->lambda_ce;
   r.overlap = d->overlap; r.tversky_alpha = d->tversky_alpha; r.tversky_beta = d->tversky_beta; r.w_type = d->w_type;
   r.voxel_term = d->voxel_term; r.focal_softmax = d->focal_softmax; r.focal_gamma = d->focal_gamma; r.focal_alpha = d->focal_alpha;
-  r.focal_use_alpha = d->focal_use_alpha; r.class_weight = d->class_weight;
+  r.focal_use_alpha = d->focal_use_alpha; r.class_weight = d->class_weight; r.hdt_weight = d->hdt_weight;
   return r;
 }
 int b200unet_dice_fwd(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c, int64_t spatial,
@@ -253,6 +253,23 @@ int b200unet_dice_ce_bwd(const b200unet_dice_ce_desc* desc, const float* logits,
                          const void* scratch, const float* grad_out, float* dlogits, void* stream) {
   NOT_NULL(desc); NOT_NULL(logits); NOT_NULL(target); NOT_NULL(scratch); NOT_NULL(grad_out); NOT_NULL(dlogits);
   return launch_dice_ce_bwd(to_dice_ce(desc), logits, target, n, c, spatial, scratch, grad_out, dlogits, to_stream(stream));
+}
+
+size_t b200unet_hausdorff_dt_scratch_bytes(const b200unet_dice_ce_desc* desc, int n, int c, int d, int h, int w) {
+  if (!desc) { set_error("%s: null argument desc", __func__); return 0; }
+  return hausdorff_dt_scratch_bytes(to_dice_ce(desc), n, c, d, h, w);
+}
+int b200unet_hausdorff_dt_weight(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c, int d, int h,
+                                 int w, float alpha, void* scratch, float* weight, void* stream) {
+  NOT_NULL(desc); NOT_NULL(logits); NOT_NULL(target); NOT_NULL(scratch); NOT_NULL(weight);
+  return launch_hausdorff_dt_fields(to_dice_ce(desc), logits, target, n, c, d, h, w, alpha, scratch, weight, nullptr, nullptr,
+                                    to_stream(stream));
+}
+int b200unet_diag_hausdorff_dt_fields(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c, int d,
+                                      int h, int w, void* scratch, float* pred_field, float* target_field, void* stream) {
+  NOT_NULL(desc); NOT_NULL(logits); NOT_NULL(target); NOT_NULL(scratch);
+  return launch_hausdorff_dt_fields(to_dice_ce(desc), logits, target, n, c, d, h, w, 1.f, scratch, nullptr, pred_field, target_field,
+                                    to_stream(stream));
 }
 
 int b200unet_tiles_gather(const float* vol, int n, int c, int d, int h, int w, const int32_t* starts, int ntiles, int rd, int rh,

@@ -227,7 +227,8 @@ int check_dice_desc(const DiceCEDesc& d, int N, int C, long long S, const char* 
   B200_REQUIRE(d.overlap == O_DICE || (!d.squared_pred && !d.jaccard), E_INVALID,
                "%s: squared_pred / jaccard apply to the Dice overlap only (overlap=%d)", who, d.overlap);
   B200_REQUIRE(d.w_type >= 0 && d.w_type <= 2, E_INVALID, "%s: w_type=%d (0 square, 1 simple, 2 uniform)", who, d.w_type);
-  B200_REQUIRE(d.voxel_term == V_CE || d.voxel_term == V_FOCAL, E_INVALID, "%s: voxel_term=%d (0 CE, 1 focal)", who, d.voxel_term);
+  B200_REQUIRE(d.voxel_term >= V_CE && d.voxel_term <= V_HDT, E_INVALID, "%s: voxel_term=%d (0 CE, 1 focal, 2 distance-weighted)", who,
+               d.voxel_term);
   B200_REQUIRE(d.focal_gamma >= 0.f, E_INVALID, "%s: focal_gamma=%g (>= 0)", who, d.focal_gamma);
   return OK;
 }

@@ -13,6 +13,9 @@
 //   include_background keeps.  Sigmoid form per element, softmax form over the kept channels -- under include_background = 0
 //   a softmax Dice takes its softmax over all C channels and the focal term over 1..C-1, so a voxel then needs both sums of
 //   exponentials.  The focal term leaves the raw logits in the staged tile (a softmax Dice recomputes exp(x - max)).
+//   monai.losses.HausdorffDTLoss runs the distance-weighted term alone (lambda_dice = 0): (p_c - t_c)^2 w_c on the kept
+//   channels, p = act(x), with the weights w = pdt^alpha + tdt^alpha of hausdorff_dt.cu read per voxel; its gradient
+//   2 (p_c - t_c) w_c goes through the activation Jacobian as the Dice part's does.
 // A label outside [0, C) is an all-zero target row: it adds nothing to I, T or CE and is never used as an index.
 //
 // Logits are NCDHW fp32, so every channel of a sample is a contiguous run of S floats.  Both passes stage a tile of kV voxels x
@@ -25,7 +28,7 @@
 //   backward: thread v of the tile: g_c = a_nc t_c + b_nc dP/dp_c from the coefficients, the activation Jacobian
 //             (softmax: p_c (g_c - sum_k p_k g_k)) and the CE gradient cg (q_c sum_k t_k - t_c); dlogits written coalesced.
 // HBM bytes: forward N*S*(4C + b_t), backward N*S*(8C + b_t), b_t = target bytes per voxel (1 / 8 for uint8 / int64 label maps,
-// C / 4C for uint8 / fp32 C-channel targets).
+// C / 4C for uint8 / fp32 C-channel targets); the distance-weighted term reads 4C' more per voxel in each.
 #include <type_traits>
 
 #include "kernels.h"
@@ -49,14 +52,15 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 
 __device__ __forceinline__ float sigm(float x) { return 1.f / (1.f + __expf(-x)); }
 
-// The per-voxel term of a launch (uniform): none (lambda_ce = 0), CE, or focal in either form
-enum VoxKind { VX_NONE = 0, VX_CE = 1, VX_FOCAL_SIG = 2, VX_FOCAL_SMX = 3 };
+// The per-voxel term of a launch (uniform): none (lambda_ce = 0), CE, focal in either form, or distance-weighted
+enum VoxKind { VX_NONE = 0, VX_CE = 1, VX_FOCAL_SIG = 2, VX_FOCAL_SMX = 3, VX_HDT = 4 };
 struct Vox {
   int kind;          // VoxKind
-  int lo;            // focal: first kept channel (1 when include_background = 0 drops channel 0 of a C > 1 input)
+  int lo;            // focal, distance-weighted: first kept channel (1 when include_background = 0 drops channel 0 of a C > 1 input)
   float gamma, alpha;
   int use_alpha;
   const float* w;    // focal: [C - lo] class factors or nullptr
+  const float* hdt;  // distance-weighted: [N][C - lo][S] weights
 };
 
 // focal class factor of channel c (the softmax form's alpha folded in); 0 on a dropped channel
@@ -111,6 +115,65 @@ __device__ __forceinline__ float lse_from1(const float* xs, int C, int v) {
   for (int k = 1; k < C; ++k) m = fmaxf(m, xs[k * kP + v]);
   for (int k = 1; k < C; ++k) sum += __expf(xs[k * kP + v] - m);
   return m + logf(sum);
+}
+
+// act(x) of channel k of voxel v of the staged tile; softmax: m and inv are the voxel's maximum and 1 / sum of exponentials
+template <int ACT>
+__device__ __forceinline__ float act_prob(float r, float m, float inv) {
+  return ACT == A_SOFTMAX ? __expf(r - m) * inv : ACT == A_SIGMOID ? sigm(r) : r;
+}
+
+// the distance-weighted term: softmax statistics of voxel v over all C channels (the tile keeps the raw logits)
+template <int ACT>
+__device__ __forceinline__ void hdt_softmax(const float* xs, int C, int v, float* m, float* inv) {
+  *m = -INFINITY;
+  *inv = 0.f;
+  if constexpr (ACT == A_SOFTMAX) {
+    for (int k = 0; k < C; ++k) *m = fmaxf(*m, xs[k * kP + v]);
+    float sum = 0.f;
+    for (int k = 0; k < C; ++k) sum += __expf(xs[k * kP + v] - *m);
+    *inv = 1.f / sum;
+  }
+}
+
+// sum over the kept channels of (p_c - t_c)^2 w_c at voxel v; wv: the voxel's weight of the first kept channel, channel stride S
+template <int TK, int ACT>
+__device__ __forceinline__ float hdt_term(const float* xs, const float* ts, const int* lab, int C, int v, int lo, const float* wv,
+                                          long long S) {
+  float m, inv;
+  hdt_softmax<ACT>(xs, C, v, &m, &inv);
+  const int l = TK < T_ONEHOT_U8 ? lab[v] : -1;
+  float f = 0.f;
+  for (int k = lo; k < C; ++k) {
+    const float e = act_prob<ACT>(xs[k * kP + v], m, inv) - (TK >= T_ONEHOT_U8 ? ts[k * kP + v] : (k == l ? 1.f : 0.f));
+    f += e * e * __ldg(wv + (long long)(k - lo) * S);
+  }
+  return f;
+}
+
+// dlogits of the distance-weighted term at voxel v: g_c = cg 2 (p_c - t_c) w_c on the kept channels, through the activation
+template <int TK, int ACT>
+__device__ __forceinline__ void hdt_grad(const float* xs, const float* ts, const int* lab, int C, int v, int lo, const float* wv,
+                                         long long S, float cg, float* o) {
+  float m, inv;
+  hdt_softmax<ACT>(xs, C, v, &m, &inv);
+  const int l = TK < T_ONEHOT_U8 ? lab[v] : -1;
+  auto g_of = [&](int k, float p) -> float {
+    if (k < lo) return 0.f;
+    const float t = TK >= T_ONEHOT_U8 ? ts[k * kP + v] : (k == l ? 1.f : 0.f);
+    return cg * 2.f * (p - t) * __ldg(wv + (long long)(k - lo) * S);
+  };
+  float s = 0.f;                                   // softmax: sum_k p_k g_k
+  if (ACT == A_SOFTMAX)
+    for (int k = lo; k < C; ++k) {
+      const float p = act_prob<ACT>(xs[k * kP + v], m, inv);
+      s += p * g_of(k, p);
+    }
+  for (int k = 0; k < C; ++k) {
+    const float p = act_prob<ACT>(xs[k * kP + v], m, inv);
+    const float g = g_of(k, p);
+    o[(long long)k * S] = ACT == A_SOFTMAX ? p * (g - s) : ACT == A_SIGMOID ? g * p * (1.f - p) : g;
+  }
 }
 
 __device__ __forceinline__ double warp_sum(double v) {
@@ -200,7 +263,7 @@ __global__ void __launch_bounds__(kThreads) k_dice_ce_fwd(const float* __restric
   const int K = kThreads / C, c = tid % C, slice = tid / C;   // phase B: thread (c, slice) walks voxels slice, slice + K, ...
   // the reduction buffer is free until the end: the focal class factors, and each voxel's maximum when a focal term keeps the
   // raw logits in the tile under a softmax Dice
-  const bool keep = vx.kind >= VX_FOCAL_SIG;
+  const bool keep = vx.kind == VX_FOCAL_SIG || vx.kind == VX_FOCAL_SMX;
   float* mrow = reinterpret_cast<float*>(sm.red);
   float* fw = mrow + kV;
   if (keep)
@@ -214,7 +277,9 @@ __global__ void __launch_bounds__(kThreads) k_dice_ce_fwd(const float* __restric
     if ((vx.kind != VX_NONE || ACT == A_SOFTMAX) && tid < nv) {
       const int v = tid;
       float ce = 0.f;
-      if (C == 1) {
+      if (vx.kind == VX_HDT) {
+        ce = hdt_term<TK, ACT>(sm.xs, sm.ts, sm.lab, C, v, vx.lo, vx.hdt + (long long)n * (C - vx.lo) * S + s0 + v, S);
+      } else if (C == 1) {
         const float xv = sm.xs[v], t = sm.ts[v];
         if (vx.kind <= VX_CE) ce = fmaxf(xv, 0.f) - xv * t + log1pf(__expf(-fabsf(xv)));
         else if (vx.kind == VX_FOCAL_SIG) ce = focal_sig<TK != T_SOFT_F32>(xv, t, fw[0], vx, nullptr);
@@ -345,7 +410,7 @@ __global__ void __launch_bounds__(kThreads, 8) k_dice_ce_bwd(const float* __rest
   float* fw = b + C;                                // [C] focal class factors
   const int n = blockIdx.y, v = threadIdx.x;
   const float go = *grad_out;
-  const bool keep = vx.kind >= VX_FOCAL_SIG;        // the focal term reads the raw logits: the tile keeps them
+  const bool keep = vx.kind == VX_FOCAL_SIG || vx.kind == VX_FOCAL_SMX;   // the focal term reads the raw logits: the tile keeps them
   for (int c = v; c < C; c += kThreads) {
     a[c] = (float)(coef[((long long)n * C + c) * 2] * go);
     b[c] = (float)(coef[((long long)n * C + c) * 2 + 1] * go);
@@ -361,7 +426,9 @@ __global__ void __launch_bounds__(kThreads, 8) k_dice_ce_bwd(const float* __rest
     stage_tile<TK>(xn, tgt, n, C, S, s0, nv, sm.xs, sm.ts, sm.lab);   // its barrier also publishes a / b / fw
     if (v < nv) {
       float* o = dxn + s0 + v;
-      if (C == 1) {
+      if (vx.kind == VX_HDT) {
+        hdt_grad<TK, ACT>(sm.xs, sm.ts, sm.lab, C, v, vx.lo, vx.hdt + (long long)n * (C - vx.lo) * S + s0 + v, S, cg, o);
+      } else if (C == 1) {
         const float xv = sm.xs[v], t = sm.ts[v];
         const float q = sigm(xv);
         const float p = ACT == A_SIGMOID ? q : xv;
@@ -464,6 +531,8 @@ struct Shape {
 int check_shape(const DiceCEDesc& d, int N, int C, long long S, Shape* sh) {
   B200_TRY(check_dice_desc(d, N, C, S, "dice_ce"));
   B200_REQUIRE(C <= 128, E_UNSUPPORTED, "dice_ce: %d channels (at most 128)", C);
+  B200_REQUIRE(d.voxel_term != V_HDT || (d.lambda_dice == 0.f && d.overlap == O_DICE && !d.squared_pred && !d.jaccard), E_UNSUPPORTED,
+               "dice_ce: the distance-weighted term runs alone (lambda_dice=%g, overlap=%d)", d.lambda_dice, d.overlap);
   sh->N = N; sh->C = C; sh->S = S; sh->kind = d.target_kind; sh->act = d.act;
   if (C == 1) {
     // one channel: softmax and the label-map expansion do not apply (MONAI ignores them); a uint8 map is the uint8 target itself
@@ -478,9 +547,14 @@ int check_shape(const DiceCEDesc& d, int N, int C, long long S, Shape* sh) {
 // the per-voxel term of a launch: none when lambda_ce = 0
 Vox vox_of(const DiceCEDesc& d, int C) {
   Vox v;
-  v.kind = d.lambda_ce == 0.f ? VX_NONE : d.voxel_term == V_CE ? VX_CE : d.focal_softmax ? VX_FOCAL_SMX : VX_FOCAL_SIG;
+  v.kind = d.lambda_ce == 0.f        ? VX_NONE
+           : d.voxel_term == V_CE    ? VX_CE
+           : d.voxel_term == V_HDT   ? VX_HDT
+           : d.focal_softmax         ? VX_FOCAL_SMX
+                                     : VX_FOCAL_SIG;
   v.lo = (!d.include_background && C > 1) ? 1 : 0;
   v.gamma = d.focal_gamma; v.alpha = d.focal_alpha; v.use_alpha = d.focal_use_alpha; v.w = d.class_weight;
+  v.hdt = d.hdt_weight;
   return v;
 }
 
@@ -527,6 +601,7 @@ int launch_dice_ce_fwd(const DiceCEDesc& d, const float* logits, const void* tar
   const size_t smem = tile_smem(sh.C, sh.kind);
   const dim3 grid(sh.slots, N);
   const Vox vx = vox_of(d, C);
+  B200_REQUIRE(vx.kind != VX_HDT || vx.hdt, E_INVALID, "dice_ce: the distance-weighted term needs hdt_weight");
 #define B200_FWD(tk, ac)                                                                                                \
   B200_TRY(set_smem(k_dice_ce_fwd<tk, ac>, smem));                                                                      \
   k_dice_ce_fwd<tk, ac><<<grid, kThreads, smem, st>>>(logits, target, C, S, d.squared_pred, d.lambda_dice != 0.f, vx, s.part,  \
@@ -548,6 +623,7 @@ int launch_dice_ce_bwd(const DiceCEDesc& d, const float* logits, const void* tar
   const size_t smem = tile_smem(sh.C, sh.kind);
   const dim3 grid(sh.slots, N);
   const Vox vx = vox_of(d, C);
+  B200_REQUIRE(vx.kind != VX_HDT || vx.hdt, E_INVALID, "dice_ce: the distance-weighted term needs hdt_weight");
   const double ce_scale = d.lambda_ce * (1.0 / voxel_divisor(d, N, C, S));
 #define B200_BWD(tk, ac)                                                                                                 \
   B200_TRY(set_smem(k_dice_ce_bwd<tk, ac>, smem));                                                                       \

@@ -89,7 +89,7 @@ enum TargetKind { T_LABEL_U8 = 0, T_LABEL_I64 = 1, T_ONEHOT_U8 = 2, T_SOFT_F32 =
 enum ActKind { A_NONE = 0, A_SIGMOID = 1, A_SOFTMAX = 2 };
 enum OverlapKind { O_DICE = 0, O_TVERSKY = 1, O_GDICE = 2 };
 enum GDiceWeight { W_SQUARE = 0, W_SIMPLE = 1, W_UNIFORM = 2 };
-enum VoxelTerm { V_CE = 0, V_FOCAL = 1 };
+enum VoxelTerm { V_CE = 0, V_FOCAL = 1, V_HDT = 2 };
 struct DiceCEDesc {
   int act;               // ActKind: 0 identity, 1 sigmoid, 2 softmax over channels
   int target_kind;       // TargetKind: 0 uint8 label map [N][1][S], 1 int64 label map, 2 uint8 [N][C][S], 3 fp32 [N][C][S]
@@ -105,14 +105,17 @@ struct DiceCEDesc {
   float focal_gamma, focal_alpha;
   int focal_use_alpha;
   const float* class_weight;   // focal: DEVICE fp32 [C'] (C' = channels kept), nullptr = none
+  const float* hdt_weight;     // V_HDT: DEVICE fp32 [N][C'][S] distance weights (launch_hausdorff_dt_fields)
 };
 // the checks both criteria make: a non-empty shape and in-range options ("who" prefixes the error message)
 int check_dice_desc(const DiceCEDesc& d, int N, int C, long long S, const char* who);
 // The per-voxel term's total is divided by this: CE: N*S (mean) or 1 (sum); focal: N*C'*S (mean) or S (sum, MONAI's
-// FocalLoss averages over the voxels before it sums over samples and classes)
+// FocalLoss averages over the voxels before it sums over samples and classes); distance-weighted: as focal, and N*S for sum
+// with batch (the mean per class then runs over the samples too)
 __host__ __device__ inline double voxel_divisor(const DiceCEDesc& d, int N, int C, long long S) {
   if (d.voxel_term == V_CE) return d.reduction == 0 ? (double)N * S : 1.0;
   const int kept = (!d.include_background && C > 1) ? C - 1 : C;
+  if (d.reduction != 0 && d.voxel_term == V_HDT && d.batch) return (double)N * S;
   return d.reduction == 0 ? (double)N * kept * S : (double)S;
 }
 // The loss and coef [N][C][2] (the backward's dF/dI, dF/dP per (n, c)) from sums [N][C][3] (I, P, T) in one single-block
@@ -211,6 +214,15 @@ size_t surface_scratch_bytes(int nb, int nc, int d, int h, int w);   // 0: the s
 int launch_surface_distance(const SurfaceMask& pred, const SurfaceMask& gt, int nb, int nc, int d, int h, int w, const double* spacing,
                             float q, int hd_dirs, int asd_dirs, const float* tau, float* hd, float* asd, float* nsd, void* scratch,
                             cudaStream_t st);
+
+// ---- distance fields of the Hausdorff distance-transform loss (hausdorff_dt.cu): for each kept (n, c) the field
+// edt(mask) + edt(~mask) of the prediction mask act(x) > 0.5 and of the target mask t > 0.5 (0 for an empty or full mask), on the
+// descriptor's act, target_kind and include_background; extents 1..B200_SURFACE_MAX_EXTENT, N x C' <= B200_SURFACE_MAX_PAIRS
+size_t hausdorff_dt_scratch_bytes(const DiceCEDesc& d, int N, int C, int D, int H, int W);   // 0: the shape is rejected
+// weight != nullptr: weight [N][C'][S] = pdt^alpha + tdt^alpha (alpha > 0); else the raw fields pdt / tdt [N][C'][S] (either
+// nullptr = not computed)
+int launch_hausdorff_dt_fields(const DiceCEDesc& d, const float* logits, const void* target, int N, int C, int D, int H, int W,
+                               float alpha, void* scratch, float* weight, float* pdt, float* tdt, cudaStream_t st);
 
 // ---- overlap counts of segmentations: P, G, I per (item, class) (overlap.cu)
 #define B200_OVERLAP_MAX_CLASSES 128

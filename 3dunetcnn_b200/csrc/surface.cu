@@ -4,7 +4,7 @@
 //
 // V = B x C' pairs (prediction, ground truth) of one D x H x W extent.  Direction k = 0 is pred -> gt (queries: the edge voxels
 // of the prediction, features: the edge voxels of the ground truth), k = 1 the reverse.  Exact Euclidean distance transform,
-// separable (Felzenszwalb & Huttenlocher 2012), carrying the offsets of the nearest feature through the passes:
+// separable (Felzenszwalb & Huttenlocher 2012, edt.cuh), carrying the offsets of the nearest feature through the passes:
 //
 //   k_sf_rows     one block per row (v, d, h): fg = (value == 1), edge = fg & ~erode6(fg) for both masks (outside = background),
 //                 integer edge counts, and along W the offset to the nearest edge voxel of the row from a ballot bitmask
@@ -20,16 +20,14 @@
 //
 // Every envelope comparison is a cross-multiplication in fp64: with unit spacing all operands are integers below 2^53, so the
 // nearest feature is exact and every distance equals scipy's bit for bit.  No floating-point atomics; nothing is read back.
-#include "kernels.h"
+#include "edt.cuh"
 
 namespace b200 {
 namespace {
 
-constexpr int kColThreads = 128;                   // columns per block of the H and D passes
+using edt::kColThreads;
 constexpr int kBins = 1 << 16;                     // 16-bit digits of the two-pass select
 constexpr int kSelThreads = 256;
-constexpr int16_t kNone = 0x7fff;                  // W pass: no edge voxel in the row
-constexpr uint32_t kNone32 = 0x7fff7fffu;          // H pass: no edge voxel in the plane column
 
 struct Geo {
   int V, D, H, W, Cp;
@@ -101,87 +99,9 @@ __global__ void __launch_bounds__(B200_SURFACE_MAX_EXTENT) k_sf_rows(SurfaceMask
     if (n) atomicAdd(ecount + v * 2 + threadIdx.x, n);
   }
   if (w >= g.W) return;
-  const int i0 = w >> 5, b0 = w & 31;
-  for (int m = 0; m < 2; ++m) {
-    int left = -1, right = -1;
-    for (int i = i0; i >= 0 && left < 0; --i) {          // nearest set bit at or below w
-      const unsigned x = i == i0 ? bits[m][i] & (0xffffffffu >> (31 - b0)) : bits[m][i];
-      if (x) left = i * 32 + 31 - __clz(x);
-    }
-    for (int i = i0; i < nw && right < 0; ++i) {         // nearest set bit at or above w
-      const unsigned x = i == i0 ? bits[m][i] & (0xffffffffu << b0) : bits[m][i];
-      if (x) right = i * 32 + __ffs(x) - 1;
-    }
-    int16_t off = kNone;
-    if (left >= 0) off = (int16_t)(left - w);
-    if (right >= 0 && (left < 0 || right - w < w - left)) off = (int16_t)(right - w);
-    dw[(long long)(v * 2 + m) * g.S + ((long long)d * g.H + h) * g.W + w] = off;
-  }
+  for (int m = 0; m < 2; ++m)
+    dw[(long long)(v * 2 + m) * g.S + ((long long)d * g.H + h) * g.W + w] = edt::row_offset(bits[m], nw, w);
 }
-
-// Lower envelope of the parabolas F(i) + s2 (x - i)^2 - s2 x^2 over the sites with a finite cost, F(i) = cost(i) + s2 i^2.
-// stk: this thread's stack of site indices (stride kColThreads).  Returns the number of envelope sites (0: no finite cost).
-// sep(a, b) = (F(b) - F(a)) / (2 s2 (b - a)) is never divided out: both tests cross-multiply.
-template <class Cost>
-__device__ __forceinline__ int fh_envelope(const Cost& F, int n, uint8_t* stk) {
-  int top = -1;
-  double Fa = 0.0, Fb = 0.0;                     // F of stk[top - 1], stk[top]
-  for (int q = 0; q < n; ++q) {
-    const double Fq = F(q);
-    if (!(Fq < INFINITY)) continue;
-    while (top >= 1) {
-      const int a = stk[(top - 1) * kColThreads], bb = stk[top * kColThreads];
-      // pop b when sep(b, q) <= sep(a, b)
-      if ((Fq - Fb) * (double)(bb - a) <= (Fb - Fa) * (double)(q - bb)) {
-        --top;
-        Fb = Fa;
-        if (top >= 1) Fa = F(stk[(top - 1) * kColThreads]);
-      } else {
-        break;
-      }
-    }
-    stk[++top * kColThreads] = (uint8_t)q;
-    Fa = Fb;
-    Fb = Fq;
-  }
-  return top + 1;
-}
-
-// walks the envelope for x = 0, 1, ...: the site nearest to x
-template <class Cost>
-struct EnvelopeWalk {
-  const Cost& F;
-  const uint8_t* stk;
-  int sites, k;
-  double s2, F0, F1;
-  __device__ EnvelopeWalk(const Cost& f, const uint8_t* s, int n, double s2_) : F(f), stk(s), sites(n), k(0), s2(s2_) {
-    F0 = F(stk[0]);
-    F1 = sites > 1 ? F(stk[kColThreads]) : 0.0;
-  }
-  __device__ int site(int x) {
-    // advance while sep(stk[k], stk[k + 1]) < x
-    while (k + 1 < sites) {
-      const int a = stk[k * kColThreads], b = stk[(k + 1) * kColThreads];
-      if (!(F1 - F0 < 2.0 * s2 * (double)x * (double)(b - a))) break;
-      ++k;
-      F0 = F1;
-      if (k + 1 < sites) F1 = F(stk[(k + 1) * kColThreads]);
-    }
-    return stk[k * kColThreads];
-  }
-};
-
-struct CostH {   // F(h') = (dw s_w)^2 + s_h^2 h'^2 along one (d, w) column of the W offsets
-  const int16_t* col;
-  long long step;
-  double sw, s2;
-  __device__ double operator()(int i) const {
-    const int16_t o = col[i * step];
-    if (o == kNone) return INFINITY;
-    const double a = o * sw;
-    return a * a + s2 * (double)i * (double)i;
-  }
-};
 
 __global__ void __launch_bounds__(kColThreads) k_sf_cols_h(Geo g, const int16_t* __restrict__ dw, const double* __restrict__ spacing,
                                                            uint32_t* __restrict__ hw) {
@@ -191,33 +111,9 @@ __global__ void __launch_bounds__(kColThreads) k_sf_cols_h(Geo g, const int16_t*
   const int pl = blockIdx.y, v = pl / g.dirs, k = pl % g.dirs;
   const double* sp = spacing + (v / g.Cp) * 3;
   const long long off = (long long)d * g.HW + w;
-  CostH F{dw + (long long)(v * 2 + 1 - k) * g.S + off, g.W, sp[2], sp[1] * sp[1]};
-  uint8_t* stk = stk_all + threadIdx.x;
-  uint32_t* out = hw + (long long)pl * g.S + off;
-  const int sites = fh_envelope(F, g.H, stk);
-  if (sites == 0) {
-    for (int x = 0; x < g.H; ++x) out[(long long)x * g.W] = kNone32;
-    return;
-  }
-  EnvelopeWalk<CostH> walk(F, stk, sites, F.s2);
-  for (int x = 0; x < g.H; ++x) {
-    const int i = walk.site(x);
-    const int16_t o = F.col[i * F.step];
-    out[(long long)x * g.W] = ((uint32_t)(uint16_t)(int16_t)(i - x) << 16) | (uint16_t)o;
-  }
+  const edt::CostH F{dw + (long long)(v * 2 + 1 - k) * g.S + off, g.W, sp[2], sp[1] * sp[1]};
+  edt::cols_h(F, g.H, stk_all + threadIdx.x, hw + (long long)pl * g.S + off);
 }
-
-struct CostD {   // F(d') = (dh s_h)^2 + (dw s_w)^2 + s_d^2 d'^2 along one (h, w) column of the H pass
-  const uint32_t* col;
-  long long step;
-  double sh, sw, s2;
-  __device__ double operator()(int i) const {
-    const uint32_t p = col[i * step];
-    if (p == kNone32) return INFINITY;
-    const double a = (int16_t)(p >> 16) * sh, b = (int16_t)(p & 0xffffu) * sw;
-    return a * a + b * b + s2 * (double)i * (double)i;
-  }
-};
 
 __global__ void __launch_bounds__(kColThreads) k_sf_cols_d(Geo g, const int16_t* __restrict__ dw, const uint32_t* __restrict__ hw,
                                                            const double* __restrict__ spacing, const float* __restrict__ tau, int select,
@@ -237,22 +133,20 @@ __global__ void __launch_bounds__(kColThreads) k_sf_cols_d(Geo g, const int16_t*
   unsigned cnt = 0;
   if (w < g.W) {
     const long long off = (long long)h * g.W + w;
-    CostD F{hw + (long long)pl * g.S + off, g.HW, sp[1], sp[2], sp[0] * sp[0]};
+    const edt::CostD F{hw + (long long)pl * g.S + off, g.HW, sp[1], sp[2], sp[0] * sp[0]};
     const int16_t* query = dw + (long long)(v * 2 + k) * g.S + off;   // W offset 0 = an edge voxel of the query mask
     uint8_t* stk = stk_all + threadIdx.x;
-    const int sites = fh_envelope(F, g.D, stk);
+    const int sites = edt::fh_envelope(F, g.D, stk);
     int nk = 0;
     if (sites > 0) {
       uint32_t* kc = keys + ((long long)pl * g.HW + off) * g.D;
       uint32_t* h1 = hist1 + (long long)pl * kBins;
-      EnvelopeWalk<CostD> walk(F, stk, sites, F.s2);
+      edt::EnvelopeWalk<edt::CostD> walk(F, stk, sites, F.s2);
       for (int x = 0; x < g.D; ++x) {
         if (query[x * g.HW] != 0) continue;
         const int i = walk.site(x);
         const uint32_t p = F.col[i * F.step];
-        const double a = __dmul_rn((double)(i - x), sp[0]), b = __dmul_rn((double)(int16_t)(p >> 16), sp[1]),
-                     c = __dmul_rn((double)(int16_t)(p & 0xffffu), sp[2]);
-        const float dist = __double2float_rn(__dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(a, a), __dmul_rn(b, b)), __dmul_rn(c, c))));
+        const float dist = edt::distance(i, x, p, sp[0], sp[1], sp[2]);
         mx = fmaxf(mx, dist);
         sum += (double)dist;
         cnt += dist <= t;

@@ -60,13 +60,13 @@ WGRAD_KINDS = ("simt", "tap", "halo")               # b200unet_wgrad_route.kind
 
 class DiceCEDesc(C.Structure):
     """``b200unet_dice_ce_desc``: options of every fused criterion (DiceLoss, DiceCELoss, TverskyLoss, GeneralizedDiceLoss,
-    FocalLoss, DiceFocalLoss)."""
+    FocalLoss, DiceFocalLoss, HausdorffDTLoss)."""
     _fields_ = [("act", C.c_int32), ("target_kind", C.c_int32), ("include_background", C.c_int32), ("squared_pred", C.c_int32),
                 ("jaccard", C.c_int32), ("batch", C.c_int32), ("reduction", C.c_int32), ("smooth_nr", C.c_float),
                 ("smooth_dr", C.c_float), ("lambda_dice", C.c_float), ("lambda_ce", C.c_float),
                 ("overlap", C.c_int32), ("tversky_alpha", C.c_float), ("tversky_beta", C.c_float), ("w_type", C.c_int32),
                 ("voxel_term", C.c_int32), ("focal_softmax", C.c_int32), ("focal_gamma", C.c_float), ("focal_alpha", C.c_float),
-                ("focal_use_alpha", C.c_int32), ("class_weight", C.c_void_p)]
+                ("focal_use_alpha", C.c_int32), ("class_weight", C.c_void_p), ("hdt_weight", C.c_void_p)]
 
 
 class NetDesc(C.Structure):
@@ -146,6 +146,9 @@ _SIGS = {
                                        C.c_void_p, C.c_void_p]),
     "b200unet_dice_ce_bwd": (C.c_int, [C.POINTER(DiceCEDesc), C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200unet_hausdorff_dt_scratch_bytes": (C.c_size_t, [C.POINTER(DiceCEDesc)] + [C.c_int] * 5),
+    "b200unet_hausdorff_dt_weight": (C.c_int, [C.POINTER(DiceCEDesc), C.c_void_p, C.c_void_p] + [C.c_int] * 5 + [C.c_float, C.c_void_p,
+                                               C.c_void_p, C.c_void_p]),
     "b200unet_act_bwd": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_float,
                                    C.POINTER(Tensor5), C.c_void_p, C.c_int, C.c_void_p]),
     "b200unet_prelu_apply": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
@@ -223,6 +226,7 @@ _DIAG_SIGS = {
     "b200unet_diag_input_pack": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(Tensor5), C.c_void_p, C.c_int, C.c_void_p]),
     "b200unet_diag_input_grad": (C.c_int, [C.POINTER(Tensor5), C.POINTER(Tensor5), C.c_void_p, C.c_void_p, C.c_int, C.POINTER(Tensor5),
                                            C.c_int, C.c_void_p, C.c_void_p]),
+    "b200unet_diag_hausdorff_dt_fields": (C.c_int, [C.POINTER(DiceCEDesc), C.c_void_p, C.c_void_p] + [C.c_int] * 5 + [C.c_void_p] * 4),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGS)
@@ -614,14 +618,15 @@ _DICE_CE_ACTS = {None: 0, "sigmoid": 1, "softmax": 2}
 # b200unet_dice_ce_desc.overlap, .w_type and .voxel_term
 DICE_CE_OVERLAPS = {"dice": 0, "tversky": 1, "generalized_dice": 2}
 GDICE_WEIGHTS = {"square": 0, "simple": 1, "uniform": 2}
-DICE_CE_VOXEL_TERMS = {"ce": 0, "focal": 1}
+DICE_CE_VOXEL_TERMS = {"ce": 0, "focal": 1, "hausdorff_dt": 2}
 
 
 def dice_ce_desc(act=None, target_kind=0, include_background=True, squared_pred=False, jaccard=False, batch=False,
                  reduction="mean", smooth_nr=1e-5, smooth_dr=1e-5, lambda_dice=1.0, lambda_ce=1.0, overlap="dice",
                  tversky_alpha=0.5, tversky_beta=0.5, w_type="square", voxel_term="ce", focal_softmax=False, focal_gamma=2.0,
-                 focal_alpha=None, class_weight=None) -> DiceCEDesc:
-    """``class_weight``: a CUDA fp32 tensor of the focal term's per-class factors, or None; the caller keeps it alive"""
+                 focal_alpha=None, class_weight=None, hdt_weight=None) -> DiceCEDesc:
+    """``class_weight``: a CUDA fp32 tensor of the focal term's per-class factors, or None; ``hdt_weight``: the distance-weighted
+    term's CUDA fp32 [n, c', ...] weights (``hausdorff_dt_weight``), or None.  The caller keeps both alive"""
     if reduction not in ("mean", "sum"):
         raise ValueError("fused DiceCE supports reduction 'mean' or 'sum', got %r" % (reduction,))
     d = DiceCEDesc()
@@ -637,6 +642,8 @@ def dice_ce_desc(act=None, target_kind=0, include_background=True, squared_pred=
         d.focal_use_alpha = int(focal_alpha is not None)
         d.focal_alpha = float(focal_alpha) if focal_alpha is not None else 0.0
         d.class_weight = class_weight.data_ptr() if class_weight is not None else None
+    if voxel_term == "hausdorff_dt":
+        d.hdt_weight = hdt_weight.data_ptr() if hdt_weight is not None else None
     return d
 
 
@@ -651,6 +658,32 @@ def dice_ce_scratch_bytes(desc: DiceCEDesc, n: int, c: int, s: int) -> int:
         msg = lib.b200unet_last_error()
         raise RuntimeError("libb200unet dice_ce_scratch_bytes rejected n=%d c=%d spatial=%d: %s" % (n, c, s, msg.decode() if msg else "?"))
     return b
+
+
+def hausdorff_dt_scratch_bytes(desc: DiceCEDesc, n: int, c: int, d: int, h: int, w: int) -> int:
+    """bytes of the distance-field scratch; raises when the shape is rejected"""
+    lib = load_library()
+    b = int(lib.b200unet_hausdorff_dt_scratch_bytes(C.byref(desc), n, c, d, h, w))
+    if b == 0:
+        msg = lib.b200unet_last_error()
+        raise RuntimeError("libb200unet hausdorff_dt_scratch_bytes rejected %d x %d x %d x %d x %d: %s" % (n, c, d, h, w,
+                                                                                                        msg.decode() if msg else "?"))
+    return b
+
+
+def hausdorff_dt_weight(desc: DiceCEDesc, logits, target, alpha: float, scratch, weight) -> None:
+    """logits fp32 [n, c, d, h, w]; weight fp32 [n, c', d, h, w] = pdt^alpha + tdt^alpha (overwritten)"""
+    n, c, d, h, w = logits.shape
+    check(load_library().b200unet_hausdorff_dt_weight(C.byref(desc), logits.data_ptr(), target.data_ptr(), n, c, d, h, w, float(alpha),
+                                                      scratch.data_ptr(), weight.data_ptr(), stream_ptr()), "hausdorff_dt_weight")
+
+
+def hausdorff_dt_fields(desc: DiceCEDesc, logits, target, scratch, pred_field, target_field) -> None:
+    """the raw fields edt(mask) + edt(~mask) of the prediction and target masks, fp32 [n, c', d, h, w] each (None: not computed)"""
+    n, c, d, h, w = logits.shape
+    check(load_library().b200unet_diag_hausdorff_dt_fields(C.byref(desc), logits.data_ptr(), target.data_ptr(), n, c, d, h, w,
+                                                           scratch.data_ptr(), _p(pred_field), _p(target_field), stream_ptr()),
+          "diag_hausdorff_dt_fields")
 
 
 def cc_scratch_bytes(nvol: int, d: int, h: int, w: int) -> int:

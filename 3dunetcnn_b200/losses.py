@@ -9,7 +9,8 @@ hand-written kernels ``b200unet_dice_fwd`` / ``b200unet_dice_bwd``; targets stay
 ``{"name": "DiceCELoss", "softmax": true, "to_onehot_y": true}`` the same way, on ``b200unet_dice_ce_fwd`` / ``_bwd``: it reads
 a one-channel label map (or a C-channel target) and adds cross-entropy to a softmax Dice.  ``TverskyLoss``,
 ``GeneralizedDiceLoss``, ``FocalLoss`` and ``DiceFocalLoss`` run on the same entry points with the same target forms: another
-overlap of the same per-(n, c) sums, or the focal term in CE's place.
+overlap of the same per-(n, c) sums, or the focal term in CE's place.  ``HausdorffDTLoss`` and ``LogHausdorffDTLoss`` take the
+distance-weighted term in its place, on weights ``b200unet_hausdorff_dt_weight`` computes from exact distance transforms.
 """
 from __future__ import annotations
 
@@ -19,6 +20,8 @@ import torch
 from torch import nn
 
 from . import lib as _lib
+
+_SURFACE_MAX_EXTENT = 256      # B200_SURFACE_MAX_EXTENT: voxels per axis of the distance transforms (HausdorffDTLoss)
 
 
 class _DiceFunction(torch.autograd.Function):
@@ -306,3 +309,68 @@ class DiceFocalLoss(_FusedCriterion):
                           reduction=reduction, smooth_nr=smooth_nr, smooth_dr=smooth_dr, lambda_dice=lambda_dice,
                           lambda_ce=lambda_focal, voxel_term="focal", focal_softmax=softmax, focal_gamma=gamma,
                           focal_alpha=_focal_alpha(alpha, softmax, include_background))
+
+
+class HausdorffDTLoss(_FusedCriterion):
+    """monai.losses.HausdorffDTLoss (Karimi & Salcudean 2019), on 3-D ``[N, C, D, H, W]`` inputs of at most 256 voxels per axis.
+
+    p = act(input) (sigmoid, softmax over all C channels, or identity); ``include_background=False`` then drops channel 0.  For
+    every kept (n, c) the prediction mask p > 0.5 and the target mask t > 0.5 each get the distance field edt(mask) + edt(~mask)
+    (Euclidean distance in voxels to the nearest voxel of the other value, as scipy's ``distance_transform_edt`` rounded to
+    fp32; 0 for an empty or full mask), computed on the device and carrying no gradient.  ``f_nc = mean over the voxels (and n
+    with ``batch``) of (p - t)^2 (pdt^alpha + tdt^alpha)``; the loss is the mean or sum of the f terms.  Targets, ``to_onehot_y``
+    and the C == 1 rules as in ``DiceCELoss``; a label outside ``[0, C)`` is an all-zero target row.  ``other_act``, 2-D inputs,
+    larger extents and ``alpha <= 0`` raise ``NotImplementedError``; ``reduction="none"`` raises ``ValueError``.
+    """
+
+    _name = "HausdorffDTLoss"
+
+    def __init__(self, alpha=2.0, include_background=False, to_onehot_y=False, sigmoid=False, softmax=False, other_act=None,
+                 reduction="mean", batch=False):
+        super().__init__()
+        if other_act is not None:
+            raise NotImplementedError("fused %s: other_act is not implemented" % self._name)
+        if not float(alpha) > 0.0:
+            raise NotImplementedError("fused %s: alpha=%r (only alpha > 0)" % (self._name, alpha))
+        act = _act_opts(self._name, sigmoid, softmax, other_act)
+        _check_reduction(self._name, reduction)
+        self.alpha = float(alpha)
+        self.to_onehot_y = bool(to_onehot_y)
+        self._opts = dict(act=act, include_background=include_background, batch=batch, reduction=reduction, lambda_dice=0.0,
+                          lambda_ce=1.0, voxel_term="hausdorff_dt")
+
+    def _check_extent(self, input: torch.Tensor) -> None:
+        if input.dim() != 5:
+            raise NotImplementedError("fused %s: only 3-D [N, C, D, H, W] inputs, got shape %s" % (self._name, tuple(input.shape)))
+        if max(input.shape[2:]) > _SURFACE_MAX_EXTENT:
+            raise NotImplementedError("fused %s: spatial extent %s; at most %d voxels per axis"
+                                      % (self._name, tuple(input.shape[2:]), _SURFACE_MAX_EXTENT))
+
+    def forward(self, input: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
+        self._check_extent(input)
+        self._check_shapes(input, target)
+        n, c, d, h, w = input.shape
+        out, tgt = _prepare(self._name, input, target)
+        tgt, kind = self._target_kind(c, tgt)
+        tgt = tgt.contiguous()
+        kept = c - 1 if (not self._opts["include_background"] and c > 1) else c
+        desc = _lib.dice_ce_desc(target_kind=kind, **self._opts)
+        with torch.cuda.device(out.device):
+            # the distance weights are constants of the loss: computed here, outside autograd, and held by the descriptor until
+            # the backward has read them
+            field_scratch = torch.empty(_lib.hausdorff_dt_scratch_bytes(desc, n, c, d, h, w), dtype=torch.uint8, device=out.device)
+            weight = torch.empty((n, kept, d, h, w), dtype=torch.float32, device=out.device)
+            _lib.hausdorff_dt_weight(desc, out, tgt, self.alpha, field_scratch, weight)
+            desc.hdt_weight = weight.data_ptr()
+            desc._hdt_weight = weight
+            scratch_len = _lib.dice_ce_scratch_bytes(desc, n, c, d * h * w) // 8
+            return _DiceFunction.apply(out, tgt, desc, _lib.dice_ce_fwd, _lib.dice_ce_bwd, scratch_len)
+
+
+class LogHausdorffDTLoss(HausdorffDTLoss):
+    """monai.losses.LogHausdorffDTLoss: ``log(HausdorffDTLoss + 1)``, same arguments."""
+
+    _name = "LogHausdorffDTLoss"
+
+    def forward(self, input: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
+        return torch.log(super().forward(input, target) + 1)

@@ -176,7 +176,9 @@ typedef struct b200unet_dice_ce_desc {
   float tversky_alpha, tversky_beta;
   int32_t w_type;               /* generalized Dice: 0 1/T^2, 1 1/T, 2 uniform */
   int32_t voxel_term;           /* the term lambda_ce scales: 0 CE, 1 focal (monai.losses.FocalLoss) on the channels include_background
-                                   keeps; mean divides its total by n * c' * spatial, sum by spatial (MONAI averages over the voxels) */
+                                   keeps; mean divides its total by n * c' * spatial, sum by spatial (MONAI averages over the voxels);
+                                   2 distance-weighted (monai.losses.HausdorffDTLoss), (p_c - t_c)^2 hdt_weight on the kept channels
+                                   with p = act(x), divided as focal, and by n * spatial for sum with batch; lambda_dice 0 */
   int32_t focal_softmax;        /* 0 sigmoid form, per element (x - x t - logsigmoid(x)) exp(gamma logsigmoid(-x (2t - 1)));
                                    1 softmax form -(1 - exp(ls))^gamma ls t, ls = log_softmax over the kept channels */
   float focal_gamma;            /* >= 0 */
@@ -184,6 +186,7 @@ typedef struct b200unet_dice_ce_desc {
                                    channel and alpha on the others */
   int32_t focal_use_alpha;
   const float* class_weight;    /* focal: DEVICE fp32 [c'] per-class factors, NULL = none */
+  const float* hdt_weight;      /* distance-weighted: DEVICE fp32 [n][c'][spatial] from b200unet_hausdorff_dt_weight */
 } b200unet_dice_ce_desc;
 
 /* DiceLoss: act 0 or 1 (softmax: E_UNSUPPORTED, b200unet_dice_ce_* runs it), target_kind 2 or 3 (label maps: E_UNSUPPORTED),
@@ -208,6 +211,19 @@ int b200unet_dice_ce_fwd(const b200unet_dice_ce_desc* desc, const float* logits,
                          int64_t spatial, void* scratch, float* loss, void* stream);
 int b200unet_dice_ce_bwd(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c,
                          int64_t spatial, const void* scratch, const float* grad_out, float* dlogits, void* stream);
+
+/* ---- distance weights of HausdorffDTLoss (monai.losses.HausdorffDTLoss, Karimi & Salcudean 2019), without scipy on the host.
+ * For each (n, c) that include_background keeps, the prediction mask act(x) > 0.5 (act, and a softmax over all c channels, as
+ * the dice_ce kernels form p) and the target mask t > 0.5 (target_kind as for dice_ce; a label outside [0, c) is no class) each
+ * get the field edt(mask) + edt(~mask): per voxel the Euclidean distance, in voxels, to the nearest voxel of the other value,
+ * scipy.ndimage.distance_transform_edt's fp64 value rounded to fp32 (bit for bit).  An empty or full mask has the field 0; the
+ * rule is applied from device counts, nothing is read back.  weight DEVICE fp32 [n][c'][d*h*w] = pdt^alpha + tdt^alpha, alpha > 0.
+ * The desc's act, target_kind and include_background are read; with c == 1 softmax is ignored and a uint8 label map is the
+ * target itself.  Extents 1..256 per axis, n * c' <= 4096, c <= 128, else B200UNET_E_UNSUPPORTED.
+ *   hausdorff_dt_scratch_bytes: from the shape alone (0 = rejected): 24 bytes per kept (n, c) and voxel. */
+size_t b200unet_hausdorff_dt_scratch_bytes(const b200unet_dice_ce_desc* desc, int n, int c, int d, int h, int w);
+int b200unet_hausdorff_dt_weight(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c, int d, int h,
+                                 int w, float alpha, void* scratch, float* weight, void* stream);
 
 /* ---- sliding-window inference on the device (monai.inferers.SlidingWindowInferer as called by
  * predict/volumetric.py:147-148 and train/training_utils.py:106-107).  `starts`: HOST array [ntiles][4] of

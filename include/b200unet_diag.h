@@ -110,6 +110,12 @@ int b200unet_diag_input_pack(const float* x, int c, const b200unet_tensor* out, 
 int b200unet_diag_input_grad(const b200unet_tensor* dz, const b200unet_tensor* x, const float* coef, const float* coef2, int coef_ld,
                              const b200unet_tensor* r, int c, float* dx, void* stream);
 
+/* the raw distance fields behind b200unet_hausdorff_dt_weight: pred_field / target_field DEVICE fp32 [n][c'][d*h*w] =
+ * edt(mask) + edt(~mask) of the prediction and target masks (0 for an empty or full mask); either NULL = not computed.  scratch:
+ * b200unet_hausdorff_dt_scratch_bytes() bytes */
+int b200unet_diag_hausdorff_dt_fields(const b200unet_dice_ce_desc* desc, const float* logits, const void* target, int n, int c, int d,
+                                      int h, int w, void* scratch, float* pred_field, float* target_field, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
