@@ -110,16 +110,13 @@ def route_table(L, config, split):
     """{label (".dgrad" for a data gradient): (kind, BN, KC, CTAs per SM)} of the config's convolutions, from the library's route
     query (include/b200unet_diag.h)"""
     import plan_launches as P
-    return {label(l.key) + (".dgrad" if l.kernel == "dgrad" else ""): tuple(P.conv_route(L, l, split)[f]
-                                                                           for f in ("kind", "bn", "kc", "blocks_per_sm"))
-            for l in config.launches() if l.kernel in ("fwd", "dgrad")}
+    return P.route_table(L, config, split, label)
 
 
 def wgrad_route_table(L, config, split):
     """{label: (kind, K chunk, BN)} of the config's weight gradients, from the library's weight-gradient route query"""
     import plan_launches as P
-    return {label(l.key): tuple(P.wgrad_route(L, l, split)[f] for f in ("kind", "cb", "bn"))
-            for l in config.launches() if l.kernel == "wgrad"}
+    return P.wgrad_route_table(L, config, split, label)
 
 
 # the routes of the two workloads on a 132-SM H100, per precision.  In bf16 the logits conv (L0 2.1.conv.unit0) runs on per-tap

@@ -58,6 +58,20 @@ def wgrad_route(L, l, split):
     return R.wgrad_query(L, l.op, pad8(l.c), pad8(l.co), l.dims, split, n=l.n)
 
 
+def route_table(L, config, split, label):
+    """{label(key) (+ ".dgrad" for a data gradient): (kind, BN, KC, CTAs per SM)} of the config's forward convolutions and
+    data gradients, from the library's route query (include/b200unet_diag.h)"""
+    return {label(l.key) + (".dgrad" if l.kernel == "dgrad" else ""): tuple(conv_route(L, l, split)[f]
+                                                                           for f in ("kind", "bn", "kc", "blocks_per_sm"))
+            for l in config.launches() if l.kernel in ("fwd", "dgrad")}
+
+
+def wgrad_route_table(L, config, split, label):
+    """{label(key): (kind, K chunk, BN)} of the config's weight gradients, from the library's weight-gradient route query"""
+    return {label(l.key): tuple(wgrad_route(L, l, split)[f] for f in ("kind", "cb", "bn"))
+            for l in config.launches() if l.kernel == "wgrad"}
+
+
 def _block_fwd(out, n, keys, cin, C, e, train, first=False, scale_in=False):
     """build_block_fwd: norm1 -> conv1 -> norm2 -> conv2 + the 1x1x1 `sample` convolution of the input when the width changes.
     build_block_bwd hands norm1's k_gn_bwd the output gradient as the residual addend when the width is kept (and the Dropout3d

@@ -1,11 +1,13 @@
 """Host logic of the DynUNet mirror (no GPU): MONAI kwarg surface, state-dict spec == the restated oracle spec == the
-library plan's spec, loud rejection of what is not implemented, the reference's JSON config builds."""
+library plan's spec, loud rejection of what is not implemented, the reference's JSON config builds, and the routes of the BraTS
+workload's convolutions as tests/dynunet_cases.py tables them."""
 import json
 import os
 
 import pytest
 import torch
 
+import dynunet_cases as D
 from oracle.dynunet_oracle import dynunet_state_dict_spec, make_dynunet_state_dict, dynunet_forward
 
 KW = dict(spatial_dims=3, in_channels=4, out_channels=3, kernel_size=[[3, 3, 3]] * 4, strides=[[1, 1, 1]] + [[2, 2, 2]] * 3,
@@ -58,3 +60,13 @@ def test_oracle_restatement_shapes():
     sd = make_dynunet_state_dict(2, 2, [8, 16, 16])
     y = dynunet_forward(sd, torch.randn(2, 2, 16, 24, 16), 3)
     assert y.shape == (2, 2, 16, 24, 16) and torch.isfinite(y).all()
+
+
+@pytest.mark.parametrize("precision", ["bf16", "split"])
+def test_brats_workload_takes_the_tabled_routes(pkg, precision):
+    """every convolution, data gradient (the input gradient's included) and weight gradient of the BraTS workload (batch 2,
+    4 x 128^3) on the route of dynunet_cases.BRATS_ROUTES / BRATS_WGRAD_ROUTES (the host query assumes 132 SMs without a device)"""
+    L = pkg.lib
+    split = precision == "split"
+    assert D.route_table(L, split) == D.BRATS_ROUTES[precision]
+    assert D.wgrad_route_table(L, split) == D.BRATS_WGRAD_ROUTES[precision]

@@ -64,20 +64,32 @@ def test_bf16_mode_gradient_error_is_torch_autocast_class(pkg, bw, seed):
     loss.backward()
     ours_g = {k: p.grad.double() for k, p in model.named_parameters()}
 
-    def rel(a, b):
-        return float((a - b).norm() / (b.norm() + 1e-300))
-
     assert abs(float(loss) - ref_loss) < 1e-3 * abs(ref_loss)
-    assert rel(out.detach().double(), ref_out) <= 1.25 * rel(ac_out, ref_out)
-    num_o = num_a = den = 0.0
+    assert _rel(out.detach().double(), ref_out) <= 1.25 * _rel(ac_out, ref_out)
+    check_autocast_class(ours_g, ac_g, ref_g)     # median per-tensor ratio measured 0.90 .. 1.04
+
+
+def _rel(a, b):
+    return float((a - b).norm() / (b.norm() + 1e-300))
+
+
+def check_autocast_class(ours_g, ac_g, ref_g):
+    """the gradient bounds of the module docstring: {key: gradient} of this library (ours_g) and of torch's bf16 autocast (ac_g)
+    against the fp64 truth (ref_g).  Returns (our whole-gradient rel-L2, autocast's, median per-tensor ratio,
+    worst gradient-norm deviation)."""
+    num_o = num_a = den = worst = 0.0
     ratios = []
     for k, r in ref_g.items():
-        eo, ea = rel(ours_g[k], r), rel(ac_g[k], r)
+        eo, ea = _rel(ours_g[k], r), _rel(ac_g[k], r)
         assert eo <= 2.0 * ea + 5e-3, (k, eo, ea)
-        assert abs(float(ours_g[k].norm() / r.norm()) - 1.0) < 0.08, k
+        dev = abs(float(ours_g[k].norm() / r.norm()) - 1.0)
+        assert dev < 0.08, (k, dev)
+        worst = max(worst, dev)
         ratios.append(eo / (ea + 1e-12))
         num_o += float((ours_g[k] - r).pow(2).sum())
         num_a += float((ac_g[k] - r).pow(2).sum())
         den += float(r.pow(2).sum())
-    assert (num_o / den) ** 0.5 <= 1.25 * (num_a / den) ** 0.5
-    assert sorted(ratios)[len(ratios) // 2] <= 1.25                # median per-tensor ratio (measured 0.90 .. 1.04)
+    whole_o, whole_a, median = (num_o / den) ** 0.5, (num_a / den) ** 0.5, sorted(ratios)[len(ratios) // 2]
+    assert whole_o <= 1.25 * whole_a
+    assert median <= 1.25
+    return whole_o, whole_a, median, worst
